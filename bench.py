@@ -4,7 +4,7 @@ corr-lookup kernel's HBM roofline and the CPU baseline beside it.
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl native|reference|reference_gpu] [--model raft_nc_dbl|raft]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
---impl reference      the UNMODIFIED reference (baseline/_ref, installed by baseline/install_reference.sh) on the host CPU cores
+--impl reference      the UNMODIFIED reference (oracle/_ref, built by build() from oracle/install_reference.sh) on the host CPU cores
 --impl reference_gpu  the same reference modules in eager PyTorch on the GPU, TF32 off (SURVEY.md §0.1: "the bar"); the native
                       arm runs this leg in a subprocess (the reference's module names clash with the drop-in's) and reports it
                       as `gpu_eager_baseline`
@@ -25,7 +25,7 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.join(ROOT, "raft-ncup_b200")
-REF_CORE = os.path.join(ROOT, "baseline", "_ref", "core")        # pip-installed copy of the unmodified reference (git-ignored)
+REF_CORE = os.path.join(ROOT, "oracle", "_ref", "core")          # copy of the unmodified reference built by build() (git-ignored)
 
 import torch  # noqa: E402
 
@@ -53,24 +53,25 @@ K5_BYTES_PER_PAIR_CALL = 19_880_960      # SURVEY.md §8(d): mask 16,220,160 + f
 K2_STORAGE_BYTES_PER_PAIR_ITER = 2 * 7040 * 256 + 8 * 7040 + 4 * 7040 * 324 + 2 * 256 * 9280
 
 
-def ncu_traffic(kernel_key):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch, from the committed ncu --set full summary of this round."""
-    path = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            return json.load(f).get(kernel_key, {}).get("dram_bytes_per_launch")
-    return None
 METRIC = "image-pairs/sec @ 1024x436, 32 iters"
 TRAIN_METRIC = "training image-pairs/sec @ 512x384, 12 iters (BASELINE configs[4])"
 
 
-def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            p = json.load(f)
-        return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md: 6.65 TB/s)"
+def hbm_copy_gbs(dev):
+    """Achievable HBM bandwidth of this GPU, measured here: a 1 GiB device-to-device copy, read + write bytes over time."""
+    n = 1 << 30
+    src, dst = torch.empty(n, dtype=torch.uint8, device=dev), torch.empty(n, dtype=torch.uint8, device=dev)
+    for _ in range(2):
+        dst.copy_(src)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(10):
+        dst.copy_(src)
+    e1.record()
+    torch.cuda.synchronize()
+    gbs = 2 * n * 10 / (e0.elapsed_time(e1) * 1e-3) / 1e9
+    del src, dst
+    return gbs, "measured in this run: 1 GiB device-to-device copy, (read + write) bytes / time"
 
 
 def synth_frames(b, seed):
@@ -95,7 +96,7 @@ def ref_args(dataset="sintel"):
 
 
 def reference_model(name):
-    """RAFT(args) of the unmodified reference (baseline/_ref/core/raft_nc_dbl.py:26 / raft.py:24), seed 1234 (train.py:345)."""
+    """RAFT(args) of the unmodified reference (oracle/_ref/core/raft_nc_dbl.py:26 / raft.py:24), seed 1234 (train.py:345)."""
     import importlib
     import warnings
     warnings.filterwarnings("ignore")
@@ -104,7 +105,7 @@ def reference_model(name):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -152,9 +153,9 @@ def host_cores():
 
 
 def cpu_reference_pairs_per_s(steps, warmup, model_name="raft_nc_dbl"):
-    """The reference's own CPU path on the host cores: RAFT(args).eval() from baseline/_ref under torch.no_grad(), fp32, all
+    """The reference's own CPU path on the host cores: RAFT(args).eval() from oracle/_ref under torch.no_grad(), fp32, all
     the cores the cgroup allows.  One step = ONE pair at the full 1024x436 / 32-iteration shape (a bounded sample of the 8-pair
-    batch: ~7 s).  Falls back to the oracle port (pinned to the reference by tests/golden) when baseline/_ref is absent.
+    batch: ~7 s).  Falls back to the oracle port (pinned to the reference by tests/golden) when oracle/_ref is absent.
     Returns (pairs/s, s/step, kind)."""
     torch.set_num_threads(host_cores())
     p1, p2 = synth_frames(1, 7)
@@ -198,16 +199,16 @@ def run_reference(args, rank):
         "dtype": "f32", "data": "synthetic",
         "config": {"workload": f"cfg2/3: 1024x436 (pad 440), 32 iters, {args.model} full path incl. the upsampler, B=1 per step "
                                "(bounded sample of the B=8 batch)", "device": "host CPU",
-                   "implementation": "unmodified reference modules from baseline/_ref" if kind == "reference" else "oracle port"},
+                   "implementation": "unmodified reference modules from oracle/_ref" if kind == "reference" else "oracle port"},
         "cpu_baseline": {"value": v, "unit": "pairs/s", "cores": cores, "kind": kind, "sample": CPU_SAMPLE},
         "e2e": {"value": v, "unit": "pairs/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}))
 
 
 def run_reference_gpu(args):
-    """SURVEY.md §0.1 / BASELINE.md §3.5: the reference's eager PyTorch path on the same B200 (cuBLAS bmm volume + grid_sample
+    """SURVEY.md §0.1 / BASELINE.md §3.5: the reference's eager PyTorch path on the same GPU (cuBLAS bmm volume + grid_sample
     + cuDNN convolutions), TF32 off so that it computes what its CPU path computes.  CUDA events, warm-up, one JSON line."""
     if not use_reference_path() or not torch.cuda.is_available():
-        print(json.dumps({"impl": "reference_gpu", "unavailable": "baseline/_ref or GPU missing"}))
+        print(json.dumps({"impl": "reference_gpu", "unavailable": "oracle/_ref or GPU missing"}))
         return
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
@@ -231,13 +232,13 @@ def run_reference_gpu(args):
     print(json.dumps({"impl": "reference_gpu", "metric": METRIC, "value": args.batch / (ms * 1e-3), "unit": "pairs/s",
                       "ms_per_step": ms, "steps": args.steps, "batch": args.batch, "model": args.model, "dtype": "f32",
                       "tf32": False, "checksum_flow_up_abs_mean": float(up.abs().mean()),
-                      "note": "unmodified reference modules (baseline/_ref) .cuda(), eager PyTorch, cudnn/matmul TF32 disabled, "
+                      "note": "unmodified reference modules (oracle/_ref) .cuda(), eager PyTorch, cudnn/matmul TF32 disabled, "
                               "inputs resident, CUDA events"}))
 
 
 def run_reference_gpu_train(args, dev):
     """The reference's own training step in eager PyTorch on the GPU (train.py:203-227 without AMP): unmodified modules from
-    baseline/_ref, train mode + freeze_bn, sequence loss (train.py:46-71 restated: train.py itself does not import), AdamW,
+    oracle/_ref, train mode + freeze_bn, sequence loss (train.py:46-71 restated: train.py itself does not import), AdamW,
     clip 1.0 — the comparator of `--mode train`."""
     B, H, W, iters = args.train_batch, 384, 512, 12
     model = reference_model(args.model).to(dev).train()
@@ -266,13 +267,13 @@ def run_reference_gpu_train(args, dev):
     print(json.dumps({"impl": "reference_gpu", "mode": "train", "metric": TRAIN_METRIC, "value": B / (ms * 1e-3), "unit": "pairs/s",
                       "ms_per_step": ms, "steps": args.steps, "batch": B, "model": args.model, "dtype": "f32", "tf32": False,
                       "loss_last": float(loss),
-                      "note": "unmodified reference modules (baseline/_ref) in eager PyTorch, cuDNN/cuBLAS TF32 disabled"}))
+                      "note": "unmodified reference modules (oracle/_ref) in eager PyTorch, cuDNN/cuBLAS TF32 disabled"}))
 
 
 def gpu_eager_baseline(args):
     """Run the reference_gpu leg in a fresh process (module names `raft_nc_dbl`, `update`, `corr`, ... clash with the drop-in)."""
     if not os.path.isdir(REF_CORE):
-        return {"unavailable": "baseline/_ref not installed (run baseline/install_reference.sh)"}
+        return {"unavailable": "oracle/_ref not installed (run oracle/install_reference.sh)"}
     cmd = [sys.executable, os.path.abspath(__file__), "--impl", "reference_gpu", "--steps", "2", "--warmup", "1",
            "--batch", str(args.batch), "--model", args.model, "--mode", args.mode, "--train-batch", str(args.train_batch)]
     try:
@@ -282,6 +283,26 @@ def gpu_eager_baseline(args):
         return json.loads(line)
     except Exception as e:     # noqa: BLE001 — the baseline leg must never take the bench down
         return {"unavailable": f"{type(e).__name__}: {e}"}
+
+
+DUMP_BYTES = 60 << 20          # 63 MB of data: the files, headers included, stay under 64 MB
+
+
+def dump_outputs(out_dir, arrays):
+    """What the timed path returned in its last step, as float32 .npy files (flow_low [B,2,55,128], flow_up [B,2,440,1024]),
+    for comparing two builds output for output.  At most DUMP_BYTES in all: an array that does not fit is replaced by a fixed
+    sample of its elements (flattened indices drawn with seed 0, sorted), the same for every run with the same arguments."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    left = DUMP_BYTES
+    for name, t in arrays.items():
+        a = t.detach().float().cpu()
+        if a.numel() * 4 > left:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(a.numel(), generator=g)[: left // 4].sort().values
+            a = a.reshape(-1)[idx]
+        left -= a.numel() * 4
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.numpy())
 
 
 def mean_ms(pairs):
@@ -300,7 +321,7 @@ def run_native(args, rank, world, local_rank):
     p1, p2 = synth_frames(args.batch, 7 + rank)
     h1, h2 = p1.pin_memory(), p2.pin_memory()                      # host buffers of the e2e arm
     d1, d2 = h1.to(dev), h2.to(dev)                                # resident inputs of the `value` arm
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2
     out_lo = torch.empty(args.batch, 2, 55, 128).pin_memory()
     out_up = torch.empty(args.batch, 2, 440, 1024).pin_memory()
 
@@ -343,14 +364,14 @@ def run_native(args, rank, world, local_rank):
         return lo, up
 
     def timed(fn, steps):
-        evs = []
+        evs, out = [], None
         barrier()
         t0 = time.perf_counter()
         for _ in range(steps):
             flush.zero_()                                           # L2 flush between timed iterations (not timed)
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            fn()
+            out = fn()
             e1.record()
             evs.append((e0, e1))
         barrier()
@@ -359,7 +380,7 @@ def run_native(args, rank, world, local_rank):
         t = torch.tensor([dev_ms], dtype=torch.float64, device=dev)
         if world > 1:
             dist.all_reduce(t, op=dist.ReduceOp.MAX)                # max over ranks
-        return t.item(), wall
+        return t.item(), wall, out
 
     for _ in range(max(args.warmup, 3)):
         step_resident()
@@ -372,10 +393,12 @@ def run_native(args, rank, world, local_rank):
     eng = model.engine()
     eng.profile = {}
     native.launch_count_reset()
-    ms_total, wall = timed(step_resident, args.steps)
+    ms_total, wall, last = timed(step_resident, args.steps)
     launches = native.launch_count()
     prof, eng.profile = eng.profile, None
-    ms_e2e, _ = timed(step_e2e, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"flow_low": last[0], "flow_up": last[1]})
+    ms_e2e, _, _ = timed(step_e2e, args.steps)
     # the lookup kernel alone (in the timed region convf1 runs underneath it on a side stream): 32 back-to-back launches
     iso_ms = None
     if hasattr(eng, "lookup_resident"):
@@ -448,7 +471,7 @@ def run_native(args, rank, world, local_rank):
     e2e = pairs / (ms_e2e * 1e-3)
     if rank != 0:
         return
-    peak, peak_src = peaks()
+    peak, peak_src = hbm_copy_gbs(dev)
     k2_ms = mean_ms(prof.get("corr_lookup", []))
     k2_bytes = K2_BYTES_PER_PAIR_ITER * args.batch
     k2_gbs = k2_bytes / (k2_ms * 1e-3) / 1e9 if k2_ms else 0.0
@@ -469,8 +492,8 @@ def run_native(args, rank, world, local_rank):
                 "d2h_bytes_per_step": int(out_lo.numel() + out_up.numel()) * 4, "ms_per_step": ms_e2e / args.steps},
         "gpu_launches": int(launches),
         "clocks": clocks,
-        "roofline": {"kernel": "corr_lookup_umma_kernel (tcgen05 fused corr lookup, K2; incoherent units recomputed exactly inside the same launch)", "bound": "hbm",
-                     "achieved": k2_gbs, "peak": peak, "unit": "GB/s", "frac": k2_gbs / peak, "traffic": ncu_traffic("corr_lookup"),
+        "roofline": {"kernel": "corr_lookup_umma_kernel (wgmma fused corr lookup, K2; incoherent units recomputed exactly inside the same launch)", "bound": "hbm",
+                     "achieved": k2_gbs, "peak": peak, "unit": "GB/s", "frac": k2_gbs / peak,
                      "peak_source": peak_src, "algorithmic_bytes_per_launch": k2_bytes,
                      "algorithmic_bytes_note": "SURVEY §8d contract figure (fp32 storage: 25,891,840 B/pair-iter); at the storage "
                                                "width actually used (fp16 features, 4 B hi/lo outputs) one launch moves "
@@ -491,9 +514,8 @@ def run_native(args, rank, world, local_rank):
                           "frac": k4_gbs / peak, "avg_launch_ms": k4_ms,
                           "algorithmic_bytes_per_launch": K4_BYTES_PER_PAIR_CALL * args.batch,
                           "fma_pipe": {"tflops_fp32": (K4_FMA_PER_PIXEL * 2 * args.batch * 2 * 440 * 1024 / (k4_ms * 1e-3) / 1e12) if k4_ms else None,
-                                       "peak_tflops_fp32": 74.5,
                                        "note": "the chain is ~300 multiply-adds per output pixel (4 normalized convolutions, num and den "
-                                               "streams): bound by the FP32 FMA pipe (148 SMs x 128 lanes x 2 x 1.965 GHz), not by HBM"}},
+                                               "streams): bound by the FP32 FMA pipe, not by HBM"}},
         "roofline_convex": {"kernel": "convex_upsample_kernel (K5, model raft)", "bound": "hbm",
                             "achieved": (K5_BYTES_PER_PAIR_CALL * args.batch / (k5_ms * 1e-3) / 1e9) if k5_ms else None, "peak": peak,
                             "unit": "GB/s", "frac": (K5_BYTES_PER_PAIR_CALL * args.batch / (k5_ms * 1e-3) / 1e9 / peak) if k5_ms else None,
@@ -637,7 +659,7 @@ def run_train(args, rank, world, local_rank):
         "tflops_fp32": 3 * fwd_gflop * B * 1e9 / (ms / args.steps * 1e-3) / 1e12,
         "gpu_launches": int(launches), "clocks": clocks,
         "tf32x3_convs": {"ms_per_step": tc_ms, "value": (B / (tc_ms * 1e-3)) if tc_ms else None,
-                         "note": "RNC_TRAIN_CONV=tf32: forward and data-gradient convolutions on tcgen05 kind::tf32 (hi/lo operand "
+                         "note": "RNC_TRAIN_CONV=tf32: forward and data-gradient convolutions on wgmma .tf32 (hi/lo operand "
                                  "planes, 3 MMAs per K step); per-layer error 1e-6..5e-6 instead of 1.5e-7, opt-in"},
         "gpu_eager_baseline": gpu_eager_baseline(args) if world == 1 and not args.no_cpu_baseline else None}))
 
@@ -653,7 +675,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--mode", default="infer", choices=["infer", "train"], help="train: one optimisation step per timed step (cfg 5)")
     ap.add_argument("--train-batch", type=int, default=2, help="pairs per GPU in --mode train")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the flows of the last timed inference step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl != "native" or args.mode != "infer"):
+        ap.error("--dump-outputs writes the outputs of the native inference path (--impl native --mode infer)")
     rank = int(os.environ.get("RANK", 0))
     world = int(os.environ.get("WORLD_SIZE", 1))
     local_rank = int(os.environ.get("LOCAL_RANK", 0))

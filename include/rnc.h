@@ -1,4 +1,4 @@
-/* rnc.h — C ABI of librnc.so: the B200 (sm_100a) kernels behind RAFT-NCUP's per-iteration hot path.
+/* rnc.h — C ABI of librnc.so: the H100 (sm_90a) kernels behind RAFT-NCUP's per-iteration hot path.
  *
  * The reference (abdo-eldesokey/RAFT-NCUP @ 51ac387) has NO native layer: every op below is a chain of
  * PyTorch eager calls.  Each entry point therefore cites the reference *Python* interface it replaces
@@ -34,7 +34,7 @@ typedef enum {
 
 /* Library identity / diagnostics. */
 int rnc_abi_version(void);                 /* bumps on any signature change (now 10) */
-const char* rnc_build_info(void);          /* e.g. "sm_100a nvcc 12.9" */
+const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
 /* Number of kernels launched by this library on the calling thread since the last reset (bench.py's
@@ -81,7 +81,7 @@ int rnc_corr_lookup_split_fwd(const float* f1_cl, const float* f2_pyr, const flo
  * permuted to match): tap (i, j) -> j*8 + i for i < 8, tap (8, j) -> 72 + j  — a pixel's 8 values of one window row are
  * one aligned 16-byte group.  The reference order k = i*9 + j is what rnc_corr_lookup_fwd returns. */
 
-/* Tensor-core version of the lookup (tcgen05 + TMA; same reference code, corr.py:7-55 + utils.py:59-73).
+/* Tensor-core version of the lookup (wgmma + TMA; same reference code, corr.py:7-55 + utils.py:59-73).
  *   f1h_cl / f2h_pyr : the CL feature map / pyramid of rnc_fmap_prepare rounded once to halves (rnc_f32_to_f16), same
  *                      element offsets (rnc_pyramid_offset)
  *   f1_cl / f2_pyr   : the fp32 originals, used by the exact CUDA-core kernel for tiles whose lookup windows do not
@@ -125,10 +125,10 @@ typedef enum {
 #define RNC_CONV_BASE_OFFSET 2      /* reserved (round-1 debug switch for the descriptor base_offset; ignored)  */
 #define RNC_CONV_AUX_BLOCKED 16     /* aux0 (z gate) and add are tile-blocked: element (tile, channel c, row r) at ((tile*ld + c)*128 + r) */
 #define RNC_CONV_OUT_BLOCKED 32     /* RNC_EPI_LINEAR: out_f32 in the same tile-blocked layout (produces an `add` operand)          */
-#define RNC_CONV_NO_PAIR 8          /* never use the CTA-pair (cta_group::2) form for this call */
-#define RNC_CONV_SPLIT_N 4          /* 256-column layers as two 128-column items per pixel tile (double-buffered TMEM) */
+#define RNC_CONV_NO_PAIR 8          /* accepted; sm_90 has one (single-CTA) form              */
+#define RNC_CONV_SPLIT_N 4          /* accepted; column tiles are at most 128 wide on sm_90           */
 #define RNC_CONV_WINDOW 128        /* in0 is a sliding-window view of a padded plane, see rnc_conv_umma_desc.win_pitch */
-#define RNC_CONV_TF32 64            /* operands are fp32 hi/lo planes consumed as TF32 (tcgen05 kind::tf32, K = 8): value = hi + lo with
+#define RNC_CONV_TF32 64            /* operands are fp32 hi/lo planes consumed as TF32 (wgmma .tf32, K = 8): value = hi + lo with
                                      * hi = tf32(value), 3 MMAs per K step as in the fp16 form but with fp32's exponent range — the
                                      * training path's layers (output gradients underflow the fp16 split).  The in / w pointers address float
                                      * planes, ld / ktot count floats, K blocks hold 32 channels, only out_f32 is written. */
@@ -148,8 +148,8 @@ typedef struct {
 
 int rnc_conv2d_cl_fwd(const rnc_conv_desc* desc, void* stream);
 
-/* Tensor-core version of rnc_conv2d_cl_fwd (same reference code, same epilogues): tcgen05.mma on fp16 hi/lo split
- * operands with fp32 accumulation in TMEM (3 MMAs per K step: hi*hi + hi*lo + lo*hi), TMA-staged tiles.
+/* Tensor-core version of rnc_conv2d_cl_fwd (same reference code, same epilogues): wgmma on fp16 hi/lo split
+ * operands with fp32 accumulation in registers (3 MMAs per K step: hi*hi + hi*lo + lo*hi), TMA-staged tiles.
  * Activations live as two CL planes of halves (value = hi + lo); weights are pre-split and pre-scaled by a power of two:
  *   w_hi/w_lo : [coutpad][ktot] halves, ktot = kh*kw * nblocks * 64, K index = (tap * nblocks + block) * 64 + c,
  *               blocks enumerate 64-channel slices of segment 0 then segment 1, zero rows for channels beyond Cin

@@ -87,8 +87,7 @@ conv_cl_ffma_kernel(const ConvParams p) {
   };
 
   const int tx = tid & 7, ty = tid >> 3;
-  // accumulators as pairs of adjacent output columns: one packed FFMA2 (fma.rn.f32x2) per pair halves the FMA instruction
-  // count of the 8x8 micro tile (same IEEE fma per element: bit-identical to the scalar form)
+  // accumulators as pairs of adjacent output columns (same IEEE fma per element: bit-identical to the scalar form)
   float2 acc2[8][4];
 #pragma unroll
   for (int i = 0; i < 8; ++i)
@@ -113,7 +112,7 @@ conv_cl_ffma_kernel(const ConvParams p) {
       for (int i = 0; i < 8; ++i) {
         const float2 ai = make_float2(av[i], av[i]);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc2[i][j] = __ffma2_rn(ai, bv2[j], acc2[i][j]);
+        for (int j = 0; j < 4; ++j) acc2[i][j] = ffma2(ai, bv2[j], acc2[i][j]);
       }
     }
     if (kc + 1 < nchunks) store_chunk(buf ^ 1);

@@ -1,6 +1,6 @@
-// tcgen05 implicit-GEMM convolution (v3): persistent CTAs, TMA-staged 128B-swizzled operand rings, tcgen05.mma
-// (kind::f16, M128 x N<=256 x K16) issued by one thread, fp32 accumulators double-buffered in TMEM so that the epilogue
-// of tile i overlaps the main loop of tile i+1.
+// wgmma implicit-GEMM convolution: persistent CTAs, TMA-staged 128B-swizzled operand rings fed by one producer warp, two
+// consumer warpgroups that each issue wgmma (M64 x N<=256 x K16) for 64 of the tile's 128 rows and keep the fp32
+// accumulators in registers, then run the epilogue of the tile themselves.
 // Replaces: core/update.py:33-60 (SepConvGRU), :79-97 (BasicMotionEncoder), :6-14 (FlowHead), :123-126 (mask head), the 3x3
 // layers of core/interp_weights_est.py:10-47 and (stride 1/2, residual epilogue) the convolutions of
 // core/extractor.py:6-56,118-192.
@@ -13,24 +13,29 @@
 // 4-D TMA boxes whose out-of-image elements are zero-filled.  Three A-staging modes cut the L2->SM traffic of the taps:
 //   TAP      one 128-row box per filter tap (any geometry, strides 1 and 2 via TMA element strides)
 //   ROWHALO  tile = 1 image row x 128 px: one (128 + 8)-row box per (ky, channel block); the kw horizontal taps are
-//            operand descriptors shifted by kx rows (descriptor base_offset carries the swizzle phase)
+//            operand descriptors shifted by kx rows
 //   COLHALO  kw == 1: tile = 8 x 16 px with a vertical halo, the kh taps are descriptors shifted by ky*16 rows
 // A fourth input form, RNC_CONV_WINDOW, reads in0 through a sliding-window tensor map (dimension 1 steps fewer bytes than
 // dimension 0 spans): the TMA unit builds im2col rows of a small-Cin layer (the encoders' 7x7/2 stem) without a copy.
-// Epilogue: TMEM -> registers -> per-warp swizzled staging in shared memory -> cp.async.bulk.tensor stores (split halves,
-// fp32 outputs, the GRU state); fused InstanceNorm sums read the staged chunk column-wise.
+// Epilogue: registers -> a staged accumulator tile (thread = pixel) -> per-warp swizzled staging in shared memory ->
+// cp.async.bulk.tensor stores (split halves, fp32 outputs, the GRU state); fused InstanceNorm sums read the staged chunk column-wise.
 #include "umma_ptx.cuh"
 
 namespace rnc {
 namespace umma {
 
-constexpr int kThreads = 320;        // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-9: epilogue (2 per lane group)
+constexpr int kThreads = 288;        // warps 0-7: two consumer warpgroups (wgmma on 64 rows each + epilogue), warp 8: TMA producer
 constexpr int kBM = 128;
 constexpr int kBK = 64;
 constexpr int kMaxSA = 4, kMaxSB = 12;
-constexpr int kStageWarp = 4096;     // epilogue staging per epilogue warp: 32 px x 32 ch as [hi 2 KB | lo 2 KB] halves or 4 KB of fp32
+constexpr int kStageWarp = 4096;     // epilogue staging per consumer warp: 32 px x 32 ch as [hi 2 KB | lo 2 KB] halves or 4 KB of fp32
 constexpr int kStageBytes = 8 * kStageWarp;
-constexpr int kRingBudget = 184 * 1024;   // A + B rings; + barriers, statistics slots and the epilogue staging = 227 KB
+constexpr int kAccCols = 64;         // accumulator columns staged in shared memory per epilogue pass
+constexpr int kAccStride = kAccCols + 4;    // floats per staged pixel row: conflict-free 16-byte reads of a pixel's chunk
+constexpr int kAccBytes = kBM * kAccStride * 4;
+constexpr int kSmemFixed = 1024 + 512 + 8192 + 1024 + kAccBytes + kStageBytes;   // alignment, barriers, statistics, staging
+constexpr int kSmemMax = 226 * 1024;      // 227 KB per block, less the 1 KB the system reserves on sm_90
+constexpr int kRingBudget = kSmemMax - kSmemFixed;   // A + B rings
 enum { MODE_TAP = 0, MODE_ROWHALO = 1, MODE_COLHALO = 2 };
 
 struct Params {
@@ -40,7 +45,7 @@ struct Params {
   int sx;                             // x stride (1 for a window view, whose positions already step by the stride)
   int nblk0, nblk;                    // K blocks (128 bytes of channels: 64 halves or 32 TF32 words) in segment 0 / total
   int bk;                             // channels per K block: 64 (fp16 hi/lo operands) or 32 (TF32 hi/lo operands)
-  int tf32;                           // operands are fp32 planes consumed as TF32 (kind::tf32): training-path layers
+  int tf32;                           // operands are fp32 planes consumed as TF32 (wgmma .tf32): training-path layers
   int a_plane, SA, SB;                // bytes per A half-plane stage (rows*128, 1024-aligned), ring depths
   int resident_b;                     // the layer's whole weight matrix fits the B ring: loaded once per CTA, never released
   int probe_nob;                      // developer probe (RNC_CONV_PROBE_NOB=1): skip the weight loads after the first ring fill
@@ -69,24 +74,46 @@ __device__ __forceinline__ void split8(const float* v, uint4& hi, uint4& lo) {
 template <int BN>
 struct Cfg {
   static constexpr int kBTile = BN * kBK * 2;                     // bytes per half-plane of weights
-  // Each tile owns TWO accumulators: `main` takes the x_hi*w_hi products, `corr` the two 2^-11-smaller cross terms.
-  // The tensor core truncates on every accumulate, so the error grows with the number of full-magnitude adds; keeping
-  // the cross terms out of `main` cuts it 3x (measured: 4.8e-5 -> 1.7e-5 on a 3x3x256 layer).  BN <= 128 double-buffers
-  // the pair (epilogue overlaps the next tile's main loop); wider tiles fit only one pair in the 512 TMEM columns.
-  static constexpr int kBufs = BN <= 128 ? 2 : 1;
-  static constexpr int kTmemCols = BN <= 32 ? 128 : BN <= 64 ? 256 : 512;
+  static constexpr int kChunksN = BN / 32;                        // 32-channel epilogue chunks
+  static constexpr int kPasses = (BN + kAccCols - 1) / kAccCols;  // epilogue passes over the staged accumulator tile
 };
 
-// PAIR: two CTAs of a cluster (adjacent pixel tiles, same weights) run each MMA together (cta_group::2, M = 256): every CTA
-// stages its own A tile and HALF of the weight tile, so the shared-memory fill and operand-read traffic per SM drop by the
-// weight share — the resource that bounds the single-CTA form.  The leader (rank 0) issues all MMAs.
-// EC: epilogue class, compiled separately so that a launch carries only its own epilogue code (the union of all epilogues cost
-// the gate layers instruction-cache misses — 18 % of the epilogue warps' stall samples — and registers): 0 = plain layers
-// (linear / relu / sigmoid), 1 = GRU z|r gates, 2 = GRU q, 3 = the rest (flow append, residual tail, tanh|relu head,
-// coords update, fused InstanceNorm sums).
+// Each thread's accumulators of one 64-row half of the tile: `main` (d[0, BN/2)) takes the x_hi*w_hi products, `corr`
+// (d[BN/2, BN)) the two 2^-11-smaller cross terms.  The tensor core truncates on every accumulate, so the error grows with the
+// number of full-magnitude adds; keeping the cross terms out of `main` cuts it 3x (measured: 4.8e-5 -> 1.7e-5 on a 3x3x256
+// layer).  All three instructions have the same shape, so their accumulator accesses are ordered without a fence.
+template <int BN, bool TF32>
+__device__ __forceinline__ void mma_block(float* d, uint64_t ah, uint64_t al, uint64_t bh, uint64_t bl, int first) {
+  constexpr int kSteps = 4;          // 128 bytes of K per block: 4 x (16 halves | 8 TF32 words)
+#pragma unroll
+  for (int k = 0; k < kSteps; ++k) {
+    const int acc = (first && k == 0) ? 0 : 1;
+    wgmma<BN, TF32>(d, ah + 2 * k, bh + 2 * k, acc);
+    wgmma<BN, TF32>(d + BN / 2, ah + 2 * k, bl + 2 * k, acc);
+    wgmma<BN, TF32>(d + BN / 2, al + 2 * k, bh + 2 * k, 1);
+  }
+}
+
+// Columns [P*64, P*64 + 64) of main + corr (already summed into d[0, BN/2)) -> the staged accumulator tile [128 px][kAccStride] (rows of this warpgroup)
+template <int BN, int P>
+__device__ __forceinline__ void stash_acc(const float* d, float* acc_tile, int row0, int lane) {
+  constexpr int j0 = P * kAccCols / 8, j1 = (P + 1) * kAccCols / 8 < BN / 8 ? (P + 1) * kAccCols / 8 : BN / 8;
+  const int c0 = 2 * (lane & 3);
+#pragma unroll
+  for (int j = j0; j < j1; ++j) {
+    const int col = 8 * j + c0 - P * kAccCols;
+    *reinterpret_cast<float2*>(acc_tile + row0 * kAccStride + col) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(acc_tile + (row0 + 8) * kAccStride + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  }
+}
+
+// EC: epilogue class, compiled separately so that a launch carries only its own epilogue code (the union of all epilogues
+// costs the gate layers instruction-cache misses and registers): 0 = plain layers (linear / relu / sigmoid), 1 = GRU z|r
+// gates, 2 = GRU q, 3 = the rest (flow append, residual tail, tanh|relu head, coords update, fused InstanceNorm sums).
 enum { EC_PLAIN = 0, EC_GRU_ZR = 1, EC_GRU_Q = 2, EC_MISC = 3 };
 
-template <int BN, bool PAIR, int EC>
+// 9 warps: the SM sub-partition holding three of them caps the kernel at 168 registers per thread
+template <int BN, int EC>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant__ CUtensorMap mA0l,
                  const __grid_constant__ CUtensorMap mA1h, const __grid_constant__ CUtensorMap mA1l,
@@ -97,333 +124,214 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
   extern __shared__ unsigned char smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int a_stage = 2 * p.a_plane;
+  constexpr int kBStageBytes = 2 * C::kBTile;                   // [w_hi | w_lo] rows of one K block
   unsigned char* sA = smem;
   unsigned char* sB = smem + p.SA * a_stage;
-  // Pair form of narrow tiles (BN <= 64): an MMA of 64 columns is bound by the issue rate, so the two products that share x_hi
-  // become ONE instruction of 2*BN columns — the leader stages all BN rows of w_hi, its peer all BN rows of w_lo at the same
-  // offset X (a cta_group::2 MMA takes half of its N columns from each CTA: columns [0, BN) = x_hi*w_hi -> main, [BN, 2BN) =
-  // x_hi*w_lo -> corr, adjacent in TMEM) — and x_lo*w_hi reads each CTA's half of w_hi from a second region Y.
-  constexpr bool kFusedPair = PAIR && BN <= 64;
-  constexpr int kBStageBytes = kFusedPair ? C::kBTile + C::kBTile / 2 : PAIR ? C::kBTile : 2 * C::kBTile;   // weight bytes per K block and CTA
   uint64_t* bars = reinterpret_cast<uint64_t*>(sB + p.SB * kBStageBytes);
   uint64_t* a_full = bars;
   uint64_t* a_empty = a_full + kMaxSA;
   uint64_t* b_full = a_empty + kMaxSA;
   uint64_t* b_empty = b_full + kMaxSB;
-  uint64_t* acc_full = b_empty + kMaxSB;
-  uint64_t* acc_empty = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  double* stat_acc = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(bars) + 512);   // [8 warps][kHalfN][32 lanes][2], BN <= 128 only
-  // epilogue staging (TMA-store source), 1024-aligned so the 64B / 128B swizzle patterns are functions of the buffer offset
+  double* stat_acc = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(bars) + 512);   // [8 warps][passes][32 lanes][2]
+  // epilogue staging (TMA-store source), 1024-aligned so the 64B / 128B swizzle patterns are functions of the buffer offset,
+  // then the staged accumulator tile
   unsigned char* stage_base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(bars) + 512 + (BN <= 128 ? 8192 : 0) + 1023) & ~uintptr_t(1023));
+      (reinterpret_cast<uintptr_t>(bars) + 512 + 8192 + 1023) & ~uintptr_t(1023));
+  float* acc_tile = reinterpret_cast<float*>(stage_base + kStageBytes);
 
   pdl_trigger();                       // the next kernel in the stream may begin its prologue on SMs this grid has left
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tpi = p.tiles_x * p.tiles_y;
   const int G = p.mode == MODE_TAP ? p.kh * p.kw : p.mode == MODE_ROWHALO ? p.kh : 1;     // A-stage groups per channel block
   const int T = p.mode == MODE_TAP ? 1 : p.mode == MODE_ROWHALO ? p.kw : p.kh;            // taps sharing one A stage
-  // work items: (pixel tile [pair], column tile); a pair's two CTAs take adjacent pixel tiles of the same item
-  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
-  const bool leader = rank == 0;
-  const int ptiles = PAIR ? (p.ntiles + 1) / 2 : p.ntiles;
-  const int items = ptiles * p.ntn;
-  const int item0 = PAIR ? static_cast<int>(blockIdx.x >> 1) : static_cast<int>(blockIdx.x);
-  const int item_step = PAIR ? static_cast<int>(gridDim.x >> 1) : static_cast<int>(gridDim.x);
-  constexpr int kBHalf = PAIR ? C::kBTile / 2 : C::kBTile;          // bytes of one weight half-plane staged by this CTA
+  const int items = p.ntiles * p.ntn;                                                     // (pixel tile, column tile)
+  const int item0 = static_cast<int>(blockIdx.x), item_step = static_cast<int>(gridDim.x);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int s = 0; s < p.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], PAIR ? 16 : 8); }
+    for (int s = 0; s < p.SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 8); }
+    for (int s = 0; s < p.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) { if (PAIR) tmem_alloc_pair(tmem_slot, C::kTmemCols); else tmem_alloc(tmem_slot, C::kTmemCols); }
-  tcgen05_fence_before();
   __syncthreads();
-  if (PAIR) cluster_sync_all();        // the peer's barriers exist before anything signals them
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                          // everything above overlapped the predecessor's tail; its results are visible from here
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------------------------------------------ TMA producer
-    // The whole warp runs the loop so that addresses / coordinates stay in uniform registers (UTMALDG and UTCHMMA take
-    // uniform operands; a loop under `if (lane == 0)` forces an R2UR chain in front of every issue); one elected lane issues.
-    {
-      // pair: both CTAs' loads complete on the LEADER's full barriers (it alone waits for operands); each CTA recycles its
-      // own stages when the leader's MMA completion reaches its own empty barriers
-      const uint32_t a_full_l = PAIR ? mapa_u32(smem_u32(a_full), 0) : 0u, b_full_l = PAIR ? mapa_u32(smem_u32(b_full), 0) : 0u;
-      // ring positions as (slot, parity) counters: a runtime modulo per stage costs ~100 cycles of dependent integer code in
-      // these single-thread loops, which the 32-cycle MMAs of narrow tiles do not hide
-      int sa_n = 0, pa_n = 0, sb_n = 0, pb_n = 0, b_it = 0;
-      for (int item = item0; item < items; item += item_step) {
-        const int ptile = item / p.ntn, n0 = (item - ptile * p.ntn) * BN;
-        const int tile = PAIR ? ptile * 2 + static_cast<int>(rank) : ptile;     // a ghost tile (odd count) loads zero-filled boxes
-        const int b = tile / tpi, tr = tile - b * tpi;
-        const int y0 = (tr / p.tiles_x) * p.TH, x0 = (tr % p.tiles_x) * p.TW;
-        for (int g = 0; g < G; ++g) {
-          int cx, cy;
-          if (p.mode == MODE_TAP) { cx = x0 * p.sx + g % p.kw - p.pw; cy = y0 * p.stride + g / p.kw - p.ph; }
-          else if (p.mode == MODE_ROWHALO) { cx = x0 - p.pw; cy = y0 + g - p.ph; }
-          else { cx = x0; cy = y0 - p.ph; }
-          for (int cb = 0; cb < p.nblk; ++cb) {
-            const int sa = sa_n, pa = pa_n;
-            if (++sa_n == p.SA) { sa_n = 0; pa_n ^= 1; }
-            mbar_wait(&a_empty[sa], pa ^ 1);
-            const bool seg0 = cb < p.nblk0;
-            const int c = (seg0 ? cb : cb - p.nblk0) * p.bk;
-            if (elect_one()) {
-              if (PAIR) {
-                if (leader) mbar_expect_tx(&a_full[sa], 2 * a_stage);
-                tma_load_4d_pair(sA + sa * a_stage, seg0 ? &mA0h : &mA1h, a_full_l + sa * 8, c, cx, cy, b);
-                tma_load_4d_pair(sA + sa * a_stage + p.a_plane, seg0 ? &mA0l : &mA1l, a_full_l + sa * 8, c, cx, cy, b);
-              } else {
-                mbar_expect_tx(&a_full[sa], a_stage);
-                tma_load_4d(sA + sa * a_stage, seg0 ? &mA0h : &mA1h, &a_full[sa], c, cx, cy, b);
-                tma_load_4d(sA + sa * a_stage + p.a_plane, seg0 ? &mA0l : &mA1l, &a_full[sa], c, cx, cy, b);
-              }
-            }
-            __syncwarp();
-            for (int t = 0; t < T; ++t) {
-              const int tap = p.mode == MODE_TAP ? g : p.mode == MODE_ROWHALO ? g * p.kw + t : t;
-              const int sb = sb_n, pb = pb_n;
-              if (++sb_n == p.SB) { sb_n = 0; pb_n ^= 1; }
-              ++b_it;
-              if (p.resident_b && item != item0) continue;     // weights already resident
-              mbar_wait(&b_empty[sb], pb ^ 1);
-              const int kcol = (tap * p.nblk + cb) * p.bk;
-              if (elect_one()) {
-                if (kFusedPair) {            // X: all BN rows of w_hi (leader) / w_lo (peer) as two half boxes; Y: own half of w_hi
-                  const CUtensorMap* mx = leader ? &mBh : &mBl;
-                  unsigned char* st = sB + sb * kBStageBytes;
-                  if (leader) mbar_expect_tx(&b_full[sb], 2 * kBStageBytes);
-                  tma_load_2d_pair(st, mx, b_full_l + sb * 8, kcol, n0);
-                  tma_load_2d_pair(st + C::kBTile / 2, mx, b_full_l + sb * 8, kcol, n0 + BN / 2);
-                  tma_load_2d_pair(st + C::kBTile, &mBh, b_full_l + sb * 8, kcol, n0 + static_cast<int>(rank) * (BN / 2));
-                } else if (PAIR) {           // this CTA's half of the weight rows, hi and lo planes
-                  const int nrow = n0 + static_cast<int>(rank) * (BN / 2);
-                  if (leader) mbar_expect_tx(&b_full[sb], 2 * kBStageBytes);
-                  tma_load_2d_pair(sB + sb * kBStageBytes, &mBh, b_full_l + sb * 8, kcol, nrow);
-                  tma_load_2d_pair(sB + sb * kBStageBytes + kBHalf, &mBl, b_full_l + sb * 8, kcol, nrow);
-                } else if (p.probe_nob && b_it > p.SB) {
-                  mbar_arrive(&b_full[sb]);
-                } else {
-                  mbar_expect_tx(&b_full[sb], 2 * C::kBTile);
-                  tma_load_2d(sB + sb * 2 * C::kBTile, &mBh, &b_full[sb], kcol, n0);
-                  tma_load_2d(sB + sb * 2 * C::kBTile + C::kBTile, &mBl, &b_full[sb], kcol, n0);
-                }
-              }
-              __syncwarp();
-            }
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (warp-uniform loop, one elected lane issues)
-    if (leader) {
-      // instruction descriptor: D = F32 (bit 4), A/B format bits [7,10) / [10,13): 0 = F16, 2 = TF32; N >> 3 at 17, M >> 4 at 24
-      const uint32_t fmt = p.tf32 ? ((2u << 7) | (2u << 10)) : 0u;
-      const uint32_t idesc = (1u << 4) | fmt | (static_cast<uint32_t>(BN >> 3) << 17) | (static_cast<uint32_t>((PAIR ? 2 * kBM : kBM) >> 4) << 24);
-      const uint32_t idesc2 = (1u << 4) | fmt | (static_cast<uint32_t>((2 * BN <= 256 ? 2 * BN : BN) >> 3) << 17) | (static_cast<uint32_t>(kBM >> 4) << 24);
-      const bool tf32 = p.tf32 != 0;
-      // Operand descriptors differ only in their address field (bits [0,14) = byte address >> 4, stages and tap shifts are
-      // multiples of 16 bytes and shared memory ends below 256 KB): stage 0's descriptor + one multiply-add per use, instead
-      // of rebuilding the 64-bit word from the address in this single-thread loop.  A descriptor whose start is shifted by kx
-      // rows needs no base_offset: with 1024-byte-aligned stages the swizzle is a function of the absolute address.
-      const uint64_t a_desc0 = smem_desc_sw128(smem_u32(sA)), b_desc0 = smem_desc_sw128(smem_u32(sB));
-      const uint32_t a_step = static_cast<uint32_t>(a_stage) >> 4, a_lo = static_cast<uint32_t>(p.a_plane) >> 4;
-      const uint32_t t_step = static_cast<uint32_t>(p.mode == MODE_ROWHALO ? 1 : p.mode == MODE_COLHALO ? p.TW : 0) * 8u;   // tap shift: rows * 128 B >> 4
-      int sa_n = 0, pa_n = 0, sb_n = 0, pb_n = 0, t_it = 0;
-      for (int item = item0; item < items; item += item_step, ++t_it) {
-        const int buf = t_it % C::kBufs, use = t_it / C::kBufs;
-        mbar_wait(&acc_empty[buf], (use & 1) ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_main = tmem_base + buf * 2 * BN, d_corr = d_main + BN;
-        uint32_t acc = 0;
-        for (int g = 0; g < G; ++g)
-          for (int cb = 0; cb < p.nblk; ++cb) {
-            const int sa = sa_n, pa = pa_n;
-            if (++sa_n == p.SA) { sa_n = 0; pa_n ^= 1; }
-            mbar_wait(&a_full[sa], pa);
-            for (int t = 0; t < T; ++t) {
-              const int sb = sb_n, pb = pb_n;
-              if (++sb_n == p.SB) { sb_n = 0; pb_n ^= 1; }
-              mbar_wait(&b_full[sb], p.resident_b ? 0 : pb);
-              tcgen05_fence_after();
-              const uint64_t ah = a_desc0 + (sa * a_step + t * t_step), al = ah + a_lo;
-              const uint64_t bh = b_desc0 + sb * (kBStageBytes >> 4), bl = bh + (kBHalf >> 4);
-              if (elect_one()) {
-                if (kFusedPair) {
-                  const uint64_t bx = bh, by = bh + (C::kBTile >> 4);
-                  const uint32_t idesc_x = (1u << 4) | fmt | (static_cast<uint32_t>((2 * BN) >> 3) << 17) | (static_cast<uint32_t>((2 * kBM) >> 4) << 24);
-#pragma unroll
-                  for (int k = 0; k < kBK / 16; ++k) {
-                    if (tf32) {
-                      umma_tf32_pair(d_main, ah + 2 * k, bx + 2 * k, idesc_x, k == 0 ? acc : 1u);     // main | corr
-                      umma_tf32_pair(d_corr, al + 2 * k, by + 2 * k, idesc, 1);
-                    } else {
-                      umma_f16_pair(d_main, ah + 2 * k, bx + 2 * k, idesc_x, k == 0 ? acc : 1u);      // main | corr
-                      umma_f16_pair(d_corr, al + 2 * k, by + 2 * k, idesc, 1);
-                    }
-                  }
-                  if (!p.resident_b) umma_commit_pair(&b_empty[sb]);
-                } else if (PAIR) {
-                  // M = 256 across the pair: each CTA's tensor core reads its own A rows and both CTAs' weight halves
-#pragma unroll
-                  for (int k = 0; k < kBK / 16; ++k) {     // 4 K steps of 32 bytes per 128-byte block (16 halves or 8 TF32 words)
-                    if (tf32) {
-                      umma_tf32_pair(d_main, ah + 2 * k, bh + 2 * k, idesc, k == 0 ? acc : 1u);
-                      umma_tf32_pair(d_corr, ah + 2 * k, bl + 2 * k, idesc, k == 0 ? acc : 1u);
-                      umma_tf32_pair(d_corr, al + 2 * k, bh + 2 * k, idesc, 1);
-                    } else {
-                      umma_f16_pair(d_main, ah + 2 * k, bh + 2 * k, idesc, k == 0 ? acc : 1u);
-                      umma_f16_pair(d_corr, ah + 2 * k, bl + 2 * k, idesc, k == 0 ? acc : 1u);
-                      umma_f16_pair(d_corr, al + 2 * k, bh + 2 * k, idesc, 1);
-                    }
-                  }
-                  if (!p.resident_b) umma_commit_pair(&b_empty[sb]);
-                } else {
-                  if (BN <= 128) {
-                    // The hi and lo weight planes are adjacent in the stage and `main`, `corr` adjacent in TMEM, so
-                    // x_hi * [w_hi | w_lo] is ONE instruction of 2*BN columns: x_hi is fetched from shared memory once
-                    // instead of twice (a 128-column instruction needs the full 128 B/clk of shared-memory bandwidth).
-#pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k) {
-                      if (tf32) {
-                        umma_tf32(d_main, ah + 2 * k, bh + 2 * k, idesc2, k == 0 ? acc : 1u);
-                        umma_tf32(d_corr, al + 2 * k, bh + 2 * k, idesc, 1);
-                      } else {
-                        umma_f16(d_main, ah + 2 * k, bh + 2 * k, idesc2, k == 0 ? acc : 1u);
-                        umma_f16(d_corr, al + 2 * k, bh + 2 * k, idesc, 1);
-                      }
-                    }
-                  } else {
-#pragma unroll
-                    for (int k = 0; k < kBK / 16; ++k) {
-                      if (tf32) {
-                        umma_tf32(d_main, ah + 2 * k, bh + 2 * k, idesc, k == 0 ? acc : 1u);
-                        umma_tf32(d_corr, ah + 2 * k, bl + 2 * k, idesc, k == 0 ? acc : 1u);
-                        umma_tf32(d_corr, al + 2 * k, bh + 2 * k, idesc, 1);
-                      } else {
-                        umma_f16(d_main, ah + 2 * k, bh + 2 * k, idesc, k == 0 ? acc : 1u);
-                        umma_f16(d_corr, ah + 2 * k, bl + 2 * k, idesc, k == 0 ? acc : 1u);
-                        umma_f16(d_corr, al + 2 * k, bh + 2 * k, idesc, 1);
-                      }
-                    }
-                  }
-                  if (!p.resident_b) umma_commit(&b_empty[sb]);
-                }
-              }
-              __syncwarp();
-              acc = 1;
-            }
-            if (elect_one()) { if (PAIR) umma_commit_pair(&a_empty[sa]); else umma_commit(&a_empty[sa]); }
-            __syncwarp();
-          }
-        if (elect_one()) { if (PAIR) umma_commit_pair(&acc_full[buf]); else umma_commit(&acc_full[buf]); }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue: TMEM -> registers -> global
-    const int lg = warp & 3;                       // TMEM lane group this warp may access
-    const int ml = lg * 32 + lane;                 // row of the tile = pixel
-    const int epi = p.epilogue;
-    constexpr int kChunksN = BN / 32, kHalfN = (kChunksN + 1) / 2;
-    const int cc0 = (warp - 2) < 4 ? 0 : kHalfN, cc1 = (warp - 2) < 4 ? kHalfN : kChunksN;
-    const bool use_stats = EC == EC_MISC && BN <= 128 && p.stats != nullptr;
-    double* my_acc = stat_acc + (static_cast<size_t>(warp - 2) * kHalfN * 32 + lane) * 2;   // [chunk] stride 64 doubles
-    int acc_b = -1, acc_n0 = 0;
-    auto flush_stats = [&]() {
-      if (acc_b < 0) return;
-      for (int ci = 0; ci < cc1 - cc0; ++ci) {
-        const int ch = acc_n0 + (cc0 + ci) * 32 + lane;
-        if (ch < p.cout) {
-          double* dst = p.stats + (static_cast<size_t>(acc_b) * p.cout + ch) * 2;
-          atomicAdd(dst, my_acc[ci * 64]);
-          atomicAdd(dst + 1, my_acc[ci * 64 + 1]);
-        }
-        my_acc[ci * 64] = 0.0; my_acc[ci * 64 + 1] = 0.0;
-      }
-    };
-    if (use_stats) {
-      for (int ci = 0; ci < kHalfN; ++ci) { my_acc[ci * 64] = 0.0; my_acc[ci * 64 + 1] = 0.0; }
-    }
-    const uint32_t acc_empty_l = PAIR ? mapa_u32(smem_u32(acc_empty), 0) : 0u;     // the leader's MMA warp waits for both CTAs
-    // Outputs leave through shared memory and TMA stores: a warp's 32 px x 32 ch chunk is one box of the output tensor
-    // (full 64- / 128-byte rows per pixel instead of 16-byte pieces per thread; image borders and ghost tiles are clipped by
-    // the TMA unit).  The staging rows are written with the map's swizzle (64B for halves, 128B for fp32): conflict-free.
-    unsigned char* stg = stage_base + (warp - 2) * kStageWarp;
-    bool stg_busy = false;                         // warp-uniform: a TMA store may still be reading the staging buffer
-    const int lgx = (lg * 32) % p.TW, lgy = (lg * 32) / p.TW;
-    int bx = 0, by = 0, bb = 0;                    // box origin of this warp's lane group in the current tile
-    auto stage_free = [&]() {
-      if (stg_busy) { if (lane == 0) bulk_wait_read0(); __syncwarp(); stg_busy = false; }
-    };
-    auto store_split = [&](const float* v, int ch) {           // hi/lo halves of v[0..32) -> channels [ch, ch+32) of out_hi / out_lo
-      stage_free();
-      uint4* sh = reinterpret_cast<uint4*>(stg + lane * 64);
-      uint4* sl = reinterpret_cast<uint4*>(stg + 2048 + lane * 64);
-      const int sw = (lane >> 1) & 3;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) split8(v + 8 * q, sh[q ^ sw], sl[q ^ sw]);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) {
-        tma_store_4d(&mOh, stg, ch, bx, by, bb);
-        tma_store_4d(&mOl, stg + 2048, ch, bx, by, bb);
-        bulk_commit();
-      }
-      stg_busy = true;
-    };
-    auto store_f32 = [&](const float* v, int ch) {             // fp32 v[0..32) -> channels [ch, ch+32) of h (q gate) / out_f32
-      stage_free();
-      float4* sf = reinterpret_cast<float4*>(stg + lane * 128);
-      const int sw = lane & 7;
-#pragma unroll
-      for (int q = 0; q < 8; ++q) sf[q ^ sw] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-      fence_proxy_async();
-      __syncwarp();
-      if (lane == 0) { tma_store_4d(&mOf, stg, ch, bx, by, bb); bulk_commit(); }
-      stg_busy = true;
-    };
-    int t_it = 0;
-    for (int item = item0; item < items; item += item_step, ++t_it) {
-      const int ptile = item / p.ntn, n0 = (item - ptile * p.ntn) * BN;
-      const int tile = PAIR ? ptile * 2 + static_cast<int>(rank) : ptile;
+    // The whole warp runs the loop so that addresses / coordinates stay in uniform registers; one elected lane issues.
+    // Ring positions are (slot, parity) counters: a runtime modulo per stage costs ~100 cycles of dependent integer code.
+    int sa_n = 0, pa_n = 0, sb_n = 0, pb_n = 0, b_it = 0;
+    for (int item = item0; item < items; item += item_step) {
+      const int tile = item / p.ntn, n0 = (item - tile * p.ntn) * BN;
       const int b = tile / tpi, tr = tile - b * tpi;
-      const bool ghost = tile >= p.ntiles;                     // odd tile count: the pair's second CTA idles through this item
-      if (use_stats && !ghost && (b != acc_b || n0 != acc_n0)) { flush_stats(); acc_b = b; acc_n0 = n0; }
-      const int ty0 = (tr / p.tiles_x) * p.TH, tx0 = (tr % p.tiles_x) * p.TW;
-      const int y = ty0 + ml / p.TW, x = tx0 + ml % p.TW;
-      const bool valid = !ghost && y < p.H && x < p.W;
-      bx = tx0 + lgx; by = ty0 + lgy; bb = b;                  // a ghost tile has b >= B: its boxes are clipped whole
-      // tile-blocked tensors (p.aux_blocked / p.out_blocked): element (tile, channel c, row ml) at ((tile * ld + c) * 128 + ml),
-      // so a warp's 32 pixels are contiguous per channel
-      const size_t pix = (static_cast<size_t>(b) * p.H + y) * p.W + x;
-      const int buf = t_it % C::kBufs, use = t_it / C::kBufs;
-      mbar_wait(&acc_full[buf], use & 1);
-      tcgen05_fence_after();
-      // two epilogue warps per TMEM lane group: the first takes the lower half of the 32-channel chunks, the second the rest
-#pragma unroll 1
-      for (int cc = cc0; cc < cc1; ++cc) {
-        const int n = n0 + cc * 32;
-        if (n >= p.cout + (EC == EC_MISC && epi == RNC_EPI_RELU_FLOW ? 2 : 0)) break;   // warp-uniform
-        uint32_t r[32], rc[32];
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(lg * 32) << 16) + buf * 2 * BN + cc * 32;
-        tmem_ld32(taddr, r);
-        tmem_ld32(taddr + BN, rc);
-        if (ghost) continue;                                           // warp-uniform: nothing to add to the statistics either
+      const int y0 = (tr / p.tiles_x) * p.TH, x0 = (tr % p.tiles_x) * p.TW;
+      for (int g = 0; g < G; ++g) {
+        int cx, cy;
+        if (p.mode == MODE_TAP) { cx = x0 * p.sx + g % p.kw - p.pw; cy = y0 * p.stride + g / p.kw - p.ph; }
+        else if (p.mode == MODE_ROWHALO) { cx = x0 - p.pw; cy = y0 + g - p.ph; }
+        else { cx = x0; cy = y0 - p.ph; }
+        for (int cb = 0; cb < p.nblk; ++cb) {
+          const int sa = sa_n, pa = pa_n;
+          if (++sa_n == p.SA) { sa_n = 0; pa_n ^= 1; }
+          mbar_wait(&a_empty[sa], pa ^ 1);
+          const bool seg0 = cb < p.nblk0;
+          const int c = (seg0 ? cb : cb - p.nblk0) * p.bk;
+          if (elect_one()) {
+            mbar_expect_tx(&a_full[sa], a_stage);
+            tma_load_4d(sA + sa * a_stage, seg0 ? &mA0h : &mA1h, &a_full[sa], c, cx, cy, b);
+            tma_load_4d(sA + sa * a_stage + p.a_plane, seg0 ? &mA0l : &mA1l, &a_full[sa], c, cx, cy, b);
+          }
+          __syncwarp();
+          for (int t = 0; t < T; ++t) {
+            const int tap = p.mode == MODE_TAP ? g : p.mode == MODE_ROWHALO ? g * p.kw + t : t;
+            const int sb = sb_n, pb = pb_n;
+            if (++sb_n == p.SB) { sb_n = 0; pb_n ^= 1; }
+            ++b_it;
+            if (p.resident_b && item != item0) continue;     // weights already resident
+            mbar_wait(&b_empty[sb], pb ^ 1);
+            const int kcol = (tap * p.nblk + cb) * p.bk;
+            if (elect_one()) {
+              if (p.probe_nob && b_it > p.SB) {
+                mbar_arrive(&b_full[sb]);
+              } else {
+                mbar_expect_tx(&b_full[sb], kBStageBytes);
+                tma_load_2d(sB + sb * kBStageBytes, &mBh, &b_full[sb], kcol, n0);
+                tma_load_2d(sB + sb * kBStageBytes + C::kBTile, &mBl, &b_full[sb], kcol, n0);
+              }
+            }
+            __syncwarp();
+          }
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers: wgmma main loop, then the epilogue
+  const int wg = warp >> 2;                        // warpgroup: rows [64 wg, 64 wg + 64) of the tile
+  const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // accumulator rows row0, row0 + 8 of this thread
+  float d[BN];                                     // main | corr
+  const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
+  const uint32_t t_rows = p.mode == MODE_ROWHALO ? 1u : p.mode == MODE_COLHALO ? static_cast<uint32_t>(p.TW) : 0u;   // tap shift in rows
+
+  // epilogue: thread = pixel; warp w takes lane group w & 3 (pixels 32 (w & 3) + lane), half h = w >> 2 takes the chunks
+  // 2 * pass + h of the staged accumulator columns
+  const int lg = warp & 3, hsel = warp >> 2;
+  const int ml = lg * 32 + lane;
+  const int epi = p.epilogue;
+  const bool use_stats = EC == EC_MISC && p.stats != nullptr;
+  double* my_acc = stat_acc + (static_cast<size_t>(warp) * C::kPasses * 32 + lane) * 2;   // [pass] stride 64 doubles
+  int acc_b = -1, acc_n0 = 0;
+  auto flush_stats = [&]() {
+    if (acc_b < 0) return;
+    for (int ci = 0; ci < C::kPasses; ++ci) {
+      const int ch = acc_n0 + (2 * ci + hsel) * 32 + lane;
+      if (2 * ci + hsel < C::kChunksN && ch < p.cout) {
+        double* dst = p.stats + (static_cast<size_t>(acc_b) * p.cout + ch) * 2;
+        atomicAdd(dst, my_acc[ci * 64]);
+        atomicAdd(dst + 1, my_acc[ci * 64 + 1]);
+      }
+      my_acc[ci * 64] = 0.0; my_acc[ci * 64 + 1] = 0.0;
+    }
+  };
+  if (use_stats) {
+    for (int ci = 0; ci < C::kPasses; ++ci) { my_acc[ci * 64] = 0.0; my_acc[ci * 64 + 1] = 0.0; }
+  }
+  // Outputs leave through shared memory and TMA stores: a warp's 32 px x 32 ch chunk is one box of the output tensor
+  // (full 64- / 128-byte rows per pixel instead of 16-byte pieces per thread; image borders are clipped by the TMA unit).
+  // The staging rows are written with the map's swizzle (64B for halves, 128B for fp32): conflict-free.
+  unsigned char* stg = stage_base + warp * kStageWarp;
+  bool stg_busy = false;                           // warp-uniform: a TMA store may still be reading the staging buffer
+  const int lgx = (lg * 32) % p.TW, lgy = (lg * 32) / p.TW;
+  int bx = 0, by = 0, bb = 0;                      // box origin of this warp's lane group in the current tile
+  auto stage_free = [&]() {
+    if (stg_busy) { if (lane == 0) bulk_wait_read0(); __syncwarp(); stg_busy = false; }
+  };
+  auto store_split = [&](const float* v, int ch) {           // hi/lo halves of v[0..32) -> channels [ch, ch+32) of out_hi / out_lo
+    stage_free();
+    uint4* sh = reinterpret_cast<uint4*>(stg + lane * 64);
+    uint4* sl = reinterpret_cast<uint4*>(stg + 2048 + lane * 64);
+    const int sw = (lane >> 1) & 3;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) split8(v + 8 * q, sh[q ^ sw], sl[q ^ sw]);
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) {
+      tma_store_4d(&mOh, stg, ch, bx, by, bb);
+      tma_store_4d(&mOl, stg + 2048, ch, bx, by, bb);
+      bulk_commit();
+    }
+    stg_busy = true;
+  };
+  auto store_f32 = [&](const float* v, int ch) {             // fp32 v[0..32) -> channels [ch, ch+32) of h (q gate) / out_f32
+    stage_free();
+    float4* sf = reinterpret_cast<float4*>(stg + lane * 128);
+    const int sw = lane & 7;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) sf[q ^ sw] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    fence_proxy_async();
+    __syncwarp();
+    if (lane == 0) { tma_store_4d(&mOf, stg, ch, bx, by, bb); bulk_commit(); }
+    stg_busy = true;
+  };
+
+  int sa_n = 0, pa_n = 0, sb_n = 0, pb_n = 0;
+  for (int item = item0; item < items; item += item_step) {
+    const int tile = item / p.ntn, n0 = (item - tile * p.ntn) * BN;
+    // ---- main loop: K = taps x channel blocks, one wgmma batch per weight stage
+    int first = 1;
+    for (int g = 0; g < G; ++g)
+      for (int cb = 0; cb < p.nblk; ++cb) {
+        const int sa = sa_n, pa = pa_n;
+        if (++sa_n == p.SA) { sa_n = 0; pa_n ^= 1; }
+        mbar_wait(&a_full[sa], pa);
+        for (int t = 0; t < T; ++t) {
+          const int sb = sb_n, pb = pb_n;
+          if (++sb_n == p.SB) { sb_n = 0; pb_n ^= 1; }
+          mbar_wait(&b_full[sb], p.resident_b ? 0 : pb);
+          // A rows of this warpgroup, shifted by the tap (ROWHALO: kx rows, COLHALO: ky image rows of TW pixels)
+          const uint32_t a_addr = sA_u + sa * a_stage + (64u * wg + t * t_rows) * 128u;
+          // no base_offset: with 1024-byte aligned stages the swizzle is a function of the absolute address
+          const uint64_t ah = smem_desc_sw128(a_addr);
+          const uint64_t al = ah + (static_cast<uint32_t>(p.a_plane) >> 4);
+          const uint64_t bh = smem_desc_sw128(sB_u + sb * kBStageBytes), bl = bh + (C::kBTile >> 4);
+          wgmma_fence();
+          if (p.tf32) mma_block<BN, true>(d, ah, al, bh, bl, first); else mma_block<BN, false>(d, ah, al, bh, bl, first);
+          wgmma_commit();
+          wgmma_wait<0>();
+          first = 0;
+          __syncwarp();
+          if (!p.resident_b && lane == 0) mbar_arrive(&b_empty[sb]);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&a_empty[sa]);
+      }
+#pragma unroll
+    for (int i = 0; i < BN; ++i) reg_fence(d[i]);
+    // main + corr once, so that only half of the accumulator registers stay live through the epilogue passes
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) d[i] += d[BN / 2 + i];
+
+    // ---- epilogue
+    const int b = tile / tpi, tr = tile - b * tpi;
+    if (use_stats && (b != acc_b || n0 != acc_n0)) { flush_stats(); acc_b = b; acc_n0 = n0; }
+    const int ty0 = (tr / p.tiles_x) * p.TH, tx0 = (tr % p.tiles_x) * p.TW;
+    const int y = ty0 + ml / p.TW, x = tx0 + ml % p.TW;
+    const bool valid = y < p.H && x < p.W;
+    bx = tx0 + lgx; by = ty0 + lgy; bb = b;
+    // tile-blocked tensors (p.aux_blocked / p.out_blocked): element (tile, channel c, row ml) at ((tile * ld + c) * 128 + ml),
+    // so a warp's 32 pixels are contiguous per channel
+    const size_t pix = (static_cast<size_t>(b) * p.H + y) * p.W + x;
+    auto chunk = [&](int pass, int cc) {
+      const int n = n0 + cc * 32;
         float v[32];
+        const float4* sv = reinterpret_cast<const float4*>(acc_tile + ml * kAccStride + (cc - 2 * pass) * 32);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
-          const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + n) + q);
-          v[4 * q + 0] = fmaf(__uint_as_float(r[4 * q + 0]) + __uint_as_float(rc[4 * q + 0]), p.unscale, bv.x);
-          v[4 * q + 1] = fmaf(__uint_as_float(r[4 * q + 1]) + __uint_as_float(rc[4 * q + 1]), p.unscale, bv.y);
-          v[4 * q + 2] = fmaf(__uint_as_float(r[4 * q + 2]) + __uint_as_float(rc[4 * q + 2]), p.unscale, bv.z);
-          v[4 * q + 3] = fmaf(__uint_as_float(r[4 * q + 3]) + __uint_as_float(rc[4 * q + 3]), p.unscale, bv.w);
+          const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + n) + q), s = sv[q];
+          v[4 * q + 0] = fmaf(s.x, p.unscale, bv.x);
+          v[4 * q + 1] = fmaf(s.y, p.unscale, bv.y);
+          v[4 * q + 2] = fmaf(s.z, p.unscale, bv.z);
+          v[4 * q + 3] = fmaf(s.w, p.unscale, bv.w);
         }
         if (p.add != nullptr && valid) {
           // hoisted part of the layer (input channels that are constant across calls), computed once by another launch
@@ -460,9 +368,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
             s1 += x;
             s2 = fmaf(x, x, s2);
           }
-          my_acc[(cc - cc0) * 64] += static_cast<double>(s1);
-          my_acc[(cc - cc0) * 64 + 1] += static_cast<double>(s2);
-          continue;
+          my_acc[pass * 64] += static_cast<double>(s1);
+          my_acc[pass * 64 + 1] += static_cast<double>(s2);
+          return;
         }
         if (EC == EC_GRU_ZR) {
           const int Ch = p.cout >> 1;
@@ -492,7 +400,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
             }
             store_split(v, n - Ch);
           }
-          continue;
+          return;
         }
         if (EC == EC_MISC && epi == RNC_EPI_FLOW_DELTA) {
           // FlowHead.conv2 + `coords1 = coords1 + delta_flow` (update.py:14, raft_nc_dbl.py:157); only channels 0,1 are real
@@ -503,7 +411,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
             p.aux0[i0 + HW] += v[1];
             if (p.out_f32) { p.out_f32[i0] = v[0]; p.out_f32[i0 + HW] = v[1]; }
           }
-          continue;
+          return;
         }
         bool want_f32 = p.out_f32 != nullptr;
         if (EC == EC_GRU_Q) {
@@ -597,24 +505,19 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
           }
         }
         if (p.out_hi) store_split(v, n);
-      }
-      // this warp has finished reading the accumulator buffer (tcgen05.wait::ld inside tmem_ld32)
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) { if (PAIR) mbar_arrive_cluster(acc_empty_l + buf * 8); else mbar_arrive(&acc_empty[buf]); }
+    };
+#pragma unroll 1
+    for (int pass = 0; pass < C::kPasses; ++pass) {
+      named_bar_sync(1, 256);                      // every consumer warp is done with the staged tile of the previous pass
+      if (pass == 0) stash_acc<BN, 0>(d, acc_tile, row0, lane);
+      else if (C::kPasses > 1) stash_acc<BN, (C::kPasses > 1 ? 1 : 0)>(d, acc_tile, row0, lane);
+      named_bar_sync(1, 256);
+      const int cc = 2 * pass + hsel;
+      if (cc < C::kChunksN && n0 + cc * 32 < p.cout + (EC == EC_MISC && epi == RNC_EPI_RELU_FLOW ? 2 : 0)) chunk(pass, cc);
     }
-    if (use_stats) flush_stats();
-    if (lane == 0) bulk_wait_all0();               // the staging buffer must outlive its TMA stores; their writes complete here
   }
-
-  // ------------------------------------------------------------------ teardown
-  tcgen05_fence_before();
-  __syncthreads();
-  if (PAIR) cluster_sync_all();        // the peer may still be multicasting to this CTA's barriers / reading its weight half
-  if (warp == 1) {
-    tcgen05_fence_after();
-    if (PAIR) tmem_dealloc_pair(tmem_base, C::kTmemCols); else tmem_dealloc(tmem_base, C::kTmemCols);
-  }
+  if (use_stats) flush_stats();
+  if (lane == 0) bulk_wait_all0();                 // the staging buffer must outlive its TMA stores; their writes complete here
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -662,79 +565,52 @@ static int sm_count() {
   if (!n) {
     int dev = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
   }
   return n;
 }
 
-template <int BN, bool PAIR, int EC>
+template <int BN, int EC>
 static int launch(const CUtensorMap* maps, Params& p, cudaStream_t stream, int max_sa, int max_sb) {
   using C = Cfg<BN>;
   const int a_stage = 2 * p.a_plane;
-  // ring depths within kRingBudget: both rings hide the same TMA latency, so deepen A (up to 4) while B keeps >= 3 stages
-  // a pair's CTA stages half of the weight rows; narrow pair tiles: a whole plane + half of w_hi (see the kernel)
-  const int budget = kRingBudget, b_stage = (PAIR && BN <= 64) ? C::kBTile * 3 / 2 : PAIR ? C::kBTile : 2 * C::kBTile;
+  // ring depths within kRingBudget: both rings hide the same TMA latency, so deepen A (up to 4) while B keeps >= 2 stages
+  const int budget = kRingBudget, b_stage = 2 * C::kBTile;
   const int sa_cap = max_sa > 0 && max_sa < kMaxSA ? max_sa : kMaxSA;      // debug knobs (rnc_conv_umma_desc.flags bits 8-15)
   p.SA = 2;
-  while (p.SA < sa_cap && budget - (p.SA + 1) * a_stage >= 3 * b_stage) ++p.SA;
+  while (p.SA < sa_cap && budget - (p.SA + 1) * a_stage >= 2 * b_stage) ++p.SA;
   int sb = (budget - p.SA * a_stage) / b_stage;
   p.SB = sb > 8 ? 8 : sb < 2 ? 2 : sb;
   if (max_sb > 0 && p.SB > max_sb) p.SB = max_sb;
   // Small layers (64 -> 64 3x3: 9 stages of 16 KB): keep the whole weight matrix in the ring for the CTA's lifetime instead
-  // of re-streaming it for every pixel tile (the shared-memory fill bandwidth is what bounds narrow tiles).
+  // of re-streaming it for every pixel tile.
   p.resident_b = 0;
   {
     const int nb = p.kh * p.kw * p.nblk;
-    const int hard = 227 * 1024 - 1024 - 512 - 8192 - 1024 - kStageBytes;
-    if (p.ntn == 1 && nb <= kMaxSB && nb > p.SB && max_sb == 0 && 2 * a_stage + nb * b_stage <= hard) {
-      p.resident_b = 1; p.SB = nb; p.SA = (hard - nb * b_stage) / a_stage;
+    if (p.ntn == 1 && nb <= kMaxSB && nb > p.SB && max_sb == 0 && 2 * a_stage + nb * b_stage <= kRingBudget) {
+      p.resident_b = 1; p.SB = nb; p.SA = (kRingBudget - nb * b_stage) / a_stage;
       if (p.SA > kMaxSA) p.SA = kMaxSA;
     }
   }
-  // + alignment slack, barriers, fp64 statistics slots, 1024-aligned epilogue staging
-  const int smem = p.SA * a_stage + p.SB * b_stage + 1024 + 512 + (BN <= 128 ? 8192 : 0) + 1024 + kStageBytes;
-  if (smem > 227 * 1024) return RNC_ERR_UNSUPPORTED;
+  const int smem = p.SA * a_stage + p.SB * b_stage + kSmemFixed;
+  if (smem > kSmemMax) return RNC_ERR_UNSUPPORTED;
   static unsigned long long done = 0;
-  if (int st = ensure_dyn_smem(conv_umma_kernel<BN, PAIR, EC>, 227 * 1024, &done)) return st;
-  const int items = (PAIR ? (p.ntiles + 1) / 2 : p.ntiles) * p.ntn;
-  const int slots = PAIR ? sm_count() / 2 : sm_count();
-  const int grid = (items < slots ? items : slots) * (PAIR ? 2 : 1);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  if (PAIR) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 2; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attr; cfg.numAttrs = na;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, conv_umma_kernel<BN, PAIR, EC>, maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], maps[6], maps[7],
-                                     maps[8], p);
-  if (e != cudaSuccess) { g_last_cuda_error = static_cast<int>(e); return RNC_ERR_CUDA; }
+  if (int st = ensure_dyn_smem(conv_umma_kernel<BN, EC>, kSmemMax, &done)) return st;
+  const int items = p.ntiles * p.ntn;
+  const int grid = items < sm_count() ? items : sm_count();
+  cudaError_t e = launch_pdl(conv_umma_kernel<BN, EC>, dim3(grid), dim3(kThreads), smem, stream, maps[0], maps[1], maps[2], maps[3],
+                             maps[4], maps[5], maps[6], maps[7], maps[8], p);
+  if (e != cudaSuccess) { cudaGetLastError(); g_last_cuda_error = static_cast<int>(e); return RNC_ERR_CUDA; }
   return after_launch();
 }
 
-template <bool PAIR, int EC>
+template <int EC>
 static int launch_bn(int bn, const CUtensorMap* maps, Params& p, cudaStream_t s, int msa, int msb) {
   switch (bn) {
-    case 32: return launch<32, PAIR, EC>(maps, p, s, msa, msb);
-    case 64: return launch<64, PAIR, EC>(maps, p, s, msa, msb);
-    case 128: return launch<128, PAIR, EC>(maps, p, s, msa, msb);
-    case 192: return launch<192, PAIR, EC>(maps, p, s, msa, msb);
-    default: return launch<256, PAIR, EC>(maps, p, s, msa, msb);
+    case 32: return launch<32, EC>(maps, p, s, msa, msb);
+    case 64: return launch<64, EC>(maps, p, s, msa, msb);
+    default: return launch<128, EC>(maps, p, s, msa, msb);
   }
-}
-
-// CTA-pair (cta_group::2) form of the convolution: the default; RNC_CONV_PAIR=0 selects the single-CTA form
-static bool pair_enabled() {
-  static const int on = [] { const char* e = getenv("RNC_CONV_PAIR"); return (e && e[0] == '0') ? 0 : 1; }();
-  return on != 0;
 }
 
 }  // namespace umma
@@ -757,39 +633,30 @@ extern "C" long long rnc_conv_umma_tiles(int kh, int kw, int stride, int B, int 
 }
 
 // Column-tile width.  The widest tile that divides coutpad is the default; a narrower one (more, smaller work items per
-// pixel tile) wins when the grid is under-filled (small batches: 56 pixel tiles on 148 SMs), when the tile count just
-// misses a multiple of the SM count (448 tiles = 4 rounds of 256 columns but 7 half-size rounds), or when K is so short
-// that the single-buffered 256-column epilogue dominates (1x1 layers).  Cost model in K-step units, fitted to B200
-// measurements (tools/bn_probe.py): per K-step 1.0 / 0.77 / 0.53 / 0.36 / 0.30 for 256 / 192 / 128 / 64 / 32 columns, + 3
-// K-steps of exposed epilogue for tiles wider than 128 columns (one TMEM accumulator pair), + 0.5 per item, x1.08 when the
-// A tile is loaded more than once.
+// pixel tile) wins when the grid is under-filled (small batches: 56 pixel tiles on 132 SMs) or when the tile count just
+// misses a multiple of the SM count.  Tiles are at most 128 columns: the main and correction accumulators of a 128-column
+// tile already take 128 registers per consumer thread.  Cost model in K-step units: per K-step 1.0 / 0.68 / 0.57 for
+// 128 / 64 / 32 columns (operand bytes per K-step: the A tile plus the weight tile), + 0.5 per item, x1.08 when the A tile
+// is loaded more than once.
 static int choose_bn(const rnc_conv_umma_desc& d, int bn_max, int stride) {
-  if (d.flags & RNC_CONV_SPLIT_N) return bn_max == 256 ? 128 : bn_max;
+  if (d.flags & RNC_CONV_SPLIT_N) return bn_max;
   const int bkc = (d.flags & RNC_CONV_TF32) ? 32 : 64;
   const int taps = d.kh * d.kw, ksteps = taps * ((d.c0 + bkc - 1) / bkc + (d.c1 + bkc - 1) / bkc);
   int TW, TH;
-  if (stride == 1 && (d.flags & RNC_CONV_NO_HALO) == 0 && d.kw > 1 && d.W > 64) { TW = 128; TH = 1; }
-  else if (stride == 1 && (d.flags & RNC_CONV_NO_HALO) == 0 && d.kw == 1 && d.kh > 1 && d.W >= 16 && d.H >= 8) { TW = 16; TH = 8; }
-  else { TW = 8; while (TW < d.W && TW < umma::kBM) TW <<= 1; TH = umma::kBM / TW; }
+  tile_shape(d.kh, d.kw, stride, d.H, d.W, d.flags, TW, TH);
   const long ntiles = static_cast<long>(d.B) * ((d.W + TW - 1) / TW) * ((d.H + TH - 1) / TH);
-  // CTA-pair form (fitted to the same probe): the pair's leader waits for both CTAs' epilogues, so a single-buffered
-  // (> 128 columns) tile exposes ~12 K-steps per item, while narrow tiles no longer sit on the shared-memory bandwidth
-  const bool pair = umma::pair_enabled() && (d.flags & RNC_CONV_NO_PAIR) == 0;
-  static const int cand[5] = {256, 192, 128, 64, 32};
-  static const float per_k1[5] = {1.0f, 0.77f, 0.53f, 0.36f, 0.30f}, per_k2[5] = {1.0f, 0.8f, 0.6f, 0.40f, 0.34f};
-  const float* per_k = pair ? per_k2 : per_k1;
-  const float expose = pair ? 12.0f : 3.0f, per_item = pair ? 1.2f : 0.5f;
-  const long slots = pair ? umma::sm_count() / 2 : umma::sm_count();
-  const long ptiles = pair ? (ntiles + 1) / 2 : ntiles;
+  static const int cand[3] = {128, 64, 32};
+  static const float per_k[3] = {1.0f, 0.68f, 0.57f};
+  const long slots = umma::sm_count();
   int best = bn_max;
   float best_cost = 1e30f;
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < 3; ++i) {
     const int bn = cand[i];
     if (bn > bn_max || d.coutpad % bn != 0) continue;
     if ((d.epilogue == RNC_EPI_TANH_RELU || d.epilogue == RNC_EPI_GRU_ZR) && bn < 64) continue;
     const int ntn = d.coutpad / bn;
-    const long rounds = (ptiles * ntn + slots - 1) / slots;
-    float item = ksteps * per_k[i] + per_item + (bn > 128 ? expose * bn / 256.0f : 0.f);
+    const long rounds = (ntiles * ntn + slots - 1) / slots;
+    float item = ksteps * per_k[i] + 0.5f;
     if (ntn > 1) item *= 1.08f;
     const float cost = rounds * item;
     if (cost < best_cost * 0.97f) { best_cost = cost; best = bn; }     // wider wins near-ties
@@ -820,11 +687,10 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
   const int nblk0 = (d.c0 + bk - 1) / bk, nblk1 = (d.c1 + bk - 1) / bk, nblk = nblk0 + nblk1;
   const int ntaps = d.kh * d.kw;
   if (d.ktot != ntaps * nblk * bk) return RNC_ERR_BAD_SHAPE;           // weight planes are [coutpad][taps * blocks * bk]
-  int bn;
-  if (d.coutpad <= 32) bn = 32; else if (d.coutpad <= 64) bn = 64; else if (d.coutpad <= 128) bn = 128;
-  else if (d.coutpad % 192 == 0) bn = 192; else bn = 256;
-  // a single CTA stages whole weight tiles: two 64 KB stages of a 256-column tile no longer fit beside the epilogue staging
-  if (bn == 256 && !(umma::pair_enabled() && (d.flags & RNC_CONV_NO_PAIR) == 0)) bn = 128;
+  const int bn0 = d.coutpad <= 32 ? 32 : d.coutpad <= 64 ? 64 : 128;
+  int bn = bn0;
+  while (bn > 32 && d.coutpad % bn != 0) bn >>= 1;            // the widest column tile that divides coutpad
+  if (d.coutpad % bn != 0) bn = bn0;
   if (d.coutpad % bn == 0 && d.epilogue != RNC_EPI_RELU_FLOW && d.epilogue != RNC_EPI_FLOW_DELTA)
     bn = choose_bn(d, bn, stride);
   if (d.coutpad % bn != 0 || d.coutpad < d.cout) return RNC_ERR_BAD_SHAPE;
@@ -885,6 +751,9 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
   p.tiles_x = (d.W + TW - 1) / TW; p.tiles_y = (d.H + TH - 1) / TH;
   p.ntiles = d.B * p.tiles_x * p.tiles_y; p.ntn = d.coutpad / bn;
   p.a_plane = box_w * box_h * 128;
+  // tall halo boxes (COLHALO, kh >= 5) beside 128-column weight stages leave no room for two stages of each ring
+  while (bn > 32 && 2 * 2 * p.a_plane + 2 * 2 * bn * bk * (tf32 ? 4 : 2) > kRingBudget && d.coutpad % (bn >> 1) == 0) bn >>= 1;
+  p.ntn = d.coutpad / bn;
   p.nblk0 = nblk0; p.nblk = nblk; p.bk = bk; p.tf32 = tf32 ? 1 : 0;
   p.cout = d.cout; p.epilogue = d.epilogue; p.unscale = d.unscale; p.bias = d.bias;
   p.out_f32 = d.out_f32; p.ldo_f32 = d.ldo_f32;
@@ -907,10 +776,9 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
   } else {
     maps[2] = maps[0]; maps[3] = maps[1];
   }
-  const bool pair = umma::pair_enabled() && (d.flags & RNC_CONV_NO_PAIR) == 0;
-  ok = ok && make_w_map(&maps[4], d.w_hi, d.ktot, d.coutpad, pair ? bn / 2 : bn, tf32) &&
-       make_w_map(&maps[5], d.w_lo, d.ktot, d.coutpad, pair ? bn / 2 : bn, tf32);
-  // epilogue stores: out_hi / out_lo (and h for the q gate) as boxes of 32 channels x one TMEM lane group's pixels
+  ok = ok && make_w_map(&maps[4], d.w_hi, d.ktot, d.coutpad, bn, tf32) &&
+       make_w_map(&maps[5], d.w_lo, d.ktot, d.coutpad, bn, tf32);
+  // epilogue stores: out_hi / out_lo (and h for the q gate) as boxes of 32 channels x one epilogue warp's 32 pixels
   {
     const int obw = TW < 32 ? TW : 32, obh = 32 / obw;
     const int flow2 = d.epilogue == RNC_EPI_RELU_FLOW ? 2 : 0;
@@ -939,18 +807,10 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
   const int msa = (d.flags >> 8) & 15, msb = (d.flags >> 12) & 15;
   const bool plain = (d.epilogue == RNC_EPI_LINEAR || d.epilogue == RNC_EPI_RELU || d.epilogue == RNC_EPI_SIGMOID) && !d.stats;
   const int ec = d.epilogue == RNC_EPI_GRU_ZR ? EC_GRU_ZR : d.epilogue == RNC_EPI_GRU_Q ? EC_GRU_Q : plain ? EC_PLAIN : EC_MISC;
-  if (pair) {
-    switch (ec) {
-      case EC_GRU_ZR: return launch_bn<true, EC_GRU_ZR>(bn, maps, p, s, msa, msb);
-      case EC_GRU_Q: return launch_bn<true, EC_GRU_Q>(bn, maps, p, s, msa, msb);
-      case EC_MISC: return launch_bn<true, EC_MISC>(bn, maps, p, s, msa, msb);
-      default: return launch_bn<true, EC_PLAIN>(bn, maps, p, s, msa, msb);
-    }
-  }
   switch (ec) {
-    case EC_GRU_ZR: return launch_bn<false, EC_GRU_ZR>(bn, maps, p, s, msa, msb);
-    case EC_GRU_Q: return launch_bn<false, EC_GRU_Q>(bn, maps, p, s, msa, msb);
-    case EC_MISC: return launch_bn<false, EC_MISC>(bn, maps, p, s, msa, msb);
-    default: return launch_bn<false, EC_PLAIN>(bn, maps, p, s, msa, msb);
+    case EC_GRU_ZR: return launch_bn<EC_GRU_ZR>(bn, maps, p, s, msa, msb);
+    case EC_GRU_Q: return launch_bn<EC_GRU_Q>(bn, maps, p, s, msa, msb);
+    case EC_MISC: return launch_bn<EC_MISC>(bn, maps, p, s, msa, msb);
+    default: return launch_bn<EC_PLAIN>(bn, maps, p, s, msa, msb);
   }
 }

@@ -1,36 +1,33 @@
 // Tensor-core fused correlation lookup (v2 of corr_lookup.cu; same math, SURVEY.md Appendix A.1; replaces
 // core/corr.py:7-55 + core/utils/utils.py:59-73).  The 4-D volume is never built: per tile of 8x16 query pixels the
-// kernel computes, on tcgen05, the dot products of the tile's 128 fmap1 vectors against a bounding box of fmap2^l
+// kernel computes, with wgmma, the dot products of the tile's 128 fmap1 vectors against a bounding box of fmap2^l
 // positions that covers every pixel's 10x10 lattice window, then each pixel gathers its own window from the
 // accumulator and blends it bilinearly.
 //
 //   A  = fmap1 tile      [128 px][256 ch] halves, TMA box {64,16,8,1} x 4 K-blocks, resident while its levels are processed
-//   B  = fmap2^l box     chunks of <= 256 positions x 256 ch streamed through a ring of 32 KB stages as 2-row TMA boxes
-//                        {64, BW, 2, 1}; only the box rows some window needs are loaded and multiplied (N is set per chunk);
-//                        out-of-image positions are zero-filled by TMA = the reference's zero padding (grid_sample
-//                        padding_mode='zeros')
-//   D  = [128][<=256] fp32 in TMEM, double buffered: the MMA warp fills one chunk while the epilogue drains the other
+//   B  = fmap2^l box     chunks of <= 128 positions x 256 ch streamed through a ring of 16 KB stages as TMA boxes of the
+//                        needed rows {64, BW, rows, 1}; only the box rows some window needs are loaded and multiplied (N is
+//                        set per chunk); out-of-image positions are zero-filled by TMA = the reference's zero padding
+//                        (grid_sample padding_mode='zeros')
+//   D  = [128][<=128] fp32 in the registers of one warpgroup (two M = 64 halves), staged to shared memory per chunk
 //
-// Persistent CTAs (one per SM) walk work units (tile, level); producer / MMA / epilogue warps are decoupled by mbarrier
-// rings, so the loads and MMAs of the next unit overlap the epilogue of the current one (see the kernel's comment).
+// Persistent CTAs (one per SM) walk work units (tile, level); a producer warp and the consumer warpgroup are decoupled by
+// mbarrier rings, so the loads of the next chunks and units overlap the MMAs and the epilogue of the current one.
 //
-// Epilogue (thread = pixel = TMEM lane): two box rows (BW columns each) at a time are read with tcgen05.ld and parked in
-// a thread-private shared-memory row (128-bit stores; dynamic addressing is what shared memory is needed for), the 10
-// lattice values of the pixel's window row are read back, interpolated in x, combined with the previous row in y -> 9
-// outputs (fixed j, i = 0..8), which are split into hi/lo halves (the tcgen05 convolutions' operand format) and stored
-// straight into the level's output tile in shared memory; the tile leaves with one TMA store per plane and warp.
+// Epilogue (thread = pixel): the chunk's accumulator is staged as [pixel][129 words] (odd pitch: the gather's scalar loads
+// of 32 pixels hit distinct banks); each pixel reads the 10 lattice values of its window row, interpolates in x, combines
+// with the previous row in y -> 9 outputs (fixed j, i = 0..8), which are split into hi/lo halves (the tensor-core
+// convolutions' operand format) and stored straight into the level's output tile in shared memory; the tile leaves with one
+// TMA store per plane and warp.
 //
 // Output channel order inside a level (kLvlStride = 88 channels; consumed only by convc1, whose weights are permuted to
 // match at pack time — the reference order k = i*9 + j exists only in the seam API, corr_lookup.cu):
 //     tap (i, j), i < 8  ->  j*8 + i          tap (8, j)  ->  72 + j          81..87 = zero pads
-// so the 8 values a thread produces per window row are ONE aligned 16-byte store per plane (conflict-free at the 176-byte
-// pixel pitch) instead of 9 scattered words, and no second pass re-reads / re-packs the level.
+// so the 8 values a thread produces per window row are ONE aligned 16-byte store per plane instead of 9 scattered words,
+// and no second pass re-reads / re-packs the level.
 //
 // Units whose windows do not fit the fixed boxes (incoherent flow) are flagged and recomputed exactly in fp32 by the same
 // CTA after its tensor-core units (exact_unit), so the result never depends on the coherence assumption.
-//
-// Measured on B200 (B=8, 55x128, profiles/): the three engines are balanced within 2x of each other — L2->SM operand
-// traffic ~45 us, tensor pipe ~45 us, epilogue ~70 us per launch when each runs alone, ~95 us together.
 //
 // Precision: fmaps are rounded once to fp16 (fp32 accumulate): 2.4e-4 EPE after 32 iterations in SURVEY.md Appendix D.
 #include <type_traits>
@@ -42,75 +39,37 @@ namespace lookup_umma {
 
 using namespace rnc::umma;
 
-// RNC_LOOKUP_EPI2=1 (compile-time variant): TWO epilogue warps per TMEM lane group share every accumulator chunk — the rows a
-// chunk holds for the lane group are cut in half, the halves alternate between the two warps from chunk to chunk (so each warp's
-// rows are consecutive across a chunk boundary and its y-blend state carries over; the warp taking a second half re-derives the
-// x-interpolated row in front of it), one box row per step with a one-row scratch each.  Bit-identical results; measured on
-// B200 at B=8: 67.1 us per launch against 67.0 us for the default one-warp form (two rows per step) — after the round-2 rework
-// the kernel is bound by its TMA feed (loads alone ~40 us, loads + MMA ~54 us), not by the epilogue any more, so the default
-// stays the simpler form.
-#ifndef RNC_LOOKUP_EPI2
-#define RNC_LOOKUP_EPI2 0
-#endif
-constexpr int kEpiWarps = RNC_LOOKUP_EPI2 ? 8 : 4;
-constexpr int kThreads = 64 + 32 * kEpiWarps;   // warp 0 TMA, warp 1 MMA + TMEM, then the epilogue warps
+constexpr int kThreads = 160;            // warps 0-3: consumer warpgroup (wgmma + epilogue, thread = pixel), warp 4: TMA producer
 constexpr int kTY = 8, kTX = 16;         // query tile (level-0 pixels)
 constexpr int kD = 256;                  // feature channels
 constexpr int kKB = kD / 64;             // K blocks of 64 halves
 constexpr int kLevels = 4;
 constexpr int kS = 9, kG = 10, kR = 4;
-// per-level box: width, rows per chunk, chunks   (union boxes seen on the benchmark stimuli at iteration 31: 28x24, 19x17,
-// 15x14, 13x12; anything larger is handled by the exact fallback kernel)
-// boxes: 32x24, 24x20, 16x16, 16x14 positions = chunks of 256, 240, 256, 224 MMA columns
-#ifndef RNC_LOOKUP_CHUNKN
-#define RNC_LOOKUP_CHUNKN 192    // 3 stages of 24 KB beat 2 of 32 KB (70.6 vs 75.9 us per B=8 launch): more loads in flight
-#endif
+// per-level box: width, rows per chunk, chunks.  Union boxes seen on the benchmark stimuli at iteration 31: 28x24, 19x17,
+// 15x14, 13x12; anything larger is handled by the exact fallback.  Chunks of <= 128 MMA columns (the accumulator of 128
+// pixels x 128 columns is 128 registers per consumer thread): 4x32, 4x24, 8x16, 8x16 positions; boxes 32x24, 24x24, 16x24.
 __host__ __device__ constexpr int box_w(int l) { return l == 0 ? 32 : l == 1 ? 24 : 16; }
-#if RNC_LOOKUP_CHUNKN == 256
-__host__ __device__ constexpr int chunk_rows(int l) { return l == 0 ? 8 : l == 1 ? 10 : l == 2 ? 16 : 14; }
-__host__ __device__ constexpr int n_chunks(int l) { return l == 0 ? 3 : l == 1 ? 2 : 1; }
-#else   // chunks of <= 192 MMA columns (24 KB stages: a third stage fits): 6x32, 8x24, 12x16, 12x16
-__host__ __device__ constexpr int chunk_rows(int l) { return l == 0 ? 6 : l == 1 ? 8 : 12; }
-__host__ __device__ constexpr int n_chunks(int l) { return l == 0 ? 4 : l == 1 ? 3 : 2; }
-#endif
+__host__ __device__ constexpr int chunk_rows(int l) { return l <= 1 ? 4 : 8; }
+__host__ __device__ constexpr int n_chunks(int l) { return l <= 1 ? 6 : 3; }
 __host__ __device__ constexpr int box_h(int l) { return chunk_rows(l) * n_chunks(l); }
 __host__ __device__ constexpr int chunk_n(int l) { return box_w(l) * chunk_rows(l); }
-static_assert(chunk_rows(0) <= 16 && chunk_rows(1) <= 16 && chunk_rows(2) <= 16 && chunk_rows(3) <= 16, "one box kind per even row count");
-#ifndef RNC_LOOKUP_L2HINT
-#define RNC_LOOKUP_L2HINT 0      // evict_last on the feature loads measured 3 % slower on B200 (81.6 vs 78.8 us per B=8 launch)
-#endif
-#ifndef RNC_LOOKUP_STAGES
-#define RNC_LOOKUP_STAGES (RNC_LOOKUP_CHUNKN == 192 ? 3 : 2)
-#endif
-constexpr int kStages = RNC_LOOKUP_STAGES;   // B ring (a third stage does not fit beside the two-row scratch and measures the same)
+constexpr int kChunkN = 128;
+static_assert(chunk_n(0) <= kChunkN && chunk_n(1) <= kChunkN && chunk_n(2) <= kChunkN, "chunk wider than the accumulator");
+constexpr int kStages = 3;               // B ring
 constexpr int kATile = 128 * 64 * 2;     // 16 KB per K block
-constexpr int kBStage = RNC_LOOKUP_CHUNKN * 64 * 2;    // 32 KB: 256 positions x 64 halves (24 KB with 192-column chunks)
+constexpr int kBStage = kChunkN * 64 * 2;    // 16 KB: 128 positions x 64 halves
 constexpr int kLvlStride = 88;           // channels per level in the output row (81 taps + 7 zero pads): 16-byte groups
-#ifndef RNC_LOOKUP_TIRING
-#define RNC_LOOKUP_TIRING 4
-#endif
-constexpr int kTiRing = RNC_LOOKUP_TIRING;    // unit records in flight between the producer and its consumers (power of two)
-constexpr int kTiShift = kTiRing == 2 ? 1 : kTiRing == 4 ? 2 : 3;
+constexpr int kTiRing = 4;               // unit records in flight between the producer and the consumers (power of two)
+constexpr int kTiShift = 2;
 constexpr int kSmemA = kKB * kATile;                         // 64 KB
-constexpr int kSmemB = kStages * kBStage;                    // 64 KB
-// Epilogue buffers are pixel-major with 16-byte aligned rows, so a thread moves its data with 128-bit accesses:
-//   scratch [pixel][68]: two box rows (32 words each) of the accumulator; 68 = 4*17 -> the 8 lanes of a quarter warp hit
-//                        8 distinct bank quads
-// scratch [pixel][68] words: two box rows (32 words each); the pixels of the odd tile row of a warp are skewed by 16 words, so
-// that the gather's scalar loads (lane address = 68*pixel + skew + window offset, window offset ~ pixel's x) hit 32 distinct
-// banks: bank = 5*lane + spread (mod 32)
-constexpr int kScrStride = RNC_LOOKUP_EPI2 ? 36 : 68, kScrSkew = 16;   // one (EPI2) or two box rows of 32 words + 4: 36 = 68 = 4 (mod 32)
-constexpr int kScrWarp = 32 * kScrStride + kScrSkew;         // words per epilogue warp (its 16 skewed pixels run 16 words past 32*68)
-constexpr int kSmemScratch = kEpiWarps * kScrWarp * 4;       // 34.25 KB (4 warps x two rows) / 36.5 KB (8 warps x one row)
+constexpr int kSmemB = kStages * kBStage;                    // 48 KB
 // output tile of one (tile, level) unit: [plane hi | lo][128 px][88 halves], dense = the TMA store's box {88, 16, 2} per warp
 constexpr int kStgPlane = 128 * kLvlStride * 2;              // 22 KB
 constexpr int kSmemStage = 2 * kStgPlane;                    // 44 KB
-static_assert(kSmemScratch % 128 == 0 && (32 * kLvlStride * 2) % 128 == 0, "TMA store sources must be 128-byte aligned");
-#ifdef RNC_PROBE_NOEPI
-constexpr int kSmemTotal = kSmemA + kSmemB + 1024 + 512;     // probe: the epilogue buffers are never touched
-#else
-constexpr int kSmemTotal = kSmemA + kSmemB + kSmemScratch + kSmemStage + 1024 + 512;
-#endif
+constexpr int kAccPitch = kChunkN + 1;                       // words per pixel of the staged accumulator chunk
+constexpr int kSmemAcc = 128 * kAccPitch * 4;                // 64.5 KB
+static_assert((32 * kLvlStride * 2) % 128 == 0, "TMA store sources must be 128-byte aligned");
+constexpr int kSmemTotal = kSmemA + kSmemB + kSmemStage + kSmemAcc + 1024 + 512;
 
 struct Params {
   const float* f1_cl; const float* f2_pyr;   // fp32 originals: exact path of the units whose windows do not fit the boxes
@@ -122,9 +81,9 @@ struct Params {
   float scale;
 };
 
-// fmap2^l boxes of every even row count up to 16 per level: the rows a chunk needs are ONE TMA operation (the per-operation
-// cost dominates: 2-row boxes measured 49.6 us per B=8 launch for the loads alone, whole-chunk boxes 40.9 us with more bytes)
-constexpr int kBoxKinds = 8;
+// fmap2^l boxes of every even row count up to the chunk height per level: the rows a chunk needs are ONE TMA operation
+constexpr int kBoxKinds = 4;
+static_assert(2 * kBoxKinds >= chunk_rows(0) && 2 * kBoxKinds >= chunk_rows(2), "a box kind per even row count of a chunk");
 struct LevelMaps { CUtensorMap m[kLevels][kBoxKinds]; };
 
 struct TileInfo {                      // shared: origin of the unit's union box (0,0 when no window is live), the box rows
@@ -140,24 +99,78 @@ __device__ __forceinline__ bool window_origin(float cx, float cy, float inv, int
 
 __device__ __forceinline__ float clamp_coord(float v) { return fminf(fmaxf(v, -1.0e6f), 1.0e6f); }
 
-struct EpiCtx {
-  const Params& p; const TileInfo* ti; float* scratch; __half* stage; uint64_t* acc_full; uint64_t* acc_empty;
-  uint32_t tmem_base; int b, y0, x0, lg, ml, lane; bool valid; float cx, cy;
-  int team;                            // EPI2: 0 / 1 = first / second epilogue warp of the lane group
+// The consumer warpgroup's view of the operand rings and of the staged accumulator.
+struct MmaCtx {
+  uint32_t a_base, b_base;
+  uint64_t* a_full; uint64_t* a_empty; uint64_t* b_full; uint64_t* b_empty;
+  float* acc;                          // [128 px][kAccPitch]
+  int it, na;                          // B ring position, A tile uses
 };
 
-template <int BW>
-__device__ __forceinline__ void tmem_row_issue(uint32_t taddr, uint32_t* v) {
-  if (BW > 16) tmem_ld32_issue(taddr, v); else tmem_ld16_issue(taddr, v);
+struct EpiCtx {
+  const Params& p; const TileInfo* ti; __half* stage;
+  int b, y0, x0, lg, ml, lane; bool valid; float cx, cy;
+  bool load_a, free_a;                 // the unit's first chunk waits for the A tile / its last chunk releases it
+};
+
+// Accumulator rows of one chunk: N columns = the positions of the rows the chunk holds (two M = 64 halves), K = 256.
+template <int N>
+__device__ __forceinline__ void chunk_mma(MmaCtx& m, float* d0, float* d1, bool wait_a, bool free_a) {
+  for (int kb = 0; kb < kKB; ++kb, ++m.it) {
+    const int s = m.it % kStages, ph = (m.it / kStages) & 1;
+    if (wait_a) mbar_wait(&m.a_full[kb], m.na & 1);
+    mbar_wait(&m.b_full[s], ph);
+    const uint64_t ad = smem_desc_sw128(m.a_base + kb * kATile), bd = smem_desc_sw128(m.b_base + s * kBStage);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      wgmma<N, false>(d0, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0);
+      wgmma<N, false>(d1, ad + (64 * 128 >> 4) + 2 * kk, bd + 2 * kk, (kb | kk) != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) {
+      mbar_arrive(&m.b_empty[s]);
+      if (free_a) mbar_arrive(&m.a_empty[kb]);   // this K block of A is free for the next tile
+    }
+  }
 }
 
-// Rows of one level (box width BW columns) for the warp's 32 pixels: two box rows per step, so that two independent
-// store -> gather -> interpolate chains are in flight for the single epilogue warp of each scheduler.
+// One chunk: MMAs into registers, then the accumulator -> shared memory [pixel][column] (every consumer thread first waits
+// until all have finished reading the previous chunk).
+__device__ __forceinline__ void chunk_acc(MmaCtx& m, int nn, bool wait_a, bool free_a) {
+  float d0[kChunkN / 2], d1[kChunkN / 2];
+  switch (nn) {
+    case 32: chunk_mma<32>(m, d0, d1, wait_a, free_a); break;
+    case 48: chunk_mma<48>(m, d0, d1, wait_a, free_a); break;
+    case 64: chunk_mma<64>(m, d0, d1, wait_a, free_a); break;
+    case 96: chunk_mma<96>(m, d0, d1, wait_a, free_a); break;
+    default: chunk_mma<128>(m, d0, d1, wait_a, free_a); break;
+  }
+#pragma unroll
+  for (int i = 0; i < kChunkN / 2; ++i) { reg_fence(d0[i]); reg_fence(d1[i]); }
+  named_bar_sync(1, 128);
+  const int lane = threadIdx.x & 31, r = 16 * (threadIdx.x >> 5) + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+  for (int j = 0; j < kChunkN / 8; ++j) {
+    if (8 * j >= nn) break;
+    float* p0 = m.acc + r * kAccPitch + 8 * j + c;
+    p0[0] = d0[4 * j]; p0[1] = d0[4 * j + 1];
+    p0[8 * kAccPitch] = d0[4 * j + 2]; p0[8 * kAccPitch + 1] = d0[4 * j + 3];
+    float* p1 = p0 + 64 * kAccPitch;
+    p1[0] = d1[4 * j]; p1[1] = d1[4 * j + 1];
+    p1[8 * kAccPitch] = d1[4 * j + 2]; p1[8 * kAccPitch + 1] = d1[4 * j + 3];
+  }
+  named_bar_sync(1, 128);
+}
+
+// Rows of one level (box width BW columns) for the warp's 32 pixels, two box rows per step, so that two independent
+// gather -> interpolate chains are in flight.
 template <int BW>
-__device__ __forceinline__ void lookup_level_rows(const EpiCtx& c, int& ch, int l, bool live, int ox, int oy, float ax, float ay) {
+__device__ __forceinline__ void lookup_level_rows(const EpiCtx& c, MmaCtx& m, int l, bool live, int ox, int oy, float ax, float ay) {
   const Params& p = c.p;
   const int cr = chunk_rows(l);
-  float* sc = c.scratch + c.lg * kScrWarp + c.lane * kScrStride + (c.lane >> 4) * kScrSkew;   // thread-private: two box rows of 32 words
   __half* sth = c.stage + c.ml * kLvlStride;                  // this pixel's row of the level's output tile, hi plane
   __half* stl = sth + 128 * kLvlStride;                       // lo plane
   // window row j of this pixel is complete: taps (0..7, j) -> one 16-byte store per plane, tap (8, j) -> the tail
@@ -179,18 +192,19 @@ __device__ __forceinline__ void lookup_level_rows(const EpiCtx& c, int& ch, int 
   float hprev[kS];
 #pragma unroll
   for (int i = 0; i < kS; ++i) hprev[i] = 0.f;
-  const float* gp = sc + (live ? ox : 0);
+  const float* gbase = m.acc + c.ml * kAccPitch + (live ? ox : 0);
 
-  // one step: box rows `row`, `row + 1` (TWO) are in the scratch; cidx = lattice row of the pixel's window held by `row`
-  auto step = [&](int row, auto two_tag) {
+  // one step: chunk rows r, r + 1 (TWO); cidx = lattice row of the pixel's window held by box row `row`
+  auto step = [&](int r, int row, auto two_tag) {
     constexpr bool TWO = decltype(two_tag)::value;
+    const float* gp = gbase + r * BW;
     const int cidx = row - oy;
     float g0[kG], g1[kG], h0[kS], h1[kS];
 #pragma unroll
     for (int a = 0; a < kG; ++a) g0[a] = gp[a];
     if (TWO) {
 #pragma unroll
-      for (int a = 0; a < kG; ++a) g1[a] = gp[32 + a];
+      for (int a = 0; a < kG; ++a) g1[a] = gp[BW + a];
     }
 #pragma unroll
     for (int i = 0; i < kS; ++i) h0[i] = wx0 * g0[i] + wx1 * g0[i + 1];
@@ -213,130 +227,21 @@ __device__ __forceinline__ void lookup_level_rows(const EpiCtx& c, int& ch, int 
 #pragma unroll
     for (int i = 0; i < kS; ++i) hprev[i] = TWO ? h1[i] : h0[i];
   };
-  auto park = [&](const uint32_t* v, int half) {
-#pragma unroll
-    for (int g4 = 0; g4 < BW / 4; ++g4)
-      *reinterpret_cast<uint4*>(sc + half * 32 + 4 * g4) = make_uint4(v[4 * g4], v[4 * g4 + 1], v[4 * g4 + 2], v[4 * g4 + 3]);
-  };
 
   const int nch = (c.ti->nrows + cr - 1) / cr;
-  for (int cc = 0; cc < nch; ++cc, ++ch) {
-    const int buf = ch & 1, use = ch >> 1;
-    mbar_wait(&c.acc_full[buf], use & 1);
-    tcgen05_fence_after();
+  for (int cc = 0; cc < nch; ++cc) {
+    const int nn = min(cr, c.ti->nrows - cc * cr) * BW;
+    chunk_acc(m, nn, cc == 0 && c.load_a, cc == nch - 1 && c.free_a);
     const int r0 = max(0, row_lo - cc * cr), r1 = min(cr - 1, row_hi - cc * cr);   // rows of this chunk the warp needs
-    const uint32_t tbase = c.tmem_base + (static_cast<uint32_t>(c.lg * 32) << 16) + buf * 256;
-#ifdef RNC_PROBE_NOEPI
-    if (false) {
-#else
-    if (r0 <= r1) {
-#endif
-      // software pipeline: the TMEM loads of the next two rows are in flight while this pair is processed
-      uint32_t va[32] = {}, vb[32] = {};
-      tmem_row_issue<BW>(tbase + r0 * BW, va);
-      if (r0 + 1 <= r1) tmem_row_issue<BW>(tbase + (r0 + 1) * BW, vb);
-      tmem_ld_wait32(va);
-      tmem_ld_wait32(vb);
-      for (int r = r0; r <= r1; r += 2) {
-        const bool two = r + 1 <= r1, more = r + 2 <= r1;
-        park(va, 0);
-        if (two) park(vb, 1);
-        if (more) tmem_row_issue<BW>(tbase + (r + 2) * BW, va);
-        if (r + 3 <= r1) tmem_row_issue<BW>(tbase + (r + 3) * BW, vb);
-        if (two) step(cc * cr + r, std::true_type{}); else step(cc * cr + r, std::false_type{});
-        if (more) { tmem_ld_wait32(va); tmem_ld_wait32(vb); }
-      }
+    for (int r = r0; r <= r1; r += 2) {
+      if (r + 1 <= r1) step(r, cc * cr + r, std::true_type{}); else step(r, cc * cr + r, std::false_type{});
     }
-    // all of this warp's reads of the TMEM buffer are complete
-    tcgen05_fence_before();
-    __syncwarp();
-    if (c.lane == 0) mbar_arrive(&c.acc_empty[buf]);
   }
 }
 
-#if RNC_LOOKUP_EPI2
-// Rows of one level for one of the lane group's two warps (see RNC_LOOKUP_EPI2 above): one box row per step.
-template <int BW>
-__device__ __forceinline__ void lookup_level_rows2(const EpiCtx& c, int& ch, int l, bool live, int ox, int oy, float ax, float ay) {
-  const Params& p = c.p;
-  const int cr = chunk_rows(l);
-  float* sc = c.scratch + (c.team * 4 + c.lg) * kScrWarp + c.lane * kScrStride + (c.lane >> 4) * kScrSkew;   // one box row of 32 words
-  __half* sth = c.stage + c.ml * kLvlStride;
-  __half* stl = sth + 128 * kLvlStride;
-  auto emit = [&](int j, const float (&o)[kS]) {
-    uint32_t hh[4], ll[4];
-#pragma unroll
-    for (int q = 0; q < 4; ++q) split_pair(o[2 * q], o[2 * q + 1], hh[q], ll[q]);
-    *reinterpret_cast<uint4*>(sth + j * 8) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-    *reinterpret_cast<uint4*>(stl + j * 8) = make_uint4(ll[0], ll[1], ll[2], ll[3]);
-    uint32_t h8, l8;
-    split_pair(o[8], 0.f, h8, l8);
-    reinterpret_cast<unsigned short*>(sth)[72 + j] = static_cast<unsigned short>(h8 & 0xffffu);
-    reinterpret_cast<unsigned short*>(stl)[72 + j] = static_cast<unsigned short>(l8 & 0xffffu);
-  };
-  const float wx1 = ax * p.scale, wx0 = p.scale - wx1, wy0 = 1.f - ay;
-  const int row_lo = __reduce_min_sync(0xffffffffu, live ? oy : 0x7fffffff);
-  const int row_hi = __reduce_max_sync(0xffffffffu, live ? oy + kG - 1 : -1);
-  float hprev[kS];
-#pragma unroll
-  for (int i = 0; i < kS; ++i) hprev[i] = 0.f;
-  const float* gp = sc + (live ? ox : 0);
-  // one box row: x-interpolate; unless it only primes the y-blend state, blend with the previous row and store window row cidx-1
-  auto step = [&](const uint32_t* v, int row, bool prime) {
-#pragma unroll
-    for (int g4 = 0; g4 < BW / 4; ++g4)
-      *reinterpret_cast<uint4*>(sc + 4 * g4) = make_uint4(v[4 * g4], v[4 * g4 + 1], v[4 * g4 + 2], v[4 * g4 + 3]);
-    const int cidx = row - oy;
-    float g[kG], h[kS];
-#pragma unroll
-    for (int a = 0; a < kG; ++a) g[a] = gp[a];
-#pragma unroll
-    for (int i = 0; i < kS; ++i) h[i] = wx0 * g[i] + wx1 * g[i + 1];
-    if (!prime && live && cidx >= 1 && cidx < kG) {
-      float o[kS];
-#pragma unroll
-      for (int i = 0; i < kS; ++i) o[i] = wy0 * hprev[i] + ay * h[i];
-      emit(cidx - 1, o);
-    }
-#pragma unroll
-    for (int i = 0; i < kS; ++i) hprev[i] = h[i];
-  };
-
-  const int nch = (c.ti->nrows + cr - 1) / cr;
-  for (int cc = 0; cc < nch; ++cc, ++ch) {
-    const int buf = ch & 1, use = ch >> 1;
-    mbar_wait(&c.acc_full[buf], use & 1);
-    tcgen05_fence_after();
-    const int r0 = max(0, row_lo - cc * cr), r1 = min(cr - 1, row_hi - cc * cr);   // rows of this chunk the lane group needs
-    const uint32_t tbase = c.tmem_base + (static_cast<uint32_t>(c.lg * 32) << 16) + buf * 256;
-    if (r0 <= r1) {
-      // halves alternate between the two warps: role 0 = first half (continues this warp's rows of the previous chunk),
-      // role 1 = second half (re-derives the row in front of it to prime hprev)
-      const int role = (cc & 1) ^ c.team, nfirst = (r1 - r0 + 2) >> 1;
-      const int a = role == 0 ? r0 : r0 + nfirst - 1, b = role == 0 ? r0 + nfirst - 1 : r1;   // role 1 starts on its priming row
-      uint32_t va[32] = {}, vb[32] = {};
-      tmem_row_issue<BW>(tbase + a * BW, va);
-      for (int r = a; r <= b; r += 2) {
-        tmem_ld_wait32(va);
-        if (r + 1 <= b) tmem_row_issue<BW>(tbase + (r + 1) * BW, vb);
-        step(va, cc * cr + r, role == 1 && r == a);
-        if (r + 1 <= b) {
-          tmem_ld_wait32(vb);
-          if (r + 2 <= b) tmem_row_issue<BW>(tbase + (r + 2) * BW, va);
-          step(vb, cc * cr + r + 1, false);
-        }
-      }
-    }
-    tcgen05_fence_before();
-    __syncwarp();
-    if (c.lane == 0) mbar_arrive(&c.acc_empty[buf]);
-  }
-}
-#endif
-
-// Epilogue of one warp (thread = pixel = TMEM lane) for one unit = (tile, level l): rows into the output tile, then one TMA
-// store per plane of the warp's 2 x 16 pixels (the TMA unit clips pixels beyond the image).
-__device__ __forceinline__ void lookup_epilogue(const EpiCtx& c, int& ch, int l, const CUtensorMap* map_hi, const CUtensorMap* map_lo) {
+// Epilogue of one warp (thread = pixel) for one unit = (tile, level l): rows into the output tile, then one TMA store per
+// plane of the warp's 2 x 16 pixels (the TMA unit clips pixels beyond the image).
+__device__ __forceinline__ void lookup_epilogue(const EpiCtx& c, MmaCtx& m, int l, const CUtensorMap* map_hi, const CUtensorMap* map_lo) {
   const Params& p = c.p;
   __half* sth = c.stage + c.ml * kLvlStride;
   __half* stl = sth + 128 * kLvlStride;
@@ -348,15 +253,9 @@ __device__ __forceinline__ void lookup_epilogue(const EpiCtx& c, int& ch, int l,
   const int ox = ix0 - c.ti->bx0, oy = iy0 - c.ti->by0;
   const bool live = c.valid && !empty;
   // the previous unit's TMA stores have finished READING this lane group's rows of the output tile
-#if RNC_LOOKUP_EPI2
-  if (c.team == 0 && c.lane == 0) bulk_wait_read0();
-  named_bar_sync(1 + c.lg, 64);                // both warps of the lane group: the tile may be rewritten
-#else
   if (c.lane == 0) bulk_wait_read0();
   __syncwarp();
-#endif
-#ifndef RNC_PROBE_NOEPI
-  if (!live && (!RNC_LOOKUP_EPI2 || c.team == 0)) {   // window fully outside the level image (or pixel outside the frame): zeros
+  if (!live) {                                 // window fully outside the level image (or pixel outside the frame): zeros
     const uint4 z = make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
     for (int q = 0; q < 10; ++q) {
@@ -366,42 +265,28 @@ __device__ __forceinline__ void lookup_epilogue(const EpiCtx& c, int& ch, int l,
     reinterpret_cast<unsigned short*>(sth)[80] = 0;
     reinterpret_cast<unsigned short*>(stl)[80] = 0;
   }
-#endif
-#if RNC_LOOKUP_EPI2
-  if (l == 0) lookup_level_rows2<box_w(0)>(c, ch, l, live, ox, oy, ax, ay);
-  else if (l == 1) lookup_level_rows2<box_w(1)>(c, ch, l, live, ox, oy, ax, ay);
-  else lookup_level_rows2<box_w(2)>(c, ch, l, live, ox, oy, ax, ay);
-#else
-  if (l == 0) lookup_level_rows<box_w(0)>(c, ch, l, live, ox, oy, ax, ay);
-  else if (l == 1) lookup_level_rows<box_w(1)>(c, ch, l, live, ox, oy, ax, ay);
-  else lookup_level_rows<box_w(2)>(c, ch, l, live, ox, oy, ax, ay);
-#endif
+  if (l == 0) lookup_level_rows<box_w(0)>(c, m, l, live, ox, oy, ax, ay);
+  else if (l == 1) lookup_level_rows<box_w(1)>(c, m, l, live, ox, oy, ax, ay);
+  else lookup_level_rows<box_w(2)>(c, m, l, live, ox, oy, ax, ay);
   static_assert(box_w(2) == box_w(3), "levels 2 and 3 share the row code");
-#ifndef RNC_PROBE_NOEPI
   fence_proxy_async();                         // this thread's shared-memory writes are visible to the TMA unit
-#if RNC_LOOKUP_EPI2
-  named_bar_sync(1 + c.lg, 64);                // both warps' window rows are in the tile
-  if (c.team == 0 && c.lane == 0) {
-#else
   __syncwarp();
   if (c.lane == 0) {
-#endif
     const __half* src = c.stage + c.lg * 32 * kLvlStride;
     tma_store_4d(map_hi, src, l * kLvlStride, c.x0, c.y0 + 2 * c.lg, c.b);
     tma_store_4d(map_lo, src + 128 * kLvlStride, l * kLvlStride, c.x0, c.y0 + 2 * c.lg, c.b);
     bulk_commit();
   }
-#endif
 }
 
-// Work units.  A unit is (tile, level): 3, 2, 1, 1 accumulator chunks.  Schedules (Params.tile_major):
+// Work units.  A unit is (tile, level): up to 6, 6, 3, 3 accumulator chunks.  Schedules (Params.tile_major):
 //   0  level-major: units listed level-major (all level-0 units first = longest first) and dealt to the CTAs in snake order
 //      (round k runs left-to-right for even k, right-to-left for odd k); every unit loads its own A tile
 //   1  tile-major: the four levels of a tile back to back on one CTA, A loaded once per tile (4x less A traffic, no A reload
-//      bubble between levels), but whole tiles balance badly (B=8: 448 tiles on 148 CTAs -> the busiest CTA gets 4)
+//      bubble between levels), but whole tiles balance badly (B=8: 448 tiles on 132 CTAs -> the busiest CTA gets 4)
 //   2  hybrid (default): the complete rounds of tiles (floor(ntiles / CTAs) per CTA) tile-major, the remaining tiles
-//      level-major over all CTAs.  B=8: 3 tile-major rounds + 16 units -> busiest CTA 24 chunks (level-major: 23) with a
-//      quarter of the A loads; a single image (56 tiles < 148 CTAs) is all level-major and still fills the SMs.
+//      level-major over all CTAs.  B=8: 3 tile-major rounds, then 52 tiles' units over all CTAs, with a quarter of the
+//      A loads; a single image (56 tiles < 132 CTAs) is all level-major and still fills the SMs.
 // Returns the k-th unit of this CTA as (tile-major flag << 30) | (level * ntiles + tile), or -1 (none in round k).
 constexpr int kUnitTm = 1 << 30;
 __device__ __forceinline__ int unit_id(int u) { return u & (kUnitTm - 1); }
@@ -498,12 +383,11 @@ __device__ __noinline__ void exact_unit(const Params& p, int l, int tile, float*
   }
 }
 
-// Persistent kernel: one CTA per SM walks tiles blockIdx.x, blockIdx.x + gridDim.x, ...  The three roles run decoupled
-// through mbarrier rings, so the TMA loads and MMAs of tile n+1 overlap the gather/blend/store epilogue of tile n:
-//   warp 0      producer: loads the tile's coords, reduces the per-level union boxes, publishes them (ti ring, 2 slots),
-//               then streams A (per K block, as soon as the previous tile's last chunk released it) and the B chunks
-//   warp 1      MMA issuer; TMEM accumulators are double buffered across chunks and tiles
-//   warps 2..   epilogue
+// Persistent kernel: one CTA per SM walks its work units.  The producer warp runs ahead of the consumers through mbarrier
+// rings, so the TMA loads of the next chunks (and of the next unit) overlap the MMAs and the epilogue of the current one:
+//   warp 4      producer: loads the tile's coords, reduces the per-level union boxes, publishes them (ti ring), then streams
+//               A (per K block, as soon as the previous tile's last chunk released it) and the B chunks
+//   warps 0-3   consumer warpgroup: wgmma per chunk, accumulator -> shared memory, gather + bilinear blend + store
 __global__ void __launch_bounds__(kThreads, 1)
 corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_constant__ LevelMaps mLv,
                         const __grid_constant__ CUtensorMap mOutHi,
@@ -512,20 +396,17 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
   unsigned char* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // 1024-aligned, stays in the shared window
   unsigned char* sA = smem;
   unsigned char* sB = smem + kSmemA;
-  float* scratch = reinterpret_cast<float*>(smem + kSmemA + kSmemB);
-  __half* stage = reinterpret_cast<__half*>(smem + kSmemA + kSmemB + kSmemScratch);
+  __half* stage = reinterpret_cast<__half*>(smem + kSmemA + kSmemB);
+  float* acc = reinterpret_cast<float*>(smem + kSmemA + kSmemB + kSmemStage);
   unsigned char* tail = smem + kSmemTotal - 1024 - 512;
   uint64_t* a_full = reinterpret_cast<uint64_t*>(tail);       // [kKB]
   uint64_t* a_empty = a_full + kKB;                           // [kKB]
   uint64_t* b_full = a_empty + kKB;
   uint64_t* b_empty = b_full + kStages;
-  uint64_t* acc_full = b_empty + kStages;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* ti_full = acc_empty + 2;                          // [kTiRing]
+  uint64_t* ti_full = b_empty + kStages;                      // [kTiRing]
   uint64_t* ti_empty = ti_full + kTiRing;                     // [kTiRing]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(ti_empty + kTiRing);
-  int* ov_count = reinterpret_cast<int*>(tmem_slot + 1);      // units of this CTA that overflowed their box
-  TileInfo* ti = reinterpret_cast<TileInfo*>(tmem_slot + 2);  // [kTiRing]
+  int* ov_count = reinterpret_cast<int*>(ti_empty + kTiRing); // units of this CTA that overflowed their box
+  TileInfo* ti = reinterpret_cast<TileInfo*>(ov_count + 2);   // [kTiRing]
 
   pdl_trigger();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -535,29 +416,21 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
 
   if (threadIdx.x == 0) {
     *ov_count = 0;
-    for (int kb = 0; kb < kKB; ++kb) { mbar_init(&a_full[kb], 1); mbar_init(&a_empty[kb], 1); }
-    for (int s = 0; s < kStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], kEpiWarps); }
-    for (int i = 0; i < kTiRing; ++i) { mbar_init(&ti_full[i], 1); mbar_init(&ti_empty[i], kEpiWarps + 1); }
+    for (int kb = 0; kb < kKB; ++kb) { mbar_init(&a_full[kb], 1); mbar_init(&a_empty[kb], 4); }
+    for (int s = 0; s < kStages; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 4); }
+    for (int i = 0; i < kTiRing; ++i) { mbar_init(&ti_full[i], 1); mbar_init(&ti_empty[i], 4); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                          // coords1 of the previous iteration's flow update is visible from here
 
   const int sched = p.tile_major;
   const int rounds = unit_rounds(ntiles, sched);
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ------------------------------------------------------------------ producer (warp-uniform loops, one elected lane issues)
     // lane owns pixels lane, lane+32, lane+64, lane+96 of the tile for the box reduction
     float pcx[4], pcy[4];
-#if RNC_LOOKUP_L2HINT
-    const uint64_t pol_keep = l2_policy_evict_last();   // the feature maps are re-read by every tile and every iteration
-#endif
     auto load_coords = [&](int tile, float (&ox)[4], float (&oy)[4]) {
       const int b = tile / tpi, tr = tile - b * tpi;
       const int y0 = (tr / p.tiles_x) * kTY, x0 = (tr % p.tiles_x) * kTX;
@@ -588,11 +461,7 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
       Rec r;
       r.ov = any && (lx1 - lx0 + 1 > box_w(l) || ly1 - ly0 + 1 > box_h(l)) ? 1 : 0;
       r.bx0 = any ? lx0 : 0; r.by0 = any ? ly0 : 0;
-#ifdef RNC_PROBE_NOTRIM
-      r.nrows = any ? box_h(l) : 0;
-#else
       r.nrows = any ? min((ly1 - ly0 + 2) & ~1, box_h(l)) : 0;
-#endif
       return r;
     };
     int n = 0;
@@ -644,16 +513,8 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
         for (int kb = 0; kb < kKB; ++kb) {
           mbar_wait(&a_empty[kb], (na & 1) ^ 1);
           if (elect_one()) {
-#ifdef RNC_PROBE_NOLOAD
-            mbar_arrive(&a_full[kb]);
-#else
             mbar_expect_tx(&a_full[kb], kATile);
-#if RNC_LOOKUP_L2HINT
-            tma_load_4d_hint(sA + kb * kATile, &mF1, &a_full[kb], kb * 64, x0, y0, b, pol_keep);
-#else
             tma_load_4d(sA + kb * kATile, &mF1, &a_full[kb], kb * 64, x0, y0, b);
-#endif
-#endif
           }
           __syncwarp();
         }
@@ -672,8 +533,7 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
         }
       };
       if (!skip) {
-        // B: only the box rows some window needs, as 2-row TMA boxes (2 * bw positions = a multiple of 1024 bytes of the
-        // SWIZZLE_128B stage, so the pieces tile the stage exactly as one big box would)
+        // B: only the box rows some window needs, as one TMA box of the chunk's (even) row count
         const CUtensorMap* map = &mLv.m[l][0];
         const int cr = chunk_rows(l), bw = box_w(l);
         int issued = 0;
@@ -683,16 +543,8 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
             const int s = it % kStages, ph = (it / kStages) & 1;
             mbar_wait(&b_empty[s], ph ^ 1);
             if (elect_one()) {
-#ifdef RNC_PROBE_NOLOAD
-              mbar_arrive(&b_full[s]);
-#else
               mbar_expect_tx(&b_full[s], rows * bw * 128);
-#if RNC_LOOKUP_L2HINT
-              tma_load_4d_hint(sB + s * kBStage, map + (rows >> 1) - 1, &b_full[s], kb * 64, bx0, by0 + c * cr, b, pol_keep);
-#else
               tma_load_4d(sB + s * kBStage, map + (rows >> 1) - 1, &b_full[s], kb * 64, bx0, by0 + c * cr, b);   // rows is even
-#endif
-#endif
             }
             __syncwarp();
             if (++issued == kStages) ahead();
@@ -702,71 +554,11 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
       ahead();
       unit = next; cur = nxt; next = after;
     }
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer (warp-uniform loops, one elected lane issues)
-    const uint32_t a_base = smem_u32(sA), b_base = smem_u32(sB);
-    int it = 0, ch = 0, n = 0, na = 0;
-    for (int k = 0; k < rounds; ++k) {
-      const int unit = unit_at(k, ntiles, sched);
-      if (unit < 0) continue;
-      const bool tm = unit_tm(unit);
-      const int l = unit_id(unit) / ntiles;
-      const int slot = n & (kTiRing - 1);
-      mbar_wait(&ti_full[slot], (n >> kTiShift) & 1);
-      const int ov = ti[slot].overflow, nrows = ti[slot].nrows;
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&ti_empty[slot]);
-      ++n;
-      const bool skip = ov || nrows == 0;
-      const bool load_a = tm ? l == 0 : !skip, free_a = tm ? l == kLevels - 1 : !skip;
-      if (skip) {                            // tile-major order: the A tile's barriers still turn over once per tile
-        if (load_a) {
-          for (int kb = 0; kb < kKB; ++kb) mbar_wait(&a_full[kb], na & 1);
-          ++na;
-        }
-        if (free_a) {
-          if (elect_one()) {
-            for (int kb = 0; kb < kKB; ++kb) umma_commit(&a_empty[kb]);
-          }
-          __syncwarp();
-        }
-        continue;
-      }
-      const int cr = chunk_rows(l), nc = (nrows + cr - 1) / cr;
-      for (int c = 0; c < nc; ++c, ++ch) {
-        const bool first = c == 0, final = c == nc - 1;
-        // instruction descriptor: D = F32, A = B = F16, K-major, N = positions of the rows this chunk holds, M = 128
-        const uint32_t nn = min(cr, nrows - c * cr) * box_w(l);
-        const uint32_t idesc = (1u << 4) | ((nn >> 3) << 17) | (static_cast<uint32_t>(128 >> 4) << 24);
-        const int buf = ch & 1, use = ch >> 1;
-        mbar_wait(&acc_empty[buf], (use & 1) ^ 1);
-        tcgen05_fence_after();
-        for (int kb = 0; kb < kKB; ++kb, ++it) {
-          const int s = it % kStages, ph = (it / kStages) & 1;
-          if (first && load_a) mbar_wait(&a_full[kb], na & 1);
-          mbar_wait(&b_full[s], ph);
-          tcgen05_fence_after();
-          const uint64_t ad = smem_desc_sw128(a_base + kb * kATile), bd = smem_desc_sw128(b_base + s * kBStage);
-          if (elect_one()) {
-#pragma unroll
-#ifndef RNC_PROBE_NOMMA
-            for (int kk = 0; kk < 4; ++kk) umma_f16(tmem_base + buf * 256, ad + 2 * kk, bd + 2 * kk, idesc, (kb | kk) != 0);
-#endif
-            umma_commit(&b_empty[s]);
-            if (final && free_a) umma_commit(&a_empty[kb]);   // this K block of A is free for the next tile
-          }
-          __syncwarp();
-        }
-        if (elect_one()) umma_commit(&acc_full[buf]);
-        __syncwarp();
-      }
-      if (load_a) ++na;
-    }
   } else {
-    // ------------------------------------------------------------------ epilogue: gather + bilinear blend + store
-    // thread = pixel = TMEM lane
-    const int lg = warp & 3, ml = lg * 32 + lane;
-    const int team = RNC_LOOKUP_EPI2 ? (warp - 2) >> 2 : 0;
+    // ------------------------------------------------------------------ consumers: MMA + gather + bilinear blend + store
+    // thread = pixel = accumulator row
+    const int lg = warp, ml = lg * 32 + lane;
+    MmaCtx m{smem_u32(sA), smem_u32(sB), a_full, a_empty, b_full, b_empty, acc, 0, 0};
     auto load_coord = [&](int tile, float& ox, float& oy, bool& v) {
       const int b = tile / tpi, tr = tile - b * tpi;
       const int py = (tr / p.tiles_x) * kTY + (ml >> 4), px = (tr % p.tiles_x) * kTX + (ml & 15);
@@ -776,51 +568,56 @@ corr_lookup_umma_kernel(const __grid_constant__ CUtensorMap mF1, const __grid_co
     };
     float cx = 0.f, cy = 0.f, ncx = 0.f, ncy = 0.f;
     bool valid = false, nvalid = false;
-#ifndef RNC_PROBE_NOEPI
-    if (team == 0) {                           // the 7 pad channels of this pixel's output rows stay zero for the whole kernel
+    {                                          // the 7 pad channels of this pixel's output rows stay zero for the whole kernel
       const uint4 z = make_uint4(0u, 0u, 0u, 0u);
       *reinterpret_cast<uint4*>(stage + ml * kLvlStride + 80) = z;
       *reinterpret_cast<uint4*>(stage + (128 + ml) * kLvlStride + 80) = z;
     }
-#endif
     int unit = unit_at(0, ntiles, sched);
     if (unit >= 0) load_coord(unit_id(unit) % ntiles, ncx, ncy, nvalid);
-    int ch = 0, n = 0;
+    int n = 0;
     for (int k = 0; k < rounds; ++k) {
       const int cur = unit;
       cx = ncx; cy = ncy; valid = nvalid;
       unit = k + 1 < rounds ? unit_at(k + 1, ntiles, sched) : -1;
       if (unit >= 0) load_coord(unit_id(unit) % ntiles, ncx, ncy, nvalid);
       if (cur < 0) continue;
+      const bool tm = unit_tm(cur);
       const int l = unit_id(cur) / ntiles, tile = unit_id(cur) - l * ntiles;
       const int b = tile / tpi, tr = tile - b * tpi;
       const int y0 = (tr / p.tiles_x) * kTY, x0 = (tr % p.tiles_x) * kTX;
       const int slot = n & (kTiRing - 1);
       mbar_wait(&ti_full[slot], (n >> kTiShift) & 1);
-      if (!ti[slot].overflow) {
-        EpiCtx c{p, &ti[slot], scratch, stage, acc_full, acc_empty, tmem_base, b, y0, x0, lg, ml, lane, valid, cx, cy, team};
-        lookup_epilogue(c, ch, l, &mOutHi, &mOutLo);
+      const int ov = ti[slot].overflow, nrows = ti[slot].nrows;
+      const bool skip = ov || nrows == 0;
+      const bool load_a = tm ? l == 0 : !skip, free_a = tm ? l == kLevels - 1 : !skip;
+      if (skip) {                              // tile-major order: the A tile's barriers still turn over once per tile
+        if (load_a)
+          for (int kb = 0; kb < kKB; ++kb) mbar_wait(&a_full[kb], m.na & 1);
+        __syncwarp();
+        if (free_a && lane == 0)
+          for (int kb = 0; kb < kKB; ++kb) mbar_arrive(&a_empty[kb]);
       }
+      if (!ov) {
+        EpiCtx c{p, &ti[slot], stage, b, y0, x0, lg, ml, lane, valid, cx, cy, load_a, free_a};
+        lookup_epilogue(c, m, l, &mOutHi, &mOutLo);
+      }
+      if (load_a) ++m.na;
       __syncwarp();
       if (lane == 0) mbar_arrive(&ti_empty[slot]);
       ++n;
     }
-    if (lane == 0 && team == 0) bulk_wait_all0();   // the output tile must outlive its TMA stores
+    if (lane == 0) bulk_wait_all0();           // the output tile must outlive its TMA stores
   }
 
-  tcgen05_fence_before();
   __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
   // ---- units of this CTA that overflowed their box (flagged by this CTA's own producer warp): exact path, all warps
   if (*ov_count == 0) return;                  // the common case: nothing to redo
   for (int k = 0; k < rounds; ++k) {
     const int unit = unit_at(k, ntiles, sched);
     if (unit < 0) continue;
     const int l = unit_id(unit) / ntiles, tile = unit_id(unit) - l * ntiles;
-    if (p.flags[tile * kLevels + l] != 0) exact_unit(p, l, tile, scratch, warp, lane, kThreads / 32);
+    if (p.flags[tile * kLevels + l] != 0) exact_unit(p, l, tile, acc, warp, lane, kThreads / 32);
   }
 }
 
@@ -844,7 +641,7 @@ extern "C" int rnc_f32_to_f16(const float* src, void* dst, size_t n, void* strea
   if (n == 0 || (n & 3)) return RNC_ERR_BAD_SHAPE;
   if (!src || !dst || !aligned16(src) || (reinterpret_cast<uintptr_t>(dst) & 7)) return RNC_ERR_BAD_POINTER;
   size_t blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   lookup_umma::f32_to_f16_kernel<<<static_cast<int>(blocks), 256, 0, as_stream(stream)>>>(
       reinterpret_cast<const float4*>(src), static_cast<uint2*>(dst), n / 4);
   return after_launch();
@@ -860,7 +657,7 @@ static int sm_count() {
   if (cached == 0) {
     int dev = 0, n = 0;
     cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached = n;
   }
   return cached;

@@ -19,7 +19,7 @@ constexpr int ST_SMEM = (3 * ST_IN_H * ST_PW + 147 * 64) * 4;   // 17.6 KB patch
 
 // weight layout [147 = (c*7+ky)*7+kx][64].  Thread = (4 horizontally adjacent output pixels, 16-channel group): per
 // (channel, filter row) the 13 input values of the quad are loaded once and every weight float4 feeds 16 multiply-adds, issued
-// as 8 packed FFMA2 (fma.rn.f32x2: two adjacent output channels per instruction) — the kernel is FMA-issue-bound.  In shared
+// as 8 FMA pairs (ffma2: two adjacent output channels) — the kernel is FMA-issue-bound.  In shared
 // memory a tap's 64 weights are stored as [quad q][channel group cg][4], so that the four channel groups of a quarter warp
 // read four consecutive 16-byte chunks (the plain [64] order put groups 0/2 and 1/3 into the same banks).
 __global__ void __launch_bounds__(256)
@@ -68,8 +68,8 @@ stem_conv7x7s2_kernel(const float* __restrict__ img, const float* __restrict__ w
           const float2 w01 = make_float2(w.x, w.y), w23 = make_float2(w.z, w.w);
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
-            acc2[i][2 * q] = __ffma2_rn(a[2 * i + kx], w01, acc2[i][2 * q]);
-            acc2[i][2 * q + 1] = __ffma2_rn(a[2 * i + kx], w23, acc2[i][2 * q + 1]);
+            acc2[i][2 * q] = ffma2(a[2 * i + kx], w01, acc2[i][2 * q]);
+            acc2[i][2 * q + 1] = ffma2(a[2 * i + kx], w23, acc2[i][2 * q + 1]);
           }
         }
       }
@@ -290,7 +290,7 @@ int rnc_stem_window_prep(const float* img, int N, int Hin, int Win, int pitch_px
   if (N <= 0 || Hin <= 0 || Win <= 0 || pitch_px < Win + 6 || (pitch_px & 1)) return RNC_ERR_BAD_SHAPE;
   if (!img || !out_hi || !out_lo || !aligned16(out_hi) || !aligned16(out_lo)) return RNC_ERR_BAD_POINTER;
   const size_t total = static_cast<size_t>(N) * Hin * pitch_px;
-  const int blocks = static_cast<int>(total / 256 < 148 * 16 ? total / 256 + 1 : 148 * 16);
+  const int blocks = static_cast<int>(total / 256 < 132 * 16 ? total / 256 + 1 : 132 * 16);
   stem_window_prep_kernel<<<blocks, 256, 0, as_stream(stream)>>>(img, N, Hin, Win, pitch_px, static_cast<uint2*>(out_hi),
                                                                   static_cast<uint2*>(out_lo));
   return after_launch();
@@ -323,7 +323,7 @@ int rnc_instnorm_apply(const float* x, const float* mean_rstd, const float* res,
   if (!aligned16(x) || (res && !aligned16(res)) || (out_f32 && !aligned16(out_f32))) return RNC_ERR_BAD_POINTER;
   const size_t total = (size_t)N * P * (C / 4);
   size_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   instnorm_apply_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(x, mean_rstd, res, N, P, C, mode, out_f32,
                                                                    static_cast<__half*>(out_hi), static_cast<__half*>(out_lo));
   return after_launch();
@@ -333,7 +333,7 @@ int rnc_add_relu_split(const float* a, const float* b, size_t n, float* out_f32,
   if (n == 0 || (n & 3)) return RNC_ERR_BAD_SHAPE;
   if (!a || !b || !out_hi || !out_lo || !aligned16(a) || !aligned16(b)) return RNC_ERR_BAD_POINTER;
   size_t blocks = (n / 4 + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   add_relu_split_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(reinterpret_cast<const float4*>(a), reinterpret_cast<const float4*>(b), n / 4,
                                                                     reinterpret_cast<float4*>(out_f32), static_cast<uint2*>(out_hi),
                                                                     static_cast<uint2*>(out_lo));
@@ -350,7 +350,7 @@ int rnc_fmap_pyramid(float* f2_pyr, int B, int D, int H, int W, int levels, void
     const size_t n = (size_t)B * (Hs >> 1) * (Ws >> 1) * (D / 4);
     if (n == 0) return RNC_ERR_BAD_SHAPE;
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     pool2_cl_kernel2<<<blocks, 256, 0, as_stream(stream)>>>(reinterpret_cast<const float4*>(s), reinterpret_cast<float4*>(d), B, Hs, Ws, D / 4);
     if (int st = after_launch()) return st;
   }

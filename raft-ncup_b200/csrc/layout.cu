@@ -89,7 +89,7 @@ using namespace rnc;
 extern "C" {
 
 int rnc_abi_version(void) { return 10; }
-const char* rnc_build_info(void) { return "librnc sm_100a (CUDA " RNC_STR_CUDA ")"; }
+const char* rnc_build_info(void) { return "librnc sm_90a (CUDA " RNC_STR_CUDA ")"; }
 const char* rnc_status_string(int s) {
   switch (s) {
     case RNC_OK: return "ok";
@@ -144,7 +144,7 @@ int rnc_fmap_prepare(const float* fmap1, const float* fmap2, int B, int D, int H
     int Hs = H >> (l - 1), Ws = W >> (l - 1);
     size_t n = (size_t)B * (Hs >> 1) * (Ws >> 1) * (D / 4);
     int blocks = (int)((n + 255) / 256);
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     pool2_cl_kernel<<<blocks, 256, 0, as_stream(stream)>>>((const float4*)s, (float4*)d, B, Hs, Ws, D / 4);
     st = after_launch();
     if (st) return st;

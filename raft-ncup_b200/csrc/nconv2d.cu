@@ -226,7 +226,7 @@ __global__ void nconv2d_bwd_weight_finish_kernel(double* __restrict__ gw, double
 
 inline int grid_for(long long total) {
   long long g = (total + 255) / 256;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > 132 * 8) g = 132 * 8;
   return static_cast<int>(g < 1 ? 1 : g);
 }
 

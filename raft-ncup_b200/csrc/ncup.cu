@@ -14,7 +14,7 @@
 //
 // The kernel is bound by the FP32 FMA pipe (~300 multiply-adds per output pixel), not by HBM, so it is organised around the
 // instruction count: the (data*conf, conf) pair of a position is one float2 and both streams share every weight, so
-// num/den accumulate with ONE packed FFMA2 (Blackwell fma.rn.f32x2) per tap; threads own 1x4 (stage 2) / 1x2 (stage 3)
+// num/den accumulate as one FMA pair (ffma2) per tap; threads own 1x4 (stage 2) / 1x2 (stage 3)
 // register tiles and fetch their input rows with 128-bit shared-memory loads (8 lanes = 256 contiguous bytes: conflict-free).
 // Tile sides are chosen so that stage 2 is exactly one 1x4 item per thread (32 rows x 8 groups = 256).
 #include "rnc_common.cuh"
@@ -30,7 +30,7 @@ constexpr int P2 = R2 + 2;         // stage-2 row pitch (float2): 272-byte rows 
 constexpr int LT = 12;             // lattice samples per side
 constexpr float kEps = 1e-20f;     // nconv_modules.py:149
 
-struct NcupWeights {               // lives in the kernel parameter (constant) bank; every weight duplicated for FFMA2
+struct NcupWeights {               // lives in the kernel parameter (constant) bank; every weight duplicated for the FMA pairs
   float2 w1[2][25];                // nconv_in   [2,1,5,5]
   float2 w2[2][2][25];             // nconv_x2.0 [2,2,5,5]
   float2 w3[2][2][9];              // decoder.0  [2,4,3,3] folded: W[:, :2] + W[:, 2:]  (input is cat(x1, x1))
@@ -85,8 +85,8 @@ ncup_fused_kernel(const float* __restrict__ x_lowres, const float* __restrict__ 
           const int kx = 4 * ix + 2 - x + 2;
           const float cv = lc[iy - iy_base][ix - ix_base];
           const float2 pc = make_float2(lx[iy - iy_base][ix - ix_base] * cv, cv);
-          a0 = __ffma2_rn(pc, w.w1[0][ky * 5 + kx], a0);
-          a1 = __ffma2_rn(pc, w.w1[1][ky * 5 + kx], a1);
+          a0 = ffma2(pc, w.w1[0][ky * 5 + kx], a0);
+          a1 = ffma2(pc, w.w1[1][ky * 5 + kx], a1);
         }
       }
       o0 = nconv_out_pair(a0, w.inv_s1[0]);
@@ -120,8 +120,8 @@ ncup_fused_kernel(const float* __restrict__ x_lowres, const float* __restrict__ 
           const float2 wa = w.w2[0][i][ky * 5 + kx], wb = w.w2[1][i][ky * 5 + kx];
 #pragma unroll
           for (int x = 0; x < 4; ++x) {
-            acc[x][0] = __ffma2_rn(row[x + kx], wa, acc[x][0]);
-            acc[x][1] = __ffma2_rn(row[x + kx], wb, acc[x][1]);
+            acc[x][0] = ffma2(row[x + kx], wa, acc[x][0]);
+            acc[x][1] = ffma2(row[x + kx], wb, acc[x][1]);
           }
         }
       }
@@ -159,8 +159,8 @@ ncup_fused_kernel(const float* __restrict__ x_lowres, const float* __restrict__ 
           const float2 wa = w.w3[0][i][ky * 3 + kx], wb = w.w3[1][i][ky * 3 + kx];
 #pragma unroll
           for (int x = 0; x < 2; ++x) {
-            acc[x][0] = __ffma2_rn(row[x + kx], wa, acc[x][0]);
-            acc[x][1] = __ffma2_rn(row[x + kx], wb, acc[x][1]);
+            acc[x][0] = ffma2(row[x + kx], wa, acc[x][0]);
+            acc[x][1] = ffma2(row[x + kx], wb, acc[x][1]);
           }
         }
       }

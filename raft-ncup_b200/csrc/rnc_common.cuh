@@ -1,4 +1,4 @@
-// Shared helpers for the rnc kernels (sm_100a only).
+// Shared helpers for the rnc kernels (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cstdlib>
@@ -45,7 +45,7 @@ inline int after_launch(int n = 1) {
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
 // Programmatic dependent launch (PDL).  A kernel launched with launch_pdl() may start while its predecessor in the stream is
-// still draining: it runs its prologue (barrier init, TMEM allocation, descriptor prefetch), then pdl_wait() blocks until the
+// still draining: it runs its prologue (barrier init, descriptor prefetch), then pdl_wait() blocks until the
 // predecessor has completed and its writes are visible.  pdl_trigger() in the predecessor lets the dependent start early;
 // without it the dependent starts at the predecessor's exit (plain stream order).  RNC_PDL=0 disables the attribute.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -79,6 +79,9 @@ __device__ __forceinline__ void split_pair(float v0, float v1, uint32_t& hi, uin
   const float2 back = __half22float2(*reinterpret_cast<const __half2*>(&hi));
   lo = pack_half2_sat(v0 - back.x, v1 - back.y);
 }
+
+// Two independent fp32 FMAs on a pair of adjacent outputs (Hopper has no packed fp32 FMA; each lane rounds as fmaf does).
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 

@@ -47,7 +47,7 @@ extern "C" int rnc_bilinear_sample_fwd(const float* img, const float* coords, in
   if (N <= 0 || C <= 0 || H <= 1 || W <= 1 || h <= 0 || w <= 0) return RNC_ERR_BAD_SHAPE;   // W-1 / H-1 divide (utils.py:63-64)
   if (!img || !coords || !out) return RNC_ERR_BAD_POINTER;
   long long blocks = (static_cast<long long>(N) * h * w + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   bilinear_sample_kernel<<<static_cast<int>(blocks), 256, 0, as_stream(stream)>>>(img, coords, N, C, H, W, h, w, out, mask);
   return after_launch();
 }

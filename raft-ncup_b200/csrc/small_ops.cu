@@ -346,7 +346,7 @@ int rnc_flow_head2_fwd(const float* in, int cin, int ldi, const float* weight, c
   if (!in || !weight || !bias || !coords1 || !aligned16(in) || !aligned16(weight)) return RNC_ERR_BAD_POINTER;
   const int M = B * H * W;
   int blocks = (M + 7) / 8;
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  if (blocks > 132 * 4) blocks = 132 * 4;
   const size_t smem = (size_t)9 * cin * 2 * sizeof(float);
   flow_head2_kernel<<<blocks, 256, smem, as_stream(stream)>>>(in, cin, ldi, weight, bias, B, H, W, delta, coords1);
   return after_launch();
@@ -357,7 +357,7 @@ int rnc_flow_im2col7_split_fwd(const float* coords1, int B, int H, int W, void* 
   if (!coords1 || !out_hi || !out_lo || !aligned16(out_hi) || !aligned16(out_lo)) return RNC_ERR_BAD_POINTER;
   const long long total = static_cast<long long>(B) * H * W * 16;
   long long blocks = (total + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   flow_im2col7_kernel<<<static_cast<int>(blocks), 256, 0, as_stream(stream)>>>(coords1, B, H, W, static_cast<__half*>(out_hi),
                                                                               static_cast<__half*>(out_lo), ld);
   return after_launch();
@@ -369,7 +369,7 @@ int rnc_flow_tap_gather_fwd(const float* taps, int ldt, const float* bias, int B
   if (!taps || !bias || !coords1 || (reinterpret_cast<uintptr_t>(taps) & 7)) return RNC_ERR_BAD_POINTER;
   const long long M = static_cast<long long>(B) * H * W;
   long long blocks = (M + 127) / 128;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   flow_tap_gather_kernel<<<static_cast<int>(blocks), 128, 0, as_stream(stream)>>>(taps, ldt, bias, B, H, W, coords1, delta);
   return after_launch();
 }
@@ -389,7 +389,7 @@ int rnc_f32_to_split(const float* src, int lds, int C, long long M, void* dst_hi
   if (C <= 0 || M <= 0 || lds < C || ldd < C + ch_off || ch_off < 0) return RNC_ERR_BAD_SHAPE;
   if (!src || !dst_hi || !dst_lo) return RNC_ERR_BAD_POINTER;
   long long blocks = (M * C + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   f32_to_split_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(src, lds, C, M, static_cast<__half*>(dst_hi),
                                                                  static_cast<__half*>(dst_lo), ldd, ch_off);
   return after_launch();
@@ -400,7 +400,7 @@ int rnc_f32_to_tf32_split(const float* src, int lds, int C, long long M, float* 
   if (C <= 0 || M <= 0 || lds < C || ldd < C + ch_off || ch_off < 0) return RNC_ERR_BAD_SHAPE;
   if (!src || !dst_hi || !dst_lo) return RNC_ERR_BAD_POINTER;
   long long blocks = (M * C + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   f32_to_tf32_split_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(src, lds, C, M, dst_hi, dst_lo, ldd, ch_off);
   return after_launch();
 }
@@ -419,7 +419,7 @@ int rnc_ncup_guidance_fwd(const float* x_lowres, const float* net, int ldg, int 
   if (!x_lowres || !net || !out) return RNC_ERR_BAD_POINTER;
   const size_t n = (size_t)B * 4 * H8 * W8 * ldo;
   int blocks = (int)((n + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   ncup_guidance_kernel<<<blocks, 256, 0, as_stream(stream)>>>(x_lowres, net, ldg, C, B, H8, W8, out, ldo);
   return after_launch();
 }
@@ -430,7 +430,7 @@ int rnc_ncup_guidance_split_fwd(const float* x_lowres, const float* net, int ldg
   if (!x_lowres || !net || !out_hi || !out_lo || !aligned16(out_hi) || !aligned16(out_lo)) return RNC_ERR_BAD_POINTER;
   const long long n = static_cast<long long>(B) * 4 * H8 * W8 * (ldo >> 3);
   long long blocks = (n + 255) / 256;
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   ncup_guidance_split_kernel<<<static_cast<int>(blocks), 256, 0, as_stream(stream)>>>(
       x_lowres, net, ldg, C, B, H8, W8, static_cast<__half*>(out_hi), static_cast<__half*>(out_lo), ldo);
   return after_launch();
@@ -442,7 +442,7 @@ int rnc_convex_upsample_fwd(const float* flow, const float* mask, int ldm, int B
   if (!flow || !mask || !out) return RNC_ERR_BAD_POINTER;
   const int M = B * H8 * W8;
   int blocks = (M + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   convex_upsample_kernel<<<blocks, 256, 0, as_stream(stream)>>>(flow, mask, ldm, B, H8, W8, out);
   return after_launch();
 }

@@ -121,7 +121,7 @@ conv_wgrad_kernel(const float* __restrict__ x, int ldx, int cin, const float* __
   const long long p0 = static_cast<long long>(blockIdx.z) * px_per_block;
   const long long p1 = p0 + px_per_block < P ? p0 + px_per_block : P;
   const int ty = tid >> 3, tx = tid & 7;        // thread = 8 (ci) x 8 (co) micro tile
-  float2 acc2[8][4];                              // pairs of adjacent output channels: one packed FFMA2 per pair
+  float2 acc2[8][4];                              // pairs of adjacent output channels (ffma2)
 #pragma unroll
   for (int i = 0; i < 8; ++i)
 #pragma unroll
@@ -174,7 +174,7 @@ conv_wgrad_kernel(const float* __restrict__ x, int ldx, int cin, const float* __
       for (int i = 0; i < 8; ++i) {
         const float2 xi = make_float2(xa[i], xa[i]);
 #pragma unroll
-        for (int j = 0; j < 4; ++j) acc2[i][j] = __ffma2_rn(xi, g2[j], acc2[i][j]);
+        for (int j = 0; j < 4; ++j) acc2[i][j] = ffma2(xi, g2[j], acc2[i][j]);
       }
       if (do_bias) {
 #pragma unroll
@@ -214,7 +214,7 @@ extern "C" int rnc_corr_lookup_bwd(const float* f1_cl, const float* f2_pyr, cons
   if (!aligned16(f1_cl) || !aligned16(f2_pyr) || !aligned16(g_f1) || !aligned16(g_f2_pyr)) return RNC_ERR_BAD_POINTER;
   const long long total = static_cast<long long>(B) * H * W;
   long long blocks = (total + 7) / 8;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   train::corr_lookup_bwd_kernel<<<static_cast<int>(blocks), 256, 0, as_stream(stream)>>>(
       f1_cl, f2_pyr, coords, g_out, ldg, B, H, W, levels, 1.0f / sqrtf(static_cast<float>(D)), g_f1, g_f2_pyr);
   return after_launch();
@@ -230,7 +230,7 @@ extern "C" int rnc_pyramid_pool_bwd(float* g_f2_pyr, int B, int D, int H, int W,
     const int Hf = H >> l, Wf = W >> l;
     const size_t n = static_cast<size_t>(B) * Hf * Wf * (D / 4);
     size_t blocks = (n + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     train::pool2_adjoint_kernel<<<static_cast<int>(blocks), 256, 0, as_stream(stream)>>>(
         reinterpret_cast<float4*>(fine), reinterpret_cast<const float4*>(coarse), B, Hf, Wf, D / 4);
     ++launches;
@@ -249,7 +249,7 @@ extern "C" int rnc_conv2d_cl_wgrad(const float* x, int ldx, int cin, const float
   const int tiles = ((cin + train::WT - 1) / train::WT) * ((cout + train::WT - 1) / train::WT);
   const int taps = kh * kw;
   // enough blocks to fill the machine a few times over; every block takes a multiple of WK pixels
-  long long want = (148LL * 24 + tiles * taps - 1) / (static_cast<long long>(tiles) * taps);
+  long long want = (132LL * 24 + tiles * taps - 1) / (static_cast<long long>(tiles) * taps);
   if (want < 1) want = 1;
   long long per = (P + want - 1) / want;
   per = (per + train::WK - 1) / train::WK * train::WK;

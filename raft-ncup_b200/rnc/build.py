@@ -1,9 +1,9 @@
-"""Build librnc.so (the sm_100a kernels + C ABI) in-tree with nvcc.
+"""Build librnc.so (the sm_90a kernels + C ABI) in-tree with nvcc.
 
     python raft-ncup_b200/rnc/build.py [--force] [--verbose]
 
-nvcc cross-compiles for sm_100a without a GPU.  The .so lands next to this file so that it travels to the
-GPU box with the repo snapshot (it is git-ignored, not gpurun-ignored).
+nvcc cross-compiles for sm_90a without a GPU.  The .so lands next to this file (git-ignored), so the package imports
+straight from the source tree.
 """
 import hashlib
 import os
@@ -18,7 +18,7 @@ CSRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(PKG, "build")
 LIB = os.path.join(HERE, "librnc.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
               "--expt-relaxed-constexpr", "-Xptxas", "-warn-spills"]
 
@@ -45,7 +45,7 @@ def _digest():
 
 
 def build(force=False, verbose=False):
-    """Compile every .cu under csrc/ for sm_100a and link librnc.so.  Returns the path."""
+    """Compile every .cu under csrc/ for sm_90a and link librnc.so.  Returns the path."""
     stamp = os.path.join(OBJ, "stamp")
     dig = _digest()
     if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == dig:

@@ -41,7 +41,7 @@ def _require_cuda(*tensors):
             continue
         if not t.is_cuda:
             raise native.RncUnavailable(
-                "the RAFT-NCUP hot path runs only on CUDA (sm_100a) tensors; got a CPU tensor and there is no CPU fallback")
+                "the RAFT-NCUP hot path runs only on CUDA (sm_90a) tensors; got a CPU tensor and there is no CPU fallback")
         if dev is None:
             dev = t.device
         elif t.device != dev:
@@ -251,7 +251,7 @@ def engine_for(device):
     device, shallow-copied module __dict__) never share packed weights or workspaces across devices."""
     device = torch.device(device)
     if device.type != "cuda":
-        raise native.RncUnavailable("the RAFT-NCUP hot path runs only on CUDA (sm_100a) devices; there is no CPU fallback")
+        raise native.RncUnavailable("the RAFT-NCUP hot path runs only on CUDA (sm_90a) devices; there is no CPU fallback")
     idx = device.index if device.index is not None else torch.cuda.current_device()
     key = (idx,) + tuple(os.environ.get(k, "") for k in _ENGINE_ENV)      # developer switches select distinct engines
     eng = _ENGINES.get(key)
@@ -266,7 +266,7 @@ def engine_for(device):
 
 
 def make_engine():
-    """RNC_CONV=umma (default): tcgen05 tensor-core convolutions on fp16 hi/lo split operands;
+    """RNC_CONV=umma (default): wgmma tensor-core convolutions on fp16 hi/lo split operands;
     RNC_CONV=ffma: exact-fp32 CUDA-core convolutions (v1, kept as the on-GPU cross-check)."""
     mode = os.environ.get("RNC_CONV", "umma").lower()
     if mode == "ffma":

@@ -1,5 +1,5 @@
 """Tensor-core variant of rnc.engine: the same loop body (raft_nc_dbl.py:148-165, update.py:130-141), with every
-wide convolution on tcgen05 (rnc_conv2d_umma_fwd) and the 1/8-resolution activations resident as fp16 hi/lo split
+wide convolution on wgmma (rnc_conv2d_umma_fwd) and the 1/8-resolution activations resident as fp16 hi/lo split
 planes (value = hi + lo).  Thin layers (7x7 on flow, 3x3 -> 2 flow head, 1x1 -> 2 confidence head) stay on CUDA cores.
 """
 import ctypes as C
@@ -192,7 +192,7 @@ class UmmaEngine(Engine):
     def __init__(self):
         super().__init__()
         import os
-        # RNC_LOOKUP=umma (default): tcgen05 lookup on fp16 features; RNC_LOOKUP=ffma: exact fp32 CUDA-core lookup
+        # RNC_LOOKUP=umma (default): wgmma lookup on fp16 features; RNC_LOOKUP=ffma: exact fp32 CUDA-core lookup
         self.lookup_mode = os.environ.get("RNC_LOOKUP", "umma").lower()
         if self.lookup_mode not in ("umma", "ffma"):
             raise ValueError(f"RNC_LOOKUP={self.lookup_mode!r}: expected 'umma' or 'ffma'")

@@ -50,8 +50,8 @@ def _ceil4(c):
 def _conv_mode():
     """RNC_TRAIN_CONV selects how the training path's convolutions (forward and data gradient) run:
       ffma (default)  exact fp32 on CUDA cores (rnc_conv2d_cl_fwd): per-layer error 1.5e-7; every non-fnet parameter's gradient
-                      within 1e-3 of the reference's autograd (cfg 5 step on B200: 149 ms)
-      tf32            tcgen05 kind::tf32 on TF32 hi/lo operand planes, 3 MMAs per K step (x_hi*w_hi + x_hi*w_lo + x_lo*w_hi):
+                      within 1e-3 of the reference's autograd
+      tf32            wgmma .tf32 on TF32 hi/lo operand planes, 3 MMAs per K step (x_hi*w_hi + x_hi*w_lo + x_lo*w_hi):
                       ~2^-21 per product (per-layer 1e-6 .. 5e-6) with fp32's exponent range, so output gradients of 1e-9
                       survive; 112 ms per step, ill-conditioned parameters (cnet.conv1) move to 5e-3
       umma            fp16 hi/lo split operands (the inference kernels): output gradients underflow the split's normal range —
@@ -116,7 +116,7 @@ def _packed_umma(weight, kind, cin_pad, fmt="f16"):
 
 
 def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16"):
-    """Same contract as _conv_launch on the tcgen05 path: x fp32 CL -> hi/lo operand planes (halves or TF32 words) ->
+    """Same contract as _conv_launch on the tensor-core path: x fp32 CL -> hi/lo operand planes (halves or TF32 words) ->
     rnc_conv2d_umma_fwd with an fp32 channel-last output; stride 2 is native (TMA element strides), no subsampling pass."""
     B, H, W, Cx = x.shape
     Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride

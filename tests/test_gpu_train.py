@@ -44,7 +44,7 @@ def test_conv_cl_forward_and_gradients(cin, cout, kh, kw, stride, mode, monkeypa
     wd, bd = w.to(DEV).requires_grad_(True), b.to(DEV).requires_grad_(True)
     y = ConvCL.apply(xd, wd, bd, stride)
     assert y.shape[:3] == (B, ref.shape[2], ref.shape[3])
-    # ffma: exact fp32 CUDA cores throughout; tf32: tcgen05 TF32x3 (~2^-21 per product) for forward and data gradient where the
+    # ffma: exact fp32 CUDA cores throughout; tf32: wgmma TF32x3 (~2^-21 per product) for forward and data gradient where the
     # layer's shape allows (the weight gradient stays exact fp32)
     e_y = rel(to_nchw(y, cout), ref.detach())
     assert (y[..., cout:] == 0).all()
@@ -110,11 +110,11 @@ def test_training_loss_and_gradients_match_the_oracle(name):
     """Config-5-style step at 128x160, B = 2, 3 iterations, train mode with frozen BatchNorm (train.py:185-186): loss and every
     parameter's gradient against the differentiable oracle (= the reference's autograd, tests/test_r2_golden.py), evaluated
       (a) on the CPU in fp32 — the pinned reference numbers, and
-      (b) by PyTorch on the same GPU in fp32 (cuDNN / cuBLAS, TF32 off) — what the reference itself computes on a B200.
+      (b) by PyTorch on the same GPU in fp32 (cuDNN / cuBLAS, TF32 off) — what the reference itself computes on a GPU.
     The gradients of the fnet convolutions below layer3 are ill-conditioned in fp32 (a long chain of InstanceNorm backward
-    passes, sums with heavy cancellation): measured on B200, cuDNN's own fp32 evaluation of the encoder sits 4-5e-3 from fp64
-    there, and any two fp32 GPU evaluations differ from each other by as much (test_encoder_gradients_match_torch_fp64), while
-    with BatchNorm the kernels agree with cuDNN to 4e-6.  Hence two bounds: 2e-2 for fnet, 2e-3 for every other parameter."""
+    passes, sums with heavy cancellation): cuDNN's own fp32 evaluation of the encoder sits several 1e-3 from fp64
+    there, and any two fp32 GPU evaluations differ from each other by as much (test_encoder_gradients_match_torch_fp64).
+    Hence two bounds: 2e-2 for fnet, 2e-3 for every other parameter."""
     from rnc.train import sequence_loss
     with open(os.path.join(ROOT, "tests", "golden", "r2_meta.json")) as f:
         meta = json.load(f)
@@ -180,13 +180,42 @@ def test_train_step_updates_parameters_and_lowers_the_loss(mode, monkeypatch):
     assert torch.isfinite(up).all()
 
 
+class _FixedReLU:
+    """Stand-in for F.relu: the first evaluation records where each ReLU's input is positive, later evaluations (NCHW or
+    channel-last) apply the recorded regions in call order.  A few pre-activations of the test encoder lie within fp32
+    rounding of zero, and which side of zero an fp32 evaluation puts them on moves the gradients of the parameters upstream
+    by up to 4e-3; with the regions fixed, every evaluation computes the same piecewise-linear function and the comparison
+    measures arithmetic only."""
+
+    def __init__(self):
+        self.masks, self.replay, self.i = [], False, 0
+
+    def start_replay(self):
+        self.replay, self.i = True, 0
+
+    def __call__(self, x, inplace=False):
+        if not self.replay:
+            m = x.detach() > 0
+            self.masks.append(m.cpu())
+        else:
+            m = self.masks[self.i].to(x.device)
+            self.i += 1
+            if m.shape != x.shape:
+                m = m.permute(0, 2, 3, 1)                    # channel-last evaluation
+            assert m.shape == x.shape
+        return x.mul_(m) if inplace else x * m
+
+
 @pytest.mark.parametrize("norm", ["instance", "batch"])
-def test_encoder_gradients_match_torch_fp64(norm):
+def test_encoder_gradients_match_torch_fp64(norm, monkeypatch):
     """BasicEncoder (extractor.py:118-192) forward + backward through the ConvCL / norm graph against the nn.Module's own
-    layer graph evaluated in fp64 on the CPU: input gradient flows through both stride-2 residual blocks."""
+    layer graph evaluated in fp64 on the CPU: input gradient flows through both stride-2 residual blocks.  All three
+    evaluations use the ReLU regions of the fp64 one (_FixedReLU)."""
     import copy
     from rnc.modules import BasicEncoder
     from rnc.train import encoder_cl, to_cl, to_nchw
+    relu = _FixedReLU()
+    monkeypatch.setattr(F, "relu", relu)
     torch.manual_seed(5)
     enc = BasicEncoder(output_dim=256, norm_fn=norm).train()
     if norm == "batch":
@@ -201,11 +230,14 @@ def test_encoder_gradients_match_torch_fp64(norm):
     # how far does an fp32 GPU evaluation of the SAME layer graph (cuDNN, TF32 off) sit from fp64?  (conditioning yardstick)
     lib = copy.deepcopy(enc)
     torch.backends.cudnn.allow_tf32 = False
+    relu.start_replay()
     lib(x.to(DEV)).backward(gy.to(DEV))
     for (k, p), (_, q) in zip(lib.named_parameters(), ref.named_parameters()):
         if q.grad is not None and q.grad.norm() > 1e-9 and rel(p.grad, q.grad) > 1e-4:
             print(f"   [cuDNN fp32 vs fp64] {k}: rel {rel(p.grad, q.grad):.2e}")
+    relu.start_replay()
     out = encoder_cl(enc, to_cl(x.to(DEV)))
+    assert relu.i == len(relu.masks)
     assert rel(to_nchw(out), out_ref.detach()) < 1e-5
     out.backward(to_cl(gy.to(DEV)))
     worst = 0.0

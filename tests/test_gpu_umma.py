@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 (tensor-core) convolution path against fp32 references: the fp16 hi/lo split must stay
+"""GPU parity of the wgmma (tensor-core) convolution path against fp32 references: the fp16 hi/lo split must stay
 fp32-faithful (north star: 1e-3 EPE after 32 recurrent iterations; plain TF32/bf16 operands fail it, SURVEY.md App. D)."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""tcgen05 convolution: A-staging modes (per-tap / row halo / column halo), stride 2, residual and encoder-head epilogues,
+"""wgmma convolution: A-staging modes (per-tap / row halo / column halo), stride 2, residual and encoder-head epilogues,
 persistent scheduling over many tiles — each against an fp64 torch convolution."""
 import pytest
 import torch
@@ -103,7 +103,7 @@ def test_residual_and_head_epilogues(ueng):
 
 
 def test_persistent_many_tiles_and_n_tiles(ueng):
-    # 3 images x 40 x 256 = 30720 px = 240 tiles > 148 SMs: every CTA loops; Cout 576 = 3 N tiles of 192
+    # 3 images x 40 x 256 = 30720 px = 240 tiles > 132 SMs: every CTA loops; Cout 576 = 9 N tiles of 64
     g = torch.Generator().manual_seed(5)
     x = torch.randn(3, 64, 40, 256, generator=g)
     w = torch.randn(576, 64, 1, 1, generator=g) / 8.0

@@ -60,7 +60,7 @@ def test_cabi_exports_every_declared_symbol():
         assert hasattr(lib, name), name
     L = native.lib()
     assert L.rnc_abi_version() == native.ABI_VERSION
-    assert b"sm_100a" in L.rnc_build_info()
+    assert b"sm_90a" in L.rnc_build_info()
     assert L.rnc_status_string(-1) == b"bad shape"
     # pure host helper: pyramid offsets (55x128 -> 27x64 -> 13x32 -> 6x16, floor mode)
     assert L.rnc_pyramid_offset(8, 256, 55, 128, 4) == 8 * 256 * (55 * 128 + 27 * 64 + 13 * 32 + 6 * 16)

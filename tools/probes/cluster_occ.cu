@@ -1,5 +1,5 @@
 // Developer probe: how many clusters of 2 / 4 / 8 CTAs with ~226 KB of dynamic shared memory (one CTA per SM) are co-resident?
-// nvcc -gencode arch=compute_100a,code=sm_100a -o /tmp/cluster_occ tools/probes/cluster_occ.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -o /tmp/cluster_occ tools/probes/cluster_occ.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 __global__ void dummy(int* p) { extern __shared__ char s[]; if (p) p[0] = s[0]; }
@@ -9,7 +9,7 @@ int main() {
   cudaFuncSetAttribute(dummy, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
   for (int cs : {1, 2, 4, 8, 16}) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(148 / cs * cs); cfg.blockDim = dim3(320); cfg.dynamicSmemBytes = smem;
+    cfg.gridDim = dim3(132 / cs * cs); cfg.blockDim = dim3(320); cfg.dynamicSmemBytes = smem;
     cudaLaunchAttribute a[1];
     a[0].id = cudaLaunchAttributeClusterDimension; a[0].val.clusterDim.x = cs; a[0].val.clusterDim.y = 1; a[0].val.clusterDim.z = 1;
     cfg.attrs = a; cfg.numAttrs = 1;

@@ -1,6 +1,6 @@
 // Developer probe: does cuTensorMapEncodeTiled accept a sliding-window (overlapping) view — stride of dimension 1 (16 B)
 // smaller than the extent of dimension 0 (128 B) — and does the TMA unit load it as expected?
-// nvcc -gencode arch=compute_100a,code=sm_100a -o /tmp/tmap_overlap tools/probes/tmap_overlap.cu -lcuda
+// nvcc -gencode arch=compute_90a,code=sm_90a -o /tmp/tmap_overlap tools/probes/tmap_overlap.cu -lcuda
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
