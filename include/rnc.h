@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 10) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 11) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -317,6 +317,25 @@ int rnc_conf_head_fwd(const float* in, int cin, int ldi, const float* weight, co
  */
 int rnc_ncup_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
                  float out_scale, float* out, void* stream);
+
+/* Training form of the same chain (fine-tuning the upsampler on a frozen trunk).
+ * rnc_ncup_train_fwd: rnc_ncup_fwd with the 224 positive weights read from DEVICE memory (weights_dev, same order), so a
+ *   trainable upsampler needs no device-to-host copy per call; outputs are bit-identical to rnc_ncup_fwd on the same weights.
+ * rnc_ncup_bwd: gradients of L = sum(g_out * out) for out = rnc_ncup_train_fwd(...):
+ *   g_out      : NCHW [B][2][4*H4][4*W4]
+ *   g_x_lowres : NCHW [B][2][H4][W4] (may be NULL)        g_conf : NCHW [B][2][H4][W4] (may be NULL)
+ *   g_weights  : [224] w.r.t. the UNFOLDED positive weights (may be NULL): decoder.0's folded gradient goes to both halves
+ *                W[:, :2] and W[:, 2:], and every layer's 1/sum(W) normalisation contributes to all of that layer's weights
+ *   workspace  : rnc_ncup_bwd_workspace_bytes(B,H4,W4) bytes, 16-byte aligned, needed only with g_weights (no zeroing needed)
+ * The kernel recomputes the forward per tile with the forward's own code and differentiates the (y*c, c) pairs it carries,
+ * so gradients stay finite where the confidence is zero.  Deterministic: every input gradient is written by one CTA, the
+ * weight gradient is a fixed-order fp64 reduction of per-CTA partials; identical inputs give bit-identical gradients. */
+int rnc_ncup_train_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
+                       float out_scale, float* out, void* stream);
+size_t rnc_ncup_bwd_workspace_bytes(int B, int H4, int W4);
+int rnc_ncup_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4, float out_scale,
+                 const float* g_out, float* g_x_lowres, float* g_conf, float* g_weights, void* workspace,
+                 size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * A3  bilinear_sampler  (core/utils/utils.py:59-73) as a standalone operator: grid_sample(align_corners=True, bilinear,

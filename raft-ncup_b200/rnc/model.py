@@ -76,6 +76,9 @@ class _RAFTBase(nn.Module):
             # training path (train.py:215): the same graph with autograd, exact-fp32 kernels forward and backward
             if image1.shape[2] % 8 or image1.shape[3] % 8:
                 raise ValueError("image height/width must be multiples of 8 (pad with utils.utils.InputPadder, evaluate.py:125)")
+            if frozen_trunk(self, image1, image2, flow_init):
+                # only the upsampler trains: the trunk runs on the inference engine, the upsampler on autograd
+                return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, upsample=self._upsample_frozen)
             from .train import raft_forward_train
             return raft_forward_train(self, image1, image2, iters, flow_init, test_mode)
         B, _, Him, Wim = image1.shape
@@ -85,15 +88,20 @@ class _RAFTBase(nn.Module):
             return eng.graph_forward(self, image1, image2, iters, flow_init)
         return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode)
 
-    def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode):
+    def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode, upsample=None):
+        """The iteration loop on the engine's resident buffers.  upsample(eng, ws, pu) produces each full-resolution prediction
+        from the workspace; the default is the inference upsampler (self._upsample on packed weights)."""
         B, _, Him, Wim = image1.shape
         H8, W8 = Him // 8, Wim // 8
         L = eng.L
         pk = eng.packed_update(self.update_block)
-        pu = eng.packed_upsampler(self.upsampler) if self.ncup else None
-        if self.ncup and any(isinstance(m, nn.BatchNorm2d) and m.training for m in self.upsampler.modules()):
-            raise NotImplementedError("weights-net BatchNorm with batch statistics needs the training path (enable grad) "
-                                      "or eval mode: call .eval() / freeze_bn()")
+        pu = None
+        if upsample is None:
+            upsample = self._upsample
+            pu = eng.packed_upsampler(self.upsampler) if self.ncup else None
+            if self.ncup and any(isinstance(m, nn.BatchNorm2d) and m.training for m in self.upsampler.modules()):
+                raise NotImplementedError("weights-net BatchNorm with batch statistics needs the training path (enable grad) "
+                                          "or eval mode: call .eval() / freeze_bn()")
         ws = eng.workspace(image1.device, B, H8, W8, pk.has_mask, self.ncup)
         s = _stream()
         amp = bool(getattr(self.args, "mixed_precision", False))
@@ -131,7 +139,7 @@ class _RAFTBase(nn.Module):
             eng.lookup_resident(ws)
             eng.update_iter(ws, pk, want_mask=(pk.has_mask and need_up))
             if need_up:
-                flow_up = self._upsample(eng, ws, pu)
+                flow_up = upsample(eng, ws, pu)
                 preds.append(flow_up)
         self.update_block.net = eng.net_nchw(ws)
         if test_mode:
@@ -184,10 +192,47 @@ class RAFTNcup(_RAFTBase):
         gptr, gld = eng.guidance(ws)
         return eng.ncup_from_lowres(ws, pu, ws.x4, gptr, gld, 8.0)   # `8 *` of raft_nc_dbl.py:161
 
+    def _upsample_frozen(self, eng, ws, pu):
+        """Upsampling step of the frozen-trunk forward: snapshots what the upsampler consumes into tensors of this forward
+        (the workspace is overwritten by the next iteration, and autograd's backward runs after the engine lock is released),
+        then runs the differentiable upsampler on them."""
+        from .train import ncup_upsampler_frozen
+        B, H8, W8 = ws.B, ws.H8, ws.W8
+        dev = ws.coords1.device
+        s = _stream()
+        x4 = torch.empty(B, 2, 2 * H8, 2 * W8, dtype=torch.float32, device=dev)
+        native.check(eng.L.rnc_flow_x2_fwd(_ptr(ws.coords1), B, H8, W8, _ptr(x4), s), "flow_x2")
+        # the weights-net input cat(x4, area-resized guidance) built straight from the fp32 guidance, channels padded to 136:
+        # the tensor of to_cl(cat(x4, g4), pad_to=136) in ncup_upsampler_train
+        gptr, gld = eng.guidance(ws)
+        gin = torch.empty(B, 2 * H8, 2 * W8, 136, dtype=torch.float32, device=dev)
+        native.check(eng.L.rnc_ncup_guidance_fwd(_ptr(x4), C.c_void_p(gptr), gld, 128, B, H8, W8, _ptr(gin), 136, s), "ncup_guidance")
+        return ncup_upsampler_frozen(self.upsampler, x4, gin, 8.0)   # `8 *` of raft_nc_dbl.py:161
+
     def upsample_flow(self, flow_lr, guidance):
         """raft_nc_dbl.py:107-112 (without the caller's x8): nearest x2, then the NConv upsampler."""
         x4 = torch.nn.functional.interpolate(flow_lr, scale_factor=2, mode="nearest")
         return self.upsampler(x4, guidance)
+
+
+def frozen_trunk(model, image1=None, image2=None, flow_init=None):
+    """Does this forward train the NCUP upsampler of a frozen RAFT only (the reference's --freeze_raft, train.py:295,
+    raft_nc_dbl.py:70-72)?  Then the trunk runs on the inference engine and only the upsampler on autograd.  True when grad is
+    enabled, the model is RAFTNcup, no parameter of fnet / cnet / update_block requires grad while some upsampler parameter
+    does, no input requires grad, every trunk BatchNorm is in eval mode (the tensor-core encoder has no batch statistics) and
+    mixed precision is off."""
+    if not torch.is_grad_enabled() or not isinstance(model, RAFTNcup):
+        return False
+    trunk = (model.fnet, model.cnet, model.update_block)
+    if any(p.requires_grad for m in trunk for p in m.parameters()):
+        return False
+    if not any(p.requires_grad for p in model.upsampler.parameters()):
+        return False
+    if any(t is not None and t.requires_grad for t in (image1, image2, flow_init)):
+        return False
+    if any(isinstance(m, nn.BatchNorm2d) and m.training for t in trunk for m in t.modules()):
+        return False
+    return not getattr(model.args, "mixed_precision", False)
 
 
 class _Dims:

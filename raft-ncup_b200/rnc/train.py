@@ -9,6 +9,8 @@
     CorrLookup      CorrBlock.__call__ (corr.py:23-44): rnc_corr_lookup_fwd / rnc_corr_lookup_bwd (d fmap1, d fmap2 pyramid; coords
                     are detached, raft_nc_dbl.py:149)
     NConv2dFn       NConv2d.forward (nconv_modules.py:164-199): rnc_nconv2d_fwd / rnc_nconv2d_bwd (quotient rule, confidence path)
+    NcupChainFn     the whole NConvUNet chain after the weights net: rnc_ncup_train_fwd / rnc_ncup_bwd (fused, deterministic);
+                    used by the frozen-trunk forward (rnc.model.frozen_trunk), which runs the trunk on the inference engine
 
 Activations stay channel-last ([B, H, W, C] fp32) between convolutions.  Pointwise glue (ReLU / sigmoid / tanh / gate blend,
 cat, nearest x2, zero-stuffing, the loss) and the normalisation layers (InstanceNorm / BatchNorm: library kernels, like cuDNN
@@ -446,6 +448,78 @@ def nconv_unet_train(net, data, conf):
     x, c = NConv2dFn.apply(x, c, net.nconv_x2[0].weight, net.nconv_x2[0].eps)
     x, c = NConv2dFn.apply(torch.cat((x, x), 1), torch.cat((c, c), 1), net.decoder[0].weight, net.decoder[0].eps)
     return NConv2dFn.apply(x, c, net.nconv_out.weight, net.nconv_out.eps)
+
+
+class NcupChainFn(torch.autograd.Function):
+    """Zero-stuffing + the live NConvUNet chain + out_scale (upsampler.py:143-177 after the weights net, nconv_modules.py:106-136)
+    as one fused kernel forward (rnc_ncup_train_fwd) and one fused backward (rnc_ncup_bwd):
+    (x_lowres, conf) NCHW [B,2,H4,W4], the positive kernels W1 [2,1,5,5], W2 [2,2,5,5], W3 [2,4,3,3], W4 [1,2,1,1]
+    -> out NCHW [B,2,4*H4,4*W4].  The same function as the per-layer NConv2dFn chain of ncup_upsampler_train, with gradients
+    that are bit-identical from call to call."""
+
+    SHAPES = ((2, 1, 5, 5), (2, 2, 5, 5), (2, 4, 3, 3), (1, 2, 1, 1))
+
+    @staticmethod
+    def forward(ctx, x_lowres, conf, w1, w2, w3, w4, out_scale):
+        if x_lowres.dim() != 4 or x_lowres.shape[1] != 2 or conf.shape != x_lowres.shape:
+            raise ValueError("NcupChainFn: x_lowres and conf must both be [B,2,H4,W4]")
+        if tuple(tuple(w.shape) for w in (w1, w2, w3, w4)) != NcupChainFn.SHAPES:
+            raise ValueError(f"NcupChainFn: weights must have shapes {NcupChainFn.SHAPES}")
+        eng = engine_for(x_lowres.device)
+        x_lowres, conf = x_lowres.detach().float().contiguous(), conf.detach().float().contiguous()
+        wts = torch.cat([w.detach().float().reshape(-1) for w in (w1, w2, w3, w4)])
+        B, _, H4, W4 = x_lowres.shape
+        out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
+        native.check(eng.L.rnc_ncup_train_fwd(_ptr(x_lowres), _ptr(conf), _ptr(wts), B, H4, W4, float(out_scale), _ptr(out),
+                                              _stream()), "ncup_train_fwd")
+        ctx.save_for_backward(x_lowres, conf, wts)
+        ctx.out_scale = float(out_scale)
+        return out
+
+    @staticmethod
+    def backward(ctx, g_out):
+        x_lowres, conf, wts = ctx.saved_tensors
+        eng = engine_for(x_lowres.device)
+        B, _, H4, W4 = x_lowres.shape
+        need_w = any(ctx.needs_input_grad[2:6])
+        with torch.cuda.device(x_lowres.device):
+            g_out = g_out.float().contiguous()
+            g_x = torch.empty_like(x_lowres) if ctx.needs_input_grad[0] else None
+            g_c = torch.empty_like(conf) if ctx.needs_input_grad[1] else None
+            g_w = ws = None
+            if need_w:
+                g_w = torch.empty(224, dtype=torch.float32, device=x_lowres.device)
+                nbytes = eng.L.rnc_ncup_bwd_workspace_bytes(B, H4, W4)
+                ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=x_lowres.device)
+            if g_x is None and g_c is None and g_w is None:
+                return (None,) * 7
+            native.check(eng.L.rnc_ncup_bwd(_ptr(x_lowres), _ptr(conf), _ptr(wts), B, H4, W4, ctx.out_scale, _ptr(g_out), _ptr(g_x),
+                                            _ptr(g_c), _ptr(g_w), _ptr(ws), ws.numel() * 8 if ws is not None else 0, _stream()),
+                         "ncup_bwd")
+        gws = [None] * 4
+        if g_w is not None:
+            off = 0
+            for k, shp in enumerate(NcupChainFn.SHAPES):
+                n = shp[0] * shp[1] * shp[2] * shp[3]
+                gws[k] = g_w[off:off + n].view(shp) if ctx.needs_input_grad[2 + k] else None
+                off += n
+        return (g_x, g_c, *gws, None)
+
+
+def ncup_chain_autograd(net, x_lowres, conf, out_scale=1.0):
+    """The NConvUNet `net` (live path) on zero-stuffed (x_lowres, conf), times out_scale, through NcupChainFn."""
+    _require_cuda(x_lowres, conf)
+    return NcupChainFn.apply(x_lowres, conf, net.nconv_in.weight, net.nconv_x2[0].weight, net.decoder[0].weight,
+                             net.nconv_out.weight, out_scale)
+
+
+def ncup_upsampler_frozen(up, x4, gin, out_scale=8.0):
+    """NConvUpsampler.forward (upsampler.py:143-177) for a frozen trunk: x4 NCHW [B,2,H4,W4] and the weights-net input gin
+    (CL [B,H4,W4,136] = cat(x4, area-resized guidance), zero channels beyond 130; rnc_ncup_guidance_fwd) are the trunk's
+    detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn."""
+    with torch.cuda.device(x4.device):
+        conf = simple_cl(up.weights_est_net, gin)
+        return ncup_chain_autograd(up.interpolation_net, x4, conf, out_scale)
 
 
 def zero_stuff(x, scale=4):
