@@ -1,6 +1,7 @@
-// wgmma implicit-GEMM convolution: persistent CTAs, TMA-staged 128B-swizzled operand rings fed by one producer warp, two
-// consumer warpgroups that each issue wgmma (M64 x N<=256 x K16) for 64 of the tile's 128 rows and keep the fp32
-// accumulators in registers, then run the epilogue of the tile themselves.
+// wgmma implicit-GEMM convolution: persistent CTAs of four warpgroups.  A producer warp feeds TMA-staged 128B-swizzled
+// operand rings; two MMA warpgroups each issue wgmma (M64 x N<=256 x K16) for 64 of the tile's 128 rows with the fp32
+// accumulators in registers and hand the finished tile to an epilogue warpgroup through a shared-memory accumulator
+// tile, then go straight on to the next tile's K loop: the epilogue of tile i runs under the MMAs of tile i + 1.
 // Replaces: core/update.py:33-60 (SepConvGRU), :79-97 (BasicMotionEncoder), :6-14 (FlowHead), :123-126 (mask head), the 3x3
 // layers of core/interp_weights_est.py:10-47 and (stride 1/2, residual epilogue) the convolutions of
 // core/extractor.py:6-56,118-192.
@@ -17,25 +18,25 @@
 //   COLHALO  kw == 1: tile = 8 x 16 px with a vertical halo, the kh taps are descriptors shifted by ky*16 rows
 // A fourth input form, RNC_CONV_WINDOW, reads in0 through a sliding-window tensor map (dimension 1 steps fewer bytes than
 // dimension 0 spans): the TMA unit builds im2col rows of a small-Cin layer (the encoders' 7x7/2 stem) without a copy.
-// Epilogue: registers -> a staged accumulator tile (thread = pixel) -> per-warp swizzled staging in shared memory ->
+// Epilogue: registers -> the staged accumulator tile (thread = pixel) -> per-warp swizzled staging in shared memory ->
 // cp.async.bulk.tensor stores (split halves, fp32 outputs, the GRU state); fused InstanceNorm sums read the staged chunk column-wise.
 #include "umma_ptx.cuh"
 
 namespace rnc {
 namespace umma {
 
-constexpr int kThreads = 288;        // warps 0-7: two consumer warpgroups (wgmma on 64 rows each + epilogue), warp 8: TMA producer
+// warpgroup 0: TMA producer (one warp issues, the rest exit), 1-2: wgmma on rows 0-63 / 64-127, 3: epilogue (thread = pixel)
+constexpr int kThreads = 512;
+// Registers per thread after setmaxnreg: 40 + 2 x 168 + 136 = 512 (x 128 threads = the 64K register file).  168 holds
+// the 128 fp32 accumulators of a 128-column tile plus the K loop's addresses without spilling.
+constexpr int kRegProducer = 40, kRegMma = 168, kRegEpilogue = 136;
 constexpr int kBM = 128;
 constexpr int kBK = 64;
 constexpr int kMaxSA = 4, kMaxSB = 12;
-constexpr int kStageWarp = 4096;     // epilogue staging per consumer warp: 32 px x 32 ch as [hi 2 KB | lo 2 KB] halves or 4 KB of fp32
-constexpr int kStageBytes = 8 * kStageWarp;
-constexpr int kAccCols = 64;         // accumulator columns staged in shared memory per epilogue pass
-constexpr int kAccStride = kAccCols + 4;    // floats per staged pixel row: conflict-free 16-byte reads of a pixel's chunk
-constexpr int kAccBytes = kBM * kAccStride * 4;
-constexpr int kSmemFixed = 1024 + 512 + 8192 + 1024 + kAccBytes + kStageBytes;   // alignment, barriers, statistics, staging
+constexpr int kStageWarp = 4096;     // epilogue staging per epilogue warp: 32 px x 32 ch as [hi 2 KB | lo 2 KB] halves or 4 KB of fp32
+constexpr int kStageBytes = 4 * kStageWarp;
+constexpr int kStatBytes = 8192;     // fused InstanceNorm partial sums: [4 warps][<= 4 chunks][32 lanes][2] doubles
 constexpr int kSmemMax = 226 * 1024;      // 227 KB per block, less the 1 KB the system reserves on sm_90
-constexpr int kRingBudget = kSmemMax - kSmemFixed;   // A + B rings
 enum { MODE_TAP = 0, MODE_ROWHALO = 1, MODE_COLHALO = 2 };
 
 struct Params {
@@ -75,8 +76,15 @@ template <int BN>
 struct Cfg {
   static constexpr int kBTile = BN * kBK * 2;                     // bytes per half-plane of weights
   static constexpr int kChunksN = BN / 32;                        // 32-channel epilogue chunks
-  static constexpr int kPasses = (BN + kAccCols - 1) / kAccCols;  // epilogue passes over the staged accumulator tile
+  static constexpr int kAccStride = BN + 4;                       // floats per staged pixel row: conflict-free 16-byte reads of a pixel's chunk
+  static constexpr int kAccBytes = kBM * kAccStride * 4;
+  static constexpr int kSmemFixed = 1024 + 512 + kStatBytes + 1024 + kStageBytes + kAccBytes;   // alignment, barriers, statistics, staging, accumulators
+  static constexpr int kRingBudget = kSmemMax - kSmemFixed;      // A + B rings
 };
+
+static int ring_budget(int bn) {
+  return bn == 32 ? Cfg<32>::kRingBudget : bn == 64 ? Cfg<64>::kRingBudget : Cfg<128>::kRingBudget;
+}
 
 // Each thread's accumulators of one 64-row half of the tile: `main` (d[0, BN/2)) takes the x_hi*w_hi products, `corr`
 // (d[BN/2, BN)) the two 2^-11-smaller cross terms.  The tensor core truncates on every accumulate, so the error grows with the
@@ -94,16 +102,15 @@ __device__ __forceinline__ void mma_block(float* d, uint64_t ah, uint64_t al, ui
   }
 }
 
-// Columns [P*64, P*64 + 64) of main + corr (already summed into d[0, BN/2)) -> the staged accumulator tile [128 px][kAccStride] (rows of this warpgroup)
-template <int BN, int P>
+// main + corr (already summed into d[0, BN/2)) -> the staged accumulator tile [128 px][kAccStride] (rows of this warpgroup)
+template <int BN>
 __device__ __forceinline__ void stash_acc(const float* d, float* acc_tile, int row0, int lane) {
-  constexpr int j0 = P * kAccCols / 8, j1 = (P + 1) * kAccCols / 8 < BN / 8 ? (P + 1) * kAccCols / 8 : BN / 8;
+  constexpr int S = Cfg<BN>::kAccStride;
   const int c0 = 2 * (lane & 3);
 #pragma unroll
-  for (int j = j0; j < j1; ++j) {
-    const int col = 8 * j + c0 - P * kAccCols;
-    *reinterpret_cast<float2*>(acc_tile + row0 * kAccStride + col) = make_float2(d[4 * j], d[4 * j + 1]);
-    *reinterpret_cast<float2*>(acc_tile + (row0 + 8) * kAccStride + col) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(acc_tile + row0 * S + 8 * j + c0) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(acc_tile + (row0 + 8) * S + 8 * j + c0) = make_float2(d[4 * j + 2], d[4 * j + 3]);
   }
 }
 
@@ -112,7 +119,6 @@ __device__ __forceinline__ void stash_acc(const float* d, float* acc_tile, int r
 // gates, 2 = GRU q, 3 = the rest (flow append, residual tail, tanh|relu head, coords update, fused InstanceNorm sums).
 enum { EC_PLAIN = 0, EC_GRU_ZR = 1, EC_GRU_Q = 2, EC_MISC = 3 };
 
-// 9 warps: the SM sub-partition holding three of them caps the kernel at 168 registers per thread
 template <int BN, int EC>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant__ CUtensorMap mA0l,
@@ -132,15 +138,17 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
   uint64_t* a_empty = a_full + kMaxSA;
   uint64_t* b_full = a_empty + kMaxSA;
   uint64_t* b_empty = b_full + kMaxSB;
-  double* stat_acc = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(bars) + 512);   // [8 warps][passes][32 lanes][2]
+  uint64_t* acc_full = b_empty + kMaxSB;           // the MMA warpgroups have written a tile into acc_tile
+  uint64_t* acc_empty = acc_full + 1;              // the epilogue warpgroup has read it
+  double* stat_acc = reinterpret_cast<double*>(reinterpret_cast<unsigned char*>(bars) + 512);   // [4 warps][chunks][32 lanes][2]
   // epilogue staging (TMA-store source), 1024-aligned so the 64B / 128B swizzle patterns are functions of the buffer offset,
   // then the staged accumulator tile
   unsigned char* stage_base = reinterpret_cast<unsigned char*>(
-      (reinterpret_cast<uintptr_t>(bars) + 512 + 8192 + 1023) & ~uintptr_t(1023));
+      (reinterpret_cast<uintptr_t>(bars) + 512 + kStatBytes + 1023) & ~uintptr_t(1023));
   float* acc_tile = reinterpret_cast<float*>(stage_base + kStageBytes);
 
   pdl_trigger();                       // the next kernel in the stream may begin its prologue on SMs this grid has left
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wgi = warp >> 2;
   const int tpi = p.tiles_x * p.tiles_y;
   const int G = p.mode == MODE_TAP ? p.kh * p.kw : p.mode == MODE_ROWHALO ? p.kh : 1;     // A-stage groups per channel block
   const int T = p.mode == MODE_TAP ? 1 : p.mode == MODE_ROWHALO ? p.kw : p.kh;            // taps sharing one A stage
@@ -150,12 +158,16 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.SA; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 8); }
     for (int s = 0; s < p.SB; ++s) { mbar_init(&b_full[s], 1); mbar_init(&b_empty[s], 8); }
+    mbar_init(acc_full, 256);
+    mbar_init(acc_empty, 128);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
   pdl_wait();                          // everything above overlapped the predecessor's tail; its results are visible from here
 
-  if (warp == 8) {
+  if (wgi == 0) {
+    setmaxnreg_dec<kRegProducer>();
+    if (warp != 0) return;
     // ------------------------------------------------------------------ TMA producer
     // The whole warp runs the loop so that addresses / coordinates stay in uniform registers; one elected lane issues.
     // Ring positions are (slot, parity) counters: a runtime modulo per stage costs ~100 cycles of dependent integer code.
@@ -206,40 +218,104 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
     return;
   }
 
-  // -------------------------------------------------------------------- consumers: wgmma main loop, then the epilogue
-  const int wg = warp >> 2;                        // warpgroup: rows [64 wg, 64 wg + 64) of the tile
-  const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // accumulator rows row0, row0 + 8 of this thread
-  float d[BN];                                     // main | corr
-  const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-  const uint32_t t_rows = p.mode == MODE_ROWHALO ? 1u : p.mode == MODE_COLHALO ? static_cast<uint32_t>(p.TW) : 0u;   // tap shift in rows
+  if (wgi < 3) {
+    // ------------------------------------------------------------------ MMA warpgroups: K loop, then hand the tile over
+    setmaxnreg_inc<kRegMma>();
+    const int wg = wgi - 1;                        // rows [64 wg, 64 wg + 64) of the tile
+    const int row0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // accumulator rows row0, row0 + 8 of this thread
+    float d[BN];                                   // main | corr
+    const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
+    const uint32_t t_rows = p.mode == MODE_ROWHALO ? 1u : p.mode == MODE_COLHALO ? static_cast<uint32_t>(p.TW) : 0u;   // tap shift in rows
+    int sa_n = 0, pa_n = 0, sb_n = 0, pb_n = 0;
+    uint32_t acc_ph = 0;
+    // With deeper rings one batch stays in flight: a batch's stages are released once the next batch has been issued and
+    // wgmma_wait<1> has seen the earlier one complete.  A 2-stage ring would then leave the producer nothing to refill
+    // ahead, so there each batch is drained and released at once.
+    const bool lag = p.SA > 2 && p.SB > 2;
+    for (int item = item0; item < items; item += item_step) {
+      // K = taps x channel blocks, one wgmma batch per weight stage
+      int first = 1, rel_a = -1, rel_b = -1;
+      for (int g = 0; g < G; ++g)
+        for (int cb = 0; cb < p.nblk; ++cb) {
+          const int sa = sa_n, pa = pa_n;
+          if (++sa_n == p.SA) { sa_n = 0; pa_n ^= 1; }
+          mbar_wait(&a_full[sa], pa);
+          for (int t = 0; t < T; ++t) {
+            const int sb = sb_n, pb = pb_n;
+            if (++sb_n == p.SB) { sb_n = 0; pb_n ^= 1; }
+            mbar_wait(&b_full[sb], p.resident_b ? 0 : pb);
+            // A rows of this warpgroup, shifted by the tap (ROWHALO: kx rows, COLHALO: ky image rows of TW pixels)
+            const uint32_t a_addr = sA_u + sa * a_stage + (64u * wg + t * t_rows) * 128u;
+            // no base_offset: with 1024-byte aligned stages the swizzle is a function of the absolute address
+            const uint64_t ah = smem_desc_sw128(a_addr);
+            const uint64_t al = ah + (static_cast<uint32_t>(p.a_plane) >> 4);
+            const uint64_t bh = smem_desc_sw128(sB_u + sb * kBStageBytes), bl = bh + (C::kBTile >> 4);
+            wgmma_fence();
+            if (p.tf32) mma_block<BN, true>(d, ah, al, bh, bl, first); else mma_block<BN, false>(d, ah, al, bh, bl, first);
+            wgmma_commit();
+            first = 0;
+            if (lag) {
+              wgmma_wait<1>();
+            } else {
+              wgmma_wait<0>();
+              rel_b = sb;
+              rel_a = t == T - 1 ? sa : -1;
+            }
+            __syncwarp();
+            if (lane == 0) {
+              if (rel_b >= 0 && !p.resident_b) mbar_arrive(&b_empty[rel_b]);
+              if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+            }
+            rel_b = lag ? sb : -1;
+            rel_a = lag && t == T - 1 ? sa : -1;   // the A stage is free after its last tap's batch
+          }
+        }
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) {
+        if (rel_b >= 0 && !p.resident_b) mbar_arrive(&b_empty[rel_b]);
+        if (rel_a >= 0) mbar_arrive(&a_empty[rel_a]);
+      }
+#pragma unroll
+      for (int i = 0; i < BN; ++i) reg_fence(d[i]);
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] += d[BN / 2 + i];
+      mbar_wait(acc_empty, acc_ph ^ 1);            // the epilogue has read the previous tile
+      stash_acc<BN>(d, acc_tile, row0, lane);
+      mbar_arrive(acc_full);
+      acc_ph ^= 1;
+    }
+    return;
+  }
 
-  // epilogue: thread = pixel; warp w takes lane group w & 3 (pixels 32 (w & 3) + lane), half h = w >> 2 takes the chunks
-  // 2 * pass + h of the staged accumulator columns
-  const int lg = warp & 3, hsel = warp >> 2;
+  // -------------------------------------------------------------------- epilogue warpgroup: thread = pixel
+  // warp w takes pixels 32 (w & 3) + lane of the tile and every 32-channel chunk of the staged accumulator columns
+  setmaxnreg_inc<kRegEpilogue>();
+  const int lg = warp & 3;
   const int ml = lg * 32 + lane;
   const int epi = p.epilogue;
   const bool use_stats = EC == EC_MISC && p.stats != nullptr;
-  double* my_acc = stat_acc + (static_cast<size_t>(warp) * C::kPasses * 32 + lane) * 2;   // [pass] stride 64 doubles
+  double* my_acc = stat_acc + (static_cast<size_t>(lg) * C::kChunksN * 32 + lane) * 2;   // [chunk] stride 64 doubles
   int acc_b = -1, acc_n0 = 0;
   auto flush_stats = [&]() {
     if (acc_b < 0) return;
-    for (int ci = 0; ci < C::kPasses; ++ci) {
-      const int ch = acc_n0 + (2 * ci + hsel) * 32 + lane;
-      if (2 * ci + hsel < C::kChunksN && ch < p.cout) {
+    for (int cc = 0; cc < C::kChunksN; ++cc) {
+      const int ch = acc_n0 + cc * 32 + lane;
+      if (ch < p.cout) {
         double* dst = p.stats + (static_cast<size_t>(acc_b) * p.cout + ch) * 2;
-        atomicAdd(dst, my_acc[ci * 64]);
-        atomicAdd(dst + 1, my_acc[ci * 64 + 1]);
+        atomicAdd(dst, my_acc[cc * 64]);
+        atomicAdd(dst + 1, my_acc[cc * 64 + 1]);
       }
-      my_acc[ci * 64] = 0.0; my_acc[ci * 64 + 1] = 0.0;
+      my_acc[cc * 64] = 0.0; my_acc[cc * 64 + 1] = 0.0;
     }
   };
   if (use_stats) {
-    for (int ci = 0; ci < C::kPasses; ++ci) { my_acc[ci * 64] = 0.0; my_acc[ci * 64 + 1] = 0.0; }
+    for (int cc = 0; cc < C::kChunksN; ++cc) { my_acc[cc * 64] = 0.0; my_acc[cc * 64 + 1] = 0.0; }
   }
   // Outputs leave through shared memory and TMA stores: a warp's 32 px x 32 ch chunk is one box of the output tensor
   // (full 64- / 128-byte rows per pixel instead of 16-byte pieces per thread; image borders are clipped by the TMA unit).
   // The staging rows are written with the map's swizzle (64B for halves, 128B for fp32): conflict-free.
-  unsigned char* stg = stage_base + warp * kStageWarp;
+  unsigned char* stg = stage_base + lg * kStageWarp;
   bool stg_busy = false;                           // warp-uniform: a TMA store may still be reading the staging buffer
   const int lgx = (lg * 32) % p.TW, lgy = (lg * 32) / p.TW;
   int bx = 0, by = 0, bb = 0;                      // box origin of this warp's lane group in the current tile
@@ -274,44 +350,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
     stg_busy = true;
   };
 
-  int sa_n = 0, pa_n = 0, sb_n = 0, pb_n = 0;
+  uint32_t acc_ph = 0;
   for (int item = item0; item < items; item += item_step) {
     const int tile = item / p.ntn, n0 = (item - tile * p.ntn) * BN;
-    // ---- main loop: K = taps x channel blocks, one wgmma batch per weight stage
-    int first = 1;
-    for (int g = 0; g < G; ++g)
-      for (int cb = 0; cb < p.nblk; ++cb) {
-        const int sa = sa_n, pa = pa_n;
-        if (++sa_n == p.SA) { sa_n = 0; pa_n ^= 1; }
-        mbar_wait(&a_full[sa], pa);
-        for (int t = 0; t < T; ++t) {
-          const int sb = sb_n, pb = pb_n;
-          if (++sb_n == p.SB) { sb_n = 0; pb_n ^= 1; }
-          mbar_wait(&b_full[sb], p.resident_b ? 0 : pb);
-          // A rows of this warpgroup, shifted by the tap (ROWHALO: kx rows, COLHALO: ky image rows of TW pixels)
-          const uint32_t a_addr = sA_u + sa * a_stage + (64u * wg + t * t_rows) * 128u;
-          // no base_offset: with 1024-byte aligned stages the swizzle is a function of the absolute address
-          const uint64_t ah = smem_desc_sw128(a_addr);
-          const uint64_t al = ah + (static_cast<uint32_t>(p.a_plane) >> 4);
-          const uint64_t bh = smem_desc_sw128(sB_u + sb * kBStageBytes), bl = bh + (C::kBTile >> 4);
-          wgmma_fence();
-          if (p.tf32) mma_block<BN, true>(d, ah, al, bh, bl, first); else mma_block<BN, false>(d, ah, al, bh, bl, first);
-          wgmma_commit();
-          wgmma_wait<0>();
-          first = 0;
-          __syncwarp();
-          if (!p.resident_b && lane == 0) mbar_arrive(&b_empty[sb]);
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&a_empty[sa]);
-      }
-#pragma unroll
-    for (int i = 0; i < BN; ++i) reg_fence(d[i]);
-    // main + corr once, so that only half of the accumulator registers stay live through the epilogue passes
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) d[i] += d[BN / 2 + i];
-
-    // ---- epilogue
     const int b = tile / tpi, tr = tile - b * tpi;
     if (use_stats && (b != acc_b || n0 != acc_n0)) { flush_stats(); acc_b = b; acc_n0 = n0; }
     const int ty0 = (tr / p.tiles_x) * p.TH, tx0 = (tr % p.tiles_x) * p.TW;
@@ -321,10 +362,10 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
     // tile-blocked tensors (p.aux_blocked / p.out_blocked): element (tile, channel c, row ml) at ((tile * ld + c) * 128 + ml),
     // so a warp's 32 pixels are contiguous per channel
     const size_t pix = (static_cast<size_t>(b) * p.H + y) * p.W + x;
-    auto chunk = [&](int pass, int cc) {
+    auto chunk = [&](int cc) {
       const int n = n0 + cc * 32;
         float v[32];
-        const float4* sv = reinterpret_cast<const float4*>(acc_tile + ml * kAccStride + (cc - 2 * pass) * 32);
+        const float4* sv = reinterpret_cast<const float4*>(acc_tile + ml * C::kAccStride + cc * 32);
 #pragma unroll
         for (int q = 0; q < 8; ++q) {
           const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + n) + q), s = sv[q];
@@ -368,8 +409,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
             s1 += x;
             s2 = fmaf(x, x, s2);
           }
-          my_acc[pass * 64] += static_cast<double>(s1);
-          my_acc[pass * 64 + 1] += static_cast<double>(s2);
+          my_acc[cc * 64] += static_cast<double>(s1);
+          my_acc[cc * 64 + 1] += static_cast<double>(s2);
           return;
         }
         if (EC == EC_GRU_ZR) {
@@ -506,15 +547,12 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
         }
         if (p.out_hi) store_split(v, n);
     };
+    mbar_wait(acc_full, acc_ph);
+    acc_ph ^= 1;
 #pragma unroll 1
-    for (int pass = 0; pass < C::kPasses; ++pass) {
-      named_bar_sync(1, 256);                      // every consumer warp is done with the staged tile of the previous pass
-      if (pass == 0) stash_acc<BN, 0>(d, acc_tile, row0, lane);
-      else if (C::kPasses > 1) stash_acc<BN, (C::kPasses > 1 ? 1 : 0)>(d, acc_tile, row0, lane);
-      named_bar_sync(1, 256);
-      const int cc = 2 * pass + hsel;
-      if (cc < C::kChunksN && n0 + cc * 32 < p.cout + (EC == EC_MISC && epi == RNC_EPI_RELU_FLOW ? 2 : 0)) chunk(pass, cc);
-    }
+    for (int cc = 0; cc < C::kChunksN; ++cc)
+      if (n0 + cc * 32 < p.cout + (EC == EC_MISC && epi == RNC_EPI_RELU_FLOW ? 2 : 0)) chunk(cc);
+    mbar_arrive(acc_empty);                        // every read of the staged tile is done; its stores may still be in flight
   }
   if (use_stats) flush_stats();
   if (lane == 0) bulk_wait_all0();                 // the staging buffer must outlive its TMA stores; their writes complete here
@@ -574,8 +612,9 @@ template <int BN, int EC>
 static int launch(const CUtensorMap* maps, Params& p, cudaStream_t stream, int max_sa, int max_sb) {
   using C = Cfg<BN>;
   const int a_stage = 2 * p.a_plane;
-  // ring depths within kRingBudget: both rings hide the same TMA latency, so deepen A (up to 4) while B keeps >= 2 stages
-  const int budget = kRingBudget, b_stage = 2 * C::kBTile;
+  // ring depths within the shared memory the accumulator tile and the staging leave: both rings hide the same TMA
+  // latency, so deepen A (up to 4) while B keeps >= 2 stages
+  const int budget = C::kRingBudget, b_stage = 2 * C::kBTile;
   const int sa_cap = max_sa > 0 && max_sa < kMaxSA ? max_sa : kMaxSA;      // debug knobs (rnc_conv_umma_desc.flags bits 8-15)
   p.SA = 2;
   while (p.SA < sa_cap && budget - (p.SA + 1) * a_stage >= 2 * b_stage) ++p.SA;
@@ -587,12 +626,12 @@ static int launch(const CUtensorMap* maps, Params& p, cudaStream_t stream, int m
   p.resident_b = 0;
   {
     const int nb = p.kh * p.kw * p.nblk;
-    if (p.ntn == 1 && nb <= kMaxSB && nb > p.SB && max_sb == 0 && 2 * a_stage + nb * b_stage <= kRingBudget) {
-      p.resident_b = 1; p.SB = nb; p.SA = (kRingBudget - nb * b_stage) / a_stage;
+    if (p.ntn == 1 && nb <= kMaxSB && nb > p.SB && max_sb == 0 && 2 * a_stage + nb * b_stage <= budget) {
+      p.resident_b = 1; p.SB = nb; p.SA = (budget - nb * b_stage) / a_stage;
       if (p.SA > kMaxSA) p.SA = kMaxSA;
     }
   }
-  const int smem = p.SA * a_stage + p.SB * b_stage + kSmemFixed;
+  const int smem = p.SA * a_stage + p.SB * b_stage + C::kSmemFixed;
   if (smem > kSmemMax) return RNC_ERR_UNSUPPORTED;
   static unsigned long long done = 0;
   if (int st = ensure_dyn_smem(conv_umma_kernel<BN, EC>, kSmemMax, &done)) return st;
@@ -752,7 +791,7 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
   p.ntiles = d.B * p.tiles_x * p.tiles_y; p.ntn = d.coutpad / bn;
   p.a_plane = box_w * box_h * 128;
   // tall halo boxes (COLHALO, kh >= 5) beside 128-column weight stages leave no room for two stages of each ring
-  while (bn > 32 && 2 * 2 * p.a_plane + 2 * 2 * bn * bk * (tf32 ? 4 : 2) > kRingBudget && d.coutpad % (bn >> 1) == 0) bn >>= 1;
+  while (bn > 32 && 2 * 2 * p.a_plane + 2 * 2 * bn * bk * (tf32 ? 4 : 2) > ring_budget(bn) && d.coutpad % (bn >> 1) == 0) bn >>= 1;
   p.ntn = d.coutpad / bn;
   p.nblk0 = nblk0; p.nblk = nblk; p.bk = bk; p.tf32 = tf32 ? 1 : 0;
   p.cout = d.cout; p.epilogue = d.epilogue; p.unscale = d.unscale; p.bias = d.bias;

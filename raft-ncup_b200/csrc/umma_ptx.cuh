@@ -116,6 +116,12 @@ template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // keeps the compiler from moving accumulator reads above wgmma_wait
 __device__ __forceinline__ void reg_fence(float& r) { asm volatile("" : "+f"(r)::"memory"); }
+// Per-warpgroup register budget (all four warps of the warpgroup execute it): a producer hands registers back, the
+// accumulator-holding warpgroups take them.  R is a multiple of 8 in [24, 256].
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R) : "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R) : "memory"); }
 
 template <int N, bool TF32>
 __device__ __forceinline__ void wgmma(float* d, uint64_t a, uint64_t b, int scale_d);
