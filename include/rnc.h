@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 11) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 12) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -347,25 +347,48 @@ int rnc_bilinear_sample_fwd(const float* img, const float* coords, int N, int C,
 
 /* ------------------------------------------------------------------------------------------------
  * U6  NConv2d.forward  (core/nconv_modules.py:164-199) — ONE normalized-convolution layer, the operator seam
- *     `NConv2d((data, conf)) -> (y, conf_out)`, and the per-layer form the training path differentiates through
- *     (the inference path runs the fused chain rnc_ncup_fwd instead).
- *   data, conf : NCHW [N][Cin][H][W] fp32;  weight: [Cout][Cin][kh][kw] fp32 = softplus_{beta=10}(weight_p)
- *                (nconv_modules.py:250-264; the caller applies it), zero padding k/2, stride 1, no bias
- *   y = conv(data*conf, W) / (conv(conf, W) + eps),   conf_out = conv(conf, W) / sum_{i,ky,kx} W[o]
- * Supported: Cin, Cout <= 4, odd kh, kw <= 7.
+ *     `NConv2d((data, conf)) -> (y, conf_out)`, the per-layer form the training path differentiates through, and the
+ *     per-level chain of every NConvUNet configuration other than the shipped one (which runs the fused rnc_ncup_fwd).
+ *   The input is the channel concatenation [up, full]: Cup channels of up_data/up_conf NCHW [N][Cup][Hup][Wup], read at
+ *   full resolution through F.interpolate(mode='nearest', size=(H, W))'s index map min(floor(dst * (in/out)), in-1)
+ *   (the decoder's `cat(F.interpolate(x_prev), skip)`, nconv_modules.py:129-131; Cup = 0 -> no up source, pointers
+ *   ignored), then Cin channels of data/conf NCHW [N][Cin][H][W].
+ *   weight: [Cout][Cup+Cin][kh][kw] fp32 = softplus_{beta=10}(weight_p) (nconv_modules.py:250-264; the caller applies it),
+ *   zero padding k/2, stride 1;  bias: [Cout] or NULL
+ *   y = (conv(data*conf, W) / (conv(conf, W) + eps) + bias) * y_scale,   conf_out = conv(conf, W) / sum_{i,ky,kx} W[o]
+ *   (y_scale folds a caller's output scale into the last layer; 1 elsewhere.)
+ * Supported: Cup + Cin <= 8, Cout <= 4, odd kh, kw <= 7.
  */
-int rnc_nconv2d_fwd(const float* data, const float* conf, const float* weight, int N, int Cin, int Cout, int H, int W,
-                    int kh, int kw, float eps, float* y, float* conf_out, void* stream);
-/* Backward of rnc_nconv2d_fwd (autograd of nconv_modules.py:169-194: quotient rule through num/(den+eps), confidence
- * propagation incl. its dependence on sum(W)).  g_y / g_conf_out: upstream gradients (either may be NULL = zero);
- * g_data, g_conf, g_weight ([Cout][Cin][kh][kw], w.r.t. the POSITIVE kernel; the caller chains softplus'): outputs, each
- * may be NULL.  workspace: rnc_nconv2d_bwd_workspace_bytes(N,Cout,H,W) bytes, ZERO-INITIALISED by the caller before its
- * first use (the call leaves its accumulators zeroed again). */
-size_t rnc_nconv2d_bwd_workspace_bytes(int N, int Cout, int H, int W);
-int rnc_nconv2d_bwd(const float* data, const float* conf, const float* weight, const float* y, const float* conf_out,
-                    const float* g_y, const float* g_conf_out, int N, int Cin, int Cout, int H, int W, int kh, int kw,
-                    float eps, float* g_data, float* g_conf, float* g_weight, void* workspace, size_t workspace_bytes,
-                    void* stream);
+int rnc_nconv2d_fwd(const float* data, const float* conf, const float* weight, const float* bias, int N, int Cin, int Cout,
+                    int H, int W, int kh, int kw, float eps, const float* up_data, const float* up_conf, int Cup, int Hup,
+                    int Wup, float y_scale, float* y, float* conf_out, void* stream);
+/* Backward of rnc_nconv2d_fwd at y_scale = 1 (autograd of nconv_modules.py:169-194: quotient rule through num/(den+eps),
+ * bias, confidence propagation incl. its dependence on sum(W)).  y, conf_out: the forward's outputs (same bias).
+ * g_y / g_conf_out: upstream gradients (either may be NULL = zero); g_data, g_conf ([N][Cin][H][W]), g_up_data, g_up_conf
+ * ([N][Cup][Hup][Wup]: each coarse pixel sums the full-resolution pixels that read it), g_weight ([Cout][Cup+Cin][kh][kw],
+ * w.r.t. the POSITIVE kernel; the caller chains softplus'), g_bias ([Cout], needs g_weight): outputs, each may be NULL.
+ * With a bias, the quotient num/(den+eps) is recovered as y - bias from the forward's rounded output (an error of an ulp
+ * of y, against autograd's exact quotient); den is recovered as conf_out * sum(W), as without a bias.
+ * workspace: rnc_nconv2d_bwd_workspace_bytes(...) bytes, 16-byte aligned, no zeroing needed.  Every reduction runs in a
+ * fixed order: identical inputs give bit-identical gradients. */
+size_t rnc_nconv2d_bwd_workspace_bytes(int N, int Cin, int Cup, int Cout, int H, int W, int kh);
+int rnc_nconv2d_bwd(const float* data, const float* conf, const float* weight, const float* bias, const float* y,
+                    const float* conf_out, const float* g_y, const float* g_conf_out, int N, int Cin, int Cout, int H, int W,
+                    int kh, int kw, float eps, const float* up_data, const float* up_conf, int Cup, int Hup, int Wup,
+                    float* g_data, float* g_conf, float* g_up_data, float* g_up_conf, float* g_weight, float* g_bias,
+                    void* workspace, size_t workspace_bytes, void* stream);
+
+/* U6  NConvUNet.downsample_data_conf (core/nconv_modules.py:94-104), ds_factor 2:
+ *   conf_out = max_pool2d(conf, 2, 2) / 4 (floor mode; the first maximum in row-major window order wins, as F.max_pool2d);
+ *   data_out = data at the confidence argmax (max_pool_data = 0, 'conf_based') or max_pool2d(data, 2, 2) (1, 'max_pooling').
+ *   data, conf NCHW [N][C][H][W], H, W >= 2;  data_out, conf_out [N][C][H/2][W/2];
+ *   idx: int32 [2][N][C][H/2][W/2], written: the in-plane flat index (y*W + x) of the confidence argmax, then of the data's.
+ * rnc_nconv_pool2_bwd routes g_conf_out / 4 and g_data_out (either may be NULL = zero) to those argmaxes; g_data, g_conf
+ * [N][C][H][W] (either may be NULL) are fully written (zero elsewhere). */
+int rnc_nconv_pool2_fwd(const float* data, const float* conf, int N, int C, int H, int W, int max_pool_data, float* data_out,
+                        float* conf_out, int* idx, void* stream);
+int rnc_nconv_pool2_bwd(const int* idx, const float* g_data_out, const float* g_conf_out, int N, int C, int H, int W,
+                        float* g_data, float* g_conf, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * Training path (train.py:203-227; SURVEY.md §8f-3, Appendix G): backward kernels, exact fp32.

@@ -19,6 +19,7 @@ import torch.nn.functional as F
 
 from . import native
 from .native import ConvDesc
+from .nconv_unet import PackedUNet, is_fused
 
 CORR_CH = 324          # 4 levels * 9 * 9
 HX_LD = 384            # [h | inp | motion(126) flow(2)]
@@ -149,11 +150,13 @@ class PackedUpsampler:
         self.c_mid0, self.c_mid1 = convs[0][0].shape[0], convs[1][0].shape[0]
         self.gout = (pack_thin(wn.out.weight), wn.out.bias.detach().float().contiguous())
         net = up.interpolation_net
-        ws = [F.softplus(p.detach().float(), beta=10).reshape(-1).cpu() for p in
-              (net.nconv_in.weight_p, net.nconv_x2[0].weight_p, net.decoder[0].weight_p, net.nconv_out.weight_p)]
-        host = torch.cat(ws).contiguous()
-        assert host.numel() == 224, "NCUP kernel is built for the shipped interp_net config (SURVEY.md §5)"
-        self.nconv_host = (C.c_float * 224)(*host.tolist())
+        self.nconv_host = self.unet = None
+        if is_fused(net):
+            ws = [F.softplus(p.detach().float(), beta=10).reshape(-1).cpu() for p in
+                  (net.nconv_in.weight_p, net.nconv_x2[0].weight_p, net.decoder[0].weight_p, net.nconv_out.weight_p)]
+            self.nconv_host = (C.c_float * 224)(*torch.cat(ws).tolist())
+        else:
+            self.unet = PackedUNet(net)       # every other configuration: the per-level chain of rnc/nconv_unet.py
 
 
 def _checksum(tensors):
@@ -522,7 +525,27 @@ class Engine:
         self.conv(B, H4, W4, ws.g1.data_ptr(), pu.c_mid0, 64, pu.g1, pu.c_mid1, 3, 3, native.EPI_RELU, ws.g2.data_ptr(), 32)
         native.check(self.L.rnc_conf_head_fwd(_ptr(ws.g2), pu.c_mid1, 32, _ptr(pu.gout[0]), _ptr(pu.gout[1]), B, H4, W4,
                                               _ptr(ws.conf), s), "conf_head")
-        out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
+        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)
+
+    def ncup_chain(self, ws, pu, x_lowres, conf, out_scale):
+        """Zero-stuffing + NConvUNet + out_scale (upsampler.py:150-177) on x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4]:
+        the fused rnc_ncup_fwd for the shipped network, the per-level chain of rnc/nconv_unet.py for any other.  Neither
+        synchronises with the host, so graph capture records either."""
+        B, _, H4, W4 = x_lowres.shape
+        if pu.unet is None:
+            out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
+            with _Timed(self, "ncup"):
+                native.check(self.L.rnc_ncup_fwd(_ptr(x_lowres), _ptr(conf), pu.nconv_host, B, H4, W4, out_scale, _ptr(out),
+                                                 _stream()), "ncup")
+            return out
+        # intermediates live in the workspace (allocated by the first, eager forward of a shape; graph capture reuses them)
+        bufs = ws.__dict__.setdefault("nconv_bufs", {})
+        if "stuffed" not in bufs:
+            # zero-stuffing (upsampler.py:179-210): only the lattice is ever written, so the zeros are laid down once
+            bufs["stuffed"] = torch.zeros(2, B * 2, 1, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
+        xh, ch = bufs["stuffed"]
         with _Timed(self, "ncup"):
-            native.check(self.L.rnc_ncup_fwd(_ptr(x_lowres), _ptr(ws.conf), pu.nconv_host, B, H4, W4, out_scale, _ptr(out), s), "ncup")
-        return out
+            xh.view(B, 2, 4 * H4, 4 * W4)[:, :, 2::4, 2::4] = x_lowres
+            ch.view(B, 2, 4 * H4, 4 * W4)[:, :, 2::4, 2::4] = conf
+            out, _ = pu.unet.run(xh, ch, out_scale, bufs)
+        return out.view(B, 2, 4 * H4, 4 * W4)

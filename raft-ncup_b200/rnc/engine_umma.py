@@ -380,7 +380,6 @@ class UmmaEngine(Engine):
     def ncup_from_lowres(self, ws, pu, x_lowres, guid_ptr, ldg, out_scale):
         B, H8, W8 = ws.B, ws.H8, ws.W8
         H4, W4 = 2 * H8, 2 * W8
-        M4 = B * H4 * W4
         s = _stream()
         L = self.L
         native.check(L.rnc_ncup_guidance_split_fwd(_ptr(x_lowres), C.c_void_p(guid_ptr), ldg, 128, B, H8, W8, _ptr(ws.gin.hi),
@@ -389,7 +388,4 @@ class UmmaEngine(Engine):
         self.uconv(B, H4, W4, ws.g1.ptrs(), 64, 64, pu.u1, native.EPI_RELU, out_f32=ws.g2.data_ptr(), ldo_f32=32)
         native.check(L.rnc_conf_head_fwd(_ptr(ws.g2), pu.c_mid1, 32, _ptr(pu.gout[0]), _ptr(pu.gout[1]), B, H4, W4, _ptr(ws.conf), s),
                      "conf_head")
-        out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
-        with _Timed(self, "ncup"):
-            native.check(L.rnc_ncup_fwd(_ptr(x_lowres), _ptr(ws.conf), pu.nconv_host, B, H4, W4, out_scale, _ptr(out), s), "ncup")
-        return out
+        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)

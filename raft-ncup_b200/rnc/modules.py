@@ -14,6 +14,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import native
+from .nconv_unet import PackedUNet, is_fused, nconv_fwd
 from .engine import (CORR_CH, HX_LD, PackedFlowHead, PackedGRU, PackedMotionEncoder, _ptr, _require_cuda, _stream, engine_for,
                      module_tensors, pack_conv, pack_thin)
 
@@ -299,18 +300,27 @@ class BasicUpdateBlock(nn.Module):
 
 class NConv2d(nn.Module):
     """core/nconv_modules.py:140-215: stores ``weight_p``; the effective kernel is softplus(weight_p, beta=10) (EnforcePos,
-    :218-269), recomputed at every forward.  forward((data, conf)) -> (nconv, conf_out), NCHW, through rnc_nconv2d_fwd."""
+    :218-269), recomputed at every forward.  forward((data, conf)) -> (nconv, conf_out), NCHW, through rnc_nconv2d_fwd.
+    With bias, ``nconv += bias`` follows the division and the confidence is unaffected (:175-179)."""
 
     def __init__(self, in_channels, out_channels, kernel_size, pos_fn="softplus", bias=False):
         super().__init__()
-        if bias or pos_fn.lower() != "softplus":
-            raise NotImplementedError("only the shipped NConv config (SoftPlus, no bias) is built")
+        if pos_fn.lower() != "softplus":
+            raise NotImplementedError(f"NConv2d pos_fn={pos_fn!r}: only SoftPlus is built")
         self.in_channels, self.out_channels, self.kernel_size = in_channels, out_channels, tuple(kernel_size)
         self.eps = 1e-20
         w = torch.empty(out_channels, in_channels, *self.kernel_size)
-        nn.init.kaiming_uniform_(w, a=math.sqrt(5))         # _ConvNd.reset_parameters: consumed, then overwritten (:207-209)
+        # _ConvNd.reset_parameters draws the weight, then the bias; both are drawn again by init_parameters (:201-215)
+        nn.init.kaiming_uniform_(w, a=math.sqrt(5))
+        bound = 1 / math.sqrt(in_channels * self.kernel_size[0] * self.kernel_size[1])
+        if bias:
+            torch.empty(out_channels).uniform_(-bound, bound)
         n = self.kernel_size[0] * self.kernel_size[1] * out_channels
         w.normal_(2, math.sqrt(2.0 / n))
+        if bias:
+            self.bias = nn.Parameter(torch.empty(out_channels).uniform_(-bound, bound))
+        else:
+            self.register_parameter("bias", None)
         self.weight_p = nn.Parameter(F.softplus(w, beta=10))
 
     @property
@@ -321,51 +331,70 @@ class NConv2d(nn.Module):
         data, conf = inpt[0], inpt[1]
         if _grad_needed(self, data, conf):
             from .train import nconv2d_autograd
-            return nconv2d_autograd(data, conf, self.weight, self.eps)
-        return nconv2d_forward(data, conf, self.weight.detach(), self.eps)
+            return nconv2d_autograd(data, conf, self.weight, self.eps, self.bias)
+        return nconv2d_forward(data, conf, self.weight.detach(), self.eps, self.bias)
 
 
-def nconv2d_forward(data, conf, weight, eps=1e-20):
+def nconv2d_forward(data, conf, weight, eps=1e-20, bias=None):
     """One normalized convolution through the C ABI (nconv_modules.py:164-199); weight = the positive kernel."""
-    with _Seam(data, conf, weight) as eng:
-        N, Cin, H, W = data.shape
-        Cout, _, kh, kw = weight.shape
-        if conf.shape != data.shape or weight.shape[1] != Cin:
-            raise ValueError("NConv2d: data/conf/weight shapes do not match")
-        y = torch.empty(N, Cout, H, W, dtype=torch.float32, device=data.device)
-        c = torch.empty_like(y)
-        native.check(eng.L.rnc_nconv2d_fwd(_ptr(data.detach().float().contiguous()), _ptr(conf.detach().float().contiguous()),
-                                           _ptr(weight.detach().float().contiguous()), N, Cin, Cout, H, W, kh, kw, eps,
-                                           _ptr(y), _ptr(c), _stream()), "nconv2d")
-        return y, c
+    with _Seam(data, conf, weight):
+        b = None if bias is None else bias.detach().float().contiguous()
+        return nconv_fwd(data.detach().float().contiguous(), conf.detach().float().contiguous(),
+                         weight.detach().float().contiguous(), b, eps)
 
 
 class NConvUNet(nn.Module):
-    """core/nconv_modules.py:25-136 at the configuration every reference script ships.  forward((data, conf)) ->
-    (xout, cout): at num_downsampling = 1 the decoder consumes x[1] twice (index quirk at :128-131), so the pooled branch
-    never reaches the output and only nconv_in -> nconv_x2[0] -> decoder[0](cat(x1, x1)) -> nconv_out is computed."""
+    """core/nconv_modules.py:25-136 for in_ch 1, groups 1, SoftPlus, channels_multiplier <= 4 and odd filters <= 7, with
+    the reference's module structure, state_dict keys (incl. the ``encoder.*`` aliases of shared layers) and RNG draws.
+    forward((data, conf)) -> (xout, cout) runs the live path of rnc/nconv_unet.py: the decoder reads x[i+N] (index quirk
+    at :128-131), so the deepest level never reaches the output and is not computed."""
 
-    def __init__(self, in_ch=1, channels_multiplier=2, num_downsampling=1, encoder_filter_sz=5, decoder_filter_sz=3,
+    def __init__(self, in_ch=1, channels_multiplier=2, num_downsampling=3, encoder_filter_sz=5, decoder_filter_sz=3,
                  out_filter_sz=1, pos_fn="SoftPlus", groups=1, use_bias=False, data_pooling="conf_based",
-                 shared_encoder=True, use_double_conv=False):
+                 shared_encoder=True, use_double_conv=True):
         super().__init__()
         self.__name__ = "NConvUNet"
-        if (in_ch, channels_multiplier, num_downsampling, encoder_filter_sz, decoder_filter_sz, out_filter_sz,
-                shared_encoder, use_double_conv, use_bias, groups) != (1, 2, 1, 5, 3, 1, True, False, False, 1):
-            raise NotImplementedError("NCUP kernel is built for the configuration every reference script ships (SURVEY.md §5)")
+        if in_ch != 1:
+            raise NotImplementedError(f"NConvUNet in_ch={in_ch}: only in_ch 1 is built")
+        if groups != 1:
+            raise NotImplementedError(f"NConvUNet groups={groups}: only groups 1 is built")
+        if pos_fn.lower() != "softplus":
+            raise NotImplementedError(f"NConvUNet pos_fn={pos_fn!r}: only SoftPlus is built")
+        if not 1 <= channels_multiplier <= 4:
+            raise NotImplementedError(f"NConvUNet channels_multiplier={channels_multiplier}: the kernels take 1 to 4")
+        for name, k in (("encoder_filter_sz", encoder_filter_sz), ("decoder_filter_sz", decoder_filter_sz),
+                        ("out_filter_sz", out_filter_sz)):
+            if not isinstance(k, int) or k < 1 or k > 7 or k % 2 == 0:
+                raise NotImplementedError(f"NConvUNet {name}={k}: the kernels take odd square filters up to 7")
+        if num_downsampling < 0:
+            raise ValueError(f"NConvUNet num_downsampling={num_downsampling}")
+        if data_pooling not in ("conf_based", "max_pooling"):
+            raise NotImplementedError("Choose `self.data_pooling` from [conf_based, max_pooling]!")
         c = in_ch * channels_multiplier
-        self.num_downsampling, self.data_pooling = num_downsampling, data_pooling
-        self.nconv_in = NConv2d(in_ch, c, (5, 5), pos_fn)
-        self.nconv_x2 = nn.Sequential(NConv2d(c, c, (5, 5), pos_fn))
-        self.encoder = nn.ModuleList([nn.Sequential(self.nconv_in, self.nconv_x2), self.nconv_x2[0]])
-        self.decoder = nn.ModuleList([NConv2d(2 * c, c, (3, 3), pos_fn)])
-        self.nconv_out = NConv2d(c, in_ch, (1, 1), pos_fn)
+        self.channels, self.num_downsampling, self.data_pooling = c, num_downsampling, data_pooling
+        self.shared_encoder, self.use_double_conv, self.use_bias = shared_encoder, use_double_conv, use_bias
+        self.use_double_conf = use_double_conv                  # the reference's attribute name
+        self.filter_sizes = (encoder_filter_sz, decoder_filter_sz, out_filter_sz)
+        ek, dk, ok = ((k, k) for k in self.filter_sizes)
+        self.nconv_in = NConv2d(in_ch, c, ek, pos_fn, bias=use_bias)
+        self.nconv_x2 = nn.Sequential(*[NConv2d(c, c, ek, pos_fn, bias=use_bias) for _ in range(2 if use_double_conv else 1)])
+        self.encoder = nn.ModuleList([nn.Sequential(self.nconv_in, self.nconv_x2)])
+        for _ in range(num_downsampling):
+            self.encoder.append(self.nconv_x2[0] if shared_encoder else NConv2d(c, c, ek, pos_fn, bias=use_bias))
+        self.decoder = nn.ModuleList([NConv2d(2 * c, c, dk, pos_fn, bias=use_bias) for _ in range(num_downsampling)])
+        self.nconv_out = NConv2d(c, in_ch, ok, pos_fn, bias=False)
 
     def forward(self, inpt):
-        x, c = self.nconv_in((inpt[0], inpt[1]))
-        x, c = self.nconv_x2[0]((x, c))
-        x, c = self.decoder[0]((torch.cat((x, x), 1), torch.cat((c, c), 1)))
-        return self.nconv_out((x, c))
+        if is_fused(self):
+            x, c = self.nconv_in((inpt[0], inpt[1]))
+            x, c = self.nconv_x2[0]((x, c))
+            x, c = self.decoder[0]((torch.cat((x, x), 1), torch.cat((c, c), 1)))
+            return self.nconv_out((x, c))
+        if _grad_needed(self, inpt[0], inpt[1]):
+            from .train import nconv_unet_train
+            return nconv_unet_train(self, inpt[0], inpt[1])
+        with _Seam(inpt[0], inpt[1]):
+            return PackedUNet(self).run(inpt[0].detach().float().contiguous(), inpt[1].detach().float().contiguous())
 
 
 class Simple(nn.Module):
@@ -452,9 +481,12 @@ class NConvUpsampler(nn.Module):
             raise ValueError("You can set either scale or size at a time!")
         if interpolation_net is None:
             raise ValueError("An interpolation network mush be provided!")
-        if scale != 4 or not use_data_for_guidance or not channels_to_batch or use_residuals or est_on_high_res \
-                or weights_est_net is None:
-            raise NotImplementedError("NCUP kernel is built for scale 4 / data-for-guidance / channels-to-batch (SURVEY.md §5)")
+        for name, bad in (("scale", scale != 4), ("use_data_for_guidance", not use_data_for_guidance),
+                          ("channels_to_batch", not channels_to_batch), ("use_residuals", use_residuals),
+                          ("est_on_high_res", est_on_high_res), ("weights_est_net", weights_est_net is None)):
+            if bad:
+                raise NotImplementedError(f"NConvUpsampler {name}: the NCUP kernels are built for scale 4, data for guidance, "
+                                          "channels to batch, no residuals, estimation at low resolution and a weights net")
         self.scaleH = self.scaleW = float(scale)
         self.interpolation_net, self.weights_est_net = interpolation_net, weights_est_net
         self.use_data_for_guidance, self.channels_to_batch = use_data_for_guidance, channels_to_batch
@@ -495,7 +527,8 @@ def get_upsampler(in_ch, guidance_ch, args):
     num_channels.insert(0, guidance_ch + in_ch if args.final_upsampling_use_data_for_guidance else guidance_ch)
     use_bn = args.dataset == "sintel"                        # upsampler.py:42
     if args.weights_est_net.lower() != "simple":
-        raise NotImplementedError("only the `Simple` weights-estimation net is built (every reference script selects it)")
+        raise NotImplementedError(f"weights_est_net={args.weights_est_net!r}: only the `Simple` weights-estimation net is "
+                                  "built (every reference script selects it)")
     weights_est_net = Simple(num_ch=num_channels, out_ch=in_ch, use_bn=use_bn, filter_sz=args.weights_est_net_filter_sz,
                              dilation=args.weights_est_net_dilation, final_act=torch.sigmoid)
     return NConvUpsampler(scale=args.final_upsampling_scale, interpolation_net=interpolation_net,

@@ -9,8 +9,11 @@
     CorrLookup      CorrBlock.__call__ (corr.py:23-44): rnc_corr_lookup_fwd / rnc_corr_lookup_bwd (d fmap1, d fmap2 pyramid; coords
                     are detached, raft_nc_dbl.py:149)
     NConv2dFn       NConv2d.forward (nconv_modules.py:164-199): rnc_nconv2d_fwd / rnc_nconv2d_bwd (quotient rule, confidence path)
-    NcupChainFn     the whole NConvUNet chain after the weights net: rnc_ncup_train_fwd / rnc_ncup_bwd (fused, deterministic);
-                    used by the frozen-trunk forward (rnc.model.frozen_trunk), which runs the trunk on the inference engine
+    NConvPoolFn     NConvUNet.downsample_data_conf (nconv_modules.py:94-104): rnc_nconv_pool2_fwd / rnc_nconv_pool2_bwd
+    NcupChainFn     the whole NConvUNet chain after the weights net at the shipped configuration: rnc_ncup_train_fwd /
+                    rnc_ncup_bwd (fused, deterministic); used by the frozen-trunk forward (rnc.model.frozen_trunk), which runs the
+                    trunk on the inference engine.  Other configurations run the NConv2dFn / NConvPoolFn chain of
+                    rnc/nconv_unet.py there too.
 
 Activations stay channel-last ([B, H, W, C] fp32) between convolutions.  Pointwise glue (ReLU / sigmoid / tanh / gate blend,
 cat, nearest x2, zero-stuffing, the loss) and the normalisation layers (InstanceNorm / BatchNorm: library kernels, like cuDNN
@@ -26,6 +29,7 @@ import torch.nn.functional as F
 
 from . import native
 from .engine import CORR_CH, ConvDesc, _ptr, _require_cuda, _stream, engine_for, pack_conv
+from .nconv_unet import is_fused, live_chain, nconv_fwd, pool_fwd, unused_parameters
 
 _PACK_CACHE = {}          # (id(weight), version, kind, cin_pad) -> (weight, packed); flushed at the start of every training forward
 
@@ -315,44 +319,79 @@ def corr_lookup_autograd(corr_block, coords):
 
 
 class NConv2dFn(torch.autograd.Function):
-    """(data, conf, W > 0) -> (nconv, conf_out), nconv_modules.py:164-199."""
+    """(data, conf, W > 0[, bias, up_data, up_conf]) -> (nconv, conf_out), nconv_modules.py:164-199.  up_data / up_conf: the
+    decoder's coarse half, read through the nearest-index map as input channels [0, Cup) (nconv_modules.py:129-131)."""
 
     @staticmethod
-    def forward(ctx, data, conf, weight, eps):
-        eng = engine_for(data.device)
+    def forward(ctx, data, conf, weight, eps, bias=None, up_data=None, up_conf=None):
+        dev = _require_cuda(data, conf, weight, bias, up_data, up_conf)
         data, conf, weight = data.contiguous(), conf.contiguous(), weight.contiguous()
-        N, Cin, H, W = data.shape
-        Cout, _, kh, kw = weight.shape
-        y = torch.empty(N, Cout, H, W, dtype=torch.float32, device=data.device)
-        c = torch.empty_like(y)
-        native.check(eng.L.rnc_nconv2d_fwd(_ptr(data), _ptr(conf), _ptr(weight), N, Cin, Cout, H, W, kh, kw, eps, _ptr(y), _ptr(c),
-                                           _stream()), "nconv2d")
-        ctx.save_for_backward(data, conf, weight, y, c)
+        bias = None if bias is None else bias.contiguous()
+        up = None if up_data is None else (up_data.contiguous(), up_conf.contiguous())
+        with torch.cuda.device(dev):
+            y, c = nconv_fwd(data, conf, weight, bias, eps, up)
+        ctx.save_for_backward(data, conf, weight, bias, y, c, *(up or (None, None)))
         ctx.eps = eps
         return y, c
 
     @staticmethod
     def backward(ctx, gy, gc):
-        data, conf, weight, y, c = ctx.saved_tensors
+        data, conf, weight, bias, y, c, ux, uc = ctx.saved_tensors
         eng = engine_for(data.device)
         N, Cin, H, W = data.shape
         Cout, _, kh, kw = weight.shape
+        Cup, Hup, Wup = (ux.shape[1], ux.shape[2], ux.shape[3]) if ux is not None else (0, 0, 0)
+        need = ctx.needs_input_grad
         with torch.cuda.device(data.device):
-            nbytes = eng.L.rnc_nconv2d_bwd_workspace_bytes(N, Cout, H, W)
-            ws = torch.zeros((nbytes + 7) // 8, dtype=torch.float64, device=data.device)
-            g_data = torch.empty_like(data) if ctx.needs_input_grad[0] else None
-            g_conf = torch.empty_like(conf) if ctx.needs_input_grad[1] else None
-            g_w = torch.empty_like(weight) if ctx.needs_input_grad[2] else None
-            native.check(eng.L.rnc_nconv2d_bwd(_ptr(data), _ptr(conf), _ptr(weight), _ptr(y), _ptr(c),
+            nbytes = eng.L.rnc_nconv2d_bwd_workspace_bytes(N, Cin, Cup, Cout, H, W, kh)
+            ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=data.device)
+            g_data = torch.empty_like(data) if need[0] else None
+            g_conf = torch.empty_like(conf) if need[1] else None
+            g_w = torch.empty_like(weight) if need[2] or (bias is not None and need[4]) else None
+            g_b = torch.empty_like(bias) if bias is not None and need[4] else None
+            g_ux = torch.empty_like(ux) if ux is not None and need[5] else None
+            g_uc = torch.empty_like(uc) if uc is not None and need[6] else None
+            native.check(eng.L.rnc_nconv2d_bwd(_ptr(data), _ptr(conf), _ptr(weight), _ptr(bias), _ptr(y), _ptr(c),
                                                _ptr(gy.contiguous()) if gy is not None else None,
                                                _ptr(gc.contiguous()) if gc is not None else None, N, Cin, Cout, H, W, kh, kw, ctx.eps,
-                                               _ptr(g_data), _ptr(g_conf), _ptr(g_w), _ptr(ws), ws.numel() * 8, _stream()), "nconv2d_bwd")
-        return g_data, g_conf, g_w, None
+                                               _ptr(ux), _ptr(uc), Cup, Hup, Wup, _ptr(g_data), _ptr(g_conf), _ptr(g_ux), _ptr(g_uc),
+                                               _ptr(g_w), _ptr(g_b), _ptr(ws), ws.numel() * 8, _stream()), "nconv2d_bwd")
+        return g_data, g_conf, g_w if need[2] else None, None, g_b, g_ux, g_uc
 
 
-def nconv2d_autograd(data, conf, weight, eps=1e-20):
+def nconv2d_autograd(data, conf, weight, eps=1e-20, bias=None):
     _require_cuda(data, conf, weight)
-    return NConv2dFn.apply(data.float(), conf.float(), weight.float(), eps)
+    return NConv2dFn.apply(data.float(), conf.float(), weight.float(), eps, None if bias is None else bias.float())
+
+
+class NConvPoolFn(torch.autograd.Function):
+    """NConvUNet.downsample_data_conf (nconv_modules.py:94-104), ds_factor 2: rnc_nconv_pool2_fwd / rnc_nconv_pool2_bwd."""
+
+    @staticmethod
+    def forward(ctx, data, conf, max_pool_data):
+        dev = _require_cuda(data, conf)
+        data, conf = data.contiguous(), conf.contiguous()
+        with torch.cuda.device(dev):
+            xo, co, idx = pool_fwd(data, conf, max_pool_data)
+        ctx.save_for_backward(idx)
+        ctx.shape = tuple(data.shape)
+        ctx.mark_non_differentiable(idx)
+        return xo, co
+
+    @staticmethod
+    def backward(ctx, gx, gc):
+        (idx,) = ctx.saved_tensors
+        N, C, H, W = ctx.shape
+        need = ctx.needs_input_grad
+        g_data = torch.empty(ctx.shape, dtype=torch.float32, device=idx.device) if need[0] else None
+        g_conf = torch.empty(ctx.shape, dtype=torch.float32, device=idx.device) if need[1] else None
+        if g_data is None and g_conf is None:
+            return None, None, None
+        with torch.cuda.device(idx.device):
+            native.check(native.lib().rnc_nconv_pool2_bwd(_ptr(idx), _ptr(gx.contiguous()) if gx is not None else None,
+                                                          _ptr(gc.contiguous()) if gc is not None else None, N, C, H, W,
+                                                          _ptr(g_data), _ptr(g_conf), _stream()), "nconv_pool2_bwd")
+        return g_data, g_conf, None
 
 
 # --------------------------------------------------------------------------------------------- module graphs (channel-last)
@@ -443,7 +482,18 @@ def simple_cl(wn, x_cl):
 
 
 def nconv_unet_train(net, data, conf):
-    """NConvUNet.forward live path (nconv_modules.py:106-136, SURVEY.md Appendix A.3) with autograd."""
+    """NConvUNet.forward live path (nconv_modules.py:106-136, SURVEY.md Appendix A.3, rnc/nconv_unet.py) with autograd.
+    Parameters that never reach the output (unshared encoder[N]) keep grad None, as in the reference."""
+    if not is_fused(net):
+        _require_cuda(data, conf, *net.parameters())
+
+        def layer(m, x, c, up=None, last=False):
+            return NConv2dFn.apply(x, c, m.weight, m.eps, m.bias, *(up or (None, None)))
+
+        def pool(x, c):
+            return NConvPoolFn.apply(x, c, net.data_pooling == "max_pooling")
+
+        return live_chain(net, data.float(), conf.float(), layer, pool)
     x, c = NConv2dFn.apply(data, conf, net.nconv_in.weight, net.nconv_in.eps)
     x, c = NConv2dFn.apply(x, c, net.nconv_x2[0].weight, net.nconv_x2[0].eps)
     x, c = NConv2dFn.apply(torch.cat((x, x), 1), torch.cat((c, c), 1), net.decoder[0].weight, net.decoder[0].eps)
@@ -519,7 +569,13 @@ def ncup_upsampler_frozen(up, x4, gin, out_scale=8.0):
     detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn."""
     with torch.cuda.device(x4.device):
         conf = simple_cl(up.weights_est_net, gin)
-        return ncup_chain_autograd(up.interpolation_net, x4, conf, out_scale)
+        net = up.interpolation_net
+        if is_fused(net):
+            return ncup_chain_autograd(net, x4, conf, out_scale)
+        xh, wh = zero_stuff(x4), zero_stuff(conf)
+        b, c, oh, ow = xh.shape
+        out, _ = nconv_unet_train(net, xh.view(b * c, 1, oh, ow), wh.view(b * c, 1, oh, ow))
+        return out.view(b, c, oh, ow) * out_scale
 
 
 def zero_stuff(x, scale=4):
@@ -663,10 +719,20 @@ def train_step(model, optimizer, scheduler, image1, image2, flow_gt, valid, iter
     return loss.detach(), (metrics if return_metrics else None)
 
 
+def has_unused_parameters(model):
+    """Does some parameter of `model` never reach the loss?  Only an NConvUNet with unshared encoders has such parameters
+    (encoder[N], behind the decoder's index quirk, nconv_modules.py:128-131); every other parameter receives a gradient
+    (SURVEY.md Appendix G)."""
+    m = getattr(model, "module", model)
+    up = getattr(m, "upsampler", None)
+    return up is not None and bool(unused_parameters(up.interpolation_net))
+
+
 def ddp_model(model, device, bucket_cap_mb=8):
     """train.py:169-175 wraps the model in single-process nn.DataParallel; here: one process per GPU, replicas kept in sync by
-    DistributedDataParallel's bucketed NCCL all-reduce of the gradients (19.6 MB fp32; every parameter receives a gradient,
-    SURVEY.md Appendix G, so no unused-parameter search).  The NConv encoder aliases are one Parameter object: DDP sees it once."""
+    DistributedDataParallel's bucketed NCCL all-reduce of the gradients (19.6 MB fp32).  DDP searches for unused parameters
+    only when the configuration has some (has_unused_parameters).  The NConv encoder aliases are one Parameter object: DDP
+    sees it once."""
     from torch.nn.parallel import DistributedDataParallel as DDP
     return DDP(model.to(device), device_ids=[device.index], bucket_cap_mb=bucket_cap_mb, broadcast_buffers=False,
-               gradient_as_bucket_view=True)
+               gradient_as_bucket_view=True, find_unused_parameters=has_unused_parameters(model))
