@@ -13,18 +13,10 @@ import ctypes as C
 import torch
 
 from . import native
-from .engine import _ptr, _stream
+from .engine import _ptr, _stream, fold_bn
 from .engine_umma import HX_LD, SplitBuf, UmmaWeights
 
 EPS = 1e-5
-
-
-def _fold_bn(conv, bn):
-    w, b = conv.weight.detach().float(), conv.bias.detach().float()
-    if bn is None:
-        return w, b
-    s = bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)
-    return w * s.view(-1, 1, 1, 1), (b - bn.running_mean) * s + bn.bias.detach()
 
 
 class PackedEncoder:
@@ -37,7 +29,7 @@ class PackedEncoder:
         bn = self.kind == "batch"
         if bn and any(m.training for m in enc.modules() if isinstance(m, torch.nn.BatchNorm2d)):
             raise NotImplementedError("cnet BatchNorm in training mode (batch statistics) is not built; call .eval() / freeze_bn()")
-        w, b = _fold_bn(enc.conv1, enc.norm1 if bn else None)
+        w, b = fold_bn(enc.conv1, enc.norm1 if bn else None)
         # window form of the 7x7x3 filter: input "channel" e = 4 * px + c of the 16-pixel window, one tap per filter row
         wv = torch.zeros(w.shape[0], 16, 4, 7, dtype=torch.float32, device=w.device)
         wv[:, :7, :3, :] = w.permute(0, 3, 1, 2)              # [o][kx][c][ky]
@@ -47,11 +39,11 @@ class PackedEncoder:
             for blk in layer:
                 cin, cout = blk.conv1.in_channels, blk.conv1.out_channels
                 stride = blk.conv1.stride[0]
-                w1 = UmmaWeights(*_fold_bn(blk.conv1, blk.norm1 if bn else None), [cin])
-                w2 = UmmaWeights(*_fold_bn(blk.conv2, blk.norm2 if bn else None), [cout])
+                w1 = UmmaWeights(*fold_bn(blk.conv1, blk.norm1 if bn else None), [cin])
+                w2 = UmmaWeights(*fold_bn(blk.conv2, blk.norm2 if bn else None), [cout])
                 wd = None
                 if blk.downsample is not None:
-                    wd = UmmaWeights(*_fold_bn(blk.downsample[0], blk.norm3 if bn else None), [cin])
+                    wd = UmmaWeights(*fold_bn(blk.downsample[0], blk.norm3 if bn else None), [cin])
                 self.blocks.append((cin, cout, stride, w1, w2, wd))
         self.head = UmmaWeights(enc.conv2.weight, enc.conv2.bias, [128])
 
@@ -179,7 +171,7 @@ class EncoderRunner:
         both = torch.cat([image1, image2], 0).contiguous()
         h8, w8, _ = self._trunk(pf, bufs, both, 2 * B, Hin, Win)
         P = h8 * w8
-        eng.alloc_fmaps(ws, B, 256, h8, w8, 4)
+        eng.alloc_fmaps(ws, B, 256, h8, w8, 4, dev)
         xs = bufs.XS[2]
         eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f1_cl.data_ptr(), ldo_f32=256)
         off = B * P * 128 * 2                                  # second half of the batch inside the split planes (bytes)

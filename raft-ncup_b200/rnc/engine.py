@@ -87,6 +87,16 @@ def pack_thin(weight):
     return weight.detach().float().permute(2, 3, 1, 0).reshape(kh * kw, cin, cout).contiguous()
 
 
+def fold_bn(conv, bn=None):
+    """fp32 (weight, bias) of nn.Conv2d `conv` followed by an eval-mode BatchNorm2d `bn` (running statistics), or of `conv`
+    alone when bn is None: s = gamma / sqrt(var + eps), weight * s, (bias - mean) * s + beta."""
+    w, b = conv.weight.detach().float(), conv.bias.detach().float()
+    if bn is None:
+        return w, b
+    s = bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)
+    return w * s.view(-1, 1, 1, 1), (b - bn.running_mean) * s + bn.bias.detach()
+
+
 class PackedMotionEncoder:
     """Kernel-ready weights of BasicMotionEncoder (update.py:79-87) for the exact fp32 CUDA-core kernels."""
 
@@ -128,27 +138,29 @@ class PackedUpdateBlock:
             self.m2 = pack_conv(ub.mask[2].weight, ub.mask[2].bias, scale=0.25)   # `.25 * self.mask(net)`, update.py:140
 
 
-class PackedUpsampler:
+class PackedSimple:
+    """Kernel-ready weights of the weights net Simple (interp_weights_est.py:10-47): its two 3x3 layers with eval-mode
+    BatchNorm folded in, for the exact fp32 kernels (g0, g1), and the 1x1 confidence head (gout)."""
+
+    def __init__(self, wn):
+        # Conv, BatchNorm, ReLU or Conv, ReLU (interp_weights_est.py:26-30)
+        convs = [fold_bn(blk[0], blk[1] if len(blk) == 3 else None) for blk in wn.conv]
+        self.c_mid0, self.c_mid1 = convs[0][0].shape[0], convs[1][0].shape[0]
+        self.gout = (pack_thin(wn.out.weight), wn.out.bias.detach().float().contiguous())
+        self.pack_convs(convs)
+
+    def pack_convs(self, convs):
+        """The two folded 3x3 layers in the exact kernels' format; the tensor-core upsampler pack overrides this."""
+        self.cin0_pad = (convs[0][0].shape[1] + 3) // 4 * 4
+        self.g0 = pack_conv(convs[0][0], convs[0][1], cin_pad=self.cin0_pad)
+        self.g1 = pack_conv(convs[1][0], convs[1][1])
+
+
+class PackedUpsampler(PackedSimple):
     """Kernel-ready weights of NConvUpsampler (upsampler.py:75-141): BN-folded weights net + softplus'd NConv weights."""
 
     def __init__(self, up):
-        wn = up.weights_est_net
-        convs = []
-        for blk in wn.conv:
-            conv = blk[0]
-            w, b = conv.weight.detach().float(), conv.bias.detach().float()
-            if len(blk) == 3:   # Conv, BatchNorm, ReLU — eval-mode fold (interp_weights_est.py:26-30)
-                bn = blk[1]
-                s = bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)
-                w = w * s.view(-1, 1, 1, 1)
-                b = (b - bn.running_mean) * s + bn.bias.detach()
-            convs.append((w, b))
-        cin0 = convs[0][0].shape[1]
-        self.cin0_pad = (cin0 + 3) // 4 * 4
-        self.g0 = pack_conv(convs[0][0], convs[0][1], cin_pad=self.cin0_pad)
-        self.g1 = pack_conv(convs[1][0], convs[1][1])
-        self.c_mid0, self.c_mid1 = convs[0][0].shape[0], convs[1][0].shape[0]
-        self.gout = (pack_thin(wn.out.weight), wn.out.bias.detach().float().contiguous())
+        super().__init__(up.weights_est_net)
         net = up.interpolation_net
         self.nconv_host = self.unet = None
         if is_fused(net):
@@ -190,6 +202,19 @@ _EPOCH = [0]
 def invalidate_packed():
     """Force every engine to re-pack weights on the next forward (needed only after in-place edits through ``.data``)."""
     _EPOCH[0] += 1
+
+
+def _lru_get(cache, key, capacity, build):
+    """cache[key] of an OrderedDict used as an LRU cache, marked most recently used; on a miss the least recently used entries
+    are dropped to make room for build(), which is stored under key."""
+    hit = cache.get(key)
+    if hit is None:
+        while len(cache) >= capacity:
+            cache.popitem(last=False)
+        hit = cache[key] = build()
+    else:
+        cache.move_to_end(key)
+    return hit
 
 
 class Workspace:
@@ -302,15 +327,7 @@ class Engine:
 
     # ------------------------------------------------------------------ caches
     def _packed_for(self, kind, module, build):
-        key = (kind,) + _param_key(module)
-        hit = self._packed.get(key)
-        if hit is None:
-            hit = self._packed[key] = build(module)
-            while len(self._packed) > self.MAX_PACKED:
-                self._packed.popitem(last=False)
-        else:
-            self._packed.move_to_end(key)
-        return hit
+        return _lru_get(self._packed, (kind,) + _param_key(module), self.MAX_PACKED, lambda: build(module))
 
     def packed_update(self, ub):
         return self._packed_for("ub", ub, self.PACK_UB)
@@ -318,18 +335,15 @@ class Engine:
     def packed_upsampler(self, up):
         return self._packed_for("up", up, self.PACK_UP)
 
-    def workspace(self, device, B, H8, W8, with_mask, with_ncup):
-        """Resident buffers for one problem shape.  The least recently used one is dropped when a fifth shape shows up; the
-        caller holds ``self.lock`` for the whole forward, so a workspace in use is never the one evicted."""
-        key = (self.mode, str(device), B, H8, W8, with_mask, with_ncup)
-        ws = self._ws.get(key)
-        if ws is None:
-            while len(self._ws) >= self.MAX_WS:
-                self._ws.popitem(last=False)
-            ws = self._ws[key] = self.WS(device, B, H8, W8, with_mask, with_ncup)
-        else:
-            self._ws.move_to_end(key)
-        return ws
+    def workspace(self, device, B, H8, W8, with_mask=False, with_ncup=False, mode=None):
+        """Resident buffers for one problem shape, in the format of this engine's kernels, or with mode="ffma" of the exact
+        fp32 CUDA-core kernels whatever this engine's mode is (the operator seams).  The least recently used workspace is
+        dropped when a seventh one is needed; the caller holds ``self.lock`` for the whole forward, so a workspace in use is
+        never the one evicted."""
+        mode = mode or self.mode
+        ws_cls = Workspace if mode == "ffma" else self.WS
+        return _lru_get(self._ws, (mode, str(device), B, H8, W8, with_mask, with_ncup), self.MAX_WS,
+                        lambda: ws_cls(device, B, H8, W8, with_mask, with_ncup))
 
     # ------------------------------------------------------------------ whole-forward CUDA graphs (test-mode inference)
     def graphs_enabled(self, model):
@@ -350,13 +364,10 @@ class Engine:
         if flow_init is not None and tuple(flow_init.shape) != (B, 2, Him // 8, Wim // 8):
             raise ValueError("flow_init must be [N,2,H/8,W/8]")
         key = (type(model).__name__, tuple(image1.shape), iters, flow_init is not None, _param_key(model))
-        ent = self._graphs.get(key)
-        if ent is None:
-            while len(self._graphs) >= self.MAX_GRAPHS:
-                self._graphs.popitem(last=False)
-            self._graphs[key] = {"seen": 1}
+        first = key not in self._graphs
+        ent = _lru_get(self._graphs, key, self.MAX_GRAPHS, dict)
+        if first:
             return model._forward_eager(self, image1, image2, iters, flow_init, True)     # first sight: eager (also warms caches)
-        self._graphs.move_to_end(key)
         if "graph" not in ent:
             ent["im1"], ent["im2"] = image1.detach().float().clone(), image2.detach().float().clone()
             ent["fi"] = flow_init.detach().float().clone() if flow_init is not None else None
@@ -397,15 +408,20 @@ class Engine:
         d.cout, d.kh, d.kw, d.epilogue = cout, kh, kw, epi
         native.check(self.L.rnc_conv2d_cl_fwd(C.byref(d), _stream()), "conv2d_cl")
 
-    def fmap_prepare(self, ws, fmap1, fmap2, levels=4):
-        B, D, H, W = fmap1.shape
+    def alloc_fmaps(self, ws, B, D, H, W, levels, device):
+        """Allocate the CL feature map / pyramid buffers of ws, which fmap_prepare fills and the tensor-core encoder heads
+        write into directly."""
         total = self.L.rnc_pyramid_offset(B, D, H, W, levels)
         if ws.f1_cl is None or ws.f1_cl.numel() != B * H * W * D:
-            ws.f1_cl = torch.empty(B * H * W, D, dtype=torch.float32, device=fmap1.device)
-            ws.f2_pyr = torch.empty(total, dtype=torch.float32, device=fmap1.device)
+            ws.f1_cl = torch.empty(B * H * W, D, dtype=torch.float32, device=device)
+            ws.f2_pyr = torch.empty(total, dtype=torch.float32, device=device)
+        ws.D, ws.levels = D, levels
+
+    def fmap_prepare(self, ws, fmap1, fmap2, levels=4):
+        B, D, H, W = fmap1.shape
+        self.alloc_fmaps(ws, B, D, H, W, levels, fmap1.device)
         native.check(self.L.rnc_fmap_prepare(_ptr(fmap1), _ptr(fmap2), B, D, H, W, levels, _ptr(ws.f1_cl),
                                              _ptr(ws.f2_pyr), _stream()), "fmap_prepare")
-        ws.D, ws.levels = D, levels
 
     def lookup(self, ws, coords, out, layout, ldo, radius=4):
         with _Timed(self, "corr_lookup"):
@@ -476,18 +492,6 @@ class Engine:
         native.check(self.L.rnc_flow_head2_fwd(_ptr(ws.fh), 256, 256, _ptr(pk.fh2[0]), _ptr(pk.fh2[1]), B, H, W,
                                                _ptr(ws.delta) if want_delta else C.c_void_p(0), _ptr(ws.coords1), _stream()),
                      "flow_head2")
-
-    def ffma_workspace(self, device, B, H8, W8, with_mask=False, with_ncup=False):
-        """Workspace of the exact fp32 CUDA-core kernels (operator seams), whatever this engine's own mode is."""
-        key = ("ffma", str(device), B, H8, W8, with_mask, with_ncup)
-        ws = self._ws.get(key)
-        if ws is None:
-            while len(self._ws) >= self.MAX_WS:
-                self._ws.popitem(last=False)
-            ws = self._ws[key] = Workspace(device, B, H8, W8, with_mask, with_ncup)
-        else:
-            self._ws.move_to_end(key)
-        return ws
 
     def load_state(self, ws, net, inp):
         """NCHW net/inp (raft_nc_dbl.py:137-140) -> resident hx buffer."""

@@ -114,18 +114,9 @@ class PackedUpdateUmma:
 
 
 class PackedUpsamplerUmma(PackedUpsampler):
-    def __init__(self, up):
-        super().__init__(up)
-        # re-pack the BN-folded 3x3 layers of the weights net for the tensor-core path
-        wn = up.weights_est_net
-        convs = []
-        for blk in wn.conv:
-            w, b = blk[0].weight.detach().float(), blk[0].bias.detach().float()
-            if len(blk) == 3:
-                bn = blk[1]
-                s = bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)
-                w, b = w * s.view(-1, 1, 1, 1), (b - bn.running_mean) * s + bn.bias.detach()
-            convs.append((w, b))
+    """PackedUpsampler with the weights net's BN-folded 3x3 layers packed for the tensor-core path (u0, u1)."""
+
+    def pack_convs(self, convs):
         self.u0 = UmmaWeights(convs[0][0], convs[0][1], [132])
         self.u1 = UmmaWeights(convs[1][0], convs[1][1], [64])
 
@@ -239,15 +230,6 @@ class UmmaEngine(Engine):
             from .encoder_umma import EncoderRunner
             self._encoder = EncoderRunner(self)
         return self._encoder
-
-    def alloc_fmaps(self, ws, B, D, H, W, levels):
-        """Allocate the CL feature map / pyramid buffers that the encoder heads write into directly."""
-        total = self.L.rnc_pyramid_offset(B, D, H, W, levels)
-        if ws.f1_cl is None or ws.f1_cl.numel() != B * H * W * D:
-            dev = ws.coords1.device
-            ws.f1_cl = torch.empty(B * H * W, D, dtype=torch.float32, device=dev)
-            ws.f2_pyr = torch.empty(total, dtype=torch.float32, device=dev)
-        ws.D, ws.levels = D, levels
 
     def finish_fmaps(self, ws):
         """Pool fmap2 into the pyramid (corr.py:18-21 on features) and refresh the halves copies."""

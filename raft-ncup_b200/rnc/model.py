@@ -72,18 +72,15 @@ class _RAFTBase(nn.Module):
             raise ValueError("iters must be >= 1")
         if hasattr(self, "data_idx"):
             self.data_idx += 1
+        if image1.shape[2] % 8 or image1.shape[3] % 8:
+            raise ValueError("image height/width must be multiples of 8 (pad with utils.utils.InputPadder, evaluate.py:125)")
         if self._needs_grad():
             # training path (train.py:215): the same graph with autograd, exact-fp32 kernels forward and backward
-            if image1.shape[2] % 8 or image1.shape[3] % 8:
-                raise ValueError("image height/width must be multiples of 8 (pad with utils.utils.InputPadder, evaluate.py:125)")
             if frozen_trunk(self, image1, image2, flow_init):
                 # only the upsampler trains: the trunk runs on the inference engine, the upsampler on autograd
                 return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, upsample=self._upsample_frozen)
             from .train import raft_forward_train
             return raft_forward_train(self, image1, image2, iters, flow_init, test_mode)
-        B, _, Him, Wim = image1.shape
-        if Him % 8 or Wim % 8:
-            raise ValueError("image height/width must be multiples of 8 (pad with utils.utils.InputPadder, evaluate.py:125)")
         if test_mode and eng.graphs_enabled(self):
             return eng.graph_forward(self, image1, image2, iters, flow_init)
         return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode)

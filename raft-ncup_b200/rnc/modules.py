@@ -15,8 +15,8 @@ import torch.nn.functional as F
 
 from . import native
 from .nconv_unet import PackedUNet, is_fused, nconv_fwd
-from .engine import (CORR_CH, HX_LD, PackedFlowHead, PackedGRU, PackedMotionEncoder, _ptr, _require_cuda, _stream, engine_for,
-                     module_tensors, pack_conv, pack_thin)
+from .engine import (CORR_CH, HX_LD, Engine, PackedFlowHead, PackedGRU, PackedMotionEncoder, PackedSimple, _ptr, _require_cuda,
+                     _stream, engine_for, module_tensors)
 
 # --------------------------------------------------------------------------------------------- encoders (C6)
 # RAFT.forward runs the encoders on the tensor-core path (rnc/encoder_umma.py).  The nn.Module forwards below are the
@@ -176,7 +176,7 @@ class FlowHead(nn.Module):
             raise NotImplementedError("kernels are built for the reference's FlowHead(128, 256)")
         with _Seam(x) as eng:
             B, _, H, W = x.shape
-            ws = eng.ffma_workspace(x.device, B, H, W)
+            ws = eng.workspace(x.device, B, H, W, mode="ffma")
             pk = eng._packed_for("flow_head", self, PackedFlowHead)
             native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, 128, H, W, _ptr(ws.hx), HX_LD, 0, _stream()),
                          "nchw_to_cl")
@@ -201,19 +201,13 @@ class SepConvGRU(nn.Module):
             raise NotImplementedError("kernels are built for the reference's SepConvGRU(128, 256)")
         with _Seam(h, x) as eng:
             B, _, H, W = h.shape
-            ws = eng.ffma_workspace(h.device, B, H, W)
+            ws = eng.workspace(h.device, B, H, W, mode="ffma")
             pk = eng._packed_for("gru", self, PackedGRU)
             s = _stream()
             native.check(eng.L.rnc_nchw_to_cl(_ptr(h.detach().float().contiguous()), B, 128, H, W, _ptr(ws.hx), HX_LD, 0, s), "nchw_to_cl")
             native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, 256, H, W, _ptr(ws.hx), HX_LD, 128, s), "nchw_to_cl")
             eng._gru_ffma(ws, pk)
-            return Engine_net_nchw(eng, ws)
-
-
-def Engine_net_nchw(eng, ws):
-    out = torch.empty(ws.B, 128, ws.H8, ws.W8, dtype=torch.float32, device=ws.hx.device)
-    native.check(eng.L.rnc_cl_to_nchw(_ptr(ws.hx), HX_LD, 0, ws.B, 128, ws.H8, ws.W8, _ptr(out), _stream()), "cl_to_nchw")
-    return out
+            return Engine.net_nchw(eng, ws)          # the exact kernels' hidden state, whatever the engine's mode
 
 
 class BasicMotionEncoder(nn.Module):
@@ -236,7 +230,7 @@ class BasicMotionEncoder(nn.Module):
             raise NotImplementedError("kernels are built for 4 levels x radius 4 = 324 correlation channels")
         with _Seam(flow, corr) as eng:
             B, _, H, W = flow.shape
-            ws = eng.ffma_workspace(flow.device, B, H, W)
+            ws = eng.workspace(flow.device, B, H, W, mode="ffma")
             pk = eng._packed_for("motion_encoder", self, PackedMotionEncoder)
             s = _stream()
             native.check(eng.L.rnc_nchw_to_cl(_ptr(corr.detach().float().contiguous()), B, CORR_CH, H, W, _ptr(ws.corr), CORR_CH, 0, s),
@@ -424,48 +418,25 @@ class Simple(nn.Module):
             raise NotImplementedError("the fused confidence head applies the sigmoid the reference wires in (upsampler.py:44-46)")
         if any(isinstance(m, nn.BatchNorm2d) and m.training for m in self.modules()):
             raise NotImplementedError("weights-net BatchNorm with batch statistics needs the training path (enable grad)")
+        B, Cin, h, w = x.shape
+        if Cin != self.in_ch:
+            raise ValueError(f"Simple: expected {self.in_ch} input channels, got {Cin}")
         with _Seam(x) as eng:
-            from .engine import pack_conv as _pc
-            B, Cin, h, w = x.shape
-            cpad = (Cin + 3) // 4 * 4
-            folded = eng._packed_for("simple", self, lambda m: _PackedSimple(m, cpad))
+            pk = eng._packed_for("simple", self, PackedSimple)
+            cpad = pk.cin0_pad
             s = _stream()
             M = B * h * w
             xin = torch.zeros(M, cpad, dtype=torch.float32, device=x.device) if cpad != Cin else torch.empty(M, cpad, dtype=torch.float32, device=x.device)
             native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, Cin, h, w, _ptr(xin), cpad, 0, s), "nchw_to_cl")
-            c0, c1 = folded.c_mid
+            c0, c1 = pk.c_mid0, pk.c_mid1
             g1 = torch.empty(M, (c0 + 3) // 4 * 4, dtype=torch.float32, device=x.device)
             g2 = torch.empty(M, (c1 + 3) // 4 * 4, dtype=torch.float32, device=x.device)
-            eng.conv(B, h, w, xin.data_ptr(), cpad, cpad, folded.g0, c0, 3, 3, native.EPI_RELU, g1.data_ptr(), g1.shape[1])
-            eng.conv(B, h, w, g1.data_ptr(), c0, g1.shape[1], folded.g1, c1, 3, 3, native.EPI_RELU, g2.data_ptr(), g2.shape[1])
+            eng.conv(B, h, w, xin.data_ptr(), cpad, cpad, pk.g0, c0, 3, 3, native.EPI_RELU, g1.data_ptr(), g1.shape[1])
+            eng.conv(B, h, w, g1.data_ptr(), c0, g1.shape[1], pk.g1, c1, 3, 3, native.EPI_RELU, g2.data_ptr(), g2.shape[1])
             conf = torch.empty(B, 2, h, w, dtype=torch.float32, device=x.device)
-            native.check(eng.L.rnc_conf_head_fwd(_ptr(g2), c1, g2.shape[1], _ptr(folded.gout[0]), _ptr(folded.gout[1]), B, h, w,
+            native.check(eng.L.rnc_conf_head_fwd(_ptr(g2), c1, g2.shape[1], _ptr(pk.gout[0]), _ptr(pk.gout[1]), B, h, w,
                                                  _ptr(conf), s), "conf_head")
             return conf
-
-
-def fold_simple_convs(wn):
-    """(weight, bias) of Simple's two 3x3 layers with eval-mode BatchNorm folded in (interp_weights_est.py:26-30)."""
-    convs = []
-    for blk in wn.conv:
-        conv = blk[0]
-        w, b = conv.weight.detach().float(), conv.bias.detach().float()
-        if len(blk) == 3:   # Conv, BatchNorm, ReLU
-            bn = blk[1]
-            sc = bn.weight.detach() / torch.sqrt(bn.running_var + bn.eps)
-            w = w * sc.view(-1, 1, 1, 1)
-            b = (b - bn.running_mean) * sc + bn.bias.detach()
-        convs.append((w, b))
-    return convs
-
-
-class _PackedSimple:
-    def __init__(self, wn, cin_pad):
-        convs = fold_simple_convs(wn)
-        self.g0 = pack_conv(convs[0][0], convs[0][1], cin_pad=cin_pad)
-        self.g1 = pack_conv(convs[1][0], convs[1][1], cin_pad=(convs[1][0].shape[1] + 3) // 4 * 4)
-        self.c_mid = (convs[0][0].shape[0], convs[1][0].shape[0])
-        self.gout = (pack_thin(wn.out.weight), wn.out.bias.detach().float().contiguous())
 
 
 class NConvUpsampler(nn.Module):

@@ -21,31 +21,45 @@ in the reference) are plain torch ops — plumbing around the kernels above.  `s
 `train_step` restate train.py:46-71, :83-99, :203-227; `ddp_model` replaces nn.DataParallel (train.py:169-175) with one
 process per GPU and a bucketed NCCL all-reduce of the 4.9 M fp32 gradients.
 """
-import ctypes as C
+import copy
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from . import native
-from .engine import CORR_CH, ConvDesc, _ptr, _require_cuda, _stream, engine_for, pack_conv
+from .engine import CORR_CH, _ptr, _require_cuda, _stream, engine_for, pack_conv
 from .nconv_unet import is_fused, live_chain, nconv_fwd, pool_fwd, unused_parameters
 
-_PACK_CACHE = {}          # (id(weight), version, kind, cin_pad) -> (weight, packed); flushed at the start of every training forward
+_PACK_CACHE = {}          # (id(weight), version, kind, fmt, cin_pad) -> (weight, packed); flushed at every training forward
 
 
-def _packed(weight, kind, cin_pad):
+def _packed(weight, kind, cin_pad, fmt="ffma"):
     """Kernel-ready copy of a convolution weight ('fwd') or of its flipped transpose ('dgrad'), cached for the 12 iterations of a
-    step.  The entry keeps the weight tensor alive, so neither its id nor its storage can be recycled while the entry exists."""
-    key = (id(weight), weight._version, kind, cin_pad)
+    step, in the operand format of the exact kernel (fmt 'ffma': pack_conv) or of the tensor-core kernel ('f16': UmmaWeights,
+    'tf32': _WeightsTF32).  The entry keeps the weight tensor alive, so neither its id nor its storage can be recycled while the
+    entry exists."""
+    key = (id(weight), weight._version, kind, fmt, cin_pad)
     hit = _PACK_CACHE.get(key)
     if hit is None or hit[0] is not weight:
         if len(_PACK_CACHE) > 512:
             _PACK_CACHE.clear()
-        w = weight.detach()
+        w = weight.detach().float()
         if kind == "dgrad":          # Wd[ci, co, ky, kx] = W[co, ci, kh-1-ky, kw-1-kx]
             w = w.flip(2, 3).transpose(0, 1)
-        hit = _PACK_CACHE[key] = (weight, pack_conv(w.contiguous(), None, cin_pad=cin_pad))
+        w = w.contiguous()
+        if fmt == "ffma":
+            packed = pack_conv(w, None, cin_pad=cin_pad)
+        elif fmt == "tf32":
+            packed = _WeightsTF32(w, cin_pad)
+        else:
+            from .engine_umma import UmmaWeights
+            if w.shape[1] != cin_pad:
+                w = F.pad(w, (0, 0, 0, 0, 0, cin_pad - w.shape[1]))
+            # fixed scale 2^10 (no device sync per pack): exact for |w| < 32; a lo part below the half normal range only costs an
+            # absolute 2^-34 per weight
+            packed = UmmaWeights(w, None, [cin_pad], scale_log2=10)
+        hit = _PACK_CACHE[key] = (weight, packed)
     return hit[1]
 
 
@@ -101,24 +115,12 @@ class _WeightsTF32:
         self.bias = torch.zeros(self.coutpad, dtype=torch.float32, device=w.device)
 
 
-def _packed_umma(weight, kind, cin_pad, fmt="f16"):
-    from .engine_umma import UmmaWeights
-    key = (id(weight), weight._version, kind + "_" + fmt, cin_pad)
-    hit = _PACK_CACHE.get(key)
-    if hit is None or hit[0] is not weight:
-        w = weight.detach().float()
-        if kind == "dgrad":
-            w = w.flip(2, 3).transpose(0, 1)
-        if fmt == "tf32":
-            packed = _WeightsTF32(w.contiguous(), cin_pad)
-        else:
-            if w.shape[1] != cin_pad:
-                w = F.pad(w, (0, 0, 0, 0, 0, cin_pad - w.shape[1]))
-            # fixed scale 2^10 (no device sync per pack): exact for |w| < 32; a lo part below the half normal range only costs an
-            # absolute 2^-34 per weight
-            packed = UmmaWeights(w.contiguous(), None, [cin_pad], scale_log2=10)
-        hit = _PACK_CACHE[key] = (weight, packed)
-    return hit[1]
+def _padded_bias(packed_bias, bias):
+    """This call's bias in the zero-padded layout of a packed weight's bias (packs are cached per weight; biases are tiny and
+    change with it)."""
+    b = torch.zeros_like(packed_bias)
+    b[:bias.shape[0]] = bias.detach()
+    return b
 
 
 def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16"):
@@ -135,20 +137,11 @@ def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16"):
     ldo = _ceil4(cout)
     out = torch.empty(B, Ho, Wo, ldo, dtype=torch.float32, device=x.device)
     if bias is not None:
-        wt = _WithBias(wt, bias)
+        wt = copy.copy(wt)
+        wt.bias = _padded_bias(wt.bias, bias)
     eng.uconv(B, Ho, Wo, (hi.data_ptr(), lo.data_ptr()), Cx, Cx, wt, native.EPI_LINEAR, out_f32=out.data_ptr(), ldo_f32=ldo,
               stride=stride, hin=H, win=W, flags=eng.conv_flags | (native.CONV_TF32 if fmt == "tf32" else 0))
     return out
-
-
-class _WithBias:
-    """A packed weight with this call's bias vector (the pack is cached per weight; biases are tiny and change with it)."""
-
-    def __init__(self, wt, bias):
-        self.__dict__.update(wt.__dict__)
-        b = torch.zeros_like(wt.bias)
-        b[:wt.cout] = bias.detach()
-        self.bias = b
 
 
 def _conv_launch(eng, x, packed, cout, kh, kw, bias=None):
@@ -157,18 +150,9 @@ def _conv_launch(eng, x, packed, cout, kh, kw, bias=None):
     ldo = _ceil4(cout)
     alloc = torch.empty if ldo == cout else torch.zeros          # pad channels must read as zero downstream
     out = alloc(B, H, W, ldo, dtype=torch.float32, device=x.device)
-    w, b = packed
     if bias is not None:
-        b = torch.zeros_like(b)
-        b[:cout] = bias.detach()
-    d = ConvDesc()
-    d.in0, d.c0, d.ld0 = x.data_ptr(), Cx, Cx
-    d.in1, d.c1, d.ld1 = 0, 0, 0
-    d.weight, d.bias = w.data_ptr(), b.data_ptr()
-    d.out, d.ldo = out.data_ptr(), ldo
-    d.B, d.H, d.W = B, H, W
-    d.cout, d.kh, d.kw, d.epilogue = cout, kh, kw, native.EPI_LINEAR
-    native.check(eng.L.rnc_conv2d_cl_fwd(C.byref(d), _stream()), "conv2d_cl")
+        packed = (packed[0], _padded_bias(packed[1], bias))
+    eng.conv(B, H, W, x.data_ptr(), Cx, Cx, packed, cout, kh, kw, native.EPI_LINEAR, out.data_ptr(), ldo)
     return out
 
 
@@ -188,7 +172,7 @@ class ConvCL(torch.autograd.Function):
             raise NotImplementedError("stride 1 or 2")
         fmt = _umma_ok(eng, Cx, cout)
         if fmt:
-            y = _conv_launch_umma(eng, x, _packed_umma(weight, "fwd", Cx, fmt), cout, stride, bias, fmt)
+            y = _conv_launch_umma(eng, x, _packed(weight, "fwd", Cx, fmt), cout, stride, bias, fmt)
         else:
             y = _conv_launch(eng, x, _packed(weight, "fwd", Cx), cout, kh, kw, bias)
             if stride == 2:
@@ -214,7 +198,7 @@ class ConvCL(torch.autograd.Function):
                     g_full[:, ::2, ::2] = gy
                 fmt = _umma_ok(eng, ldg, cin, dgrad=True)
                 if fmt:
-                    gx = _conv_launch_umma(eng, g_full, _packed_umma(weight, "dgrad", ldg, fmt), cin, fmt=fmt)
+                    gx = _conv_launch_umma(eng, g_full, _packed(weight, "dgrad", ldg, fmt), cin, fmt=fmt)
                 else:
                     gx = _conv_launch(eng, g_full, _packed(weight, "dgrad", ldg), cin, kh, kw)
                 if gx.shape[-1] != Cx:               # Cx > ceil4(cin) never happens; equal by construction
@@ -569,13 +553,21 @@ def ncup_upsampler_frozen(up, x4, gin, out_scale=8.0):
     detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn."""
     with torch.cuda.device(x4.device):
         conf = simple_cl(up.weights_est_net, gin)
-        net = up.interpolation_net
-        if is_fused(net):
-            return ncup_chain_autograd(net, x4, conf, out_scale)
-        xh, wh = zero_stuff(x4), zero_stuff(conf)
-        b, c, oh, ow = xh.shape
-        out, _ = nconv_unet_train(net, xh.view(b * c, 1, oh, ow), wh.view(b * c, 1, oh, ow))
-        return out.view(b, c, oh, ow) * out_scale
+        return _ncup_chain_train(up.interpolation_net, x4, conf, out_scale, fused=True)
+
+
+def _ncup_chain_train(net, x_lowres, conf, out_scale, fused):
+    """NConvUpsampler.forward after the weights net (upsampler.py:150-177) with autograd: zero-stuffing, the NConvUNet `net`,
+    out_scale; x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4].  fused: the shipped network runs on NcupChainFn, with
+    out_scale applied inside the kernel; otherwise every network runs the per-layer NConv2dFn chain (the full-training path
+    keeps it: the fused backward rounds the gradients differently)."""
+    if fused and is_fused(net):
+        return ncup_chain_autograd(net, x_lowres, conf, out_scale)
+    xh, ch = zero_stuff(x_lowres), zero_stuff(conf)
+    b, c, oh, ow = xh.shape
+    out, _ = nconv_unet_train(net, xh.view(b * c, 1, oh, ow), ch.view(b * c, 1, oh, ow))
+    out = out.view(b, c, oh, ow)
+    return out * out_scale if out_scale != 1.0 else out
 
 
 def zero_stuff(x, scale=4):
@@ -592,11 +584,7 @@ def ncup_upsampler_train(up, x_lowres, x_guidance, out_scale=1.0):
     with torch.cuda.device(x_lowres.device):
         g4 = F.interpolate(x_guidance, x_lowres.shape[2:], mode="area")           # integer x2 'area' upscale = replication
         w4 = simple_cl(up.weights_est_net, to_cl(torch.cat([x_lowres, g4], 1), pad_to=136))     # pitch % 8 == 0: tensor-core layer
-        xh, wh = zero_stuff(x_lowres), zero_stuff(w4)
-        b, c, oh, ow = xh.shape
-        out, _ = nconv_unet_train(up.interpolation_net, xh.view(b * c, 1, oh, ow), wh.view(b * c, 1, oh, ow))
-        out = out.view(b, c, oh, ow)
-        return out * out_scale if out_scale != 1.0 else out
+        return _ncup_chain_train(up.interpolation_net, x_lowres, w4, out_scale, fused=False)
 
 
 def simple_train(wn, x):

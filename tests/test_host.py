@@ -170,6 +170,7 @@ def test_pack_conv_is_an_implicit_gemm_of_the_reference_conv():
 
 def test_bn_fold_matches_eval_batchnorm():
     from rnc.engine import PackedUpsampler
+    from rnc.engine_umma import PackedUpsamplerUmma
     m = build_model("raft_nc_dbl")
     wn = m.upsampler.weights_est_net
     g = torch.Generator().manual_seed(0)
@@ -183,6 +184,11 @@ def test_bn_fold_matches_eval_batchnorm():
     out = F.relu(F.conv2d(x, w, pu.g0[1][:64], padding=1))
     assert (out - ref).abs().max() < 1e-4
     assert pu.g0[0].shape[1] == 132 and len(pu.nconv_host) == 224
+    # the tensor-core pack of the same layer: fp16 hi/lo planes [CoutPad][9 taps * 3 blocks * 64], value (hi + lo) * unscale
+    u0 = PackedUpsamplerUmma(m.upsampler).u0
+    w = ((u0.w_hi.float() + u0.w_lo.float()) * u0.unscale).view(u0.coutpad, 9, 192)[:64, :, :130]
+    out = F.relu(F.conv2d(x, w.reshape(64, 3, 3, 130).permute(0, 3, 1, 2), u0.bias[:64], padding=1))
+    assert (out - ref).abs().max() < 1e-4
 
 
 def test_input_padder_matches_reference(meta):
