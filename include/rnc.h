@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 12) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 13) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -227,6 +227,12 @@ int rnc_instnorm_stats(const float* x, int N, int P, int C, float eps, double* s
 /* Second half of rnc_instnorm_stats when the sums were accumulated elsewhere (rnc_conv_umma_desc.stats): stats [N][C][2]
  * fp64 sums over P positions -> mean_rstd, then stats is zeroed for the next producer. */
 int rnc_instnorm_finalize(double* stats, int N, int P, int C, float eps, float* mean_rstd, void* stream);
+/* Deterministic rnc_instnorm_stats (torch.use_deterministic_algorithms): each CTA of 512 positions writes its fp64 sums to
+ * workspace (rnc_instnorm_stats_det_workspace_bytes(N, P, C) bytes, 16-byte aligned, no zeroing needed), and a second kernel
+ * adds them in ascending CTA order; identical inputs give bit-identical mean_rstd.  Returns 0 bytes for a bad shape. */
+size_t rnc_instnorm_stats_det_workspace_bytes(int N, int P, int C);
+int rnc_instnorm_stats_det(const float* x, int N, int P, int C, float eps, void* workspace, size_t workspace_bytes,
+                           float* mean_rstd, void* stream);
 /* apply: mode 0: norm(x) -> out_f32;  1: relu(norm(x));  2: relu(res + relu(norm(x)))  (ResidualBlock.forward,
  * extractor.py:48-56); outputs fp32 and/or split halves, all CL [N][P][C]. */
 int rnc_instnorm_apply(const float* x, const float* mean_rstd, const float* res, int N, int P, int C, int mode,
@@ -404,14 +410,30 @@ int rnc_nconv_pool2_bwd(const int* idx, const float* g_data_out, const float* g_
 int rnc_corr_lookup_bwd(const float* f1_cl, const float* f2_pyr, const float* coords, const float* g_out, int ldg,
                         int B, int D, int H, int W, int levels, int radius, float* g_f1, float* g_f2_pyr, void* stream);
 int rnc_pyramid_pool_bwd(float* g_f2_pyr, int B, int D, int H, int W, int levels, void* stream);
+/* Deterministic rnc_corr_lookup_bwd: the same g_f1; d fmap2 without atomics, and g_f2_pyr is WRITTEN (every position of every
+ * level; no zero-fill needed).  Each pixel stages its 100 window gradients per level and its window-origin cell; a stable
+ * radix sort groups the pixels by cell; then every pyramid position sums gv * f1[p] over the 10x10 cells whose window
+ * covers it, cells in a fixed order and pixels in ascending index.  Each product is rounded as the atomic kernel rounds it,
+ * so the result is one of the sums the atomic kernel can produce.  workspace: rnc_corr_lookup_bwd_workspace_bytes(B, H, W,
+ * levels) bytes, 16-byte aligned (0 for a bad shape). */
+size_t rnc_corr_lookup_bwd_workspace_bytes(int B, int H, int W, int levels);
+int rnc_corr_lookup_bwd_det(const float* f1_cl, const float* f2_pyr, const float* coords, const float* g_out, int ldg,
+                            int B, int D, int H, int W, int levels, int radius, float* g_f1, float* g_f2_pyr,
+                            void* workspace, size_t workspace_bytes, void* stream);
 
 /* Weight and bias gradient of a channel-last convolution y = conv(x, w) + b (stride 1 or 2, zero padding k/2):
  *   x  : CL [B][Hin][Win][ldx], cin % 4 == 0;   gy : CL [B][ceil(Hin/s)][ceil(Win/s)][ldg] = d loss / d y
- *   gw : [kh*kw][cin][ldw] fp32 (the packing of rnc_conv2d_cl_fwd's weight), ACCUMULATED (caller zero-fills)
- *   gb : [cout], accumulated, may be NULL
+ *   gw : [kh*kw][cin][ldw] fp32 (the packing of rnc_conv2d_cl_fwd's weight), WRITTEN (no zero-fill needed)
+ *   gb : [cout], written, may be NULL
+ * Deterministic: 64x64 (ci, co) tiles per tap, the pixels split over blocks by a count chosen from the shape alone; every
+ * block writes its fp32 partial sums to workspace, and a second kernel adds them in ascending block order, from 0, in fp32.
+ * Identical inputs give bit-identical gradients.  workspace: rnc_conv2d_cl_wgrad_workspace_bytes(...) bytes, at most 52 MB
+ * (0 for a bad shape).
  * The data gradient is rnc_conv2d_cl_fwd on gy (zero-dilated for stride 2) with the flipped, transposed weights. */
-int rnc_conv2d_cl_wgrad(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin, int Win,
-                        int kh, int kw, int stride, float* gw, int ldw, float* gb, void* stream);
+size_t rnc_conv2d_cl_wgrad_workspace_bytes(int cin, int cout, int B, int Hin, int Win, int kh, int kw, int stride);
+int rnc_conv2d_cl_wgrad_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin, int Win,
+                            int kh, int kw, int stride, float* gw, int ldw, float* gb, void* workspace, size_t workspace_bytes,
+                            void* stream);
 
 #ifdef __cplusplus
 }

@@ -111,7 +111,11 @@ stem_conv7x7s2_kernel(const float* __restrict__ img, const float* __restrict__ w
 }
 
 // ---------------------------------------------------------------- instance norm statistics: sum / sum of squares in fp64
+constexpr int kInstnormRows = 512;            // positions per CTA
 // x CL fp32 [N][P][C] (C <= 128, C % 4 == 0); stats [N][C][2] doubles, zeroed by the caller
+// PARTS: CTA (blockIdx.x, n) writes its sums to stats[((n * gridDim.x + blockIdx.x) * C + c) * 2] instead of adding them
+// (rnc_instnorm_stats_det: instnorm_reduce_kernel adds the CTAs' partials in ascending order).
+template <bool PARTS>
 __global__ void __launch_bounds__(256)
 instnorm_stats_kernel(const float* __restrict__ x, int P, int C, int rows_per_cta, double* __restrict__ stats) {
   __shared__ double ssum[8][128], ssq[8][128];
@@ -135,6 +139,7 @@ instnorm_stats_kernel(const float* __restrict__ x, int P, int C, int rows_per_ct
     ds[0] += s.x; ds[1] += s.y; ds[2] += s.z; ds[3] += s.w; dq[0] += q.x; dq[1] += q.y; dq[2] += q.z; dq[3] += q.w;
   }
   // reduce the nsub row-groups through shared memory (nsub <= 16 for C >= 64; use 8-row chunks)
+  double pa = 0, pb = 0;
   for (int base = 0; base < nsub; base += 8) {
     if (rsub >= base && rsub < base + 8 && rsub < nsub) {
 #pragma unroll
@@ -145,21 +150,49 @@ instnorm_stats_kernel(const float* __restrict__ x, int P, int C, int rows_per_ct
     if (threadIdx.x < C) {
       double a = 0, b = 0;
       for (int k = 0; k < lim; ++k) { a += ssum[k][threadIdx.x]; b += ssq[k][threadIdx.x]; }
-      atomicAdd(&stats[((size_t)n * C + threadIdx.x) * 2 + 0], a);
-      atomicAdd(&stats[((size_t)n * C + threadIdx.x) * 2 + 1], b);
+      if (PARTS) {
+        pa += a; pb += b;
+      } else {
+        atomicAdd(&stats[((size_t)n * C + threadIdx.x) * 2 + 0], a);
+        atomicAdd(&stats[((size_t)n * C + threadIdx.x) * 2 + 1], b);
+      }
     }
     __syncthreads();
   }
+  if (PARTS && threadIdx.x < C) {
+    double* dst = stats + (((size_t)n * gridDim.x + blockIdx.x) * C + threadIdx.x) * 2;
+    dst[0] = pa;
+    dst[1] = pb;
+  }
+}
+
+__device__ __forceinline__ void instnorm_mean_rstd(double sum, double sq, int P, float eps, float* out) {
+  const double mean = sum / P;
+  const double var = fmax(sq / P - mean * mean, 0.0);     // biased variance (F.instance_norm)
+  out[0] = (float)mean;
+  out[1] = (float)(1.0 / sqrt(var + (double)eps));
+}
+
+// parts [N][nblk][C][2] -> mean_rstd [N][C][2]: the CTAs' partials added in ascending CTA order
+__global__ void instnorm_reduce_kernel(const double* __restrict__ parts, int N, int nblk, int C, int P, float eps,
+                                       float* __restrict__ mean_rstd) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= N * C) return;
+  const int n = i / C, c = i - n * C;
+  double a = 0, b = 0;
+  for (int k = 0; k < nblk; ++k) {
+    const double* p = parts + (((size_t)n * nblk + k) * C + c) * 2;
+    a += p[0];
+    b += p[1];
+  }
+  instnorm_mean_rstd(a, b, P, eps, mean_rstd + 2 * (size_t)i);
 }
 
 __global__ void instnorm_finalize_kernel(double* __restrict__ stats, int NC, int P, float eps, float* __restrict__ mean_rstd, int rezero) {
   pdl_trigger();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= NC) return;
-  const double mean = stats[2 * i] / P;
-  const double var = fmax(stats[2 * i + 1] / P - mean * mean, 0.0);     // biased variance (F.instance_norm)
-  mean_rstd[2 * i] = (float)mean;
-  mean_rstd[2 * i + 1] = (float)(1.0 / sqrt(var + (double)eps));
+  instnorm_mean_rstd(stats[2 * i], stats[2 * i + 1], P, eps, mean_rstd + 2 * i);
   if (rezero) { stats[2 * i] = 0.0; stats[2 * i + 1] = 0.0; }           // ready for the next accumulating producer
 }
 
@@ -301,11 +334,30 @@ int rnc_instnorm_stats(const float* x, int N, int P, int C, float eps, double* s
   if (!x || !stats || !mean_rstd || !aligned16(x)) return RNC_ERR_BAD_POINTER;
   cudaError_t e = cudaMemsetAsync(stats, 0, (size_t)N * C * 2 * sizeof(double), as_stream(stream));
   if (e != cudaSuccess) { g_last_cuda_error = (int)e; return RNC_ERR_CUDA; }
-  const int rows = 512;
+  const int rows = kInstnormRows;
   dim3 grid((P + rows - 1) / rows, N);
-  instnorm_stats_kernel<<<grid, 256, 0, as_stream(stream)>>>(x, P, C, rows, stats);
+  instnorm_stats_kernel<false><<<grid, 256, 0, as_stream(stream)>>>(x, P, C, rows, stats);
   if (int st = after_launch()) return st;
   instnorm_finalize_kernel<<<(N * C + 127) / 128, 128, 0, as_stream(stream)>>>(stats, N * C, P, eps, mean_rstd, 1);
+  return after_launch();
+}
+
+size_t rnc_instnorm_stats_det_workspace_bytes(int N, int P, int C) {
+  if (N <= 0 || P <= 0 || C <= 0 || C > 128 || (C & 3)) return 0;
+  return (size_t)N * ((P + kInstnormRows - 1) / kInstnormRows) * C * 2 * sizeof(double);
+}
+
+int rnc_instnorm_stats_det(const float* x, int N, int P, int C, float eps, void* workspace, size_t workspace_bytes,
+                           float* mean_rstd, void* stream) {
+  if (N <= 0 || P <= 0 || C <= 0 || C > 128 || (C & 3)) return RNC_ERR_BAD_SHAPE;
+  if (!x || !workspace || !mean_rstd || !aligned16(x) || !aligned16(workspace)) return RNC_ERR_BAD_POINTER;
+  if (workspace_bytes < rnc_instnorm_stats_det_workspace_bytes(N, P, C)) return RNC_ERR_WORKSPACE;
+  const int nblk = (P + kInstnormRows - 1) / kInstnormRows;
+  dim3 grid(nblk, N);
+  double* parts = static_cast<double*>(workspace);
+  instnorm_stats_kernel<true><<<grid, 256, 0, as_stream(stream)>>>(x, P, C, kInstnormRows, parts);
+  if (int st = after_launch()) return st;
+  instnorm_reduce_kernel<<<(N * C + 127) / 128, 128, 0, as_stream(stream)>>>(parts, N, nblk, C, P, eps, mean_rstd);
   return after_launch();
 }
 

@@ -4,7 +4,8 @@ The wide 3x3 / 1x1 layers run on rnc_conv2d_umma_fwd (fp16 hi/lo split operands,
 normalised image is repacked once as a zero-padded [H][W+8][4] plane of split halves and the convolution reads it through a
 sliding-window tensor map (16-pixel windows 16 bytes apart: the TMA unit builds the im2col rows; 7 row taps x 64 = K 448 with
 zero weights for the 9 phantom pixels and the phantom channel); InstanceNorm (fnet) is a statistics pass + an apply pass fused with
-ReLU / residual add / re-splitting; BatchNorm (cnet, eval mode) is folded into the convolution weights.  The encoders write
+ReLU / residual add / re-splitting (under torch.use_deterministic_algorithms the statistics are per-CTA partials added in a
+fixed order, rnc_instnorm_stats_det, instead of the convolution epilogue's fp64 atomics); BatchNorm (cnet, eval mode) is folded into the convolution weights.  The encoders write
 their results straight into the loop's resident buffers: fmap1 -> f1_cl, fmap2 -> level 0 of f2_pyr, tanh(net) -> h and
 hx[:, 0:128], relu(inp) -> hx[:, 128:256] (raft_nc_dbl.py:129-140).
 """
@@ -74,6 +75,13 @@ class EncoderBuffers:
         self.img_lo = torch.zeros(npx, 4, dtype=torch.float16, device=device)
         self.stats = torch.zeros(N * 128 * 2, dtype=torch.float64, device=device)   # kept zeroed by rnc_instnorm_finalize
         self.mr = torch.empty(N * 128 * 2, **f)
+        self.parts = None                                  # rnc_instnorm_stats_det's partials, sized on first use
+
+    def det_workspace(self, L, N):
+        if self.parts is None:
+            nbytes = max(L.rnc_instnorm_stats_det_workspace_bytes(N, h * w, c) for (h, w, c) in self.dims)
+            self.parts = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=self.stats.device)
+        return self.parts
 
 
 class EncoderRunner:
@@ -93,12 +101,15 @@ class EncoderRunner:
 
     # ------------------------------------------------------------------ instance-norm helpers
     def _norm(self, bufs, x32, N, P, Cc, mode, res=None, out32=None, split=None, fused_stats=False):
-        """fused_stats: the producing convolution already accumulated the sums into bufs.stats (rnc_conv_umma_desc.stats)."""
+        """fused_stats: the producing convolution already accumulated the sums into bufs.stats (rnc_conv_umma_desc.stats);
+        otherwise the deterministic statistics pass reads x32."""
         s = _stream()
         if fused_stats:
             native.check(self.L.rnc_instnorm_finalize(_ptr(bufs.stats), N, P, Cc, EPS, _ptr(bufs.mr), s), "instnorm_finalize")
         else:
-            native.check(self.L.rnc_instnorm_stats(_ptr(x32), N, P, Cc, EPS, _ptr(bufs.stats), _ptr(bufs.mr), s), "instnorm_stats")
+            ws = bufs.det_workspace(self.L, N)
+            native.check(self.L.rnc_instnorm_stats_det(_ptr(x32), N, P, Cc, EPS, _ptr(ws), ws.numel() * 8, _ptr(bufs.mr), s),
+                         "instnorm_stats_det")
         native.check(self.L.rnc_instnorm_apply(_ptr(x32), _ptr(bufs.mr), _ptr(res), N, P, Cc, mode, _ptr(out32),
                                                C.c_void_p(split.hi.data_ptr() if split else 0),
                                                C.c_void_p(split.lo.data_ptr() if split else 0), s), "instnorm_apply")
@@ -107,6 +118,8 @@ class EncoderRunner:
         """Stem + the six residual blocks.  Leaves the 128-channel features at 1/8 resolution in bufs.XS[2] (split)."""
         E, eng, s = native, self.eng, _stream()
         inst = pk.kind == "instance"
+        fused = not torch.are_deterministic_algorithms_enabled()    # epilogue statistics use fp64 atomics
+        st = bufs.stats.data_ptr() if fused else 0
         h, w, _ = bufs.dims[0]
         native.check(self.L.rnc_stem_window_prep(_ptr(image), N, Hin, Win, bufs.pitch, _ptr(bufs.img_hi), _ptr(bufs.img_lo), s),
                      "stem_window_prep")
@@ -114,8 +127,8 @@ class EncoderRunner:
         img = (bufs.img_hi.data_ptr(), bufs.img_lo.data_ptr())
         if inst:
             eng.uconv(N, h, w, img, 64, 8, pk.stem, E.EPI_LINEAR, out_f32=bufs.T32[0].data_ptr(), ldo_f32=64,
-                      stats=bufs.stats.data_ptr(), **win)
-            self._norm(bufs, bufs.T32[0], N, h * w, 64, 1, out32=bufs.X32[0], split=bufs.XS[0], fused_stats=True)
+                      stats=st, **win)
+            self._norm(bufs, bufs.T32[0], N, h * w, 64, 1, out32=bufs.X32[0], split=bufs.XS[0], fused_stats=fused)
         else:
             eng.uconv(N, h, w, img, 64, 8, pk.stem, E.EPI_RELU, out_f32=bufs.X32[0].data_ptr(), ldo_f32=64,
                       out_split=bufs.XS[0].ptrs(), ldo_split=64, **win)
@@ -131,20 +144,19 @@ class EncoderRunner:
             P = h * w
             xs_in, x32_in = bufs.XS[src], bufs.X32[src]
             if inst:
-                st = bufs.stats.data_ptr()
                 eng.uconv(N, h, w, xs_in.ptrs(), cin, cin, w1, E.EPI_LINEAR, out_f32=bufs.T32[lvl].data_ptr(), ldo_f32=cout,
                           stride=stride, hin=hi_, win=wi_, stats=st)
-                self._norm(bufs, bufs.T32[lvl], N, P, cout, 1, split=bufs.AS[lvl], fused_stats=True)
+                self._norm(bufs, bufs.T32[lvl], N, P, cout, 1, split=bufs.AS[lvl], fused_stats=fused)
                 res = x32_in
                 if wd is not None:
                     eng.uconv(N, h, w, xs_in.ptrs(), cin, cin, wd, E.EPI_LINEAR, out_f32=bufs.T32[lvl].data_ptr(), ldo_f32=cout,
                               stride=stride, hin=hi_, win=wi_, stats=st)
-                    self._norm(bufs, bufs.T32[lvl], N, P, cout, 0, out32=bufs.D32[lvl], fused_stats=True)
+                    self._norm(bufs, bufs.T32[lvl], N, P, cout, 0, out32=bufs.D32[lvl], fused_stats=fused)
                     res = bufs.D32[lvl]
                 eng.uconv(N, h, w, bufs.AS[lvl].ptrs(), cout, cout, w2, E.EPI_LINEAR, out_f32=bufs.T32[lvl].data_ptr(), ldo_f32=cout,
                           stats=st)
                 self._norm(bufs, bufs.T32[lvl], N, P, cout, 2, res=res, out32=bufs.X32[lvl] if need32 else None, split=bufs.XS[lvl],
-                           fused_stats=True)
+                           fused_stats=fused)
             else:
                 eng.uconv(N, h, w, xs_in.ptrs(), cin, cin, w1, E.EPI_RELU, out_split=bufs.AS[lvl].ptrs(), ldo_split=cout,
                           stride=stride, hin=hi_, win=wi_)

@@ -363,7 +363,9 @@ class Engine:
         B, _, Him, Wim = image1.shape
         if flow_init is not None and tuple(flow_init.shape) != (B, 2, Him // 8, Wim // 8):
             raise ValueError("flow_init must be [N,2,H/8,W/8]")
-        key = (type(model).__name__, tuple(image1.shape), iters, flow_init is not None, _param_key(model))
+        # a graph records one mode's kernels: the deterministic mode gets its own (torch.use_deterministic_algorithms)
+        key = (type(model).__name__, tuple(image1.shape), iters, flow_init is not None, _param_key(model),
+               torch.are_deterministic_algorithms_enabled())
         first = key not in self._graphs
         ent = _lru_get(self._graphs, key, self.MAX_GRAPHS, dict)
         if first:

@@ -4,7 +4,7 @@
 
     ConvCL          every nn.Conv2d (update.py, extractor.py, interp_weights_est.py): rnc_conv2d_cl_fwd; data gradient = the same
                     kernel on the (zero-dilated, for stride 2) output gradient with flipped / transposed weights; weight and bias
-                    gradient = rnc_conv2d_cl_wgrad
+                    gradient = rnc_conv2d_cl_wgrad_det (fixed-order sum of the K-split partials)
     CorrPyramid     CorrBlock.__init__ on features (corr.py:7-21): rnc_fmap_pyramid / adjoint rnc_pyramid_pool_bwd
     CorrLookup      CorrBlock.__call__ (corr.py:23-44): rnc_corr_lookup_fwd / rnc_corr_lookup_bwd (d fmap1, d fmap2 pyramid; coords
                     are detached, raft_nc_dbl.py:149)
@@ -14,6 +14,10 @@
                     rnc_ncup_bwd (fused, deterministic); used by the frozen-trunk forward (rnc.model.frozen_trunk), which runs the
                     trunk on the inference engine.  Other configurations run the NConv2dFn / NConvPoolFn chain of
                     rnc/nconv_unet.py there too.
+
+Under torch.use_deterministic_algorithms(True) the lookup backward, which otherwise scatters d fmap2 with floating-point
+atomics, switches to its fixed-order form rnc_corr_lookup_bwd_det (deterministic()); the weight gradient sums in a fixed order
+in both modes.  Identical steps then give bit-identical gradients.
 
 Activations stay channel-last ([B, H, W, C] fp32) between convolutions.  Pointwise glue (ReLU / sigmoid / tanh / gate blend,
 cat, nearest x2, zero-stuffing, the loss) and the normalisation layers (InstanceNorm / BatchNorm: library kernels, like cuDNN
@@ -61,6 +65,12 @@ def _packed(weight, kind, cin_pad, fmt="ffma"):
             packed = UmmaWeights(w, None, [cin_pad], scale_log2=10)
         hit = _PACK_CACHE[key] = (weight, packed)
     return hit[1]
+
+
+def deterministic():
+    """torch.use_deterministic_algorithms(True) is in force: the lookup backward gathers d fmap2 in a fixed order instead of
+    scattering it with atomics."""
+    return torch.are_deterministic_algorithms_enabled()
 
 
 def _ceil4(c):
@@ -204,13 +214,23 @@ class ConvCL(torch.autograd.Function):
                 if gx.shape[-1] != Cx:               # Cx > ceil4(cin) never happens; equal by construction
                     gx = F.pad(gx, (0, Cx - gx.shape[-1]))
             if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):
-                gwp = torch.zeros(kh * kw, Cx, cout, dtype=torch.float32, device=x.device)
-                gbp = torch.zeros(cout, dtype=torch.float32, device=x.device) if ctx.has_bias else None
-                native.check(eng.L.rnc_conv2d_cl_wgrad(_ptr(x), Cx, Cx, _ptr(gy), ldg, cout, B, H, W, kh, kw, ctx.stride,
-                                                       _ptr(gwp), cout, _ptr(gbp), _stream()), "conv2d_cl_wgrad")
+                gwp, gbp = _wgrad(eng, x, gy, cout, kh, kw, ctx.stride, ctx.has_bias)
                 gw = gwp.view(kh, kw, Cx, cout)[:, :, :cin].permute(3, 2, 0, 1).contiguous()
                 gb = gbp
         return gx, gw, gb, None
+
+
+def _wgrad(eng, x, gy, cout, kh, kw, stride, has_bias):
+    """Weight / bias gradient of ConvCL: [kh*kw, Cx, cout], [cout] (or None).  rnc_conv2d_cl_wgrad_det sums the K-split
+    partials in a fixed order (in either mode: it is no slower than adding them with atomics was) and writes its outputs."""
+    B, H, W, Cx = x.shape
+    gwp = torch.empty(kh * kw, Cx, cout, dtype=torch.float32, device=x.device)
+    gbp = torch.empty(cout, dtype=torch.float32, device=x.device) if has_bias else None
+    nbytes = eng.L.rnc_conv2d_cl_wgrad_workspace_bytes(Cx, cout, B, H, W, kh, kw, stride)
+    ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=x.device)
+    native.check(eng.L.rnc_conv2d_cl_wgrad_det(_ptr(x), Cx, Cx, _ptr(gy), gy.shape[-1], cout, B, H, W, kh, kw, stride, _ptr(gwp),
+                                               cout, _ptr(gbp), _ptr(ws), ws.numel() * 4, _stream()), "conv2d_cl_wgrad_det")
+    return gwp, gbp
 
 
 def conv_cl(x, conv, stride=None):
@@ -281,14 +301,27 @@ class CorrLookup(torch.autograd.Function):
     def backward(ctx, g_out):
         f1_cl, f2_pyr, coords = ctx.saved_tensors
         eng = engine_for(f1_cl.device)
-        B, H, W, D = f1_cl.shape
-        g_out = g_out.contiguous()
         with torch.cuda.device(f1_cl.device):
-            g_f1 = torch.empty_like(f1_cl)
-            g_f2 = torch.zeros_like(f2_pyr)
-            native.check(eng.L.rnc_corr_lookup_bwd(_ptr(f1_cl), _ptr(f2_pyr), _ptr(coords), _ptr(g_out), g_out.shape[-1], B, D, H, W,
-                                                   ctx.levels, 4, _ptr(g_f1), _ptr(g_f2), _stream()), "corr_lookup_bwd")
+            g_f1, g_f2 = _lookup_bwd(eng, f1_cl, f2_pyr, coords, g_out.contiguous(), ctx.levels)
         return g_f1, g_f2, None, None
+
+
+def _lookup_bwd(eng, f1_cl, f2_pyr, coords, g_out, levels):
+    """(d fmap1, d fmap2 pyramid) of CorrLookup.  Deterministic mode gathers d fmap2 per pyramid position in a fixed order
+    (rnc_corr_lookup_bwd_det, which writes every position); otherwise every pixel scatters into it with atomics."""
+    B, H, W, D = f1_cl.shape
+    args = (_ptr(f1_cl), _ptr(f2_pyr), _ptr(coords), _ptr(g_out), g_out.shape[-1], B, D, H, W, levels, 4)
+    g_f1 = torch.empty_like(f1_cl)
+    if deterministic():
+        g_f2 = torch.empty_like(f2_pyr)
+        nbytes = eng.L.rnc_corr_lookup_bwd_workspace_bytes(B, H, W, levels)
+        ws = torch.empty((nbytes + 15) // 16, 4, dtype=torch.float32, device=f1_cl.device)
+        native.check(eng.L.rnc_corr_lookup_bwd_det(*args, _ptr(g_f1), _ptr(g_f2), _ptr(ws), ws.numel() * 4, _stream()),
+                     "corr_lookup_bwd_det")
+    else:
+        g_f2 = torch.zeros_like(f2_pyr)
+        native.check(eng.L.rnc_corr_lookup_bwd(*args, _ptr(g_f1), _ptr(g_f2), _stream()), "corr_lookup_bwd")
+    return g_f1, g_f2
 
 
 def corr_lookup_autograd(corr_block, coords):
@@ -582,7 +615,11 @@ def ncup_upsampler_train(up, x_lowres, x_guidance, out_scale=1.0):
     """NConvUpsampler.forward (upsampler.py:143-177) with autograd: x_lowres NCHW [B,2,h,w], guidance NCHW [B,128,h/2,w/2]."""
     _require_cuda(x_lowres, x_guidance)
     with torch.cuda.device(x_lowres.device):
-        g4 = F.interpolate(x_guidance, x_lowres.shape[2:], mode="area")           # integer x2 'area' upscale = replication
+        # the reference's F.interpolate(mode='area') to twice the size: every area window holds one element, so it is the
+        # nearest x2 replication, whose backward adds each element's four terms in a fixed order (area's adds them atomically)
+        if tuple(x_lowres.shape[2:]) != (2 * x_guidance.shape[2], 2 * x_guidance.shape[3]):
+            raise ValueError("ncup_upsampler_train: the guidance must have half the resolution of x_lowres")
+        g4 = F.interpolate(x_guidance, scale_factor=2, mode="nearest")
         w4 = simple_cl(up.weights_est_net, to_cl(torch.cat([x_lowres, g4], 1), pad_to=136))     # pitch % 8 == 0: tensor-core layer
         return _ncup_chain_train(up.interpolation_net, x_lowres, w4, out_scale, fused=False)
 
