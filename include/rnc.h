@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 13) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 14) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -147,6 +147,9 @@ typedef struct {
 } rnc_conv_desc;
 
 int rnc_conv2d_cl_fwd(const rnc_conv_desc* desc, void* stream);
+/* rnc_conv2d_cl_fwd with filter dilation dil (1..8): tap (ky, kx) reads input (y + (ky - kh/2)*dil, x + (kx - kw/2)*dil), zero
+ * outside, i.e. nn.Conv2d(dilation=dil, padding=(k/2)*dil).  dil > 1 takes the LINEAR / RELU / SIGMOID epilogues. */
+int rnc_conv2d_cl_dil_fwd(const rnc_conv_desc* desc, int dil, void* stream);
 
 /* Tensor-core version of rnc_conv2d_cl_fwd (same reference code, same epilogues): wgmma on fp16 hi/lo split
  * operands with fp32 accumulation in registers (3 MMAs per K step: hi*hi + hi*lo + lo*hi), TMA-staged tiles.
@@ -184,6 +187,11 @@ typedef struct {
                                         * windows overlap; the TMA unit builds the im2col rows); win = positions per row (one
                                         * per output column), hin = rows, the stride applies to rows only. Used by the encoders'
                                         * 7x7/2 stem: a [hin][win_pitch/4][4] zero-padded pixel plane, 16-pixel windows, ld0 = 8 */
+  int dil;                             /* filter dilation 0..8 (0 or 1: none): tap (ky, kx) reads input (y + (ky - kh/2)*dil,
+                                        * x + (kx - kw/2)*dil), zero outside (padding (k/2)*dil, nn.Conv2d(dilation=dil)).  dil > 1:
+                                        * stride 1, LINEAR / RELU / SIGMOID, no stats / add / blocked / window operands; fp16 and TF32.
+                                        * Runs as dil^2 launches, one per output phase (y % dil, x % dil), each the undilated
+                                        * convolution of that phase's input and output sub-images (strided tensor maps). */
 } rnc_conv_umma_desc;
 
 /* Pixel tiles (128 output pixels each) a layer of this shape is cut into: a tile-blocked tensor with ld channels has
@@ -434,6 +442,14 @@ size_t rnc_conv2d_cl_wgrad_workspace_bytes(int cin, int cout, int B, int Hin, in
 int rnc_conv2d_cl_wgrad_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin, int Win,
                             int kh, int kw, int stride, float* gw, int ldw, float* gb, void* workspace, size_t workspace_bytes,
                             void* stream);
+/* The same weight / bias gradient for a stride-1 convolution with dilation dil (1..8; rnc_conv2d_cl_dil_fwd): tap (ky, kx) pairs
+ * gy at (y, x) with x at (y + (ky - kh/2)*dil, x + (kx - kw/2)*dil).  Same tiles, K split, fixed-order sum and workspace size as
+ * the undilated layer (0 bytes for a bad shape or dil).  Its data gradient is rnc_conv2d_cl_dil_fwd on gy with the flipped,
+ * transposed weights and the same dil. */
+size_t rnc_conv2d_cl_wgrad_dil_workspace_bytes(int cin, int cout, int B, int Hin, int Win, int kh, int kw, int dil);
+int rnc_conv2d_cl_wgrad_dil_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin, int Win,
+                                int kh, int kw, int dil, float* gw, int ldw, float* gb, void* workspace, size_t workspace_bytes,
+                                void* stream);
 
 #ifdef __cplusplus
 }

@@ -15,6 +15,7 @@ constexpr int APAD = 4;
 struct ConvParams {
   rnc_conv_desc d;
   int M, cin, coutpad, nchunk_per_tap;
+  int dil;                             // filter dilation: tap (ky, kx) reads (y + (ky - kh/2) * dil, x + (kx - kw/2) * dil)
 };
 
 __device__ __forceinline__ float apply_act(float v, int epi) {
@@ -48,13 +49,13 @@ conv_cl_ffma_kernel(const ConvParams p) {
 
   const int ntaps = d.kh * d.kw;
   const int nchunks = ntaps * p.nchunk_per_tap;
-  const int ph = d.kh / 2, pw = d.kw / 2;
+  const int ph = d.kh / 2 * p.dil, pw = d.kw / 2 * p.dil;
 
   float4 ra[4], rb[2];
   auto load_chunk = [&](int kc) {
     const int tap = kc / p.nchunk_per_tap;
     const int ci0 = (kc - tap * p.nchunk_per_tap) * BK;
-    const int dy = tap / d.kw - ph, dx = tap % d.kw - pw;
+    const int dy = tap / d.kw * p.dil - ph, dx = tap % d.kw * p.dil - pw;
     const int ci = ci0 + 4 * lq;
     const float* base; int ld, cc;
     if (ci < d.c0) { base = d.in0; ld = d.ld0; cc = ci; } else { base = d.in1; ld = d.ld1; cc = ci - d.c0; }
@@ -186,9 +187,11 @@ conv_cl_ffma_kernel(const ConvParams p) {
 
 using namespace rnc;
 
-extern "C" int rnc_conv2d_cl_fwd(const rnc_conv_desc* desc, void* stream) {
+static int conv_cl(const rnc_conv_desc* desc, int dil, void* stream) {
   if (!desc) return RNC_ERR_BAD_POINTER;
   const rnc_conv_desc& d = *desc;
+  if (dil < 1 || dil > 8) return RNC_ERR_BAD_SHAPE;
+  if (dil > 1 && d.epilogue != RNC_EPI_LINEAR && d.epilogue != RNC_EPI_RELU && d.epilogue != RNC_EPI_SIGMOID) return RNC_ERR_UNSUPPORTED;
   if (d.B <= 0 || d.H <= 0 || d.W <= 0 || d.cout <= 0 || d.c0 <= 0 || d.c1 < 0) return RNC_ERR_BAD_SHAPE;
   if (d.kh < 1 || d.kw < 1 || !(d.kh & 1) || !(d.kw & 1) || d.kh * d.kw > 49) return RNC_ERR_BAD_SHAPE;
   if ((d.c0 & 3) || (d.c1 & 3) || (d.ld0 & 3) || d.ld0 < d.c0) return RNC_ERR_BAD_SHAPE;
@@ -217,7 +220,12 @@ extern "C" int rnc_conv2d_cl_fwd(const rnc_conv_desc* desc, void* stream) {
   p.cin = d.c0 + d.c1;
   p.coutpad = (d.cout + BN - 1) / BN * BN;
   p.nchunk_per_tap = (p.cin + BK - 1) / BK;
+  p.dil = dil;
   dim3 grid((p.M + BM - 1) / BM, p.coutpad / BN);
   conv_cl_ffma_kernel<<<grid, CT, 0, as_stream(stream)>>>(p);
   return after_launch();
 }
+
+extern "C" int rnc_conv2d_cl_fwd(const rnc_conv_desc* desc, void* stream) { return conv_cl(desc, 1, stream); }
+
+extern "C" int rnc_conv2d_cl_dil_fwd(const rnc_conv_desc* desc, int dil, void* stream) { return conv_cl(desc, dil, stream); }

@@ -559,15 +559,24 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
 }
 
 // ---------------------------------------------------------------------------------------------- host side
+// Phase (dil, ry, rx) of a plane: its sub-image of the pixels (ry + dil * y', rx + dil * x').  A convolution with dilation dil
+// maps output phase (ry, rx) onto input phase (ry, rx) alone, as the undilated convolution of the two sub-images (tap (ky, kx)
+// reads y' + ky - kh/2, x' + kx - kw/2), so a dilated layer is dil^2 launches of the same kernel on strided views.
+struct Phase {
+  int dil = 1, ry = 0, rx = 0;
+  int len(int n, int r) const { return (n - r + dil - 1) / dil; }      // sub-image extent along an axis of n pixels
+};
+
 // activation plane [B][Hin][Win][ld] halves: 4-D map {C, Win, Hin, B}; the box spans bw x bh input elements and is
 // traversed with element strides (sx, sy) -> (bw/sx) x (bh/sy) rows of 64 channels in shared memory
 static bool make_in_map(CUtensorMap* m, const void* base, int C, int ld, int B, int Hin, int Win, int bw, int bh, int sx, int sy, bool tf32,
-                        long long row_pitch = 0) {
+                        long long row_pitch = 0, Phase ph = Phase()) {
   const cuuint64_t esz = tf32 ? 4 : 2;                        // 128-byte rows: 32 fp32 words or 64 halves
   const cuuint64_t pitch = row_pitch > 0 ? (cuuint64_t)row_pitch : (cuuint64_t)Win * ld;     // elements between image rows
-  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)Win, (cuuint64_t)Hin, (cuuint64_t)B};
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)ph.len(Win, ph.rx), (cuuint64_t)ph.len(Hin, ph.ry), (cuuint64_t)B};
+  base = static_cast<const char*>(base) + (ph.ry * pitch + (cuuint64_t)ph.rx * ld) * esz;
   // window view (RNC_CONV_WINDOW): ld < C, i.e. consecutive positions overlap -- the TMA unit walks plain strides
-  const cuuint64_t strides[3] = {(cuuint64_t)ld * esz, pitch * esz, (cuuint64_t)Hin * pitch * esz};
+  const cuuint64_t strides[3] = {(cuuint64_t)ph.dil * ld * esz, ph.dil * pitch * esz, (cuuint64_t)Hin * pitch * esz};
   const cuuint32_t box[4] = {tf32 ? 32u : 64u, (cuuint32_t)(bw * sx), (cuuint32_t)(bh * sy), 1};
   const cuuint32_t es[4] = {1, (cuuint32_t)sx, (cuuint32_t)sy, 1};
   return encode_fn()(m, tf32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
@@ -587,10 +596,12 @@ static bool make_w_map(CUtensorMap* m, const void* base, int ktot, int coutpad, 
 
 // output plane [B][H][W][ld] (halves or fp32): 4-D map {C, W, H, B}, box = 32 channels x one lane group's bw x bh pixels,
 // rows swizzled (64B for halves, 128B for fp32) to match the epilogue's conflict-free staging writes
-static bool make_out_map(CUtensorMap* m, const void* base, int C, int ld, int B, int H, int W, int bw, int bh, bool f32) {
+static bool make_out_map(CUtensorMap* m, const void* base, int C, int ld, int B, int H, int W, int bw, int bh, bool f32,
+                         Phase ph = Phase()) {
   const cuuint64_t esz = f32 ? 4 : 2;
-  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-  const cuuint64_t strides[3] = {(cuuint64_t)ld * esz, (cuuint64_t)W * ld * esz, (cuuint64_t)H * W * ld * esz};
+  const cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)ph.len(W, ph.rx), (cuuint64_t)ph.len(H, ph.ry), (cuuint64_t)B};
+  base = static_cast<const char*>(base) + ((cuuint64_t)ph.ry * W + ph.rx) * ld * esz;
+  const cuuint64_t strides[3] = {(cuuint64_t)ph.dil * ld * esz, (cuuint64_t)ph.dil * W * ld * esz, (cuuint64_t)H * W * ld * esz};
   const cuuint32_t box[4] = {32u, (cuuint32_t)bw, (cuuint32_t)bh, 1};
   const cuuint32_t es[4] = {1, 1, 1, 1};
   return encode_fn()(m, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims, strides, box, es,
@@ -677,13 +688,13 @@ extern "C" long long rnc_conv_umma_tiles(int kh, int kw, int stride, int B, int 
 // tile already take 128 registers per consumer thread.  Cost model in K-step units: per K-step 1.0 / 0.68 / 0.57 for
 // 128 / 64 / 32 columns (operand bytes per K-step: the A tile plus the weight tile), + 0.5 per item, x1.08 when the A tile
 // is loaded more than once.
-static int choose_bn(const rnc_conv_umma_desc& d, int bn_max, int stride) {
+static int choose_bn(const rnc_conv_umma_desc& d, int bn_max, int stride, int H, int W) {
   if (d.flags & RNC_CONV_SPLIT_N) return bn_max;
   const int bkc = (d.flags & RNC_CONV_TF32) ? 32 : 64;
   const int taps = d.kh * d.kw, ksteps = taps * ((d.c0 + bkc - 1) / bkc + (d.c1 + bkc - 1) / bkc);
   int TW, TH;
-  tile_shape(d.kh, d.kw, stride, d.H, d.W, d.flags, TW, TH);
-  const long ntiles = static_cast<long>(d.B) * ((d.W + TW - 1) / TW) * ((d.H + TH - 1) / TH);
+  tile_shape(d.kh, d.kw, stride, H, W, d.flags, TW, TH);
+  const long ntiles = static_cast<long>(d.B) * ((W + TW - 1) / TW) * ((H + TH - 1) / TH);
   static const int cand[3] = {128, 64, 32};
   static const float per_k[3] = {1.0f, 0.68f, 0.57f};
   const long slots = umma::sm_count();
@@ -703,10 +714,10 @@ static int choose_bn(const rnc_conv_umma_desc& d, int bn_max, int stride) {
   return best;
 }
 
-extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream) {
+// One launch: the whole layer (ph = Phase()), or the output phase ph of a dilated layer (d.H, d.W: the full planes' size).
+static int conv_umma(const rnc_conv_umma_desc& d, umma::Phase ph, void* stream) {
   using namespace rnc::umma;
-  if (!desc) return RNC_ERR_BAD_POINTER;
-  const rnc_conv_umma_desc& d = *desc;
+  const int H = ph.len(d.H, ph.ry), W = ph.len(d.W, ph.rx);       // output pixels of this launch
   const int stride = d.stride <= 0 ? 1 : d.stride;
   const int Hin = d.hin > 0 ? d.hin : d.H, Win = d.win > 0 ? d.win : d.W;
   if (d.B <= 0 || d.H <= 0 || d.W <= 0 || d.cout <= 0 || d.c0 <= 0 || d.c1 < 0 || stride > 2) return RNC_ERR_BAD_SHAPE;
@@ -731,7 +742,7 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
   while (bn > 32 && d.coutpad % bn != 0) bn >>= 1;            // the widest column tile that divides coutpad
   if (d.coutpad % bn != 0) bn = bn0;
   if (d.coutpad % bn == 0 && d.epilogue != RNC_EPI_RELU_FLOW && d.epilogue != RNC_EPI_FLOW_DELTA)
-    bn = choose_bn(d, bn, stride);
+    bn = choose_bn(d, bn, stride, H, W);
   if (d.coutpad % bn != 0 || d.coutpad < d.cout) return RNC_ERR_BAD_SHAPE;
   if (d.epilogue == RNC_EPI_RELU_FLOW && (d.coutpad < d.cout + 2 || !d.aux0 || !d.out_hi)) return RNC_ERR_BAD_SHAPE;
   if (d.out_hi && (!d.out_lo || (d.ldo_split & 7) || !aligned16(d.out_hi) || !aligned16(d.out_lo))) return RNC_ERR_BAD_POINTER;
@@ -766,19 +777,19 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
 
   // ---- tile shape and A-staging mode
   Params p;
-  p.B = d.B; p.H = d.H; p.W = d.W;
+  p.B = d.B; p.H = H; p.W = W;
   p.kh = d.kh; p.kw = d.kw; p.ph = d.kh / 2; p.pw = d.kw / 2; p.stride = stride; p.sx = window ? 1 : stride;
   int mode = MODE_TAP;
   if (stride == 1 && (d.flags & RNC_CONV_NO_HALO) == 0) {
-    if (d.kw > 1 && d.W > 64) mode = MODE_ROWHALO;                 // one image row x 128 px per tile
-    else if (d.kw == 1 && d.kh > 1 && d.W >= 16 && d.H >= 8) mode = MODE_COLHALO;
+    if (d.kw > 1 && W > 64) mode = MODE_ROWHALO;                   // one image row x 128 px per tile
+    else if (d.kw == 1 && d.kh > 1 && W >= 16 && H >= 8) mode = MODE_COLHALO;
   }
   int TW, TH, box_w, box_h;
   if (mode == MODE_ROWHALO) { TW = 128; TH = 1; box_w = 136; box_h = 1; }
   else if (mode == MODE_COLHALO) { TW = 16; TH = 8; box_w = 16; box_h = TH + 2 * p.ph; }
   else {
     TW = 8;
-    while (TW < d.W && TW < kBM) TW <<= 1;
+    while (TW < W && TW < kBM) TW <<= 1;
     TH = kBM / TW; box_w = TW; box_h = TH;
   }
   if (box_w * box_h > 256 - 8 && mode == MODE_COLHALO) return RNC_ERR_UNSUPPORTED;   // kh <= 9
@@ -787,7 +798,7 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
     static const char* env = getenv("RNC_CONV_PROBE_NOB");
     p.probe_nob = env != nullptr && env[0] == '1';
   }
-  p.tiles_x = (d.W + TW - 1) / TW; p.tiles_y = (d.H + TH - 1) / TH;
+  p.tiles_x = (W + TW - 1) / TW; p.tiles_y = (H + TH - 1) / TH;
   p.ntiles = d.B * p.tiles_x * p.tiles_y; p.ntn = d.coutpad / bn;
   p.a_plane = box_w * box_h * 128;
   // tall halo boxes (COLHALO, kh >= 5) beside 128-column weight stages leave no room for two stages of each ring
@@ -807,11 +818,11 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
 
   CUtensorMap maps[9];
   const long long pitch0 = window ? d.win_pitch : 0;
-  bool ok = make_in_map(&maps[0], d.in0_hi, d.c0, d.ld0, d.B, Hin, Win, box_w, box_h, p.sx, stride, tf32, pitch0) &&
-            make_in_map(&maps[1], d.in0_lo, d.c0, d.ld0, d.B, Hin, Win, box_w, box_h, p.sx, stride, tf32, pitch0);
+  bool ok = make_in_map(&maps[0], d.in0_hi, d.c0, d.ld0, d.B, Hin, Win, box_w, box_h, p.sx, stride, tf32, pitch0, ph) &&
+            make_in_map(&maps[1], d.in0_lo, d.c0, d.ld0, d.B, Hin, Win, box_w, box_h, p.sx, stride, tf32, pitch0, ph);
   if (d.c1 > 0) {
-    ok = ok && make_in_map(&maps[2], d.in1_hi, d.c1, d.ld1, d.B, Hin, Win, box_w, box_h, stride, stride, tf32) &&
-         make_in_map(&maps[3], d.in1_lo, d.c1, d.ld1, d.B, Hin, Win, box_w, box_h, stride, stride, tf32);
+    ok = ok && make_in_map(&maps[2], d.in1_hi, d.c1, d.ld1, d.B, Hin, Win, box_w, box_h, stride, stride, tf32, 0, ph) &&
+         make_in_map(&maps[3], d.in1_lo, d.c1, d.ld1, d.B, Hin, Win, box_w, box_h, stride, stride, tf32, 0, ph);
   } else {
     maps[2] = maps[0]; maps[3] = maps[1];
   }
@@ -824,8 +835,8 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
     const int cw = d.epilogue == RNC_EPI_GRU_ZR ? d.cout / 2 : (d.cout + flow2 + 31) / 32 * 32;
     if (d.out_hi) {
       if ((d.ldo_split & 7) || !aligned16(d.out_hi) || !aligned16(d.out_lo) || d.ldo_split < cw) return RNC_ERR_BAD_POINTER;
-      ok = ok && make_out_map(&maps[6], d.out_hi, cw, d.ldo_split, d.B, d.H, d.W, obw, obh, false) &&
-           make_out_map(&maps[7], d.out_lo, cw, d.ldo_split, d.B, d.H, d.W, obw, obh, false);
+      ok = ok && make_out_map(&maps[6], d.out_hi, cw, d.ldo_split, d.B, d.H, d.W, obw, obh, false, ph) &&
+           make_out_map(&maps[7], d.out_lo, cw, d.ldo_split, d.B, d.H, d.W, obw, obh, false, ph);
     } else {
       maps[6] = maps[0]; maps[7] = maps[0];
     }
@@ -835,7 +846,7 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
     } else if (d.out_f32 && !p.out_blocked && d.epilogue != RNC_EPI_FLOW_DELTA) {
       const int cf = d.epilogue == RNC_EPI_TANH_RELU ? d.cout / 2 : (d.cout + 31) / 32 * 32;   // TANH_RELU: only the tanh half
       if (d.ldo_f32 < cf) return RNC_ERR_BAD_SHAPE;
-      ok = ok && make_out_map(&maps[8], d.out_f32, cf, d.ldo_f32, d.B, d.H, d.W, obw, obh, true);
+      ok = ok && make_out_map(&maps[8], d.out_f32, cf, d.ldo_f32, d.B, d.H, d.W, obw, obh, true, ph);
     } else {
       maps[8] = maps[0];
     }
@@ -852,4 +863,21 @@ extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream)
     case EC_MISC: return launch_bn<EC_MISC>(bn, maps, p, s, msa, msb);
     default: return launch_bn<EC_PLAIN>(bn, maps, p, s, msa, msb);
   }
+}
+
+extern "C" int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream) {
+  if (!desc) return RNC_ERR_BAD_POINTER;
+  const rnc_conv_umma_desc& d = *desc;
+  if (d.dil < 0 || d.dil > 8) return RNC_ERR_BAD_SHAPE;
+  if (d.dil <= 1) return conv_umma(d, umma::Phase(), stream);
+  if (d.B <= 0 || d.H <= 0 || d.W <= 0) return RNC_ERR_BAD_SHAPE;
+  // dilated: plain layers at stride 1, one launch per output phase (Phase)
+  const bool plain = d.epilogue == RNC_EPI_LINEAR || d.epilogue == RNC_EPI_RELU || d.epilogue == RNC_EPI_SIGMOID;
+  if (!plain || d.stride > 1 || (d.hin > 0 && d.hin != d.H) || (d.win > 0 && d.win != d.W) || d.stats || d.add ||
+      (d.flags & (RNC_CONV_WINDOW | RNC_CONV_AUX_BLOCKED | RNC_CONV_OUT_BLOCKED)))
+    return RNC_ERR_UNSUPPORTED;
+  for (int ry = 0; ry < d.dil && ry < d.H; ++ry)
+    for (int rx = 0; rx < d.dil && rx < d.W; ++rx)
+      if (int st = conv_umma(d, umma::Phase{d.dil, ry, rx}, stream)) return st;
+  return RNC_OK;
 }

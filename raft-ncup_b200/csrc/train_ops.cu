@@ -183,7 +183,7 @@ constexpr int WT = 64;       // tile side (ci and co)
 constexpr int WK = 16;       // pixels per step
 __global__ void __launch_bounds__(64)
 conv_wgrad_kernel(const float* __restrict__ x, int ldx, int cin, const float* __restrict__ gy, int ldg, int cout, int B, int Hin,
-                  int Win, int Ho, int Wo, int kh, int kw, int stride, int px_per_block, float* __restrict__ part,
+                  int Win, int Ho, int Wo, int kh, int kw, int stride, int dil, int px_per_block, float* __restrict__ part,
                   float* __restrict__ part_bias) {
   float* const gw = part + static_cast<size_t>(blockIdx.z) * kh * kw * cin * cout;
   float* const gb = part_bias ? part_bias + static_cast<size_t>(blockIdx.z) * cout : nullptr;
@@ -193,7 +193,7 @@ conv_wgrad_kernel(const float* __restrict__ x, int ldx, int cin, const float* __
   const int ntc = (cout + WT - 1) / WT;
   const int ci0 = (blockIdx.x / ntc) * WT, co0 = (blockIdx.x % ntc) * WT;
   const int tap = blockIdx.y, ky = tap / kw, kx = tap - ky * kw;
-  const int ph = kh / 2, pw = kw / 2;
+  const int ph = kh / 2 * dil, pw = kw / 2 * dil;
   const long long P = static_cast<long long>(B) * Ho * Wo;
   const long long p0 = static_cast<long long>(blockIdx.z) * px_per_block;
   const long long p1 = p0 + px_per_block < P ? p0 + px_per_block : P;
@@ -218,7 +218,7 @@ conv_wgrad_kernel(const float* __restrict__ x, int ldx, int cin, const float* __
       if (p < p1) {
         const int b = static_cast<int>(p / (Ho * Wo)), r = static_cast<int>(p - static_cast<long long>(b) * Ho * Wo);
         const int yo = r / Wo, xo = r - yo * Wo;
-        const int yi = yo * stride + ky - ph, xi = xo * stride + kx - pw;
+        const int yi = yo * stride + ky * dil - ph, xi = xo * stride + kx * dil - pw;
         if (yi >= 0 && yi < Hin && xi >= 0 && xi < Win && ci0 + 4 * sq < cin)
           xv = __ldg(reinterpret_cast<const float4*>(x + ((static_cast<size_t>(b) * Hin + yi) * Win + xi) * ldx + ci0 + 4 * sq));
         if (co0 + 4 * sq < cout) {
@@ -461,9 +461,8 @@ extern "C" size_t rnc_conv2d_cl_wgrad_workspace_bytes(int cin, int cout, int B, 
   return static_cast<size_t>(ksplit) * (static_cast<size_t>(kh) * kw * cin * cout + cout) * sizeof(float);
 }
 
-extern "C" int rnc_conv2d_cl_wgrad_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin,
-                                       int Win, int kh, int kw, int stride, float* gw, int ldw, float* gb, void* workspace,
-                                       size_t workspace_bytes, void* stream) {
+static int wgrad_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin, int Win, int kh, int kw,
+                     int stride, int dil, float* gw, int ldw, float* gb, void* workspace, size_t workspace_bytes, void* stream) {
   if (!wgrad_shape_ok(cin, cout, B, Hin, Win, kh, kw, stride) || (ldx & 3) || ldx < cin || ldg < cout || ldw < cout)
     return RNC_ERR_BAD_SHAPE;
   if (!x || !gy || !gw || !workspace || !aligned16(x) || !aligned16(gy) || (ldg & 3)) return RNC_ERR_BAD_POINTER;
@@ -477,11 +476,29 @@ extern "C" int rnc_conv2d_cl_wgrad_det(const float* x, int ldx, int cin, const f
   const int tiles = ((cin + train::WT - 1) / train::WT) * ((cout + train::WT - 1) / train::WT);
   dim3 grid(tiles, kh * kw, ksplit);
   train::conv_wgrad_kernel<<<grid, 64, 0, as_stream(stream)>>>(x, ldx, cin, gy, ldg, cout, B, Hin, Win, Ho, Wo, kh, kw, stride,
-                                                                static_cast<int>(per), part,
+                                                                dil, static_cast<int>(per), part,
                                                                 gb ? part + static_cast<size_t>(ksplit) * n : nullptr);
   if (int st = after_launch()) return st;
   const size_t total = n + (gb ? cout : 0);
   const int blocks = static_cast<int>(total / 256 + 1 < 132 * 16 ? total / 256 + 1 : 132 * 16);
   train::wgrad_reduce_kernel<<<blocks, 256, 0, as_stream(stream)>>>(part, ksplit, kh * kw * cin, cout, gw, ldw, gb);
   return after_launch();
+}
+
+extern "C" int rnc_conv2d_cl_wgrad_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin,
+                                       int Win, int kh, int kw, int stride, float* gw, int ldw, float* gb, void* workspace,
+                                       size_t workspace_bytes, void* stream) {
+  return wgrad_det(x, ldx, cin, gy, ldg, cout, B, Hin, Win, kh, kw, stride, 1, gw, ldw, gb, workspace, workspace_bytes, stream);
+}
+
+// Stride 1 with dilation dil: the same tiles, K split and workspace as the undilated layer of that shape.
+extern "C" size_t rnc_conv2d_cl_wgrad_dil_workspace_bytes(int cin, int cout, int B, int Hin, int Win, int kh, int kw, int dil) {
+  return dil >= 1 && dil <= 8 ? rnc_conv2d_cl_wgrad_workspace_bytes(cin, cout, B, Hin, Win, kh, kw, 1) : 0;
+}
+
+extern "C" int rnc_conv2d_cl_wgrad_dil_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin,
+                                           int Win, int kh, int kw, int dil, float* gw, int ldw, float* gb, void* workspace,
+                                           size_t workspace_bytes, void* stream) {
+  if (dil < 1 || dil > 8) return RNC_ERR_BAD_SHAPE;
+  return wgrad_det(x, ldx, cin, gy, ldg, cout, B, Hin, Win, kh, kw, 1, dil, gw, ldw, gb, workspace, workspace_bytes, stream);
 }

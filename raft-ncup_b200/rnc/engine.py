@@ -138,22 +138,53 @@ class PackedUpdateBlock:
             self.m2 = pack_conv(ub.mask[2].weight, ub.mask[2].bias, scale=0.25)   # `.25 * self.mask(net)`, update.py:140
 
 
+def conv_dilation(conv):
+    """The dilation a kernel applies for nn.Conv2d `conv` (square, odd filter): a 1x1 filter reads one pixel whatever it is."""
+    return conv.dilation[0] if conv.kernel_size[0] > 1 else 1
+
+
+def _ceil4(c):
+    return (c + 3) // 4 * 4
+
+
 class PackedSimple:
-    """Kernel-ready weights of the weights net Simple (interp_weights_est.py:10-47): its two 3x3 layers with eval-mode
-    BatchNorm folded in, for the exact fp32 kernels (g0, g1), and the 1x1 confidence head (gout)."""
+    """Kernel-ready weights of the weights net Simple (interp_weights_est.py:10-47) for the exact fp32 kernels: its hidden
+    layers with eval-mode BatchNorm folded in (g[i]; layers[i] = (cout, k, dilation)) and the head `out` + sigmoid: a 1x1 head
+    runs on rnc_conf_head_fwd (gout, its weight rows padded to the input's ceil4 channels), any other on the convolution with a
+    sigmoid epilogue (g_out, head = (k, dilation))."""
 
     def __init__(self, wn):
         # Conv, BatchNorm, ReLU or Conv, ReLU (interp_weights_est.py:26-30)
         convs = [fold_bn(blk[0], blk[1] if len(blk) == 3 else None) for blk in wn.conv]
-        self.c_mid0, self.c_mid1 = convs[0][0].shape[0], convs[1][0].shape[0]
-        self.gout = (pack_thin(wn.out.weight), wn.out.bias.detach().float().contiguous())
-        self.pack_convs(convs)
+        self.layers = [(w.shape[0], blk[0].kernel_size[0], conv_dilation(blk[0])) for (w, _), blk in zip(convs, wn.conv)]
+        self.cin0_pad = _ceil4(wn.in_ch)
+        self.head = (wn.out.kernel_size[0], conv_dilation(wn.out))
+        self.gout = None
+        if self.head[0] == 1:
+            w = pack_thin(wn.out.weight)
+            cin = w.shape[1]
+            self.gout = (w if cin % 4 == 0 else F.pad(w, (0, 0, 0, _ceil4(cin) - cin)), wn.out.bias.detach().float().contiguous())
+        self.pack_convs(convs, wn.out)
 
-    def pack_convs(self, convs):
-        """The two folded 3x3 layers in the exact kernels' format; the tensor-core upsampler pack overrides this."""
-        self.cin0_pad = (convs[0][0].shape[1] + 3) // 4 * 4
-        self.g0 = pack_conv(convs[0][0], convs[0][1], cin_pad=self.cin0_pad)
-        self.g1 = pack_conv(convs[1][0], convs[1][1])
+    def pack_convs(self, convs, out):
+        """The folded layers (and a head that is not 1x1) in the exact kernels' format; the tensor-core upsampler pack overrides
+        this.  Layer i reads ceil4 channels of the previous one (zero beyond its width)."""
+        pads = [self.cin0_pad] + [_ceil4(cout) for cout, _, _ in self.layers]
+        self.g = [pack_conv(w, b, cin_pad=p) for (w, b), p in zip(convs, pads)]
+        self.g_out = pack_conv(out.weight, out.bias, cin_pad=pads[-1]) if self.gout is None else None
+
+    def buffers(self, M, device):
+        """fp32 channel-last outputs of the layers for M pixels (ceil4 channels, zero-filled when that pads), then the head's
+        [M, 4] when it is a convolution."""
+        f = dict(dtype=torch.float32, device=device)
+        bufs = [(torch.empty if _ceil4(c) == c else torch.zeros)(M, _ceil4(c), **f) for c, _, _ in self.layers]
+        return bufs + ([torch.empty(M, 4, **f)] if self.gout is None else [])
+
+    # the shipped two-layer network's names
+    g0 = property(lambda self: self.g[0])
+    g1 = property(lambda self: self.g[1])
+    c_mid0 = property(lambda self: self.layers[0][0])
+    c_mid1 = property(lambda self: self.layers[1][0])
 
 
 class PackedUpsampler(PackedSimple):
@@ -244,9 +275,17 @@ class Workspace:
             M4 = 4 * M
             self.x4 = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
             self.gin = torch.empty(M4, 132, **f)
-            self.g1 = torch.empty(M4, 64, **f)
-            self.g2 = torch.empty(M4, 32, **f)
             self.conf = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
+        self.wnet = {}              # weights-net layer outputs at 1/4 resolution, per pack layout (wnet_buffers)
+
+
+def wnet_buffers(ws, pu):
+    """The weights net's layer outputs for upsampler pack pu in workspace ws, allocated by the first (eager) forward of a shape
+    and reused by graph capture; the shipped network's are [M4, 64] and [M4, 32]."""
+    key = (type(pu).__name__, tuple(pu.layers), pu.gout is None)
+    if key not in ws.wnet:
+        ws.wnet[key] = pu.buffers(4 * ws.B * ws.H8 * ws.W8, ws.conf.device)
+    return ws.wnet[key]
 
 
 class _Timed:
@@ -398,7 +437,7 @@ class Engine:
 
     # ------------------------------------------------------------------ single kernels
     def conv(self, B, H, W, in0, c0, ld0, packed, cout, kh, kw, epi, out=None, ldo=0, in1=None, c1=0, ld1=0,
-             h=None, ldh=0, aux0=None, ldaux=0):
+             h=None, ldh=0, aux0=None, ldaux=0, dil=1):
         d = ConvDesc()
         d.in0, d.c0, d.ld0 = in0, c0, ld0
         d.in1, d.c1, d.ld1 = (in1 or 0), c1, ld1
@@ -408,7 +447,10 @@ class Engine:
         d.aux0, d.ldaux = (aux0 or 0), ldaux
         d.B, d.H, d.W = B, H, W
         d.cout, d.kh, d.kw, d.epilogue = cout, kh, kw, epi
-        native.check(self.L.rnc_conv2d_cl_fwd(C.byref(d), _stream()), "conv2d_cl")
+        if dil > 1:
+            native.check(self.L.rnc_conv2d_cl_dil_fwd(C.byref(d), dil, _stream()), "conv2d_cl_dil")
+        else:
+            native.check(self.L.rnc_conv2d_cl_fwd(C.byref(d), _stream()), "conv2d_cl")
 
     def alloc_fmaps(self, ws, B, D, H, W, levels, device):
         """Allocate the CL feature map / pyramid buffers of ws, which fmap_prepare fills and the tensor-core encoder heads
@@ -527,11 +569,24 @@ class Engine:
         s = _stream()
         native.check(self.L.rnc_ncup_guidance_fwd(_ptr(x_lowres), C.c_void_p(guid_ptr), ldg, 128, B, H8, W8, _ptr(ws.gin),
                                                   132, s), "ncup_guidance")
-        self.conv(B, H4, W4, ws.gin.data_ptr(), pu.cin0_pad, 132, pu.g0, pu.c_mid0, 3, 3, native.EPI_RELU, ws.g1.data_ptr(), 64)
-        self.conv(B, H4, W4, ws.g1.data_ptr(), pu.c_mid0, 64, pu.g1, pu.c_mid1, 3, 3, native.EPI_RELU, ws.g2.data_ptr(), 32)
-        native.check(self.L.rnc_conf_head_fwd(_ptr(ws.g2), pu.c_mid1, 32, _ptr(pu.gout[0]), _ptr(pu.gout[1]), B, H4, W4,
-                                              _ptr(ws.conf), s), "conf_head")
+        self.weights_net(pu, B, H4, W4, ws.gin, wnet_buffers(ws, pu), ws.conf)
         return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)
+
+    def weights_net(self, pk, B, H, W, x, bufs, conf):
+        """Simple.forward (interp_weights_est.py:39-47) on the exact kernels: x fp32 CL [B*H*W, >= pk.cin0_pad] (zero beyond the
+        input channels) -> conf NCHW [B,2,H,W]; bufs = pk.buffers(B*H*W)."""
+        s = _stream()
+        c, ld = pk.cin0_pad, x.shape[1]
+        for (cout, k, dil), wt, y in zip(pk.layers, pk.g, bufs):
+            self.conv(B, H, W, x.data_ptr(), c, ld, wt, cout, k, k, native.EPI_RELU, y.data_ptr(), y.shape[1], dil=dil)
+            x, c, ld = y, y.shape[1], y.shape[1]
+        if pk.gout is not None:
+            native.check(self.L.rnc_conf_head_fwd(_ptr(x), c, ld, _ptr(pk.gout[0]), _ptr(pk.gout[1]), B, H, W, _ptr(conf), s),
+                         "conf_head")
+            return
+        (k, dil), y = pk.head, bufs[-1]
+        self.conv(B, H, W, x.data_ptr(), c, ld, pk.g_out, 2, k, k, native.EPI_SIGMOID, y.data_ptr(), 4, dil=dil)
+        native.check(self.L.rnc_cl_to_nchw(_ptr(y), 4, 0, B, 2, H, W, _ptr(conf), s), "cl_to_nchw(conf)")
 
     def ncup_chain(self, ws, pu, x_lowres, conf, out_scale):
         """Zero-stuffing + NConvUNet + out_scale (upsampler.py:150-177) on x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4]:

@@ -9,7 +9,7 @@ import torch
 import torch.nn.functional as F
 
 from . import native
-from .engine import CORR_CH, HX_LD, Engine, PackedUpsampler, _ptr, _stream, _Timed, pack_thin
+from .engine import CORR_CH, HX_LD, Engine, PackedUpsampler, _ptr, _stream, _Timed, pack_thin, wnet_buffers
 from .native import UmmaConvDesc
 
 CORR_LS = 88           # channels reserved per pyramid level in the resident corr row: 81 taps + 7 zero pads (16-byte groups)
@@ -113,12 +113,38 @@ class PackedUpdateUmma:
             self.m2 = UmmaWeights(ub.mask[2].weight, ub.mask[2].bias, [256], out_scale=0.25)   # update.py:140
 
 
-class PackedUpsamplerUmma(PackedUpsampler):
-    """PackedUpsampler with the weights net's BN-folded 3x3 layers packed for the tensor-core path (u0, u1)."""
+def _ceil32(c):
+    return (c + 31) // 32 * 32
 
-    def pack_convs(self, convs):
-        self.u0 = UmmaWeights(convs[0][0], convs[0][1], [132])
-        self.u1 = UmmaWeights(convs[1][0], convs[1][1], [64])
+
+class PackedUpsamplerUmma(PackedUpsampler):
+    """PackedUpsampler with the weights net's BN-folded layers packed for the tensor-core path (u[i]; u0, u1 for the shipped
+    network).  Layer 0 reads the 132 channels of the guidance staging, layer i > 0 the ceil32 columns of the previous layer's
+    output (the epilogue writes whole 32-channel chunks; zero beyond the width).  A 1x1 head after a hidden layer stays on
+    rnc_conf_head_fwd, which reads that layer's fp32 output; any other head is a tensor-core layer (u_out) with a sigmoid."""
+
+    def pack_convs(self, convs, out):
+        segs = [132] + [_ceil32(cout) for cout, _, _ in self.layers]
+        self.u = [UmmaWeights(w, b, [s]) for (w, b), s in zip(convs, segs)]
+        if convs and self.gout is not None and self.gout[0].shape[1] != _ceil32(self.layers[-1][0]):
+            w = self.gout[0]                          # conf head over the ceil32 fp32 columns of the last layer
+            self.gout = (F.pad(w, (0, 0, 0, _ceil32(self.layers[-1][0]) - w.shape[1])), self.gout[1])
+        if not convs:
+            self.gout = None                          # the staging is split halves: the head is a tensor-core layer
+        self.u_out = UmmaWeights(out.weight, out.bias, [segs[-1]]) if self.gout is None else None
+
+    def buffers(self, M, device):
+        """Split-halves outputs of the layers (ceil32 columns), except an fp32 one for the last layer when the conf head reads
+        it, then the head's fp32 [M, 32] when it is a tensor-core layer."""
+        bufs = [SplitBuf(M, _ceil32(cout), device) for cout, _, _ in self.layers]
+        f = dict(dtype=torch.float32, device=device)
+        if self.gout is not None:
+            bufs[-1] = torch.empty(M, _ceil32(self.layers[-1][0]), **f)
+            return bufs
+        return bufs + [torch.empty(M, 32, **f)]
+
+    u0 = property(lambda self: self.u[0])
+    u1 = property(lambda self: self.u[1])
 
 
 class SplitBuf:
@@ -170,9 +196,8 @@ class UmmaWorkspace:
             M4 = 4 * M
             self.x4 = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
             self.gin = SplitBuf(M4, GIN_LD, device)
-            self.g1 = SplitBuf(M4, 64, device)
-            self.g2 = torch.empty(M4, 32, **f)
             self.conf = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
+        self.wnet = {}
 
 
 class UmmaEngine(Engine):
@@ -201,9 +226,11 @@ class UmmaEngine(Engine):
 
     # ------------------------------------------------------------------ one tensor-core convolution
     def uconv(self, B, H, W, in0, c0, ld0, wt, epi, out_f32=0, ldo_f32=0, out_split=(0, 0), ldo_split=0, in1=(0, 0), c1=0, ld1=0,
-              h=0, ldh=0, aux0=0, ldaux=0, stride=1, hin=0, win=0, res=0, ldres=0, flags=None, stats=0, add=0, ldadd=0, win_pitch=0):
+              h=0, ldh=0, aux0=0, ldaux=0, stride=1, hin=0, win=0, res=0, ldres=0, flags=None, stats=0, add=0, ldadd=0, win_pitch=0,
+              dil=1):
         """One rnc_conv2d_umma_fwd call.  H, W are the OUTPUT dims; for stride 2 pass the input dims as hin, win."""
         d = UmmaConvDesc()
+        d.dil = dil
         d.stride, d.hin, d.win, d.res, d.ldres = stride, hin, win, res, ldres
         d.stats = stats
         d.add, d.ldadd = add, ldadd
@@ -366,8 +393,21 @@ class UmmaEngine(Engine):
         L = self.L
         native.check(L.rnc_ncup_guidance_split_fwd(_ptr(x_lowres), C.c_void_p(guid_ptr), ldg, 128, B, H8, W8, _ptr(ws.gin.hi),
                                                    _ptr(ws.gin.lo), GIN_LD, s), "ncup_guidance_split")
-        self.uconv(B, H4, W4, ws.gin.ptrs(), 132, GIN_LD, pu.u0, native.EPI_RELU, out_split=ws.g1.ptrs(), ldo_split=64)
-        self.uconv(B, H4, W4, ws.g1.ptrs(), 64, 64, pu.u1, native.EPI_RELU, out_f32=ws.g2.data_ptr(), ldo_f32=32)
-        native.check(L.rnc_conf_head_fwd(_ptr(ws.g2), pu.c_mid1, 32, _ptr(pu.gout[0]), _ptr(pu.gout[1]), B, H4, W4, _ptr(ws.conf), s),
-                     "conf_head")
+        # Simple.forward (interp_weights_est.py:39-47)
+        x, c, ld = ws.gin.ptrs(), 132, GIN_LD
+        bufs = wnet_buffers(ws, pu)
+        for (cout, k, dil), wt, y in zip(pu.layers, pu.u, bufs):
+            if isinstance(y, SplitBuf):
+                self.uconv(B, H4, W4, x, c, ld, wt, native.EPI_RELU, out_split=y.ptrs(), ldo_split=y.ld, dil=dil)
+                x, c, ld = y.ptrs(), y.ld, y.ld
+            else:
+                self.uconv(B, H4, W4, x, c, ld, wt, native.EPI_RELU, out_f32=y.data_ptr(), ldo_f32=y.shape[1], dil=dil)
+        if pu.gout is not None:
+            y = bufs[-1]
+            native.check(L.rnc_conf_head_fwd(_ptr(y), y.shape[1], y.shape[1], _ptr(pu.gout[0]), _ptr(pu.gout[1]), B, H4, W4,
+                                             _ptr(ws.conf), s), "conf_head")
+        else:
+            (k, dil), y = pu.head, bufs[-1]
+            self.uconv(B, H4, W4, x, c, ld, pu.u_out, native.EPI_SIGMOID, out_f32=y.data_ptr(), ldo_f32=32, dil=dil)
+            native.check(L.rnc_cl_to_nchw(_ptr(y), 32, 0, B, 2, H4, W4, _ptr(ws.conf), s), "cl_to_nchw(conf)")
         return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)

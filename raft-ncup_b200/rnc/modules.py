@@ -12,6 +12,7 @@ import math
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+from torch.nn.modules.utils import _pair
 
 from . import native
 from .nconv_unet import PackedUNet, is_fused, nconv_fwd
@@ -392,22 +393,38 @@ class NConvUNet(nn.Module):
 
 
 class Simple(nn.Module):
-    """core/interp_weights_est.py:10-47: forward(x [B,130,h,w]) -> final_act(out(conv[1](conv[0](x))))."""
+    """core/interp_weights_est.py:10-47: forward(x [B,in_ch,h,w]) -> final_act(out(conv[n-1](...conv[0](x)))), for 0 to 6
+    hidden layers of widths 1 to 256 and, in every layer, odd filter sizes 1 to 7 and dilations 1 to 4 (None: 1), with the
+    reference's module structure, padding, state_dict keys and RNG draws."""
 
     def __init__(self, num_ch, out_ch, filter_sz, dilation=None, final_act=torch.sigmoid, use_bn=False):
         super().__init__()
         self.__name__ = "Simple"
-        if list(filter_sz) != [3, 3, 1] or (dilation is not None and any(d != 1 for d in dilation)) or len(num_ch) != 3:
-            raise NotImplementedError("weights net kernels are built for filter_sz [3,3,1], dilation 1 (SURVEY.md §5)")
-        self.in_ch, self.num_layers = num_ch[0], len(num_ch) - 1
+        num_ch, filter_sz = list(num_ch), list(filter_sz)
+        dilation = [1] * len(num_ch) if dilation is None else list(dilation)
+        if len(filter_sz) != len(num_ch) or len(dilation) != len(num_ch):
+            raise ValueError(f"Simple: num_ch {num_ch}, filter_sz {filter_sz} and dilation {dilation} must have one entry per layer")
+        if not 1 <= len(num_ch) <= 7 or any(not isinstance(c, int) or not 1 <= c <= 256 for c in num_ch[1:]):
+            raise NotImplementedError(f"Simple num_ch={num_ch[1:]}: the kernels take 0 to 6 hidden layers of widths 1 to 256")
+        if any(not isinstance(k, int) or k < 1 or k > 7 or k % 2 == 0 for k in filter_sz):
+            raise NotImplementedError(f"Simple filter_sz={filter_sz}: the kernels take odd square filters up to 7")
+        if any(not isinstance(d, int) or not 1 <= d <= 4 for d in dilation):
+            raise NotImplementedError(f"Simple dilation={dilation}: the kernels take dilations 1 to 4")
+        self.in_ch = num_ch[0]  # Number of Input channels is added at the beginning of num_ch
+        self.num_layers = len(num_ch) - 1
+
+        def conv(i, cin, cout):       # interp_weights_est.py:25,36
+            return nn.Conv2d(cin, cout, filter_sz[i], padding=_pair(int(filter_sz[i] // 2 + ((filter_sz[i] - 1) * (dilation[i] - 1)) / 2)),
+                             dilation=dilation[i], stride=1)
+
         self.conv = nn.ModuleList()
         for i in range(self.num_layers):
-            layers = [nn.Conv2d(num_ch[i], num_ch[i + 1], 3, padding=1)]
+            layers = [conv(i, num_ch[i], num_ch[i + 1])]
             if use_bn:
                 layers.append(nn.BatchNorm2d(num_ch[i + 1]))
             layers.append(nn.ReLU(inplace=True))
             self.conv.append(nn.Sequential(*layers))
-        self.out = nn.Conv2d(num_ch[-1], out_ch, 1)
+        self.out = conv(-1, num_ch[-1], out_ch)
         self.final_act = final_act
 
     def forward(self, x):
@@ -424,18 +441,12 @@ class Simple(nn.Module):
         with _Seam(x) as eng:
             pk = eng._packed_for("simple", self, PackedSimple)
             cpad = pk.cin0_pad
-            s = _stream()
             M = B * h * w
             xin = torch.zeros(M, cpad, dtype=torch.float32, device=x.device) if cpad != Cin else torch.empty(M, cpad, dtype=torch.float32, device=x.device)
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, Cin, h, w, _ptr(xin), cpad, 0, s), "nchw_to_cl")
-            c0, c1 = pk.c_mid0, pk.c_mid1
-            g1 = torch.empty(M, (c0 + 3) // 4 * 4, dtype=torch.float32, device=x.device)
-            g2 = torch.empty(M, (c1 + 3) // 4 * 4, dtype=torch.float32, device=x.device)
-            eng.conv(B, h, w, xin.data_ptr(), cpad, cpad, pk.g0, c0, 3, 3, native.EPI_RELU, g1.data_ptr(), g1.shape[1])
-            eng.conv(B, h, w, g1.data_ptr(), c0, g1.shape[1], pk.g1, c1, 3, 3, native.EPI_RELU, g2.data_ptr(), g2.shape[1])
+            native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, Cin, h, w, _ptr(xin), cpad, 0, _stream()),
+                         "nchw_to_cl")
             conf = torch.empty(B, 2, h, w, dtype=torch.float32, device=x.device)
-            native.check(eng.L.rnc_conf_head_fwd(_ptr(g2), c1, g2.shape[1], _ptr(pk.gout[0]), _ptr(pk.gout[1]), B, h, w,
-                                                 _ptr(conf), s), "conf_head")
+            eng.weights_net(pk, B, h, w, xin, pk.buffers(M, x.device), conf)
             return conf
 
 

@@ -10,7 +10,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RNC_LIB") or os.path.join(_HERE, "librnc.so")      # RNC_LIB: developer override (variant builds)
-ABI_VERSION = 13
+ABI_VERSION = 14
 CONV_NO_HALO, CONV_BASE_OFFSET, CONV_SPLIT_N, CONV_NO_PAIR, CONV_AUX_BLOCKED, CONV_OUT_BLOCKED, CONV_TF32, CONV_WINDOW = 1, 2, 4, 8, 16, 32, 64, 128   # rnc_conv_umma_desc.flags
 
 (EPI_LINEAR, EPI_RELU, EPI_SIGMOID, EPI_GRU_ZR, EPI_GRU_Q, EPI_RELU_FLOW, EPI_RELU_ADD_RELU, EPI_TANH_RELU,
@@ -53,7 +53,8 @@ class UmmaConvDesc(C.Structure):
                 ("B", _i), ("H", _i), ("W", _i),
                 ("cout", _i), ("kh", _i), ("kw", _i), ("epilogue", _i),
                 ("stride", _i), ("hin", _i), ("win", _i),
-                ("res", _vp), ("ldres", _i), ("flags", _i), ("stats", _vp), ("add", _vp), ("ldadd", _i), ("win_pitch", _i)]
+                ("res", _vp), ("ldres", _i), ("flags", _i), ("stats", _vp), ("add", _vp), ("ldadd", _i), ("win_pitch", _i),
+                ("dil", _i)]
 
 
 # name -> (restype, argtypes); every symbol include/rnc.h declares
@@ -72,6 +73,7 @@ SIGNATURES = {
     "rnc_corr_lookup_umma_fwd": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _i, _i, _vp, C.c_size_t, _vp]),
     "rnc_f32_to_f16": (_i, [_vp, _vp, C.c_size_t, _vp]),
     "rnc_conv2d_cl_fwd": (_i, [C.POINTER(ConvDesc), _vp]),
+    "rnc_conv2d_cl_dil_fwd": (_i, [C.POINTER(ConvDesc), _i, _vp]),
     "rnc_conv_umma_tiles": (C.c_longlong, [_i, _i, _i, _i, _i, _i, _i]),
     "rnc_conv2d_umma_fwd": (_i, [C.POINTER(UmmaConvDesc), _vp]),
     "rnc_f32_to_split": (_i, [_vp, _i, _i, C.c_longlong, _vp, _vp, _i, _i, _vp]),
@@ -112,6 +114,8 @@ SIGNATURES = {
     "rnc_corr_lookup_bwd_det": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
     "rnc_conv2d_cl_wgrad_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i, _i, _i, _i]),
     "rnc_conv2d_cl_wgrad_det": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_conv2d_cl_wgrad_dil_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i, _i, _i, _i]),
+    "rnc_conv2d_cl_wgrad_dil_det": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, _i, _i, _i, _i, _vp, _i, _vp, _vp, C.c_size_t, _vp]),
     "rnc_nconv2d_bwd_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i, _i, _i]),
     "rnc_nconv2d_bwd": (_i, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _i, _i,
                              _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),

@@ -133,7 +133,7 @@ def _padded_bias(packed_bias, bias):
     return b
 
 
-def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16"):
+def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16", dil=1):
     """Same contract as _conv_launch on the tensor-core path: x fp32 CL -> hi/lo operand planes (halves or TF32 words) ->
     rnc_conv2d_umma_fwd with an fp32 channel-last output; stride 2 is native (TMA element strides), no subsampling pass."""
     B, H, W, Cx = x.shape
@@ -150,45 +150,46 @@ def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16"):
         wt = copy.copy(wt)
         wt.bias = _padded_bias(wt.bias, bias)
     eng.uconv(B, Ho, Wo, (hi.data_ptr(), lo.data_ptr()), Cx, Cx, wt, native.EPI_LINEAR, out_f32=out.data_ptr(), ldo_f32=ldo,
-              stride=stride, hin=H, win=W, flags=eng.conv_flags | (native.CONV_TF32 if fmt == "tf32" else 0))
+              stride=stride, hin=H, win=W, flags=eng.conv_flags | (native.CONV_TF32 if fmt == "tf32" else 0), dil=dil)
     return out
 
 
-def _conv_launch(eng, x, packed, cout, kh, kw, bias=None):
-    """x CL [B,H,W,C] contiguous (C % 4 == 0) -> CL [B,H,W,ceil4(cout)] (pad channels zero), stride 1, zero padding k/2."""
+def _conv_launch(eng, x, packed, cout, kh, kw, bias=None, dil=1):
+    """x CL [B,H,W,C] contiguous (C % 4 == 0) -> CL [B,H,W,ceil4(cout)] (pad channels zero), stride 1, dilation dil, zero
+    padding (k/2)*dil."""
     B, H, W, Cx = x.shape
     ldo = _ceil4(cout)
     alloc = torch.empty if ldo == cout else torch.zeros          # pad channels must read as zero downstream
     out = alloc(B, H, W, ldo, dtype=torch.float32, device=x.device)
     if bias is not None:
         packed = (packed[0], _padded_bias(packed[1], bias))
-    eng.conv(B, H, W, x.data_ptr(), Cx, Cx, packed, cout, kh, kw, native.EPI_LINEAR, out.data_ptr(), ldo)
+    eng.conv(B, H, W, x.data_ptr(), Cx, Cx, packed, cout, kh, kw, native.EPI_LINEAR, out.data_ptr(), ldo, dil=dil)
     return out
 
 
 class ConvCL(torch.autograd.Function):
-    """y = conv2d(x, weight, bias, stride, padding = k // 2) on channel-last tensors.
+    """y = conv2d(x, weight, bias, stride, padding = (k // 2) * dil, dilation = dil) on channel-last tensors (dil > 1: stride 1).
     x [B,H,W,Cx] (Cx = ceil4(Cin); channels beyond Cin must be zero), weight [Cout,Cin,kh,kw] -> y [B,Ho,Wo,ceil4(Cout)]."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, stride):
+    def forward(ctx, x, weight, bias, stride, dil=1):
         x = x.contiguous()
         eng = engine_for(x.device)
         cout, cin, kh, kw = weight.shape
         Cx = x.shape[-1]
         if Cx % 4 or Cx < cin:
             raise ValueError("ConvCL: input must be channel-last with ceil4(Cin) channels")
-        if stride not in (1, 2):
-            raise NotImplementedError("stride 1 or 2")
+        if stride not in (1, 2) or (dil > 1 and stride != 1):
+            raise NotImplementedError("stride 1 or 2; dilated layers at stride 1")
         fmt = _umma_ok(eng, Cx, cout)
         if fmt:
-            y = _conv_launch_umma(eng, x, _packed(weight, "fwd", Cx, fmt), cout, stride, bias, fmt)
+            y = _conv_launch_umma(eng, x, _packed(weight, "fwd", Cx, fmt), cout, stride, bias, fmt, dil)
         else:
-            y = _conv_launch(eng, x, _packed(weight, "fwd", Cx), cout, kh, kw, bias)
+            y = _conv_launch(eng, x, _packed(weight, "fwd", Cx), cout, kh, kw, bias, dil)
             if stride == 2:
                 y = y[:, ::2, ::2].contiguous()      # same padding: out(y, x) of the strided conv = full(2y, 2x)
         ctx.save_for_backward(x, weight)
-        ctx.stride, ctx.has_bias = stride, bias is not None
+        ctx.stride, ctx.dil, ctx.has_bias = stride, dil, bias is not None
         return y
 
     @staticmethod
@@ -200,44 +201,54 @@ class ConvCL(torch.autograd.Function):
         gy = gy.contiguous()
         ldg = gy.shape[-1]
         gx = gw = gb = None
+        dil = ctx.dil
         with torch.cuda.device(x.device):
             if ctx.needs_input_grad[0]:
                 g_full = gy
                 if ctx.stride == 2:
                     g_full = torch.zeros(B, H, W, ldg, dtype=torch.float32, device=x.device)
                     g_full[:, ::2, ::2] = gy
+                # the same (dilated) convolution with the flipped, transposed weights: its padding (k // 2) * dil is symmetric
                 fmt = _umma_ok(eng, ldg, cin, dgrad=True)
                 if fmt:
-                    gx = _conv_launch_umma(eng, g_full, _packed(weight, "dgrad", ldg, fmt), cin, fmt=fmt)
+                    gx = _conv_launch_umma(eng, g_full, _packed(weight, "dgrad", ldg, fmt), cin, fmt=fmt, dil=dil)
                 else:
-                    gx = _conv_launch(eng, g_full, _packed(weight, "dgrad", ldg), cin, kh, kw)
+                    gx = _conv_launch(eng, g_full, _packed(weight, "dgrad", ldg), cin, kh, kw, dil=dil)
                 if gx.shape[-1] != Cx:               # Cx > ceil4(cin) never happens; equal by construction
                     gx = F.pad(gx, (0, Cx - gx.shape[-1]))
             if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):
-                gwp, gbp = _wgrad(eng, x, gy, cout, kh, kw, ctx.stride, ctx.has_bias)
+                gwp, gbp = _wgrad(eng, x, gy, cout, kh, kw, ctx.stride, ctx.has_bias, dil)
                 gw = gwp.view(kh, kw, Cx, cout)[:, :, :cin].permute(3, 2, 0, 1).contiguous()
                 gb = gbp
-        return gx, gw, gb, None
+        return gx, gw, gb, None, None
 
 
-def _wgrad(eng, x, gy, cout, kh, kw, stride, has_bias):
-    """Weight / bias gradient of ConvCL: [kh*kw, Cx, cout], [cout] (or None).  rnc_conv2d_cl_wgrad_det sums the K-split
-    partials in a fixed order (in either mode: it is no slower than adding them with atomics was) and writes its outputs."""
+def _wgrad(eng, x, gy, cout, kh, kw, stride, has_bias, dil=1):
+    """Weight / bias gradient of ConvCL: [kh*kw, Cx, cout], [cout] (or None).  rnc_conv2d_cl_wgrad_det (rnc_conv2d_cl_wgrad_dil_det
+    for a dilated layer) sums the K-split partials in a fixed order (in either mode: it is no slower than adding them with atomics
+    was) and writes its outputs."""
     B, H, W, Cx = x.shape
     gwp = torch.empty(kh * kw, Cx, cout, dtype=torch.float32, device=x.device)
     gbp = torch.empty(cout, dtype=torch.float32, device=x.device) if has_bias else None
-    nbytes = eng.L.rnc_conv2d_cl_wgrad_workspace_bytes(Cx, cout, B, H, W, kh, kw, stride)
+    L = eng.L
+    nbytes_fn, wgrad_fn, arg = ((L.rnc_conv2d_cl_wgrad_dil_workspace_bytes, L.rnc_conv2d_cl_wgrad_dil_det, dil) if dil > 1 else
+                                (L.rnc_conv2d_cl_wgrad_workspace_bytes, L.rnc_conv2d_cl_wgrad_det, stride))
+    nbytes = nbytes_fn(Cx, cout, B, H, W, kh, kw, arg)
     ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=x.device)
-    native.check(eng.L.rnc_conv2d_cl_wgrad_det(_ptr(x), Cx, Cx, _ptr(gy), gy.shape[-1], cout, B, H, W, kh, kw, stride, _ptr(gwp),
-                                               cout, _ptr(gbp), _ptr(ws), ws.numel() * 4, _stream()), "conv2d_cl_wgrad_det")
+    native.check(wgrad_fn(_ptr(x), Cx, Cx, _ptr(gy), gy.shape[-1], cout, B, H, W, kh, kw, arg, _ptr(gwp), cout, _ptr(gbp), _ptr(ws),
+                          ws.numel() * 4, _stream()), "conv2d_cl_wgrad_det")
     return gwp, gbp
 
 
 def conv_cl(x, conv, stride=None):
-    """nn.Conv2d `conv` (zero padding k // 2, as every convolution of the reference) on a channel-last tensor."""
+    """nn.Conv2d `conv` on a channel-last tensor: zero padding (k // 2) * dilation, as every convolution of the reference (the
+    weights net's dilated ones included, interp_weights_est.py:25,36)."""
     s = conv.stride[0] if stride is None else stride
-    y = ConvCL.apply(x, conv.weight, conv.bias, s)
-    return y
+    kh, kw = conv.kernel_size
+    dil = conv.dilation[0] if max(kh, kw) > 1 else 1
+    if conv.dilation[0] != conv.dilation[1] or tuple(conv.padding) != ((kh // 2) * dil, (kw // 2) * dil):
+        raise NotImplementedError(f"conv_cl: padding {conv.padding}, dilation {conv.dilation}: the kernels pad (k // 2) * dilation")
+    return ConvCL.apply(x, conv.weight, conv.bias, s, dil)
 
 
 def to_cl(x, pad_to=None):
