@@ -114,7 +114,8 @@ def corr_lookup_direct(fmap1, fmap2, coords, num_levels=4, radius=4):
     b, d, h, w = fmap1.shape
     side = 2 * radius + 1
     f1 = fmap1.permute(0, 2, 3, 1).reshape(b, h * w, d)
-    out = torch.zeros(b, h * w, num_levels * side * side)
+    dev = fmap1.device               # (device- and dtype-agnostic: the GPU tests evaluate it in fp64 on the device)
+    out = torch.zeros(b, h * w, num_levels * side * side, dtype=fmap1.dtype, device=dev)
     f2 = fmap2
     for lvl in range(num_levels):
         hl, wl = f2.shape[-2:]
@@ -125,7 +126,7 @@ def corr_lookup_direct(fmap1, fmap2, coords, num_levels=4, radius=4):
         y0 = torch.floor(cy)
         ax = (cx - x0)[..., None, None]
         ay = (cy - y0)[..., None, None]
-        g = torch.zeros(b, h * w, side + 1, side + 1)  # G[a][c]: a -> x lattice, c -> y lattice
+        g = torch.zeros(b, h * w, side + 1, side + 1, dtype=fmap1.dtype, device=dev)  # G[a][c]: a -> x lattice, c -> y lattice
         for a in range(side + 1):
             for c in range(side + 1):
                 xi = x0 - radius + a
@@ -133,7 +134,7 @@ def corr_lookup_direct(fmap1, fmap2, coords, num_levels=4, radius=4):
                 ok = (xi >= 0) & (xi <= wl - 1) & (yi >= 0) & (yi <= hl - 1)
                 xi = xi.clamp(0, wl - 1).long()
                 yi = yi.clamp(0, hl - 1).long()
-                bi = torch.arange(b)[:, None].expand(b, h * w)
+                bi = torch.arange(b, device=dev)[:, None].expand(b, h * w)
                 v = f2l[bi, yi, xi]  # [b,P,d]
                 g[:, :, a, c] = (v * f1).sum(-1) * ok.float() / math.sqrt(float(d))
         blend = ((1 - ax) * (1 - ay) * g[:, :, :-1, :-1] + ax * (1 - ay) * g[:, :, 1:, :-1]
