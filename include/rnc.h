@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 14) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 15) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -450,6 +450,47 @@ size_t rnc_conv2d_cl_wgrad_dil_workspace_bytes(int cin, int cout, int B, int Hin
 int rnc_conv2d_cl_wgrad_dil_det(const float* x, int ldx, int cin, const float* gy, int ldg, int cout, int B, int Hin, int Win,
                                 int kh, int kw, int dil, float* gw, int ldw, float* gb, void* workspace, size_t workspace_bytes,
                                 void* stream);
+
+/* ------------------------------------------------------------------------------------------------
+ * T1  FlowAugmentor / SparseFlowAugmentor.__call__ (core/utils/augmentor.py) and the tensor conversion after it in
+ * FlowDataset.__getitem__ (core/datasets.py:75-90), for a batch of samples of any source sizes.  rnc/augment.py draws
+ * every random parameter on the host in the reference's order; these kernels apply them with Pillow's and cv2's
+ * rounding, so that the outputs equal the reference's for the same draws (images and valid bit for bit).
+ *
+ * One descriptor per sample.  Offsets are in bytes into `src`:
+ *   img1, img2 : uint8 [3][H][W] planar RGB       flow : fp32 [2][H][W]       valid : fp32 [H][W] (sparse only)
+ * rh, rw       : size after the resize (cv2's rint(W * fx), rint(H * fy)); H, W when resized == 0
+ * y0, x0       : crop origin in the resized, flipped image; 0 <= y0 <= rh - crop_h, 0 <= x0 <= rw - crop_w
+ * asym         : 1 = img1 is jittered with perm[0]/factor[0]/hue[0] and img2 with the [1] entries; 0 = both with [0],
+ *                the contrast mean taken over the stacked pair
+ * perm         : ColorJitter's op order (torch.randperm(4)): 0 brightness, 1 contrast, 2 saturation, 3 hue
+ * factor       : brightness, contrast, saturation factors;  hue: uint8 added to Pillow's H band (np.int32(h * 255))
+ * erase        : n_erase rectangles {x0, y0, dx, dy} of img2 in source pixels, painted with its jittered mean colour
+ * fx, fy       : the resize factors;  ifx, ify: 1.0 / fx, 1.0 / fy (cv2's source-coordinate step)
+ */
+typedef struct {
+  long long img1, img2, flow, valid;
+  int H, W, rh, rw;
+  int resized, hflip, vflip, y0, x0, asym;
+  int perm[2][4];
+  float factor[2][3];
+  int hue[2];
+  int n_erase;
+  int erase[2][4];
+  int pad;
+  double fx, fy, ifx, ify;
+} rnc_aug_desc;
+
+/* Workspace of rnc_augment: per-sample integer statistics, plus the crop-sized winner map when sparse (0 for a bad shape). */
+size_t rnc_augment_workspace_bytes(int B, int crop_h, int crop_w, int sparse);
+/* desc_host and desc_dev hold the same B descriptors; the host copy is checked (RNC_ERR_BAD_SHAPE for sizes, crops, offsets
+ * or draws out of range, RNC_ERR_BAD_POINTER for null or misaligned pointers), the device copy is read by the kernels.
+ * sparse = 0: FlowAugmentor semantics (valid = |u| < 1000 & |v| < 1000); 1: SparseFlowAugmentor (no vflip, no asym).
+ * Outputs: img1, img2 fp32 [B][3][crop_h][crop_w] with integer values, flow fp32 [B][2][crop_h][crop_w], valid fp32
+ * [B][crop_h][crop_w].  workspace: 16-byte aligned, zeroed by the call.  Integer reductions only: outputs repeat bit for bit. */
+int rnc_augment(const rnc_aug_desc* desc_host, const rnc_aug_desc* desc_dev, int B, const void* src, size_t src_bytes,
+                int crop_h, int crop_w, int sparse, float* img1, float* img2, float* flow, float* valid, void* workspace,
+                size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

@@ -10,7 +10,7 @@ import threading
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RNC_LIB") or os.path.join(_HERE, "librnc.so")      # RNC_LIB: developer override (variant builds)
-ABI_VERSION = 14
+ABI_VERSION = 15
 CONV_NO_HALO, CONV_BASE_OFFSET, CONV_SPLIT_N, CONV_NO_PAIR, CONV_AUX_BLOCKED, CONV_OUT_BLOCKED, CONV_TF32, CONV_WINDOW = 1, 2, 4, 8, 16, 32, 64, 128   # rnc_conv_umma_desc.flags
 
 (EPI_LINEAR, EPI_RELU, EPI_SIGMOID, EPI_GRU_ZR, EPI_GRU_Q, EPI_RELU_FLOW, EPI_RELU_ADD_RELU, EPI_TANH_RELU,
@@ -55,6 +55,16 @@ class UmmaConvDesc(C.Structure):
                 ("stride", _i), ("hin", _i), ("win", _i),
                 ("res", _vp), ("ldres", _i), ("flags", _i), ("stats", _vp), ("add", _vp), ("ldadd", _i), ("win_pitch", _i),
                 ("dil", _i)]
+
+
+class AugDesc(C.Structure):
+    """Mirror of rnc_aug_desc (include/rnc.h): one augmented sample's sizes, byte offsets and drawn parameters."""
+    _fields_ = [("img1", C.c_longlong), ("img2", C.c_longlong), ("flow", C.c_longlong), ("valid", C.c_longlong),
+                ("H", _i), ("W", _i), ("rh", _i), ("rw", _i),
+                ("resized", _i), ("hflip", _i), ("vflip", _i), ("y0", _i), ("x0", _i), ("asym", _i),
+                ("perm", (_i * 4) * 2), ("factor", (_f * 3) * 2), ("hue", _i * 2),
+                ("n_erase", _i), ("erase", (_i * 4) * 2), ("pad", _i),
+                ("fx", C.c_double), ("fy", C.c_double), ("ifx", C.c_double), ("ify", C.c_double)]
 
 
 # name -> (restype, argtypes); every symbol include/rnc.h declares
@@ -121,6 +131,8 @@ SIGNATURES = {
                              _vp, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
     "rnc_nconv_pool2_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "rnc_nconv_pool2_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
+    "rnc_augment_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
+    "rnc_augment": (_i, [_vp, _vp, _i, _vp, C.c_size_t, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
 }
 
 _lib = None
