@@ -65,15 +65,17 @@ def corr_pyramid(fmap1, fmap2, num_levels=4):
     return pyr
 
 
-def _bilinear_zero(img, x, y):
+def _bilinear_zero(img, x, y, round_trip=True):
     """core/utils/utils.py:59-73 (grid_sample, bilinear, align_corners=True, zeros padding) written
     out by hand.  img [N,1,H,W]; x,y [N,K] pixel coordinates.  Includes the reference's
-    pixel -> [-1,1] -> pixel round trip so that fp32 rounding of the sample position matches."""
+    pixel -> [-1,1] -> pixel round trip so that fp32 rounding of the sample position matches
+    (round_trip=False: sample at x, y themselves, as the kernels do)."""
     n, _, h, w = img.shape
-    xn = 2 * x / (w - 1) - 1
-    yn = 2 * y / (h - 1) - 1
-    x = ((xn + 1) / 2) * (w - 1)
-    y = ((yn + 1) / 2) * (h - 1)
+    if round_trip:
+        xn = 2 * x / (w - 1) - 1
+        yn = 2 * y / (h - 1) - 1
+        x = ((xn + 1) / 2) * (w - 1)
+        y = ((yn + 1) / 2) * (h - 1)
     x0 = torch.floor(x)
     y0 = torch.floor(y)
     ax = x - x0
@@ -90,9 +92,12 @@ def _bilinear_zero(img, x, y):
     return out
 
 
-def corr_lookup(pyr, coords, radius=4):
+def corr_lookup(pyr, coords, radius=4, dtype=torch.float32, round_trip=True):
     """core/corr.py:23-44 — channel k = l*(2r+1)^2 + i*(2r+1) + j samples level l at
-    x = cx/2^l + (i-r), y = cy/2^l + (j-r): the SLOW window index offsets x (corr.py:31-37)."""
+    x = cx/2^l + (i-r), y = cy/2^l + (j-r): the SLOW window index offsets x (corr.py:31-37).
+    dtype: of the result (torch.float64 keeps an fp64 evaluation in fp64).  round_trip: see _bilinear_zero; an fp64
+    reference of the kernels leaves it out, or a window edge on an exact integer position gets a weight of ~1e-14
+    outside the image where the kernels (and exact arithmetic) give 0."""
     b, _, h, w = coords.shape
     n = b * h * w
     side = 2 * radius + 1
@@ -104,8 +109,8 @@ def corr_lookup(pyr, coords, radius=4):
     for lvl, vol in enumerate(pyr):
         cx = c[:, 0:1] / 2 ** lvl + off_i
         cy = c[:, 1:2] / 2 ** lvl + off_j
-        outs.append(_bilinear_zero(vol, cx, cy).view(b, h, w, side * side))
-    return torch.cat(outs, dim=-1).permute(0, 3, 1, 2).contiguous().float()
+        outs.append(_bilinear_zero(vol, cx, cy, round_trip).view(b, h, w, side * side))
+    return torch.cat(outs, dim=-1).permute(0, 3, 1, 2).contiguous().to(dtype)
 
 
 def corr_lookup_direct(fmap1, fmap2, coords, num_levels=4, radius=4):
