@@ -77,8 +77,10 @@ class EncoderBuffers:
         self.mr = torch.empty(N * 128 * 2, **f)
         self.parts = None                                  # rnc_instnorm_stats_det's partials, sized on first use
 
-    def det_workspace(self, L, N):
+    def det_workspace(self, L):
         if self.parts is None:
+            # sized for all N images of the buffers: a pass may run on fewer (cnet, sequence steps), but the first not always
+            N = self.key[1]
             nbytes = max(L.rnc_instnorm_stats_det_workspace_bytes(N, h * w, c) for (h, w, c) in self.dims)
             self.parts = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=self.stats.device)
         return self.parts
@@ -107,7 +109,7 @@ class EncoderRunner:
         if fused_stats:
             native.check(self.L.rnc_instnorm_finalize(_ptr(bufs.stats), N, P, Cc, EPS, _ptr(bufs.mr), s), "instnorm_finalize")
         else:
-            ws = bufs.det_workspace(self.L, N)
+            ws = bufs.det_workspace(self.L)
             native.check(self.L.rnc_instnorm_stats_det(_ptr(x32), N, P, Cc, EPS, _ptr(ws), ws.numel() * 8, _ptr(bufs.mr), s),
                          "instnorm_stats_det")
         native.check(self.L.rnc_instnorm_apply(_ptr(x32), _ptr(bufs.mr), _ptr(res), N, P, Cc, mode, _ptr(out32),
@@ -189,9 +191,55 @@ class EncoderRunner:
         off = B * P * 128 * 2                                  # second half of the batch inside the split planes (bytes)
         eng.uconv(B, h8, w8, (xs.hi.data_ptr() + off, xs.lo.data_ptr() + off), 128, 128, pf.head, E.EPI_LINEAR,
                   out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
-        # ---- cnet on frame 1
+        self._context(pc, bufs, ws, image1, h8, w8)
+        return h8, w8
+
+    def _context(self, pc, bufs, ws, image1, h8, w8):
+        """cnet on frame 1 -> ws.h, ws.hx[:, :256]."""
+        B, _, Hin, Win = image1.shape
         self._trunk(pc, bufs, image1.contiguous(), B, Hin, Win)
         ws.gru_const_valid = False                              # inp changes: the GRU's hoisted share must be recomputed
-        eng.uconv(B, h8, w8, bufs.XS[2].ptrs(), 128, 128, pc.head, E.EPI_TANH_RELU, out_f32=ws.h.data_ptr(), ldo_f32=128,
-                  out_split=ws.hx.ptrs(), ldo_split=HX_LD)
+        self.eng.uconv(B, h8, w8, bufs.XS[2].ptrs(), 128, 128, pc.head, native.EPI_TANH_RELU, out_f32=ws.h.data_ptr(),
+                       ldo_f32=128, out_split=ws.hx.ptrs(), ldo_split=HX_LD)
+
+    def run_step(self, model, ws, image1, image2, carry, restart):
+        """One step of sequence inference (rnc.model.SequenceStage): like run, but frame 1 of the `carry` slots is the last
+        step's frame 2, whose features are still level 0 of ws.f2_pyr (and of ws.f2h, the tensor-core lookup's halves): they
+        are copied into those slots' rows of ws.f1_cl / ws.f1h, then fnet runs on cat(image2 of every slot, image1 of the
+        `restart` slots) and its head writes level 0 of f2_pyr for all slots and the f1_cl rows of the restarted ones.  Slots
+        in neither list keep their f1 rows (an idle slot recomputes its last pair).  The caller converts only the restarted
+        slots' f1 rows to halves (finish_fmaps(ws, f1_slots=restart))."""
+        eng, E = self.eng, native
+        B, _, Hin, Win = image1.shape
+        dev = image1.device
+        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
+        bufs = self.buffers(dev, 2 * B, Hin, Win)         # the size of an ordinary forward's: no reallocation as R varies
+        h8, w8, _ = bufs.dims[2]
+        n = h8 * w8 * 256                                   # elements of one slot's feature map
+        eng.alloc_fmaps(ws, B, 256, h8, w8, 4, dev)
+        f1, halves = ws.f1_cl.view(-1), eng.lookup_mode == "umma"
+        for j0, k in _runs(carry):                          # before the fnet head overwrites level 0
+            f1[j0 * n:(j0 + k) * n].copy_(ws.f2_pyr[j0 * n:(j0 + k) * n])
+            if halves:
+                ws.f1h[j0 * n:(j0 + k) * n].copy_(ws.f2h[j0 * n:(j0 + k) * n])
+        both = torch.cat([image2] + [image1[j:j + 1] for j in restart]) if restart else image2
+        self._trunk(pf, bufs, both.contiguous(), B + len(restart), Hin, Win)
+        xs = bufs.XS[2]
+        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
+        for r, j in enumerate(restart):
+            off = (B + r) * h8 * w8 * 128 * 2               # image B + r inside the 128-channel split planes (bytes)
+            eng.uconv(1, h8, w8, (xs.hi.data_ptr() + off, xs.lo.data_ptr() + off), 128, 128, pf.head, E.EPI_LINEAR,
+                      out_f32=ws.f1_cl.data_ptr() + j * n * 4, ldo_f32=256)
+        self._context(pc, bufs, ws, image1, h8, w8)
         return h8, w8
+
+
+def _runs(slots):
+    """Sorted slot indices -> (first, count) of each run of consecutive ones: one copy per run."""
+    out = []
+    for j in sorted(slots):
+        if out and out[-1][0] + out[-1][1] == j:
+            out[-1][1] += 1
+        else:
+            out.append([j, 1])
+    return out

@@ -258,12 +258,13 @@ class UmmaEngine(Engine):
             self._encoder = EncoderRunner(self)
         return self._encoder
 
-    def finish_fmaps(self, ws):
-        """Pool fmap2 into the pyramid (corr.py:18-21 on features) and refresh the halves copies."""
+    def finish_fmaps(self, ws, f1_slots=None):
+        """Pool fmap2 into the pyramid (corr.py:18-21 on features) and refresh the halves copies (of fmap1: only the rows of
+        batch items f1_slots when given, the others' halves being current)."""
         native.check(self.L.rnc_fmap_pyramid(_ptr(ws.f2_pyr), ws.B, ws.D, ws.H8, ws.W8, ws.levels, _stream()), "fmap_pyramid")
-        self._refresh_halves(ws)
+        self._refresh_halves(ws, f1_slots)
 
-    def _refresh_halves(self, ws):
+    def _refresh_halves(self, ws, f1_slots=None):
         if self.lookup_mode != "umma":
             return
         n1, n2 = ws.f1_cl.numel(), ws.f2_pyr.numel()
@@ -274,7 +275,13 @@ class UmmaEngine(Engine):
             nbytes = self.L.rnc_corr_lookup_umma_workspace_bytes(ws.B, ws.H8, ws.W8)
             ws.lookup_flags = torch.zeros(nbytes // 4, dtype=torch.int32, device=dev)
         s = _stream()
-        native.check(self.L.rnc_f32_to_f16(_ptr(ws.f1_cl), _ptr(ws.f1h), n1, s), "f32_to_f16(f1)")
+        if f1_slots is None:
+            native.check(self.L.rnc_f32_to_f16(_ptr(ws.f1_cl), _ptr(ws.f1h), n1, s), "f32_to_f16(f1)")
+        else:
+            n = n1 // ws.B
+            for j in f1_slots:
+                native.check(self.L.rnc_f32_to_f16(C.c_void_p(ws.f1_cl.data_ptr() + 4 * j * n),
+                                                   C.c_void_p(ws.f1h.data_ptr() + 2 * j * n), n, s), "f32_to_f16(f1)")
         native.check(self.L.rnc_f32_to_f16(_ptr(ws.f2_pyr), _ptr(ws.f2h), n2, s), "f32_to_f16(f2)")
 
     def lookup_resident(self, ws):

@@ -7,6 +7,8 @@ time (the model's batch items are independent; frames of a different size — KI
 warm-start forward interpolation runs on the GPU.  Metrics aggregate exactly as the reference's loops do: Sintel-style
 (`valid` absent) pools all pixels (evaluate.py:131-137), KITTI-style averages per-image means (evaluate.py:172-179).
 """
+from collections import deque, namedtuple
+
 import numpy as np
 import torch
 
@@ -76,6 +78,92 @@ def run_sequence(model, frames, iters=32, warm_start=False, mode="sintel", devic
         if warm_start:
             flow_prev = forward_interpolate(flow_low[0])[None]
     return flows
+
+
+SlotStep = namedtuple("SlotStep", "seq pair restart idle")
+
+
+def sequence_schedule(lengths, batch_size):
+    """Slot schedule of run_sequences for sequences of `lengths` frames: min(batch_size, number of sequences with a pair)
+    slots run in lockstep, one pair each per step.  Returns one list per step of each slot's SlotStep(seq, pair, restart,
+    idle): pair k of sequence seq is frames (k, k + 1); restart marks pair 0 (the slot's frame 1 is new, not the previous
+    step's frame 2); an idle slot has no sequence left and repeats its previous (seq, pair), whose result is dropped.  A slot
+    whose sequence ends takes the next sequence not yet started, in order; sequences of fewer than two frames are skipped."""
+    if batch_size < 1:
+        raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+    pending = deque(s for s, n in enumerate(lengths) if n >= 2)
+    cur = [SlotStep(pending.popleft(), 0, True, False) for _ in range(min(batch_size, len(pending)))]
+    steps = []
+    while any(not c.idle for c in cur):
+        steps.append(list(cur))
+        for j, c in enumerate(cur):
+            if c.idle:
+                continue
+            if c.pair + 2 < lengths[c.seq]:
+                cur[j] = SlotStep(c.seq, c.pair + 1, False, False)
+            elif pending:
+                cur[j] = SlotStep(pending.popleft(), 0, True, False)
+            else:
+                cur[j] = c._replace(restart=False, idle=True)
+    return steps
+
+
+def _stack(frames, device, padder):
+    x = torch.stack(frames)
+    if x.device.type == "cpu" and torch.device(device).type == "cuda":
+        x = x.pin_memory()
+    return padder.pad(x.to(device, non_blocking=True).float())[0]
+
+
+@torch.no_grad()
+def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda"):
+    """create_sintel_submission (evaluate.py:23-55) over many sequences at batch throughput.  sequences: list of frame lists,
+    every frame [3,H,W] of one size.  Yields (seq_index, pair_index, flow): the unpadded [2,H,W] flow_up of every pair, on
+    the device; per sequence the flows equal run_sequence(model, seq, iters, warm_start, mode)'s.
+
+    Slots run in lockstep (sequence_schedule).  Each step encodes only new frames: a continuing slot's frame 1 is its last
+    frame 2, whose fnet features are handed over on the device (rnc.model.SequenceStage).  With warm_start, a slot starts
+    from forward_interpolate of its own previous low-resolution flow, and from zero (a cold start) at pair 0.  The steps
+    run eagerly and never wait for the host; the caller moves or writes the flows."""
+    sizes = [tuple(f.shape) for seq in sequences for f in seq]
+    for s in sizes:
+        if len(s) != 3 or s != sizes[0]:
+            raise ValueError(f"all frames of one call must have the same [3,H,W] size: got {sizes[0]} and {s}")
+    steps = sequence_schedule([len(seq) for seq in sequences], batch_size)
+    if not steps:
+        return
+    from .engine import _require_cuda, engine_for, module_device
+    from .model import SequenceStage
+    model.eval()
+    padder = InputPadder(sizes[0], mode=mode)
+    stage = SequenceStage(model)
+    ws = fi = zero = None
+    for step in steps:
+        im1 = _stack([sequences[c.seq][c.pair] for c in step], device, padder)
+        im2 = _stack([sequences[c.seq][c.pair + 1] for c in step], device, padder)
+        if ws is None:
+            dev = _require_cuda(im1)
+            if module_device(model) != dev:
+                raise ValueError(f"model parameters are on {module_device(model)} but device is {dev}")
+            eng = engine_for(dev)
+        stage.restart = [j for j, c in enumerate(step) if c.restart]
+        stage.carry = [j for j, c in enumerate(step) if not c.restart and not c.idle]
+        with torch.cuda.device(dev), eng.lock:
+            if ws is None:
+                # this generator's own workspace: the features carried from step to step live in it, so the caller may run
+                # other forwards of the same shape between two steps
+                pk = eng.packed_update(model.update_block)
+                ws = eng.WS(dev, len(step), im1.shape[2] // 8, im1.shape[3] // 8, pk.has_mask, model.ncup)
+            for j in stage.restart if fi is not None else ():
+                fi[j].copy_(zero)           # cold start: coords0 + 0.0 is exactly coords0, as with flow_init=None
+            flow_low, flow_up = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws)
+            if warm_start:
+                fi = forward_interpolate(flow_low)
+                if zero is None:
+                    zero = torch.zeros_like(fi[0])
+        for j, c in enumerate(step):
+            if not c.idle:
+                yield c.seq, c.pair, padder.unpad(flow_up[j])
 
 
 def load_checkpoint(model, state):

@@ -85,9 +85,11 @@ class _RAFTBase(nn.Module):
             return eng.graph_forward(self, image1, image2, iters, flow_init)
         return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode)
 
-    def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode, upsample=None):
+    def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode, upsample=None, encode=None, ws=None):
         """The iteration loop on the engine's resident buffers.  upsample(eng, ws, pu) produces each full-resolution prediction
-        from the workspace; the default is the inference upsampler (self._upsample on packed weights)."""
+        from the workspace; the default is the inference upsampler (self._upsample on packed weights).  encode(eng, ws, image1,
+        image2) fills the feature maps and the GRU state; the default encodes both frames (self._encode).  ws: a workspace the
+        caller owns instead of the engine's shared one of this shape."""
         B, _, Him, Wim = image1.shape
         H8, W8 = Him // 8, Wim // 8
         L = eng.L
@@ -99,27 +101,10 @@ class _RAFTBase(nn.Module):
             if self.ncup and any(isinstance(m, nn.BatchNorm2d) and m.training for m in self.upsampler.modules()):
                 raise NotImplementedError("weights-net BatchNorm with batch statistics needs the training path (enable grad) "
                                           "or eval mode: call .eval() / freeze_bn()")
-        ws = eng.workspace(image1.device, B, H8, W8, pk.has_mask, self.ncup)
+        if ws is None:
+            ws = eng.workspace(image1.device, B, H8, W8, pk.has_mask, self.ncup)
         s = _stream()
-        amp = bool(getattr(self.args, "mixed_precision", False))
-        if eng.mode == "umma" and not amp and os.environ.get("RNC_ENCODER", "umma").lower() == "umma":
-            # encoders on the tensor-core path, writing straight into the resident buffers (raft_nc_dbl.py:118-140)
-            with _Timed(eng, "encoders"):
-                eng.encoder().run(self, ws, image1.float().contiguous(), image2.float().contiguous())
-                eng.finish_fmaps(ws)
-        else:
-            image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
-            image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
-            with torch.autocast("cuda", enabled=amp):
-                fmap1, fmap2 = self.fnet([image1, image2])
-            fmap1, fmap2 = fmap1.float().contiguous(), fmap2.float().contiguous()
-            with torch.autocast("cuda", enabled=amp):
-                cnet = self.cnet(image1)
-                net, inp = torch.split(cnet, [128, 128], dim=1)
-                net, inp = torch.tanh(net), torch.relu(inp)
-            net, inp = net.float().contiguous(), inp.float().contiguous()
-            eng.fmap_prepare(ws, fmap1, fmap2, 4)
-            eng.load_state(ws, net, inp)
+        (encode or self._encode)(eng, ws, image1, image2)
         fi = None
         if flow_init is not None:
             fi = flow_init.to(image1.device).float().contiguous()
@@ -142,6 +127,36 @@ class _RAFTBase(nn.Module):
         if test_mode:
             return eng.flow_low(ws), flow_up
         return preds
+
+    def _umma_encoders(self, eng):
+        """Do the encoders run on the tensor-core path (else on torch modules: RNC_ENCODER=cudnn, RNC_CONV=ffma, amp)?"""
+        amp = bool(getattr(self.args, "mixed_precision", False))
+        return eng.mode == "umma" and not amp and os.environ.get("RNC_ENCODER", "umma").lower() == "umma"
+
+    def _context(self, image1):
+        """cnet on the normalised frame 1 -> (tanh(net), relu(inp)) NCHW fp32 (raft_nc_dbl.py:137-140)."""
+        with torch.autocast("cuda", enabled=bool(getattr(self.args, "mixed_precision", False))):
+            cnet = self.cnet(image1)
+            net, inp = torch.split(cnet, [128, 128], dim=1)
+            net, inp = torch.tanh(net), torch.relu(inp)
+        return net.float().contiguous(), inp.float().contiguous()
+
+    def _encode(self, eng, ws, image1, image2):
+        """Encoder stage of a forward: fnet on both frames, cnet on frame 1 (raft_nc_dbl.py:118-140)."""
+        if self._umma_encoders(eng):
+            # encoders on the tensor-core path, writing straight into the resident buffers
+            with _Timed(eng, "encoders"):
+                eng.encoder().run(self, ws, image1.float().contiguous(), image2.float().contiguous())
+                eng.finish_fmaps(ws)
+            return
+        image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
+        image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
+        with torch.autocast("cuda", enabled=bool(getattr(self.args, "mixed_precision", False))):
+            fmap1, fmap2 = self.fnet([image1, image2])
+        fmap1, fmap2 = fmap1.float().contiguous(), fmap2.float().contiguous()
+        net, inp = self._context(image1)
+        eng.fmap_prepare(ws, fmap1, fmap2, 4)
+        eng.load_state(ws, net, inp)
 
     def _upsample(self, eng, ws, pu):
         raise NotImplementedError
@@ -230,6 +245,47 @@ def frozen_trunk(model, image1=None, image2=None, flow_init=None):
     if any(isinstance(m, nn.BatchNorm2d) and m.training for t in trunk for m in t.modules()):
         return False
     return not getattr(model.args, "mixed_precision", False)
+
+
+class SequenceStage:
+    """Encoder stage of one step of sequence inference (rnc.harness.run_sequences), for _forward_eager(encode=...).
+
+    Slot j of the batch holds one pair of one sequence.  Before each call the driver sets `carry` (slots whose frame 1 is the
+    previous step's frame 2) and `restart` (slots that start a sequence: their frame 1 is new); every other slot is idle and
+    recomputes its previous pair.  fnet runs on frame 2 of every slot and frame 1 of the restarted ones only: fnet normalises
+    each image on its own (InstanceNorm), so a carried slot's frame-1 features are the previous step's frame-2 features.  cnet
+    runs on frame 1 of every slot.  The object keeps the state that carries between steps; the feature maps in the workspace
+    are the rest, so one stage belongs to one workspace."""
+
+    def __init__(self, model):
+        self.model = model
+        self.carry, self.restart = [], []
+        self.fmap1 = self.fmap2 = None          # torch-encoder route: NCHW features of the last step's frames
+
+    def __call__(self, eng, ws, image1, image2):
+        m = self.model
+        if m._umma_encoders(eng):
+            with _Timed(eng, "encoders"):
+                eng.encoder().run_step(m, ws, image1.float().contiguous(), image2.float().contiguous(), self.carry, self.restart)
+                eng.finish_fmaps(ws, f1_slots=self.restart)
+            return
+        B = image1.shape[0]
+        image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
+        image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
+        new = torch.cat([image2] + [image1[j:j + 1] for j in self.restart]) if self.restart else image2
+        with torch.autocast("cuda", enabled=bool(getattr(m.args, "mixed_precision", False))):
+            f = m.fnet(new)
+        f = f.float().contiguous()
+        if self.fmap1 is None:
+            self.fmap1 = torch.empty_like(f[:B])
+        for j in self.carry:
+            self.fmap1[j].copy_(self.fmap2[j])
+        for r, j in enumerate(self.restart):
+            self.fmap1[j].copy_(f[B + r])
+        self.fmap2 = f[:B]
+        net, inp = m._context(image1)
+        eng.fmap_prepare(ws, self.fmap1, self.fmap2, 4)
+        eng.load_state(ws, net, inp)
 
 
 class _Dims:

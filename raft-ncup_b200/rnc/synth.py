@@ -42,6 +42,15 @@ def smooth_shift_frames(b, h, w, seed=7, dy=3, dx=4):
     return big[:, :, dy:, dx:].contiguous(), big[:, :, :h, :w].contiguous()
 
 
+def shift_sequence(n, h, w, seed=7, dy=3, dx=4):
+    """A sequence of n frames [3,h,w] for warm-started inference: crops of one smooth canvas (bicubic-upsampled 20x36 noise, as
+    smooth_shift_frames), frame t + 1 being frame t translated by dy px vertically and dx px horizontally."""
+    g = torch.Generator().manual_seed(seed)
+    low = torch.rand(1, 3, 20, 36, generator=g)
+    big = F.interpolate(low, size=(h + (n - 1) * dy, w + (n - 1) * dx), mode="bicubic", align_corners=False).clamp(0, 1) * 255
+    return [big[0, :, (n - 1 - t) * dy:(n - 1 - t) * dy + h, (n - 1 - t) * dx:(n - 1 - t) * dx + w].contiguous() for t in range(n)]
+
+
 def motion_boundary_flow_init(b, h8, w8, jump=24.0):
     """Stimulus 3: a warm-start flow field (raft_nc_dbl.py:144-145) with a motion boundary — the right half moves `jump` px (at
     1/8 resolution) further than the left half, and the lower third moves vertically too — so the lookup windows of the tiles on
