@@ -120,7 +120,6 @@ class _Augmentor:
 
     def _launch(self, descs, dev):
         """Run the kernels on the uploaded pack `dev` (device copy of _pack's buffer) on the current stream of its device."""
-        L = native.lib()
         B = len(descs)
         ch, cw = int(self.crop_size[0]), int(self.crop_size[1])
         device = dev.device
@@ -128,13 +127,10 @@ class _Augmentor:
         img2 = torch.empty_like(img1)
         flow = torch.empty(B, 2, ch, cw, device=device)
         valid = torch.empty(B, ch, cw, device=device)
-        ws_bytes = L.rnc_augment_workspace_bytes(B, ch, cw, int(self.sparse))
+        ws_bytes = native.rnc.augment_workspace_bytes(B, ch, cw, int(self.sparse))
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         with torch.cuda.device(device):
-            stream = torch.cuda.current_stream().cuda_stream
-            native.check(L.rnc_augment(C.addressof(descs), dev.data_ptr(), B, dev.data_ptr(), dev.numel(), ch, cw,
-                                       int(self.sparse), img1.data_ptr(), img2.data_ptr(), flow.data_ptr(), valid.data_ptr(),
-                                       ws.data_ptr(), ws_bytes, stream), "augment")
+            native.rnc.augment(descs, dev, B, dev, dev.numel(), ch, cw, int(self.sparse), img1, img2, flow, valid, ws, ws_bytes)
         return img1, img2, flow, valid
 
     def _fill(self, c, d, o):

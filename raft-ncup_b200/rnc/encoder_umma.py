@@ -9,13 +9,12 @@ fixed order, rnc_instnorm_stats_det, instead of the convolution epilogue's fp64 
 their results straight into the loop's resident buffers: fmap1 -> f1_cl, fmap2 -> level 0 of f2_pyr, tanh(net) -> h and
 hx[:, 0:128], relu(inp) -> hx[:, 128:256] (raft_nc_dbl.py:129-140).
 """
-import ctypes as C
-
 import torch
 
 from . import native
-from .engine import _ptr, _stream, fold_bn
+from .engine import fold_bn
 from .engine_umma import HX_LD, SplitBuf, UmmaWeights
+from .native import rnc
 
 EPS = 1e-5
 
@@ -77,11 +76,11 @@ class EncoderBuffers:
         self.mr = torch.empty(N * 128 * 2, **f)
         self.parts = None                                  # rnc_instnorm_stats_det's partials, sized on first use
 
-    def det_workspace(self, L):
+    def det_workspace(self):
         if self.parts is None:
             # sized for all N images of the buffers: a pass may run on fewer (cnet, sequence steps), but the first not always
             N = self.key[1]
-            nbytes = max(L.rnc_instnorm_stats_det_workspace_bytes(N, h * w, c) for (h, w, c) in self.dims)
+            nbytes = max(rnc.instnorm_stats_det_workspace_bytes(N, h * w, c) for (h, w, c) in self.dims)
             self.parts = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=self.stats.device)
         return self.parts
 
@@ -105,26 +104,21 @@ class EncoderRunner:
     def _norm(self, bufs, x32, N, P, Cc, mode, res=None, out32=None, split=None, fused_stats=False):
         """fused_stats: the producing convolution already accumulated the sums into bufs.stats (rnc_conv_umma_desc.stats);
         otherwise the deterministic statistics pass reads x32."""
-        s = _stream()
         if fused_stats:
-            native.check(self.L.rnc_instnorm_finalize(_ptr(bufs.stats), N, P, Cc, EPS, _ptr(bufs.mr), s), "instnorm_finalize")
+            rnc.instnorm_finalize(bufs.stats, N, P, Cc, EPS, bufs.mr)
         else:
-            ws = bufs.det_workspace(self.L)
-            native.check(self.L.rnc_instnorm_stats_det(_ptr(x32), N, P, Cc, EPS, _ptr(ws), ws.numel() * 8, _ptr(bufs.mr), s),
-                         "instnorm_stats_det")
-        native.check(self.L.rnc_instnorm_apply(_ptr(x32), _ptr(bufs.mr), _ptr(res), N, P, Cc, mode, _ptr(out32),
-                                               C.c_void_p(split.hi.data_ptr() if split else 0),
-                                               C.c_void_p(split.lo.data_ptr() if split else 0), s), "instnorm_apply")
+            ws = bufs.det_workspace()
+            rnc.instnorm_stats_det(x32, N, P, Cc, EPS, ws, ws.numel() * 8, bufs.mr)
+        rnc.instnorm_apply(x32, bufs.mr, res, N, P, Cc, mode, out32, split.hi if split else None, split.lo if split else None)
 
     def _trunk(self, pk, bufs, image, N, Hin, Win):
         """Stem + the six residual blocks.  Leaves the 128-channel features at 1/8 resolution in bufs.XS[2] (split)."""
-        E, eng, s = native, self.eng, _stream()
+        E, eng = native, self.eng
         inst = pk.kind == "instance"
         fused = not torch.are_deterministic_algorithms_enabled()    # epilogue statistics use fp64 atomics
         st = bufs.stats.data_ptr() if fused else 0
         h, w, _ = bufs.dims[0]
-        native.check(self.L.rnc_stem_window_prep(_ptr(image), N, Hin, Win, bufs.pitch, _ptr(bufs.img_hi), _ptr(bufs.img_lo), s),
-                     "stem_window_prep")
+        rnc.stem_window_prep(image, N, Hin, Win, bufs.pitch, bufs.img_hi, bufs.img_lo)
         win = dict(stride=2, hin=Hin, win=w, win_pitch=4 * bufs.pitch, flags=eng.conv_flags | E.CONV_WINDOW)
         img = (bufs.img_hi.data_ptr(), bufs.img_lo.data_ptr())
         if inst:
@@ -188,8 +182,8 @@ class EncoderRunner:
         eng.alloc_fmaps(ws, B, 256, h8, w8, 4, dev)
         xs = bufs.XS[2]
         eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f1_cl.data_ptr(), ldo_f32=256)
-        off = B * P * 128 * 2                                  # second half of the batch inside the split planes (bytes)
-        eng.uconv(B, h8, w8, (xs.hi.data_ptr() + off, xs.lo.data_ptr() + off), 128, 128, pf.head, E.EPI_LINEAR,
+        # the second half of the batch inside the split planes
+        eng.uconv(B, h8, w8, (xs.hi[B * P:].data_ptr(), xs.lo[B * P:].data_ptr()), 128, 128, pf.head, E.EPI_LINEAR,
                   out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
         self._context(pc, bufs, ws, image1, h8, w8)
         return h8, w8
@@ -227,9 +221,9 @@ class EncoderRunner:
         xs = bufs.XS[2]
         eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
         for r, j in enumerate(restart):
-            off = (B + r) * h8 * w8 * 128 * 2               # image B + r inside the 128-channel split planes (bytes)
-            eng.uconv(1, h8, w8, (xs.hi.data_ptr() + off, xs.lo.data_ptr() + off), 128, 128, pf.head, E.EPI_LINEAR,
-                      out_f32=ws.f1_cl.data_ptr() + j * n * 4, ldo_f32=256)
+            i = (B + r) * h8 * w8                           # image B + r inside the 128-channel split planes
+            eng.uconv(1, h8, w8, (xs.hi[i:].data_ptr(), xs.lo[i:].data_ptr()), 128, 128, pf.head, E.EPI_LINEAR,
+                      out_f32=f1[j * n:].data_ptr(), ldo_f32=256)
         self._context(pc, bufs, ws, image1, h8, w8)
         return h8, w8
 

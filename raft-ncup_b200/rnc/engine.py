@@ -18,19 +18,11 @@ import torch
 import torch.nn.functional as F
 
 from . import native
-from .native import ConvDesc
+from .native import ConvDesc, rnc
 from .nconv_unet import PackedUNet, is_fused
 
 CORR_CH = 324          # 4 levels * 9 * 9
 HX_LD = 384            # [h | inp | motion(126) flow(2)]
-
-
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 def _require_cuda(*tensors):
@@ -362,7 +354,7 @@ class Engine:
         self._ws = OrderedDict()            # workspace key -> workspace, LRU
         self.lock = threading.RLock()
         self.device = None
-        self.L = native.lib()
+        self.L = native.lib()               # the raw handle, for code that calls an entry point directly; see native.rnc
 
     # ------------------------------------------------------------------ caches
     def _packed_for(self, kind, module, build):
@@ -448,14 +440,14 @@ class Engine:
         d.B, d.H, d.W = B, H, W
         d.cout, d.kh, d.kw, d.epilogue = cout, kh, kw, epi
         if dil > 1:
-            native.check(self.L.rnc_conv2d_cl_dil_fwd(C.byref(d), dil, _stream()), "conv2d_cl_dil")
+            rnc.conv2d_cl_dil_fwd(d, dil)
         else:
-            native.check(self.L.rnc_conv2d_cl_fwd(C.byref(d), _stream()), "conv2d_cl")
+            rnc.conv2d_cl_fwd(d)
 
     def alloc_fmaps(self, ws, B, D, H, W, levels, device):
         """Allocate the CL feature map / pyramid buffers of ws, which fmap_prepare fills and the tensor-core encoder heads
         write into directly."""
-        total = self.L.rnc_pyramid_offset(B, D, H, W, levels)
+        total = rnc.pyramid_offset(B, D, H, W, levels)
         if ws.f1_cl is None or ws.f1_cl.numel() != B * H * W * D:
             ws.f1_cl = torch.empty(B * H * W, D, dtype=torch.float32, device=device)
             ws.f2_pyr = torch.empty(total, dtype=torch.float32, device=device)
@@ -464,13 +456,11 @@ class Engine:
     def fmap_prepare(self, ws, fmap1, fmap2, levels=4):
         B, D, H, W = fmap1.shape
         self.alloc_fmaps(ws, B, D, H, W, levels, fmap1.device)
-        native.check(self.L.rnc_fmap_prepare(_ptr(fmap1), _ptr(fmap2), B, D, H, W, levels, _ptr(ws.f1_cl),
-                                             _ptr(ws.f2_pyr), _stream()), "fmap_prepare")
+        rnc.fmap_prepare(fmap1, fmap2, B, D, H, W, levels, ws.f1_cl, ws.f2_pyr)
 
     def lookup(self, ws, coords, out, layout, ldo, radius=4):
         with _Timed(self, "corr_lookup"):
-            native.check(self.L.rnc_corr_lookup_fwd(_ptr(ws.f1_cl), _ptr(ws.f2_pyr), _ptr(coords), ws.B, ws.D, ws.H8, ws.W8,
-                                                    ws.levels, radius, _ptr(out), layout, ldo, _stream()), "corr_lookup")
+            rnc.corr_lookup_fwd(ws.f1_cl, ws.f2_pyr, coords, ws.B, ws.D, ws.H8, ws.W8, ws.levels, radius, out, layout, ldo)
 
     def begin_iter(self, ws, pk):
         """Hook called before the lookup of every iteration (the tensor-core engine forks independent work here)."""
@@ -481,11 +471,11 @@ class Engine:
 
     def load_corr(self, ws, corr_nchw):
         B, _, H, W = corr_nchw.shape
-        native.check(self.L.rnc_nchw_to_cl(_ptr(corr_nchw), B, CORR_CH, H, W, _ptr(ws.corr), CORR_CH, 0, _stream()), "nchw_to_cl(corr)")
+        rnc.nchw_to_cl(corr_nchw, B, CORR_CH, H, W, ws.corr, CORR_CH, 0)
 
     def guidance(self, ws):
-        """(pointer, pixel stride) of the CL fp32 hidden state used as NCUP guidance (update.py:135, raft_nc_dbl.py:161)."""
-        return ws.hx.data_ptr(), HX_LD
+        """(tensor, pixel stride) of the CL fp32 hidden state used as NCUP guidance (update.py:135, raft_nc_dbl.py:161)."""
+        return ws.hx, HX_LD
 
     # ------------------------------------------------------------------ update block on resident buffers
     def update_iter(self, ws, pk, want_mask=False, want_delta=False):
@@ -509,12 +499,11 @@ class Engine:
     def _motion_encoder_ffma(self, ws, pk):
         """BasicMotionEncoder (update.py:89-97): ws.corr, ws.coords1 -> hx[:, 256:384] = [motion(126) | flow(2)]."""
         B, H, W = ws.B, ws.H8, ws.W8
-        mot_ptr = ws.hx.data_ptr() + 256 * 4
+        mot_ptr = ws.hx[:, 256:].data_ptr()
         self.conv(B, H, W, ws.corr.data_ptr(), CORR_CH, CORR_CH, pk.convc1, 256, 1, 1, native.EPI_RELU, ws.c1.data_ptr(), 256)
         self.conv(B, H, W, ws.c1.data_ptr(), 256, 256, pk.convc2, 192, 3, 3, native.EPI_RELU, ws.corflo.data_ptr(), 256)
-        native.check(self.L.rnc_conv_flow7x7_fwd(_ptr(ws.coords1), _ptr(pk.convf1[0]), _ptr(pk.convf1[1]), B, H, W, 128,
-                                                 _ptr(ws.f1), 128, _stream()), "convf1")
-        self.conv(B, H, W, ws.f1.data_ptr(), 128, 128, pk.convf2, 64, 3, 3, native.EPI_RELU, ws.corflo.data_ptr() + 192 * 4, 256)
+        rnc.conv_flow7x7_fwd(ws.coords1, pk.convf1[0], pk.convf1[1], B, H, W, 128, ws.f1, 128)
+        self.conv(B, H, W, ws.f1.data_ptr(), 128, 128, pk.convf2, 64, 3, 3, native.EPI_RELU, ws.corflo[:, 192:].data_ptr(), 256)
         self.conv(B, H, W, ws.corflo.data_ptr(), 256, 256, pk.conv, 126, 3, 3, native.EPI_RELU_FLOW, mot_ptr, HX_LD,
                   aux0=ws.coords1.data_ptr(), ldaux=0)
 
@@ -522,7 +511,7 @@ class Engine:
         """SepConvGRU (update.py:45-60): horizontal (1x5) then vertical (5x1) half steps on hx = [h | x]; h in place."""
         B, H, W = ws.B, ws.H8, ws.W8
         hx = ws.hx.data_ptr()
-        x_ptr = hx + 128 * 4          # channels 128.. = [inp | motion | flow]
+        x_ptr = ws.hx[:, 128:].data_ptr()          # channels 128.. = [inp | motion | flow]
         for zr, q, kh, kw in ((pk.zr1, pk.q1, 1, 5), (pk.zr2, pk.q2, 5, 1)):
             self.conv(B, H, W, hx, HX_LD, HX_LD, zr, 256, kh, kw, native.EPI_GRU_ZR, ws.rh.data_ptr(), 128,
                       h=hx, ldh=HX_LD, aux0=ws.z.data_ptr(), ldaux=128)
@@ -533,60 +522,53 @@ class Engine:
         """FlowHead (update.py:13-14) + coords1 += delta (raft_nc_dbl.py:157)."""
         B, H, W = ws.B, ws.H8, ws.W8
         self.conv(B, H, W, ws.hx.data_ptr(), 128, HX_LD, pk.fh1, 256, 3, 3, native.EPI_RELU, ws.fh.data_ptr(), 256)
-        native.check(self.L.rnc_flow_head2_fwd(_ptr(ws.fh), 256, 256, _ptr(pk.fh2[0]), _ptr(pk.fh2[1]), B, H, W,
-                                               _ptr(ws.delta) if want_delta else C.c_void_p(0), _ptr(ws.coords1), _stream()),
-                     "flow_head2")
+        rnc.flow_head2_fwd(ws.fh, 256, 256, pk.fh2[0], pk.fh2[1], B, H, W, ws.delta if want_delta else None, ws.coords1)
 
     def load_state(self, ws, net, inp):
         """NCHW net/inp (raft_nc_dbl.py:137-140) -> resident hx buffer."""
         B, _, H, W = net.shape
-        s = _stream()
-        native.check(self.L.rnc_nchw_to_cl(_ptr(net), B, 128, H, W, _ptr(ws.hx), HX_LD, 0, s), "nchw_to_cl(net)")
-        native.check(self.L.rnc_nchw_to_cl(_ptr(inp), B, 128, H, W, _ptr(ws.hx), HX_LD, 128, s), "nchw_to_cl(inp)")
+        rnc.nchw_to_cl(net, B, 128, H, W, ws.hx, HX_LD, 0)
+        rnc.nchw_to_cl(inp, B, 128, H, W, ws.hx, HX_LD, 128)
 
     def net_nchw(self, ws):
         out = torch.empty(ws.B, 128, ws.H8, ws.W8, dtype=torch.float32, device=ws.hx.device)
-        native.check(self.L.rnc_cl_to_nchw(_ptr(ws.hx), HX_LD, 0, ws.B, 128, ws.H8, ws.W8, _ptr(out), _stream()), "cl_to_nchw")
+        rnc.cl_to_nchw(ws.hx, HX_LD, 0, ws.B, 128, ws.H8, ws.W8, out)
         return out
 
     def flow_low(self, ws):
         out = torch.empty_like(ws.coords1)
-        native.check(self.L.rnc_coords_to_flow(_ptr(ws.coords1), _ptr(out), ws.B, ws.H8, ws.W8, _stream()), "coords_to_flow")
+        rnc.coords_to_flow(ws.coords1, out, ws.B, ws.H8, ws.W8)
         return out
 
     # ------------------------------------------------------------------ upsamplers
     def convex_upsample(self, ws, flow_low, mask_cl, ldm):
         out = torch.empty(ws.B, 2, 8 * ws.H8, 8 * ws.W8, dtype=torch.float32, device=flow_low.device)
         with _Timed(self, "convex"):
-            native.check(self.L.rnc_convex_upsample_fwd(_ptr(flow_low), _ptr(mask_cl), ldm, ws.B, ws.H8, ws.W8, _ptr(out),
-                                                        _stream()), "convex_upsample")
+            rnc.convex_upsample_fwd(flow_low, mask_cl, ldm, ws.B, ws.H8, ws.W8, out)
         return out
 
-    def ncup_from_lowres(self, ws, pu, x_lowres, guid_ptr, ldg, out_scale):
-        """NConvUpsampler.forward (upsampler.py:143-177) on x_lowres NCHW [B,2,H4,W4] with CL guidance at H8."""
+    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale):
+        """NConvUpsampler.forward (upsampler.py:143-177) on x_lowres NCHW [B,2,H4,W4] with CL guidance guid at H8 (pixel
+        stride ldg)."""
         B, H8, W8 = ws.B, ws.H8, ws.W8
         H4, W4 = 2 * H8, 2 * W8
-        s = _stream()
-        native.check(self.L.rnc_ncup_guidance_fwd(_ptr(x_lowres), C.c_void_p(guid_ptr), ldg, 128, B, H8, W8, _ptr(ws.gin),
-                                                  132, s), "ncup_guidance")
+        rnc.ncup_guidance_fwd(x_lowres, guid, ldg, 128, B, H8, W8, ws.gin, 132)
         self.weights_net(pu, B, H4, W4, ws.gin, wnet_buffers(ws, pu), ws.conf)
         return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)
 
     def weights_net(self, pk, B, H, W, x, bufs, conf):
         """Simple.forward (interp_weights_est.py:39-47) on the exact kernels: x fp32 CL [B*H*W, >= pk.cin0_pad] (zero beyond the
         input channels) -> conf NCHW [B,2,H,W]; bufs = pk.buffers(B*H*W)."""
-        s = _stream()
         c, ld = pk.cin0_pad, x.shape[1]
         for (cout, k, dil), wt, y in zip(pk.layers, pk.g, bufs):
             self.conv(B, H, W, x.data_ptr(), c, ld, wt, cout, k, k, native.EPI_RELU, y.data_ptr(), y.shape[1], dil=dil)
             x, c, ld = y, y.shape[1], y.shape[1]
         if pk.gout is not None:
-            native.check(self.L.rnc_conf_head_fwd(_ptr(x), c, ld, _ptr(pk.gout[0]), _ptr(pk.gout[1]), B, H, W, _ptr(conf), s),
-                         "conf_head")
+            rnc.conf_head_fwd(x, c, ld, pk.gout[0], pk.gout[1], B, H, W, conf)
             return
         (k, dil), y = pk.head, bufs[-1]
         self.conv(B, H, W, x.data_ptr(), c, ld, pk.g_out, 2, k, k, native.EPI_SIGMOID, y.data_ptr(), 4, dil=dil)
-        native.check(self.L.rnc_cl_to_nchw(_ptr(y), 4, 0, B, 2, H, W, _ptr(conf), s), "cl_to_nchw(conf)")
+        rnc.cl_to_nchw(y, 4, 0, B, 2, H, W, conf)
 
     def ncup_chain(self, ws, pu, x_lowres, conf, out_scale):
         """Zero-stuffing + NConvUNet + out_scale (upsampler.py:150-177) on x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4]:
@@ -596,8 +578,7 @@ class Engine:
         if pu.unet is None:
             out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
             with _Timed(self, "ncup"):
-                native.check(self.L.rnc_ncup_fwd(_ptr(x_lowres), _ptr(conf), pu.nconv_host, B, H4, W4, out_scale, _ptr(out),
-                                                 _stream()), "ncup")
+                rnc.ncup_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out)
             return out
         # intermediates live in the workspace (allocated by the first, eager forward of a shape; graph capture reuses them)
         bufs = ws.__dict__.setdefault("nconv_bufs", {})

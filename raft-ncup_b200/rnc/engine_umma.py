@@ -2,15 +2,14 @@
 wide convolution on wgmma (rnc_conv2d_umma_fwd) and the 1/8-resolution activations resident as fp16 hi/lo split
 planes (value = hi + lo).  Thin layers (7x7 on flow, 3x3 -> 2 flow head, 1x1 -> 2 confidence head) stay on CUDA cores.
 """
-import ctypes as C
 import math
 
 import torch
 import torch.nn.functional as F
 
 from . import native
-from .engine import CORR_CH, HX_LD, Engine, PackedUpsampler, _ptr, _stream, _Timed, pack_thin, wnet_buffers
-from .native import UmmaConvDesc
+from .engine import CORR_CH, HX_LD, Engine, PackedUpsampler, _Timed, pack_thin, wnet_buffers
+from .native import UmmaConvDesc, rnc
 
 CORR_LS = 88           # channels reserved per pyramid level in the resident corr row: 81 taps + 7 zero pads (16-byte groups)
 CORR_LD = 4 * CORR_LS  # 352: row pitch of the corr halves planes; convc1 still needs only 6 K-blocks of 64
@@ -156,7 +155,9 @@ class SplitBuf:
         self.ld = ld
 
     def ptrs(self, ch_off=0):
-        return self.hi.data_ptr() + 2 * ch_off, self.lo.data_ptr() + 2 * ch_off
+        """Addresses of channel ch_off in both planes (rnc_conv_umma_desc's in*_hi / in*_lo, out_hi / out_lo).  Computed rather
+        than read off a view: uconv calls this on every layer of every iteration."""
+        return self.hi.data_ptr() + ch_off * self.hi.element_size(), self.lo.data_ptr() + ch_off * self.lo.element_size()
 
 
 class UmmaWorkspace:
@@ -175,9 +176,8 @@ class UmmaWorkspace:
         # Epilogue-only tensors live in the tile-blocked layout [tile][channel][128 px] of their layer's tiling (thread = pixel
         # then reads / writes full lines): the z gate, and the hoisted context-feature share of the GRU gate pre-activations
         # (valid until inp changes).  Horizontal (1x5) and vertical (5x1) layers tile differently; z serves both halves.
-        L = native.lib()
-        th = max(L.rnc_conv_umma_tiles(1, 5, 1, B, H8, W8, fl) for fl in (0, 1))      # with / without halo sharing (RNC_CONV_FLAGS)
-        tv = max(L.rnc_conv_umma_tiles(5, 1, 1, B, H8, W8, fl) for fl in (0, 1))
+        th = max(rnc.conv_umma_tiles(1, 5, 1, B, H8, W8, fl) for fl in (0, 1))      # with / without halo sharing (RNC_CONV_FLAGS)
+        tv = max(rnc.conv_umma_tiles(5, 1, 1, B, H8, W8, fl) for fl in (0, 1))
         self.z = torch.empty(max(th, tv) * 128 * 128, **f)
         self.czr1, self.czr2 = torch.empty(th * 256 * 128, **f), torch.empty(tv * 256 * 128, **f)
         self.cq1, self.cq2 = torch.empty(th * 128 * 128, **f), torch.empty(tv * 128 * 128, **f)
@@ -245,7 +245,7 @@ class UmmaEngine(Engine):
         d.h, d.ldh, d.aux0, d.ldaux = h, ldh, aux0, ldaux
         d.B, d.H, d.W = B, H, W
         d.cout, d.kh, d.kw, d.epilogue = wt.cout, wt.kh, wt.kw, epi
-        native.check(self.L.rnc_conv2d_umma_fwd(C.byref(d), _stream()), "conv2d_umma")
+        rnc.conv2d_umma_fwd(d)
 
     def fmap_prepare(self, ws, fmap1, fmap2, levels=4):
         super().fmap_prepare(ws, fmap1, fmap2, levels)
@@ -261,7 +261,7 @@ class UmmaEngine(Engine):
     def finish_fmaps(self, ws, f1_slots=None):
         """Pool fmap2 into the pyramid (corr.py:18-21 on features) and refresh the halves copies (of fmap1: only the rows of
         batch items f1_slots when given, the others' halves being current)."""
-        native.check(self.L.rnc_fmap_pyramid(_ptr(ws.f2_pyr), ws.B, ws.D, ws.H8, ws.W8, ws.levels, _stream()), "fmap_pyramid")
+        rnc.fmap_pyramid(ws.f2_pyr, ws.B, ws.D, ws.H8, ws.W8, ws.levels)
         self._refresh_halves(ws, f1_slots)
 
     def _refresh_halves(self, ws, f1_slots=None):
@@ -272,40 +272,33 @@ class UmmaEngine(Engine):
             dev = ws.f1_cl.device
             ws.f1h = torch.empty(n1, dtype=torch.float16, device=dev)
             ws.f2h = torch.empty(n2, dtype=torch.float16, device=dev)
-            nbytes = self.L.rnc_corr_lookup_umma_workspace_bytes(ws.B, ws.H8, ws.W8)
+            nbytes = rnc.corr_lookup_umma_workspace_bytes(ws.B, ws.H8, ws.W8)
             ws.lookup_flags = torch.zeros(nbytes // 4, dtype=torch.int32, device=dev)
-        s = _stream()
         if f1_slots is None:
-            native.check(self.L.rnc_f32_to_f16(_ptr(ws.f1_cl), _ptr(ws.f1h), n1, s), "f32_to_f16(f1)")
+            rnc.f32_to_f16(ws.f1_cl, ws.f1h, n1)
         else:
-            n = n1 // ws.B
+            f1, f1h = ws.f1_cl.view(ws.B, -1), ws.f1h.view(ws.B, -1)
             for j in f1_slots:
-                native.check(self.L.rnc_f32_to_f16(C.c_void_p(ws.f1_cl.data_ptr() + 4 * j * n),
-                                                   C.c_void_p(ws.f1h.data_ptr() + 2 * j * n), n, s), "f32_to_f16(f1)")
-        native.check(self.L.rnc_f32_to_f16(_ptr(ws.f2_pyr), _ptr(ws.f2h), n2, s), "f32_to_f16(f2)")
+                rnc.f32_to_f16(f1[j], f1h[j], n1 // ws.B)
+        rnc.f32_to_f16(ws.f2_pyr, ws.f2h, n2)
 
     def lookup_resident(self, ws):
         """corr lookup straight into the split planes convc1 consumes."""
         if self.lookup_mode == "umma":
             with _Timed(self, "corr_lookup"):
-                native.check(self.L.rnc_corr_lookup_umma_fwd(
-                    _ptr(ws.f1h), _ptr(ws.f2h), _ptr(ws.f1_cl), _ptr(ws.f2_pyr), _ptr(ws.coords1), ws.B, ws.D, ws.H8, ws.W8,
-                    ws.levels, 4, _ptr(ws.corr.hi), _ptr(ws.corr.lo), CORR_LD, CORR_LS, _ptr(ws.lookup_flags),
-                    ws.lookup_flags.numel() * 4, _stream()), "corr_lookup_umma")
+                rnc.corr_lookup_umma_fwd(ws.f1h, ws.f2h, ws.f1_cl, ws.f2_pyr, ws.coords1, ws.B, ws.D, ws.H8, ws.W8, ws.levels, 4,
+                                         ws.corr.hi, ws.corr.lo, CORR_LD, CORR_LS, ws.lookup_flags, ws.lookup_flags.numel() * 4)
             return
         with _Timed(self, "corr_lookup"):
-            native.check(self.L.rnc_corr_lookup_split_fwd(_ptr(ws.f1_cl), _ptr(ws.f2_pyr), _ptr(ws.coords1), ws.B, ws.D, ws.H8,
-                                                          ws.W8, ws.levels, 4, _ptr(ws.corr.hi), _ptr(ws.corr.lo), CORR_LD, CORR_LS,
-                                                          _stream()), "corr_lookup_split")
+            rnc.corr_lookup_split_fwd(ws.f1_cl, ws.f2_pyr, ws.coords1, ws.B, ws.D, ws.H8, ws.W8, ws.levels, 4, ws.corr.hi,
+                                      ws.corr.lo, CORR_LD, CORR_LS)
 
     def _convf1(self, ws, pk):
         if self.convf1_mode == "mm":
-            native.check(self.L.rnc_flow_im2col7_split_fwd(_ptr(ws.coords1), ws.B, ws.H8, ws.W8, _ptr(ws.fcol.hi), _ptr(ws.fcol.lo), 128,
-                                                           _stream()), "flow_im2col7")
+            rnc.flow_im2col7_split_fwd(ws.coords1, ws.B, ws.H8, ws.W8, ws.fcol.hi, ws.fcol.lo, 128)
             self.uconv(ws.B, ws.H8, ws.W8, ws.fcol.ptrs(), 98, 128, pk.convf1_mm, native.EPI_RELU, out_split=ws.f1.ptrs(), ldo_split=128)
             return
-        native.check(self.L.rnc_conv_flow7x7_split_fwd(_ptr(ws.coords1), _ptr(pk.convf1[0]), _ptr(pk.convf1[1]), ws.B, ws.H8, ws.W8,
-                                                       128, _ptr(ws.f1.hi), _ptr(ws.f1.lo), 128, _stream()), "convf1")
+        rnc.conv_flow7x7_split_fwd(ws.coords1, pk.convf1[0], pk.convf1[1], ws.B, ws.H8, ws.W8, 128, ws.f1.hi, ws.f1.lo, 128)
 
     def begin_iter(self, ws, pk):
         """Fork: convf1 (7x7 on the flow, CUDA cores, ~1 KB of shared memory) depends only on coords1, so it runs on a side
@@ -322,7 +315,6 @@ class UmmaEngine(Engine):
 
     def _update_iter(self, ws, pk, want_mask, want_delta):
         B, H, W = ws.B, ws.H8, ws.W8
-        s = _stream()
         E = native
         # BasicMotionEncoder (update.py:89-97)
         self.uconv(B, H, W, ws.corr.ptrs(), CORR_LD, CORR_LD, pk.convc1, E.EPI_RELU, out_split=ws.c1.ptrs(), ldo_split=256)
@@ -353,8 +345,7 @@ class UmmaEngine(Engine):
         # FlowHead (update.py:13-14) + coords1 += delta (raft_nc_dbl.py:157)
         self.uconv(B, H, W, ws.hx.ptrs(), 128, HX_LD, pk.fh1, E.EPI_RELU, out_split=ws.fh.ptrs(), ldo_split=256)
         self.uconv(B, H, W, ws.fh.ptrs(), 256, 256, pk.fh2, E.EPI_LINEAR, out_f32=ws.fh2p.data_ptr(), ldo_f32=32)
-        native.check(self.L.rnc_flow_tap_gather_fwd(_ptr(ws.fh2p), 32, _ptr(pk.fh2_bias), B, H, W,
-                                                    _ptr(ws.delta) if want_delta else None, _ptr(ws.coords1), s), "flow_tap_gather")
+        rnc.flow_tap_gather_fwd(ws.fh2p, 32, pk.fh2_bias, B, H, W, ws.delta if want_delta else None, ws.coords1)
         if want_mask:
             self.uconv(B, H, W, ws.hx.ptrs(), 128, HX_LD, pk.m0, E.EPI_RELU, out_split=ws.mh.ptrs(), ldo_split=256)
             self.uconv(B, H, W, ws.mh.ptrs(), 256, 256, pk.m2, E.EPI_LINEAR, out_f32=ws.mask.data_ptr(), ldo_f32=576)
@@ -362,23 +353,19 @@ class UmmaEngine(Engine):
     def load_state(self, ws, net, inp):
         ws.gru_const_valid = False
         B, _, H, W = net.shape
-        s = _stream()
-        M = B * H * W
-        L = self.L
-        native.check(L.rnc_nchw_to_cl(_ptr(net), B, 128, H, W, _ptr(ws.h), 128, 0, s), "nchw_to_cl(net)")
-        native.check(L.rnc_nchw_to_cl(_ptr(net), B, 128, H, W, _ptr(ws.tmp), 256, 0, s), "nchw_to_cl(net)")
-        native.check(L.rnc_nchw_to_cl(_ptr(inp), B, 128, H, W, _ptr(ws.tmp), 256, 128, s), "nchw_to_cl(inp)")
-        native.check(L.rnc_f32_to_split(_ptr(ws.tmp), 256, 256, M, _ptr(ws.hx.hi), _ptr(ws.hx.lo), HX_LD, 0, s), "f32_to_split")
+        rnc.nchw_to_cl(net, B, 128, H, W, ws.h, 128, 0)
+        rnc.nchw_to_cl(net, B, 128, H, W, ws.tmp, 256, 0)
+        rnc.nchw_to_cl(inp, B, 128, H, W, ws.tmp, 256, 128)
+        rnc.f32_to_split(ws.tmp, 256, 256, B * H * W, ws.hx.hi, ws.hx.lo, HX_LD, 0)
 
     def load_corr(self, ws, corr_nchw):
         """seam path (BasicUpdateBlock.forward): NCHW corr -> split planes."""
         B, _, H, W = corr_nchw.shape
         tmp = torch.empty(B * H * W, CORR_CH, dtype=torch.float32, device=corr_nchw.device)
-        native.check(self.L.rnc_nchw_to_cl(_ptr(corr_nchw), B, CORR_CH, H, W, _ptr(tmp), CORR_CH, 0, _stream()), "nchw_to_cl(corr)")
+        rnc.nchw_to_cl(corr_nchw, B, CORR_CH, H, W, tmp, CORR_CH, 0)
         res = torch.zeros(B * H * W, CORR_LD, dtype=torch.float32, device=corr_nchw.device)     # layout plumbing: resident order
         res[:, corr_resident_index(res.device)] = tmp
-        native.check(self.L.rnc_f32_to_split(_ptr(res), CORR_LD, CORR_LD, B * H * W, _ptr(ws.corr.hi), _ptr(ws.corr.lo), CORR_LD, 0,
-                                             _stream()), "f32_to_split(corr)")
+        rnc.f32_to_split(res, CORR_LD, CORR_LD, B * H * W, ws.corr.hi, ws.corr.lo, CORR_LD, 0)
 
     def corr_nchw(self, ws):
         """The resident corr row back in the reference's layout [B, 324, H8, W8] (tests / debugging)."""
@@ -387,19 +374,16 @@ class UmmaEngine(Engine):
 
     def net_nchw(self, ws):
         out = torch.empty(ws.B, 128, ws.H8, ws.W8, dtype=torch.float32, device=ws.h.device)
-        native.check(self.L.rnc_cl_to_nchw(_ptr(ws.h), 128, 0, ws.B, 128, ws.H8, ws.W8, _ptr(out), _stream()), "cl_to_nchw")
+        rnc.cl_to_nchw(ws.h, 128, 0, ws.B, 128, ws.H8, ws.W8, out)
         return out
 
     def guidance(self, ws):
-        return ws.h.data_ptr(), 128
+        return ws.h, 128
 
-    def ncup_from_lowres(self, ws, pu, x_lowres, guid_ptr, ldg, out_scale):
+    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale):
         B, H8, W8 = ws.B, ws.H8, ws.W8
         H4, W4 = 2 * H8, 2 * W8
-        s = _stream()
-        L = self.L
-        native.check(L.rnc_ncup_guidance_split_fwd(_ptr(x_lowres), C.c_void_p(guid_ptr), ldg, 128, B, H8, W8, _ptr(ws.gin.hi),
-                                                   _ptr(ws.gin.lo), GIN_LD, s), "ncup_guidance_split")
+        rnc.ncup_guidance_split_fwd(x_lowres, guid, ldg, 128, B, H8, W8, ws.gin.hi, ws.gin.lo, GIN_LD)
         # Simple.forward (interp_weights_est.py:39-47)
         x, c, ld = ws.gin.ptrs(), 132, GIN_LD
         bufs = wnet_buffers(ws, pu)
@@ -411,10 +395,9 @@ class UmmaEngine(Engine):
                 self.uconv(B, H4, W4, x, c, ld, wt, native.EPI_RELU, out_f32=y.data_ptr(), ldo_f32=y.shape[1], dil=dil)
         if pu.gout is not None:
             y = bufs[-1]
-            native.check(L.rnc_conf_head_fwd(_ptr(y), y.shape[1], y.shape[1], _ptr(pu.gout[0]), _ptr(pu.gout[1]), B, H4, W4,
-                                             _ptr(ws.conf), s), "conf_head")
+            rnc.conf_head_fwd(y, y.shape[1], y.shape[1], pu.gout[0], pu.gout[1], B, H4, W4, ws.conf)
         else:
             (k, dil), y = pu.head, bufs[-1]
             self.uconv(B, H4, W4, x, c, ld, pu.u_out, native.EPI_SIGMOID, out_f32=y.data_ptr(), ldo_f32=32, dil=dil)
-            native.check(L.rnc_cl_to_nchw(_ptr(y), 32, 0, B, 2, H4, W4, _ptr(ws.conf), s), "cl_to_nchw(conf)")
+            rnc.cl_to_nchw(y, 32, 0, B, 2, H4, W4, ws.conf)
         return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)

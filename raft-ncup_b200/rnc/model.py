@@ -4,16 +4,15 @@ Mirrors ``RAFT(nn.Module)`` of core/raft.py:24-143 (convex upsampler) and core/r
 same ctor Namespace, ``forward(image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False)``, return values
 and state_dict keys.  The iteration loop runs entirely on resident channel-last buffers through librnc.so.
 """
-import ctypes as C
 import os
 from collections import OrderedDict
 
 import torch
 import torch.nn as nn
 
-from . import native
-from .engine import _Timed, _ptr, _require_cuda, _stream, engine_for, module_device, module_tensors
+from .engine import _Timed, _require_cuda, engine_for, module_device, module_tensors
 from .modules import BasicEncoder, BasicUpdateBlock, get_upsampler
+from .native import rnc
 
 
 class _RAFTBase(nn.Module):
@@ -92,7 +91,6 @@ class _RAFTBase(nn.Module):
         caller owns instead of the engine's shared one of this shape."""
         B, _, Him, Wim = image1.shape
         H8, W8 = Him // 8, Wim // 8
-        L = eng.L
         pk = eng.packed_update(self.update_block)
         pu = None
         if upsample is None:
@@ -103,14 +101,13 @@ class _RAFTBase(nn.Module):
                                           "or eval mode: call .eval() / freeze_bn()")
         if ws is None:
             ws = eng.workspace(image1.device, B, H8, W8, pk.has_mask, self.ncup)
-        s = _stream()
         (encode or self._encode)(eng, ws, image1, image2)
         fi = None
         if flow_init is not None:
             fi = flow_init.to(image1.device).float().contiguous()
             if fi.shape != (B, 2, H8, W8):
                 raise ValueError("flow_init must be [N,2,H/8,W/8]")
-        native.check(L.rnc_coords_init(_ptr(ws.coords1), _ptr(fi), B, H8, W8, s), "coords_init")
+        rnc.coords_init(ws.coords1, fi, B, H8, W8)
 
         preds = []
         flow_up = None
@@ -176,8 +173,7 @@ class RAFTConvex(_RAFTBase):
         B, _, H8, W8 = flow.shape
         with torch.cuda.device(dev), eng.lock:
             m_cl = torch.empty(B * H8 * W8, 576, dtype=torch.float32, device=dev)
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(mask.detach().float().contiguous()), B, 576, H8, W8, _ptr(m_cl), 576, 0, _stream()),
-                         "nchw_to_cl(mask)")
+            rnc.nchw_to_cl(mask.detach().float().contiguous(), B, 576, H8, W8, m_cl, 576, 0)
             ws = _Dims(B, H8, W8)
             return eng.convex_upsample(ws, flow.detach().float().contiguous(), m_cl, 576)
 
@@ -200,9 +196,9 @@ class RAFTNcup(_RAFTBase):
         self.data_idx = 0
 
     def _upsample(self, eng, ws, pu):
-        native.check(eng.L.rnc_flow_x2_fwd(_ptr(ws.coords1), ws.B, ws.H8, ws.W8, _ptr(ws.x4), _stream()), "flow_x2")
-        gptr, gld = eng.guidance(ws)
-        return eng.ncup_from_lowres(ws, pu, ws.x4, gptr, gld, 8.0)   # `8 *` of raft_nc_dbl.py:161
+        rnc.flow_x2_fwd(ws.coords1, ws.B, ws.H8, ws.W8, ws.x4)
+        g, gld = eng.guidance(ws)
+        return eng.ncup_from_lowres(ws, pu, ws.x4, g, gld, 8.0)   # `8 *` of raft_nc_dbl.py:161
 
     def _upsample_frozen(self, eng, ws, pu):
         """Upsampling step of the frozen-trunk forward: snapshots what the upsampler consumes into tensors of this forward
@@ -211,14 +207,13 @@ class RAFTNcup(_RAFTBase):
         from .train import ncup_upsampler_frozen
         B, H8, W8 = ws.B, ws.H8, ws.W8
         dev = ws.coords1.device
-        s = _stream()
         x4 = torch.empty(B, 2, 2 * H8, 2 * W8, dtype=torch.float32, device=dev)
-        native.check(eng.L.rnc_flow_x2_fwd(_ptr(ws.coords1), B, H8, W8, _ptr(x4), s), "flow_x2")
+        rnc.flow_x2_fwd(ws.coords1, B, H8, W8, x4)
         # the weights-net input cat(x4, area-resized guidance) built straight from the fp32 guidance, channels padded to 136:
         # the tensor of to_cl(cat(x4, g4), pad_to=136) in ncup_upsampler_train
-        gptr, gld = eng.guidance(ws)
+        g, gld = eng.guidance(ws)
         gin = torch.empty(B, 2 * H8, 2 * W8, 136, dtype=torch.float32, device=dev)
-        native.check(eng.L.rnc_ncup_guidance_fwd(_ptr(x4), C.c_void_p(gptr), gld, 128, B, H8, W8, _ptr(gin), 136, s), "ncup_guidance")
+        rnc.ncup_guidance_fwd(x4, g, gld, 128, B, H8, W8, gin, 136)
         return ncup_upsampler_frozen(self.upsampler, x4, gin, 8.0)   # `8 *` of raft_nc_dbl.py:161
 
     def upsample_flow(self, flow_lr, guidance):

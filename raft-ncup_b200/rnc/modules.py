@@ -14,10 +14,10 @@ import torch.nn as nn
 import torch.nn.functional as F
 from torch.nn.modules.utils import _pair
 
-from . import native
 from .nconv_unet import PackedUNet, is_fused, nconv_fwd
-from .engine import (CORR_CH, HX_LD, Engine, PackedFlowHead, PackedGRU, PackedMotionEncoder, PackedSimple, _ptr, _require_cuda,
-                     _stream, engine_for, module_tensors)
+from .engine import (CORR_CH, HX_LD, Engine, PackedFlowHead, PackedGRU, PackedMotionEncoder, PackedSimple, _require_cuda,
+                     engine_for, module_tensors)
+from .native import rnc
 
 # --------------------------------------------------------------------------------------------- encoders (C6)
 # RAFT.forward runs the encoders on the tensor-core path (rnc/encoder_umma.py).  The nn.Module forwards below are the
@@ -179,8 +179,7 @@ class FlowHead(nn.Module):
             B, _, H, W = x.shape
             ws = eng.workspace(x.device, B, H, W, mode="ffma")
             pk = eng._packed_for("flow_head", self, PackedFlowHead)
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, 128, H, W, _ptr(ws.hx), HX_LD, 0, _stream()),
-                         "nchw_to_cl")
+            rnc.nchw_to_cl(x.detach().float().contiguous(), B, 128, H, W, ws.hx, HX_LD, 0)
             eng._flow_head_ffma(ws, pk, want_delta=True)       # also advances the workspace's scratch coords1 (unused here)
             return ws.delta.clone()
 
@@ -204,9 +203,8 @@ class SepConvGRU(nn.Module):
             B, _, H, W = h.shape
             ws = eng.workspace(h.device, B, H, W, mode="ffma")
             pk = eng._packed_for("gru", self, PackedGRU)
-            s = _stream()
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(h.detach().float().contiguous()), B, 128, H, W, _ptr(ws.hx), HX_LD, 0, s), "nchw_to_cl")
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, 256, H, W, _ptr(ws.hx), HX_LD, 128, s), "nchw_to_cl")
+            rnc.nchw_to_cl(h.detach().float().contiguous(), B, 128, H, W, ws.hx, HX_LD, 0)
+            rnc.nchw_to_cl(x.detach().float().contiguous(), B, 256, H, W, ws.hx, HX_LD, 128)
             eng._gru_ffma(ws, pk)
             return Engine.net_nchw(eng, ws)          # the exact kernels' hidden state, whatever the engine's mode
 
@@ -233,13 +231,11 @@ class BasicMotionEncoder(nn.Module):
             B, _, H, W = flow.shape
             ws = eng.workspace(flow.device, B, H, W, mode="ffma")
             pk = eng._packed_for("motion_encoder", self, PackedMotionEncoder)
-            s = _stream()
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(corr.detach().float().contiguous()), B, CORR_CH, H, W, _ptr(ws.corr), CORR_CH, 0, s),
-                         "nchw_to_cl(corr)")
-            native.check(eng.L.rnc_coords_init(_ptr(ws.coords1), _ptr(flow.detach().float().contiguous()), B, H, W, s), "coords_init")
+            rnc.nchw_to_cl(corr.detach().float().contiguous(), B, CORR_CH, H, W, ws.corr, CORR_CH, 0)
+            rnc.coords_init(ws.coords1, flow.detach().float().contiguous(), B, H, W)
             eng._motion_encoder_ffma(ws, pk)
             out = torch.empty(B, 128, H, W, dtype=torch.float32, device=flow.device)
-            native.check(eng.L.rnc_cl_to_nchw(_ptr(ws.hx), HX_LD, 256, B, 128, H, W, _ptr(out), s), "cl_to_nchw")
+            rnc.cl_to_nchw(ws.hx, HX_LD, 256, B, 128, H, W, out)
             return out
 
 
@@ -272,19 +268,17 @@ class BasicUpdateBlock(nn.Module):
         B, _, H, W = net.shape
         pk = eng.packed_update(self)
         ws = eng.workspace(net.device, B, H, W, pk.has_mask, False)
-        s = _stream()
-        L = eng.L
         eng.load_state(ws, net.float().contiguous(), inp.float().contiguous())
         eng.load_corr(ws, corr.float().contiguous())
         # the kernels read flow as coords1 - grid: rebuild coords1 from the flow argument
-        native.check(L.rnc_coords_init(_ptr(ws.coords1), _ptr(flow.float().contiguous()), B, H, W, s), "coords_init")
+        rnc.coords_init(ws.coords1, flow.float().contiguous(), B, H, W)
         eng.update_iter(ws, pk, want_mask=pk.has_mask, want_delta=True)
         net_out = eng.net_nchw(ws)
         self.net = net_out                                  # guidance tap read by raft_nc_dbl.py:161
         mask = None
         if pk.has_mask:
             mask = torch.empty(B, 576, H, W, dtype=torch.float32, device=net.device)
-            native.check(L.rnc_cl_to_nchw(_ptr(ws.mask), 576, 0, B, 576, H, W, _ptr(mask), s), "cl_to_nchw(mask)")
+            rnc.cl_to_nchw(ws.mask, 576, 0, B, 576, H, W, mask)
         else:
             mask = 0.25 * net_out                           # `.25 * Sequential()(net)` of the reference (update.py:140)
         return net_out, mask, ws.delta.clone()
@@ -443,8 +437,7 @@ class Simple(nn.Module):
             cpad = pk.cin0_pad
             M = B * h * w
             xin = torch.zeros(M, cpad, dtype=torch.float32, device=x.device) if cpad != Cin else torch.empty(M, cpad, dtype=torch.float32, device=x.device)
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(x.detach().float().contiguous()), B, Cin, h, w, _ptr(xin), cpad, 0, _stream()),
-                         "nchw_to_cl")
+            rnc.nchw_to_cl(x.detach().float().contiguous(), B, Cin, h, w, xin, cpad, 0)
             conf = torch.empty(B, 2, h, w, dtype=torch.float32, device=x.device)
             eng.weights_net(pk, B, h, w, xin, pk.buffers(M, x.device), conf)
             return conf
@@ -491,9 +484,8 @@ class NConvUpsampler(nn.Module):
             pu = eng.packed_upsampler(self)
             ws = eng.workspace(x_lowres.device, B, h // 2, w // 2, False, True)
             g_cl = torch.empty(B * (h // 2) * (w // 2), 128, dtype=torch.float32, device=x_lowres.device)
-            native.check(eng.L.rnc_nchw_to_cl(_ptr(x_guidance.float().contiguous()), B, 128, h // 2, w // 2, _ptr(g_cl), 128, 0,
-                                              _stream()), "nchw_to_cl(guidance)")
-            return eng.ncup_from_lowres(ws, pu, x_lowres.float().contiguous(), g_cl.data_ptr(), 128, out_scale)
+            rnc.nchw_to_cl(x_guidance.float().contiguous(), B, 128, h // 2, w // 2, g_cl, 128, 0)
+            return eng.ncup_from_lowres(ws, pu, x_lowres.float().contiguous(), g_cl, 128, out_scale)
 
 
 def get_upsampler(in_ch, guidance_ch, args):

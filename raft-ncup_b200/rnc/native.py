@@ -1,5 +1,11 @@
-"""ctypes binding of librnc.so (include/rnc.h).  No torch types cross this boundary: callers pass
-``tensor.data_ptr()`` integers, plain ints and the raw ``cudaStream_t``.
+"""ctypes binding of librnc.so (include/rnc.h).
+
+``rnc.<entry point without the rnc_ prefix>`` is how the product calls the library, e.g.
+``rnc.nchw_to_cl(net, B, 128, H, W, ws.hx, HX_LD, 0)``: a ``void*`` argument takes a tensor (its ``data_ptr()``, so a view
+carries its own offset), ``None`` (NULL) or a raw address; descriptors and arrays pass through; the stream argument is left
+out and the current CUDA stream (``stream()``) appended; a non-zero ``rnc_status`` raises through ``check()`` naming the
+entry point.  Size queries and the info calls return their value.  ``lib()`` is the raw ctypes handle; every call reads it
+at call time, so a test that swaps ``_lib`` sees every entry point.
 
 The library is REQUIRED on the product path: ``lib()`` raises ``RncUnavailable`` if it cannot be loaded —
 there is no CPU or PyTorch fallback for the hot path.
@@ -7,6 +13,9 @@ there is no CPU or PyTorch fallback for the hot path.
 import ctypes as C
 import os
 import threading
+import types
+
+import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RNC_LIB") or os.path.join(_HERE, "librnc.so")      # RNC_LIB: developer override (variant builds)
@@ -15,7 +24,6 @@ CONV_NO_HALO, CONV_BASE_OFFSET, CONV_SPLIT_N, CONV_NO_PAIR, CONV_AUX_BLOCKED, CO
 
 (EPI_LINEAR, EPI_RELU, EPI_SIGMOID, EPI_GRU_ZR, EPI_GRU_Q, EPI_RELU_FLOW, EPI_RELU_ADD_RELU, EPI_TANH_RELU,
  EPI_FLOW_DELTA) = range(9)
-CONV_NO_HALO, CONV_BASE_OFFSET = 1, 2
 
 _vp, _i, _f = C.c_void_p, C.c_int, C.c_float
 
@@ -168,7 +176,7 @@ def lib():
     return _lib
 
 
-def check(status, what=""):
+def check(status, what="rnc"):
     """Translate a negative rnc_status into a Python exception (the reference's error channel, SURVEY §8b)."""
     if status == 0:
         return
@@ -177,13 +185,41 @@ def check(status, what=""):
     if status == -4:
         msg += f" (cudaError {l.rnc_last_cuda_error()})"
     if status in (-1, -3):
-        raise ValueError(f"rnc {what}: {msg}")
-    raise RncError(f"rnc {what}: {msg}")
+        raise ValueError(f"{what}: {msg}")
+    raise RncError(f"{what}: {msg}")
+
+
+def stream():
+    """The raw cudaStream_t of torch's current stream, on which the bound entry points enqueue their work."""
+    return torch.cuda.current_stream().cuda_stream
+
+
+def _bind(name, restype, argtypes):
+    # kernel entry points return an rnc_status and take the stream last; which arguments are void* is fixed here, once
+    kernel = restype is _i and len(argtypes) > 0 and argtypes[-1] is _vp
+    ptrs = tuple(i for i, t in enumerate(argtypes[:-1] if kernel else argtypes) if t is _vp)
+
+    def call(*args):
+        args = list(args)
+        for i in ptrs:
+            if isinstance(args[i], torch.Tensor):
+                args[i] = args[i].data_ptr()
+        if not kernel:
+            return getattr(lib(), name)(*args)
+        status = getattr(lib(), name)(*args, stream())
+        if status:
+            check(status, name)
+
+    call.__name__ = call.__qualname__ = name
+    return call
+
+
+rnc = types.SimpleNamespace(**{name[4:]: _bind(name, *sig) for name, sig in SIGNATURES.items()})
 
 
 def launch_count():
-    return int(lib().rnc_launch_count())
+    return int(rnc.launch_count())
 
 
 def launch_count_reset():
-    lib().rnc_launch_count_reset()
+    rnc.launch_count_reset()

@@ -12,7 +12,7 @@ The decoder's concatenation is a read pattern of rnc_nconv2d_fwd (the "up" sourc
 """
 import torch
 
-from . import native
+from .native import rnc
 
 
 def is_fused(net):
@@ -49,10 +49,6 @@ def live_chain(net, data, conf, layer, pool):
     return layer(net.nconv_out, *up, last=True)
 
 
-def _p(t):
-    return None if t is None else t.data_ptr()
-
-
 def _empty(shape, like, dtype=torch.float32):
     return torch.empty(shape, dtype=dtype, device=like.device)
 
@@ -68,9 +64,7 @@ def nconv_fwd(x, c, weight, bias, eps, up=None, y_scale=1.0, alloc=_empty):
     if c.shape != x.shape or Ct != Cin + Cup or (up is not None and (uc.shape != ux.shape or ux.shape[0] != N)):
         raise ValueError("NConv2d: data/conf/weight shapes do not match")
     y, co = alloc((N, Cout, H, W), x), alloc((N, Cout, H, W), x)
-    native.check(native.lib().rnc_nconv2d_fwd(_p(x), _p(c), _p(weight), _p(bias), N, Cin, Cout, H, W, kh, kw, eps, _p(ux),
-                                              _p(uc), Cup, Hup, Wup, float(y_scale), _p(y), _p(co),
-                                              torch.cuda.current_stream().cuda_stream), "nconv2d")
+    rnc.nconv2d_fwd(x, c, weight, bias, N, Cin, Cout, H, W, kh, kw, eps, ux, uc, Cup, Hup, Wup, float(y_scale), y, co)
     return y, co
 
 
@@ -79,8 +73,7 @@ def pool_fwd(x, c, max_pool_data, alloc=_empty):
     N, C, H, W = x.shape
     xo, co = alloc((N, C, H // 2, W // 2), x), alloc((N, C, H // 2, W // 2), x)
     idx = alloc((2, N, C, H // 2, W // 2), x, torch.int32)
-    native.check(native.lib().rnc_nconv_pool2_fwd(_p(x), _p(c), N, C, H, W, int(max_pool_data), _p(xo), _p(co), _p(idx),
-                                                  torch.cuda.current_stream().cuda_stream), "nconv_pool2")
+    rnc.nconv_pool2_fwd(x, c, N, C, H, W, int(max_pool_data), xo, co, idx)
     return xo, co, idx
 
 

@@ -32,7 +32,8 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from . import native
-from .engine import CORR_CH, _ptr, _require_cuda, _stream, engine_for, pack_conv
+from .engine import CORR_CH, _require_cuda, engine_for, pack_conv
+from .native import rnc
 from .nconv_unet import is_fused, live_chain, nconv_fwd, pool_fwd, unused_parameters
 
 _PACK_CACHE = {}          # (id(weight), version, kind, fmt, cin_pad) -> (weight, packed); flushed at every training forward
@@ -142,8 +143,8 @@ def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16", dil=1):
     dt = torch.float32 if fmt == "tf32" else torch.float16
     hi = torch.empty(M, Cx, dtype=dt, device=x.device)
     lo = torch.empty(M, Cx, dtype=dt, device=x.device)
-    split = eng.L.rnc_f32_to_tf32_split if fmt == "tf32" else eng.L.rnc_f32_to_split
-    native.check(split(_ptr(x), Cx, Cx, M, _ptr(hi), _ptr(lo), Cx, 0, _stream()), "operand split")
+    split = rnc.f32_to_tf32_split if fmt == "tf32" else rnc.f32_to_split
+    split(x, Cx, Cx, M, hi, lo, Cx, 0)
     ldo = _ceil4(cout)
     out = torch.empty(B, Ho, Wo, ldo, dtype=torch.float32, device=x.device)
     if bias is not None:
@@ -217,26 +218,24 @@ class ConvCL(torch.autograd.Function):
                 if gx.shape[-1] != Cx:               # Cx > ceil4(cin) never happens; equal by construction
                     gx = F.pad(gx, (0, Cx - gx.shape[-1]))
             if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):
-                gwp, gbp = _wgrad(eng, x, gy, cout, kh, kw, ctx.stride, ctx.has_bias, dil)
+                gwp, gbp = _wgrad(x, gy, cout, kh, kw, ctx.stride, ctx.has_bias, dil)
                 gw = gwp.view(kh, kw, Cx, cout)[:, :, :cin].permute(3, 2, 0, 1).contiguous()
                 gb = gbp
         return gx, gw, gb, None, None
 
 
-def _wgrad(eng, x, gy, cout, kh, kw, stride, has_bias, dil=1):
+def _wgrad(x, gy, cout, kh, kw, stride, has_bias, dil=1):
     """Weight / bias gradient of ConvCL: [kh*kw, Cx, cout], [cout] (or None).  rnc_conv2d_cl_wgrad_det (rnc_conv2d_cl_wgrad_dil_det
     for a dilated layer) sums the K-split partials in a fixed order (in either mode: it is no slower than adding them with atomics
     was) and writes its outputs."""
     B, H, W, Cx = x.shape
     gwp = torch.empty(kh * kw, Cx, cout, dtype=torch.float32, device=x.device)
     gbp = torch.empty(cout, dtype=torch.float32, device=x.device) if has_bias else None
-    L = eng.L
-    nbytes_fn, wgrad_fn, arg = ((L.rnc_conv2d_cl_wgrad_dil_workspace_bytes, L.rnc_conv2d_cl_wgrad_dil_det, dil) if dil > 1 else
-                                (L.rnc_conv2d_cl_wgrad_workspace_bytes, L.rnc_conv2d_cl_wgrad_det, stride))
+    nbytes_fn, wgrad_fn, arg = ((rnc.conv2d_cl_wgrad_dil_workspace_bytes, rnc.conv2d_cl_wgrad_dil_det, dil) if dil > 1 else
+                                (rnc.conv2d_cl_wgrad_workspace_bytes, rnc.conv2d_cl_wgrad_det, stride))
     nbytes = nbytes_fn(Cx, cout, B, H, W, kh, kw, arg)
     ws = torch.empty((nbytes + 3) // 4, dtype=torch.float32, device=x.device)
-    native.check(wgrad_fn(_ptr(x), Cx, Cx, _ptr(gy), gy.shape[-1], cout, B, H, W, kh, kw, arg, _ptr(gwp), cout, _ptr(gbp), _ptr(ws),
-                          ws.numel() * 4, _stream()), "conv2d_cl_wgrad_det")
+    wgrad_fn(x, Cx, Cx, gy, gy.shape[-1], cout, B, H, W, kh, kw, arg, gwp, cout, gbp, ws, ws.numel() * 4)
     return gwp, gbp
 
 
@@ -274,22 +273,21 @@ class CorrPyramid(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, fmap2_cl, levels):
-        eng = engine_for(fmap2_cl.device)
+        _require_cuda(fmap2_cl)
         B, H, W, D = fmap2_cl.shape
-        total = eng.L.rnc_pyramid_offset(B, D, H, W, levels)
+        total = rnc.pyramid_offset(B, D, H, W, levels)
         pyr = torch.empty(total, dtype=torch.float32, device=fmap2_cl.device)
         pyr[:B * H * W * D] = fmap2_cl.reshape(-1)
-        native.check(eng.L.rnc_fmap_pyramid(_ptr(pyr), B, D, H, W, levels, _stream()), "fmap_pyramid")
+        rnc.fmap_pyramid(pyr, B, D, H, W, levels)
         ctx.dims = (B, H, W, D, levels)
         return pyr
 
     @staticmethod
     def backward(ctx, g_pyr):
         B, H, W, D, levels = ctx.dims
-        eng = engine_for(g_pyr.device)
         g = g_pyr.clone()
         with torch.cuda.device(g.device):
-            native.check(eng.L.rnc_pyramid_pool_bwd(_ptr(g), B, D, H, W, levels, _stream()), "pyramid_pool_bwd")
+            rnc.pyramid_pool_bwd(g, B, D, H, W, levels)
         return g[:B * H * W * D].view(B, H, W, D), None
 
 
@@ -298,12 +296,11 @@ class CorrLookup(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, f1_cl, f2_pyr, coords, levels):
-        eng = engine_for(f1_cl.device)
+        _require_cuda(f1_cl)
         B, H, W, D = f1_cl.shape
         coords = coords.detach().float().contiguous()
         out = torch.empty(B, H, W, CORR_CH, dtype=torch.float32, device=f1_cl.device)
-        native.check(eng.L.rnc_corr_lookup_fwd(_ptr(f1_cl), _ptr(f2_pyr), _ptr(coords), B, D, H, W, levels, 4, _ptr(out), 1, CORR_CH,
-                                               _stream()), "corr_lookup")
+        rnc.corr_lookup_fwd(f1_cl, f2_pyr, coords, B, D, H, W, levels, 4, out, 1, CORR_CH)
         ctx.save_for_backward(f1_cl, f2_pyr, coords)
         ctx.levels = levels
         return out
@@ -311,27 +308,25 @@ class CorrLookup(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_out):
         f1_cl, f2_pyr, coords = ctx.saved_tensors
-        eng = engine_for(f1_cl.device)
         with torch.cuda.device(f1_cl.device):
-            g_f1, g_f2 = _lookup_bwd(eng, f1_cl, f2_pyr, coords, g_out.contiguous(), ctx.levels)
+            g_f1, g_f2 = _lookup_bwd(f1_cl, f2_pyr, coords, g_out.contiguous(), ctx.levels)
         return g_f1, g_f2, None, None
 
 
-def _lookup_bwd(eng, f1_cl, f2_pyr, coords, g_out, levels):
+def _lookup_bwd(f1_cl, f2_pyr, coords, g_out, levels):
     """(d fmap1, d fmap2 pyramid) of CorrLookup.  Deterministic mode gathers d fmap2 per pyramid position in a fixed order
     (rnc_corr_lookup_bwd_det, which writes every position); otherwise every pixel scatters into it with atomics."""
     B, H, W, D = f1_cl.shape
-    args = (_ptr(f1_cl), _ptr(f2_pyr), _ptr(coords), _ptr(g_out), g_out.shape[-1], B, D, H, W, levels, 4)
+    args = (f1_cl, f2_pyr, coords, g_out, g_out.shape[-1], B, D, H, W, levels, 4)
     g_f1 = torch.empty_like(f1_cl)
     if deterministic():
         g_f2 = torch.empty_like(f2_pyr)
-        nbytes = eng.L.rnc_corr_lookup_bwd_workspace_bytes(B, H, W, levels)
+        nbytes = rnc.corr_lookup_bwd_workspace_bytes(B, H, W, levels)
         ws = torch.empty((nbytes + 15) // 16, 4, dtype=torch.float32, device=f1_cl.device)
-        native.check(eng.L.rnc_corr_lookup_bwd_det(*args, _ptr(g_f1), _ptr(g_f2), _ptr(ws), ws.numel() * 4, _stream()),
-                     "corr_lookup_bwd_det")
+        rnc.corr_lookup_bwd_det(*args, g_f1, g_f2, ws, ws.numel() * 4)
     else:
         g_f2 = torch.zeros_like(f2_pyr)
-        native.check(eng.L.rnc_corr_lookup_bwd(*args, _ptr(g_f1), _ptr(g_f2), _stream()), "corr_lookup_bwd")
+        rnc.corr_lookup_bwd(*args, g_f1, g_f2)
     return g_f1, g_f2
 
 
@@ -365,13 +360,12 @@ class NConv2dFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, gy, gc):
         data, conf, weight, bias, y, c, ux, uc = ctx.saved_tensors
-        eng = engine_for(data.device)
         N, Cin, H, W = data.shape
         Cout, _, kh, kw = weight.shape
         Cup, Hup, Wup = (ux.shape[1], ux.shape[2], ux.shape[3]) if ux is not None else (0, 0, 0)
         need = ctx.needs_input_grad
         with torch.cuda.device(data.device):
-            nbytes = eng.L.rnc_nconv2d_bwd_workspace_bytes(N, Cin, Cup, Cout, H, W, kh)
+            nbytes = rnc.nconv2d_bwd_workspace_bytes(N, Cin, Cup, Cout, H, W, kh)
             ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=data.device)
             g_data = torch.empty_like(data) if need[0] else None
             g_conf = torch.empty_like(conf) if need[1] else None
@@ -379,11 +373,9 @@ class NConv2dFn(torch.autograd.Function):
             g_b = torch.empty_like(bias) if bias is not None and need[4] else None
             g_ux = torch.empty_like(ux) if ux is not None and need[5] else None
             g_uc = torch.empty_like(uc) if uc is not None and need[6] else None
-            native.check(eng.L.rnc_nconv2d_bwd(_ptr(data), _ptr(conf), _ptr(weight), _ptr(bias), _ptr(y), _ptr(c),
-                                               _ptr(gy.contiguous()) if gy is not None else None,
-                                               _ptr(gc.contiguous()) if gc is not None else None, N, Cin, Cout, H, W, kh, kw, ctx.eps,
-                                               _ptr(ux), _ptr(uc), Cup, Hup, Wup, _ptr(g_data), _ptr(g_conf), _ptr(g_ux), _ptr(g_uc),
-                                               _ptr(g_w), _ptr(g_b), _ptr(ws), ws.numel() * 8, _stream()), "nconv2d_bwd")
+            rnc.nconv2d_bwd(data, conf, weight, bias, y, c, gy.contiguous() if gy is not None else None,
+                            gc.contiguous() if gc is not None else None, N, Cin, Cout, H, W, kh, kw, ctx.eps, ux, uc, Cup, Hup, Wup,
+                            g_data, g_conf, g_ux, g_uc, g_w, g_b, ws, ws.numel() * 8)
         return g_data, g_conf, g_w if need[2] else None, None, g_b, g_ux, g_uc
 
 
@@ -416,9 +408,8 @@ class NConvPoolFn(torch.autograd.Function):
         if g_data is None and g_conf is None:
             return None, None, None
         with torch.cuda.device(idx.device):
-            native.check(native.lib().rnc_nconv_pool2_bwd(_ptr(idx), _ptr(gx.contiguous()) if gx is not None else None,
-                                                          _ptr(gc.contiguous()) if gc is not None else None, N, C, H, W,
-                                                          _ptr(g_data), _ptr(g_conf), _stream()), "nconv_pool2_bwd")
+            rnc.nconv_pool2_bwd(idx, gx.contiguous() if gx is not None else None, gc.contiguous() if gc is not None else None,
+                                N, C, H, W, g_data, g_conf)
         return g_data, g_conf, None
 
 
@@ -543,13 +534,12 @@ class NcupChainFn(torch.autograd.Function):
             raise ValueError("NcupChainFn: x_lowres and conf must both be [B,2,H4,W4]")
         if tuple(tuple(w.shape) for w in (w1, w2, w3, w4)) != NcupChainFn.SHAPES:
             raise ValueError(f"NcupChainFn: weights must have shapes {NcupChainFn.SHAPES}")
-        eng = engine_for(x_lowres.device)
+        _require_cuda(x_lowres)
         x_lowres, conf = x_lowres.detach().float().contiguous(), conf.detach().float().contiguous()
         wts = torch.cat([w.detach().float().reshape(-1) for w in (w1, w2, w3, w4)])
         B, _, H4, W4 = x_lowres.shape
         out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
-        native.check(eng.L.rnc_ncup_train_fwd(_ptr(x_lowres), _ptr(conf), _ptr(wts), B, H4, W4, float(out_scale), _ptr(out),
-                                              _stream()), "ncup_train_fwd")
+        rnc.ncup_train_fwd(x_lowres, conf, wts, B, H4, W4, float(out_scale), out)
         ctx.save_for_backward(x_lowres, conf, wts)
         ctx.out_scale = float(out_scale)
         return out
@@ -557,7 +547,6 @@ class NcupChainFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_out):
         x_lowres, conf, wts = ctx.saved_tensors
-        eng = engine_for(x_lowres.device)
         B, _, H4, W4 = x_lowres.shape
         need_w = any(ctx.needs_input_grad[2:6])
         with torch.cuda.device(x_lowres.device):
@@ -567,13 +556,11 @@ class NcupChainFn(torch.autograd.Function):
             g_w = ws = None
             if need_w:
                 g_w = torch.empty(224, dtype=torch.float32, device=x_lowres.device)
-                nbytes = eng.L.rnc_ncup_bwd_workspace_bytes(B, H4, W4)
+                nbytes = rnc.ncup_bwd_workspace_bytes(B, H4, W4)
                 ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=x_lowres.device)
             if g_x is None and g_c is None and g_w is None:
                 return (None,) * 7
-            native.check(eng.L.rnc_ncup_bwd(_ptr(x_lowres), _ptr(conf), _ptr(wts), B, H4, W4, ctx.out_scale, _ptr(g_out), _ptr(g_x),
-                                            _ptr(g_c), _ptr(g_w), _ptr(ws), ws.numel() * 8 if ws is not None else 0, _stream()),
-                         "ncup_bwd")
+            rnc.ncup_bwd(x_lowres, conf, wts, B, H4, W4, ctx.out_scale, g_out, g_x, g_c, g_w, ws, ws.numel() * 8 if ws is not None else 0)
         gws = [None] * 4
         if g_w is not None:
             off = 0

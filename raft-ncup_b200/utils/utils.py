@@ -1,7 +1,5 @@
 """Drop-in for `core/utils/utils.py`: InputPadder, forward_interpolate, coords_grid, upflow8 — the host-side helpers the
 evaluation loops call around the model (evaluate.py:38-40, 125-129)."""
-import ctypes as C
-
 import torch
 import torch.nn.functional as F
 
@@ -31,8 +29,8 @@ def forward_interpolate(flow):
     """utils.py:28-56 — warm-start initialisation for the next frame: flow [2,H,W] (or [B,2,H,W]) on a CUDA device.
     The reference round-trips through scipy on the CPU; this runs librnc's exact nearest-sample kernel on the GPU and
     returns a tensor on the input's device (the reference returns a CPU tensor that its caller moves back with .cuda())."""
-    from rnc import native
     from rnc.engine import _require_cuda
+    from rnc.native import rnc
     _require_cuda(flow)
     squeeze = flow.dim() == 3
     f = (flow[None] if squeeze else flow).detach().float().contiguous()
@@ -40,16 +38,15 @@ def forward_interpolate(flow):
     if two != 2:
         raise ValueError("flow must be [2,H,W] or [B,2,H,W]")
     out = torch.empty_like(f)
-    native.check(native.lib().rnc_forward_interpolate_fwd(C.c_void_p(f.data_ptr()), B, H, W, C.c_void_p(out.data_ptr()),
-                                                         C.c_void_p(torch.cuda.current_stream().cuda_stream)), "forward_interpolate")
+    rnc.forward_interpolate_fwd(f, B, H, W, out)
     return out[0] if squeeze else out
 
 
 def bilinear_sampler(img, coords, mode="bilinear", mask=False):
     """utils.py:59-73 — grid_sample(align_corners=True) with pixel coordinates: img [N,C,H,W], coords [N,h,w,2] -> [N,C,h,w]
     (and, with mask=True, the in-bounds mask [N,h,w,1]).  Runs librnc's sampler kernel; zero padding outside the image."""
-    from rnc import native
     from rnc.engine import _require_cuda
+    from rnc.native import rnc
     if mode != "bilinear":
         raise NotImplementedError("only bilinear sampling is built (the reference never passes another mode)")
     dev = _require_cuda(img, coords)
@@ -60,10 +57,7 @@ def bilinear_sampler(img, coords, mode="bilinear", mask=False):
     with torch.cuda.device(dev):
         out = torch.empty(N, Cc, h, w, dtype=torch.float32, device=dev)
         m = torch.empty(N, h, w, 1, dtype=torch.float32, device=dev) if mask else None
-        native.check(native.lib().rnc_bilinear_sample_fwd(
-            C.c_void_p(img.detach().float().contiguous().data_ptr()), C.c_void_p(coords.detach().float().contiguous().data_ptr()),
-            N, Cc, H, W, h, w, C.c_void_p(out.data_ptr()), C.c_void_p(m.data_ptr() if mask else 0),
-            C.c_void_p(torch.cuda.current_stream().cuda_stream)), "bilinear_sampler")
+        rnc.bilinear_sample_fwd(img.detach().float().contiguous(), coords.detach().float().contiguous(), N, Cc, H, W, h, w, out, m)
     return (out, m) if mask else out
 
 

@@ -102,25 +102,22 @@ class _Recorder:
         return fn
 
 
-class _Eng:
-    def __init__(self):
-        self.L = _Recorder()
-
-
 @pytest.mark.parametrize("on", [False, True])
-def test_training_dispatch_follows_the_flag(on, monkeypatch, request):
+def test_training_dispatch_follows_the_flag_at_the_binding(on, monkeypatch, request):
     import rnc.train as tr
+    from rnc import native
     if on:
         request.getfixturevalue("det")
-    monkeypatch.setattr(tr, "_stream", lambda: None)
+    rec = _Recorder()
+    monkeypatch.setattr(native, "_lib", rec)
+    monkeypatch.setattr(native, "stream", lambda: None)
     assert tr.deterministic() == on
-    eng = _Eng()
-    gw, gb = tr._wgrad(eng, torch.zeros(1, 4, 4, 8), torch.zeros(1, 4, 4, 16), 16, 3, 3, 1, True)
+    gw, gb = tr._wgrad(torch.zeros(1, 4, 4, 8), torch.zeros(1, 4, 4, 16), 16, 3, 3, 1, True)
     assert gw.shape == (9, 8, 16) and gb.shape == (16,)
-    tr._lookup_bwd(eng, torch.zeros(1, 8, 8, 256), torch.zeros(100), torch.zeros(1, 2, 8, 8), torch.zeros(1, 8, 8, 324), 4)
+    tr._lookup_bwd(torch.zeros(1, 8, 8, 256), torch.zeros(100), torch.zeros(1, 2, 8, 8), torch.zeros(1, 8, 8, 324), 4)
     want = ["rnc_conv2d_cl_wgrad_workspace_bytes", "rnc_conv2d_cl_wgrad_det"]          # one weight gradient, both modes
     want += ["rnc_corr_lookup_bwd_workspace_bytes", "rnc_corr_lookup_bwd_det"] if on else ["rnc_corr_lookup_bwd"]
-    assert eng.L.calls == want
+    assert rec.calls == want
 
 
 def _float_atomics(tmp_path, src):

@@ -1,7 +1,5 @@
 """Encoders (core/extractor.py) on the tensor-core path: stem kernel, instance norm, and the full fnet/cnet against the
 reference's own outputs (tests/golden: fmap1, fmap2, net0, inp of BASELINE configs[0])."""
-import ctypes as C
-
 import pytest
 import torch
 import torch.nn.functional as F
@@ -12,18 +10,9 @@ pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
 
-def S():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def P(t):
-    return C.c_void_p(t.data_ptr() if t is not None else 0)
-
-
 @pytest.mark.parametrize("Hin,Win,relu", [(128, 256, 0), (46, 70, 1), (33, 41, 0)])
 def test_stem_conv_matches_torch(Hin, Win, relu):
     from rnc import native
-    L = native.lib()
     g = torch.Generator().manual_seed(Hin)
     img = torch.rand(2, 3, Hin, Win, generator=g) * 255
     w = torch.randn(64, 3, 7, 7, generator=g) / 12
@@ -37,7 +26,7 @@ def test_stem_conv_matches_torch(Hin, Win, relu):
     lo = torch.zeros_like(hi)
     wp = w.permute(1, 2, 3, 0).reshape(147, 64).contiguous().to(DEV)
     imgd, bd = img.to(DEV), b.to(DEV)
-    native.check(L.rnc_stem_conv7x7s2_fwd(P(imgd), P(wp), P(bd), 2, Hin, Win, relu, P(out), P(hi), P(lo), S()))
+    native.rnc.stem_conv7x7s2_fwd(imgd, wp, bd, 2, Hin, Win, relu, out, hi, lo)
     got = out.view(2, Ho, Wo, 64).permute(0, 3, 1, 2).cpu()
     assert (got - ref).abs().max() < 2e-5
     assert ((hi.float() + lo.float()) - out).abs().max() < 1e-6
@@ -74,9 +63,9 @@ def test_window_stem_matches_torch(Hin, Win, inst):
     enc = enc.to(DEV)
     pk = PackedEncoder(enc)
     bufs = EncoderBuffers(DEV, N, Hin, Win)
-    L, E = native.lib(), native
+    E = native
     imgd = img.to(DEV)
-    native.check(L.rnc_stem_window_prep(P(imgd), N, Hin, Win, bufs.pitch, P(bufs.img_hi), P(bufs.img_lo), S()))
+    native.rnc.stem_window_prep(imgd, N, Hin, Win, bufs.pitch, bufs.img_hi, bufs.img_lo)
     plane = (bufs.img_hi.float() + bufs.img_lo.float())[:N * Hin * bufs.pitch].view(N, Hin, bufs.pitch, 4).cpu()
     want = torch.zeros(N, Hin, bufs.pitch, 4, dtype=torch.float64)
     want[:, :, 3:3 + Win, :3] = x.permute(0, 2, 3, 1)
@@ -102,7 +91,6 @@ def test_window_stem_matches_torch(Hin, Win, inst):
 @pytest.mark.parametrize("Cc,mode", [(64, 1), (96, 0), (128, 2)])
 def test_instance_norm_matches_torch(Cc, mode):
     from rnc import native
-    L = native.lib()
     g = torch.Generator().manual_seed(Cc)
     N, Pn = 3, 1000
     x = torch.randn(N, Pn, Cc, generator=g) * 3 + 1.5
@@ -118,8 +106,8 @@ def test_instance_norm_matches_torch(Cc, mode):
     out = torch.zeros(N, Pn, Cc, device=DEV)
     hi = torch.zeros(N, Pn, Cc, dtype=torch.float16, device=DEV)
     lo = torch.zeros_like(hi)
-    native.check(L.rnc_instnorm_stats(P(xd), N, Pn, Cc, 1e-5, P(stats), P(mr), S()))
-    native.check(L.rnc_instnorm_apply(P(xd), P(mr), P(rd), N, Pn, Cc, mode, P(out), P(hi), P(lo), S()))
+    native.rnc.instnorm_stats(xd, N, Pn, Cc, 1e-5, stats, mr)
+    native.rnc.instnorm_apply(xd, mr, rd, N, Pn, Cc, mode, out, hi, lo)
     assert (out.cpu() - ref).abs().max() < 2e-5
     assert ((hi.float() + lo.float()) - out).abs().max() < 1e-6
 

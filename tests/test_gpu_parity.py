@@ -1,8 +1,6 @@
 """GPU parity: every kernel is called through the C ABI (librnc.so) and compared with the CPU oracle and with the golden
 fixtures generated from the unmodified reference.  Floating point -> tolerances are stated per test; the end-to-end
 bar is the north star's 1e-3 EPE."""
-import ctypes as C
-
 import pytest
 import torch
 import torch.nn.functional as F
@@ -22,14 +20,6 @@ def epe(a, b):
 def eng():
     from rnc.engine import Engine
     return Engine()
-
-
-def stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def P(t):
-    return C.c_void_p(t.data_ptr())
 
 
 # ----------------------------------------------------------------------------- K2: correlation lookup
@@ -177,7 +167,7 @@ def test_ncup_chain_non_multiple_of_tile(sd_ncup):
     pu = eng.packed_upsampler(m.upsampler)
     out = torch.empty(2, 2, 88, 104, device=DEV)
     xd, cd = x.to(DEV), c.to(DEV)
-    native.check(eng.L.rnc_ncup_fwd(P(xd), P(cd), pu.nconv_host, 2, 22, 26, 8.0, P(out), stream()))
+    native.rnc.ncup_fwd(xd, cd, pu.nconv_host, 2, 22, 26, 8.0, out)
     assert (out.cpu() - 8 * ref.view(2, 2, 88, 104)).abs().max() < 1e-4
 
 

@@ -107,11 +107,7 @@ class Recorder:
         self.ws = eng.workspace(torch.device(DEV), B, H8, W8, pk.has_mask, self.ncup)
         self.grid = orc.coords_grid(B, H8, W8).to(DEV).double()
         self.pending = {}
-        proxy = LibProxy(native.lib(), self)
-        monkeypatch.setattr(native, "_lib", proxy)
-        monkeypatch.setattr(eng, "L", proxy)
-        if self.umma:
-            monkeypatch.setattr(eng.encoder(), "L", proxy)      # (created here if needed, so that it never keeps the proxy)
+        monkeypatch.setattr(native, "_lib", LibProxy(native.lib(), self))
         if self.umma:
             orig_uconv = eng.uconv
             monkeypatch.setattr(eng, "uconv", lambda B_, H_, W_, in0, c0, ld0, wt, epi, **kw:
@@ -381,7 +377,8 @@ class Recorder:
         ws, B, H, W = self.ws, self.B, self.H, self.W
         if not self.umma:
             assert torch.equal(cl(ws.f1_cl, B, H, W), args[1]), "rnc_fmap_prepare: fmap1 channel-last copy"
-        L = self.eng.L._lib if isinstance(self.eng.L, LibProxy) else self.eng.L
+        from rnc import native
+        L = native.lib()._lib
         prev = cl(ws.f2_pyr[:B * H * W * 256], B, H, W).double()
         for lvl in range(1, ws.levels):
             o0, o1 = L.rnc_pyramid_offset(B, 256, H, W, lvl), L.rnc_pyramid_offset(B, 256, H, W, lvl + 1)

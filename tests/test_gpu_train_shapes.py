@@ -437,16 +437,10 @@ def test_train_coverage_guard(monkeypatch):
     """The librnc entry points called by one training step of every route above at T3 are exactly TRAIN_COVERAGE's: a kernel
     added to the training step fails here until it has a pointwise check."""
     from rnc import native
-    from rnc.engine import engine_for
     rec = _Names()
     for route in dict.fromkeys(r for r, _ in CASES):
         with monkeypatch.context() as mp:
-            eng = engine_for(DEV)
-            proxy = LibProxy(native.lib(), rec)
-            mp.setattr(native, "_lib", proxy)
-            mp.setattr(eng, "L", proxy)
-            if eng.mode == "umma":
-                mp.setattr(eng.encoder(), "L", proxy)
+            mp.setattr(native, "_lib", LibProxy(native.lib(), rec))
             run_step(mp, route, "T3", capture=False)
     called = rec.called
     missing = set(TRAIN_COVERAGE) - called

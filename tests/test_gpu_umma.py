@@ -28,14 +28,11 @@ def ueng():
 
 def test_split_roundtrip_is_near_exact():
     from rnc import native
-    import ctypes as C
     g = torch.Generator().manual_seed(0)
     x = (torch.randn(1000, 36, generator=g) * torch.logspace(-4, 3, 36)).to(DEV)
     hi = torch.zeros(1000, 40, dtype=torch.float16, device=DEV)
     lo = torch.zeros_like(hi)
-    L = native.lib()
-    s = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    native.check(L.rnc_f32_to_split(C.c_void_p(x.data_ptr()), 36, 36, 1000, C.c_void_p(hi.data_ptr()), C.c_void_p(lo.data_ptr()), 40, 2, s))
+    native.rnc.f32_to_split(x, 36, 36, 1000, hi, lo, 40, 2)
     rec = hi[:, 2:38].float() + lo[:, 2:38].float()
     err = (rec - x).abs()
     assert (err <= x.abs() * 2.0 ** -21 + 6e-8).all()                   # 22 significant bits, absolute floor = half subnormal
@@ -81,7 +78,6 @@ def test_umma_conv_matches_fp32(ueng, cin, cout, kh, kw, act, W):
 def test_umma_conv_fused_instance_norm_statistics(ueng, cout, W):
     """rnc_conv_umma_desc.stats + rnc_instnorm_finalize == InstanceNorm2d statistics of the layer's output
     (extractor.py:128-129): ragged tiles, several images per CTA, accumulate-and-rezero protocol."""
-    import ctypes as C
     from rnc import native
     from rnc.engine_umma import SplitBuf, UmmaWeights
     g = torch.Generator().manual_seed(cout + W)
@@ -99,8 +95,7 @@ def test_umma_conv_fused_instance_norm_statistics(ueng, cout, W):
     for _ in range(2):                                     # second round checks that finalize left the sums zeroed
         ueng.uconv(B, H, W, buf.ptrs(), cin, cin, wt, native.EPI_LINEAR, out_f32=out.data_ptr(), ldo_f32=wt.coutpad,
                    stats=stats.data_ptr())
-        native.check(ueng.L.rnc_instnorm_finalize(C.c_void_p(stats.data_ptr()), B, H * W, cout, 1e-5, C.c_void_p(mr.data_ptr()),
-                                                  C.c_void_p(torch.cuda.current_stream().cuda_stream)), "finalize")
+        native.rnc.instnorm_finalize(stats, B, H * W, cout, 1e-5, mr)
         torch.cuda.synchronize()
         assert stats.abs().max().item() == 0.0
         got = mr.view(B, cout, 2).cpu()
@@ -132,12 +127,11 @@ def test_flow_head_conv2_as_taps_plus_gather(ueng):
     delta = torch.zeros(B, 2, H, W, device=DEV)
     vp = C.c_void_p
     bd = b.to(DEV)
-    native.check(ueng.L.rnc_flow_tap_gather_fwd(vp(taps.data_ptr()), 32, vp(bd.data_ptr()), B, H, W, vp(delta.data_ptr()),
-                                                vp(coords.data_ptr()), vp(torch.cuda.current_stream().cuda_stream)), "gather")
+    native.rnc.flow_tap_gather_fwd(taps, 32, bd, B, H, W, delta, coords)
     torch.cuda.synchronize()
     assert (delta.cpu() - ref).abs().max() < 2e-5 * max(1.0, ref.abs().max().item())
     assert (coords - (c0 + delta)).abs().max().item() < 1e-6
-    assert ueng.L.rnc_flow_tap_gather_fwd(vp(taps.data_ptr()), 16, vp(0), B, H, W, None, vp(coords.data_ptr()), None) != 0
+    assert native.lib().rnc_flow_tap_gather_fwd(vp(taps.data_ptr()), 16, vp(0), B, H, W, None, vp(coords.data_ptr()), None) != 0
 
 
 @pytest.mark.parametrize("cin,cout,kh,kw,B,H,W", [(128, 256, 3, 3, 3, 9, 128), (384, 128, 5, 1, 1, 17, 40), (64, 64, 3, 3, 2, 13, 150)])

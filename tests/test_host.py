@@ -73,6 +73,53 @@ def test_cabi_exports_every_declared_symbol():
     assert L.rnc_conv_umma_tiles(0, 3, 1, 1, 16, 32, 0) == 0
 
 
+def test_binding_appends_the_stream_where_the_header_takes_one(monkeypatch):
+    """native.rnc appends the current stream to exactly the entry points whose last parameter is the stream, and passes
+    every other argument through to the handle native.lib() returns at call time."""
+    from rnc import native
+    hdr = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "rnc.h")).read(), flags=re.S)
+    streamed = {m.group(1) for m in re.finditer(r"\b(rnc_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", hdr)
+                if re.search(r"void\s*\*\s*stream\s*$", m.group(2))}
+    assert len(streamed) > 40
+    got = {}
+
+    class Handle:
+        def __getattr__(self, name):
+            return lambda *a: got.__setitem__(name, a) or 0
+
+    monkeypatch.setattr(native, "_lib", Handle())
+    monkeypatch.setattr(native, "stream", lambda: "stream")
+    for name, (_, argtypes) in native.SIGNATURES.items():
+        n = len(argtypes) - (name in streamed)
+        getattr(native.rnc, name[4:])(*range(n))
+        assert got[name] == tuple(range(n)) + (("stream",) if name in streamed else ()), name
+
+
+def test_binding_raises_naming_the_entry_point(monkeypatch):
+    """A failing status raised through native.rnc names the entry point; tensors arrive as their data_ptr(), views with
+    their offset, None as NULL."""
+    from rnc import native
+
+    class FailingHandle:
+        def rnc_status_string(self, status):
+            return b"bad shape"
+
+        def rnc_nchw_to_cl(self, *args):
+            self.args = args
+            return -1
+
+    fake = FailingHandle()
+    monkeypatch.setattr(native, "_lib", fake)
+    monkeypatch.setattr(native, "stream", lambda: 7)
+    x = torch.zeros(4, 8)
+    with pytest.raises(ValueError, match="rnc_nchw_to_cl: bad shape"):
+        native.rnc.nchw_to_cl(x, 1, 8, 2, 2, x[:, 4:], 8, 0)
+    assert fake.args == (x.data_ptr(), 1, 8, 2, 2, x.data_ptr() + 16, 8, 0, 7)
+    with pytest.raises(ValueError, match="rnc_nchw_to_cl"):
+        native.rnc.nchw_to_cl(None, 1, 8, 2, 2, x, 8, 0)
+    assert fake.args[0] is None
+
+
 def test_conv_desc_layout_matches_header():
     from rnc.native import ConvDesc
     # 4 pointer/int/int groups, then pointers and ints in header order; no implicit reordering

@@ -91,26 +91,24 @@ def bench_steps(reps):
 
 
 def bench_ops(reps, B, H, W):
-    from rnc import native
-    from rnc.engine import _ptr, _stream
-    L = native.lib()
+    from rnc.native import rnc
     res = {}
     H8, W8 = H // 8, W // 8
     f1 = torch.randn(B, H8, W8, 256, device=DEV)
-    pyr = torch.randn(L.rnc_pyramid_offset(B, 256, H8, W8, 4), device=DEV)
+    pyr = torch.randn(rnc.pyramid_offset(B, 256, H8, W8, 4), device=DEV)
     ys, xs = torch.meshgrid(torch.arange(H8, device=DEV), torch.arange(W8, device=DEV), indexing="ij")
     coords = (torch.stack([xs, ys]).float()[None] + 4 * torch.randn(B, 2, H8, W8, device=DEV)).contiguous()
     g_out = torch.randn(B, H8, W8, 324, device=DEV)
     g1, g2 = torch.empty_like(f1), torch.empty_like(pyr)
-    ws = torch.empty(L.rnc_corr_lookup_bwd_workspace_bytes(B, H8, W8, 4) // 4 + 4, device=DEV)
-    args = (_ptr(f1), _ptr(pyr), _ptr(coords), _ptr(g_out), 324, B, 256, H8, W8, 4, 4, _ptr(g1), _ptr(g2))
+    ws = torch.empty(rnc.corr_lookup_bwd_workspace_bytes(B, H8, W8, 4) // 4 + 4, device=DEV)
+    args = (f1, pyr, coords, g_out, 324, B, 256, H8, W8, 4, 4, g1, g2)
 
     def atomic():
         g2.zero_()
-        native.check(L.rnc_corr_lookup_bwd(*args, _stream()))
+        rnc.corr_lookup_bwd(*args)
 
     def det():
-        native.check(L.rnc_corr_lookup_bwd_det(*args, _ptr(ws), ws.numel() * 4, _stream()))
+        rnc.corr_lookup_bwd_det(*args, ws, ws.numel() * 4)
     res["lookup_bwd"] = alternate(atomic, det, reps)
     return res
 
