@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 15) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 16) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -350,6 +350,25 @@ size_t rnc_ncup_bwd_workspace_bytes(int B, int H4, int W4);
 int rnc_ncup_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4, float out_scale,
                  const float* g_out, float* g_x_lowres, float* g_conf, float* g_weights, void* workspace,
                  size_t workspace_bytes, void* stream);
+
+/* Output confidence of the same chain: the cout of NConvUNet.forward that upsampler.py:168 discards, i.e. nconv_out's
+ * den4 / (W4[0] + W4[1]) with den4 = W4[0]*c3[0] + W4[1]*c3[1] (c3: the decoder's output confidence).  It lies in [0, 1]
+ * and is not multiplied by out_scale.
+ * rnc_ncup_conf_fwd      : rnc_ncup_fwd (host weights) that also writes conf_out NCHW [B][2][4*H4][4*W4]; out is
+ *                          bit-identical to rnc_ncup_fwd's.
+ * rnc_ncup_train_conf_fwd: the same with the weights in device memory (as rnc_ncup_train_fwd); same outputs.
+ * rnc_ncup_conf_bwd      : gradients of L = sum(g_out * out) + sum(g_conf_out * conf_out).  Either upstream gradient may be
+ *                          NULL (not both); with g_conf_out NULL the result is bit-identical to rnc_ncup_bwd.  The extra
+ *                          adjoint enters at the last layer, dL/dc3[k] += g * W4[k] / S4 and dL/dW4[k] += g * (c3[k] / S4 -
+ *                          den4 / S4^2) with S4 = W4[0] + W4[1], and flows through the chain like the flow's.  Same workspace
+ *                          (rnc_ncup_bwd_workspace_bytes), status codes and determinism as rnc_ncup_bwd. */
+int rnc_ncup_conf_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
+                      float out_scale, float* out, float* conf_out, void* stream);
+int rnc_ncup_train_conf_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
+                            float out_scale, float* out, float* conf_out, void* stream);
+int rnc_ncup_conf_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
+                      float out_scale, const float* g_out, const float* g_conf_out, float* g_x_lowres, float* g_conf,
+                      float* g_weights, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * A3  bilinear_sampler  (core/utils/utils.py:59-73) as a standalone operator: grid_sample(align_corners=True, bilinear,

@@ -27,6 +27,9 @@
 //                           kernel computes.  Each CTA owns the lattice samples of its tile (written once, no atomics) and
 //                           writes its weight-gradient partial sums to the workspace; two small kernels reduce them in a
 //                           fixed order in fp64, so gradients are bit-identical across calls.
+// Each has a twin instantiated from the same code with a compile-time flag that also handles nconv_out's output confidence
+// den4 / sum(W4): ncup_fused_conf_kernel and ncup_train_fwd_conf_kernel write it (rnc_ncup_conf_fwd, rnc_ncup_train_conf_fwd),
+// ncup_conf_bwd_kernel adds its adjoint (rnc_ncup_conf_bwd).  The flag off compiles to the plain kernels.
 #include "rnc_common.cuh"
 
 namespace rnc {
@@ -208,9 +211,12 @@ __device__ __forceinline__ float2 stage4_nd(float2 a, float2 b, const NcupWeight
   return make_float2(num, den);
 }
 
-// The whole forward of one 30x30 output tile.
+// The whole forward of one 30x30 output tile.  kConf: also write nconv_out's output confidence den4 / sum(W4) to conf_out
+// (same layout as out, no out_scale); without it the instantiation is the plain forward.
+template <bool kConf>
 __device__ __forceinline__ void ncup_forward_tile(const float* __restrict__ x_lowres, const float* __restrict__ conf,
-                                                  const NcupWeights& w, int H4, int W4, float out_scale, float* __restrict__ out) {
+                                                  const NcupWeights& w, int H4, int W4, float out_scale, float* __restrict__ out,
+                                                  float* __restrict__ conf_out) {
   __shared__ float lx[LT][LT], lc[LT][LT];                  // lattice data (flow) and confidence
   __shared__ __align__(16) float2 s1[2][R1][P1];            // stage 1: (data*conf, conf) per channel
   __shared__ __align__(16) float2 s2[2][R2][P2];            // stage 2
@@ -231,24 +237,36 @@ __device__ __forceinline__ void ncup_forward_tile(const float* __restrict__ x_lo
   stage3<R2, P2, NT>(s2, w, [&](int oy, int g, const float2 (&acc)[2][2]) {
     const int y = ty0 + oy;
     if (y >= H) return;
-    float res[2];
+    float res[2], cres[2];
 #pragma unroll
     for (int x = 0; x < 2; ++x) {
       const float2 a = nconv_out_pair(acc[x][0], w.inv_s3[0]), b = nconv_out_pair(acc[x][1], w.inv_s3[1]);   // (y*c, c) pairs
       const float2 nd = stage4_nd(a, b, w);
       res[x] = out_scale * (nd.x / (nd.y + kEps));
+      if constexpr (kConf) cres[x] = nd.y / (w.w4[0] + w.w4[1]);    // c' = den / sum(W), nconv_modules.py:186-190
     }
     const int x0 = tx0 + 2 * g;
-    float* op = out + ((size_t)plane * H + y) * W + x0;
-    if (x0 + 1 < W) *reinterpret_cast<float2*>(op) = make_float2(res[0], res[1]);     // W = 4*W4 and x0 are even: 8-byte aligned
-    else if (x0 < W) op[0] = res[0];
+    const size_t o = ((size_t)plane * H + y) * W + x0;
+    if (x0 + 1 < W) {                                         // W = 4*W4 and x0 are even: 8-byte aligned
+      *reinterpret_cast<float2*>(out + o) = make_float2(res[0], res[1]);
+      if constexpr (kConf) *reinterpret_cast<float2*>(conf_out + o) = make_float2(cres[0], cres[1]);
+    } else if (x0 < W) {
+      out[o] = res[0];
+      if constexpr (kConf) conf_out[o] = cres[0];
+    }
   });
 }
 
 __global__ void __launch_bounds__(kThreads)
 ncup_fused_kernel(const float* __restrict__ x_lowres, const float* __restrict__ conf, const __grid_constant__ NcupWeights w,
                   int H4, int W4, float out_scale, float* __restrict__ out) {
-  ncup_forward_tile(x_lowres, conf, w, H4, W4, out_scale, out);
+  ncup_forward_tile<false>(x_lowres, conf, w, H4, W4, out_scale, out, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads)
+ncup_fused_conf_kernel(const float* __restrict__ x_lowres, const float* __restrict__ conf, const __grid_constant__ NcupWeights w,
+                       int H4, int W4, float out_scale, float* __restrict__ out, float* __restrict__ conf_out) {
+  ncup_forward_tile<true>(x_lowres, conf, w, H4, W4, out_scale, out, conf_out);
 }
 
 // The 224 positive weights (state_dict order) -> NcupWeights, with the same fp32 arithmetic as the host packing of
@@ -287,7 +305,16 @@ ncup_train_fwd_kernel(const float* __restrict__ x_lowres, const float* __restric
   __shared__ NcupWeights w;
   load_weights(wdev, w);
   __syncthreads();
-  ncup_forward_tile(x_lowres, conf, w, H4, W4, out_scale, out);
+  ncup_forward_tile<false>(x_lowres, conf, w, H4, W4, out_scale, out, nullptr);
+}
+
+__global__ void __launch_bounds__(kThreads)
+ncup_train_fwd_conf_kernel(const float* __restrict__ x_lowres, const float* __restrict__ conf, const float* __restrict__ wdev,
+                           int H4, int W4, float out_scale, float* __restrict__ out, float* __restrict__ conf_out) {
+  __shared__ NcupWeights w;
+  load_weights(wdev, w);
+  __syncthreads();
+  ncup_forward_tile<true>(x_lowres, conf, w, H4, W4, out_scale, out, conf_out);
 }
 
 // ------------------------------------------------------------------------------------------------------------------ backward
@@ -386,10 +413,22 @@ __device__ __forceinline__ void wgrad(const float2 (&ab)[2][RA][PA], int oa, con
   __syncthreads();
 }
 
-__global__ void __launch_bounds__(kThreads)
-ncup_bwd_kernel(const float* __restrict__ x_lowres, const float* __restrict__ conf, const float* __restrict__ wdev, int H4, int W4,
-                float out_scale, const float* __restrict__ g_out, float* __restrict__ g_x, float* __restrict__ g_conf,
-                double* __restrict__ partials) {
+// dL/dc3[k] of the last layer: the flow's term gy, plus t4 * W4[k] from the confidence when kConf
+template <bool kConf>
+__device__ __forceinline__ float conf_adjoint(float gy, float t4, float w4) {
+  if constexpr (kConf) return fmaf(t4, w4, gy);
+  return gy;
+}
+
+// kConf: the loss also has the term sum(g_conf_out * conf_out), conf_out = den4 / S4 with S4 = W4[0] + W4[1], and either
+// upstream gradient may be NULL.  It enters at layer 4: dL/dc3[k] += g * W4[k] / S4 (the den component of pair k, from where
+// the existing chain carries it down) and dL/dW4[k] += g * (c3[k] - den4 / S4) / S4.  Without it the instantiation is the
+// plain backward.
+template <bool kConf>
+__device__ __forceinline__ void ncup_bwd_tile(const float* __restrict__ x_lowres, const float* __restrict__ conf,
+                                              const float* __restrict__ wdev, int H4, int W4, float out_scale,
+                                              const float* __restrict__ g_out, const float* __restrict__ g_conf_out,
+                                              float* __restrict__ g_x, float* __restrict__ g_conf, double* __restrict__ partials) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   BwdSmem& S = *reinterpret_cast<BwdSmem*>(smem_raw);
   const NcupWeights& w = S.w;
@@ -418,6 +457,7 @@ ncup_bwd_kernel(const float* __restrict__ x_lowres, const float* __restrict__ co
 
   // ---- layer 4 and layer 3 on R+5: (a3, b3) replace (num3, den3)
   float gw4[2] = {0.f, 0.f}, gs3[2] = {0.f, 0.f};
+  [[maybe_unused]] const float inv_s4 = kConf ? 1.0f / (w.w4[0] + w.w4[1]) : 0.f;
   for (int idx = tid; idx < RB3 * RB3; idx += kThreads) {
     const int ry = idx / RB3, rx = idx - ry * RB3;
     const int y = ty0 - 5 + ry, x = tx0 - 5 + rx;
@@ -430,14 +470,21 @@ ncup_bwd_kernel(const float* __restrict__ x_lowres, const float* __restrict__ co
     const float2 pa = nconv_out_pair(n0, w.inv_s3[0]), pb = nconv_out_pair(n1, w.inv_s3[1]);
     const float2 nd4 = stage4_nd(pa, pb, w);
     const float D4 = nd4.y + kEps;
-    const float a4 = g_out[((size_t)plane * H + y) * W + x] * out_scale / D4;
+    const size_t gi = ((size_t)plane * H + y) * W + x;
+    const float a4 = (kConf && g_out == nullptr ? 0.f : g_out[gi]) * out_scale / D4;
     const float b4 = -a4 * (nd4.x / D4);
+    [[maybe_unused]] const float t4 = kConf && g_conf_out != nullptr ? g_conf_out[gi] * inv_s4 : 0.f;    // g / S4
     float2 ab0, ab1;
-    const float s0 = pair_bwd(a4 * w.w4[0], b4 * w.w4[0], n0, w.inv_s3[0], ab0);
-    const float s1 = pair_bwd(a4 * w.w4[1], b4 * w.w4[1], n1, w.inv_s3[1], ab1);
+    const float s0 = pair_bwd(a4 * w.w4[0], conf_adjoint<kConf>(b4 * w.w4[0], t4, w.w4[0]), n0, w.inv_s3[0], ab0);
+    const float s1 = pair_bwd(a4 * w.w4[1], conf_adjoint<kConf>(b4 * w.w4[1], t4, w.w4[1]), n1, w.inv_s3[1], ab1);
     if (own) {
       gw4[0] = fmaf(a4, pa.x, fmaf(b4, pa.y, gw4[0]));
       gw4[1] = fmaf(a4, pb.x, fmaf(b4, pb.y, gw4[1]));
+      if constexpr (kConf) {
+        const float c4 = nd4.y * inv_s4;
+        gw4[0] = fmaf(t4, pa.y - c4, gw4[0]);
+        gw4[1] = fmaf(t4, pb.y - c4, gw4[1]);
+      }
       gs3[0] += s0;
       gs3[1] += s1;
     }
@@ -560,6 +607,20 @@ ncup_bwd_kernel(const float* __restrict__ x_lowres, const float* __restrict__ co
   for (int k = tid; k < kNPart; k += kThreads) dst[k] = S.part[k];
 }
 
+__global__ void __launch_bounds__(kThreads)
+ncup_bwd_kernel(const float* __restrict__ x_lowres, const float* __restrict__ conf, const float* __restrict__ wdev, int H4, int W4,
+                float out_scale, const float* __restrict__ g_out, float* __restrict__ g_x, float* __restrict__ g_conf,
+                double* __restrict__ partials) {
+  ncup_bwd_tile<false>(x_lowres, conf, wdev, H4, W4, out_scale, g_out, nullptr, g_x, g_conf, partials);
+}
+
+__global__ void __launch_bounds__(kThreads)
+ncup_conf_bwd_kernel(const float* __restrict__ x_lowres, const float* __restrict__ conf, const float* __restrict__ wdev, int H4,
+                     int W4, float out_scale, const float* __restrict__ g_out, const float* __restrict__ g_conf_out,
+                     float* __restrict__ g_x, float* __restrict__ g_conf, double* __restrict__ partials) {
+  ncup_bwd_tile<true>(x_lowres, conf, wdev, H4, W4, out_scale, g_out, g_conf_out, g_x, g_conf, partials);
+}
+
 // Fixed-order fp64 sum of the per-CTA partials: block k reduces column k
 __global__ void __launch_bounds__(kThreads)
 ncup_bwd_reduce_kernel(const double* __restrict__ partials, int nblocks, double* __restrict__ sums) {
@@ -613,11 +674,8 @@ inline dim3 ncup_bwd_grid(int B, int H4, int W4) { return dim3((4 * W4 + NB - 1)
 
 using namespace rnc;
 
-extern "C" int rnc_ncup_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
-                            float out_scale, float* out, void* stream) {
-  if (B <= 0 || H4 <= 0 || W4 <= 0) return RNC_ERR_BAD_SHAPE;
-  if (!x_lowres || !conf || !wts_host || !out) return RNC_ERR_BAD_POINTER;
-  // wts_host: softplus'd weights in state_dict order: nconv_in[2,1,5,5], nconv_x2.0[2,2,5,5], decoder.0[2,4,3,3], nconv_out[1,2,1,1]
+// wts_host: softplus'd weights in state_dict order: nconv_in[2,1,5,5], nconv_x2.0[2,2,5,5], decoder.0[2,4,3,3], nconv_out[1,2,1,1]
+static NcupWeights pack_host_weights(const float* wts_host) {
   NcupWeights w;
   const float* p = wts_host;
   for (int o = 0; o < 2; ++o) {
@@ -643,9 +701,27 @@ extern "C" int rnc_ncup_fwd(const float* x_lowres, const float* conf, const floa
   }
   p += 72;
   w.w4[0] = p[0]; w.w4[1] = p[1];
-  const int H = 4 * H4, W = 4 * W4;
-  dim3 grid((W + NT - 1) / NT, (H + NT - 1) / NT, B * 2);
-  ncup_fused_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(x_lowres, conf, w, H4, W4, out_scale, out);
+  return w;
+}
+
+static dim3 ncup_fwd_grid(int B, int H4, int W4) { return dim3((4 * W4 + NT - 1) / NT, (4 * H4 + NT - 1) / NT, B * 2); }
+
+extern "C" int rnc_ncup_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
+                            float out_scale, float* out, void* stream) {
+  if (B <= 0 || H4 <= 0 || W4 <= 0) return RNC_ERR_BAD_SHAPE;
+  if (!x_lowres || !conf || !wts_host || !out) return RNC_ERR_BAD_POINTER;
+  const NcupWeights w = pack_host_weights(wts_host);
+  ncup_fused_kernel<<<ncup_fwd_grid(B, H4, W4), kThreads, 0, as_stream(stream)>>>(x_lowres, conf, w, H4, W4, out_scale, out);
+  return after_launch();
+}
+
+extern "C" int rnc_ncup_conf_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
+                                 float out_scale, float* out, float* conf_out, void* stream) {
+  if (int st = ncup_check_shape(B, H4, W4)) return st;
+  if (!x_lowres || !conf || !wts_host || !out || !conf_out) return RNC_ERR_BAD_POINTER;
+  const NcupWeights w = pack_host_weights(wts_host);
+  ncup_fused_conf_kernel<<<ncup_fwd_grid(B, H4, W4), kThreads, 0, as_stream(stream)>>>(x_lowres, conf, w, H4, W4, out_scale, out,
+                                                                                       conf_out);
   return after_launch();
 }
 
@@ -656,6 +732,15 @@ extern "C" int rnc_ncup_train_fwd(const float* x_lowres, const float* conf, cons
   const int H = 4 * H4, W = 4 * W4;
   dim3 grid((W + NT - 1) / NT, (H + NT - 1) / NT, B * 2);
   ncup_train_fwd_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, out);
+  return after_launch();
+}
+
+extern "C" int rnc_ncup_train_conf_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
+                                       float out_scale, float* out, float* conf_out, void* stream) {
+  if (int st = ncup_check_shape(B, H4, W4)) return st;
+  if (!x_lowres || !conf || !weights_dev || !out || !conf_out) return RNC_ERR_BAD_POINTER;
+  ncup_train_fwd_conf_kernel<<<ncup_fwd_grid(B, H4, W4), kThreads, 0, as_stream(stream)>>>(x_lowres, conf, weights_dev, H4, W4,
+                                                                                           out_scale, out, conf_out);
   return after_launch();
 }
 
@@ -681,6 +766,31 @@ extern "C" int rnc_ncup_bwd(const float* x_lowres, const float* conf, const floa
   cudaStream_t s = as_stream(stream);
   ncup_bwd_kernel<<<grid, kThreads, sizeof(BwdSmem), s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, g_out, g_x_lowres, g_conf,
                                                           partials);
+  if (!g_weights) return after_launch();
+  ncup_bwd_reduce_kernel<<<kNPart, kThreads, 0, s>>>(partials, nblocks, sums);
+  ncup_bwd_finish_kernel<<<1, kThreads, 0, s>>>(sums, weights_dev, g_weights);
+  return after_launch(3);
+}
+
+extern "C" int rnc_ncup_conf_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
+                                 float out_scale, const float* g_out, const float* g_conf_out, float* g_x_lowres, float* g_conf,
+                                 float* g_weights, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!g_conf_out)                               // no confidence term: exactly rnc_ncup_bwd
+    return rnc_ncup_bwd(x_lowres, conf, weights_dev, B, H4, W4, out_scale, g_out, g_x_lowres, g_conf, g_weights, workspace,
+                        workspace_bytes, stream);
+  if (int st = ncup_check_shape(B, H4, W4)) return st;
+  if (!x_lowres || !conf || !weights_dev || (!g_x_lowres && !g_conf && !g_weights)) return RNC_ERR_BAD_POINTER;
+  if (g_weights && (!workspace || !aligned16(workspace))) return RNC_ERR_BAD_POINTER;
+  if (g_weights && workspace_bytes < rnc_ncup_bwd_workspace_bytes(B, H4, W4)) return RNC_ERR_WORKSPACE;
+  static unsigned long long attr_done = 0;
+  if (int st = ensure_dyn_smem(ncup_conf_bwd_kernel, (int)sizeof(BwdSmem), &attr_done)) return st;
+  const dim3 grid = ncup_bwd_grid(B, H4, W4);
+  const int nblocks = grid.x * grid.y * grid.z;
+  double* partials = g_weights ? static_cast<double*>(workspace) : nullptr;
+  double* sums = g_weights ? partials + (size_t)nblocks * kPartLd : nullptr;
+  cudaStream_t s = as_stream(stream);
+  ncup_conf_bwd_kernel<<<grid, kThreads, sizeof(BwdSmem), s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, g_out, g_conf_out,
+                                                               g_x_lowres, g_conf, partials);
   if (!g_weights) return after_launch();
   ncup_bwd_reduce_kernel<<<kNPart, kThreads, 0, s>>>(partials, nblocks, sums);
   ncup_bwd_finish_kernel<<<1, kThreads, 0, s>>>(sums, weights_dev, g_weights);

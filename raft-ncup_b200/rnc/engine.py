@@ -388,19 +388,21 @@ class Engine:
         return not getattr(model.args, "mixed_precision", False) and os.environ.get("RNC_ENCODER", "umma").lower() == "umma" \
             and self.mode == "umma" and not self.fork_convf1
 
-    def graph_forward(self, model, image1, image2, iters, flow_init):
-        """Second and later forwards with the same signature (shape, iterations, warm start or not, weights) replay a captured
-        graph: inputs are copied into the graph's static buffers, results are returned as fresh copies."""
+    def graph_forward(self, model, image1, image2, iters, flow_init, return_confidence=False):
+        """Second and later forwards with the same signature (shape, iterations, warm start or not, weights, confidence or
+        not) replay a captured graph: inputs are copied into the graph's static buffers, results are returned as fresh
+        copies."""
         B, _, Him, Wim = image1.shape
         if flow_init is not None and tuple(flow_init.shape) != (B, 2, Him // 8, Wim // 8):
             raise ValueError("flow_init must be [N,2,H/8,W/8]")
         # a graph records one mode's kernels: the deterministic mode gets its own (torch.use_deterministic_algorithms)
         key = (type(model).__name__, tuple(image1.shape), iters, flow_init is not None, _param_key(model),
-               torch.are_deterministic_algorithms_enabled())
+               torch.are_deterministic_algorithms_enabled(), return_confidence)
         first = key not in self._graphs
         ent = _lru_get(self._graphs, key, self.MAX_GRAPHS, dict)
-        if first:
-            return model._forward_eager(self, image1, image2, iters, flow_init, True)     # first sight: eager (also warms caches)
+        conf = dict(return_confidence=True) if return_confidence else {}
+        if first:       # first sight: eager (also warms caches)
+            return model._forward_eager(self, image1, image2, iters, flow_init, True, **conf)
         if "graph" not in ent:
             ent["im1"], ent["im2"] = image1.detach().float().clone(), image2.detach().float().clone()
             ent["fi"] = flow_init.detach().float().clone() if flow_init is not None else None
@@ -408,11 +410,11 @@ class Engine:
             side = torch.cuda.Stream(device=image1.device)
             side.wait_stream(cur)
             with torch.cuda.stream(side):                                                  # warm-up on a side stream
-                model._forward_eager(self, ent["im1"], ent["im2"], iters, ent["fi"], True)
+                model._forward_eager(self, ent["im1"], ent["im2"], iters, ent["fi"], True, **conf)
             cur.wait_stream(side)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                ent["out"] = model._forward_eager(self, ent["im1"], ent["im2"], iters, ent["fi"], True)
+                ent["out"] = model._forward_eager(self, ent["im1"], ent["im2"], iters, ent["fi"], True, **conf)
                 ent["net"] = model.update_block.net
             ent["graph"] = g
             # the graph addresses these buffers by pointer: keep them alive even if the LRU caches let go of them
@@ -424,8 +426,7 @@ class Engine:
             ent["fi"].copy_(flow_init)
         ent["graph"].replay()
         model.update_block.net = ent["net"]
-        lo, up = ent["out"]
-        return lo.clone(), up.clone()
+        return tuple(t.clone() for t in ent["out"])
 
     # ------------------------------------------------------------------ single kernels
     def conv(self, B, H, W, in0, c0, ld0, packed, cout, kh, kw, epi, out=None, ldo=0, in1=None, c1=0, ld1=0,
@@ -547,14 +548,14 @@ class Engine:
             rnc.convex_upsample_fwd(flow_low, mask_cl, ldm, ws.B, ws.H8, ws.W8, out)
         return out
 
-    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale):
+    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale, want_conf=False):
         """NConvUpsampler.forward (upsampler.py:143-177) on x_lowres NCHW [B,2,H4,W4] with CL guidance guid at H8 (pixel
-        stride ldg)."""
+        stride ldg); want_conf: (out, output confidence) as ncup_chain."""
         B, H8, W8 = ws.B, ws.H8, ws.W8
         H4, W4 = 2 * H8, 2 * W8
         rnc.ncup_guidance_fwd(x_lowres, guid, ldg, 128, B, H8, W8, ws.gin, 132)
         self.weights_net(pu, B, H4, W4, ws.gin, wnet_buffers(ws, pu), ws.conf)
-        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)
+        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale, want_conf=want_conf)
 
     def weights_net(self, pk, B, H, W, x, bufs, conf):
         """Simple.forward (interp_weights_est.py:39-47) on the exact kernels: x fp32 CL [B*H*W, >= pk.cin0_pad] (zero beyond the
@@ -570,13 +571,20 @@ class Engine:
         self.conv(B, H, W, x.data_ptr(), c, ld, pk.g_out, 2, k, k, native.EPI_SIGMOID, y.data_ptr(), 4, dil=dil)
         rnc.cl_to_nchw(y, 4, 0, B, 2, H, W, conf)
 
-    def ncup_chain(self, ws, pu, x_lowres, conf, out_scale):
+    def ncup_chain(self, ws, pu, x_lowres, conf, out_scale, want_conf=False):
         """Zero-stuffing + NConvUNet + out_scale (upsampler.py:150-177) on x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4]:
         the fused rnc_ncup_fwd for the shipped network, the per-level chain of rnc/nconv_unet.py for any other.  Neither
-        synchronises with the host, so graph capture records either."""
+        synchronises with the host, so graph capture records either.  want_conf: return (out, confidence), the network's
+        output confidence (the cout upsampler.py:168 discards) in the layout of out, without out_scale; the shipped network
+        then runs on rnc_ncup_conf_fwd, whose out is bit-identical to rnc_ncup_fwd's."""
         B, _, H4, W4 = x_lowres.shape
         if pu.unet is None:
             out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
+            if want_conf:
+                cout = torch.empty_like(out)
+                with _Timed(self, "ncup"):
+                    rnc.ncup_conf_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out, cout)
+                return out, cout
             with _Timed(self, "ncup"):
                 rnc.ncup_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out)
             return out
@@ -589,5 +597,7 @@ class Engine:
         with _Timed(self, "ncup"):
             xh.view(B, 2, 4 * H4, 4 * W4)[:, :, 2::4, 2::4] = x_lowres
             ch.view(B, 2, 4 * H4, 4 * W4)[:, :, 2::4, 2::4] = conf
-            out, _ = pu.unet.run(xh, ch, out_scale, bufs)
-        return out.view(B, 2, 4 * H4, 4 * W4)
+            out, cout = pu.unet.run(xh, ch, out_scale, bufs)
+        out = out.view(B, 2, 4 * H4, 4 * W4)
+        # nconv_out's outputs are new tensors (PackedUNet.run), not workspace buffers: the next call does not overwrite them
+        return (out, cout.view(B, 2, 4 * H4, 4 * W4)) if want_conf else out

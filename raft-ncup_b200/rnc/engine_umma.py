@@ -380,7 +380,7 @@ class UmmaEngine(Engine):
     def guidance(self, ws):
         return ws.h, 128
 
-    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale):
+    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale, want_conf=False):
         B, H8, W8 = ws.B, ws.H8, ws.W8
         H4, W4 = 2 * H8, 2 * W8
         rnc.ncup_guidance_split_fwd(x_lowres, guid, ldg, 128, B, H8, W8, ws.gin.hi, ws.gin.lo, GIN_LD)
@@ -400,4 +400,4 @@ class UmmaEngine(Engine):
             (k, dil), y = pu.head, bufs[-1]
             self.uconv(B, H4, W4, x, c, ld, pu.u_out, native.EPI_SIGMOID, out_f32=y.data_ptr(), ldo_f32=32, dil=dil)
             rnc.cl_to_nchw(y, 32, 0, B, 2, H4, W4, ws.conf)
-        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale)
+        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale, want_conf=want_conf)

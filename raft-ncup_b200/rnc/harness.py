@@ -116,10 +116,12 @@ def _stack(frames, device, padder):
 
 
 @torch.no_grad()
-def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda"):
+def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
+                  return_confidence=False):
     """create_sintel_submission (evaluate.py:23-55) over many sequences at batch throughput.  sequences: list of frame lists,
     every frame [3,H,W] of one size.  Yields (seq_index, pair_index, flow): the unpadded [2,H,W] flow_up of every pair, on
-    the device; per sequence the flows equal run_sequence(model, seq, iters, warm_start, mode)'s.
+    the device; per sequence the flows equal run_sequence(model, seq, iters, warm_start, mode)'s.  return_confidence (NCUP
+    model): yields (seq_index, pair_index, flow, confidence), the upsampler's output confidence unpadded like the flow.
 
     Slots run in lockstep (sequence_schedule).  Each step encodes only new frames: a continuing slot's frame 1 is its last
     frame 2, whose fnet features are handed over on the device (rnc.model.SequenceStage).  With warm_start, a slot starts
@@ -129,6 +131,8 @@ def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mo
     for s in sizes:
         if len(s) != 3 or s != sizes[0]:
             raise ValueError(f"all frames of one call must have the same [3,H,W] size: got {sizes[0]} and {s}")
+    if return_confidence and not model.ncup:
+        raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
     steps = sequence_schedule([len(seq) for seq in sequences], batch_size)
     if not steps:
         return
@@ -156,14 +160,18 @@ def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mo
                 ws = eng.WS(dev, len(step), im1.shape[2] // 8, im1.shape[3] // 8, pk.has_mask, model.ncup)
             for j in stage.restart if fi is not None else ():
                 fi[j].copy_(zero)           # cold start: coords0 + 0.0 is exactly coords0, as with flow_init=None
-            flow_low, flow_up = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws)
+            flow_low, flow_up, *conf = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws,
+                                                            return_confidence=return_confidence)
             if warm_start:
                 fi = forward_interpolate(flow_low)
                 if zero is None:
                     zero = torch.zeros_like(fi[0])
         for j, c in enumerate(step):
             if not c.idle:
-                yield c.seq, c.pair, padder.unpad(flow_up[j])
+                if return_confidence:
+                    yield c.seq, c.pair, padder.unpad(flow_up[j]), padder.unpad(conf[0][j])
+                else:
+                    yield c.seq, c.pair, padder.unpad(flow_up[j])
 
 
 def load_checkpoint(model, state):

@@ -2,7 +2,8 @@
 
 Mirrors ``RAFT(nn.Module)`` of core/raft.py:24-143 (convex upsampler) and core/raft_nc_dbl.py:26-173 (NCUP upsampler):
 same ctor Namespace, ``forward(image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False)``, return values
-and state_dict keys.  The iteration loop runs entirely on resident channel-last buffers through librnc.so.
+and state_dict keys.  The iteration loop runs entirely on resident channel-last buffers through librnc.so.  The NCUP model
+also returns the upsampler's output confidence on request (``return_confidence=True``).
 """
 import os
 from collections import OrderedDict
@@ -54,8 +55,14 @@ class _RAFTBase(nn.Module):
     def _needs_grad(self):
         return torch.is_grad_enabled() and any(t.requires_grad for t in module_tensors(self))
 
-    def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False):
-        """Estimate optical flow between a pair of frames (raft_nc_dbl.py:115-173 / raft.py:87-143)."""
+    def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False, return_confidence=False):
+        """Estimate optical flow between a pair of frames (raft_nc_dbl.py:115-173 / raft.py:87-143).
+
+        return_confidence (NCUP model only): also return the NCUP upsampler's per-pixel output confidence in [0, 1], shaped
+        like flow_up ([N,2,H,W], one plane per flow component): (flow_low, flow_up, confidence_up) in test mode, else
+        (flow_predictions, confidence_predictions), one entry per iteration.  The flows are the same as without it."""
+        if return_confidence and not self.ncup:
+            raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
         dev = _require_cuda(image1, image2, flow_init)
         pdev = module_device(self)
         if pdev != dev:
@@ -64,9 +71,9 @@ class _RAFTBase(nn.Module):
         # the kernels launch on `dev`'s current stream whatever device is current in the calling thread (nn.DataParallel
         # worker threads, a model on cuda:1 in a cuda:0 process); one forward at a time per device
         with torch.cuda.device(dev), eng.lock:
-            return self._forward(eng, image1, image2, iters, flow_init, test_mode)
+            return self._forward(eng, image1, image2, iters, flow_init, test_mode, bool(return_confidence))
 
-    def _forward(self, eng, image1, image2, iters, flow_init, test_mode):
+    def _forward(self, eng, image1, image2, iters, flow_init, test_mode, conf=False):
         if iters < 1:
             raise ValueError("iters must be >= 1")
         if hasattr(self, "data_idx"):
@@ -77,18 +84,21 @@ class _RAFTBase(nn.Module):
             # training path (train.py:215): the same graph with autograd, exact-fp32 kernels forward and backward
             if frozen_trunk(self, image1, image2, flow_init):
                 # only the upsampler trains: the trunk runs on the inference engine, the upsampler on autograd
-                return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, upsample=self._upsample_frozen)
+                return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, upsample=self._upsample_frozen,
+                                           return_confidence=conf)
             from .train import raft_forward_train
-            return raft_forward_train(self, image1, image2, iters, flow_init, test_mode)
+            return raft_forward_train(self, image1, image2, iters, flow_init, test_mode, return_confidence=conf)
         if test_mode and eng.graphs_enabled(self):
-            return eng.graph_forward(self, image1, image2, iters, flow_init)
-        return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode)
+            return eng.graph_forward(self, image1, image2, iters, flow_init, return_confidence=conf)
+        return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, return_confidence=conf)
 
-    def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode, upsample=None, encode=None, ws=None):
+    def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode, upsample=None, encode=None, ws=None,
+                       return_confidence=False):
         """The iteration loop on the engine's resident buffers.  upsample(eng, ws, pu) produces each full-resolution prediction
         from the workspace; the default is the inference upsampler (self._upsample on packed weights).  encode(eng, ws, image1,
         image2) fills the feature maps and the GRU state; the default encodes both frames (self._encode).  ws: a workspace the
-        caller owns instead of the engine's shared one of this shape."""
+        caller owns instead of the engine's shared one of this shape.  return_confidence: upsample(eng, ws, pu, True) returns
+        (flow, confidence), and the forward returns the confidences next to the flows (forward's return_confidence)."""
         B, _, Him, Wim = image1.shape
         H8, W8 = Him // 8, Wim // 8
         pk = eng.packed_update(self.update_block)
@@ -109,8 +119,8 @@ class _RAFTBase(nn.Module):
                 raise ValueError("flow_init must be [N,2,H/8,W/8]")
         rnc.coords_init(ws.coords1, fi, B, H8, W8)
 
-        preds = []
-        flow_up = None
+        preds, confs = [], []
+        flow_up = conf_up = None
         for itr in range(iters):
             last = itr == iters - 1
             need_up = last or not test_mode     # inference upsamples once (SURVEY.md finding 9); list mode needs all
@@ -118,12 +128,16 @@ class _RAFTBase(nn.Module):
             eng.lookup_resident(ws)
             eng.update_iter(ws, pk, want_mask=(pk.has_mask and need_up))
             if need_up:
-                flow_up = upsample(eng, ws, pu)
+                if return_confidence:
+                    flow_up, conf_up = upsample(eng, ws, pu, True)
+                    confs.append(conf_up)
+                else:
+                    flow_up = upsample(eng, ws, pu)
                 preds.append(flow_up)
         self.update_block.net = eng.net_nchw(ws)
         if test_mode:
-            return eng.flow_low(ws), flow_up
-        return preds
+            return (eng.flow_low(ws), flow_up, conf_up) if return_confidence else (eng.flow_low(ws), flow_up)
+        return (preds, confs) if return_confidence else preds
 
     def _umma_encoders(self, eng):
         """Do the encoders run on the tensor-core path (else on torch modules: RNC_ENCODER=cudnn, RNC_CONV=ffma, amp)?"""
@@ -195,15 +209,15 @@ class RAFTNcup(_RAFTBase):
         self.upsampler = get_upsampler(2, 128, args)
         self.data_idx = 0
 
-    def _upsample(self, eng, ws, pu):
+    def _upsample(self, eng, ws, pu, want_conf=False):
         rnc.flow_x2_fwd(ws.coords1, ws.B, ws.H8, ws.W8, ws.x4)
         g, gld = eng.guidance(ws)
-        return eng.ncup_from_lowres(ws, pu, ws.x4, g, gld, 8.0)   # `8 *` of raft_nc_dbl.py:161
+        return eng.ncup_from_lowres(ws, pu, ws.x4, g, gld, 8.0, want_conf=want_conf)   # `8 *` of raft_nc_dbl.py:161 (not on the conf)
 
-    def _upsample_frozen(self, eng, ws, pu):
+    def _upsample_frozen(self, eng, ws, pu, want_conf=False):
         """Upsampling step of the frozen-trunk forward: snapshots what the upsampler consumes into tensors of this forward
         (the workspace is overwritten by the next iteration, and autograd's backward runs after the engine lock is released),
-        then runs the differentiable upsampler on them."""
+        then runs the differentiable upsampler on them.  want_conf: (flow, confidence), both differentiable."""
         from .train import ncup_upsampler_frozen
         B, H8, W8 = ws.B, ws.H8, ws.W8
         dev = ws.coords1.device
@@ -214,7 +228,7 @@ class RAFTNcup(_RAFTBase):
         g, gld = eng.guidance(ws)
         gin = torch.empty(B, 2 * H8, 2 * W8, 136, dtype=torch.float32, device=dev)
         rnc.ncup_guidance_fwd(x4, g, gld, 128, B, H8, W8, gin, 136)
-        return ncup_upsampler_frozen(self.upsampler, x4, gin, 8.0)   # `8 *` of raft_nc_dbl.py:161
+        return ncup_upsampler_frozen(self.upsampler, x4, gin, 8.0, want_conf)   # `8 *` of raft_nc_dbl.py:161
 
     def upsample_flow(self, flow_lr, guidance):
         """raft_nc_dbl.py:107-112 (without the caller's x8): nearest x2, then the NConv upsampler."""

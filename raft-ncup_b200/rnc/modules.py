@@ -444,7 +444,9 @@ class Simple(nn.Module):
 
 
 class NConvUpsampler(nn.Module):
-    """Drop-in for core/upsampler.py:75-210.  forward(x_lowres [B,2,h,w], x_guidance [B,128,h/2,w/2]) -> [B,2,4h,4w]."""
+    """Drop-in for core/upsampler.py:75-210.  forward(x_lowres [B,2,h,w], x_guidance [B,128,h/2,w/2]) -> [B,2,4h,4w];
+    with return_confidence=True -> (out, confidence): the interpolation network's output confidence in [0, 1] (the cout
+    upsampler.py:168 discards), shaped like out and not multiplied by out_scale."""
 
     def __init__(self, scale=None, size=None, interpolation_net=None, weights_est_net=None, use_data_for_guidance=True,
                  channels_to_batch=True, use_residuals=False, est_on_high_res=False):
@@ -471,10 +473,10 @@ class NConvUpsampler(nn.Module):
         from .engine import module_device
         return engine_for(device if device is not None else module_device(self))
 
-    def forward(self, x_lowres, x_guidance=None, out_scale=1.0):
+    def forward(self, x_lowres, x_guidance=None, out_scale=1.0, return_confidence=False):
         if _grad_needed(self, x_lowres, x_guidance):
             from .train import ncup_upsampler_train
-            return ncup_upsampler_train(self, x_lowres, x_guidance, out_scale)
+            return ncup_upsampler_train(self, x_lowres, x_guidance, out_scale, return_confidence=bool(return_confidence))
         if any(isinstance(m, nn.BatchNorm2d) and m.training for m in self.weights_est_net.modules()):
             raise NotImplementedError("weights-net BatchNorm with batch statistics needs the training path (enable grad)")
         B, C, h, w = x_lowres.shape
@@ -485,7 +487,8 @@ class NConvUpsampler(nn.Module):
             ws = eng.workspace(x_lowres.device, B, h // 2, w // 2, False, True)
             g_cl = torch.empty(B * (h // 2) * (w // 2), 128, dtype=torch.float32, device=x_lowres.device)
             rnc.nchw_to_cl(x_guidance.float().contiguous(), B, 128, h // 2, w // 2, g_cl, 128, 0)
-            return eng.ncup_from_lowres(ws, pu, x_lowres.float().contiguous(), g_cl, 128, out_scale)
+            return eng.ncup_from_lowres(ws, pu, x_lowres.float().contiguous(), g_cl, 128, out_scale,
+                                        want_conf=bool(return_confidence))
 
 
 def get_upsampler(in_ch, guidance_ch, args):

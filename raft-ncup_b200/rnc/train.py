@@ -14,6 +14,8 @@
                     rnc_ncup_bwd (fused, deterministic); used by the frozen-trunk forward (rnc.model.frozen_trunk), which runs the
                     trunk on the inference engine.  Other configurations run the NConv2dFn / NConvPoolFn chain of
                     rnc/nconv_unet.py there too.
+    NcupChainConfFn NcupChainFn that also returns the chain's output confidence: rnc_ncup_train_conf_fwd / rnc_ncup_conf_bwd;
+                    the frozen-trunk forward uses it when the confidence is requested.
 
 Under torch.use_deterministic_algorithms(True) the lookup backward, which otherwise scatters d fmap2 with floating-point
 atomics, switches to its fixed-order form rnc_corr_lookup_bwd_det (deterministic()); the weight gradient sums in a fixed order
@@ -571,34 +573,94 @@ class NcupChainFn(torch.autograd.Function):
         return (g_x, g_c, *gws, None)
 
 
-def ncup_chain_autograd(net, x_lowres, conf, out_scale=1.0):
-    """The NConvUNet `net` (live path) on zero-stuffed (x_lowres, conf), times out_scale, through NcupChainFn."""
+class NcupChainConfFn(torch.autograd.Function):
+    """NcupChainFn that also returns the chain's output confidence: the same inputs -> (out, conf_out), both NCHW
+    [B,2,4*H4,4*W4]; conf_out = den4 / sum(W4) of nconv_out, without out_scale.  Forward rnc_ncup_train_conf_fwd (out
+    bit-identical to NcupChainFn's), backward rnc_ncup_conf_bwd: when the loss does not use conf_out its gradients are
+    NcupChainFn's, bit for bit."""
+
+    @staticmethod
+    def forward(ctx, x_lowres, conf, w1, w2, w3, w4, out_scale):
+        if x_lowres.dim() != 4 or x_lowres.shape[1] != 2 or conf.shape != x_lowres.shape:
+            raise ValueError("NcupChainConfFn: x_lowres and conf must both be [B,2,H4,W4]")
+        if tuple(tuple(w.shape) for w in (w1, w2, w3, w4)) != NcupChainFn.SHAPES:
+            raise ValueError(f"NcupChainConfFn: weights must have shapes {NcupChainFn.SHAPES}")
+        _require_cuda(x_lowres)
+        x_lowres, conf = x_lowres.detach().float().contiguous(), conf.detach().float().contiguous()
+        wts = torch.cat([w.detach().float().reshape(-1) for w in (w1, w2, w3, w4)])
+        B, _, H4, W4 = x_lowres.shape
+        out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
+        cout = torch.empty_like(out)
+        rnc.ncup_train_conf_fwd(x_lowres, conf, wts, B, H4, W4, float(out_scale), out, cout)
+        ctx.save_for_backward(x_lowres, conf, wts)
+        ctx.out_scale = float(out_scale)
+        ctx.set_materialize_grads(False)        # an unused output's gradient stays None: the kernel skips its term
+        return out, cout
+
+    @staticmethod
+    def backward(ctx, g_out, g_cout):
+        x_lowres, conf, wts = ctx.saved_tensors
+        B, _, H4, W4 = x_lowres.shape
+        need_w = any(ctx.needs_input_grad[2:6])
+        if g_out is None and g_cout is None:
+            return (None,) * 7
+        with torch.cuda.device(x_lowres.device):
+            g_out = g_out.float().contiguous() if g_out is not None else None
+            g_cout = g_cout.float().contiguous() if g_cout is not None else None
+            g_x = torch.empty_like(x_lowres) if ctx.needs_input_grad[0] else None
+            g_c = torch.empty_like(conf) if ctx.needs_input_grad[1] else None
+            g_w = ws = None
+            if need_w:
+                g_w = torch.empty(224, dtype=torch.float32, device=x_lowres.device)
+                nbytes = rnc.ncup_bwd_workspace_bytes(B, H4, W4)
+                ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=x_lowres.device)
+            if g_x is None and g_c is None and g_w is None:
+                return (None,) * 7
+            rnc.ncup_conf_bwd(x_lowres, conf, wts, B, H4, W4, ctx.out_scale, g_out, g_cout, g_x, g_c, g_w, ws,
+                              ws.numel() * 8 if ws is not None else 0)
+        gws = [None] * 4
+        if g_w is not None:
+            off = 0
+            for k, shp in enumerate(NcupChainFn.SHAPES):
+                n = shp[0] * shp[1] * shp[2] * shp[3]
+                gws[k] = g_w[off:off + n].view(shp) if ctx.needs_input_grad[2 + k] else None
+                off += n
+        return (g_x, g_c, *gws, None)
+
+
+def ncup_chain_autograd(net, x_lowres, conf, out_scale=1.0, want_conf=False):
+    """The NConvUNet `net` (live path) on zero-stuffed (x_lowres, conf), times out_scale, through NcupChainFn; want_conf:
+    (out, output confidence) through NcupChainConfFn."""
     _require_cuda(x_lowres, conf)
-    return NcupChainFn.apply(x_lowres, conf, net.nconv_in.weight, net.nconv_x2[0].weight, net.decoder[0].weight,
-                             net.nconv_out.weight, out_scale)
+    fn = NcupChainConfFn if want_conf else NcupChainFn
+    return fn.apply(x_lowres, conf, net.nconv_in.weight, net.nconv_x2[0].weight, net.decoder[0].weight, net.nconv_out.weight,
+                    out_scale)
 
 
-def ncup_upsampler_frozen(up, x4, gin, out_scale=8.0):
+def ncup_upsampler_frozen(up, x4, gin, out_scale=8.0, want_conf=False):
     """NConvUpsampler.forward (upsampler.py:143-177) for a frozen trunk: x4 NCHW [B,2,H4,W4] and the weights-net input gin
     (CL [B,H4,W4,136] = cat(x4, area-resized guidance), zero channels beyond 130; rnc_ncup_guidance_fwd) are the trunk's
-    detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn."""
+    detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn (NcupChainConfFn
+    with want_conf, which returns (out, confidence))."""
     with torch.cuda.device(x4.device):
         conf = simple_cl(up.weights_est_net, gin)
-        return _ncup_chain_train(up.interpolation_net, x4, conf, out_scale, fused=True)
+        return _ncup_chain_train(up.interpolation_net, x4, conf, out_scale, fused=True, want_conf=want_conf)
 
 
-def _ncup_chain_train(net, x_lowres, conf, out_scale, fused):
+def _ncup_chain_train(net, x_lowres, conf, out_scale, fused, want_conf=False):
     """NConvUpsampler.forward after the weights net (upsampler.py:150-177) with autograd: zero-stuffing, the NConvUNet `net`,
     out_scale; x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4].  fused: the shipped network runs on NcupChainFn, with
     out_scale applied inside the kernel; otherwise every network runs the per-layer NConv2dFn chain (the full-training path
-    keeps it: the fused backward rounds the gradients differently)."""
+    keeps it: the fused backward rounds the gradients differently).  want_conf: (out, the network's output confidence in the
+    layout of out, without out_scale)."""
     if fused and is_fused(net):
-        return ncup_chain_autograd(net, x_lowres, conf, out_scale)
+        return ncup_chain_autograd(net, x_lowres, conf, out_scale, want_conf)
     xh, ch = zero_stuff(x_lowres), zero_stuff(conf)
     b, c, oh, ow = xh.shape
-    out, _ = nconv_unet_train(net, xh.view(b * c, 1, oh, ow), ch.view(b * c, 1, oh, ow))
+    out, cout = nconv_unet_train(net, xh.view(b * c, 1, oh, ow), ch.view(b * c, 1, oh, ow))
     out = out.view(b, c, oh, ow)
-    return out * out_scale if out_scale != 1.0 else out
+    out = out * out_scale if out_scale != 1.0 else out
+    return (out, cout.view(b, c, oh, ow)) if want_conf else out
 
 
 def zero_stuff(x, scale=4):
@@ -609,8 +671,9 @@ def zero_stuff(x, scale=4):
     return out
 
 
-def ncup_upsampler_train(up, x_lowres, x_guidance, out_scale=1.0):
-    """NConvUpsampler.forward (upsampler.py:143-177) with autograd: x_lowres NCHW [B,2,h,w], guidance NCHW [B,128,h/2,w/2]."""
+def ncup_upsampler_train(up, x_lowres, x_guidance, out_scale=1.0, return_confidence=False):
+    """NConvUpsampler.forward (upsampler.py:143-177) with autograd: x_lowres NCHW [B,2,h,w], guidance NCHW [B,128,h/2,w/2].
+    return_confidence: (out, output confidence [B,2,4h,4w]), both differentiable."""
     _require_cuda(x_lowres, x_guidance)
     with torch.cuda.device(x_lowres.device):
         # the reference's F.interpolate(mode='area') to twice the size: every area window holds one element, so it is the
@@ -619,7 +682,7 @@ def ncup_upsampler_train(up, x_lowres, x_guidance, out_scale=1.0):
             raise ValueError("ncup_upsampler_train: the guidance must have half the resolution of x_lowres")
         g4 = F.interpolate(x_guidance, scale_factor=2, mode="nearest")
         w4 = simple_cl(up.weights_est_net, to_cl(torch.cat([x_lowres, g4], 1), pad_to=136))     # pitch % 8 == 0: tensor-core layer
-        return _ncup_chain_train(up.interpolation_net, x_lowres, w4, out_scale, fused=False)
+        return _ncup_chain_train(up.interpolation_net, x_lowres, w4, out_scale, fused=False, want_conf=return_confidence)
 
 
 def simple_train(wn, x):
@@ -661,9 +724,10 @@ def convex_upsample_train(flow, mask):
     return up.reshape(n, 2, 8 * h, 8 * w)
 
 
-def raft_forward_train(model, image1, image2, iters=12, flow_init=None, test_mode=False):
+def raft_forward_train(model, image1, image2, iters=12, flow_init=None, test_mode=False, return_confidence=False):
     """RAFT.forward with autograd (raft_nc_dbl.py:115-173 / raft.py:87-143): returns the list of `iters` full-resolution
-    predictions (or (flow_low, flow_up) in test_mode)."""
+    predictions (or (flow_low, flow_up) in test_mode).  return_confidence (NCUP model): also the NCUP output confidences,
+    as (predictions, confidences) or (flow_low, flow_up, confidence_up)."""
     _PACK_CACHE.clear()
     B, _, Him, Wim = image1.shape
     H8, W8 = Him // 8, Wim // 8
@@ -680,7 +744,7 @@ def raft_forward_train(model, image1, image2, iters=12, flow_init=None, test_mod
     coords1 = coords0.clone()
     if flow_init is not None:
         coords1 = coords1 + flow_init
-    preds = []
+    preds, confs = [], []
     ub = model.update_block
     for _ in range(iters):
         coords1 = coords1.detach()                                                  # raft_nc_dbl.py:149
@@ -692,14 +756,19 @@ def raft_forward_train(model, image1, image2, iters=12, flow_init=None, test_mod
         flow_lr = coords1 - coords0
         if model.ncup:
             x4 = F.interpolate(flow_lr, scale_factor=2, mode="nearest")             # raft_nc_dbl.py:110
-            flow_up = 8 * ncup_upsampler_train(model.upsampler, x4, to_nchw(net))   # raft_nc_dbl.py:161
+            if return_confidence:
+                flow_up, conf_up = ncup_upsampler_train(model.upsampler, x4, to_nchw(net), return_confidence=True)
+                flow_up = 8 * flow_up                                               # raft_nc_dbl.py:161 (not on the conf)
+                confs.append(conf_up)
+            else:
+                flow_up = 8 * ncup_upsampler_train(model.upsampler, x4, to_nchw(net))   # raft_nc_dbl.py:161
         else:
             flow_up = convex_upsample_train(flow_lr, to_nchw(mask))
         preds.append(flow_up)
     ub.net = to_nchw(net)
     if test_mode:
-        return coords1 - coords0, preds[-1]
-    return preds
+        return (coords1 - coords0, preds[-1], confs[-1]) if return_confidence else (coords1 - coords0, preds[-1])
+    return (preds, confs) if return_confidence else preds
 
 
 # --------------------------------------------------------------------------------------------- loss / optimiser / step (train.py)
