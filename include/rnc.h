@@ -179,7 +179,8 @@ typedef struct {
   const float* res; int ldres;         /* residual (fp32 CL at output resolution) for RELU_ADD_RELU                 */
   int flags;                           /* RNC_CONV_*                                                                 */
   double* stats;                       /* optional (RNC_EPI_LINEAR + out_f32 only): [B][cout][2] sum / sum of squares of the
-                                        * outputs, ACCUMULATED (caller keeps it zeroed: rnc_instnorm_finalize re-zeroes) */
+                                        * outputs, every term added in fp64, ACCUMULATED (caller keeps it zeroed:
+                                        * rnc_instnorm_finalize re-zeroes) */
   const float* add; int ldadd;         /* optional: fp32 [B*H*W][ldadd] added to the pre-activation (after bias), e.g. the
                                         * hoisted contribution of input channels that do not change between calls */
   int win_pitch;                       /* RNC_CONV_WINDOW (kw = 1, stride 2, c1 = 0): position x of input row y exposes the c0
@@ -230,7 +231,10 @@ int rnc_stem_conv7x7s2_fwd(const float* img, const float* weight, const float* b
  * [64][7 rows][16 px x 4 ch] (zeros for px >= 7 and channel 3): the TMA unit builds the im2col rows, no copy. */
 int rnc_stem_window_prep(const float* img, int N, int Hin, int Win, int pitch_px, void* out_hi, void* out_lo, void* stream);
 /* nn.InstanceNorm2d (no affine, biased variance; extractor.py:28-33,128-129) statistics of x CL fp32 [N][P][C], C <= 128:
- * stats = fp64 scratch [N][C][2]; mean_rstd = [N][C][2] floats (mean, 1/sqrt(var+eps)). */
+ * stats = fp64 scratch [N][C][2]; mean_rstd = [N][C][2] floats (mean, 1/sqrt(var+eps)).  Every route (this one,
+ * rnc_instnorm_stats_det, and rnc_conv_umma_desc.stats + rnc_instnorm_finalize) adds x and x^2 in fp64 from the first term
+ * and takes var = sum(x^2)/P - mean^2 in fp64, so at fnet's sizes (P up to 1.2e5 positions per image)
+ * rstd stays within 1e-6 relative up to |mean|/std = 1e4. */
 int rnc_instnorm_stats(const float* x, int N, int P, int C, float eps, double* stats, float* mean_rstd, void* stream);
 /* Second half of rnc_instnorm_stats when the sums were accumulated elsewhere (rnc_conv_umma_desc.stats): stats [N][C][2]
  * fp64 sums over P positions -> mean_rstd, then stats is zeroed for the next producer. */

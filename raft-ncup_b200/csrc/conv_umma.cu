@@ -393,24 +393,26 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap mA0h, const __grid_constant
           // InstanceNorm statistics of this layer's output (extractor.py:128-129), fused here instead of a pass over the fp32
           // tensor.  The chunk is staged in shared memory for its TMA store anyway ([pixel][32 ch], 128B-swizzled), which is
           // the transposition the reduction over pixels needs: lane = channel walks its column (conflict-free: a row's 32
-          // words are a permutation of the 32 banks), fp32 partial sums over the warp's 32 pixels, accumulated in fp64 per
-          // lane in shared memory across the CTA's tiles and flushed with fp64 atomics when the image changes.  Pixels beyond
+          // words are a permutation of the 32 banks), fp64 sums over the warp's 32 pixels, accumulated in fp64 per lane in
+          // shared memory across the CTA's tiles and flushed with fp64 atomics when the image changes.  Pixels beyond
           // the image are staged as zeros (the TMA store clips them).
           if (!valid) {
 #pragma unroll
             for (int j = 0; j < 32; ++j) v[j] = 0.f;
           }
           store_f32(v, n);                       // stats layers are RNC_EPI_LINEAR with a channel-last fp32 output (host check)
-          float s1 = 0.f, s2 = 0.f;
+          // fp64 from the first term: the variance is sum(x^2)/P - mean^2, which cancels the leading digits when |mean| >> std
+          // (a flat frame's stem output is almost its bias), so fp32 partial sums would turn into the variance's error
+          double s1 = 0.0, s2 = 0.0;
           const int cw = lane >> 2, ce = lane & 3;
 #pragma unroll
           for (int px = 0; px < 32; ++px) {
-            const float x = *reinterpret_cast<const float*>(stg + px * 128 + ((cw ^ (px & 7)) << 4) + ce * 4);
+            const double x = *reinterpret_cast<const float*>(stg + px * 128 + ((cw ^ (px & 7)) << 4) + ce * 4);
             s1 += x;
-            s2 = fmaf(x, x, s2);
+            s2 = fma(x, x, s2);
           }
-          my_acc[cc * 64] += static_cast<double>(s1);
-          my_acc[cc * 64 + 1] += static_cast<double>(s2);
+          my_acc[cc * 64] += s1;
+          my_acc[cc * 64 + 1] += s2;
           return;
         }
         if (EC == EC_GRU_ZR) {

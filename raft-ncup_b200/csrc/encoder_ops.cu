@@ -112,7 +112,11 @@ stem_conv7x7s2_kernel(const float* __restrict__ img, const float* __restrict__ w
 
 // ---------------------------------------------------------------- instance norm statistics: sum / sum of squares in fp64
 constexpr int kInstnormRows = 512;            // positions per CTA
-// x CL fp32 [N][P][C] (C <= 128, C % 4 == 0); stats [N][C][2] doubles, zeroed by the caller
+// x CL fp32 [N][P][C] (C <= 128, C % 4 == 0); stats [N][C][2] doubles, zeroed by the caller.
+// Every x and x^2 (exact in fp64) is added in fp64 from the first term: the variance sum(x^2)/P - mean^2 cancels the leading
+// digits when |mean| >> std (a flat frame puts fnet's norm1 at |mean|/std ~ 2000), and the rounding of fp32 partial sums would
+// become the variance's error.  At fnet's sizes (P up to 1.2e5 positions per image) fp64 keeps rstd within 1e-6 relative
+// up to |mean|/std = 1e4.
 // PARTS: CTA (blockIdx.x, n) writes its sums to stats[((n * gridDim.x + blockIdx.x) * C + c) * 2] instead of adding them
 // (rnc_instnorm_stats_det: instnorm_reduce_kernel adds the CTAs' partials in ascending order).
 template <bool PARTS>
@@ -123,20 +127,14 @@ instnorm_stats_kernel(const float* __restrict__ x, int P, int C, int rows_per_ct
   const int c4 = C >> 2;                         // float4 columns
   const int col = threadIdx.x % c4, rsub = threadIdx.x / c4, nsub = 256 / c4;
   const int r0 = blockIdx.x * rows_per_cta, r1 = min(P, r0 + rows_per_cta);
-  float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
   double ds[4] = {0, 0, 0, 0}, dq[4] = {0, 0, 0, 0};
-  int cnt = 0;
   if (rsub < nsub) {
     for (int r = r0 + rsub; r < r1; r += nsub) {
       const float4 v = *reinterpret_cast<const float4*>(x + ((size_t)n * P + r) * C + col * 4);
-      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-      q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
-      if (++cnt == 32) {                           // flush short fp32 runs into fp64
-        ds[0] += s.x; ds[1] += s.y; ds[2] += s.z; ds[3] += s.w; dq[0] += q.x; dq[1] += q.y; dq[2] += q.z; dq[3] += q.w;
-        s = make_float4(0.f, 0.f, 0.f, 0.f); q = s; cnt = 0;
-      }
+      const double w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { ds[j] += w[j]; dq[j] = fma(w[j], w[j], dq[j]); }
     }
-    ds[0] += s.x; ds[1] += s.y; ds[2] += s.z; ds[3] += s.w; dq[0] += q.x; dq[1] += q.y; dq[2] += q.z; dq[3] += q.w;
   }
   // reduce the nsub row-groups through shared memory (nsub <= 16 for C >= 64; use 8-row chunks)
   double pa = 0, pb = 0;
