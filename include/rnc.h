@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 16) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 17) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -249,8 +249,6 @@ int rnc_instnorm_stats_det(const float* x, int N, int P, int C, float eps, void*
  * extractor.py:48-56); outputs fp32 and/or split halves, all CL [N][P][C]. */
 int rnc_instnorm_apply(const float* x, const float* mean_rstd, const float* res, int N, int P, int C, int mode,
                        float* out_f32, void* out_hi, void* out_lo, void* stream);
-/* relu(a + b) on n fp32 elements -> fp32 (optional) + split halves (block tail when the downsample branch has its own norm). */
-int rnc_add_relu_split(const float* a, const float* b, size_t n, float* out_f32, void* out_hi, void* out_lo, void* stream);
 /* Pooling half of rnc_fmap_prepare for feature maps that are already CL: fills levels 1..levels-1 of f2_pyr from level 0. */
 int rnc_fmap_pyramid(float* f2_pyr, int B, int D, int H, int W, int levels, void* stream);
 
@@ -332,47 +330,38 @@ int rnc_conf_head_fwd(const float* in, int cin, int ldi, const float* weight, co
  *             into the kernel's parameter bank at launch (read before the call returns), so the call stays
  *             re-entrant with no device-side global state.
  *   out     : NCHW [B][2][4*H4][4*W4] = out_scale * NConvUNet output  (out_scale = 8 in RAFT, raft_nc_dbl.py:161)
- */
-int rnc_ncup_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
-                 float out_scale, float* out, void* stream);
-
-/* Training form of the same chain (fine-tuning the upsampler on a frozen trunk).
+ *   conf_out: NCHW [B][2][4*H4][4*W4] or NULL: the chain's output confidence, the cout of NConvUNet.forward that
+ *             upsampler.py:168 discards, i.e. nconv_out's den4 / (W4[0] + W4[1]) with den4 = W4[0]*c3[0] + W4[1]*c3[1] (c3: the
+ *             decoder's output confidence).  It lies in [0, 1] and is not multiplied by out_scale.  NULL skips it.
+ * out does not depend on whether conf_out is requested: it is bit-identical either way.
+ * Returns RNC_ERR_UNSUPPORTED, before any launch, when 2*B or the rows of 30x30 output tiles exceed 65535.
+ *
+ * Training form of the same chain (fine-tuning the upsampler on a frozen trunk).
  * rnc_ncup_train_fwd: rnc_ncup_fwd with the 224 positive weights read from DEVICE memory (weights_dev, same order), so a
- *   trainable upsampler needs no device-to-host copy per call; outputs are bit-identical to rnc_ncup_fwd on the same weights.
- * rnc_ncup_bwd: gradients of L = sum(g_out * out) for out = rnc_ncup_train_fwd(...):
- *   g_out      : NCHW [B][2][4*H4][4*W4]
+ *   trainable upsampler needs no device-to-host copy per call; out and conf_out (may be NULL, as above) are bit-identical to
+ *   rnc_ncup_fwd's on the same weights.
+ * rnc_ncup_bwd: gradients of L = sum(g_out * out) + sum(g_conf_out * conf_out) for (out, conf_out) = rnc_ncup_train_fwd(...):
+ *   g_out      : NCHW [B][2][4*H4][4*W4] (may be NULL when g_conf_out is given)
+ *   g_conf_out : NCHW [B][2][4*H4][4*W4] (may be NULL: no confidence term; at least one of g_out and g_conf_out is required)
  *   g_x_lowres : NCHW [B][2][H4][W4] (may be NULL)        g_conf : NCHW [B][2][H4][W4] (may be NULL)
  *   g_weights  : [224] w.r.t. the UNFOLDED positive weights (may be NULL): decoder.0's folded gradient goes to both halves
  *                W[:, :2] and W[:, 2:], and every layer's 1/sum(W) normalisation contributes to all of that layer's weights
  *   workspace  : rnc_ncup_bwd_workspace_bytes(B,H4,W4) bytes, 16-byte aligned, needed only with g_weights (no zeroing needed)
  * The kernel recomputes the forward per tile with the forward's own code and differentiates the (y*c, c) pairs it carries,
- * so gradients stay finite where the confidence is zero.  Deterministic: every input gradient is written by one CTA, the
- * weight gradient is a fixed-order fp64 reduction of per-CTA partials; identical inputs give bit-identical gradients. */
+ * so gradients stay finite where the confidence is zero.  The confidence's adjoint enters at the last layer, dL/dc3[k] +=
+ * g * W4[k] / S4 and dL/dW4[k] += g * (c3[k] / S4 - den4 / S4^2) with S4 = W4[0] + W4[1], and flows through the chain like
+ * the flow's.  With g_conf_out NULL the call differentiates sum(g_out * out) alone: the gradients do not depend on whether
+ * the forward wrote conf_out.  Deterministic: every input gradient is written by one CTA, the weight gradient is a fixed-order fp64 reduction of per-CTA
+ * partials; identical inputs give bit-identical gradients.  Returns RNC_ERR_UNSUPPORTED, before any launch, when 2*B or the
+ * rows of 32x32 output tiles exceed 65535 (rnc_ncup_bwd_workspace_bytes returns 0 then). */
+int rnc_ncup_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
+                 float out_scale, float* out, float* conf_out, void* stream);
 int rnc_ncup_train_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                       float out_scale, float* out, void* stream);
+                       float out_scale, float* out, float* conf_out, void* stream);
 size_t rnc_ncup_bwd_workspace_bytes(int B, int H4, int W4);
 int rnc_ncup_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4, float out_scale,
-                 const float* g_out, float* g_x_lowres, float* g_conf, float* g_weights, void* workspace,
-                 size_t workspace_bytes, void* stream);
-
-/* Output confidence of the same chain: the cout of NConvUNet.forward that upsampler.py:168 discards, i.e. nconv_out's
- * den4 / (W4[0] + W4[1]) with den4 = W4[0]*c3[0] + W4[1]*c3[1] (c3: the decoder's output confidence).  It lies in [0, 1]
- * and is not multiplied by out_scale.
- * rnc_ncup_conf_fwd      : rnc_ncup_fwd (host weights) that also writes conf_out NCHW [B][2][4*H4][4*W4]; out is
- *                          bit-identical to rnc_ncup_fwd's.
- * rnc_ncup_train_conf_fwd: the same with the weights in device memory (as rnc_ncup_train_fwd); same outputs.
- * rnc_ncup_conf_bwd      : gradients of L = sum(g_out * out) + sum(g_conf_out * conf_out).  Either upstream gradient may be
- *                          NULL (not both); with g_conf_out NULL the result is bit-identical to rnc_ncup_bwd.  The extra
- *                          adjoint enters at the last layer, dL/dc3[k] += g * W4[k] / S4 and dL/dW4[k] += g * (c3[k] / S4 -
- *                          den4 / S4^2) with S4 = W4[0] + W4[1], and flows through the chain like the flow's.  Same workspace
- *                          (rnc_ncup_bwd_workspace_bytes), status codes and determinism as rnc_ncup_bwd. */
-int rnc_ncup_conf_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
-                      float out_scale, float* out, float* conf_out, void* stream);
-int rnc_ncup_train_conf_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                            float out_scale, float* out, float* conf_out, void* stream);
-int rnc_ncup_conf_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                      float out_scale, const float* g_out, const float* g_conf_out, float* g_x_lowres, float* g_conf,
-                      float* g_weights, void* workspace, size_t workspace_bytes, void* stream);
+                 const float* g_out, const float* g_conf_out, float* g_x_lowres, float* g_conf, float* g_weights,
+                 void* workspace, size_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------------
  * A3  bilinear_sampler  (core/utils/utils.py:59-73) as a standalone operator: grid_sample(align_corners=True, bilinear,

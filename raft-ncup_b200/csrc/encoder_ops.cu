@@ -235,25 +235,6 @@ __global__ void instnorm_apply_kernel(const float* __restrict__ x, const float* 
   }
 }
 
-// y = relu(a + b) on CL fp32 (block tail when the norm is folded into the convolutions), -> fp32 + split
-__global__ void add_relu_split_kernel(const float4* __restrict__ a, const float4* __restrict__ b, size_t n4, float4* __restrict__ out_f32,
-                                      uint2* __restrict__ out_hi, uint2* __restrict__ out_lo) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n4; i += (size_t)gridDim.x * blockDim.x) {
-    const float4 x = a[i], y = b[i];
-    float o[4] = {fmaxf(x.x + y.x, 0.f), fmaxf(x.y + y.y, 0.f), fmaxf(x.z + y.z, 0.f), fmaxf(x.w + y.w, 0.f)};
-    if (out_f32) out_f32[i] = make_float4(o[0], o[1], o[2], o[3]);
-    __half h[4], l[4];
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float vc = fminf(o[j], 65504.f);
-      h[j] = __float2half_rn(vc);
-      l[j] = __float2half_rn(vc - __half2float(h[j]));
-    }
-    out_hi[i] = *reinterpret_cast<uint2*>(h);
-    out_lo[i] = *reinterpret_cast<uint2*>(l);
-  }
-}
-
 __global__ void pool2_cl_kernel2(const float4* __restrict__ src, float4* __restrict__ dst, int B, int Hs, int Ws, int D4) {
   const int Hd = Hs >> 1, Wd = Ws >> 1;
   const size_t n = (size_t)B * Hd * Wd * D4;
@@ -376,17 +357,6 @@ int rnc_instnorm_apply(const float* x, const float* mean_rstd, const float* res,
   if (blocks > 132 * 32) blocks = 132 * 32;
   instnorm_apply_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(x, mean_rstd, res, N, P, C, mode, out_f32,
                                                                    static_cast<__half*>(out_hi), static_cast<__half*>(out_lo));
-  return after_launch();
-}
-
-int rnc_add_relu_split(const float* a, const float* b, size_t n, float* out_f32, void* out_hi, void* out_lo, void* stream) {
-  if (n == 0 || (n & 3)) return RNC_ERR_BAD_SHAPE;
-  if (!a || !b || !out_hi || !out_lo || !aligned16(a) || !aligned16(b)) return RNC_ERR_BAD_POINTER;
-  size_t blocks = (n / 4 + 255) / 256;
-  if (blocks > 132 * 32) blocks = 132 * 32;
-  add_relu_split_kernel<<<(int)blocks, 256, 0, as_stream(stream)>>>(reinterpret_cast<const float4*>(a), reinterpret_cast<const float4*>(b), n / 4,
-                                                                    reinterpret_cast<float4*>(out_f32), static_cast<uint2*>(out_hi),
-                                                                    static_cast<uint2*>(out_lo));
   return after_launch();
 }
 

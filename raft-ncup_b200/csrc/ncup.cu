@@ -28,8 +28,8 @@
 //                           writes its weight-gradient partial sums to the workspace; two small kernels reduce them in a
 //                           fixed order in fp64, so gradients are bit-identical across calls.
 // Each has a twin instantiated from the same code with a compile-time flag that also handles nconv_out's output confidence
-// den4 / sum(W4): ncup_fused_conf_kernel and ncup_train_fwd_conf_kernel write it (rnc_ncup_conf_fwd, rnc_ncup_train_conf_fwd),
-// ncup_conf_bwd_kernel adds its adjoint (rnc_ncup_conf_bwd).  The flag off compiles to the plain kernels.
+// den4 / sum(W4): ncup_fused_conf_kernel and ncup_train_fwd_conf_kernel write it, ncup_conf_bwd_kernel adds its adjoint.  The
+// entry points launch a twin only when the caller passes conf_out / g_conf_out; the flag off compiles to the plain kernels.
 #include "rnc_common.cuh"
 
 namespace rnc {
@@ -662,13 +662,17 @@ ncup_bwd_finish_kernel(const double* __restrict__ sums, const float* __restrict_
   if (tid < 2) g_w[222 + tid] = static_cast<float>(sums[kOffW4 + tid]);
 }
 
-inline int ncup_check_shape(int B, int H4, int W4) {
-  if (B <= 0 || H4 <= 0 || W4 <= 0) return RNC_ERR_BAD_SHAPE;
-  if (H4 > (1 << 20) || W4 > (1 << 20) || 2LL * B > 65535 || (4LL * H4 + NB - 1) / NB > 65535) return RNC_ERR_UNSUPPORTED;
-  return RNC_OK;
+// The grid of tile x tile output tiles (NT for the forwards, NB for the backward) over the B * 2 planes
+inline dim3 ncup_grid(int B, int H4, int W4, int tile) {
+  return dim3((4 * W4 + tile - 1) / tile, (4 * H4 + tile - 1) / tile, B * 2);
 }
 
-inline dim3 ncup_bwd_grid(int B, int H4, int W4) { return dim3((4 * W4 + NB - 1) / NB, (4 * H4 + NB - 1) / NB, B * 2); }
+// Rejects, before anything is launched, a shape whose ncup_grid(B, H4, W4, tile) exceeds the 65535 limit of grid.y and grid.z
+inline int ncup_check_shape(int B, int H4, int W4, int tile) {
+  if (B <= 0 || H4 <= 0 || W4 <= 0) return RNC_ERR_BAD_SHAPE;
+  if (H4 > (1 << 20) || W4 > (1 << 20) || 2LL * B > 65535 || (4LL * H4 + tile - 1) / tile > 65535) return RNC_ERR_UNSUPPORTED;
+  return RNC_OK;
+}
 
 }  // namespace rnc
 
@@ -704,94 +708,66 @@ static NcupWeights pack_host_weights(const float* wts_host) {
   return w;
 }
 
-static dim3 ncup_fwd_grid(int B, int H4, int W4) { return dim3((4 * W4 + NT - 1) / NT, (4 * H4 + NT - 1) / NT, B * 2); }
-
+// conf_out NULL launches the plain kernels, non-NULL their confidence twins (ncup_forward_tile<kConf>)
 extern "C" int rnc_ncup_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
-                            float out_scale, float* out, void* stream) {
-  if (B <= 0 || H4 <= 0 || W4 <= 0) return RNC_ERR_BAD_SHAPE;
+                            float out_scale, float* out, float* conf_out, void* stream) {
+  if (int st = ncup_check_shape(B, H4, W4, NT)) return st;
   if (!x_lowres || !conf || !wts_host || !out) return RNC_ERR_BAD_POINTER;
   const NcupWeights w = pack_host_weights(wts_host);
-  ncup_fused_kernel<<<ncup_fwd_grid(B, H4, W4), kThreads, 0, as_stream(stream)>>>(x_lowres, conf, w, H4, W4, out_scale, out);
-  return after_launch();
-}
-
-extern "C" int rnc_ncup_conf_fwd(const float* x_lowres, const float* conf, const float* wts_host, int B, int H4, int W4,
-                                 float out_scale, float* out, float* conf_out, void* stream) {
-  if (int st = ncup_check_shape(B, H4, W4)) return st;
-  if (!x_lowres || !conf || !wts_host || !out || !conf_out) return RNC_ERR_BAD_POINTER;
-  const NcupWeights w = pack_host_weights(wts_host);
-  ncup_fused_conf_kernel<<<ncup_fwd_grid(B, H4, W4), kThreads, 0, as_stream(stream)>>>(x_lowres, conf, w, H4, W4, out_scale, out,
-                                                                                       conf_out);
+  const dim3 grid = ncup_grid(B, H4, W4, NT);
+  cudaStream_t s = as_stream(stream);
+  if (conf_out)
+    ncup_fused_conf_kernel<<<grid, kThreads, 0, s>>>(x_lowres, conf, w, H4, W4, out_scale, out, conf_out);
+  else
+    ncup_fused_kernel<<<grid, kThreads, 0, s>>>(x_lowres, conf, w, H4, W4, out_scale, out);
   return after_launch();
 }
 
 extern "C" int rnc_ncup_train_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                                  float out_scale, float* out, void* stream) {
-  if (int st = ncup_check_shape(B, H4, W4)) return st;
+                                  float out_scale, float* out, float* conf_out, void* stream) {
+  if (int st = ncup_check_shape(B, H4, W4, NT)) return st;
   if (!x_lowres || !conf || !weights_dev || !out) return RNC_ERR_BAD_POINTER;
-  const int H = 4 * H4, W = 4 * W4;
-  dim3 grid((W + NT - 1) / NT, (H + NT - 1) / NT, B * 2);
-  ncup_train_fwd_kernel<<<grid, kThreads, 0, as_stream(stream)>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, out);
-  return after_launch();
-}
-
-extern "C" int rnc_ncup_train_conf_fwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                                       float out_scale, float* out, float* conf_out, void* stream) {
-  if (int st = ncup_check_shape(B, H4, W4)) return st;
-  if (!x_lowres || !conf || !weights_dev || !out || !conf_out) return RNC_ERR_BAD_POINTER;
-  ncup_train_fwd_conf_kernel<<<ncup_fwd_grid(B, H4, W4), kThreads, 0, as_stream(stream)>>>(x_lowres, conf, weights_dev, H4, W4,
-                                                                                           out_scale, out, conf_out);
+  const dim3 grid = ncup_grid(B, H4, W4, NT);
+  cudaStream_t s = as_stream(stream);
+  if (conf_out)
+    ncup_train_fwd_conf_kernel<<<grid, kThreads, 0, s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, out, conf_out);
+  else
+    ncup_train_fwd_kernel<<<grid, kThreads, 0, s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, out);
   return after_launch();
 }
 
 extern "C" size_t rnc_ncup_bwd_workspace_bytes(int B, int H4, int W4) {
-  if (ncup_check_shape(B, H4, W4)) return 0;
-  const dim3 g = ncup_bwd_grid(B, H4, W4);
+  if (ncup_check_shape(B, H4, W4, NB)) return 0;
+  const dim3 g = ncup_grid(B, H4, W4, NB);
   return sizeof(double) * ((size_t)g.x * g.y * g.z * kPartLd + kPartLd);
 }
 
+// g_conf_out NULL launches ncup_bwd_kernel, non-NULL ncup_conf_bwd_kernel; then, with g_weights, the fixed-order reduction of
+// the per-CTA partials and the finish
 extern "C" int rnc_ncup_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                            float out_scale, const float* g_out, float* g_x_lowres, float* g_conf, float* g_weights,
-                            void* workspace, size_t workspace_bytes, void* stream) {
-  if (int st = ncup_check_shape(B, H4, W4)) return st;
-  if (!x_lowres || !conf || !weights_dev || !g_out || (!g_x_lowres && !g_conf && !g_weights)) return RNC_ERR_BAD_POINTER;
+                            float out_scale, const float* g_out, const float* g_conf_out, float* g_x_lowres, float* g_conf,
+                            float* g_weights, void* workspace, size_t workspace_bytes, void* stream) {
+  if (int st = ncup_check_shape(B, H4, W4, NB)) return st;
+  if (!x_lowres || !conf || !weights_dev || (!g_out && !g_conf_out) || (!g_x_lowres && !g_conf && !g_weights))
+    return RNC_ERR_BAD_POINTER;
   if (g_weights && (!workspace || !aligned16(workspace))) return RNC_ERR_BAD_POINTER;
   if (g_weights && workspace_bytes < rnc_ncup_bwd_workspace_bytes(B, H4, W4)) return RNC_ERR_WORKSPACE;
-  static unsigned long long attr_done = 0;
-  if (int st = ensure_dyn_smem(ncup_bwd_kernel, (int)sizeof(BwdSmem), &attr_done)) return st;
-  const dim3 grid = ncup_bwd_grid(B, H4, W4);
+  static unsigned long long attr_done = 0, attr_done_conf = 0;       // one per kernel
+  if (int st = g_conf_out ? ensure_dyn_smem(ncup_conf_bwd_kernel, (int)sizeof(BwdSmem), &attr_done_conf)
+                          : ensure_dyn_smem(ncup_bwd_kernel, (int)sizeof(BwdSmem), &attr_done))
+    return st;
+  const dim3 grid = ncup_grid(B, H4, W4, NB);
   const int nblocks = grid.x * grid.y * grid.z;
   double* partials = g_weights ? static_cast<double*>(workspace) : nullptr;
-  double* sums = g_weights ? partials + (size_t)nblocks * kPartLd : nullptr;
   cudaStream_t s = as_stream(stream);
-  ncup_bwd_kernel<<<grid, kThreads, sizeof(BwdSmem), s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, g_out, g_x_lowres, g_conf,
-                                                          partials);
+  if (g_conf_out)
+    ncup_conf_bwd_kernel<<<grid, kThreads, sizeof(BwdSmem), s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, g_out,
+                                                                 g_conf_out, g_x_lowres, g_conf, partials);
+  else
+    ncup_bwd_kernel<<<grid, kThreads, sizeof(BwdSmem), s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, g_out, g_x_lowres,
+                                                            g_conf, partials);
   if (!g_weights) return after_launch();
-  ncup_bwd_reduce_kernel<<<kNPart, kThreads, 0, s>>>(partials, nblocks, sums);
-  ncup_bwd_finish_kernel<<<1, kThreads, 0, s>>>(sums, weights_dev, g_weights);
-  return after_launch(3);
-}
-
-extern "C" int rnc_ncup_conf_bwd(const float* x_lowres, const float* conf, const float* weights_dev, int B, int H4, int W4,
-                                 float out_scale, const float* g_out, const float* g_conf_out, float* g_x_lowres, float* g_conf,
-                                 float* g_weights, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!g_conf_out)                               // no confidence term: exactly rnc_ncup_bwd
-    return rnc_ncup_bwd(x_lowres, conf, weights_dev, B, H4, W4, out_scale, g_out, g_x_lowres, g_conf, g_weights, workspace,
-                        workspace_bytes, stream);
-  if (int st = ncup_check_shape(B, H4, W4)) return st;
-  if (!x_lowres || !conf || !weights_dev || (!g_x_lowres && !g_conf && !g_weights)) return RNC_ERR_BAD_POINTER;
-  if (g_weights && (!workspace || !aligned16(workspace))) return RNC_ERR_BAD_POINTER;
-  if (g_weights && workspace_bytes < rnc_ncup_bwd_workspace_bytes(B, H4, W4)) return RNC_ERR_WORKSPACE;
-  static unsigned long long attr_done = 0;
-  if (int st = ensure_dyn_smem(ncup_conf_bwd_kernel, (int)sizeof(BwdSmem), &attr_done)) return st;
-  const dim3 grid = ncup_bwd_grid(B, H4, W4);
-  const int nblocks = grid.x * grid.y * grid.z;
-  double* partials = g_weights ? static_cast<double*>(workspace) : nullptr;
-  double* sums = g_weights ? partials + (size_t)nblocks * kPartLd : nullptr;
-  cudaStream_t s = as_stream(stream);
-  ncup_conf_bwd_kernel<<<grid, kThreads, sizeof(BwdSmem), s>>>(x_lowres, conf, weights_dev, H4, W4, out_scale, g_out, g_conf_out,
-                                                               g_x_lowres, g_conf, partials);
-  if (!g_weights) return after_launch();
+  double* sums = partials + (size_t)nblocks * kPartLd;
   ncup_bwd_reduce_kernel<<<kNPart, kThreads, 0, s>>>(partials, nblocks, sums);
   ncup_bwd_finish_kernel<<<1, kThreads, 0, s>>>(sums, weights_dev, g_weights);
   return after_launch(3);

@@ -575,19 +575,15 @@ class Engine:
         """Zero-stuffing + NConvUNet + out_scale (upsampler.py:150-177) on x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4]:
         the fused rnc_ncup_fwd for the shipped network, the per-level chain of rnc/nconv_unet.py for any other.  Neither
         synchronises with the host, so graph capture records either.  want_conf: return (out, confidence), the network's
-        output confidence (the cout upsampler.py:168 discards) in the layout of out, without out_scale; the shipped network
-        then runs on rnc_ncup_conf_fwd, whose out is bit-identical to rnc_ncup_fwd's."""
+        output confidence (the cout upsampler.py:168 discards) in the layout of out, without out_scale; out is the same
+        either way."""
         B, _, H4, W4 = x_lowres.shape
         if pu.unet is None:
             out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
-            if want_conf:
-                cout = torch.empty_like(out)
-                with _Timed(self, "ncup"):
-                    rnc.ncup_conf_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out, cout)
-                return out, cout
+            cout = torch.empty_like(out) if want_conf else None
             with _Timed(self, "ncup"):
-                rnc.ncup_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out)
-            return out
+                rnc.ncup_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out, cout)
+            return (out, cout) if want_conf else out
         # intermediates live in the workspace (allocated by the first, eager forward of a shape; graph capture reuses them)
         bufs = ws.__dict__.setdefault("nconv_bufs", {})
         if "stuffed" not in bufs:

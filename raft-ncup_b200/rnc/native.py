@@ -19,7 +19,7 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RNC_LIB") or os.path.join(_HERE, "librnc.so")      # RNC_LIB: developer override (variant builds)
-ABI_VERSION = 16
+ABI_VERSION = 17
 CONV_NO_HALO, CONV_BASE_OFFSET, CONV_SPLIT_N, CONV_NO_PAIR, CONV_AUX_BLOCKED, CONV_OUT_BLOCKED, CONV_TF32, CONV_WINDOW = 1, 2, 4, 8, 16, 32, 64, 128   # rnc_conv_umma_desc.flags
 
 (EPI_LINEAR, EPI_RELU, EPI_SIGMOID, EPI_GRU_ZR, EPI_GRU_Q, EPI_RELU_FLOW, EPI_RELU_ADD_RELU, EPI_TANH_RELU,
@@ -103,7 +103,6 @@ SIGNATURES = {
     "rnc_instnorm_stats_det_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
     "rnc_instnorm_stats_det": (_i, [_vp, _i, _i, _i, _f, _vp, C.c_size_t, _vp, _vp]),
     "rnc_instnorm_apply": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
-    "rnc_add_relu_split": (_i, [_vp, _vp, C.c_size_t, _vp, _vp, _vp, _vp]),
     "rnc_fmap_pyramid": (_i, [_vp, _i, _i, _i, _i, _i, _vp]),
     "rnc_conv_flow7x7_split_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "rnc_conv_flow7x7_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
@@ -120,13 +119,10 @@ SIGNATURES = {
     "rnc_ncup_guidance_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _i, _vp]),
     "rnc_ncup_guidance_split_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "rnc_conf_head_fwd": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp]),
-    "rnc_ncup_fwd": (_i, [_vp, _vp, C.POINTER(_f), _i, _i, _i, _f, _vp, _vp]),
-    "rnc_ncup_train_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp]),
+    "rnc_ncup_fwd": (_i, [_vp, _vp, C.POINTER(_f), _i, _i, _i, _f, _vp, _vp, _vp]),
+    "rnc_ncup_train_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp]),
     "rnc_ncup_bwd_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
-    "rnc_ncup_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
-    "rnc_ncup_conf_fwd": (_i, [_vp, _vp, C.POINTER(_f), _i, _i, _i, _f, _vp, _vp, _vp]),
-    "rnc_ncup_train_conf_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp]),
-    "rnc_ncup_conf_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_ncup_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
     "rnc_bilinear_sample_fwd": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "rnc_nconv2d_fwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _f, _vp, _vp, _i, _i, _i, _f, _vp, _vp, _vp]),
     "rnc_corr_lookup_bwd": (_i, [_vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp, _vp, _vp]),

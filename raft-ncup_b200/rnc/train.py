@@ -13,9 +13,9 @@
     NcupChainFn     the whole NConvUNet chain after the weights net at the shipped configuration: rnc_ncup_train_fwd /
                     rnc_ncup_bwd (fused, deterministic); used by the frozen-trunk forward (rnc.model.frozen_trunk), which runs the
                     trunk on the inference engine.  Other configurations run the NConv2dFn / NConvPoolFn chain of
-                    rnc/nconv_unet.py there too.
-    NcupChainConfFn NcupChainFn that also returns the chain's output confidence: rnc_ncup_train_conf_fwd / rnc_ncup_conf_bwd;
-                    the frozen-trunk forward uses it when the confidence is requested.
+                    rnc/nconv_unet.py there too.  With want_conf it also returns the chain's output confidence (the same
+                    entry points, given conf_out / g_conf_out); the frozen-trunk forward asks for it when the confidence is
+                    requested.
 
 Under torch.use_deterministic_algorithms(True) the lookup backward, which otherwise scatters d fmap2 with floating-point
 atomics, switches to its fixed-order form rnc_corr_lookup_bwd_det (deterministic()); the weight gradient sums in a fixed order
@@ -525,13 +525,15 @@ class NcupChainFn(torch.autograd.Function):
     """Zero-stuffing + the live NConvUNet chain + out_scale (upsampler.py:143-177 after the weights net, nconv_modules.py:106-136)
     as one fused kernel forward (rnc_ncup_train_fwd) and one fused backward (rnc_ncup_bwd):
     (x_lowres, conf) NCHW [B,2,H4,W4], the positive kernels W1 [2,1,5,5], W2 [2,2,5,5], W3 [2,4,3,3], W4 [1,2,1,1]
-    -> out NCHW [B,2,4*H4,4*W4].  The same function as the per-layer NConv2dFn chain of ncup_upsampler_train, with gradients
-    that are bit-identical from call to call."""
+    -> out NCHW [B,2,4*H4,4*W4], or with want_conf (out, conf_out): the chain's output confidence den4 / sum(W4) of nconv_out
+    in the layout of out, without out_scale; out is the same either way.  The same function as the per-layer NConv2dFn chain
+    of ncup_upsampler_train, with gradients that are bit-identical from call to call; when the loss does not use conf_out
+    they are those of want_conf=False, bit for bit."""
 
     SHAPES = ((2, 1, 5, 5), (2, 2, 5, 5), (2, 4, 3, 3), (1, 2, 1, 1))
 
     @staticmethod
-    def forward(ctx, x_lowres, conf, w1, w2, w3, w4, out_scale):
+    def forward(ctx, x_lowres, conf, w1, w2, w3, w4, out_scale, want_conf=False):
         if x_lowres.dim() != 4 or x_lowres.shape[1] != 2 or conf.shape != x_lowres.shape:
             raise ValueError("NcupChainFn: x_lowres and conf must both be [B,2,H4,W4]")
         if tuple(tuple(w.shape) for w in (w1, w2, w3, w4)) != NcupChainFn.SHAPES:
@@ -541,69 +543,20 @@ class NcupChainFn(torch.autograd.Function):
         wts = torch.cat([w.detach().float().reshape(-1) for w in (w1, w2, w3, w4)])
         B, _, H4, W4 = x_lowres.shape
         out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
-        rnc.ncup_train_fwd(x_lowres, conf, wts, B, H4, W4, float(out_scale), out)
-        ctx.save_for_backward(x_lowres, conf, wts)
-        ctx.out_scale = float(out_scale)
-        return out
-
-    @staticmethod
-    def backward(ctx, g_out):
-        x_lowres, conf, wts = ctx.saved_tensors
-        B, _, H4, W4 = x_lowres.shape
-        need_w = any(ctx.needs_input_grad[2:6])
-        with torch.cuda.device(x_lowres.device):
-            g_out = g_out.float().contiguous()
-            g_x = torch.empty_like(x_lowres) if ctx.needs_input_grad[0] else None
-            g_c = torch.empty_like(conf) if ctx.needs_input_grad[1] else None
-            g_w = ws = None
-            if need_w:
-                g_w = torch.empty(224, dtype=torch.float32, device=x_lowres.device)
-                nbytes = rnc.ncup_bwd_workspace_bytes(B, H4, W4)
-                ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=x_lowres.device)
-            if g_x is None and g_c is None and g_w is None:
-                return (None,) * 7
-            rnc.ncup_bwd(x_lowres, conf, wts, B, H4, W4, ctx.out_scale, g_out, g_x, g_c, g_w, ws, ws.numel() * 8 if ws is not None else 0)
-        gws = [None] * 4
-        if g_w is not None:
-            off = 0
-            for k, shp in enumerate(NcupChainFn.SHAPES):
-                n = shp[0] * shp[1] * shp[2] * shp[3]
-                gws[k] = g_w[off:off + n].view(shp) if ctx.needs_input_grad[2 + k] else None
-                off += n
-        return (g_x, g_c, *gws, None)
-
-
-class NcupChainConfFn(torch.autograd.Function):
-    """NcupChainFn that also returns the chain's output confidence: the same inputs -> (out, conf_out), both NCHW
-    [B,2,4*H4,4*W4]; conf_out = den4 / sum(W4) of nconv_out, without out_scale.  Forward rnc_ncup_train_conf_fwd (out
-    bit-identical to NcupChainFn's), backward rnc_ncup_conf_bwd: when the loss does not use conf_out its gradients are
-    NcupChainFn's, bit for bit."""
-
-    @staticmethod
-    def forward(ctx, x_lowres, conf, w1, w2, w3, w4, out_scale):
-        if x_lowres.dim() != 4 or x_lowres.shape[1] != 2 or conf.shape != x_lowres.shape:
-            raise ValueError("NcupChainConfFn: x_lowres and conf must both be [B,2,H4,W4]")
-        if tuple(tuple(w.shape) for w in (w1, w2, w3, w4)) != NcupChainFn.SHAPES:
-            raise ValueError(f"NcupChainConfFn: weights must have shapes {NcupChainFn.SHAPES}")
-        _require_cuda(x_lowres)
-        x_lowres, conf = x_lowres.detach().float().contiguous(), conf.detach().float().contiguous()
-        wts = torch.cat([w.detach().float().reshape(-1) for w in (w1, w2, w3, w4)])
-        B, _, H4, W4 = x_lowres.shape
-        out = torch.empty(B, 2, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)
-        cout = torch.empty_like(out)
-        rnc.ncup_train_conf_fwd(x_lowres, conf, wts, B, H4, W4, float(out_scale), out, cout)
+        cout = torch.empty_like(out) if want_conf else None
+        rnc.ncup_train_fwd(x_lowres, conf, wts, B, H4, W4, float(out_scale), out, cout)
         ctx.save_for_backward(x_lowres, conf, wts)
         ctx.out_scale = float(out_scale)
         ctx.set_materialize_grads(False)        # an unused output's gradient stays None: the kernel skips its term
-        return out, cout
+        return (out, cout) if want_conf else out
 
     @staticmethod
-    def backward(ctx, g_out, g_cout):
+    def backward(ctx, g_out, g_cout=None):
         x_lowres, conf, wts = ctx.saved_tensors
         B, _, H4, W4 = x_lowres.shape
         need_w = any(ctx.needs_input_grad[2:6])
         if g_out is None and g_cout is None:
-            return (None,) * 7
+            return (None,) * 8
         with torch.cuda.device(x_lowres.device):
             g_out = g_out.float().contiguous() if g_out is not None else None
             g_cout = g_cout.float().contiguous() if g_cout is not None else None
@@ -615,9 +568,9 @@ class NcupChainConfFn(torch.autograd.Function):
                 nbytes = rnc.ncup_bwd_workspace_bytes(B, H4, W4)
                 ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=x_lowres.device)
             if g_x is None and g_c is None and g_w is None:
-                return (None,) * 7
-            rnc.ncup_conf_bwd(x_lowres, conf, wts, B, H4, W4, ctx.out_scale, g_out, g_cout, g_x, g_c, g_w, ws,
-                              ws.numel() * 8 if ws is not None else 0)
+                return (None,) * 8
+            rnc.ncup_bwd(x_lowres, conf, wts, B, H4, W4, ctx.out_scale, g_out, g_cout, g_x, g_c, g_w, ws,
+                         ws.numel() * 8 if ws is not None else 0)
         gws = [None] * 4
         if g_w is not None:
             off = 0
@@ -625,23 +578,24 @@ class NcupChainConfFn(torch.autograd.Function):
                 n = shp[0] * shp[1] * shp[2] * shp[3]
                 gws[k] = g_w[off:off + n].view(shp) if ctx.needs_input_grad[2 + k] else None
                 off += n
-        return (g_x, g_c, *gws, None)
+        return (g_x, g_c, *gws, None, None)
 
 
 def ncup_chain_autograd(net, x_lowres, conf, out_scale=1.0, want_conf=False):
     """The NConvUNet `net` (live path) on zero-stuffed (x_lowres, conf), times out_scale, through NcupChainFn; want_conf:
-    (out, output confidence) through NcupChainConfFn."""
+    (out, output confidence)."""
     _require_cuda(x_lowres, conf)
-    fn = NcupChainConfFn if want_conf else NcupChainFn
-    return fn.apply(x_lowres, conf, net.nconv_in.weight, net.nconv_x2[0].weight, net.decoder[0].weight, net.nconv_out.weight,
-                    out_scale)
+    args = (x_lowres, conf, net.nconv_in.weight, net.nconv_x2[0].weight, net.decoder[0].weight, net.nconv_out.weight, out_scale)
+    # want_conf goes to apply only when set: a flow-only call passes the chain's seven inputs alone, the arguments that
+    # wrappers of NcupChainFn.apply (tests/test_gpu_train_shapes.py) unpack
+    return NcupChainFn.apply(*args, True) if want_conf else NcupChainFn.apply(*args)
 
 
 def ncup_upsampler_frozen(up, x4, gin, out_scale=8.0, want_conf=False):
     """NConvUpsampler.forward (upsampler.py:143-177) for a frozen trunk: x4 NCHW [B,2,H4,W4] and the weights-net input gin
     (CL [B,H4,W4,136] = cat(x4, area-resized guidance), zero channels beyond 130; rnc_ncup_guidance_fwd) are the trunk's
-    detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn (NcupChainConfFn
-    with want_conf, which returns (out, confidence))."""
+    detached outputs.  The weights net runs on ConvCL (BatchNorm as configured), the chain on NcupChainFn (with want_conf it
+    returns (out, confidence))."""
     with torch.cuda.device(x4.device):
         conf = simple_cl(up.weights_est_net, gin)
         return _ncup_chain_train(up.interpolation_net, x4, conf, out_scale, fused=True, want_conf=want_conf)

@@ -1,5 +1,5 @@
-"""NCUP output confidence on the GPU: the fused kernels (rnc_ncup_conf_fwd / rnc_ncup_train_conf_fwd / rnc_ncup_conf_bwd)
-against fp64, the per-level chain of every other NConvUNet configuration, the model's test mode on both engines (eager,
+"""NCUP output confidence on the GPU: the fused kernels (rnc_ncup_fwd / rnc_ncup_train_fwd / rnc_ncup_bwd given conf_out /
+g_conf_out) against fp64, the per-level chain of every other NConvUNet configuration, the model's test mode on both engines (eager,
 graph replay, nn.DataParallel), the frozen-trunk and exact training routes against the reference's gradients
 (tests/golden/conf.npz, oracle/make_golden_conf.py) and sequence inference."""
 import ctypes
@@ -67,7 +67,7 @@ def stream():
 
 
 @pytest.mark.parametrize("B,H4,W4", [(8, 110, 256), (1, 22, 26)])
-def test_fused_confidence_matches_fp64(B, H4, W4):
+def test_ncup_fwd_conf_out_matches_fp64(B, H4, W4):
     """At the benchmark shape and at 22x26 (88x104 outputs: partial 30x30 tiles) with exact zero confidences.  The
     confidence is a chain of normalised non-negative averages: measured on an H100, 3.4e-8 (bench shape) and 1.5e-8 from
     fp64, against the 1e-5 bound."""
@@ -82,9 +82,10 @@ def test_fused_confidence_matches_fp64(B, H4, W4):
     shape = (B, 2, 4 * H4, 4 * W4)
     out_ref, out, conf = (torch.empty(shape, device=DEV) for _ in range(3))
     out_t, conf_t = torch.empty(shape, device=DEV), torch.empty(shape, device=DEV)
-    native.check(L.rnc_ncup_fwd(xd.data_ptr(), cd.data_ptr(), hw, B, H4, W4, 8.0, ctypes.c_void_p(out_ref.data_ptr()), stream()))
-    native.rnc.ncup_conf_fwd(xd, cd, hw, B, H4, W4, 8.0, out, conf)
-    native.rnc.ncup_train_conf_fwd(xd, cd, wdev, B, H4, W4, 8.0, out_t, conf_t)
+    native.check(L.rnc_ncup_fwd(xd.data_ptr(), cd.data_ptr(), hw, B, H4, W4, 8.0, ctypes.c_void_p(out_ref.data_ptr()), None,
+                                stream()))
+    native.rnc.ncup_fwd(xd, cd, hw, B, H4, W4, 8.0, out, conf)
+    native.rnc.ncup_train_fwd(xd, cd, wdev, B, H4, W4, 8.0, out_t, conf_t)
     torch.cuda.synchronize()
     o64, c64 = chain64(xd.double(), cd.double(), [w.to(DEV) for w in wp], 8.0)
     err = (conf.double() - c64).abs().max().item()
@@ -193,10 +194,10 @@ def test_data_parallel_gathers_the_confidence():
 
 
 def chain_grads(fn, x, c, wp, gy, gc, conf_out=True):
-    """Gradients of sum(gy * out) + sum(gc * conf) through fn(x, c, *softplus(wp), 8): [x, c, weight_p...]."""
+    """Gradients of sum(gy * out) + sum(gc * conf) through fn(x, c, *softplus(wp), 8, conf_out): [x, c, weight_p...]."""
     xd, cd = x.to(DEV).requires_grad_(True), c.to(DEV).requires_grad_(True)
     wpd = [w.to(DEV).requires_grad_(True) for w in wp]
-    res = fn(xd, cd, *[F.softplus(w, beta=10) for w in wpd], 8.0)
+    res = fn(xd, cd, *[F.softplus(w, beta=10) for w in wpd], 8.0, conf_out)
     if conf_out:
         out, conf = res
         loss = (out * gy).sum() + ((conf * gc).sum() if gc is not None else 0.0)
@@ -206,7 +207,7 @@ def chain_grads(fn, x, c, wp, gy, gc, conf_out=True):
     return [xd.grad, cd.grad] + [w.grad for w in wpd]
 
 
-def per_layer(x, c, w1, w2, w3, w4, out_scale):
+def per_layer(x, c, w1, w2, w3, w4, out_scale, conf_out):
     from rnc.train import NConv2dFn, zero_stuff
     xh, ch = zero_stuff(x), zero_stuff(c)
     b, C, oh, ow = xh.shape
@@ -217,17 +218,18 @@ def per_layer(x, c, w1, w2, w3, w4, out_scale):
     return out_scale * y.view(b, C, oh, ow), k.view(b, C, oh, ow)
 
 
-def test_fused_confidence_backward():
-    """NcupChainConfFn against the per-layer NConv2dFn chain and fp64 autograd (the bounds of test_gpu_ncup_finetune: 1e-4,
-    1e-3 for the scale-invariant nconv_out), the flow-only gradient bit-identical to NcupChainFn, and determinism."""
-    from rnc.train import NcupChainConfFn, NcupChainFn
+def test_ncup_chain_fn_confidence_backward():
+    """NcupChainFn with want_conf against the per-layer NConv2dFn chain and fp64 autograd (the bounds of
+    test_gpu_ncup_finetune: 1e-4, 1e-3 for the scale-invariant nconv_out), the flow-only gradient bit-identical to
+    want_conf=False's, and determinism."""
+    from rnc.train import NcupChainFn
     x, c, wp = chain_inputs(2, 24, 40, seed=31)
     gen = torch.Generator().manual_seed(32)
     with torch.no_grad():
         _, c64 = chain64(x.double(), c.double(), wp, 8.0)
     gy = (torch.randn(c64.shape, generator=gen, dtype=torch.float64) * (c64 > 0)).float().to(DEV)
     gc = torch.randn(c64.shape, generator=gen).to(DEV)
-    fused = chain_grads(NcupChainConfFn.apply, x, c, wp, gy, gc)
+    fused = chain_grads(NcupChainFn.apply, x, c, wp, gy, gc)
     layer = chain_grads(per_layer, x, c, wp, gy, gc)
     xr, cr = x.double().requires_grad_(True), c.double().requires_grad_(True)
     wr = [w.double().requires_grad_(True) for w in wp]
@@ -242,33 +244,13 @@ def test_fused_confidence_backward():
             errs[t] = rel(a.cpu()[ok], b.cpu()[ok])
         print(f"fused vs {what}: " + " ".join(f"{k} {v:.2e}" for k, v in errs.items()))
         assert errs.pop("W4") < 1e-3 and all(v < 1e-4 for v in errs.values()), errs
-    # the confidence term absent: NcupChainFn's gradients, bit for bit
+    # the confidence term absent: want_conf=False's gradients, bit for bit
     plain = chain_grads(NcupChainFn.apply, x, c, wp, gy, None, conf_out=False)
-    no_conf = chain_grads(NcupChainConfFn.apply, x, c, wp, gy, None)
+    no_conf = chain_grads(NcupChainFn.apply, x, c, wp, gy, None)
     assert all(torch.equal(a, b) for a, b in zip(plain, no_conf))
     # deterministic
-    again = chain_grads(NcupChainConfFn.apply, x, c, wp, gy, gc)
+    again = chain_grads(NcupChainFn.apply, x, c, wp, gy, gc)
     assert all(torch.equal(a, b) for a, b in zip(fused, again))
-
-
-def test_conf_bwd_without_confidence_gradient_is_rnc_ncup_bwd():
-    from rnc import native
-    B, H4, W4 = 2, 24, 40
-    x, c, wp = chain_inputs(B, H4, W4, seed=41)
-    xd, cd = x.to(DEV), c.to(DEV)
-    wdev = torch.cat([F.softplus(w, beta=10).reshape(-1) for w in wp]).to(DEV)
-    g = torch.randn(B, 2, 4 * H4, 4 * W4, generator=torch.Generator().manual_seed(42)).to(DEV)
-    nbytes = native.rnc.ncup_bwd_workspace_bytes(B, H4, W4)
-    res = []
-    for fn in ("ncup_bwd", "ncup_conf_bwd"):
-        gx, gcf, gw = torch.empty_like(xd), torch.empty_like(cd), torch.empty(224, device=DEV)
-        ws = torch.empty((nbytes + 7) // 8, dtype=torch.float64, device=DEV)
-        if fn == "ncup_bwd":
-            native.rnc.ncup_bwd(xd, cd, wdev, B, H4, W4, 8.0, g, gx, gcf, gw, ws, nbytes)
-        else:
-            native.rnc.ncup_conf_bwd(xd, cd, wdev, B, H4, W4, 8.0, g, None, gx, gcf, gw, ws, nbytes)
-        res.append((gx, gcf, gw))
-    assert all(torch.equal(a, b) for a, b in zip(*res))
 
 
 def _check_grads(grads, meta, tag, loss, bound_fnet=2e-3, bound=2e-3):
@@ -290,8 +272,8 @@ def _check_grads(grads, meta, tag, loss, bound_fnet=2e-3, bound=2e-3):
 
 
 @pytest.mark.parametrize("mode", ["ffma", "umma"])
-def test_frozen_trunk_confidence_gradients_match_the_reference(mode, monkeypatch):
-    """The frozen-trunk route (trunk on the inference engine, upsampler through NcupChainConfFn) against the reference.
+def test_frozen_trunk_want_conf_gradients_match_the_reference(mode, monkeypatch):
+    """The frozen-trunk route (trunk on the inference engine, upsampler through NcupChainFn with want_conf) against the reference.
     On the exact-fp32 engine (ffma) the bound is test_gpu_ncup_finetune's 2e-3; measured on an H100: every upsampler
     gradient within 1e-6 of raft_forward_train's.  On the tensor-core engine (umma, the default) the weights net's hidden-layer
     gradients move by up to 8e-3 of their norm (2.7e-3 against the reference): the confidence term's seeded projections
@@ -309,12 +291,12 @@ def test_frozen_trunk_confidence_gradients_match_the_reference(mode, monkeypatch
     m = raft_nc_dbl.RAFT(a).to(DEV).train()
     m.freeze_bn()
     used = []
-    real = rnc.train.NcupChainConfFn.apply
-    monkeypatch.setattr(rnc.train.NcupChainConfFn, "apply", lambda *a: used.append(1) or real(*a))
+    real = rnc.train.NcupChainFn.apply
+    monkeypatch.setattr(rnc.train.NcupChainFn, "apply", lambda *a: used.append(a[7]) or real(*a))
     monkeypatch.setattr(rnc.train, "raft_forward_train", None)     # the frozen-trunk route, not the exact one
     im1, im2, gt, valid = (t.to(DEV) for t in train_inputs())
     preds, confs = m(im1, im2, iters=GRAD_ITERS, return_confidence=True)
-    assert len(preds) == len(confs) == GRAD_ITERS and len(used) == GRAD_ITERS
+    assert len(preds) == len(confs) == GRAD_ITERS and used == [True] * GRAD_ITERS
     loss = sequence_loss(preds, gt, valid, gamma=0.85)[0] + conf_loss(confs)
     loss.backward()
     b = 2e-3 if mode == "ffma" else 2e-2

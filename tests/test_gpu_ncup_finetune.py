@@ -66,7 +66,7 @@ def upstream(conf_out, seed):
 
 @gpu
 @pytest.mark.parametrize("B,H4,W4", [(1, 7, 9), (2, 24, 40), (2, 96, 128)])
-def test_fused_chain_matches_fp64_autograd(B, H4, W4):
+def test_ncup_chain_fn_matches_fp64_autograd(B, H4, W4):
     from rnc import native
     from rnc.train import NcupChainFn
     x, c, ws = chain_inputs(B, H4, W4, seed=H4 * 100 + W4)
@@ -98,7 +98,7 @@ def test_fused_chain_matches_fp64_autograd(B, H4, W4):
     host = torch.cat([w.reshape(-1) for w in ws]).float()
     hw = (ctypes.c_float * 224)(*host.tolist())
     ref_out = torch.empty_like(out)
-    native.check(L.rnc_ncup_fwd(xd.data_ptr(), cd.data_ptr(), hw, B, H4, W4, 8.0, ctypes.c_void_p(ref_out.data_ptr()),
+    native.check(L.rnc_ncup_fwd(xd.data_ptr(), cd.data_ptr(), hw, B, H4, W4, 8.0, ctypes.c_void_p(ref_out.data_ptr()), None,
                                 ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), "ncup")
     assert torch.equal(out.detach(), ref_out)
 
@@ -368,7 +368,7 @@ def test_frozen_trunk_predicate():
     assert not frozen_trunk(convex, im, im)
 
 
-def test_ncup_backward_entry_points_reject_bad_arguments():
+def test_ncup_train_entry_points_reject_bad_arguments():
     from rnc import native
     L = native.lib()
     v = ctypes.c_void_p
@@ -376,10 +376,10 @@ def test_ncup_backward_entry_points_reject_bad_arguments():
     assert L.rnc_ncup_bwd_workspace_bytes(0, 4, 4) == 0
     ws = L.rnc_ncup_bwd_workspace_bytes(2, 96, 128)
     assert ws == 8 * (12 * 16 * 4 * 196 + 196)                 # per-CTA partial rows + the reduced sums
-    assert L.rnc_ncup_bwd(p, p, p, 0, 4, 4, 8.0, p, p, p, p, p, 1 << 20, None) == -1
-    assert L.rnc_ncup_bwd(None, p, p, 1, 4, 4, 8.0, p, p, p, p, p, 1 << 20, None) == -2
-    assert L.rnc_ncup_bwd(p, p, p, 1, 4, 4, 8.0, p, None, None, None, None, 0, None) == -2
-    assert L.rnc_ncup_bwd(p, p, p, 1, 4, 4, 8.0, p, p, p, p, None, 1 << 20, None) == -2
-    assert L.rnc_ncup_bwd(p, p, p, 1, 4, 4, 8.0, p, p, p, p, p, 8, None) == -5
-    assert L.rnc_ncup_train_fwd(p, p, p, 1, 0, 4, 8.0, p, None) == -1
-    assert L.rnc_ncup_train_fwd(p, p, None, 1, 4, 4, 8.0, p, None) == -2
+    assert L.rnc_ncup_bwd(p, p, p, 0, 4, 4, 8.0, p, None, p, p, p, p, 1 << 20, None) == -1
+    assert L.rnc_ncup_bwd(None, p, p, 1, 4, 4, 8.0, p, None, p, p, p, p, 1 << 20, None) == -2
+    assert L.rnc_ncup_bwd(p, p, p, 1, 4, 4, 8.0, p, None, None, None, None, None, 0, None) == -2
+    assert L.rnc_ncup_bwd(p, p, p, 1, 4, 4, 8.0, p, None, p, p, p, None, 1 << 20, None) == -2
+    assert L.rnc_ncup_bwd(p, p, p, 1, 4, 4, 8.0, p, None, p, p, p, p, 8, None) == -5
+    assert L.rnc_ncup_train_fwd(p, p, p, 1, 0, 4, 8.0, p, None, None) == -1
+    assert L.rnc_ncup_train_fwd(p, p, None, 1, 4, 4, 8.0, p, None, None) == -2

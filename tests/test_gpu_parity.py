@@ -152,7 +152,7 @@ def test_ncup_teacher_forced(gold, it):
     assert (out.cpu() - ref).abs().max() < 5e-5 * max(1.0, ref.abs().max().item())
 
 
-def test_ncup_chain_non_multiple_of_tile(sd_ncup):
+def test_ncup_fwd_non_multiple_of_tile(sd_ncup):
     # 4*h = 88, 4*w = 104: tiles overhang; random confidences incl. exact zeros exercise the 1e-20 epsilon
     from rnc import native
     from rnc.engine import Engine
@@ -167,7 +167,7 @@ def test_ncup_chain_non_multiple_of_tile(sd_ncup):
     pu = eng.packed_upsampler(m.upsampler)
     out = torch.empty(2, 2, 88, 104, device=DEV)
     xd, cd = x.to(DEV), c.to(DEV)
-    native.rnc.ncup_fwd(xd, cd, pu.nconv_host, 2, 22, 26, 8.0, out)
+    native.rnc.ncup_fwd(xd, cd, pu.nconv_host, 2, 22, 26, 8.0, out, None)
     assert (out.cpu() - 8 * ref.view(2, 2, 88, 104)).abs().max() < 1e-4
 
 

@@ -2,13 +2,13 @@
 
     python tools/confidence_bench.py [--reps 200] [--steps 10] [--warmup 3]
 
-  kernel   rnc_ncup_fwd against rnc_ncup_conf_fwd at the benchmark shape (B = 8, H4 x W4 = 110 x 256: 440x1024 outputs),
+  kernel   rnc_ncup_fwd with conf_out NULL against non-NULL at the benchmark shape (B = 8, H4 x W4 = 110 x 256: 440x1024 outputs),
            alternating call by call, CUDA events around each call; the confidence adds one division and one 4-byte store per
            output pixel.
   frozen   a cfg-5 frozen-trunk fine-tuning step (raft_nc_dbl with freeze_raft, train mode, freeze_bn(); B = 2, 384x512,
            12 iterations; forward, sequence_loss, backward, AdamW step) without and with return_confidence, alternating step
            by step; with the confidence the step adds sum(0.01 * conf) per prediction to the loss, so its backward runs the
-           confidence adjoint (NcupChainConfFn / rnc_ncup_conf_bwd).
+           confidence adjoint (NcupChainFn with want_conf / rnc_ncup_bwd given g_conf_out).
 Medians after warm-up.  Prints one JSON line with the device name and its power limit (read-only query).  Writes nothing to
 the tree."""
 import argparse
@@ -56,8 +56,8 @@ def kernel_bench(reps, warmup):
     w = torch.cat([F.softplus(0.3 * torch.randn(n, generator=g), beta=10) for n in (50, 100, 72, 2)])
     hw = (ctypes.c_float * 224)(*w.tolist())
     out, out2, conf = (torch.empty(B, 2, 4 * H4, 4 * W4, device=dev) for _ in range(3))
-    plain = lambda: rnc.ncup_fwd(x, c, hw, B, H4, W4, 8.0, out)                # noqa: E731
-    with_conf = lambda: rnc.ncup_conf_fwd(x, c, hw, B, H4, W4, 8.0, out2, conf)   # noqa: E731
+    plain = lambda: rnc.ncup_fwd(x, c, hw, B, H4, W4, 8.0, out, None)          # noqa: E731
+    with_conf = lambda: rnc.ncup_fwd(x, c, hw, B, H4, W4, 8.0, out2, conf)     # noqa: E731
     t = {"plain": [], "conf": []}
     for i in range(warmup + reps):
         a, b = timed(plain), timed(with_conf)
@@ -115,7 +115,7 @@ def main():
     k = kernel_bench(args.reps, max(args.warmup, 10))
     f = frozen_bench(args.steps, args.warmup)
     res = {"device": torch.cuda.get_device_name(0), "power_limit_w": power_limit_w(),
-           "ncup_fwd_ms": round(k["plain"], 4), "ncup_conf_fwd_ms": round(k["conf"], 4),
+           "ncup_fwd_ms": round(k["plain"], 4), "ncup_fwd_conf_ms": round(k["conf"], 4),
            "kernel_overhead_pct": round(100 * (k["conf"] / k["plain"] - 1), 2),
            "frozen_step_ms": round(f["plain"], 2), "frozen_step_conf_ms": round(f["conf"], 2),
            "frozen_overhead_pct": round(100 * (f["conf"] / f["plain"] - 1), 2)}
