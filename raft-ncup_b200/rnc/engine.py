@@ -12,7 +12,7 @@ re-packing at load time.  All arithmetic of the path runs in librnc.so; there is
 import ctypes as C
 import os
 import threading
-from collections import OrderedDict
+from collections import OrderedDict, namedtuple
 
 import torch
 import torch.nn.functional as F
@@ -139,51 +139,70 @@ def _ceil4(c):
     return (c + 3) // 4 * 4
 
 
+class ExactWnet:
+    """The weights net's format on the exact fp32 kernels: fp32 channel-last layer outputs of ceil4 channels, a convolution
+    head's output [M, 4]."""
+    split, head_pitch = False, 4
+    pitch = staticmethod(_ceil4)
+
+    @staticmethod
+    def pack(w, b, cin):
+        return pack_conv(w, b, cin_pad=cin)
+
+    @staticmethod
+    def buffer(M, layer, device):
+        # the next layer reads the whole pitch: zero the columns the kernel does not write
+        return (torch.empty if layer.pitch == layer.cout else torch.zeros)(M, layer.pitch, dtype=torch.float32, device=device)
+
+    @staticmethod
+    def conv(eng, B, H, W, x, c, ld, layer, epi, y):
+        eng.conv(B, H, W, x.data_ptr(), c, ld, layer.wt, layer.cout, layer.k, layer.k, epi, y.data_ptr(), layer.pitch, dil=layer.dil)
+
+
+# one convolution of the weights net: packed weights, filter size, dilation, output width, and its output's form (split
+# halves or fp32) and pitch
+WnetLayer = namedtuple("WnetLayer", "wt cout k dil split pitch")
+
+
 class PackedSimple:
-    """Kernel-ready weights of the weights net Simple (interp_weights_est.py:10-47) for the exact fp32 kernels: its hidden
-    layers with eval-mode BatchNorm folded in (g[i]; layers[i] = (cout, k, dilation)) and the head `out` + sigmoid: a 1x1 head
-    runs on rnc_conf_head_fwd (gout, its weight rows padded to the input's ceil4 channels), any other on the convolution with a
-    sigmoid epilogue (g_out, head = (k, dilation))."""
+    """Kernel-ready weights of the weights net Simple (interp_weights_est.py:10-47) in one engine format fmt (ExactWnet,
+    engine_umma.UmmaWnet).  It reads cin channels of its input (zero beyond in_ch); its hidden layers, eval-mode BatchNorm folded
+    in, each read the previous output's pitch columns.  The head `out` + sigmoid: a 1x1 head on an fp32 input runs on
+    rnc_conf_head_fwd (conf_head, its weight rows padded to that pitch), any other is a convolution with a sigmoid epilogue
+    (conv_head).  The last hidden layer writes fp32 when the conf head reads it."""
 
-    def __init__(self, wn):
-        # Conv, BatchNorm, ReLU or Conv, ReLU (interp_weights_est.py:26-30)
-        convs = [fold_bn(blk[0], blk[1] if len(blk) == 3 else None) for blk in wn.conv]
-        self.layers = [(w.shape[0], blk[0].kernel_size[0], conv_dilation(blk[0])) for (w, _), blk in zip(convs, wn.conv)]
-        self.cin0_pad = _ceil4(wn.in_ch)
-        self.head = (wn.out.kernel_size[0], conv_dilation(wn.out))
-        self.gout = None
-        if self.head[0] == 1:
-            w = pack_thin(wn.out.weight)
-            cin = w.shape[1]
-            self.gout = (w if cin % 4 == 0 else F.pad(w, (0, 0, 0, _ceil4(cin) - cin)), wn.out.bias.detach().float().contiguous())
-        self.pack_convs(convs, wn.out)
-
-    def pack_convs(self, convs, out):
-        """The folded layers (and a head that is not 1x1) in the exact kernels' format; the tensor-core upsampler pack overrides
-        this.  Layer i reads ceil4 channels of the previous one (zero beyond its width)."""
-        pads = [self.cin0_pad] + [_ceil4(cout) for cout, _, _ in self.layers]
-        self.g = [pack_conv(w, b, cin_pad=p) for (w, b), p in zip(convs, pads)]
-        self.g_out = pack_conv(out.weight, out.bias, cin_pad=pads[-1]) if self.gout is None else None
+    def __init__(self, wn, fmt):
+        self.fmt, self.cin = fmt, _ceil4(wn.in_ch)
+        out, n = wn.out, len(wn.conv)
+        conf = out.kernel_size[0] == 1 and (n > 0 or not fmt.split)
+        self.layers, pitch = [], self.cin
+        for i, blk in enumerate(wn.conv):
+            w, b = fold_bn(blk[0], blk[1] if len(blk) == 3 else None)      # Conv, BatchNorm, ReLU or Conv, ReLU (:26-30)
+            cout = w.shape[0]
+            self.layers.append(WnetLayer(fmt.pack(w, b, pitch), cout, blk[0].kernel_size[0], conv_dilation(blk[0]),
+                                         fmt.split and not (conf and i == n - 1), fmt.pitch(cout)))
+            pitch = self.layers[-1].pitch
+        self.conf_head = self.conv_head = None
+        if conf:
+            w = pack_thin(out.weight)
+            self.conf_head = (F.pad(w, (0, 0, 0, pitch - w.shape[1])), out.bias.detach().float().contiguous())
+        else:
+            self.conv_head = WnetLayer(fmt.pack(out.weight, out.bias, pitch), 2, out.kernel_size[0], conv_dilation(out), False,
+                                       fmt.head_pitch)
+        self.outputs = self.layers + ([self.conv_head] if self.conv_head else [])
+        self.layout = tuple((l.cout, l.split, l.pitch) for l in self.outputs)
 
     def buffers(self, M, device):
-        """fp32 channel-last outputs of the layers for M pixels (ceil4 channels, zero-filled when that pads), then the head's
-        [M, 4] when it is a convolution."""
-        f = dict(dtype=torch.float32, device=device)
-        bufs = [(torch.empty if _ceil4(c) == c else torch.zeros)(M, _ceil4(c), **f) for c, _, _ in self.layers]
-        return bufs + ([torch.empty(M, 4, **f)] if self.gout is None else [])
-
-    # the shipped two-layer network's names
-    g0 = property(lambda self: self.g[0])
-    g1 = property(lambda self: self.g[1])
-    c_mid0 = property(lambda self: self.layers[0][0])
-    c_mid1 = property(lambda self: self.layers[1][0])
+        """The outputs of the layers, then of a convolution head, for M pixels."""
+        return [self.fmt.buffer(M, l, device) for l in self.outputs]
 
 
-class PackedUpsampler(PackedSimple):
-    """Kernel-ready weights of NConvUpsampler (upsampler.py:75-141): BN-folded weights net + softplus'd NConv weights."""
+class PackedUpsampler:
+    """Kernel-ready weights of NConvUpsampler (upsampler.py:75-141): the BN-folded weights net in one engine format (wnet) and
+    the NConvUNet: the fused network's softplus'd NConv weights (nconv_host) or the per-level chain (unet)."""
 
-    def __init__(self, up):
-        super().__init__(up.weights_est_net)
+    def __init__(self, up, fmt):
+        self.wnet = PackedSimple(up.weights_est_net, fmt)
         net = up.interpolation_net
         self.nconv_host = self.unet = None
         if is_fused(net):
@@ -268,16 +287,8 @@ class Workspace:
             self.x4 = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
             self.gin = torch.empty(M4, 132, **f)
             self.conf = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
-        self.wnet = {}              # weights-net layer outputs at 1/4 resolution, per pack layout (wnet_buffers)
-
-
-def wnet_buffers(ws, pu):
-    """The weights net's layer outputs for upsampler pack pu in workspace ws, allocated by the first (eager) forward of a shape
-    and reused by graph capture; the shipped network's are [M4, 64] and [M4, 32]."""
-    key = (type(pu).__name__, tuple(pu.layers), pu.gout is None)
-    if key not in ws.wnet:
-        ws.wnet[key] = pu.buffers(4 * ws.B * ws.H8 * ws.W8, ws.conf.device)
-    return ws.wnet[key]
+        self.wnet = {}              # weights-net layer outputs at 1/4 resolution, per PackedSimple.layout
+        self.nconv_bufs = {}        # NConvUNet chain intermediates (PackedUNet.run)
 
 
 class _Timed:
@@ -341,7 +352,7 @@ class Engine:
     forwards of one device (nn.DataParallel drives different devices from different threads: different engines)."""
     mode = "ffma"
     fork_convf1 = False
-    PACK_UB, PACK_UP = PackedUpdateBlock, PackedUpsampler
+    PACK_UB, PACK_UP = PackedUpdateBlock, ExactWnet         # PACK_UP: the upsampler's weights-net format
     WS = Workspace
     MAX_WS, MAX_PACKED = 6, 64
 
@@ -364,7 +375,7 @@ class Engine:
         return self._packed_for("ub", ub, self.PACK_UB)
 
     def packed_upsampler(self, up):
-        return self._packed_for("up", up, self.PACK_UP)
+        return self._packed_for("up", up, lambda m: PackedUpsampler(m, self.PACK_UP))
 
     def workspace(self, device, B, H8, W8, with_mask=False, with_ncup=False, mode=None):
         """Resident buffers for one problem shape, in the format of this engine's kernels, or with mode="ffma" of the exact
@@ -548,28 +559,36 @@ class Engine:
             rnc.convex_upsample_fwd(flow_low, mask_cl, ldm, ws.B, ws.H8, ws.W8, out)
         return out
 
+    def stage_guidance(self, ws, x_lowres, guid, ldg):
+        """The weights net's input [x_lowres | guidance upsampled x2 | 0 0] at 1/4 resolution, written to ws.gin -> (ws.gin,
+        its pitch)."""
+        rnc.ncup_guidance_fwd(x_lowres, guid, ldg, 128, ws.B, ws.H8, ws.W8, ws.gin, 132)
+        return ws.gin, 132
+
     def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale, want_conf=False):
         """NConvUpsampler.forward (upsampler.py:143-177) on x_lowres NCHW [B,2,H4,W4] with CL guidance guid at H8 (pixel
         stride ldg); want_conf: (out, output confidence) as ncup_chain."""
-        B, H8, W8 = ws.B, ws.H8, ws.W8
-        H4, W4 = 2 * H8, 2 * W8
-        rnc.ncup_guidance_fwd(x_lowres, guid, ldg, 128, B, H8, W8, ws.gin, 132)
-        self.weights_net(pu, B, H4, W4, ws.gin, wnet_buffers(ws, pu), ws.conf)
+        x, ld = self.stage_guidance(ws, x_lowres, guid, ldg)
+        wn = pu.wnet
+        bufs = ws.wnet.get(wn.layout)
+        if bufs is None:            # allocated by the first (eager) forward of a shape, reused by graph capture
+            bufs = ws.wnet[wn.layout] = wn.buffers(4 * ws.B * ws.H8 * ws.W8, ws.conf.device)
+        self.weights_net(wn, ws.B, 2 * ws.H8, 2 * ws.W8, x, ld, bufs, ws.conf)
         return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale, want_conf=want_conf)
 
-    def weights_net(self, pk, B, H, W, x, bufs, conf):
-        """Simple.forward (interp_weights_est.py:39-47) on the exact kernels: x fp32 CL [B*H*W, >= pk.cin0_pad] (zero beyond the
-        input channels) -> conf NCHW [B,2,H,W]; bufs = pk.buffers(B*H*W)."""
-        c, ld = pk.cin0_pad, x.shape[1]
-        for (cout, k, dil), wt, y in zip(pk.layers, pk.g, bufs):
-            self.conv(B, H, W, x.data_ptr(), c, ld, wt, cout, k, k, native.EPI_RELU, y.data_ptr(), y.shape[1], dil=dil)
-            x, c, ld = y, y.shape[1], y.shape[1]
-        if pk.gout is not None:
-            rnc.conf_head_fwd(x, c, ld, pk.gout[0], pk.gout[1], B, H, W, conf)
+    def weights_net(self, pk, B, H, W, x, ld, bufs, conf):
+        """Simple.forward (interp_weights_est.py:39-47) on the kernels of pk's format: x CL [B*H*W, >= pk.cin] of pitch ld
+        (zero beyond the input channels) -> conf NCHW [B,2,H,W]; bufs = pk.buffers(B*H*W)."""
+        c = pk.cin
+        for layer, y in zip(pk.layers, bufs):
+            pk.fmt.conv(self, B, H, W, x, c, ld, layer, native.EPI_RELU, y)
+            x, c, ld = y, layer.pitch, layer.pitch
+        if pk.conf_head is not None:
+            rnc.conf_head_fwd(x, c, ld, *pk.conf_head, B, H, W, conf)
             return
-        (k, dil), y = pk.head, bufs[-1]
-        self.conv(B, H, W, x.data_ptr(), c, ld, pk.g_out, 2, k, k, native.EPI_SIGMOID, y.data_ptr(), 4, dil=dil)
-        rnc.cl_to_nchw(y, 4, 0, B, 2, H, W, conf)
+        y = bufs[-1]
+        pk.fmt.conv(self, B, H, W, x, c, ld, pk.conv_head, native.EPI_SIGMOID, y)
+        rnc.cl_to_nchw(y, pk.conv_head.pitch, 0, B, 2, H, W, conf)
 
     def ncup_chain(self, ws, pu, x_lowres, conf, out_scale, want_conf=False):
         """Zero-stuffing + NConvUNet + out_scale (upsampler.py:150-177) on x_lowres, conf NCHW [B,2,H4,W4] -> [B,2,4*H4,4*W4]:
@@ -585,7 +604,7 @@ class Engine:
                 rnc.ncup_fwd(x_lowres, conf, pu.nconv_host, B, H4, W4, out_scale, out, cout)
             return (out, cout) if want_conf else out
         # intermediates live in the workspace (allocated by the first, eager forward of a shape; graph capture reuses them)
-        bufs = ws.__dict__.setdefault("nconv_bufs", {})
+        bufs = ws.nconv_bufs
         if "stuffed" not in bufs:
             # zero-stuffing (upsampler.py:179-210): only the lattice is ever written, so the zeros are laid down once
             bufs["stuffed"] = torch.zeros(2, B * 2, 1, 4 * H4, 4 * W4, dtype=torch.float32, device=x_lowres.device)

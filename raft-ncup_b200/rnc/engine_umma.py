@@ -5,10 +5,9 @@ planes (value = hi + lo).  Thin layers (7x7 on flow, 3x3 -> 2 flow head, 1x1 -> 
 import math
 
 import torch
-import torch.nn.functional as F
 
 from . import native
-from .engine import CORR_CH, HX_LD, Engine, PackedUpsampler, _Timed, pack_thin, wnet_buffers
+from .engine import CORR_CH, HX_LD, Engine, _Timed, pack_thin
 from .native import UmmaConvDesc, rnc
 
 CORR_LS = 88           # channels reserved per pyramid level in the resident corr row: 81 taps + 7 zero pads (16-byte groups)
@@ -116,34 +115,25 @@ def _ceil32(c):
     return (c + 31) // 32 * 32
 
 
-class PackedUpsamplerUmma(PackedUpsampler):
-    """PackedUpsampler with the weights net's BN-folded layers packed for the tensor-core path (u[i]; u0, u1 for the shipped
-    network).  Layer 0 reads the 132 channels of the guidance staging, layer i > 0 the ceil32 columns of the previous layer's
-    output (the epilogue writes whole 32-channel chunks; zero beyond the width).  A 1x1 head after a hidden layer stays on
-    rnc_conf_head_fwd, which reads that layer's fp32 output; any other head is a tensor-core layer (u_out) with a sigmoid."""
+class UmmaWnet:
+    """The weights net's format on the tensor-core path: layer outputs of ceil32 columns (the epilogue writes whole 32-channel
+    chunks; zero beyond the width) in split halves, or in fp32 where the conf head reads them; a convolution head's output
+    [M, 32].  The input is the split staging of the guidance (GIN_LD), so a head without hidden layers is a convolution."""
+    split, head_pitch = True, 32
+    pitch = staticmethod(_ceil32)
 
-    def pack_convs(self, convs, out):
-        segs = [132] + [_ceil32(cout) for cout, _, _ in self.layers]
-        self.u = [UmmaWeights(w, b, [s]) for (w, b), s in zip(convs, segs)]
-        if convs and self.gout is not None and self.gout[0].shape[1] != _ceil32(self.layers[-1][0]):
-            w = self.gout[0]                          # conf head over the ceil32 fp32 columns of the last layer
-            self.gout = (F.pad(w, (0, 0, 0, _ceil32(self.layers[-1][0]) - w.shape[1])), self.gout[1])
-        if not convs:
-            self.gout = None                          # the staging is split halves: the head is a tensor-core layer
-        self.u_out = UmmaWeights(out.weight, out.bias, [segs[-1]]) if self.gout is None else None
+    @staticmethod
+    def pack(w, b, cin):
+        return UmmaWeights(w, b, [cin])
 
-    def buffers(self, M, device):
-        """Split-halves outputs of the layers (ceil32 columns), except an fp32 one for the last layer when the conf head reads
-        it, then the head's fp32 [M, 32] when it is a tensor-core layer."""
-        bufs = [SplitBuf(M, _ceil32(cout), device) for cout, _, _ in self.layers]
-        f = dict(dtype=torch.float32, device=device)
-        if self.gout is not None:
-            bufs[-1] = torch.empty(M, _ceil32(self.layers[-1][0]), **f)
-            return bufs
-        return bufs + [torch.empty(M, 32, **f)]
+    @staticmethod
+    def buffer(M, layer, device):
+        return SplitBuf(M, layer.pitch, device) if layer.split else torch.empty(M, layer.pitch, dtype=torch.float32, device=device)
 
-    u0 = property(lambda self: self.u[0])
-    u1 = property(lambda self: self.u[1])
+    @staticmethod
+    def conv(eng, B, H, W, x, c, ld, layer, epi, y):
+        out = dict(out_split=y.ptrs(), ldo_split=layer.pitch) if layer.split else dict(out_f32=y.data_ptr(), ldo_f32=layer.pitch)
+        eng.uconv(B, H, W, x.ptrs(), c, ld, layer.wt, epi, dil=layer.dil, **out)
 
 
 class SplitBuf:
@@ -198,11 +188,12 @@ class UmmaWorkspace:
             self.gin = SplitBuf(M4, GIN_LD, device)
             self.conf = torch.empty(B, 2, 2 * H8, 2 * W8, **f)
         self.wnet = {}
+        self.nconv_bufs = {}
 
 
 class UmmaEngine(Engine):
     mode = "umma"
-    PACK_UB, PACK_UP = PackedUpdateUmma, PackedUpsamplerUmma
+    PACK_UB, PACK_UP = PackedUpdateUmma, UmmaWnet
     WS = UmmaWorkspace
 
     def __init__(self):
@@ -380,24 +371,6 @@ class UmmaEngine(Engine):
     def guidance(self, ws):
         return ws.h, 128
 
-    def ncup_from_lowres(self, ws, pu, x_lowres, guid, ldg, out_scale, want_conf=False):
-        B, H8, W8 = ws.B, ws.H8, ws.W8
-        H4, W4 = 2 * H8, 2 * W8
-        rnc.ncup_guidance_split_fwd(x_lowres, guid, ldg, 128, B, H8, W8, ws.gin.hi, ws.gin.lo, GIN_LD)
-        # Simple.forward (interp_weights_est.py:39-47)
-        x, c, ld = ws.gin.ptrs(), 132, GIN_LD
-        bufs = wnet_buffers(ws, pu)
-        for (cout, k, dil), wt, y in zip(pu.layers, pu.u, bufs):
-            if isinstance(y, SplitBuf):
-                self.uconv(B, H4, W4, x, c, ld, wt, native.EPI_RELU, out_split=y.ptrs(), ldo_split=y.ld, dil=dil)
-                x, c, ld = y.ptrs(), y.ld, y.ld
-            else:
-                self.uconv(B, H4, W4, x, c, ld, wt, native.EPI_RELU, out_f32=y.data_ptr(), ldo_f32=y.shape[1], dil=dil)
-        if pu.gout is not None:
-            y = bufs[-1]
-            rnc.conf_head_fwd(y, y.shape[1], y.shape[1], pu.gout[0], pu.gout[1], B, H4, W4, ws.conf)
-        else:
-            (k, dil), y = pu.head, bufs[-1]
-            self.uconv(B, H4, W4, x, c, ld, pu.u_out, native.EPI_SIGMOID, out_f32=y.data_ptr(), ldo_f32=32, dil=dil)
-            rnc.cl_to_nchw(y, 32, 0, B, 2, H4, W4, ws.conf)
-        return self.ncup_chain(ws, pu, x_lowres, ws.conf, out_scale, want_conf=want_conf)
+    def stage_guidance(self, ws, x_lowres, guid, ldg):
+        rnc.ncup_guidance_split_fwd(x_lowres, guid, ldg, 128, ws.B, ws.H8, ws.W8, ws.gin.hi, ws.gin.lo, GIN_LD)
+        return ws.gin, GIN_LD

@@ -15,8 +15,8 @@ import torch.nn.functional as F
 from torch.nn.modules.utils import _pair
 
 from .nconv_unet import PackedUNet, is_fused, nconv_fwd
-from .engine import (CORR_CH, HX_LD, Engine, PackedFlowHead, PackedGRU, PackedMotionEncoder, PackedSimple, _require_cuda,
-                     engine_for, module_tensors)
+from .engine import (CORR_CH, HX_LD, Engine, ExactWnet, PackedFlowHead, PackedGRU, PackedMotionEncoder, PackedSimple,
+                     _require_cuda, engine_for, module_tensors)
 from .native import rnc
 
 # --------------------------------------------------------------------------------------------- encoders (C6)
@@ -433,13 +433,13 @@ class Simple(nn.Module):
         if Cin != self.in_ch:
             raise ValueError(f"Simple: expected {self.in_ch} input channels, got {Cin}")
         with _Seam(x) as eng:
-            pk = eng._packed_for("simple", self, PackedSimple)
-            cpad = pk.cin0_pad
+            pk = eng._packed_for("simple", self, lambda wn: PackedSimple(wn, ExactWnet))
+            cpad = pk.cin
             M = B * h * w
             xin = torch.zeros(M, cpad, dtype=torch.float32, device=x.device) if cpad != Cin else torch.empty(M, cpad, dtype=torch.float32, device=x.device)
             rnc.nchw_to_cl(x.detach().float().contiguous(), B, Cin, h, w, xin, cpad, 0)
             conf = torch.empty(B, 2, h, w, dtype=torch.float32, device=x.device)
-            eng.weights_net(pk, B, h, w, xin, pk.buffers(M, x.device), conf)
+            eng.weights_net(pk, B, h, w, xin, cpad, pk.buffers(M, x.device), conf)
             return conf
 
 

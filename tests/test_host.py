@@ -215,24 +215,25 @@ def test_pack_conv_is_an_implicit_gemm_of_the_reference_conv():
     assert pw[:, :, 126:].abs().max() == 0 and pb[126:].abs().max() == 0
 
 
-def test_bn_fold_matches_eval_batchnorm():
-    from rnc.engine import PackedUpsampler
-    from rnc.engine_umma import PackedUpsamplerUmma
+def test_bn_fold_matches_eval_batchnorm_in_both_formats():
+    from rnc.engine import ExactWnet, PackedUpsampler
+    from rnc.engine_umma import UmmaWnet
     m = build_model("raft_nc_dbl")
     wn = m.upsampler.weights_est_net
     g = torch.Generator().manual_seed(0)
     for blk in wn.conv:                                                   # make the running stats non-trivial
         blk[1].running_mean.copy_(torch.randn(blk[1].num_features, generator=g) * 0.1)
         blk[1].running_var.copy_(torch.rand(blk[1].num_features, generator=g) + 0.5)
-    pu = PackedUpsampler(m.upsampler)
+    pu = PackedUpsampler(m.upsampler, ExactWnet)
+    g0 = pu.wnet.layers[0].wt
     x = torch.randn(1, 130, 6, 7, generator=g)
     ref = wn.conv[0](x)
-    w = pu.g0[0][:, :130, :64].reshape(3, 3, 130, 64).permute(3, 2, 0, 1)
-    out = F.relu(F.conv2d(x, w, pu.g0[1][:64], padding=1))
+    w = g0[0][:, :130, :64].reshape(3, 3, 130, 64).permute(3, 2, 0, 1)
+    out = F.relu(F.conv2d(x, w, g0[1][:64], padding=1))
     assert (out - ref).abs().max() < 1e-4
-    assert pu.g0[0].shape[1] == 132 and len(pu.nconv_host) == 224
+    assert g0[0].shape[1] == 132 and len(pu.nconv_host) == 224
     # the tensor-core pack of the same layer: fp16 hi/lo planes [CoutPad][9 taps * 3 blocks * 64], value (hi + lo) * unscale
-    u0 = PackedUpsamplerUmma(m.upsampler).u0
+    u0 = PackedUpsampler(m.upsampler, UmmaWnet).wnet.layers[0].wt
     w = ((u0.w_hi.float() + u0.w_lo.float()) * u0.unscale).view(u0.coutpad, 9, 192)[:64, :, :130]
     out = F.relu(F.conv2d(x, w.reshape(64, 3, 3, 130).permute(0, 3, 1, 2), u0.bias[:64], padding=1))
     assert (out - ref).abs().max() < 1e-4

@@ -109,39 +109,46 @@ def test_dilated_entry_points_reject_bad_arguments():
         assert L.rnc_conv2d_umma_fwd(ctypes.byref(v), None) == status, bad
 
 
-def test_shipped_pack_is_unchanged():
-    """The shipped network packs as before: two exact 3x3 layers (g0, g1), the fused 1x1 head (gout) and the tensor-core
-    u0 / u1 with segments [132] and [64]."""
-    from rnc.engine import PackedUpsampler
-    from rnc.engine_umma import PackedUpsamplerUmma
+def packs(up):
+    """The weights-net packs of upsampler `up` in the exact and the tensor-core format."""
+    from rnc.engine import ExactWnet, PackedSimple
+    from rnc.engine_umma import UmmaWnet
+    return PackedSimple(up.weights_est_net, ExactWnet), PackedSimple(up.weights_est_net, UmmaWnet)
+
+
+def shapes(layers):
+    return [(l.cout, l.k, l.dil) for l in layers]
+
+
+def test_shipped_layer_list_is_unchanged():
+    """The shipped network packs as before: two exact 3x3 layers, the fused 1x1 head (conf_head) and the tensor-core layers
+    with segments [132] and [64]."""
     from rnc.synth import build_model
     m = build_model("raft_nc_dbl")
-    pu = PackedUpsampler(m.upsampler)
-    assert (pu.cin0_pad, pu.c_mid0, pu.c_mid1, pu.layers) == (132, 64, 32, [(64, 3, 1), (32, 3, 1)])
-    assert pu.g0[0].shape == (9, 132, 64) and pu.g1[0].shape == (9, 64, 64) and pu.g_out is None
-    assert pu.gout[0].shape == (1, 32, 2) and torch.equal(pu.gout[0][0], m.upsampler.weights_est_net.out.weight[:, :, 0, 0].t())
-    pum = PackedUpsamplerUmma(m.upsampler)
-    assert (pum.u0.ktot, pum.u0.coutpad, pum.u1.ktot, pum.u1.coutpad) == (9 * 192, 64, 9 * 64, 32) and pum.u_out is None
-    assert pum.gout[0].shape == (1, 32, 2)
-    bufs = pum.buffers(10, "cpu")
+    pk, pkm = packs(m.upsampler)
+    assert (pk.cin, shapes(pk.layers)) == (132, [(64, 3, 1), (32, 3, 1)])
+    assert pk.layers[0].wt[0].shape == (9, 132, 64) and pk.layers[1].wt[0].shape == (9, 64, 64) and pk.conv_head is None
+    assert pk.conf_head[0].shape == (1, 32, 2)
+    assert torch.equal(pk.conf_head[0][0], m.upsampler.weights_est_net.out.weight[:, :, 0, 0].t())
+    assert [(l.wt.ktot, l.wt.coutpad) for l in pkm.layers] == [(9 * 192, 64), (9 * 64, 32)] and pkm.conv_head is None
+    assert pkm.conf_head[0].shape == (1, 32, 2)
+    bufs = pkm.buffers(10, "cpu")
     assert [b.ld for b in bufs[:1]] == [64] and bufs[1].shape == (10, 32) and len(bufs) == 2
-    assert [b.shape for b in pu.buffers(10, "cpu")] == [(10, 64), (10, 32)]
+    assert [b.shape for b in pk.buffers(10, "cpu")] == [(10, 64), (10, 32)]
 
 
-def test_variant_packs():
-    from rnc.engine import PackedUpsampler
-    from rnc.engine_umma import PackedUpsamplerUmma
+def test_variant_layer_lists():
     m = variant_model("wide_k").eval()
-    pu = PackedUpsampler(m.upsampler)
-    assert pu.layers == [(96, 5, 2), (48, 7, 1)] and pu.head == (3, 3) and pu.gout is None and pu.g_out[0].shape == (9, 48, 64)
-    pum = PackedUpsamplerUmma(m.upsampler)
-    assert pum.u1.ktot == 49 * 2 * 64 and pum.u_out.ktot == 9 * 64 and len(pum.buffers(4, "cpu")) == 3
+    pk, pkm = packs(m.upsampler)
+    assert shapes(pk.layers) == [(96, 5, 2), (48, 7, 1)] and (pk.conv_head.k, pk.conv_head.dil) == (3, 3)
+    assert pk.conf_head is None and pk.conv_head.wt[0].shape == (9, 48, 64)
+    assert pkm.layers[1].wt.ktot == 49 * 2 * 64 and pkm.conv_head.wt.ktot == 9 * 64 and len(pkm.buffers(4, "cpu")) == 3
     m = variant_model("head_only").eval()
-    pu, pum = PackedUpsampler(m.upsampler), PackedUpsamplerUmma(m.upsampler)
-    assert pu.layers == [] and pu.head == (5, 2) and pu.g_out[0].shape == (25, 132, 64)
-    assert pum.u_out.ktot == 25 * 192 and [b.shape for b in pum.buffers(4, "cpu")] == [(4, 32)]
-    narrow = PackedUpsamplerUmma(variant_model("narrow").eval().upsampler)      # 1x1 head on the 16-wide layer's 32 columns
-    assert narrow.gout[0].shape == (1, 32, 2) and narrow.gout[0][0, 16:].abs().max() == 0
+    pk, pkm = packs(m.upsampler)
+    assert pk.layers == [] and (pk.conv_head.k, pk.conv_head.dil) == (5, 2) and pk.conv_head.wt[0].shape == (25, 132, 64)
+    assert pkm.conv_head.wt.ktot == 25 * 192 and [b.shape for b in pkm.buffers(4, "cpu")] == [(4, 32)]
+    _, narrow = packs(variant_model("narrow").eval().upsampler)      # 1x1 head on the 16-wide layer's 32 columns
+    assert narrow.conf_head[0].shape == (1, 32, 2) and narrow.conf_head[0][0, 16:].abs().max() == 0
 
 
 def test_dilated_wgrad_has_no_float_atomics(tmp_path):
