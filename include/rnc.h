@@ -200,8 +200,9 @@ typedef struct {
 long long rnc_conv_umma_tiles(int kh, int kw, int stride, int B, int H, int W, int flags);
 int rnc_conv2d_umma_fwd(const rnc_conv_umma_desc* desc, void* stream);
 
-/* fp32 CL [M][lds] channels [0,C) -> split halves planes [M][ldd] at channel offset ch_off (hi + lo == value exactly
- * when |value| <= 65504). */
+/* fp32 CL [M][lds] channels [0,C) -> split halves planes [M][ldd] at channel offset ch_off, by the convolution epilogues'
+ * rule: hi = rn_satfinite(value), lo = rn_satfinite(value - hi); hi + lo reproduces |value| <= 65504 to 22 bits, carries
+ * 11 bits of the excess up to 131008 and saturates there. */
 int rnc_f32_to_split(const float* src, int lds, int C, long long M, void* dst_hi, void* dst_lo, int ldd, int ch_off,
                      void* stream);
 

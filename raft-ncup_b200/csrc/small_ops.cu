@@ -185,10 +185,11 @@ __global__ void f32_to_split_kernel(const float* __restrict__ src, int lds, int 
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const long long m = i / C;
     const int c = (int)(i - m * C);
-    const float v = fminf(fmaxf(src[m * lds + c], -65504.f), 65504.f);
-    const __half h = __float2half_rn(v);
-    hi[m * ldd + ch_off + c] = h;
-    lo[m * ldd + ch_off + c] = __float2half_rn(v - __half2float(h));
+    // the epilogues' split (split_pair): beyond 65504 lo carries the excess up to 131008, and a NaN stays a NaN
+    uint32_t h, l;
+    split_pair(src[m * lds + c], 0.f, h, l);
+    hi[m * ldd + ch_off + c] = __ushort_as_half(static_cast<unsigned short>(h & 0xffffu));
+    lo[m * ldd + ch_off + c] = __ushort_as_half(static_cast<unsigned short>(l & 0xffffu));
   }
 }
 

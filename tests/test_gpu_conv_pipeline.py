@@ -3,7 +3,8 @@ run the K loop of tile i + 1, and one wgmma batch stays in flight across ring st
 work items than SMs, so every CTA runs several tiles and the accumulator hand-off is exercised in steady state."""
 import pytest
 import torch
-import torch.nn.functional as F
+
+from test_conv_error_model import check_model, conv_split_ref
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -28,8 +29,8 @@ def _layer(cin, cout, kh, kw, B, H, W, seed):
     b = torch.randn(cout, generator=g)
     buf = SplitBuf(B * H * W, cin, DEV)
     buf.hi[:], buf.lo[:] = split(x.permute(0, 2, 3, 1).reshape(-1, cin).to(DEV))
-    ref = F.conv2d(x.double(), w.double(), b.double(), padding=(kh // 2, kw // 2))
-    return buf, UmmaWeights(w.to(DEV), b.to(DEV), [cin]), ref
+    wt = UmmaWeights(w.to(DEV), b.to(DEV), [cin])
+    return buf, wt, conv_split_ref(x.to(DEV), wt, weight=w)      # the error model of tests/test_conv_error_model.py
 
 
 # (cin, cout, kh, kw): row-halo 3x3 and 1x5, column-halo 5x1, per-tap 1x1; 32- / 64- / 128-column tiles
@@ -45,9 +46,9 @@ def test_many_tiles_per_cta_match_fp64(ueng, cin, cout, kh, kw):
     out = torch.zeros(B * H * W, wt.coutpad, device=DEV)
     ueng.uconv(B, H, W, buf.ptrs(), cin, cin, wt, native.EPI_RELU, out_f32=out.data_ptr(), ldo_f32=wt.coutpad)
     torch.cuda.synchronize()
-    got = out[:, :cout].view(B, H, W, cout).permute(0, 3, 1, 2).double().cpu()
-    exp = torch.relu(ref)
-    assert (got - exp).abs().max().item() < 2e-4 * max(1.0, exp.abs().max().item())
+    got = out[:, :cout].view(B, H, W, cout).permute(0, 3, 1, 2)
+    for against in ("split", "exact"):
+        check_model(f"{cin}->{cout} {kh}x{kw} relu", got, ref, against, act=torch.relu)
 
 
 @pytest.mark.parametrize("cin,cout,kh,kw", SHAPES)
@@ -78,7 +79,8 @@ def test_fused_stats_over_many_tiles(ueng):
                stats=stats.data_ptr())
     torch.cuda.synchronize()
     got = out[:, :cout].view(B, H * W, cout).double()
-    assert (got.permute(0, 2, 1).reshape(B, cout, H, W).cpu() - ref).abs().max().item() < 2e-4 * ref.abs().max().item()
+    for against in ("split", "exact"):
+        check_model("fused stats 64->96 3x3", got.permute(0, 2, 1).reshape(B, cout, H, W), ref, against)
     s1, s2 = got.sum(1), (got * got).sum(1)
     assert torch.allclose(stats[..., 0], s1, rtol=1e-6, atol=1e-6 * H * W)
     assert torch.allclose(stats[..., 1], s2, rtol=1e-6, atol=1e-6 * H * W)

@@ -6,6 +6,7 @@ import torch.nn.functional as F
 
 from conftest import build_model, frames
 from oracle import raft_oracle as orc
+from test_conv_error_model import check_model, conv_split_ref, split_emulate
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -50,8 +51,8 @@ def test_umma_conv_matches_fp32(ueng, cin, cout, kh, kw, act, W):
     x = torch.randn(B, cin, H, W, generator=g)
     w = torch.randn(cout, cin, kh, kw, generator=g) / (cin * kh * kw) ** 0.5
     b = torch.randn(cout, generator=g)
-    ref = F.conv2d(x.double(), w.double(), b.double(), padding=(kh // 2, kw // 2)).float()
-    ref = {"relu": F.relu, "sigmoid": torch.sigmoid, "none": lambda t: t}[act](ref)
+    s = conv_split_ref(x.to(DEV), UmmaWeights(w.to(DEV), b.to(DEV), [cin]), weight=w)
+    fn = {"relu": F.relu, "sigmoid": torch.sigmoid, "none": None}[act]
     ld = (cin + 7) // 8 * 8
     buf = SplitBuf(B * H * W, ld, DEV)
     x_cl = x.permute(0, 2, 3, 1).reshape(-1, cin).to(DEV)
@@ -62,16 +63,18 @@ def test_umma_conv_matches_fp32(ueng, cin, cout, kh, kw, act, W):
     epi = {"relu": native.EPI_RELU, "sigmoid": native.EPI_SIGMOID, "none": native.EPI_LINEAR}[act]
     ueng.uconv(B, H, W, buf.ptrs(), cin, ld, wt, epi, out_f32=out.data_ptr(), ldo_f32=wt.coutpad)
     torch.cuda.synchronize()
-    got = out[:, :cout].view(B, H, W, cout).permute(0, 3, 1, 2).cpu()
-    err = (got - ref).abs().max().item()
-    scale = max(1.0, ref.abs().max().item())
-    print(f"umma conv {cin}->{cout} {kh}x{kw}: max err {err:.2e} (scale {scale:.2f})")
-    assert err < 2e-5 * scale                                             # fp32-class accuracy (TF32 would be ~1e-3)
-    # split output of the same conv reproduces the fp32 output
+    got = out[:, :cout].view(B, H, W, cout).permute(0, 3, 1, 2)
+    # the error model of tests/test_conv_error_model.py; sigmoid_fast (ex2.approx, rcp.approx) adds < 2^-18 relative
+    extra = 2.0 ** -18 * torch.sigmoid(s.ref) if act == "sigmoid" else 0.0
+    for against in ("split", "exact"):
+        check_model(f"umma conv {cin}->{cout} {kh}x{kw} {act}", got, s, against, act=fn, floor=extra)
+    # the split output of the same conv is split_pair of the fp32 output, bit for bit
     obuf = SplitBuf(B * H * W, wt.coutpad, DEV)
     ueng.uconv(B, H, W, buf.ptrs(), cin, ld, wt, epi, out_split=obuf.ptrs(), ldo_split=wt.coutpad)
-    rec = (obuf.hi.float() + obuf.lo.float())[:, :cout]
-    assert (rec - out[:, :cout]).abs().max().item() < 1e-6 * scale + 1e-7
+    torch.cuda.synchronize()
+    eh, el = split_emulate(out[:, :cout])
+    assert torch.equal(obuf.hi[:, :cout].view(torch.int16), eh.view(torch.int16))
+    assert torch.equal(obuf.lo[:, :cout].view(torch.int16), el.view(torch.int16))
 
 
 @pytest.mark.parametrize("cout,W", [(64, 150), (96, 40), (128, 21)])
