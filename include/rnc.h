@@ -505,6 +505,20 @@ int rnc_augment(const rnc_aug_desc* desc_host, const rnc_aug_desc* desc_dev, int
                 int crop_h, int crop_w, int sparse, float* img1, float* img2, float* flow, float* valid, void* workspace,
                 size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V1  flow_to_image (core/utils/flow_viz.py:240-275, with compute_color :196-237) for a batch of float32 flows, as evaluate.py
+ * and demo.py call it before cv2.imwrite, with numpy 2.x's float32 / float64 promotion.
+ *   flow      : fp32, element (b, c, y, x) at flow[b*sb + c*sc + y*sy + x*sx] (c = 0 is u, 1 is v); 4-byte aligned
+ *   out       : uint8 [B][H][W][3] contiguous, the reference's channel order (RGB, handed unchanged to cv2.imwrite)
+ *   workspace : rnc_flow_to_image_workspace_bytes(B) bytes, 4-byte aligned, zeroed by the call (per-image maximum radius)
+ * Two launches, no host synchronisation.  Every output bit repeats from run to run.  Radius and maximum are float32, the rest
+ * float64 (np.finfo(float).eps is a float64 scalar), every step rounded as numpy rounds it.  The arc tangent is CUDA's float64
+ * atan2 (within 2 ulp) where the reference's is numpy's, so a channel could differ by one level where the two land on either
+ * side of a level boundary. */
+size_t rnc_flow_to_image_workspace_bytes(int B);   /* 0 for B <= 0 */
+int rnc_flow_to_image(const float* flow, long long sb, long long sc, long long sy, long long sx, int B, int H, int W,
+                      unsigned char* out, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

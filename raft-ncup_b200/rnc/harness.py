@@ -7,11 +7,14 @@ time (the model's batch items are independent; frames of a different size — KI
 warm-start forward interpolation runs on the GPU.  Metrics aggregate exactly as the reference's loops do: Sintel-style
 (`valid` absent) pools all pixels (evaluate.py:131-137), KITTI-style averages per-image means (evaluate.py:172-179).
 """
+import os
 from collections import deque, namedtuple
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 import torch
 
+from utils import frame_utils
 from utils.utils import InputPadder, forward_interpolate
 
 
@@ -172,6 +175,140 @@ def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mo
                     yield c.seq, c.pair, padder.unpad(flow_up[j]), padder.unpad(conf[0][j])
                 else:
                     yield c.seq, c.pair, padder.unpad(flow_up[j])
+
+
+def size_batches(items, batch_size, key):
+    """Batches of create_kitti_submission: the items of one key(item) (a frame size) in order of appearance, batch_size at a
+    time.  A batch is yielded as soon as it is full, the partial batches at the end in order of their size's first
+    appearance, so that at most batch_size items of each size are held at once."""
+    if batch_size < 1:
+        raise ValueError(f"batch_size must be >= 1, got {batch_size}")
+    open_batches = {}
+    for it in items:
+        b = open_batches.setdefault(key(it), [])
+        b.append(it)
+        if len(b) == batch_size:
+            yield open_batches.pop(key(it))
+    yield from open_batches.values()
+
+
+class _SubmissionWriter:
+    """Writes each step's flows, and with write_png their colour coding, to files on a thread pool while the next step
+    computes.  step() colour-codes the step's flows in one rnc.viz launch and enqueues their copies to pinned host buffers;
+    the pool's threads wait for those copies and encode the files (cv2.imwrite and file writes release the GIL).  The pool
+    has a thread per core this process may run on, and at most MAX_STEPS steps are in flight, so host memory stays
+    bounded.  Leaving the context waits for every file; a writer thread's exception is raised there or from step()."""
+    MAX_STEPS = 2
+
+    def __init__(self):
+        cores = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else os.cpu_count()
+        self.pool = ThreadPoolExecutor(max_workers=max(1, cores or 1), thread_name_prefix="rnc-submission")
+        self.inflight = deque()
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        try:
+            if exc_type is None:
+                while self.inflight:
+                    self._retire()
+        finally:
+            for futs in self.inflight:
+                for f in futs:
+                    f.cancel()
+            self.pool.shutdown(wait=True)
+
+    def _retire(self):
+        for f in self.inflight.popleft():
+            f.result()
+
+    def step(self, flows, files, write_flow):
+        """flows: [n,2,H,W] (any strides); files: n (flow path, png path or None); write_flow(path, [H,W,2] float32)."""
+        png = None
+        if any(p is not None for _, p in files):
+            from .viz import flow_to_image
+            png = _to_host(flow_to_image(flows))
+        flo = _to_host(flows.permute(0, 2, 3, 1))
+        done = None
+        if flows.is_cuda:
+            done = torch.cuda.Event()
+            done.record(torch.cuda.current_stream(flows.device))
+        for f, p in files:
+            os.makedirs(os.path.dirname(f) or ".", exist_ok=True)
+            if p is not None:
+                os.makedirs(os.path.dirname(p) or ".", exist_ok=True)
+        self.inflight.append([self.pool.submit(_write_pair, done, write_flow, f, flo[j], p, None if p is None else png[j])
+                              for j, (f, p) in enumerate(files)])
+        while len(self.inflight) > self.MAX_STEPS:
+            self._retire()
+
+
+def _to_host(x):
+    """Enqueue a copy of x into a contiguous (pinned, for a CUDA x) host tensor."""
+    x = x.contiguous()
+    if not x.is_cuda:
+        return x.clone()
+    return torch.empty(x.shape, dtype=x.dtype, pin_memory=True).copy_(x, non_blocking=True)
+
+
+def _write_pair(done, write_flow, flo_path, flo, png_path, png):
+    if done is not None:
+        done.synchronize()
+    write_flow(flo_path, flo.numpy())
+    if png_path is not None:
+        import cv2
+        if not cv2.imwrite(png_path, png.numpy()):
+            raise OSError(f"cv2.imwrite could not write {png_path}")
+
+
+def _model_device(model):
+    from .engine import module_device
+    return module_device(model) or torch.device("cuda", torch.cuda.current_device())
+
+
+@torch.no_grad()
+def create_sintel_submission(model, sequences, iters=32, warm_start=False, output_path="sintel_submission", write_png=False,
+                             batch_size=8):
+    """create_sintel_submission (evaluate.py:23-55) on run_sequences.  sequences: iterable of (dstype, scene, frames), frames
+    a list of [3,H,W] images of one size for all sequences.  Writes output_path/dstype/scene/frame%04d.flo for pair k (frames
+    k, k + 1) with k + 1 in the name, and with write_png its colour coding (rnc.viz, as utils.flow_viz) to
+    output_path + "_png"/dstype/scene/frame%04d.png.  Files are written on a thread pool while the next step computes;
+    returns when all are written."""
+    seqs = list(sequences)
+    frames = [f for _, _, f in seqs]
+    steps = sequence_schedule([len(f) for f in frames], batch_size)
+    flows = run_sequences(model, frames, iters=iters, warm_start=warm_start, batch_size=batch_size,
+                          device=_model_device(model))
+    with _SubmissionWriter() as w:
+        for step in steps:
+            got = [next(flows) for c in step if not c.idle]
+            files = []
+            for s, k, _ in got:
+                dstype, scene, _ = seqs[s]
+                name = "frame%04d" % (k + 1)
+                files.append((os.path.join(output_path, dstype, scene, name + ".flo"),
+                              os.path.join(output_path + "_png", dstype, scene, name + ".png") if write_png else None))
+            w.step(torch.stack([f for _, _, f in got]), files, frame_utils.writeFlow)
+
+
+@torch.no_grad()
+def create_kitti_submission(model, pairs, iters=24, output_path="kitti_submission", write_png=False, batch_size=8):
+    """create_kitti_submission (evaluate.py:58-87) in batches.  pairs: iterable of (frame_id, image1 [3,H,W], image2), of any
+    mix of sizes; pairs of one size run together, batch_size at a time (size_batches), padded as InputPadder(mode="kitti").
+    Writes output_path/frame_id (frame_utils.writeFlowKITTI) and with write_png output_path + "_png"/(frame_id + ".png").
+    Files are written on a thread pool while the next batch computes; returns when all are written."""
+    model.eval()
+    device = _model_device(model)
+    with _SubmissionWriter() as w:
+        for batch in size_batches(pairs, batch_size, key=lambda p: tuple(p[1].shape)):
+            padder = InputPadder(batch[0][1].shape, mode="kitti")
+            im1 = _stack([p[1] for p in batch], device, padder)
+            im2 = _stack([p[2] for p in batch], device, padder)
+            _, flow_pr = model(im1, im2, iters=iters, test_mode=True)
+            files = [(os.path.join(output_path, fid), os.path.join(output_path + "_png", fid + ".png") if write_png else None)
+                     for fid, _, _ in batch]
+            w.step(padder.unpad(flow_pr), files, frame_utils.writeFlowKITTI)
 
 
 def load_checkpoint(model, state):

@@ -140,6 +140,9 @@ SIGNATURES = {
     "rnc_nconv_pool2_bwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
     "rnc_augment_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
     "rnc_augment": (_i, [_vp, _vp, _i, _vp, C.c_size_t, _i, _i, _i, _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_flow_to_image_workspace_bytes": (C.c_size_t, [_i]),
+    "rnc_flow_to_image": (_i, [_vp, C.c_longlong, C.c_longlong, C.c_longlong, C.c_longlong, _i, _i, _i, _vp, _vp, C.c_size_t,
+                               _vp]),
 }
 
 _lib = None
