@@ -83,8 +83,10 @@ def test_motion_boundary_stimulus_uses_the_fallback_and_stays_exact():
 
 def test_realistic_feature_magnitudes_in_the_lookup():
     """Feature maps 30x larger than the random-init ones (trained checkpoints are not available offline): the tensor-core
-    lookup rounds features to fp16 once; its output must stay within 1e-3 relative of the exact fp32 kernel."""
+    lookup rounds features to fp16 once; its output must stay within its error model (tests/test_lookup_error_model.py) of
+    the fp64 lookup, and close to the exact fp32 CorrBlock."""
     from rnc.engine import engine_for
+    from test_gpu_lookup_error_model import umma_lookup_model
     eng = engine_for(torch.device(DEV))
     if eng.mode != "umma":
         pytest.skip("tensor-core engine only")
@@ -92,15 +94,9 @@ def test_realistic_feature_magnitudes_in_the_lookup():
     f1, f2 = torch.randn(2, 256, 55, 128, generator=g) * 45, torch.randn(2, 256, 55, 128, generator=g) * 45
     co = orc.coords_grid(2, 55, 128) + torch.randn(2, 2, 55, 128, generator=g) * 3
     from corr import CorrBlock
-    cb = CorrBlock(f1.to(DEV), f2.to(DEV))
-    exact = cb(co.to(DEV))
-    ws = eng.workspace(torch.device(DEV), 2, 55, 128, False, False)
-    with torch.cuda.device(0), eng.lock:
-        eng.fmap_prepare(ws, f1.to(DEV), f2.to(DEV), 4)
-        ws.coords1.copy_(co.to(DEV))
-        eng.lookup_resident(ws)
-        got = eng.corr_nchw(ws)
+    exact = CorrBlock(f1.to(DEV), f2.to(DEV))(co.to(DEV)).cpu()
+    got, flags = umma_lookup_model("|fmap| ~ 45", f1, f2, co)
     scale = exact.abs().max().item()
     err = (got - exact).abs().max().item()
-    print(f"lookup with |fmap| ~ 45: max err {err:.3e} on scale {scale:.1f}")
+    print(f"lookup with |fmap| ~ 45: max err {err:.3e} on scale {scale:.1f} vs CorrBlock, {int(flags.sum())} units flagged")
     assert err < 1e-3 * scale

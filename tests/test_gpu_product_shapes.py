@@ -15,7 +15,7 @@ import torch.nn.functional as F
 
 from conftest import build_model
 from oracle import raft_oracle as orc
-from test_product_shapes import CFG5_CONV_SIGNATURES, SHAPES, TOL, cl, compare, fp16_tol, unblock
+from test_product_shapes import CFG5_CONV_SIGNATURES, SHAPES, TOL, cl, compare, unblock
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
@@ -222,17 +222,20 @@ class Recorder:
             ref = self.grid + (self.flow_init.double() if self.flow_init is not None else 0)
             self.cmp(st, ws.coords1, ref, TOL["move"])
         elif st == "lookup":
-            ref, f1, f2 = self.lookup_ref(self.pending.pop("lookup"))
-            if self.umma:
-                got = self.eng.corr_nchw(ws)
-            else:
-                got = cl(ws.corr, B, H, W)
+            coords = self.pending.pop("lookup")
             if self.umma and self.eng.lookup_mode == "umma":
+                # the error model of tests/test_lookup_error_model.py: tensor-core units against the fp64 lookup of the
+                # halves, flagged units against the fp64 lookup of the fp32 features, flags against the host records
+                from test_gpu_lookup_error_model import check_launch
+                lv, _, wr, ex = check_launch(f"{self.tag} lookup", ws, self.eng.corr_nchw(ws), coords.cpu())
+                self.worst[st] = max(self.worst.get(st, 0.0), wr, ex, *(r for r, _ in lv))
                 self.fallback = int(ws.lookup_flags.sum())
-                self.cmp(st + " (tensor cores)", got, ref, 0.0, fp16_tol(f1, f2))
-                print(f"  {self.tag} lookup: fallback tiles {self.fallback}/{ws.lookup_flags.numel()}")
-            else:
-                self.cmp(st + " (exact)", got, ref, TOL["lookup_exact"])
+                print(f"  {self.tag} lookup: fallback tiles {self.fallback}/{ws.lookup_flags.numel()}, C_A needed per level "
+                      f"{', '.join(f'{c:.3f}' for _, c in lv)}")
+                return
+            ref, f1, f2 = self.lookup_ref(coords)
+            got = self.eng.corr_nchw(ws) if self.umma else cl(ws.corr, B, H, W)
+            self.cmp(st + " (exact)", got, ref, TOL["lookup_exact"])
         elif st == "convc1":
             x = self.eng.corr_nchw(ws).double() if self.umma else cl(ws.corr, B, H, W).double()
             self.cmp(st, self.nchw(self.val(ws.c1), 0, 256), F.relu(self.conv(p + "encoder.convc1", x)), TOL["conv"])

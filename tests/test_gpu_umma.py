@@ -274,19 +274,17 @@ def resident_lookup(f1, f2, coords, lookup_mode):
     return eng.corr_nchw(ws).cpu(), flags                                   # resident channel order -> reference order
 
 
-def fp16_tol(f1, f2):
-    # |err| of a 256-term dot product of fp16-rounded operands / 16: ~ sqrt(256) * |f1||f2| * 2^-11 * sqrt(2) / 16
-    return 6.0 * (256 ** 0.5) * f1.abs().max().item() * f2.abs().max().item() * 2.0 ** -11 / 16 / 4
-
-
 @pytest.mark.parametrize("it", [0, 3])
 def test_umma_lookup_matches_reference_golden(gold, it):
-    out, flags = resident_lookup(gold["fmap1"], gold["fmap2"], gold[f"coords_it{it}"], "umma")
+    """The tensor-core lookup on the reference's features and coordinates: within its error model
+    (tests/test_lookup_error_model.py) of the fp64 lookup, and close to the reference's own output."""
+    from test_gpu_lookup_error_model import umma_lookup_model
+    out, flags = umma_lookup_model(f"golden it{it}", gold["fmap1"], gold["fmap2"], gold[f"coords_it{it}"])
     ref = gold[f"corr_it{it}"]
     err = (out - ref).abs()
     print(f"umma lookup it{it}: max err {err.max():.2e} mean {err.mean():.2e} (|ref| max {ref.abs().max():.1f}), fallback tiles {int(flags.sum())}")
     assert flags.sum() == 0
-    assert err.max() < fp16_tol(gold["fmap1"], gold["fmap2"]) and err.mean() < 1e-3
+    assert err.mean() < 1e-3
     exact, _ = resident_lookup(gold["fmap1"], gold["fmap2"], gold[f"coords_it{it}"], "ffma")
     assert (exact - ref).abs().max() < 1e-4
 
@@ -302,20 +300,25 @@ def test_umma_lookup_full_size_borders_and_fallback():
     flow[1, :, 20:30, 40:70] += torch.randn(2, 10, 30, generator=g) * 12
     flow[0, :, 0, 0] = torch.tensor([1e9, -1e9])
     co = orc.coords_grid(B, H, W) + flow
-    out, flags = resident_lookup(f1, f2, co, "umma")
+    from test_gpu_lookup_error_model import umma_lookup_model
+    out, flags = umma_lookup_model("55x128 borders and fallback", f1, f2, co)
     exact, _ = resident_lookup(f1, f2, co, "ffma")
     nf = int(flags.sum())
     err = (out - exact).abs()
     print(f"umma lookup 55x128: max err {err.max():.2e} mean {err.mean():.2e}, fallback tiles {nf}/{flags.numel()}")
     assert 0 < nf < flags.numel() // 2
-    assert err.max() < fp16_tol(f1, f2) and err.mean() < 1e-3
+    assert err.mean() < 1e-3
     # spot check the exact path itself against the oracle on one image
     ref = orc.corr_lookup_direct(f1[:1], f2[:1], co[:1].clamp(-1e6, 1e6))
     assert (exact[:1] - ref).abs().max() < 2e-4
 
 
 def test_umma_lookup_odd_size(gold):
-    out, flags = resident_lookup(gold["odd_f1"], gold["odd_f2"], gold["odd_coords"], "umma")
+    """17x21 (ragged tiles in both directions): within the model of the fp64 lookup, pointwise within that bound plus the
+    fp32 bound of the reference's own output, and close to it on average."""
+    from test_gpu_lookup_error_model import umma_lookup_model
+    out, flags = umma_lookup_model("17x21 randn*6", gold["odd_f1"], gold["odd_f2"], gold["odd_coords"], golden=gold["odd_corr"])
     err = (out - gold["odd_corr"]).abs()
-    print(f"umma lookup 17x21 randn*6: max err {err.max():.2e}, fallback tiles {int(flags.sum())}/{flags.numel()}")
-    assert err.max() < fp16_tol(gold["odd_f1"], gold["odd_f2"])
+    print(f"umma lookup 17x21 randn*6: max err {err.max():.2e} mean {err.mean():.2e} vs the reference's output, fallback tiles "
+          f"{int(flags.sum())}/{flags.numel()}")
+    assert err.mean() < 1e-3

@@ -34,12 +34,6 @@ TOL = {
 }
 
 
-def fp16_tol(f1, f2):
-    """Tolerance of the tensor-core lookup (fp16-rounded operands, test_gpu_umma.py::fp16_tol): |err| of a 256-term dot product
-    of fp16-rounded operands / 16 ~ sqrt(256) * |f1||f2| * 2^-11 * sqrt(2) / 16."""
-    return 6.0 * (256 ** 0.5) * float(f1.abs().max()) * float(f2.abs().max()) * 2.0 ** -11 / 16 / 4
-
-
 class Mismatch(AssertionError):
     pass
 
