@@ -41,35 +41,44 @@ def _coutpad(cout):
 
 
 class UmmaWeights:
-    """[Cout,Cin,KH,KW] -> hi/lo halves planes [CoutPad][taps * blocks * 64] scaled by 2^s (s chosen so the largest
-    weight lands in [512, 1024): w_lo then stays a normal half) + fp32 bias [CoutPad] + unscale = 2^-s."""
+    """[Cout,Cin,KH,KW] -> hi/lo operand planes [CoutPad][taps * blocks * bk] + fp32 bias [CoutPad] + unscale.
+    fp16 (default): halves in 64-channel K blocks, scaled by 2^s (s chosen so the largest weight lands in [512, 1024): w_lo
+    then stays a normal half), unscale = 2^-s.
+    tf32: the RNC_CONV_TF32 format, fp32 planes in 32-channel K blocks (hi = w rounded to TF32, ties away from zero; lo = w - hi),
+    unscale = 1: fp32's exponent range needs no scaling, and no device sync (training re-packs every step)."""
 
-    def __init__(self, weight, bias, segs, extra_cout=0, out_scale=1.0, scale_log2=None):
+    def __init__(self, weight, bias, segs, extra_cout=0, out_scale=1.0, tf32=False):
         cout, cin, kh, kw = weight.shape
-        w = weight.detach().float() * out_scale
-        nblks = [(c + 63) // 64 for c in segs]
+        w = weight.detach().float()
+        if out_scale != 1.0:                                 # (training re-packs every step: no pass for a scale of 1)
+            w = w * out_scale
+        bk = 32 if tf32 else 64
+        nblks = [(c + bk - 1) // bk for c in segs]
         nblk = sum(nblks)
         self.cout, self.kh, self.kw = cout, kh, kw
         self.coutpad = _coutpad(cout + extra_cout)
-        self.ktot = kh * kw * nblk * 64
-        wp = torch.zeros(self.coutpad, kh * kw, nblk * 64, dtype=torch.float32, device=w.device)
+        self.ktot = kh * kw * nblk * bk
+        wp = torch.zeros(self.coutpad, kh * kw, nblk * bk, dtype=torch.float32, device=w.device)
         ci = col = 0
         for c, nb in zip(segs, nblks):
             take = min(c, cin - ci)
             if take > 0:
                 wp[:cout, :, col:col + take] = w[:, ci:ci + take].permute(0, 2, 3, 1).reshape(cout, kh * kw, take)
             ci += take
-            col += nb * 64
+            col += nb * bk
         assert ci == cin, "segments do not cover the weight's input channels"
-        if scale_log2 is None:
+        ws = wp.reshape(self.coutpad, self.ktot)
+        if tf32:
+            self.w_hi = ((ws.view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32).contiguous()
+            self.w_lo = (ws - self.w_hi).contiguous()
+            self.unscale = 1.0
+        else:
             mx = float(wp.abs().max())                       # (one device sync; inference packs once per checkpoint)
             s = math.floor(math.log2(1000.0 / mx)) if mx > 0 else 0
-        else:
-            s = scale_log2                                   # training re-packs every step: fixed scale, no sync (|w| < 2^(15-s))
-        ws = wp.reshape(self.coutpad, self.ktot) * (2.0 ** s)
-        self.w_hi = ws.half().contiguous()
-        self.w_lo = (ws - self.w_hi.float()).half().contiguous()
-        self.unscale = 2.0 ** (-s)
+            ws = ws * (2.0 ** s)
+            self.w_hi = ws.half().contiguous()
+            self.w_lo = (ws - self.w_hi.float()).half().contiguous()
+            self.unscale = 2.0 ** (-s)
         self.bias = torch.zeros(self.coutpad, dtype=torch.float32, device=w.device)
         if bias is not None:
             self.bias[:cout] = bias.detach().float() * out_scale

@@ -28,6 +28,7 @@ in the reference) are plain torch ops — plumbing around the kernels above.  `s
 process per GPU and a bucketed NCCL all-reduce of the 4.9 M fp32 gradients.
 """
 import copy
+import os
 
 import torch
 import torch.nn as nn
@@ -35,6 +36,7 @@ import torch.nn.functional as F
 
 from . import native
 from .engine import CORR_CH, _require_cuda, engine_for, pack_conv
+from .engine_umma import UmmaWeights, _ceil32
 from .native import rnc
 from .nconv_unet import is_fused, live_chain, nconv_fwd, pool_fwd, unused_parameters
 
@@ -43,9 +45,9 @@ _PACK_CACHE = {}          # (id(weight), version, kind, fmt, cin_pad) -> (weight
 
 def _packed(weight, kind, cin_pad, fmt="ffma"):
     """Kernel-ready copy of a convolution weight ('fwd') or of its flipped transpose ('dgrad'), cached for the 12 iterations of a
-    step, in the operand format of the exact kernel (fmt 'ffma': pack_conv) or of the tensor-core kernel ('f16': UmmaWeights,
-    'tf32': _WeightsTF32).  The entry keeps the weight tensor alive, so neither its id nor its storage can be recycled while the
-    entry exists."""
+    step, in the operand format of the exact kernel (fmt 'ffma': pack_conv) or of the TF32 tensor-core kernel ('tf32':
+    UmmaWeights(tf32=True)).  The entry keeps the weight tensor alive, so neither its id nor its storage can be recycled while
+    the entry exists."""
     key = (id(weight), weight._version, kind, fmt, cin_pad)
     hit = _PACK_CACHE.get(key)
     if hit is None or hit[0] is not weight:
@@ -55,17 +57,7 @@ def _packed(weight, kind, cin_pad, fmt="ffma"):
         if kind == "dgrad":          # Wd[ci, co, ky, kx] = W[co, ci, kh-1-ky, kw-1-kx]
             w = w.flip(2, 3).transpose(0, 1)
         w = w.contiguous()
-        if fmt == "ffma":
-            packed = pack_conv(w, None, cin_pad=cin_pad)
-        elif fmt == "tf32":
-            packed = _WeightsTF32(w, cin_pad)
-        else:
-            from .engine_umma import UmmaWeights
-            if w.shape[1] != cin_pad:
-                w = F.pad(w, (0, 0, 0, 0, 0, cin_pad - w.shape[1]))
-            # fixed scale 2^10 (no device sync per pack): exact for |w| < 32; a lo part below the half normal range only costs an
-            # absolute 2^-34 per weight
-            packed = UmmaWeights(w, None, [cin_pad], scale_log2=10)
+        packed = pack_conv(w, None, cin_pad=cin_pad) if fmt == "ffma" else UmmaWeights(w, None, [cin_pad], tf32=True)
         hit = _PACK_CACHE[key] = (weight, packed)
     return hit[1]
 
@@ -87,45 +79,20 @@ def _conv_mode():
       tf32            wgmma .tf32 on TF32 hi/lo operand planes, 3 MMAs per K step (x_hi*w_hi + x_hi*w_lo + x_lo*w_hi):
                       ~2^-21 per product (per-layer 1e-6 .. 5e-6) with fp32's exponent range, so output gradients of 1e-9
                       survive; 112 ms per step, ill-conditioned parameters (cnet.conv1) move to 5e-3
-      umma            fp16 hi/lo split operands (the inference kernels): output gradients underflow the split's normal range —
-                      per-parameter gradient errors of 5e-3 (forward only) to 4e-2 (with RNC_TRAIN_DGRAD=umma)
-    Parity first: the default is the exact path; the tensor-core forms are opt-in and reported beside it by bench.py."""
-    import os
-    return os.environ.get("RNC_TRAIN_CONV", "ffma")
+    The inference kernels' fp16 hi/lo split is not offered: output gradients fall below its normal range (DESIGN.md §3.8).
+    Parity first: the default is the exact path; the tensor-core form is opt-in and reported beside it by bench.py.  Read at
+    every call, so a process may switch between steps."""
+    mode = os.environ.get("RNC_TRAIN_CONV", "ffma")
+    if mode not in ("ffma", "tf32"):
+        raise ValueError(f"RNC_TRAIN_CONV={mode!r}: expected 'ffma' or 'tf32'")
+    return mode
 
 
-def _umma_ok(eng, Cx, cout, dgrad=False):
-    """Can this layer run on the tensor-core convolution?  The kernel stores whole 32-channel chunks of fp32 output, so the
-    output row must not need wider padding than the channel-last tensors use; the fp16 form also needs a pitch of 8 halves."""
-    import os
-    mode = _conv_mode()
-    if eng.mode != "umma" or mode == "ffma" or (cout + 31) // 32 * 32 != _ceil4(cout):
-        return None
-    if mode == "tf32":
-        return "tf32" if Cx % 4 == 0 else None
-    if dgrad and os.environ.get("RNC_TRAIN_DGRAD", "ffma") != "umma":
-        return None
-    return "f16" if Cx % 8 == 0 and Cx >= 32 and cout >= 32 else None
-
-
-class _WeightsTF32:
-    """[Cout,Cin,KH,KW] -> TF32 hi/lo planes of floats [CoutPad][taps * blocks * 32] (hi = round-to-nearest TF32, lo = w - hi), the
-    operand format of RNC_CONV_TF32 layers; no scaling is needed (fp32 exponent range)."""
-
-    def __init__(self, w, cin_pad):
-        from .engine_umma import _coutpad
-        cout, cin, kh, kw = w.shape
-        nblk = (cin_pad + 31) // 32
-        self.cout, self.kh, self.kw = cout, kh, kw
-        self.coutpad = _coutpad(cout)
-        self.ktot = kh * kw * nblk * 32
-        wp = torch.zeros(self.coutpad, kh * kw, nblk * 32, dtype=torch.float32, device=w.device)
-        wp[:cout, :, :cin] = w.permute(0, 2, 3, 1).reshape(cout, kh * kw, cin)
-        ws = wp.reshape(self.coutpad, self.ktot)
-        self.w_hi = ((ws.view(torch.int32) + 0x1000) & ~0x1FFF).view(torch.float32).contiguous()
-        self.w_lo = (ws - self.w_hi).contiguous()
-        self.unscale = 1.0
-        self.bias = torch.zeros(self.coutpad, dtype=torch.float32, device=w.device)
+def _tf32_ok(eng, Cx, cout):
+    """Does this layer run on the TF32 tensor-core convolution (RNC_TRAIN_CONV=tf32 on the tensor-core engine)?  The kernel
+    stores whole 32-channel chunks of fp32 output, so the output row must not need wider padding than the channel-last tensors
+    use, and the operand planes need a pitch of 4 floats."""
+    return _conv_mode() == "tf32" and eng.mode == "umma" and _ceil32(cout) == _ceil4(cout) and Cx % 4 == 0
 
 
 def _padded_bias(packed_bias, bias):
@@ -136,24 +103,22 @@ def _padded_bias(packed_bias, bias):
     return b
 
 
-def _conv_launch_umma(eng, x, wt, cout, stride=1, bias=None, fmt="f16", dil=1):
-    """Same contract as _conv_launch on the tensor-core path: x fp32 CL -> hi/lo operand planes (halves or TF32 words) ->
-    rnc_conv2d_umma_fwd with an fp32 channel-last output; stride 2 is native (TMA element strides), no subsampling pass."""
+def _conv_launch_tf32(eng, x, wt, cout, stride=1, bias=None, dil=1):
+    """Same contract as _conv_launch on the TF32 tensor-core path: x fp32 CL -> TF32 hi/lo operand planes -> rnc_conv2d_umma_fwd
+    with an fp32 channel-last output; stride 2 is native (TMA element strides), no subsampling pass."""
     B, H, W, Cx = x.shape
     Ho, Wo = (H + stride - 1) // stride, (W + stride - 1) // stride
     M = B * H * W
-    dt = torch.float32 if fmt == "tf32" else torch.float16
-    hi = torch.empty(M, Cx, dtype=dt, device=x.device)
-    lo = torch.empty(M, Cx, dtype=dt, device=x.device)
-    split = rnc.f32_to_tf32_split if fmt == "tf32" else rnc.f32_to_split
-    split(x, Cx, Cx, M, hi, lo, Cx, 0)
+    hi = torch.empty(M, Cx, dtype=torch.float32, device=x.device)
+    lo = torch.empty(M, Cx, dtype=torch.float32, device=x.device)
+    rnc.f32_to_tf32_split(x, Cx, Cx, M, hi, lo, Cx, 0)
     ldo = _ceil4(cout)
     out = torch.empty(B, Ho, Wo, ldo, dtype=torch.float32, device=x.device)
     if bias is not None:
         wt = copy.copy(wt)
         wt.bias = _padded_bias(wt.bias, bias)
     eng.uconv(B, Ho, Wo, (hi.data_ptr(), lo.data_ptr()), Cx, Cx, wt, native.EPI_LINEAR, out_f32=out.data_ptr(), ldo_f32=ldo,
-              stride=stride, hin=H, win=W, flags=eng.conv_flags | (native.CONV_TF32 if fmt == "tf32" else 0), dil=dil)
+              stride=stride, hin=H, win=W, flags=eng.conv_flags | native.CONV_TF32, dil=dil)
     return out
 
 
@@ -170,6 +135,17 @@ def _conv_launch(eng, x, packed, cout, kh, kw, bias=None, dil=1):
     return out
 
 
+def _conv(eng, x, weight, kind, cout, stride=1, bias=None, dil=1):
+    """x CL [B,H,W,Cx] -> CL [B,Ho,Wo,ceil4(cout)]: the convolution by `weight` ('fwd') or by its flipped transpose ('dgrad'),
+    on the TF32 tensor-core form where _tf32_ok allows it, else exact fp32."""
+    Cx = x.shape[-1]
+    if _tf32_ok(eng, Cx, cout):
+        return _conv_launch_tf32(eng, x, _packed(weight, kind, Cx, "tf32"), cout, stride, bias, dil)
+    kh, kw = weight.shape[2:]
+    y = _conv_launch(eng, x, _packed(weight, kind, Cx), cout, kh, kw, bias, dil)
+    return y[:, ::2, ::2].contiguous() if stride == 2 else y      # same padding: out(y, x) of the strided conv = full(2y, 2x)
+
+
 class ConvCL(torch.autograd.Function):
     """y = conv2d(x, weight, bias, stride, padding = (k // 2) * dil, dilation = dil) on channel-last tensors (dil > 1: stride 1).
     x [B,H,W,Cx] (Cx = ceil4(Cin); channels beyond Cin must be zero), weight [Cout,Cin,kh,kw] -> y [B,Ho,Wo,ceil4(Cout)]."""
@@ -184,13 +160,7 @@ class ConvCL(torch.autograd.Function):
             raise ValueError("ConvCL: input must be channel-last with ceil4(Cin) channels")
         if stride not in (1, 2) or (dil > 1 and stride != 1):
             raise NotImplementedError("stride 1 or 2; dilated layers at stride 1")
-        fmt = _umma_ok(eng, Cx, cout)
-        if fmt:
-            y = _conv_launch_umma(eng, x, _packed(weight, "fwd", Cx, fmt), cout, stride, bias, fmt, dil)
-        else:
-            y = _conv_launch(eng, x, _packed(weight, "fwd", Cx), cout, kh, kw, bias, dil)
-            if stride == 2:
-                y = y[:, ::2, ::2].contiguous()      # same padding: out(y, x) of the strided conv = full(2y, 2x)
+        y = _conv(eng, x, weight, "fwd", cout, stride, bias, dil)
         ctx.save_for_backward(x, weight)
         ctx.stride, ctx.dil, ctx.has_bias = stride, dil, bias is not None
         return y
@@ -212,11 +182,7 @@ class ConvCL(torch.autograd.Function):
                     g_full = torch.zeros(B, H, W, ldg, dtype=torch.float32, device=x.device)
                     g_full[:, ::2, ::2] = gy
                 # the same (dilated) convolution with the flipped, transposed weights: its padding (k // 2) * dil is symmetric
-                fmt = _umma_ok(eng, ldg, cin, dgrad=True)
-                if fmt:
-                    gx = _conv_launch_umma(eng, g_full, _packed(weight, "dgrad", ldg, fmt), cin, fmt=fmt, dil=dil)
-                else:
-                    gx = _conv_launch(eng, g_full, _packed(weight, "dgrad", ldg), cin, kh, kw, dil=dil)
+                gx = _conv(eng, g_full, weight, "dgrad", cin, dil=dil)
                 if gx.shape[-1] != Cx:               # Cx > ceil4(cin) never happens; equal by construction
                     gx = F.pad(gx, (0, Cx - gx.shape[-1]))
             if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):

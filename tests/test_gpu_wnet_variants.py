@@ -50,10 +50,14 @@ def layer_data(B, H, W, cin, cout, k, dil):
 
 
 @pytest.mark.parametrize("shape", LAYERS)
-def test_dilated_conv_forward_matches_fp64(shape):
+def test_dilated_conv_operand_forms_match_fp64(shape):
+    """The dilated convolution's forward on each operand form against fp64: exact fp32 (CUDA cores), the training path's TF32
+    hi/lo planes, and the inference weights net's fp16 hi/lo split, launched directly."""
+    from rnc import native
     from rnc.engine import engine_for
     from rnc.engine_umma import UmmaWeights
-    from rnc.train import _conv_launch, _conv_launch_umma, _packed, _WeightsTF32, to_cl
+    from rnc.native import rnc
+    from rnc.train import _conv_launch, _conv_launch_tf32, _packed, to_cl
     B, H, W, cin, cout, k, dil = shape
     x, w, b, ref = layer_data(*shape)
     ref_cl = ref.permute(0, 2, 3, 1)
@@ -63,9 +67,17 @@ def test_dilated_conv_forward_matches_fp64(shape):
     scale = ref.abs().max().item()
     exact = _conv_launch(eng, xc, _packed(w.to(DEV), "fwd", Cx), cout, k, k, b.to(DEV), dil=dil)
     assert (exact[..., :cout].cpu().double() - ref_cl).abs().max() < 5e-6 * scale
-    for fmt, wt in (("tf32", _WeightsTF32(w.to(DEV), Cx)), ("f16", UmmaWeights(F.pad(w, (0, 0, 0, 0, 0, Cx - cin)).to(DEV), None, [Cx]))):
-        # the epilogue stores whole 32-channel chunks: an output pitch of ceil32(cout)
-        out = _conv_launch_umma(eng, xc, wt, (cout + 31) // 32 * 32, 1, b.to(DEV), fmt, dil)
+    # the epilogue stores whole 32-channel chunks: an output pitch of ceil32(cout)
+    ldo = (cout + 31) // 32 * 32
+    tf32 = _conv_launch_tf32(eng, xc, UmmaWeights(w.to(DEV), None, [Cx], tf32=True), ldo, 1, b.to(DEV), dil)
+    # fp16 hi/lo split operands, the format of the inference weights net (UmmaWnet)
+    M = B * H * W
+    hi, lo = (torch.empty(M, Cx, dtype=torch.float16, device=DEV) for _ in range(2))
+    rnc.f32_to_split(xc, Cx, Cx, M, hi, lo, Cx, 0)
+    f16 = torch.empty(B, H, W, ldo, dtype=torch.float32, device=DEV)
+    eng.uconv(B, H, W, (hi.data_ptr(), lo.data_ptr()), Cx, Cx, UmmaWeights(w.to(DEV), b.to(DEV), [Cx]), native.EPI_LINEAR,
+              out_f32=f16.data_ptr(), ldo_f32=ldo, dil=dil)
+    for fmt, out in (("tf32", tf32), ("f16", f16)):
         assert (out[..., :cout].cpu().double() - ref_cl).abs().max() < 2e-5 * scale, fmt
 
 
