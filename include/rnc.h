@@ -519,6 +519,23 @@ size_t rnc_flow_to_image_workspace_bytes(int B);   /* 0 for B <= 0 */
 int rnc_flow_to_image(const float* flow, long long sb, long long sc, long long sy, long long sx, int B, int H, int W,
                       unsigned char* out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V2  validation metrics (evaluate.py:88-182 validate_chairs / validate_sintel / validate_kitti) for a batch of float32 flows.
+ *   flow, gt  : fp32, element (b, c, y, x) at flow[b*fb + c*fc + y*fy + x*fx] (gt likewise; c = 0 is u, 1 is v); 4-byte aligned
+ *   valid     : fp32, pixel (b, y, x) at valid[b*vb + y*vy + x*vx], valid where >= 0.5; NULL: every pixel is valid
+ *   counts    : int64 [B][5], per image the valid pixels, of them epe < 1, < 3, < 5, and KITTI outliers
+ *               (epe > 3 and epe / |gt| > 0.05); 8-byte aligned
+ *   epe_sum   : fp64 [B], per image the sum of the valid pixels' epe; 8-byte aligned
+ *   workspace : rnc_flow_metrics_workspace_bytes(B, H, W) bytes, 16-byte aligned, no zeroing needed (per-CTA partials)
+ * Each pixel is rounded as torch's float32 formulas round it (no FMA; IEEE division, so x/0 = inf and 0/0 = NaN).  Two launches,
+ * no host synchronisation; the sums are added in a fixed order that depends only on H*W, so an image's results are bit for
+ * bit the same whatever B, its position in the batch or the GPU.  Bad arguments return before any launch. */
+size_t rnc_flow_metrics_workspace_bytes(int B, int H, int W);   /* 0 for a bad shape */
+int rnc_flow_metrics(const float* flow, long long fb, long long fc, long long fy, long long fx, const float* gt, long long gb,
+                     long long gc, long long gy, long long gx, const float* valid, long long vb, long long vy, long long vx,
+                     int B, int H, int W, long long* counts, double* epe_sum, void* workspace, size_t workspace_bytes,
+                     void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -17,6 +17,59 @@ def shard_range(n, world, rank):
     return lo, lo + base + (1 if rank < extra else 0)
 
 
+def world_rank():
+    """(world size, rank) of the initialised process group, or (1, 0)."""
+    if dist.is_initialized():
+        return dist.get_world_size(), dist.get_rank()
+    return 1, 0
+
+
+def strided_items(items, world, rank):
+    """The items of index = rank (mod world), in order (validate's samples, create_kitti_submission's pairs).  A sequence (len
+    and indexing, such as the reference's FlowDataset) is indexed, so only this rank's items are loaded; any other iterable is
+    walked and filtered."""
+    if world <= 0 or not (0 <= rank < world):
+        raise ValueError("bad world/rank")
+    if world == 1:
+        return iter(items)
+    if hasattr(items, "__len__") and hasattr(items, "__getitem__") and not isinstance(items, dict):
+        return (items[i] for i in range(rank, len(items), world))
+    return (it for i, it in enumerate(items) if i % world == rank)
+
+
+def greedy_assignment(sizes, world):
+    """Rank of each item for `world` ranks by longest-first greedy on `sizes` (create_sintel_submission: whole sequences by pair
+    count): items in decreasing size, ties by index, each to the least loaded rank, ties to the lowest rank."""
+    if world <= 0:
+        raise ValueError("bad world")
+    load = [0] * world
+    owner = [0] * len(sizes)
+    for i in sorted(range(len(sizes)), key=lambda i: (-sizes[i], i)):
+        r = min(range(world), key=lambda r: (load[r], r))
+        owner[i] = r
+        load[r] += sizes[i]
+    return owner
+
+
+def gather_strided(local, world):
+    """Every rank's list of `local` objects (rank r's holding the items of index = r (mod world), in order), all-gathered and
+    interleaved back into the global order.  Returns `local` itself at world 1."""
+    if world == 1:
+        return local
+    parts = [None] * world
+    dist.all_gather_object(parts, local)
+    out = []
+    for k in range(max(len(p) for p in parts)):
+        out.extend(p[k] for p in parts if k < len(p))
+    return out
+
+
+def barrier():
+    """dist.barrier() when more than one rank runs."""
+    if dist.is_initialized() and dist.get_world_size() > 1:
+        dist.barrier()
+
+
 def infer_sharded(fn, image1, image2, gather=True, **kw):
     """Run `fn(image1_shard, image2_shard, **kw) -> (flow_low, flow_up)` on this rank's slice of the batch.
     With gather=True every rank returns the full-batch results (all_gather of the per-rank outputs, padded to the

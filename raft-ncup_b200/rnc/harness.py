@@ -4,65 +4,109 @@ themselves are out of scope (no data offline, SURVEY.md C12), so `bench.py` / th
 
 Differences from the reference, all behaviour-preserving: pairs of equal size are evaluated in batches instead of one at a
 time (the model's batch items are independent; frames of a different size — KITTI's vary — start a new batch), and the
-warm-start forward interpolation runs on the GPU.  Metrics aggregate exactly as the reference's loops do: Sintel-style
-(`valid` absent) pools all pixels (evaluate.py:131-137), KITTI-style averages per-image means (evaluate.py:172-179).
+warm-start forward interpolation runs on the GPU.  Metrics aggregate as the reference's loops do (rnc.metrics): Sintel-style
+(`valid` absent) pools all pixels (evaluate.py:131-137), KITTI-style averages per-image means (evaluate.py:172-179).  Under
+torch.distributed every rank takes a share of the samples, sequences or pairs (rnc.dist).
 """
 import os
 from collections import deque, namedtuple
 from concurrent.futures import ThreadPoolExecutor
 
-import numpy as np
 import torch
 
 from utils import frame_utils
 from utils.utils import InputPadder, forward_interpolate
 
 
+def _shape_batches(samples, batch_size):
+    """Consecutive samples of one frame size, batch_size at a time; a new size (KITTI's vary) closes the batch."""
+    batch = []
+    for s in samples:
+        s = tuple(s) if len(s) == 4 else (s[0], s[1], s[2], None)
+        if batch and batch[0][0].shape != s[0].shape:
+            yield batch
+            batch = []
+        batch.append(s)
+        if len(batch) == batch_size:
+            yield batch
+            batch = []
+    if batch:
+        yield batch
+
+
+_Staged = namedtuple("_Staged", "im1 im2 gt valid sparse ready")
+
+
+def _stage(batch, dev, copy_stream):
+    """Enqueue the upload of a batch: each field stacked into a pinned host tensor and copied without blocking on copy_stream,
+    so that it overlaps the forward running on the compute stream.  valid is None when no sample has one; a sample without
+    one among samples with one counts every pixel valid."""
+    sparse = [s[3] is not None for s in batch]
+    H, W = batch[0][0].shape[-2:]
+    fields = [[s[0] for s in batch], [s[1] for s in batch], [s[2].float() for s in batch]]
+    if any(sparse):
+        fields.append([torch.ones(H, W) if s[3] is None else s[3].float() for s in batch])
+    if dev.type != "cuda":
+        host = [torch.stack(f).to(dev) for f in fields]
+        return _Staged(*host[:3], host[3] if len(host) == 4 else None, sparse, None)
+    out = []
+    for f in fields:
+        pinned = torch.empty((len(f),) + tuple(f[0].shape), dtype=f[0].dtype, pin_memory=True)
+        torch.stack(f, out=pinned)
+        with torch.cuda.stream(copy_stream):          # allocated on copy_stream: its memory is never in use by older work
+            out.append(pinned.to(dev, non_blocking=True))
+    ready = torch.cuda.Event()
+    ready.record(copy_stream)
+    return _Staged(*out[:3], out[3] if len(out) == 4 else None, sparse, ready)
+
+
 @torch.no_grad()
 def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda"):
     """samples: iterable of (image1 [3,H,W], image2 [3,H,W], flow_gt [2,H,W], valid [H,W] or None).
-    Returns the metrics validate_sintel / validate_kitti print: EPE, 1px/3px/5px, and KITTI F1 when `valid` is given."""
+    Returns the metrics validate_sintel / validate_kitti print: EPE, 1px/3px/5px, and KITTI F1 when `valid` is given
+    (rnc.metrics.summarize: Sintel-style pools every pixel, KITTI-style averages the per-image mean EPE).
+
+    On a CUDA device each batch is uploaded through pinned buffers on a side stream while the previous batch computes, its
+    metrics are taken on the device (rnc_flow_metrics) and stay there as per-image partials; the host reads them once, at the
+    end.  Under torch.distributed with more than one rank, rank r evaluates the samples of index = r (mod world) (a sequence,
+    such as the reference's FlowDataset, is indexed, so each rank loads only its own samples), the per-image partials are
+    all-gathered, and every rank returns the same dict, bit for bit the single-process one."""
+    from .dist import gather_strided, strided_items, world_rank
+    from .metrics import Partials, cat, flow_metrics, summarize
     model.eval()
-    epe_all, f1_all, batch = [], [], []
-    epe_img = []                                            # KITTI: per-image mean EPE (evaluate.py:172)
+    world, rank = world_rank()
+    dev = torch.device(device)
+    if dev.type == "cuda" and dev.index is None:
+        dev = torch.device("cuda", torch.cuda.current_device())
+    copy_stream = torch.cuda.Stream(dev) if dev.type == "cuda" else None
+    parts, sparse = [], []
+    batches = _shape_batches(strided_items(samples, world, rank), batch_size)
 
-    def flush():
-        if not batch:
-            return
-        im1 = torch.stack([b[0] for b in batch]).to(device).float()
-        im2 = torch.stack([b[1] for b in batch]).to(device).float()
-        padder = InputPadder(im1.shape, mode=mode)
-        p1, p2 = padder.pad(im1, im2)
+    def stage_next():
+        b = next(batches, None)
+        return None if b is None else _stage(b, dev, copy_stream)
+    nxt = stage_next()
+    while nxt is not None:
+        cur = nxt
+        if cur.ready is not None:
+            compute = torch.cuda.current_stream(dev)
+            compute.wait_event(cur.ready)
+            for t in cur[:4]:
+                if t is not None:
+                    t.record_stream(compute)
+        padder = InputPadder(cur.im1.shape, mode=mode)
+        p1, p2 = padder.pad(cur.im1.float(), cur.im2.float())
         _, flow_pr = model(p1, p2, iters=iters, test_mode=True)
-        flow = padder.unpad(flow_pr).cpu()
-        for k, (_, _, gt, valid) in enumerate(batch):
-            epe = torch.sum((flow[k] - gt) ** 2, dim=0).sqrt()
-            if valid is None:
-                epe_all.append(epe.view(-1).numpy())
-            else:                                           # evaluate.py:163-171
-                mag = torch.sum(gt ** 2, dim=0).sqrt().view(-1)
-                val = valid.view(-1) >= 0.5
-                e = epe.view(-1)
-                out = ((e > 3.0) & ((e / mag) > 0.05)).float()
-                epe_img.append(e[val].mean().item())
-                epe_all.append(e[val].numpy())
-                f1_all.append(out[val].numpy())
-        batch.clear()
-
-    for s in samples:
-        s = s if len(s) == 4 else (s[0], s[1], s[2], None)
-        if batch and batch[0][0].shape != s[0].shape:       # frame sizes differ (KITTI): close the batch
-            flush()
-        batch.append(s)
-        if len(batch) == batch_size:
-            flush()
-    flush()
-    e = np.concatenate(epe_all)
-    res = {"epe": float(np.mean(e)), "1px": float(np.mean(e < 1)), "3px": float(np.mean(e < 3)), "5px": float(np.mean(e < 5))}
-    if f1_all:
-        res["epe"] = float(np.mean(epe_img))                # evaluate.py:178: mean of the per-image means
-        res["f1"] = float(100 * np.mean(np.concatenate(f1_all)))   # evaluate.py:175,179: pooled over all valid pixels
-    return res
+        parts.append(flow_metrics(padder.unpad(flow_pr), cur.gt, cur.valid))
+        sparse += cur.sparse
+        del cur, p1, p2, flow_pr
+        nxt = stage_next()                          # staged while this batch computes
+    local = cat(parts)
+    rows = list(zip(local.counts.cpu().tolist(), local.epe_sum.cpu().tolist(), sparse))
+    rows = gather_strided(rows, world)
+    every = Partials(torch.tensor([r[0] for r in rows], dtype=torch.int64).view(-1, 5),
+                     torch.tensor([r[1] for r in rows], dtype=torch.float64))
+    return summarize(every, "kitti" if any(r[2] for r in rows) else "sintel")
 
 
 @torch.no_grad()
@@ -274,22 +318,31 @@ def create_sintel_submission(model, sequences, iters=32, warm_start=False, outpu
     a list of [3,H,W] images of one size for all sequences.  Writes output_path/dstype/scene/frame%04d.flo for pair k (frames
     k, k + 1) with k + 1 in the name, and with write_png its colour coding (rnc.viz, as utils.flow_viz) to
     output_path + "_png"/dstype/scene/frame%04d.png.  Files are written on a thread pool while the next step computes;
-    returns when all are written."""
+    returns when all are written.  Under torch.distributed each rank runs whole sequences, assigned longest-first by pair count
+    (rnc.dist.greedy_assignment), and no rank returns before every rank's files are written."""
+    from .dist import barrier, greedy_assignment, world_rank
     seqs = list(sequences)
-    frames = [f for _, _, f in seqs]
-    steps = sequence_schedule([len(f) for f in frames], batch_size)
-    flows = run_sequences(model, frames, iters=iters, warm_start=warm_start, batch_size=batch_size,
-                          device=_model_device(model))
-    with _SubmissionWriter() as w:
-        for step in steps:
-            got = [next(flows) for c in step if not c.idle]
-            files = []
-            for s, k, _ in got:
-                dstype, scene, _ = seqs[s]
-                name = "frame%04d" % (k + 1)
-                files.append((os.path.join(output_path, dstype, scene, name + ".flo"),
-                              os.path.join(output_path + "_png", dstype, scene, name + ".png") if write_png else None))
-            w.step(torch.stack([f for _, _, f in got]), files, frame_utils.writeFlow)
+    world, rank = world_rank()
+    if world > 1:
+        owner = greedy_assignment([max(len(f) - 1, 0) for _, _, f in seqs], world)
+        seqs = [s for s, r in zip(seqs, owner) if r == rank]
+    try:
+        frames = [f for _, _, f in seqs]
+        steps = sequence_schedule([len(f) for f in frames], batch_size)
+        flows = run_sequences(model, frames, iters=iters, warm_start=warm_start, batch_size=batch_size,
+                              device=_model_device(model))
+        with _SubmissionWriter() as w:
+            for step in steps:
+                got = [next(flows) for c in step if not c.idle]
+                files = []
+                for s, k, _ in got:
+                    dstype, scene, _ = seqs[s]
+                    name = "frame%04d" % (k + 1)
+                    files.append((os.path.join(output_path, dstype, scene, name + ".flo"),
+                                  os.path.join(output_path + "_png", dstype, scene, name + ".png") if write_png else None))
+                w.step(torch.stack([f for _, _, f in got]), files, frame_utils.writeFlow)
+    finally:
+        barrier()
 
 
 @torch.no_grad()
@@ -297,18 +350,24 @@ def create_kitti_submission(model, pairs, iters=24, output_path="kitti_submissio
     """create_kitti_submission (evaluate.py:58-87) in batches.  pairs: iterable of (frame_id, image1 [3,H,W], image2), of any
     mix of sizes; pairs of one size run together, batch_size at a time (size_batches), padded as InputPadder(mode="kitti").
     Writes output_path/frame_id (frame_utils.writeFlowKITTI) and with write_png output_path + "_png"/(frame_id + ".png").
-    Files are written on a thread pool while the next batch computes; returns when all are written."""
+    Files are written on a thread pool while the next batch computes; returns when all are written.  Under torch.distributed
+    rank r runs the pairs of index = r (mod world), and no rank returns before every rank's files are written."""
+    from .dist import barrier, strided_items, world_rank
     model.eval()
     device = _model_device(model)
-    with _SubmissionWriter() as w:
-        for batch in size_batches(pairs, batch_size, key=lambda p: tuple(p[1].shape)):
-            padder = InputPadder(batch[0][1].shape, mode="kitti")
-            im1 = _stack([p[1] for p in batch], device, padder)
-            im2 = _stack([p[2] for p in batch], device, padder)
-            _, flow_pr = model(im1, im2, iters=iters, test_mode=True)
-            files = [(os.path.join(output_path, fid), os.path.join(output_path + "_png", fid + ".png") if write_png else None)
-                     for fid, _, _ in batch]
-            w.step(padder.unpad(flow_pr), files, frame_utils.writeFlowKITTI)
+    world, rank = world_rank()
+    try:
+        with _SubmissionWriter() as w:
+            for batch in size_batches(strided_items(pairs, world, rank), batch_size, key=lambda p: tuple(p[1].shape)):
+                padder = InputPadder(batch[0][1].shape, mode="kitti")
+                im1 = _stack([p[1] for p in batch], device, padder)
+                im2 = _stack([p[2] for p in batch], device, padder)
+                _, flow_pr = model(im1, im2, iters=iters, test_mode=True)
+                files = [(os.path.join(output_path, fid), os.path.join(output_path + "_png", fid + ".png") if write_png else None)
+                         for fid, _, _ in batch]
+                w.step(padder.unpad(flow_pr), files, frame_utils.writeFlowKITTI)
+    finally:
+        barrier()
 
 
 def load_checkpoint(model, state):

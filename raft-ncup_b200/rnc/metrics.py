@@ -1,0 +1,113 @@
+"""Validation metrics (evaluate.py:88-182) as per-image partials that any number of batches, or of GPUs, combine exactly.
+
+`flow_metrics(flow, gt, valid)` gives per image the int64 counts of valid pixels, of EPE < 1, < 3 and < 5 and of KITTI
+outliers, and the fp64 sum of the valid pixels' EPE.  CUDA tensors go through rnc_flow_metrics (csrc/flow_metrics.cu), CPU
+tensors through `host_partials`, the same float32 formulas in torch; the kernel's counts equal the host's and its sums agree
+to the last few bits.  `summarize(partials, mode)` turns the partials of a whole split, in image order, into the numbers the
+reference prints.  Both paths give an image's partials independently of the batch it came in, so a split's result does not
+depend on the batch size or on how the images were spread over ranks.
+"""
+from collections import namedtuple
+
+import torch
+
+from . import native
+
+# counts: int64 [N, 5] (valid, epe < 1, < 3, < 5, outliers); epe_sum: float64 [N]
+Partials = namedtuple("Partials", "counts epe_sum")
+
+
+def _check(flow, gt, valid):
+    if flow.dim() != 4 or flow.shape[1] != 2 or gt.shape != flow.shape:
+        raise ValueError(f"flow_metrics: expected flow and gt of one [B,2,H,W] shape, got {tuple(flow.shape)} and "
+                         f"{tuple(gt.shape)}")
+    if valid is not None and tuple(valid.shape) != (flow.shape[0],) + tuple(flow.shape[2:]):
+        raise ValueError(f"flow_metrics: expected valid [B,H,W] = {(flow.shape[0],) + tuple(flow.shape[2:])}, got "
+                         f"{tuple(valid.shape)}")
+    if len({t.device for t in (flow, gt, valid) if t is not None}) != 1:
+        raise ValueError("flow_metrics: flow, gt and valid must be on one device")
+
+
+def flow_metrics(flow, gt, valid=None):
+    """flow, gt: [B,2,H,W] (any strides; float32, or converted to it); valid: [B,H,W] or None (every pixel valid).
+    Returns Partials of B images on the tensors' device; on CUDA it is enqueued on the current stream."""
+    _check(flow, gt, valid)
+    if not flow.is_cuda:
+        return host_partials(flow, gt, valid)
+    flow, gt = flow.float(), gt.float()
+    valid = None if valid is None else valid.float()
+    B, _, H, W = flow.shape
+    dev = flow.device
+    counts = torch.empty(B, 5, dtype=torch.int64, device=dev)
+    epe_sum = torch.empty(B, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        ws = torch.empty(native.rnc.flow_metrics_workspace_bytes(B, H, W), dtype=torch.uint8, device=dev)
+        vs = (0, 0, 0) if valid is None else valid.stride()
+        native.rnc.flow_metrics(flow, *flow.stride(), gt, *gt.stride(), valid, *vs, B, H, W, counts, epe_sum, ws, ws.numel())
+    return Partials(counts, epe_sum)
+
+
+def _f32(x):
+    """x (fp64) rounded to float32, kept in fp64.  Each of + - * / sqrt evaluated in fp64 on float32 operands and rounded once
+    to float32 is the IEEE float32 result (53 >= 2 * 24 + 2 bits), whatever the CPU's vector library rounds."""
+    return x.float().double()
+
+
+def _norm(v):
+    return _f32(_f32(_f32(v[0] * v[0]) + _f32(v[1] * v[1])).sqrt())
+
+
+def host_partials(flow, gt, valid=None):
+    """The partials of the reference's float32 formulas (evaluate.py:163-171), one image at a time, summed in fp64.  Every
+    operation is rounded as IEEE float32 rounds it, as numpy, CUDA and torch on the GPU do; torch's CPU float32 sqrt is not
+    correctly rounded on every CPU (AVX-512: one ulp off for a fraction of a percent of inputs)."""
+    _check(flow, gt, valid)
+    counts, sums = [], []
+    for b in range(flow.shape[0]):
+        f, g = flow[b].float().double(), gt[b].float().double()
+        epe = _norm(_f32(f - g))
+        mag = _norm(g)
+        val = torch.ones_like(epe, dtype=torch.bool) if valid is None else valid[b] >= 0.5
+        out = (epe > 3.0) & (_f32(epe / mag).float() > 0.05)     # compared in float32: 0.05 is rounded to 0.05f
+        counts.append(torch.stack([val.sum(), (val & (epe < 1)).sum(), (val & (epe < 3)).sum(), (val & (epe < 5)).sum(),
+                                   (val & out).sum()]))
+        sums.append(torch.where(val, epe, 0.0).double().sum())
+    if not counts:
+        return Partials(torch.zeros(0, 5, dtype=torch.int64), torch.zeros(0, dtype=torch.float64))
+    return Partials(torch.stack(counts).to(torch.int64), torch.stack(sums))
+
+
+def cat(parts):
+    """One Partials of a list of them, in order."""
+    if not parts:
+        return Partials(torch.zeros(0, 5, dtype=torch.int64), torch.zeros(0, dtype=torch.float64))
+    return Partials(torch.cat([p.counts for p in parts]), torch.cat([p.epe_sum for p in parts]))
+
+
+def _ratio(a, b):
+    return a / b if b else float("nan")
+
+
+def summarize(partials, mode):
+    """The metrics of a split from its per-image partials, combined in image order in fp64.
+    mode "sintel" or "chairs" (evaluate.py:95-137): EPE, 1px, 3px, 5px pooled over every pixel.
+    mode "kitti" (evaluate.py:163-179): EPE is the mean over images of each image's mean EPE over its valid pixels (NaN for an
+    image without one, as in the reference); 1px/3px/5px and F1 (in percent) are pooled over all valid pixels."""
+    if mode not in ("sintel", "chairs", "kitti"):
+        raise ValueError(f"summarize: mode must be 'sintel', 'chairs' or 'kitti', got {mode!r}")
+    counts = partials.counts.cpu().tolist()
+    sums = partials.epe_sum.cpu().tolist()
+    tot = [sum(c[k] for c in counts) for k in range(5)]
+    res = {"1px": _ratio(tot[1], tot[0]), "3px": _ratio(tot[2], tot[0]), "5px": _ratio(tot[3], tot[0])}
+    if mode == "kitti":
+        epe = 0.0
+        for s, c in zip(sums, counts):
+            epe += s / c[0] if c[0] else float("nan")
+        res["epe"] = _ratio(epe, len(counts))
+        res["f1"] = 100 * _ratio(tot[4], tot[0])
+    else:
+        epe = 0.0
+        for s in sums:
+            epe += s
+        res["epe"] = _ratio(epe, tot[0])
+    return {k: res[k] for k in ("epe", "1px", "3px", "5px", "f1") if k in res}
