@@ -536,6 +536,25 @@ int rnc_flow_metrics(const float* flow, long long fb, long long fc, long long fy
                      int B, int H, int W, long long* counts, double* epe_sum, void* workspace, size_t workspace_bytes,
                      void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V3  sparsification curves of a confidence score (AUSE) for a batch of float32 flows, over the fractions f_k = k/100, k < 100.
+ *   flow, gt, valid : as rnc_flow_metrics (epe rounded as it rounds it; valid where >= 0.5, NULL: every pixel is valid)
+ *   score           : fp32, pixel (b, y, x) at score[b*sb + y*sy + x*sx], higher is more confident; 4-byte aligned
+ *   count           : int64 [B][100], N - m_k, with N the image's valid pixels and m_k = floor(k*N/100); 8-byte aligned
+ *   kept_epe        : fp64 [B][100], the sum of the epe of the valid pixels left once the m_k of lowest score are removed
+ *                     (ties: lower row-major index first; a NaN score ranks below -inf); 8-byte aligned
+ *   ideal_epe       : fp64 [B][100], the same once the m_k of largest epe are removed (a NaN epe ranks largest); 8-byte aligned
+ *   workspace       : rnc_sparsification_workspace_bytes(B, H, W) bytes, 16-byte aligned, no zeroing needed (sort buffers)
+ * One device-wide radix sort per order with the image index in the key's high bits, then fixed-order fp64 range sums and
+ * suffix sums: no atomics and no host synchronisation, so an image's results are bit for bit the same whatever B, its position
+ * in the batch or the GPU.  An image without a valid pixel gives zeros.  RNC_ERR_BAD_SHAPE when B*H*W >= 2^31 (the sort's
+ * index range) or B > 65535.  Bad arguments return before any launch. */
+size_t rnc_sparsification_workspace_bytes(int B, int H, int W);   /* 0 for a bad shape */
+int rnc_sparsification(const float* flow, long long fb, long long fc, long long fy, long long fx, const float* gt, long long gb,
+                       long long gc, long long gy, long long gx, const float* valid, long long vb, long long vy, long long vx,
+                       const float* score, long long sb, long long sy, long long sx, int B, int H, int W, long long* count,
+                       double* kept_epe, double* ideal_epe, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -61,7 +61,7 @@ def _stage(batch, dev, copy_stream):
 
 
 @torch.no_grad()
-def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda"):
+def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda", confidence=False):
     """samples: iterable of (image1 [3,H,W], image2 [3,H,W], flow_gt [2,H,W], valid [H,W] or None).
     Returns the metrics validate_sintel / validate_kitti print: EPE, 1px/3px/5px, and KITTI F1 when `valid` is given
     (rnc.metrics.summarize: Sintel-style pools every pixel, KITTI-style averages the per-image mean EPE).
@@ -70,16 +70,22 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
     metrics are taken on the device (rnc_flow_metrics) and stay there as per-image partials; the host reads them once, at the
     end.  Under torch.distributed with more than one rank, rank r evaluates the samples of index = r (mod world) (a sequence,
     such as the reference's FlowDataset, is indexed, so each rank loads only its own samples), the per-image partials are
-    all-gathered, and every rank returns the same dict, bit for bit the single-process one."""
+    all-gathered, and every rank returns the same dict, bit for bit the single-process one.
+
+    confidence=True (NCUP model) also evaluates the upsampler's output confidence: the forward returns it, unpadded like the
+    flow, each pixel is scored by rnc.metrics.confidence_score, and rnc.metrics.sparsification's per-image partials travel
+    with the flow metrics'.  The dict gains "sparsification" and "ideal" (100 mean EPEs each, at the removed fractions k/100)
+    and "ause" (rnc.metrics.summarize_sparsification); its other keys are those of confidence=False, bit for bit."""
     from .dist import gather_strided, strided_items, world_rank
-    from .metrics import Partials, cat, flow_metrics, summarize
+    from .metrics import (FRACTIONS, Partials, SparsPartials, cat, confidence_score, flow_metrics, sparsification, summarize,
+                          summarize_sparsification)
     model.eval()
     world, rank = world_rank()
     dev = torch.device(device)
     if dev.type == "cuda" and dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     copy_stream = torch.cuda.Stream(dev) if dev.type == "cuda" else None
-    parts, sparse = [], []
+    parts, sparse, sparts = [], [], []
     batches = _shape_batches(strided_items(samples, world, rank), batch_size)
 
     def stage_next():
@@ -96,17 +102,33 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
                     t.record_stream(compute)
         padder = InputPadder(cur.im1.shape, mode=mode)
         p1, p2 = padder.pad(cur.im1.float(), cur.im2.float())
-        _, flow_pr = model(p1, p2, iters=iters, test_mode=True)
-        parts.append(flow_metrics(padder.unpad(flow_pr), cur.gt, cur.valid))
+        if confidence:
+            _, flow_pr, conf = model(p1, p2, iters=iters, test_mode=True, return_confidence=True)
+        else:
+            _, flow_pr = model(p1, p2, iters=iters, test_mode=True)
+        flow = padder.unpad(flow_pr)
+        parts.append(flow_metrics(flow, cur.gt, cur.valid))
+        if confidence:
+            sparts.append(sparsification(flow, cur.gt, cur.valid, confidence_score(padder.unpad(conf))))
+            del conf
         sparse += cur.sparse
-        del cur, p1, p2, flow_pr
+        del cur, p1, p2, flow_pr, flow
         nxt = stage_next()                          # staged while this batch computes
     local = cat(parts)
     rows = list(zip(local.counts.cpu().tolist(), local.epe_sum.cpu().tolist(), sparse))
+    if confidence:
+        cols = [torch.cat(c).cpu().tolist() for c in zip(*sparts)] if sparts else [[], [], []]
+        rows = [r + s for r, s in zip(rows, zip(*cols))]
     rows = gather_strided(rows, world)
     every = Partials(torch.tensor([r[0] for r in rows], dtype=torch.int64).view(-1, 5),
                      torch.tensor([r[1] for r in rows], dtype=torch.float64))
-    return summarize(every, "kitti" if any(r[2] for r in rows) else "sintel")
+    res = summarize(every, "kitti" if any(r[2] for r in rows) else "sintel")
+    if confidence:
+        res.update(summarize_sparsification(SparsPartials(
+            torch.tensor([r[3] for r in rows], dtype=torch.int64).view(-1, FRACTIONS),
+            torch.tensor([r[4] for r in rows], dtype=torch.float64).view(-1, FRACTIONS),
+            torch.tensor([r[5] for r in rows], dtype=torch.float64).view(-1, FRACTIONS))))
+    return res
 
 
 @torch.no_grad()

@@ -6,15 +6,24 @@ tensors through `host_partials`, the same float32 formulas in torch; the kernel'
 to the last few bits.  `summarize(partials, mode)` turns the partials of a whole split, in image order, into the numbers the
 reference prints.  Both paths give an image's partials independently of the batch it came in, so a split's result does not
 depend on the batch size or on how the images were spread over ranks.
+
+`sparsification(flow, gt, valid, score)` evaluates a per-pixel confidence score the same way: per image, the sparsification
+curve (the mean EPE of the valid pixels left once the lowest-scored fraction f_k = k/100 is removed) and its ideal (the
+largest errors removed instead) as partial sums; `summarize_sparsification` gives the split's curves and their AUSE.  CUDA
+tensors go through rnc_sparsification (csrc/sparsification.cu), CPU tensors through `host_sparsification`.
 """
 from collections import namedtuple
 
+import numpy as np
 import torch
 
 from . import native
 
 # counts: int64 [N, 5] (valid, epe < 1, < 3, < 5, outliers); epe_sum: float64 [N]
 Partials = namedtuple("Partials", "counts epe_sum")
+# count: int64 [N, 100] (valid pixels kept at f_k); kept_epe, ideal_epe: float64 [N, 100] (their EPE sum, score / ideal order)
+SparsPartials = namedtuple("SparsPartials", "count kept_epe ideal_epe")
+FRACTIONS = 100
 
 
 def _check(flow, gt, valid):
@@ -111,3 +120,110 @@ def summarize(partials, mode):
             epe += s
         res["epe"] = _ratio(epe, tot[0])
     return {k: res[k] for k in ("epe", "1px", "3px", "5px", "f1") if k in res}
+
+
+def _check_score(flow, score):
+    want = (flow.shape[0],) + tuple(flow.shape[2:])
+    if score is None or tuple(score.shape) != want:
+        raise ValueError(f"sparsification: expected score [B,H,W] = {want}, got "
+                         f"{None if score is None else tuple(score.shape)}")
+    if score.device != flow.device:
+        raise ValueError("sparsification: flow, gt, valid and score must be on one device")
+
+
+def sparsification(flow, gt, valid, score):
+    """flow, gt: [B,2,H,W]; valid: [B,H,W] or None (every pixel valid); score: [B,H,W], higher is more confident (any
+    strides; float32, or converted to it).  Returns SparsPartials of B images on the tensors' device: for k = 0..99, with N
+    valid pixels and m_k = floor(k*N/100) of them removed, count[:, k] = N - m_k and the fp64 EPE sums of the pixels kept in
+    score order (kept_epe) and in ideal order (ideal_epe); see host_sparsification.  On CUDA it is enqueued on the current
+    stream."""
+    _check(flow, gt, valid)
+    _check_score(flow, score)
+    if not flow.is_cuda:
+        return host_sparsification(flow, gt, valid, score)
+    flow, gt, score = flow.float(), gt.float(), score.float()
+    valid = None if valid is None else valid.float()
+    B, _, H, W = flow.shape
+    dev = flow.device
+    count = torch.empty(B, FRACTIONS, dtype=torch.int64, device=dev)
+    kept = torch.empty(B, FRACTIONS, dtype=torch.float64, device=dev)
+    ideal = torch.empty(B, FRACTIONS, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        nbytes = native.rnc.sparsification_workspace_bytes(B, H, W)
+        if nbytes == 0:
+            raise ValueError(f"sparsification: {B} images of {H}x{W} exceed the sort's 2^31 pixels")
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+        vs = (0, 0, 0) if valid is None else valid.stride()
+        native.rnc.sparsification(flow, *flow.stride(), gt, *gt.stride(), valid, *vs, score, *score.stride(), B, H, W, count,
+                                  kept, ideal, ws, ws.numel())
+    return SparsPartials(count, kept, ideal)
+
+
+def _nan_first_order(v):
+    """Stable ascending order of v with every NaN first (ties keep their index order)."""
+    nan = torch.isnan(v)
+    o = torch.argsort(torch.where(nan, float("-inf"), v), stable=True)
+    return o[torch.argsort((~nan[o]).to(torch.int8), stable=True)]
+
+
+def host_sparsification(flow, gt, valid, score):
+    """sparsification's definition, one image at a time in fp64 on float32 values.  EPE as host_partials rounds it; valid
+    where valid >= 0.5.  Score order: the valid pixels by score ascending, a NaN score below -inf, ties by row-major index.
+    Ideal order: by EPE descending, a NaN EPE largest.  Removing the first m_k = floor(k*N/100) (k = 0..99) of each order
+    leaves count = N - m_k pixels; kept_epe / ideal_epe are the fp64 sums of their EPE.  An image with N = 0 gives zeros."""
+    _check(flow, gt, valid)
+    _check_score(flow, score)
+    B = flow.shape[0]
+    count = torch.zeros(B, FRACTIONS, dtype=torch.int64)
+    kept = torch.zeros(B, FRACTIONS, dtype=torch.float64)
+    ideal = torch.zeros(B, FRACTIONS, dtype=torch.float64)
+    for b in range(B):
+        f, g = flow[b].float().double(), gt[b].float().double()
+        epe = _norm(_f32(f - g)).reshape(-1)
+        val = torch.ones_like(epe, dtype=torch.bool) if valid is None else (valid[b] >= 0.5).reshape(-1)
+        e, s = epe[val], score[b].float().reshape(-1)[val]
+        n = e.numel()
+        if n == 0:
+            continue
+        m = torch.tensor([k * n // FRACTIONS for k in range(FRACTIONS)])
+        count[b] = n - m
+        for out, order in ((kept, _nan_first_order(s)), (ideal, _nan_first_order(-e))):
+            tail = e[order].flip(0).cumsum(0).flip(0)            # tail[j]: the sum of the pixels from j on
+            out[b] = tail[m]
+    return SparsPartials(count, kept, ideal)
+
+
+def summarize_sparsification(partials):
+    """The split's curves from per-image SparsPartials, in image order in fp64 over the images with a valid pixel:
+    sparsification[k] (and ideal[k]) is the mean over those images of kept_epe[k] / count[k] (ideal_epe[k] / count[k]), and
+    ause = numpy.trapezoid(sparsification - ideal, x=f_k) over f_k = k/100.  NaN everywhere when no image has a valid pixel."""
+    count = partials.count.cpu().tolist()
+    kept = partials.kept_epe.cpu().tolist()
+    orc = partials.ideal_epe.cpu().tolist()
+    sp, orr, n = [0.0] * FRACTIONS, [0.0] * FRACTIONS, 0
+    for c, ke, oe in zip(count, kept, orc):
+        if c[0] == 0:
+            continue
+        n += 1
+        for k in range(FRACTIONS):
+            sp[k] += ke[k] / c[k]
+            orr[k] += oe[k] / c[k]
+    if n == 0:
+        nan = float("nan")
+        return {"sparsification": [nan] * FRACTIONS, "ideal": [nan] * FRACTIONS, "ause": nan}
+    sp = [v / n for v in sp]
+    orr = [v / n for v in orr]
+    x = np.arange(FRACTIONS) / FRACTIONS
+    ause = float(np.trapezoid(np.array(sp) - np.array(orr), x=x))
+    return {"sparsification": sp, "ideal": orr, "ause": ause}
+
+
+def confidence_score(conf):
+    """The score validate ranks pixels by: the harmonic mean of the NCUP output confidence's two planes, [B,2,H,W] ->
+    [B,H,W] float32, 2*c_u*c_v / (c_u + c_v) and 0 where c_u + c_v == 0, each operation rounded once.  With a per-component
+    variance proportional to 1/c, the EPE's variance goes as 1/c_u + 1/c_v, whose order is the harmonic mean's reversed."""
+    if conf.dim() != 4 or conf.shape[1] != 2:
+        raise ValueError(f"confidence_score: expected a [B,2,H,W] confidence, got {tuple(conf.shape)}")
+    cu, cv = conf[:, 0].float(), conf[:, 1].float()
+    den = cu + cv
+    return torch.where(den == 0, torch.zeros_like(den), (2 * cu * cv) / den)

@@ -146,6 +146,9 @@ SIGNATURES = {
     "rnc_flow_metrics_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
     "rnc_flow_metrics": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp,
                               _vp, C.c_size_t, _vp]),
+    "rnc_sparsification_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "rnc_sparsification": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 3,
+                                _vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
 }
 
 _lib = None
