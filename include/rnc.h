@@ -555,6 +555,22 @@ int rnc_sparsification(const float* flow, long long fb, long long fc, long long 
                        const float* score, long long sb, long long sy, long long sx, int B, int H, int W, long long* count,
                        double* kept_epe, double* ideal_epe, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V4  forward-backward consistency of B flow pairs, both directions in one launch.
+ *   flow_fw, flow_bw : fp32 [B,2,H,W] through element strides (fb..fx, gb..gx), component c of pixel (b, y, x) at
+ *                      flow[b*fb + c*fc + y*fy + x*fx]; 4-byte aligned
+ *   occ_fw, occ_bw   : uint8 [B][H][W] contiguous.  For pixel x of direction F -> G (G -> F for the _bw outputs), p = x + F(x)
+ *                      and G^(p) bilinear with zero padding on align_corners=True pixel coordinates: bit 0 when
+ *                      |F + G^|^2 > alpha1 (|F|^2 + |G^|^2) + alpha2 or that sum is not finite; bit 1 when p lies outside
+ *                      [0, W-1] x [0, H-1] (a NaN target is outside, and gets bit 0 too)
+ *   err_fw, err_bw   : fp32 [B][H][W] contiguous, |F(x) + G^(p)|; +inf where p is outside or the sum is not finite
+ * Every operation rounded once in float32 (no FMA).  No atomics, no host synchronisation: a pixel's outputs depend only on its
+ * own image.  RNC_ERR_BAD_SHAPE for B > 65535 or H*W >= 2^31. */
+int rnc_fb_consistency(const float* flow_fw, long long fb, long long fc, long long fy, long long fx, const float* flow_bw,
+                       long long gb, long long gc, long long gy, long long gx, int B, int H, int W, float alpha1,
+                       float alpha2, unsigned char* occ_fw, unsigned char* occ_bw, float* err_fw, float* err_bw,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

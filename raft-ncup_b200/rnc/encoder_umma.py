@@ -196,6 +196,27 @@ class EncoderRunner:
         self.eng.uconv(B, h8, w8, bufs.XS[2].ptrs(), 128, 128, pc.head, native.EPI_TANH_RELU, out_f32=ws.h.data_ptr(),
                        ldo_f32=128, out_split=ws.hx.ptrs(), ldo_split=HX_LD)
 
+    def run_bidirectional(self, model, ws, image1, image2):
+        """The encoders of the bidirectional pass (rnc.model.BidirectionalStage) on a workspace of 2B slots: fnet on the 2B
+        frames cat(image1, image2), in the encoder buffers of an ordinary B-pair forward; its head writes ws.f1_cl for all 2B
+        slots in frame order, and two device-to-device copies of the halves give level 0 of ws.f2_pyr (slot j: image2[j],
+        slot B + j: image1[j]).  cnet on the same 2B frames -> ws.h, ws.hx[:, :256].  The caller finishes the pyramid."""
+        eng, E = self.eng, native
+        B, _, Hin, Win = image1.shape
+        dev = image1.device
+        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
+        bufs = self.buffers(dev, 2 * B, Hin, Win)
+        both = torch.cat([image1, image2], 0).contiguous()
+        h8, w8, _ = self._trunk(pf, bufs, both, 2 * B, Hin, Win)
+        eng.alloc_fmaps(ws, 2 * B, 256, h8, w8, 4, dev)
+        eng.uconv(2 * B, h8, w8, bufs.XS[2].ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f1_cl.data_ptr(), ldo_f32=256)
+        n = B * h8 * w8 * 256                               # elements of one half's feature maps
+        f1 = ws.f1_cl.view(-1)
+        ws.f2_pyr[:n].copy_(f1[n:])
+        ws.f2_pyr[n:2 * n].copy_(f1[:n])
+        self._context(pc, bufs, ws, both, h8, w8)
+        return h8, w8
+
     def run_step(self, model, ws, image1, image2, carry, restart):
         """One step of sequence inference (rnc.model.SequenceStage): like run, but frame 1 of the `carry` slots is the last
         step's frame 2, whose features are still level 0 of ws.f2_pyr (and of ws.f2h, the tensor-core lookup's halves): they

@@ -399,21 +399,26 @@ class Engine:
         return not getattr(model.args, "mixed_precision", False) and os.environ.get("RNC_ENCODER", "umma").lower() == "umma" \
             and self.mode == "umma" and not self.fork_convf1
 
-    def graph_forward(self, model, image1, image2, iters, flow_init, return_confidence=False):
+    def graph_forward(self, model, image1, image2, iters, flow_init, return_confidence=False, bidirectional=False):
         """Second and later forwards with the same signature (shape, iterations, warm start or not, weights, confidence or
-        not) replay a captured graph: inputs are copied into the graph's static buffers, results are returned as fresh
-        copies."""
+        not, bidirectional or not) replay a captured graph: inputs are copied into the graph's static buffers, results are
+        returned as fresh copies.  bidirectional: the pass of model.forward_bidirectional, flow_init [2B,2,H/8,W/8]."""
         B, _, Him, Wim = image1.shape
-        if flow_init is not None and tuple(flow_init.shape) != (B, 2, Him // 8, Wim // 8):
+        if flow_init is not None and tuple(flow_init.shape) != ((2 if bidirectional else 1) * B, 2, Him // 8, Wim // 8):
             raise ValueError("flow_init must be [N,2,H/8,W/8]")
         # a graph records one mode's kernels: the deterministic mode gets its own (torch.use_deterministic_algorithms)
         key = (type(model).__name__, tuple(image1.shape), iters, flow_init is not None, _param_key(model),
-               torch.are_deterministic_algorithms_enabled(), return_confidence)
+               torch.are_deterministic_algorithms_enabled(), return_confidence) + (("bidirectional",) if bidirectional else ())
         first = key not in self._graphs
         ent = _lru_get(self._graphs, key, self.MAX_GRAPHS, dict)
         conf = dict(return_confidence=True) if return_confidence else {}
+
+        def eager(im1, im2, fi):
+            if bidirectional:
+                return model._forward_bidirectional(self, im1, im2, iters, fi, return_confidence)
+            return model._forward_eager(self, im1, im2, iters, fi, True, **conf)
         if first:       # first sight: eager (also warms caches)
-            return model._forward_eager(self, image1, image2, iters, flow_init, True, **conf)
+            return eager(image1, image2, flow_init)
         if "graph" not in ent:
             ent["im1"], ent["im2"] = image1.detach().float().clone(), image2.detach().float().clone()
             ent["fi"] = flow_init.detach().float().clone() if flow_init is not None else None
@@ -421,11 +426,11 @@ class Engine:
             side = torch.cuda.Stream(device=image1.device)
             side.wait_stream(cur)
             with torch.cuda.stream(side):                                                  # warm-up on a side stream
-                model._forward_eager(self, ent["im1"], ent["im2"], iters, ent["fi"], True, **conf)
+                eager(ent["im1"], ent["im2"], ent["fi"])
             cur.wait_stream(side)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                ent["out"] = model._forward_eager(self, ent["im1"], ent["im2"], iters, ent["fi"], True, **conf)
+                ent["out"] = eager(ent["im1"], ent["im2"], ent["fi"])
                 ent["net"] = model.update_block.net
             ent["graph"] = g
             # the graph addresses these buffers by pointer: keep them alive even if the LRU caches let go of them

@@ -60,8 +60,36 @@ def _stage(batch, dev, copy_stream):
     return _Staged(*out[:3], out[3] if len(out) == 4 else None, sparse, ready)
 
 
+def bidirectional_flow(model, image1, image2, iters=32, flow_init=None, mode="sintel", return_confidence=False, alpha1=0.01,
+                       alpha2=0.5):
+    """Flow in both directions of B pairs from one encoder pass, with their forward-backward consistency.  image1, image2:
+    [B,3,H,W] (0..255) on the model's device, of any size: they are padded with InputPadder(mode) and the results unpadded.
+    flow_init: None or a pair (fw, bw) of low-resolution warm starts, each [B,2,H'/8,W'/8] at the padded size or None.
+    Returns a dict of flow_low / flow_up (image1 -> image2), flow_low_bw / flow_up_bw (image2 -> image1), each the flow
+    model(...) gives for that order of the frames (flow_low stays at the padded 1/8 resolution, as the forward's), and of
+    occ / occ_bw (uint8 [B,H,W]) and fb_err / fb_err_bw (float32 [B,H,W]) of rnc.metrics.fb_consistency(flow_up, flow_up_bw,
+    alpha1, alpha2) on the unpadded flows.  return_confidence (NCUP model): also confidence / confidence_bw, the upsampler's
+    output confidence unpadded like the flows.  Inference only: with grad enabled on a model that requires grad it raises
+    ValueError."""
+    from .metrics import fb_consistency
+    if image1.dim() != 4 or image1.shape != image2.shape:
+        raise ValueError(f"bidirectional_flow: expected two [B,3,H,W] images of one shape, got {tuple(image1.shape)} and "
+                         f"{tuple(image2.shape)}")
+    B = image1.shape[0]
+    padder = InputPadder(image1.shape, mode=mode)
+    p1, p2 = padder.pad(image1.float(), image2.float())
+    out = model.forward_bidirectional(p1, p2, iters=iters, flow_init=flow_init, return_confidence=return_confidence)
+    flow_low, flow_up = out[0], padder.unpad(out[1])
+    res = {"flow_low": flow_low[:B], "flow_up": flow_up[:B], "flow_low_bw": flow_low[B:], "flow_up_bw": flow_up[B:]}
+    if return_confidence:
+        conf = padder.unpad(out[2])
+        res["confidence"], res["confidence_bw"] = conf[:B], conf[B:]
+    res["occ"], res["occ_bw"], res["fb_err"], res["fb_err_bw"] = fb_consistency(res["flow_up"], res["flow_up_bw"], alpha1, alpha2)
+    return res
+
+
 @torch.no_grad()
-def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda", confidence=False):
+def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda", confidence=False, consistency=False):
     """samples: iterable of (image1 [3,H,W], image2 [3,H,W], flow_gt [2,H,W], valid [H,W] or None).
     Returns the metrics validate_sintel / validate_kitti print: EPE, 1px/3px/5px, and KITTI F1 when `valid` is given
     (rnc.metrics.summarize: Sintel-style pools every pixel, KITTI-style averages the per-image mean EPE).
@@ -75,17 +103,24 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
     confidence=True (NCUP model) also evaluates the upsampler's output confidence: the forward returns it, unpadded like the
     flow, each pixel is scored by rnc.metrics.confidence_score, and rnc.metrics.sparsification's per-image partials travel
     with the flow metrics'.  The dict gains "sparsification" and "ideal" (100 mean EPEs each, at the removed fractions k/100)
-    and "ause" (rnc.metrics.summarize_sparsification); its other keys are those of confidence=False, bit for bit."""
+    and "ause" (rnc.metrics.summarize_sparsification); its other keys are those of confidence=False, bit for bit.
+
+    consistency=True evaluates forward-backward consistency as a reliability score: each batch runs the bidirectional pass
+    (model.forward_bidirectional), its forward flow is scored as above, and each pixel is ranked by -fb_err of
+    rnc.metrics.fb_consistency.  The dict gains "fb_sparsification", "fb_ause" and "ideal" (which depends on the EPE only,
+    so one serves both scores).  The forward rows of the bidirectional pass are the flows of model(image1, image2), so the
+    other keys are those of consistency=False: bit for bit wherever the forward itself repeats bit for bit (the exact lookup
+    under torch.use_deterministic_algorithms), and within its run-to-run spread otherwise."""
     from .dist import gather_strided, strided_items, world_rank
-    from .metrics import (FRACTIONS, Partials, SparsPartials, cat, confidence_score, flow_metrics, sparsification, summarize,
-                          summarize_sparsification)
+    from .metrics import (FRACTIONS, Partials, SparsPartials, cat, confidence_score, fb_consistency, flow_metrics, sparsification,
+                          summarize, summarize_sparsification)
     model.eval()
     world, rank = world_rank()
     dev = torch.device(device)
     if dev.type == "cuda" and dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     copy_stream = torch.cuda.Stream(dev) if dev.type == "cuda" else None
-    parts, sparse, sparts = [], [], []
+    parts, sparse, sparts, fparts = [], [], [], []
     batches = _shape_batches(strided_items(samples, world, rank), batch_size)
 
     def stage_next():
@@ -102,7 +137,12 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
                     t.record_stream(compute)
         padder = InputPadder(cur.im1.shape, mode=mode)
         p1, p2 = padder.pad(cur.im1.float(), cur.im2.float())
-        if confidence:
+        B = p1.shape[0]
+        if consistency:
+            _, flow_pr, *conf = model.forward_bidirectional(p1, p2, iters=iters, return_confidence=confidence)
+            flow_bw, flow_pr = padder.unpad(flow_pr[B:]), flow_pr[:B]
+            conf = conf[0][:B] if confidence else None
+        elif confidence:
             _, flow_pr, conf = model(p1, p2, iters=iters, test_mode=True, return_confidence=True)
         else:
             _, flow_pr = model(p1, p2, iters=iters, test_mode=True)
@@ -111,23 +151,30 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
         if confidence:
             sparts.append(sparsification(flow, cur.gt, cur.valid, confidence_score(padder.unpad(conf))))
             del conf
+        if consistency:
+            fb_err = fb_consistency(flow, flow_bw)[2]
+            fparts.append(sparsification(flow, cur.gt, cur.valid, -fb_err))
+            del flow_bw, fb_err
         sparse += cur.sparse
         del cur, p1, p2, flow_pr, flow
         nxt = stage_next()                          # staged while this batch computes
     local = cat(parts)
     rows = list(zip(local.counts.cpu().tolist(), local.epe_sum.cpu().tolist(), sparse))
-    if confidence:
-        cols = [torch.cat(c).cpu().tolist() for c in zip(*sparts)] if sparts else [[], [], []]
+    scores = [sp for on, sp in ((confidence, sparts), (consistency, fparts)) if on]
+    for sp in scores:
+        cols = [torch.cat(c).cpu().tolist() for c in zip(*sp)] if sp else [[], [], []]
         rows = [r + s for r, s in zip(rows, zip(*cols))]
     rows = gather_strided(rows, world)
     every = Partials(torch.tensor([r[0] for r in rows], dtype=torch.int64).view(-1, 5),
                      torch.tensor([r[1] for r in rows], dtype=torch.float64))
     res = summarize(every, "kitti" if any(r[2] for r in rows) else "sintel")
-    if confidence:
-        res.update(summarize_sparsification(SparsPartials(
-            torch.tensor([r[3] for r in rows], dtype=torch.int64).view(-1, FRACTIONS),
-            torch.tensor([r[4] for r in rows], dtype=torch.float64).view(-1, FRACTIONS),
-            torch.tensor([r[5] for r in rows], dtype=torch.float64).view(-1, FRACTIONS))))
+    for i, prefix in enumerate(p for on, p in ((confidence, ""), (consistency, "fb_")) if on):
+        c = 3 + 3 * i
+        summ = summarize_sparsification(SparsPartials(
+            torch.tensor([r[c] for r in rows], dtype=torch.int64).view(-1, FRACTIONS),
+            torch.tensor([r[c + 1] for r in rows], dtype=torch.float64).view(-1, FRACTIONS),
+            torch.tensor([r[c + 2] for r in rows], dtype=torch.float64).view(-1, FRACTIONS)))
+        res.update({prefix + "sparsification": summ["sparsification"], "ideal": summ["ideal"], prefix + "ause": summ["ause"]})
     return res
 
 

@@ -227,3 +227,92 @@ def confidence_score(conf):
     cu, cv = conf[:, 0].float(), conf[:, 1].float()
     den = cu + cv
     return torch.where(den == 0, torch.zeros_like(den), (2 * cu * cv) / den)
+
+
+OCC_INCONSISTENT, OCC_OUTSIDE = 1, 2          # bits of fb_consistency's occ
+
+
+def _check_fb(flow_fw, flow_bw):
+    if flow_fw.dim() != 4 or flow_fw.shape[1] != 2 or flow_bw.shape != flow_fw.shape:
+        raise ValueError(f"fb_consistency: expected forward and backward flows of one [B,2,H,W] shape, got "
+                         f"{tuple(flow_fw.shape)} and {tuple(flow_bw.shape)}")
+    if flow_fw.device != flow_bw.device:
+        raise ValueError(f"fb_consistency: the flows are on {flow_fw.device} and {flow_bw.device}; they must be on one device")
+    if flow_fw.numel() == 0:
+        raise ValueError(f"fb_consistency: empty flows {tuple(flow_fw.shape)}")
+
+
+def fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5):
+    """Forward-backward consistency (UnFlow, Meister et al. 2018) of B flow pairs at full resolution.  flow_fw: [B,2,H,W]
+    from frame 1 to frame 2, flow_bw: from frame 2 to frame 1 (any strides; float32, or converted to it).
+
+    Per pixel x of direction F -> G (and G -> F): the target p = x + F(x), G^(p) sampled bilinearly with zero padding on
+    align_corners=True pixel coordinates (utils.utils.bilinear_sampler), err = |F(x) + G^(p)|, and occ with bit 0
+    (OCC_INCONSISTENT) where |F + G^|^2 > alpha1 (|F|^2 + |G^|^2) + alpha2 or that sum is not finite, and bit 1 (OCC_OUTSIDE)
+    where p lies outside [0, W-1] x [0, H-1].  A pixel whose target is outside, or whose inputs hold a NaN, gets err = +inf
+    and the bits that apply.  Returns (occ_fw, occ_bw) uint8 [B,H,W] and (err_fw, err_bw) float32 [B,H,W]: CUDA tensors
+    through rnc_fb_consistency (one launch, enqueued on the current stream), CPU tensors through host_fb_consistency; both
+    round every operation once in float32, in the same order, so they give the same bits."""
+    _check_fb(flow_fw, flow_bw)
+    if not flow_fw.is_cuda:
+        return host_fb_consistency(flow_fw, flow_bw, alpha1, alpha2)
+    fw, bw = flow_fw.float(), flow_bw.float()
+    B, _, H, W = fw.shape
+    dev = fw.device
+    occ = torch.empty(2, B, H, W, dtype=torch.uint8, device=dev)
+    err = torch.empty(2, B, H, W, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        native.rnc.fb_consistency(fw, *fw.stride(), bw, *bw.stride(), B, H, W, float(alpha1), float(alpha2), occ[0], occ[1],
+                                  err[0], err[1])
+    return occ[0], occ[1], err[0], err[1]
+
+
+def _fb_direction(f, g, a1, a2):
+    """One direction of host_fb_consistency: f, g fp64 [B,2,H,W] holding float32 values; a1, a2 float32 values."""
+    B, _, H, W = f.shape
+    u = torch.arange(W, dtype=torch.float64).view(1, 1, W)
+    v = torch.arange(H, dtype=torch.float64).view(1, H, 1)
+    fu, fv = f[:, 0], f[:, 1]
+    px, py = _f32(u + fu), _f32(v + fv)
+    inside = (px >= 0) & (px <= W - 1) & (py >= 0) & (py <= H - 1)
+    x0, y0 = torch.floor(px), torch.floor(py)
+    ax, ay = _f32(px - x0), _f32(py - y0)
+    bx, by = _f32(1 - ax), _f32(1 - ay)
+    ix = torch.where(inside, x0, 0).long()
+    iy = torch.where(inside, y0, 0).long()
+    bi = torch.arange(B).view(B, 1, 1).expand_as(ix)
+
+    def tap(dx, dy, c):
+        x, y = ix + dx, iy + dy
+        ok = (x < W) & (y < H)
+        return torch.where(ok, g[bi, c, y.clamp(max=H - 1), x.clamp(max=W - 1)], 0.0)
+
+    w00, w01, w10, w11 = _f32(bx * by), _f32(ax * by), _f32(bx * ay), _f32(ax * ay)
+    gs = []
+    for c in range(2):
+        s = _f32(tap(0, 0, c) * w00)
+        s = _f32(s + _f32(tap(1, 0, c) * w01))
+        s = _f32(s + _f32(tap(0, 1, c) * w10))
+        gs.append(_f32(s + _f32(tap(1, 1, c) * w11)))
+    su, sv = _f32(fu + gs[0]), _f32(fv + gs[1])
+    lhs = _f32(_f32(su * su) + _f32(sv * sv))
+    mf = _f32(_f32(fu * fu) + _f32(fv * fv))
+    mg = _f32(_f32(gs[0] * gs[0]) + _f32(gs[1] * gs[1]))
+    rhs = _f32(_f32(a1 * _f32(mf + mg)) + a2)
+    finite = torch.isfinite(lhs)
+    inf = torch.full_like(lhs, float("inf"))
+    err = torch.where(inside & finite, _f32(torch.where(finite, lhs, 0.0).sqrt()), inf)
+    occ = torch.where(inside, (~finite | (lhs > rhs)).to(torch.uint8), torch.full_like(lhs, 3, dtype=torch.uint8))
+    return occ, err.float()
+
+
+def host_fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5):
+    """fb_consistency's definition in torch: each operation evaluated in fp64 on float32 operands and rounded once to float32
+    (the IEEE float32 result, as in host_partials), in the kernel's order.  Serves CPU tensors and is the kernel's test
+    reference."""
+    _check_fb(flow_fw, flow_bw)
+    f, g = flow_fw.detach().cpu().float().double(), flow_bw.detach().cpu().float().double()
+    a1, a2 = float(torch.tensor(alpha1, dtype=torch.float32)), float(torch.tensor(alpha2, dtype=torch.float32))
+    occ_fw, err_fw = _fb_direction(f, g, a1, a2)
+    occ_bw, err_bw = _fb_direction(g, f, a1, a2)
+    return occ_fw, occ_bw, err_fw, err_bw

@@ -97,7 +97,8 @@ class _RAFTBase(nn.Module):
         """The iteration loop on the engine's resident buffers.  upsample(eng, ws, pu) produces each full-resolution prediction
         from the workspace; the default is the inference upsampler (self._upsample on packed weights).  encode(eng, ws, image1,
         image2) fills the feature maps and the GRU state; the default encodes both frames (self._encode).  ws: a workspace the
-        caller owns instead of the engine's shared one of this shape.  return_confidence: upsample(eng, ws, pu, True) returns
+        caller owns instead of the engine's shared one of this shape; with an encode that fills more slots than the images'
+        batch (BidirectionalStage), flow_init is [ws.B,2,H/8,W/8].  return_confidence: upsample(eng, ws, pu, True) returns
         (flow, confidence), and the forward returns the confidences next to the flows (forward's return_confidence)."""
         B, _, Him, Wim = image1.shape
         H8, W8 = Him // 8, Wim // 8
@@ -115,9 +116,9 @@ class _RAFTBase(nn.Module):
         fi = None
         if flow_init is not None:
             fi = flow_init.to(image1.device).float().contiguous()
-            if fi.shape != (B, 2, H8, W8):
+            if fi.shape != (ws.B, 2, H8, W8):
                 raise ValueError("flow_init must be [N,2,H/8,W/8]")
-        rnc.coords_init(ws.coords1, fi, B, H8, W8)
+        rnc.coords_init(ws.coords1, fi, ws.B, H8, W8)
 
         preds, confs = [], []
         flow_up = conf_up = None
@@ -138,6 +139,60 @@ class _RAFTBase(nn.Module):
         if test_mode:
             return (eng.flow_low(ws), flow_up, conf_up) if return_confidence else (eng.flow_low(ws), flow_up)
         return (preds, confs) if return_confidence else preds
+
+    def forward_bidirectional(self, image1, image2, iters=12, flow_init=None, return_confidence=False):
+        """Test-mode flow in both directions of B pairs from one encoder pass (rnc.harness.bidirectional_flow pads, unpads and
+        checks consistency on top).  image1, image2: [B,3,H,W] in 0..255, H and W multiples of 8.  flow_init: None or a pair
+        (fw, bw), each [B,2,H/8,W/8] or None (a cold start for that direction).  Returns (flow_low, flow_up), with
+        return_confidence (NCUP model) (flow_low, flow_up, confidence), of 2B rows: row j is image1[j] -> image2[j], row B + j
+        image2[j] -> image1[j], each what forward(..., test_mode=True) gives for that order of the frames.  Inference only."""
+        if return_confidence and not self.ncup:
+            raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
+        if self._needs_grad():
+            raise ValueError("forward_bidirectional is inference only: call it under torch.no_grad() (training through the "
+                             "bidirectional pass is not built)")
+        if image1.shape != image2.shape or image1.dim() != 4:
+            raise ValueError(f"forward_bidirectional: expected two [B,3,H,W] images of one shape, got {tuple(image1.shape)} "
+                             f"and {tuple(image2.shape)}")
+        B, _, Him, Wim = image1.shape
+        fi = None
+        if flow_init is not None:
+            if not isinstance(flow_init, (tuple, list)) or len(flow_init) != 2:
+                raise ValueError("flow_init: expected a pair (fw, bw), each [B,2,H/8,W/8] or None")
+            fw, bw = flow_init
+            for f in (fw, bw):
+                if f is not None and tuple(f.shape) != (B, 2, Him // 8, Wim // 8):
+                    raise ValueError(f"flow_init: expected [B,2,H/8,W/8] = {(B, 2, Him // 8, Wim // 8)}, got {tuple(f.shape)}")
+            if fw is not None or bw is not None:
+                ref = fw if fw is not None else bw
+                # a missing direction starts cold: coords0 + 0.0 is exactly coords0, as with no flow_init
+                fi = torch.cat([(f if f is not None else torch.zeros_like(ref)).float() for f in (fw, bw)])
+        dev = _require_cuda(image1, image2, fi)
+        pdev = module_device(self)
+        if pdev != dev:
+            raise ValueError(f"model parameters are on {pdev} but the images are on {dev}")
+        eng = engine_for(dev)
+        conf = bool(return_confidence)
+        with torch.cuda.device(dev), eng.lock:
+            if iters < 1:
+                raise ValueError("iters must be >= 1")
+            if Him % 8 or Wim % 8:
+                raise ValueError("image height/width must be multiples of 8 (pad with utils.utils.InputPadder, evaluate.py:125)")
+            if hasattr(self, "data_idx"):
+                self.data_idx += 1
+            if eng.graphs_enabled(self):
+                return eng.graph_forward(self, image1, image2, iters, fi, return_confidence=conf, bidirectional=True)
+            return self._forward_bidirectional(eng, image1, image2, iters, fi, conf)
+
+    def _forward_bidirectional(self, eng, image1, image2, iters, flow_init, return_confidence=False):
+        """The bidirectional pass on the engine: _forward_eager over 2B slots of the engine's workspace, slot j holding
+        (image1[j], image2[j]) and slot B + j (image2[j], image1[j]), encoded by BidirectionalStage.  flow_init: [2B,2,H/8,W/8]
+        or None."""
+        B, _, Him, Wim = image1.shape
+        pk = eng.packed_update(self.update_block)
+        ws = eng.workspace(image1.device, 2 * B, Him // 8, Wim // 8, pk.has_mask, self.ncup)
+        return self._forward_eager(eng, image1, image2, iters, flow_init, True, encode=BidirectionalStage(self), ws=ws,
+                                   return_confidence=return_confidence)
 
     def _umma_encoders(self, eng):
         """Do the encoders run on the tensor-core path (else on torch modules: RNC_ENCODER=cudnn, RNC_CONV=ffma, amp)?"""
@@ -294,6 +349,34 @@ class SequenceStage:
         self.fmap2 = f[:B]
         net, inp = m._context(image1)
         eng.fmap_prepare(ws, self.fmap1, self.fmap2, 4)
+        eng.load_state(ws, net, inp)
+
+
+class BidirectionalStage:
+    """Encoder stage of the bidirectional pass (_RAFTBase.forward_bidirectional), for _forward_eager(encode=...) on a
+    workspace of 2B slots: slot j holds the pair (image1[j], image2[j]), slot B + j the pair (image2[j], image1[j]).  fnet
+    runs once on the 2B frames cat(image1, image2), the images a one-directional forward encodes: its features are fmap1 of
+    the slots in frame order, and fmap2 with the two halves swapped.  cnet runs on the same 2B frames, so each direction gets
+    the context of its own first frame."""
+
+    def __init__(self, model):
+        self.model = model
+
+    def __call__(self, eng, ws, image1, image2):
+        m = self.model
+        if m._umma_encoders(eng):
+            with _Timed(eng, "encoders"):
+                eng.encoder().run_bidirectional(m, ws, image1.float().contiguous(), image2.float().contiguous())
+                eng.finish_fmaps(ws)
+            return
+        B = image1.shape[0]
+        both = torch.cat([image1, image2])
+        both = (2 * (both / 255.0) - 1.0).contiguous()
+        with torch.autocast("cuda", enabled=bool(getattr(m.args, "mixed_precision", False))):
+            f = m.fnet(both)
+        f = f.float().contiguous()
+        net, inp = m._context(both)
+        eng.fmap_prepare(ws, f, torch.cat([f[B:], f[:B]]), 4)
         eng.load_state(ws, net, inp)
 
 

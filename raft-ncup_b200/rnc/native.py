@@ -149,6 +149,8 @@ SIGNATURES = {
     "rnc_sparsification_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
     "rnc_sparsification": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 3,
                                 _vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_fb_consistency": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp,
+                                _vp]),
 }
 
 _lib = None
