@@ -33,7 +33,7 @@ typedef enum {
 } rnc_status;
 
 /* Library identity / diagnostics. */
-int rnc_abi_version(void);                 /* bumps on any signature change (now 17) */
+int rnc_abi_version(void);                 /* bumps on any signature change (now 18) */
 const char* rnc_build_info(void);          /* e.g. "sm_90a nvcc 12.9" */
 const char* rnc_status_string(int status);
 int rnc_last_cuda_error(void);             /* cudaError_t of the last failed launch on this thread */
@@ -122,11 +122,8 @@ typedef enum {
 
 /* rnc_conv_umma_desc.flags */
 #define RNC_CONV_NO_HALO 1          /* force one A tile per filter tap (disable the row/column halo sharing) */
-#define RNC_CONV_BASE_OFFSET 2      /* reserved (round-1 debug switch for the descriptor base_offset; ignored)  */
 #define RNC_CONV_AUX_BLOCKED 16     /* aux0 (z gate) and add are tile-blocked: element (tile, channel c, row r) at ((tile*ld + c)*128 + r) */
 #define RNC_CONV_OUT_BLOCKED 32     /* RNC_EPI_LINEAR: out_f32 in the same tile-blocked layout (produces an `add` operand)          */
-#define RNC_CONV_NO_PAIR 8          /* accepted; sm_90 has one (single-CTA) form              */
-#define RNC_CONV_SPLIT_N 4          /* accepted; column tiles are at most 128 wide on sm_90           */
 #define RNC_CONV_WINDOW 128        /* in0 is a sliding-window view of a padded plane, see rnc_conv_umma_desc.win_pitch */
 #define RNC_CONV_TF32 64            /* operands are fp32 hi/lo planes consumed as TF32 (wgmma .tf32, K = 8): value = hi + lo with
                                      * hi = tf32(value), 3 MMAs per K step as in the fp16 form but with fp32's exponent range — the
@@ -252,10 +249,6 @@ int rnc_instnorm_apply(const float* x, const float* mean_rstd, const float* res,
                        float* out_f32, void* out_hi, void* out_lo, void* stream);
 /* Pooling half of rnc_fmap_prepare for feature maps that are already CL: fills levels 1..levels-1 of f2_pyr from level 0. */
 int rnc_fmap_pyramid(float* f2_pyr, int B, int D, int H, int W, int levels, void* stream);
-
-/* convf1 with split-halves CL output (feeds the tensor-core convf2). */
-int rnc_conv_flow7x7_split_fwd(const float* coords1, const float* weight, const float* bias, int B, int H, int W,
-                               int cout, void* out_hi, void* out_lo, int ldo, void* stream);
 
 /* FlowHead.conv2 (update.py:10,14) fused with `coords1 = coords1 + delta_flow` (raft_nc_dbl.py:157):
  * in CL [B][H][W][cin]; weight packed [9][cin][2]; delta (optional, may be NULL) and coords1 NCHW [B][2][H][W]. */

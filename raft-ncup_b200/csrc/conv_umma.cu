@@ -622,24 +622,22 @@ static int sm_count() {
 }
 
 template <int BN, int EC>
-static int launch(const CUtensorMap* maps, Params& p, cudaStream_t stream, int max_sa, int max_sb) {
+static int launch(const CUtensorMap* maps, Params& p, cudaStream_t stream) {
   using C = Cfg<BN>;
   const int a_stage = 2 * p.a_plane;
   // ring depths within the shared memory the accumulator tile and the staging leave: both rings hide the same TMA
   // latency, so deepen A (up to 4) while B keeps >= 2 stages
   const int budget = C::kRingBudget, b_stage = 2 * C::kBTile;
-  const int sa_cap = max_sa > 0 && max_sa < kMaxSA ? max_sa : kMaxSA;      // debug knobs (rnc_conv_umma_desc.flags bits 8-15)
   p.SA = 2;
-  while (p.SA < sa_cap && budget - (p.SA + 1) * a_stage >= 2 * b_stage) ++p.SA;
+  while (p.SA < kMaxSA && budget - (p.SA + 1) * a_stage >= 2 * b_stage) ++p.SA;
   int sb = (budget - p.SA * a_stage) / b_stage;
   p.SB = sb > 8 ? 8 : sb < 2 ? 2 : sb;
-  if (max_sb > 0 && p.SB > max_sb) p.SB = max_sb;
   // Small layers (64 -> 64 3x3: 9 stages of 16 KB): keep the whole weight matrix in the ring for the CTA's lifetime instead
   // of re-streaming it for every pixel tile.
   p.resident_b = 0;
   {
     const int nb = p.kh * p.kw * p.nblk;
-    if (p.ntn == 1 && nb <= kMaxSB && nb > p.SB && max_sb == 0 && 2 * a_stage + nb * b_stage <= budget) {
+    if (p.ntn == 1 && nb <= kMaxSB && nb > p.SB && 2 * a_stage + nb * b_stage <= budget) {
       p.resident_b = 1; p.SB = nb; p.SA = (budget - nb * b_stage) / a_stage;
       if (p.SA > kMaxSA) p.SA = kMaxSA;
     }
@@ -657,11 +655,11 @@ static int launch(const CUtensorMap* maps, Params& p, cudaStream_t stream, int m
 }
 
 template <int EC>
-static int launch_bn(int bn, const CUtensorMap* maps, Params& p, cudaStream_t s, int msa, int msb) {
+static int launch_bn(int bn, const CUtensorMap* maps, Params& p, cudaStream_t s) {
   switch (bn) {
-    case 32: return launch<32, EC>(maps, p, s, msa, msb);
-    case 64: return launch<64, EC>(maps, p, s, msa, msb);
-    default: return launch<128, EC>(maps, p, s, msa, msb);
+    case 32: return launch<32, EC>(maps, p, s);
+    case 64: return launch<64, EC>(maps, p, s);
+    default: return launch<128, EC>(maps, p, s);
   }
 }
 
@@ -691,7 +689,6 @@ extern "C" long long rnc_conv_umma_tiles(int kh, int kw, int stride, int B, int 
 // 128 / 64 / 32 columns (operand bytes per K-step: the A tile plus the weight tile), + 0.5 per item, x1.08 when the A tile
 // is loaded more than once.
 static int choose_bn(const rnc_conv_umma_desc& d, int bn_max, int stride, int H, int W) {
-  if (d.flags & RNC_CONV_SPLIT_N) return bn_max;
   const int bkc = (d.flags & RNC_CONV_TF32) ? 32 : 64;
   const int taps = d.kh * d.kw, ksteps = taps * ((d.c0 + bkc - 1) / bkc + (d.c1 + bkc - 1) / bkc);
   int TW, TH;
@@ -856,14 +853,13 @@ static int conv_umma(const rnc_conv_umma_desc& d, umma::Phase ph, void* stream) 
   if (!ok) return RNC_ERR_BAD_SHAPE;
 
   cudaStream_t s = as_stream(stream);
-  const int msa = (d.flags >> 8) & 15, msb = (d.flags >> 12) & 15;
   const bool plain = (d.epilogue == RNC_EPI_LINEAR || d.epilogue == RNC_EPI_RELU || d.epilogue == RNC_EPI_SIGMOID) && !d.stats;
   const int ec = d.epilogue == RNC_EPI_GRU_ZR ? EC_GRU_ZR : d.epilogue == RNC_EPI_GRU_Q ? EC_GRU_Q : plain ? EC_PLAIN : EC_MISC;
   switch (ec) {
-    case EC_GRU_ZR: return launch_bn<EC_GRU_ZR>(bn, maps, p, s, msa, msb);
-    case EC_GRU_Q: return launch_bn<EC_GRU_Q>(bn, maps, p, s, msa, msb);
-    case EC_MISC: return launch_bn<EC_MISC>(bn, maps, p, s, msa, msb);
-    default: return launch_bn<EC_PLAIN>(bn, maps, p, s, msa, msb);
+    case EC_GRU_ZR: return launch_bn<EC_GRU_ZR>(bn, maps, p, s);
+    case EC_GRU_Q: return launch_bn<EC_GRU_Q>(bn, maps, p, s);
+    case EC_MISC: return launch_bn<EC_MISC>(bn, maps, p, s);
+    default: return launch_bn<EC_PLAIN>(bn, maps, p, s);
   }
 }
 

@@ -88,7 +88,7 @@ using namespace rnc;
 
 extern "C" {
 
-int rnc_abi_version(void) { return 17; }
+int rnc_abi_version(void) { return 18; }
 const char* rnc_build_info(void) { return "librnc sm_90a (CUDA " RNC_STR_CUDA ")"; }
 const char* rnc_status_string(int s) {
   switch (s) {

@@ -47,14 +47,9 @@ inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s
 // Programmatic dependent launch (PDL).  A kernel launched with launch_pdl() may start while its predecessor in the stream is
 // still draining: it runs its prologue (barrier init, descriptor prefetch), then pdl_wait() blocks until the
 // predecessor has completed and its writes are visible.  pdl_trigger() in the predecessor lets the dependent start early;
-// without it the dependent starts at the predecessor's exit (plain stream order).  RNC_PDL=0 disables the attribute.
+// without it the dependent starts at the predecessor's exit (plain stream order).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-inline bool pdl_enabled() {
-  static const int on = [] { const char* e = getenv("RNC_PDL"); return (e && e[0] == '0') ? 0 : 1; }();
-  return on != 0;
-}
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
@@ -63,7 +58,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 

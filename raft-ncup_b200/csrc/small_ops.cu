@@ -13,8 +13,7 @@ namespace rnc {
 constexpr int F7_PX = 16;   // pixels (along x) per CTA
 __global__ void __launch_bounds__(128)
 conv_flow7x7_kernel(const float* __restrict__ coords1, const float* __restrict__ weight, const float* __restrict__ bias,
-                    int B, int H, int W, int cout, float* __restrict__ out, int ldo, __half* __restrict__ out_hi,
-                    __half* __restrict__ out_lo) {
+                    int B, int H, int W, int cout, float* __restrict__ out, int ldo) {
   __shared__ float patch[2][7][F7_PX + 6];
   const int b = blockIdx.z, y = blockIdx.y, x0 = blockIdx.x * F7_PX;
   const int HW = H * W;
@@ -46,17 +45,7 @@ conv_flow7x7_kernel(const float* __restrict__ coords1, const float* __restrict__
       }
 #pragma unroll
     for (int i = 0; i < F7_PX; ++i)
-      if (x0 + i < W) {
-        const size_t idx = ((size_t)b * HW + y * W + x0 + i) * ldo + co;
-        const float v = fmaxf(acc[i], 0.f);
-        if (out) out[idx] = v;
-        if (out_hi) {
-          const float vc = fminf(v, 65504.f);
-          const __half hi = __float2half_rn(vc);
-          out_hi[idx] = hi;
-          out_lo[idx] = __float2half_rn(vc - __half2float(hi));
-        }
-      }
+      if (x0 + i < W) out[((size_t)b * HW + y * W + x0 + i) * ldo + co] = fmaxf(acc[i], 0.f);
   }
 }
 
@@ -327,17 +316,7 @@ int rnc_conv_flow7x7_fwd(const float* coords1, const float* weight, const float*
   if (B <= 0 || H <= 0 || W <= 0 || cout <= 0 || ldo < cout) return RNC_ERR_BAD_SHAPE;
   if (!coords1 || !weight || !bias || !out) return RNC_ERR_BAD_POINTER;
   dim3 grid((W + F7_PX - 1) / F7_PX, H, B);
-  conv_flow7x7_kernel<<<grid, 128, 0, as_stream(stream)>>>(coords1, weight, bias, B, H, W, cout, out, ldo, nullptr, nullptr);
-  return after_launch();
-}
-
-int rnc_conv_flow7x7_split_fwd(const float* coords1, const float* weight, const float* bias, int B, int H, int W,
-                               int cout, void* out_hi, void* out_lo, int ldo, void* stream) {
-  if (B <= 0 || H <= 0 || W <= 0 || cout <= 0 || ldo < cout) return RNC_ERR_BAD_SHAPE;
-  if (!coords1 || !weight || !bias || !out_hi || !out_lo) return RNC_ERR_BAD_POINTER;
-  dim3 grid((W + F7_PX - 1) / F7_PX, H, B);
-  conv_flow7x7_kernel<<<grid, 128, 0, as_stream(stream)>>>(coords1, weight, bias, B, H, W, cout, nullptr, ldo,
-                                                           static_cast<__half*>(out_hi), static_cast<__half*>(out_lo));
+  conv_flow7x7_kernel<<<grid, 128, 0, as_stream(stream)>>>(coords1, weight, bias, B, H, W, cout, out, ldo);
   return after_launch();
 }
 

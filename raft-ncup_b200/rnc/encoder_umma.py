@@ -119,7 +119,7 @@ class EncoderRunner:
         st = bufs.stats.data_ptr() if fused else 0
         h, w, _ = bufs.dims[0]
         rnc.stem_window_prep(image, N, Hin, Win, bufs.pitch, bufs.img_hi, bufs.img_lo)
-        win = dict(stride=2, hin=Hin, win=w, win_pitch=4 * bufs.pitch, flags=eng.conv_flags | E.CONV_WINDOW)
+        win = dict(stride=2, hin=Hin, win=w, win_pitch=4 * bufs.pitch, flags=E.CONV_WINDOW)
         img = (bufs.img_hi.data_ptr(), bufs.img_lo.data_ptr())
         if inst:
             eng.uconv(N, h, w, img, 64, 8, pk.stem, E.EPI_LINEAR, out_f32=bufs.T32[0].data_ptr(), ldo_f32=64,

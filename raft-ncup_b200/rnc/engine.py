@@ -312,18 +312,18 @@ class _Timed:
 
 _ENGINES = {}
 _ENGINES_LOCK = threading.Lock()
-_ENGINE_ENV = ("RNC_CONV", "RNC_LOOKUP", "RNC_CONVF1", "RNC_FORK", "RNC_BLOCKED", "RNC_CONV_FLAGS")
+_ENGINE_ENV = ("RNC_CONV", "RNC_LOOKUP")
 
 
 def engine_for(device):
-    """The engine of one CUDA device.  Engines (packed weights, workspaces, side streams) are per-device process-wide state
+    """The engine of one CUDA device.  Engines (packed weights, workspaces) are per-device process-wide state
     that lives OUTSIDE the nn.Modules: modules stay deep-copyable / picklable, and nn.DataParallel replicas (one thread per
     device, shallow-copied module __dict__) never share packed weights or workspaces across devices."""
     device = torch.device(device)
     if device.type != "cuda":
         raise native.RncUnavailable("the RAFT-NCUP hot path runs only on CUDA (sm_90a) devices; there is no CPU fallback")
     idx = device.index if device.index is not None else torch.cuda.current_device()
-    key = (idx,) + tuple(os.environ.get(k, "") for k in _ENGINE_ENV)      # developer switches select distinct engines
+    key = (idx,) + tuple(os.environ.get(k, "") for k in _ENGINE_ENV)      # RNC_CONV / RNC_LOOKUP select distinct engines
     eng = _ENGINES.get(key)
     if eng is None:
         with _ENGINES_LOCK:
@@ -351,7 +351,6 @@ class Engine:
     """Issues the kernels.  One per CUDA device (engine_for); keeps packed weights and workspaces.  ``lock`` serialises the
     forwards of one device (nn.DataParallel drives different devices from different threads: different engines)."""
     mode = "ffma"
-    fork_convf1 = False
     PACK_UB, PACK_UP = PackedUpdateBlock, ExactWnet         # PACK_UP: the upsampler's weights-net format
     WS = Workspace
     MAX_WS, MAX_PACKED = 6, 64
@@ -397,7 +396,7 @@ class Engine:
         if os.environ.get("RNC_PARAM_CHECK", "") == "checksum" or getattr(model, "_is_replica", False):
             return False
         return not getattr(model.args, "mixed_precision", False) and os.environ.get("RNC_ENCODER", "umma").lower() == "umma" \
-            and self.mode == "umma" and not self.fork_convf1
+            and self.mode == "umma"
 
     def graph_forward(self, model, image1, image2, iters, flow_init, return_confidence=False, bidirectional=False):
         """Second and later forwards with the same signature (shape, iterations, warm start or not, weights, confidence or
@@ -478,9 +477,6 @@ class Engine:
     def lookup(self, ws, coords, out, layout, ldo, radius=4):
         with _Timed(self, "corr_lookup"):
             rnc.corr_lookup_fwd(ws.f1_cl, ws.f2_pyr, coords, ws.B, ws.D, ws.H8, ws.W8, ws.levels, radius, out, layout, ldo)
-
-    def begin_iter(self, ws, pk):
-        """Hook called before the lookup of every iteration (the tensor-core engine forks independent work here)."""
 
     def lookup_resident(self, ws):
         """Per-iteration lookup at ws.coords1 into the resident corr buffer (CL fp32)."""

@@ -7,7 +7,7 @@ import math
 import torch
 
 from . import native
-from .engine import CORR_CH, HX_LD, Engine, _Timed, pack_thin
+from .engine import CORR_CH, HX_LD, Engine, _Timed
 from .native import UmmaConvDesc, rnc
 
 CORR_LS = 88           # channels reserved per pyramid level in the resident corr row: 81 taps + 7 zero pads (16-byte groups)
@@ -90,7 +90,6 @@ class PackedUpdateUmma:
         cat = torch.cat
         self.convc1 = UmmaWeights(expand_corr_weight(e.convc1.weight), e.convc1.bias, [CORR_LD])
         self.convc2 = UmmaWeights(e.convc2.weight, e.convc2.bias, [256])
-        self.convf1 = (pack_thin(e.convf1.weight), e.convf1.bias.detach().float().contiguous())    # CUDA-core form (RNC_CONVF1=ffma)
         # convf1 (7x7, 2 -> 128) as a 1x1 layer over the im2col'ed flow neighbourhood: k = 2*(7*ky+kx)+c, K = 98 (+30)
         wf = e.convf1.weight.detach().float()
         self.convf1_mm = UmmaWeights(wf.permute(0, 2, 3, 1).reshape(wf.shape[0], 98, 1, 1), e.convf1.bias, [98])
@@ -175,8 +174,7 @@ class UmmaWorkspace:
         # Epilogue-only tensors live in the tile-blocked layout [tile][channel][128 px] of their layer's tiling (thread = pixel
         # then reads / writes full lines): the z gate, and the hoisted context-feature share of the GRU gate pre-activations
         # (valid until inp changes).  Horizontal (1x5) and vertical (5x1) layers tile differently; z serves both halves.
-        th = max(rnc.conv_umma_tiles(1, 5, 1, B, H8, W8, fl) for fl in (0, 1))      # with / without halo sharing (RNC_CONV_FLAGS)
-        tv = max(rnc.conv_umma_tiles(5, 1, 1, B, H8, W8, fl) for fl in (0, 1))
+        th, tv = rnc.conv_umma_tiles(1, 5, 1, B, H8, W8, 0), rnc.conv_umma_tiles(5, 1, 1, B, H8, W8, 0)
         self.z = torch.empty(max(th, tv) * 128 * 128, **f)
         self.czr1, self.czr2 = torch.empty(th * 256 * 128, **f), torch.empty(tv * 256 * 128, **f)
         self.cq1, self.cq2 = torch.empty(th * 128 * 128, **f), torch.empty(tv * 128 * 128, **f)
@@ -187,7 +185,6 @@ class UmmaWorkspace:
         self.coords1 = torch.empty(B, 2, H8, W8, **f)
         self.delta = torch.empty(B, 2, H8, W8, **f)
         self.f1_cl = self.f2_pyr = None
-        self.convf1_forked = False
         if with_mask:
             self.mh = SplitBuf(M, 256, device)
             self.mask = torch.empty(M, 576, **f)
@@ -212,21 +209,10 @@ class UmmaEngine(Engine):
         self.lookup_mode = os.environ.get("RNC_LOOKUP", "umma").lower()
         if self.lookup_mode not in ("umma", "ffma"):
             raise ValueError(f"RNC_LOOKUP={self.lookup_mode!r}: expected 'umma' or 'ffma'")
-        # RNC_CONV_FLAGS: bit 0 = one A tile per tap (no halo sharing), bit 1 = no descriptor base_offset (debug)
-        self.conv_flags = int(os.environ.get("RNC_CONV_FLAGS", "0"))
-        # RNC_CONVF1=mm (default): convf1 as flow im2col + 1x1 tensor-core layer on the main stream; ffma: the CUDA-core 7x7
-        # kernel, forked onto a side stream underneath the lookup (RNC_FORK=0 keeps it on the main stream)
-        self.convf1_mode = os.environ.get("RNC_CONVF1", "mm").lower()
-        if self.convf1_mode not in ("mm", "ffma"):
-            raise ValueError(f"RNC_CONVF1={self.convf1_mode!r}: expected 'mm' or 'ffma'")
-        # RNC_BLOCKED=0: keep the z gate / hoisted addends channel-last instead of tile-blocked (developer A/B switch)
-        self.blocked = os.environ.get("RNC_BLOCKED", "1") != "0"
-        self.fork_convf1 = self.convf1_mode == "ffma" and os.environ.get("RNC_FORK", "1") != "0"
-        self._side = None
 
     # ------------------------------------------------------------------ one tensor-core convolution
     def uconv(self, B, H, W, in0, c0, ld0, wt, epi, out_f32=0, ldo_f32=0, out_split=(0, 0), ldo_split=0, in1=(0, 0), c1=0, ld1=0,
-              h=0, ldh=0, aux0=0, ldaux=0, stride=1, hin=0, win=0, res=0, ldres=0, flags=None, stats=0, add=0, ldadd=0, win_pitch=0,
+              h=0, ldh=0, aux0=0, ldaux=0, stride=1, hin=0, win=0, res=0, ldres=0, flags=0, stats=0, add=0, ldadd=0, win_pitch=0,
               dil=1):
         """One rnc_conv2d_umma_fwd call.  H, W are the OUTPUT dims; for stride 2 pass the input dims as hin, win."""
         d = UmmaConvDesc()
@@ -235,7 +221,7 @@ class UmmaEngine(Engine):
         d.stats = stats
         d.add, d.ldadd = add, ldadd
         d.win_pitch = win_pitch
-        d.flags = self.conv_flags if flags is None else flags
+        d.flags = flags
         d.in0_hi, d.in0_lo, d.c0, d.ld0 = in0[0], in0[1], c0, ld0
         d.in1_hi, d.in1_lo, d.c1, d.ld1 = in1[0], in1[1], c1, ld1
         d.w_hi, d.w_lo, d.ktot, d.coutpad = wt.w_hi.data_ptr(), wt.w_lo.data_ptr(), wt.ktot, wt.coutpad
@@ -293,37 +279,15 @@ class UmmaEngine(Engine):
             rnc.corr_lookup_split_fwd(ws.f1_cl, ws.f2_pyr, ws.coords1, ws.B, ws.D, ws.H8, ws.W8, ws.levels, 4, ws.corr.hi,
                                       ws.corr.lo, CORR_LD, CORR_LS)
 
-    def _convf1(self, ws, pk):
-        if self.convf1_mode == "mm":
-            rnc.flow_im2col7_split_fwd(ws.coords1, ws.B, ws.H8, ws.W8, ws.fcol.hi, ws.fcol.lo, 128)
-            self.uconv(ws.B, ws.H8, ws.W8, ws.fcol.ptrs(), 98, 128, pk.convf1_mm, native.EPI_RELU, out_split=ws.f1.ptrs(), ldo_split=128)
-            return
-        rnc.conv_flow7x7_split_fwd(ws.coords1, pk.convf1[0], pk.convf1[1], ws.B, ws.H8, ws.W8, 128, ws.f1.hi, ws.f1.lo, 128)
-
-    def begin_iter(self, ws, pk):
-        """Fork: convf1 (7x7 on the flow, CUDA cores, ~1 KB of shared memory) depends only on coords1, so it runs on a side
-        stream underneath the tensor-core lookup / convc1 / convc2 CTAs that own the SMs; _update_iter joins before convf2."""
-        if not self.fork_convf1:
-            return
-        main = torch.cuda.current_stream()
-        if self._side is None or self._side.device != main.device:
-            self._side = torch.cuda.Stream(device=main.device)
-        self._side.wait_stream(main)
-        with torch.cuda.stream(self._side):
-            self._convf1(ws, pk)
-        ws.convf1_forked = True
-
     def _update_iter(self, ws, pk, want_mask, want_delta):
         B, H, W = ws.B, ws.H8, ws.W8
         E = native
         # BasicMotionEncoder (update.py:89-97)
         self.uconv(B, H, W, ws.corr.ptrs(), CORR_LD, CORR_LD, pk.convc1, E.EPI_RELU, out_split=ws.c1.ptrs(), ldo_split=256)
         self.uconv(B, H, W, ws.c1.ptrs(), 256, 256, pk.convc2, E.EPI_RELU, out_split=ws.corflo.ptrs(), ldo_split=256)
-        if getattr(ws, "convf1_forked", False):
-            torch.cuda.current_stream().wait_stream(self._side)       # join
-            ws.convf1_forked = False
-        else:
-            self._convf1(ws, pk)
+        # convf1 (7x7, 2 -> 128) as the im2col of the flow and a 1x1 layer
+        rnc.flow_im2col7_split_fwd(ws.coords1, B, H, W, ws.fcol.hi, ws.fcol.lo, 128)
+        self.uconv(B, H, W, ws.fcol.ptrs(), 98, 128, pk.convf1_mm, E.EPI_RELU, out_split=ws.f1.ptrs(), ldo_split=128)
         self.uconv(B, H, W, ws.f1.ptrs(), 128, 128, pk.convf2, E.EPI_RELU, out_split=ws.corflo.ptrs(192), ldo_split=256)
         self.uconv(B, H, W, ws.corflo.ptrs(), 256, 256, pk.conv, E.EPI_RELU_FLOW, out_split=ws.hx.ptrs(256), ldo_split=HX_LD,
                    aux0=ws.coords1.data_ptr())
@@ -333,15 +297,15 @@ class UmmaEngine(Engine):
             # the context channels' share of the gate pre-activations (+ biases): once per forward
             for wt, buf in ((pk.zr1_c, ws.czr1), (pk.q1_c, ws.cq1), (pk.zr2_c, ws.czr2), (pk.q2_c, ws.cq2)):
                 self.uconv(B, H, W, ws.hx.ptrs(128), 128, HX_LD, wt, E.EPI_LINEAR, out_f32=buf.data_ptr(), ldo_f32=wt.coutpad,
-                           flags=self.conv_flags | (E.CONV_OUT_BLOCKED if self.blocked else 0))
+                           flags=E.CONV_OUT_BLOCKED)
             ws.gru_const_valid = True
         for zr, q, czr, cq in ((pk.zr1, pk.q1, ws.czr1, ws.cq1), (pk.zr2, pk.q2, ws.czr2, ws.cq2)):
             self.uconv(B, H, W, ws.hx.ptrs(), 128, HX_LD, zr, E.EPI_GRU_ZR, in1=ws.hx.ptrs(256), c1=128, ld1=HX_LD,
                        out_split=ws.rh.ptrs(), ldo_split=128, h=hp, ldh=128, aux0=ws.z.data_ptr(), ldaux=128,
-                       add=czr.data_ptr(), ldadd=256, flags=self.conv_flags | (E.CONV_AUX_BLOCKED if self.blocked else 0))
+                       add=czr.data_ptr(), ldadd=256, flags=E.CONV_AUX_BLOCKED)
             self.uconv(B, H, W, ws.rh.ptrs(), 128, 128, q, E.EPI_GRU_Q, in1=ws.hx.ptrs(256), c1=128, ld1=HX_LD,
                        out_split=ws.hx.ptrs(), ldo_split=HX_LD, h=hp, ldh=128, aux0=ws.z.data_ptr(), ldaux=128,
-                       add=cq.data_ptr(), ldadd=128, flags=self.conv_flags | (E.CONV_AUX_BLOCKED if self.blocked else 0))
+                       add=cq.data_ptr(), ldadd=128, flags=E.CONV_AUX_BLOCKED)
         # FlowHead (update.py:13-14) + coords1 += delta (raft_nc_dbl.py:157)
         self.uconv(B, H, W, ws.hx.ptrs(), 128, HX_LD, pk.fh1, E.EPI_RELU, out_split=ws.fh.ptrs(), ldo_split=256)
         self.uconv(B, H, W, ws.fh.ptrs(), 256, 256, pk.fh2, E.EPI_LINEAR, out_f32=ws.fh2p.data_ptr(), ldo_f32=32)

@@ -125,7 +125,6 @@ class _RAFTBase(nn.Module):
         for itr in range(iters):
             last = itr == iters - 1
             need_up = last or not test_mode     # inference upsamples once (SURVEY.md finding 9); list mode needs all
-            eng.begin_iter(ws, pk)      # forks convf1 (CUDA cores) onto a side stream; it co-runs with the tensor-core lookup
             eng.lookup_resident(ws)
             eng.update_iter(ws, pk, want_mask=(pk.has_mask and need_up))
             if need_up:

@@ -19,8 +19,8 @@ import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("RNC_LIB") or os.path.join(_HERE, "librnc.so")      # RNC_LIB: developer override (variant builds)
-ABI_VERSION = 17
-CONV_NO_HALO, CONV_BASE_OFFSET, CONV_SPLIT_N, CONV_NO_PAIR, CONV_AUX_BLOCKED, CONV_OUT_BLOCKED, CONV_TF32, CONV_WINDOW = 1, 2, 4, 8, 16, 32, 64, 128   # rnc_conv_umma_desc.flags
+ABI_VERSION = 18
+CONV_NO_HALO, CONV_AUX_BLOCKED, CONV_OUT_BLOCKED, CONV_TF32, CONV_WINDOW = 1, 16, 32, 64, 128   # rnc_conv_umma_desc.flags
 
 (EPI_LINEAR, EPI_RELU, EPI_SIGMOID, EPI_GRU_ZR, EPI_GRU_Q, EPI_RELU_FLOW, EPI_RELU_ADD_RELU, EPI_TANH_RELU,
  EPI_FLOW_DELTA) = range(9)
@@ -104,7 +104,6 @@ SIGNATURES = {
     "rnc_instnorm_stats_det": (_i, [_vp, _i, _i, _i, _f, _vp, C.c_size_t, _vp, _vp]),
     "rnc_instnorm_apply": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp, _vp]),
     "rnc_fmap_pyramid": (_i, [_vp, _i, _i, _i, _i, _i, _vp]),
-    "rnc_conv_flow7x7_split_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _i, _vp]),
     "rnc_conv_flow7x7_fwd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _i, _vp]),
     "rnc_flow_head2_fwd": (_i, [_vp, _i, _i, _vp, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "rnc_flow_im2col7_split_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp]),

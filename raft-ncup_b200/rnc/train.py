@@ -118,7 +118,7 @@ def _conv_launch_tf32(eng, x, wt, cout, stride=1, bias=None, dil=1):
         wt = copy.copy(wt)
         wt.bias = _padded_bias(wt.bias, bias)
     eng.uconv(B, Ho, Wo, (hi.data_ptr(), lo.data_ptr()), Cx, Cx, wt, native.EPI_LINEAR, out_f32=out.data_ptr(), ldo_f32=ldo,
-              stride=stride, hin=H, win=W, flags=eng.conv_flags | native.CONV_TF32, dil=dil)
+              stride=stride, hin=H, win=W, flags=native.CONV_TF32, dil=dil)
     return out
 
 

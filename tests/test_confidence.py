@@ -110,9 +110,9 @@ def test_ncup_entry_points_are_declared_bound_and_versioned():
         layout = f.read()
     declared = set(re.findall(r"\b(rnc_\w+)\s*\(", header))
     assert all(n in declared and n in native.SIGNATURES for n in NCUP)
-    assert native.ABI_VERSION == 17 and "(now 17)" in header and "rnc_abi_version(void) { return 17; }" in layout
+    assert native.ABI_VERSION == 18 and "(now 18)" in header and "rnc_abi_version(void) { return 18; }" in layout
     L = native.lib()
-    assert L.rnc_abi_version() == 17
+    assert L.rnc_abi_version() == 18
     for n in REMOVED:
         assert n not in header and n not in native.SIGNATURES and not hasattr(L, n), n
 

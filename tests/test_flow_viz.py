@@ -83,7 +83,7 @@ def test_entry_point_declared_and_bound():
         declared = set(re.findall(r"\b(rnc_\w+)\s*\(", f.read()))
     for n in ("rnc_flow_to_image", "rnc_flow_to_image_workspace_bytes"):
         assert n in declared and n in native.SIGNATURES, n
-    assert native.ABI_VERSION == 17
+    assert native.ABI_VERSION == 18
 
 
 def test_entry_point_rejects_bad_arguments():

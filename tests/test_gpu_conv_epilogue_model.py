@@ -221,9 +221,7 @@ class EpilogueRecorder(Recorder):
         return self.ws.coords1 - self.grid.float()
 
     def blocked_read(self, buf, ld, C, kh, kw):
-        if self.eng.blocked:
-            return unblock(buf, ld, C, kh, kw, self.B, self.H, self.W, self.eng.conv_flags)
-        return buf[:self.M * ld].view(self.M, ld)
+        return unblock(buf, ld, C, kh, kw, self.B, self.H, self.W)
 
     def check_umma(self, st):
         ws, tag = self.ws, f"{self.tag} {st}"
@@ -294,7 +292,6 @@ class EpilogueRecorder(Recorder):
 
 EPILOGUE_STAGES = ("convc1", "convc2", "convf2", "conv", "czr1", "cq1", "czr2", "cq2", "zr1", "q1", "zr2", "q2", "fh1", "m0", "m2")
 PRODUCT_CASES = ([("umma", m, s) for m in ("raft_nc_dbl", "raft") for s in SHAPES]
-                 + [(c, "raft_nc_dbl", s) for c in ("umma-channel-last", "umma-no-halo") for s in ("S1", "S2")]
                  + [("ffma", m, s) for m in ("raft_nc_dbl", "raft") for s in ("S1", "S2")])
 
 
@@ -552,7 +549,7 @@ def test_epilogue_stress_ffma(form):
 
 # ----------------------------------------------------------------------------------------------------------- coverage
 # Every epilogue form (engine, epilogue, aux blocked, out blocked, add, h, res, fp32 out, split out) the forwards launch in
-# test mode (both models, S1, on umma, umma-channel-last and ffma) -> the test that checks it against the model.
+# test mode (both models, S1, on umma and ffma) -> the test that checks it against the model.
 P, ST, SWP = "test_product_epilogues", "test_epilogue_stress", "test_activation_sweep"
 _ERR = "test_gpu_conv_error_model.py (every launch signature, LINEAR fp32)"
 EPILOGUE_COVERAGE = {
@@ -562,11 +559,7 @@ EPILOGUE_COVERAGE = {
     ("umma", 1, False, False, False, False, False, True, False): f"{ST}_umma[relu] (fp32 and split)",
     ("umma", 1, False, False, False, False, False, True, True): f"{ST}_umma[relu] (fp32 and split)",
     ("umma", 3, True, False, True, True, False, False, True): f"{P}[*-umma-*]: zr1, zr2; {ST}_umma[gru-zr-blocked]",
-    ("umma", 3, False, False, True, True, False, False, True):
-        f"{P}[*-umma-channel-last-*]: zr1, zr2; {ST}_umma[gru-zr-channel-last]",
     ("umma", 4, True, False, True, True, False, False, True): f"{P}[*-umma-*]: q1, q2; {ST}_umma[gru-q-blocked]",
-    ("umma", 4, False, False, True, True, False, False, True):
-        f"{P}[*-umma-channel-last-*]: q1, q2; {ST}_umma[gru-q-channel-last]",
     ("umma", 5, False, False, False, False, False, False, True): f"{P}: conv; {ST}_umma[relu-flow]",
     ("umma", 6, False, False, False, False, True, False, True): f"{ST}_umma[relu-add-relu]",
     ("umma", 6, False, False, False, False, True, True, True): f"{ST}_umma[relu-add-relu]",
@@ -589,10 +582,10 @@ def _form(engine, epi, flags, kw):
 
 
 def test_epilogue_coverage_guard(monkeypatch):
-    """The epilogue forms of test-mode forwards of both models at S1 on umma, umma-channel-last and ffma are exactly the
+    """The epilogue forms of test-mode forwards of both models at S1 on umma and ffma are exactly the
     table's: a form added to an engine fails here until it has a check."""
     seen = {}
-    for cfg, env in (("umma", {}), ("umma-channel-last", {"RNC_BLOCKED": "0"}), ("ffma", {"RNC_CONV": "ffma"})):
+    for cfg, env in (("umma", {}), ("ffma", {"RNC_CONV": "ffma"})):
         for name in ("raft_nc_dbl", "raft"):
             with monkeypatch.context() as mp:
                 for k, v in env.items():
@@ -603,9 +596,8 @@ def test_epilogue_coverage_guard(monkeypatch):
                 if eng.mode == "umma":
                     orig = eng.uconv
 
-                    def uconv(B, H, W, in0, c0, ld0, wt, epi, _o=orig, _e=eng, **kw):
-                        f = _e.conv_flags if kw.get("flags") is None else kw["flags"]
-                        seen.setdefault(_form("umma", epi, f, kw), cfg)
+                    def uconv(B, H, W, in0, c0, ld0, wt, epi, _o=orig, **kw):
+                        seen.setdefault(_form("umma", epi, kw.get("flags", 0), kw), cfg)
                         return _o(B, H, W, in0, c0, ld0, wt, epi, **kw)
                     mp.setattr(eng, "uconv", uconv)
                 else:

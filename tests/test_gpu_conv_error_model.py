@@ -49,7 +49,7 @@ def device_split(x):
     return hi, lo
 
 
-def run(ueng, planes, pk, B, H, W, segs=None, stride=1, hin=0, win=0, dil=1, flags=None, split_out=False):
+def run(ueng, planes, pk, B, H, W, segs=None, stride=1, hin=0, win=0, dil=1, flags=0, split_out=False):
     """One uconv of the pack pk on channel-last planes (hi, lo) [rows, Cin] (two input buffers for two segments), LINEAR,
     fp32 output.  H, W: output dims.  Returns the output [B, cout, H, W] (and its split planes, same layout, with
     split_out)."""
@@ -186,7 +186,7 @@ def test_sign_structure(ueng, kind, cin, k):
 
 # ----------------------------------------------------------------------------------------------------------- signatures
 EPI = dict(LINEAR=0, RELU=1, SIGMOID=2, GRU_ZR=3, GRU_Q=4, RELU_FLOW=5, RELU_ADD_RELU=6, TANH_RELU=7, FLOW_DELTA=8)
-NO_HALO, SPLIT_N, WINDOW = 1, 4, 128
+NO_HALO, WINDOW = 1, 128
 MODES = ("tap", "rowhalo", "colhalo")
 
 
@@ -223,7 +223,7 @@ def launch_shape(c0, c1, coutpad, kh, kw, stride, epi, flags, B, H, W):
         bn >>= 1
     if coutpad % bn:
         bn = bn0
-    if coutpad % bn == 0 and epi not in (EPI["RELU_FLOW"], EPI["FLOW_DELTA"]) and not flags & SPLIT_N:
+    if coutpad % bn == 0 and epi not in (EPI["RELU_FLOW"], EPI["FLOW_DELTA"]):
         ksteps = kh * kw * (-(-c0 // 64) + -(-c1 // 64))
         sms = sm_count()
         best, best_cost = bn, np.float32(1e30)
@@ -331,8 +331,7 @@ def record_signatures(monkeypatch, eng, seen):
     orig = eng.uconv
 
     def uconv(B, H, W, in0, c0, ld0, wt, epi, **kw):
-        flags = eng.conv_flags if kw.get("flags") is None else kw["flags"]
-        seen.setdefault(signature(B, H, W, c0, wt, epi, kw.get("c1", 0), kw.get("stride", 1), kw.get("dil", 1), flags),
+        seen.setdefault(signature(B, H, W, c0, wt, epi, kw.get("c1", 0), kw.get("stride", 1), kw.get("dil", 1), kw.get("flags", 0)),
                         (B, H, W))
         return orig(B, H, W, in0, c0, ld0, wt, epi, **kw)
     monkeypatch.setattr(eng, "uconv", uconv)
@@ -430,11 +429,10 @@ def test_layer_signature(ueng, sig):
     judge(f"{sig}", got, s)
 
 
-@pytest.mark.parametrize("flag", ["no-halo", "no-pair"])
+@pytest.mark.parametrize("flag", ["no-halo"])
 @pytest.mark.parametrize("kh,kw,cin,cout", [(3, 3, 128, 256), (1, 5, 256, 128), (5, 1, 256, 256), (3, 3, 64, 64)])
 def test_layer_flags(ueng, flag, kh, kw, cin, cout):
-    """RNC_CONV_NO_HALO (one A tile per tap) and RNC_CONV_NO_PAIR (accepted; single-CTA form) on row-halo, column-halo and
-    per-tap layers; NO_PAIR is bit-identical to the default launch."""
+    """RNC_CONV_NO_HALO (one A tile per tap) on row-halo, column-halo and per-tap layers."""
     from rnc import native
     from rnc.engine_umma import UmmaWeights
     B, H, W = 2, 24, 130
@@ -443,8 +441,5 @@ def test_layer_flags(ueng, flag, kh, kw, cin, cout):
     w = torch.randn(cout, cin, kh, kw, generator=g) / (cin * kh * kw) ** 0.5
     pk = UmmaWeights(w.to(DEV), torch.randn(cout, generator=g).to(DEV), [cin])
     hi, lo = device_split(x)
-    fl = native.CONV_NO_HALO if flag == "no-halo" else native.CONV_NO_PAIR
-    got = run(ueng, (hi, lo), pk, B, H, W, flags=fl)
+    got = run(ueng, (hi, lo), pk, B, H, W, flags=native.CONV_NO_HALO)
     judge(f"{flag} {kh}x{kw} {cin}->{cout}", got, conv_split_ref(x.to(DEV), pk, weight=w))
-    if flag == "no-pair":
-        assert torch.equal(got, run(ueng, (hi, lo), pk, B, H, W, flags=0))

@@ -70,7 +70,7 @@ def test_window_stem_matches_torch(Hin, Win, inst):
     want = torch.zeros(N, Hin, bufs.pitch, 4, dtype=torch.float64)
     want[:, :, 3:3 + Win, :3] = x.permute(0, 2, 3, 1)
     assert (plane.double() - want).abs().max() < 1e-6                  # split halves reproduce the normalised image, zero border
-    win = dict(stride=2, hin=Hin, win=Wo, win_pitch=4 * bufs.pitch, flags=eng.conv_flags | E.CONV_WINDOW)
+    win = dict(stride=2, hin=Hin, win=Wo, win_pitch=4 * bufs.pitch, flags=E.CONV_WINDOW)
     ptrs = (bufs.img_hi.data_ptr(), bufs.img_lo.data_ptr())
     out = torch.zeros(N * Ho * Wo, 64, device=DEV)
     if inst:

@@ -367,7 +367,7 @@ def test_trained_like_layer_by_layer(cfg, sid, monkeypatch):
         with torch.no_grad():
             m(im1, im2, iters=2, flow_init=fi, test_mode=True)
         torch.cuda.synchronize()
-    assert rec.stages == expected_stages(cfg, "raft_nc_dbl", 2, False)
+    assert rec.stages == expected_stages(cfg, "raft_nc_dbl", 2)
     print(f"[{sid} {cfg} trained-like] worst err/bound: " + ", ".join(f"{k} {v:.2f}" for k, v in rec.worst.items()))
 
 

@@ -20,12 +20,9 @@ from test_product_shapes import CFG5_CONV_SIGNATURES, SHAPES, TOL, cl, compare, 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 
-# developer switches of the tensor-core engine (rnc/engine_umma.py), and the exact fp32 engine
+# the tensor-core engine, with its exact fp32 lookup, and the exact fp32 engine
 CONFIGS = {
     "umma": {},
-    "umma-no-halo": {"RNC_CONV_FLAGS": "1"},
-    "umma-channel-last": {"RNC_BLOCKED": "0"},
-    "umma-convf1-ffma": {"RNC_CONVF1": "ffma"},
     "umma-lookup-ffma": {"RNC_LOOKUP": "ffma"},
     "ffma": {"RNC_CONV": "ffma"},
 }
@@ -33,7 +30,7 @@ CONFIGS = {
 # librnc entry points that complete a checked stage
 NATIVE_STAGES = {
     "rnc_corr_lookup_umma_fwd": "lookup", "rnc_corr_lookup_split_fwd": "lookup", "rnc_corr_lookup_fwd": "lookup",
-    "rnc_flow_im2col7_split_fwd": "im2col", "rnc_conv_flow7x7_split_fwd": "convf1", "rnc_conv_flow7x7_fwd": "convf1",
+    "rnc_flow_im2col7_split_fwd": "im2col", "rnc_conv_flow7x7_fwd": "convf1",
     "rnc_flow_tap_gather_fwd": "gather", "rnc_flow_head2_fwd": "flow_head2", "rnc_coords_init": "coords_init",
     "rnc_flow_x2_fwd": "flow_x2", "rnc_ncup_guidance_fwd": "guidance", "rnc_ncup_guidance_split_fwd": "guidance",
     "rnc_conf_head_fwd": "conf",
@@ -44,17 +41,14 @@ PACKED_STAGES = {"convc1": "convc1", "convc2": "convc2", "convf1_mm": "convf1", 
                  "q2": "q2", "fh1": "fh1", "fh2": "fh2", "m0": "m0", "m2": "m2"}
 
 
-def expected_stages(engine, model, iters, convf1_fork):
+def expected_stages(engine, model, iters):
     """The stage order of one test-mode forward: a change to the engine's call sequence fails here, loudly, instead of
     comparing the wrong pairs."""
     umma = engine == "umma"
     seq = ["encoders", "pyramid"] + ([] if umma else ["context"]) + ["coords_init"]
     for it in range(iters):
         last = it == iters - 1
-        seq += (["convf1"] if convf1_fork else []) + ["lookup", "convc1", "convc2"]
-        if not convf1_fork:
-            seq += ["im2col", "convf1"] if umma else ["convf1"]
-        seq += ["convf2", "conv"]
+        seq += ["lookup", "convc1", "convc2"] + (["im2col", "convf1"] if umma else ["convf1"]) + ["convf2", "conv"]
         if umma and it == 0:
             seq += ["czr1", "cq1", "czr2", "cq2"]                  # hoisted context addends: once per forward
         seq += ["zr1", "q1", "zr2", "q2", "fh1"] + (["fh2", "gather"] if umma else ["flow_head2"])
@@ -169,12 +163,9 @@ class Recorder:
         return self.ws.h if self.umma else self.ws.hx[:, :128]
 
     def zgate(self, kh, kw):
-        ws, M = self.ws, self.M
         if not self.umma:
-            return self.nchw(ws.z, 0, 128)
-        if self.eng.blocked:
-            return self.nchw(unblock(ws.z, 128, 128, kh, kw, self.B, self.H, self.W, self.eng.conv_flags), 0, 128)
-        return self.nchw(ws.z[:M * 128].view(M, 128), 0, 128)
+            return self.nchw(self.ws.z, 0, 128)
+        return self.nchw(unblock(self.ws.z, 128, 128, kh, kw, self.B, self.H, self.W), 0, 128)
 
     def conv(self, name, x, w=None, b=None):
         mod = self.m.get_submodule(name)
@@ -200,12 +191,12 @@ class Recorder:
             self.stages.append(st)
         if not self.check:
             return
-        ws, B, H, W, M = self.ws, self.B, self.H, self.W, self.M
+        ws, B, H, W = self.ws, self.B, self.H, self.W
         p = "update_block."
         if when == "before":
             if st in ("lookup", "gather", "flow_head2"):
                 self.pending[st] = ws.coords1.clone()
-            # the flow convf1 sees: at the im2col of the 1x1 form, else at the 7x7 kernel (a forked one: on the side stream)
+            # the flow convf1 sees: at the im2col of the 1x1 form, else at the 7x7 kernel
             if st == "im2col" or (st == "convf1" and self.stages[-2:-1] != ["im2col"]):
                 self.pending["flow"] = ws.coords1.double() - self.grid
             if st in ("q1", "q2"):
@@ -248,7 +239,7 @@ class Recorder:
             ref = torch.cat([u, torch.zeros(B, 30, H, W, dtype=u.dtype, device=DEV)], 1)
             self.cmp(st, self.nchw(self.val(ws.fcol), 0, 128), ref, TOL["move"])
         elif st == "convf1":
-            self.pending["f1_flow"] = self.pending.pop("flow")      # checked at convf2, after a forked convf1 is joined
+            self.pending["f1_flow"] = self.pending.pop("flow")      # checked at convf2
         elif st == "convf2":
             ref_f1 = F.relu(self.conv(p + "encoder.convf1", self.pending.pop("f1_flow")))
             f1 = self.nchw(self.val(ws.f1), 0, 128)
@@ -268,10 +259,7 @@ class Recorder:
             buf = getattr(ws, st)
             ld = 256 if st.startswith("czr") else 128                 # the packs' coutpad
             kh, kw = (1, 5) if tag == "1" else (5, 1)
-            if self.eng.blocked:
-                got = unblock(buf, ld, ld, kh, kw, B, H, W, self.eng.conv_flags)
-            else:
-                got = buf[:M * ld].view(M, ld)
+            got = unblock(buf, ld, ld, kh, kw, B, H, W)
             self.cmp(st, self.nchw(got, 0, ld), ref, TOL["conv"])
         elif st in ("zr1", "zr2"):
             tag = st[-1]
@@ -412,24 +400,20 @@ def run_forward(monkeypatch, cfg, model_name, sid, check=True, seed=1, iters=2):
 
 CASES = ([("umma", mdl, s) for mdl in ("raft_nc_dbl", "raft") for s in SHAPES]
          + [("ffma", "raft_nc_dbl", s) for s in SHAPES] + [("ffma", "raft", "S1")]
-         + [(c, "raft_nc_dbl", s) for c in ("umma-no-halo", "umma-channel-last", "umma-convf1-ffma", "umma-lookup-ffma")
-            for s in ("S1", "S2")])
+         + [("umma-lookup-ffma", "raft_nc_dbl", s) for s in ("S1", "S2")])
 
 
 @pytest.mark.parametrize("cfg,model_name,sid", CASES, ids=[f"{s}-{c}-{m}" for c, m, s in CASES])
 def test_update_iteration_layer_by_layer(cfg, model_name, sid, monkeypatch):
     """Two iterations of a test-mode forward, every stage against its fp64 reference layer (teacher forcing): encoders and
-    pyramid, lookup, convc1, convc2, convf1 (im2col + 1x1, or the forked 7x7), convf2, conv + flow append, the hoisted context
-    addends, z / r*h / h of both GRU halves (z read back from the tile-blocked layout), fh1, fh2 in tap form + coords1 += delta,
-    the mask head, and the upsampler stages.  The second iteration reuses the hoisted addends and joins the forked convf1."""
+    pyramid, lookup, convc1, convc2, convf1 (im2col + 1x1, or the 7x7 of the exact engine), convf2, conv + flow append, the
+    hoisted context addends, z / r*h / h of both GRU halves (z read back from the tile-blocked layout), fh1, fh2 in tap form +
+    coords1 += delta, the mask head, and the upsampler stages.  The second iteration reuses the hoisted addends."""
     import time
     t0 = time.time()
     rec, m, eng, _, _ = run_forward(monkeypatch, cfg, model_name, sid)
     engine = "umma" if cfg.startswith("umma") else "ffma"
-    fork = engine == "umma" and eng.fork_convf1
-    assert rec.stages == expected_stages(engine, model_name, 2, fork)
-    if engine == "umma":
-        assert eng.blocked == ("RNC_BLOCKED" not in CONFIGS[cfg]) and eng.conv_flags == int(CONFIGS[cfg].get("RNC_CONV_FLAGS", 0))
+    assert rec.stages == expected_stages(engine, model_name, 2)
     if sid == "S1" and engine == "umma" and eng.lookup_mode == "umma":
         assert rec.fallback and rec.fallback > 0, "the motion boundary must send some lookup tiles to the exact fallback"
     print(f"[{sid} {cfg} {model_name}] {len(rec.stages)} stages checked in {time.time() - t0:.1f} s; worst errors: "
@@ -448,7 +432,7 @@ def test_second_forward_and_graph_replay(sid, monkeypatch):
         rec.images(im1, im2, fi)
         with torch.no_grad():
             lo_b, up_b = m(im1, im2, iters=2, flow_init=fi, test_mode=True)
-    assert rec.stages == expected_stages("umma", "raft_nc_dbl", 2, False)
+    assert rec.stages == expected_stages("umma", "raft_nc_dbl", 2)
     monkeypatch.setenv("RNC_GRAPH", "1")
     a1, a2, afi = stimulus(B, H8, W8, seed=1)
     with torch.no_grad():
@@ -485,7 +469,6 @@ COVERAGE = {
     "rnc_corr_lookup_split_fwd": f"{LAYERS}[*-umma-lookup-ffma-*]: 'lookup (exact)'",
     "rnc_corr_lookup_fwd": f"{LAYERS}[*-ffma-*]: 'lookup (exact)'",
     "rnc_flow_im2col7_split_fwd": f"{LAYERS}: 'im2col'",
-    "rnc_conv_flow7x7_split_fwd": f"{LAYERS}[*-umma-convf1-ffma-*]: 'convf1'",
     "rnc_conv_flow7x7_fwd": f"{LAYERS}[*-ffma-*]: 'convf1'",
     "rnc_conv2d_cl_fwd": f"{LAYERS}[*-ffma-*]: every exact-engine layer",
     "rnc_flow_tap_gather_fwd": f"{LAYERS}: 'fh2 + coords1 += delta'",
@@ -500,7 +483,7 @@ COVERAGE = {
     "rnc_convex_upsample_fwd": f"{LAYERS}[*-raft]: 'convex'",
 }
 QUERIES = {k for k, v in COVERAGE.items() if v.startswith("size query")}
-SWITCH_ONLY = {"rnc_corr_lookup_split_fwd", "rnc_conv_flow7x7_split_fwd", "rnc_instnorm_stats_det"}
+SWITCH_ONLY = {"rnc_corr_lookup_split_fwd", "rnc_instnorm_stats_det"}
 
 
 def test_coverage_guard(monkeypatch):

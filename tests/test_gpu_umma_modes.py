@@ -22,8 +22,6 @@ def ueng():
 def run_conv(ueng, x, w, b, stride=1, flags=0, epi="none", res=None):
     from rnc import native
     from rnc.engine_umma import SplitBuf, UmmaWeights
-    import os
-    flags |= int(os.environ.get("RNC_CONV_FLAGS", "0"))
     B, cin, Hin, Win = x.shape
     cout, _, kh, kw = w.shape
     H, W = (Hin + stride - 1) // stride, (Win + stride - 1) // stride

@@ -161,7 +161,7 @@ def test_flag_and_epilogue_constants_match_header():
     from rnc import native
     hdr = open(os.path.join(ROOT, "include", "rnc.h")).read()
     flags = {m.group(1): int(m.group(2)) for m in re.finditer(r"#define\s+RNC_CONV_([A-Z0-9_]+)\s+(\d+)", hdr)}
-    for name in ("NO_HALO", "SPLIT_N", "NO_PAIR", "AUX_BLOCKED", "OUT_BLOCKED", "TF32", "WINDOW"):
+    for name in ("NO_HALO", "AUX_BLOCKED", "OUT_BLOCKED", "TF32", "WINDOW"):
         assert getattr(native, "CONV_" + name) == flags[name], name
     epis = {m.group(1): int(m.group(2)) for m in re.finditer(r"RNC_EPI_([A-Z_]+)\s*=\s*(\d+)", hdr)}
     for name in ("LINEAR", "RELU", "SIGMOID", "GRU_ZR", "GRU_Q", "RELU_FLOW", "RELU_ADD_RELU", "TANH_RELU", "FLOW_DELTA"):

@@ -17,8 +17,8 @@ def epe(a, b):
 im1, im2 = frames(8, 436, 1024)
 p1, p2 = InputPadder(im1.shape, "sintel").pad(im1, im2)
 p1, p2 = p1.cuda(), p2.cuda()
-for env in ({}, {"RNC_LOOKUP": "ffma"}, {"RNC_CONV_PAIR": "0"}, {"RNC_ENCODER": "cudnn"}, {"RNC_CONV": "ffma"}):
-    for k in ("RNC_LOOKUP", "RNC_CONV", "RNC_CONV_PAIR", "RNC_ENCODER"):
+for env in ({}, {"RNC_LOOKUP": "ffma"}, {"RNC_ENCODER": "cudnn"}, {"RNC_CONV": "ffma"}):
+    for k in ("RNC_LOOKUP", "RNC_CONV", "RNC_ENCODER"):
         os.environ.pop(k, None)
     os.environ.update(env)
     m = build_model("raft_nc_dbl").cuda()

@@ -6,8 +6,6 @@ Records every uconv call of the second update-block iteration of a B x 440x1024 
 epilogues), then replays each call back to back and times it with CUDA events after a warm-up:
   ms          the layer as the benchmark runs it
   ms_nob      the same launches with RNC_CONV_PROBE_NOB=1 (weights loaded once per ring fill: the weight stream's cost)
-  ms_nopair   the same launches with flag RNC_CONV_NO_PAIR (the single-CTA form; the sm_90 kernel has only that form,
-              so this column repeats `ms` within noise)
 and the useful / tensor-issued FLOP computed from the shapes (three fp16 MMAs per product, padded to whole tiles, K blocks
 and column tiles).  `peak_frac` is the issued rate over the dense fp16 peak (989 TFLOP/s at 1830 MHz, data sheet) scaled
 to the SM clock sampled during the run.  Then tools/step_breakdown.py splits one step.  The last stdout line is JSON.
@@ -24,7 +22,6 @@ for p in (ROOT, os.path.join(ROOT, "raft-ncup_b200")):
     sys.path.insert(0, p)
 
 PEAK_FP16_DENSE, PEAK_MHZ = 989e12, 1830.0
-NO_PAIR = 8
 
 
 def measure(batch, launches):
@@ -69,25 +66,22 @@ def measure(batch, launches):
     sampler.start()
     for a, k in calls:
         B, H, W, wt = a[0], a[1], a[2], a[6]
-        flags = k.get("flags")
-        flags = eng.conv_flags if flags is None else flags
+        flags = k.get("flags", 0)
         c_in = a[4] + k.get("c1", 0)
         ntiles = L.rnc_conv_umma_tiles(wt.kh, wt.kw, k.get("stride", 1), B, H, W, flags)
         row = {"layer": state["names"].get(id(wt), "?"), "epilogue": a[7], "flags": flags, "k": f"{wt.kh}x{wt.kw}",
                "cin": c_in, "cout": wt.cout, "coutpad": wt.coutpad,
                "gflop_useful": 2.0 * B * H * W * wt.cout * wt.kh * wt.kw * c_in / 1e9,
                "gflop_issued": 3 * 2.0 * ntiles * 128 * wt.coutpad * wt.ktot / 1e9}
-        for key, fl in (("ms", flags), ("ms_nopair", flags | NO_PAIR)):
-            kk = dict(k, flags=fl)
-            for _ in range(5):
-                uconv(*a, **kk)
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(launches):
-                uconv(*a, **kk)
-            e1.record()
-            torch.cuda.synchronize()
-            row[key] = e0.elapsed_time(e1) / launches
+        for _ in range(5):
+            uconv(*a, **k)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(launches):
+            uconv(*a, **k)
+        e1.record()
+        torch.cuda.synchronize()
+        row["ms"] = e0.elapsed_time(e1) / launches
         rows.append(row)
     clocks = sampler.stop()
     return {"rows": rows, "clocks": clocks}
@@ -147,13 +141,13 @@ def main():
     for r, rn in zip(rows, nob["rows"]):
         r["ms_nob"] = rn["ms"]
         r["peak_frac"] = r["gflop_issued"] * 1e9 / (r["ms"] * 1e-3) / peak
-    tot = {k: sum(r[k] for r in rows) for k in ("ms", "ms_nob", "ms_nopair", "gflop_useful", "gflop_issued")}
-    hdr = f"{'layer':10s} {'k':>4s} {'cin':>4s} {'cout':>4s} {'epi':>3s} {'ms':>7s} {'ms_nob':>7s} {'nopair':>7s} {'GF use':>7s} {'GF iss':>7s} {'peak':>5s}"
+    tot = {k: sum(r[k] for r in rows) for k in ("ms", "ms_nob", "gflop_useful", "gflop_issued")}
+    hdr = f"{'layer':10s} {'k':>4s} {'cin':>4s} {'cout':>4s} {'epi':>3s} {'ms':>7s} {'ms_nob':>7s} {'GF use':>7s} {'GF iss':>7s} {'peak':>5s}"
     print(hdr, file=sys.stderr)
     for r in rows:
         print(f"{r['layer']:10s} {r['k']:>4s} {r['cin']:4d} {r['cout']:4d} {r['epilogue']:3d} {r['ms']:7.3f} {r['ms_nob']:7.3f} "
-              f"{r['ms_nopair']:7.3f} {r['gflop_useful']:7.1f} {r['gflop_issued']:7.1f} {r['peak_frac']:5.2f}", file=sys.stderr)
-    print(f"{'total':10s} {'':>4s} {'':>4s} {'':>4s} {'':>3s} {tot['ms']:7.3f} {tot['ms_nob']:7.3f} {tot['ms_nopair']:7.3f} "
+              f"{r['gflop_useful']:7.1f} {r['gflop_issued']:7.1f} {r['peak_frac']:5.2f}", file=sys.stderr)
+    print(f"{'total':10s} {'':>4s} {'':>4s} {'':>4s} {'':>3s} {tot['ms']:7.3f} {tot['ms_nob']:7.3f} "
           f"{tot['gflop_useful']:7.1f} {tot['gflop_issued']:7.1f}", file=sys.stderr)
     res = {"card": card(), "clocks": base["clocks"], "batch": args.batch, "shape": [55, 128], "layers": rows, "total": tot,
            "peak_tflops_at_clock": peak / 1e12}

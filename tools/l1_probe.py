@@ -19,8 +19,6 @@ variants = {
     "linear f32": dict(epi=E.EPI_LINEAR, out_f32=out32.data_ptr(), ldo_f32=64),
     "relu split": dict(epi=E.EPI_RELU, out_split=outs.ptrs(), ldo_split=64),
     "relu split, no halo": dict(epi=E.EPI_RELU, out_split=outs.ptrs(), ldo_split=64, flags=E.CONV_NO_HALO),
-    "relu split, no pair": dict(epi=E.EPI_RELU, out_split=outs.ptrs(), ldo_split=64, flags=E.CONV_NO_PAIR),
-    "relu split, streamed weights": dict(epi=E.EPI_RELU, out_split=outs.ptrs(), ldo_split=64, flags=8 << 12),
 }
 for name, kw in variants.items():
     epi = kw.pop("epi")
