@@ -564,6 +564,46 @@ int rnc_fb_consistency(const float* flow_fw, long long fb, long long fc, long lo
                        float alpha2, unsigned char* occ_fw, unsigned char* occ_bw, float* err_fw, float* err_bw,
                        void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V5  per-region validation metrics: Sintel's matched / unmatched, boundary-distance and speed regions, KITTI 2015's
+ * background / foreground over all and non-occluded pixels (definitions: rnc/metrics.py, DESIGN §3.14).
+ *
+ * rnc_boundary_dist2: the exact squared Euclidean distance, in pixels, of every pixel to the nearest occlusion-boundary pixel
+ * of its image.  A boundary pixel has a 4-neighbour inside the image whose label (occluded where occ >= 0.5) differs from its
+ * own; pixels on both sides of the boundary count.
+ *   occ : fp32, pixel (b, y, x) at occ[b*ob + y*oy + x*ox]; 4-byte aligned
+ *   d2  : int32 [B][H][W] contiguous; RNC_DIST2_NONE in an image without a boundary pixel
+ * A column pass, then the lower envelope of parabolas along each row, in integers only (intersections compared by
+ * cross-multiplying in int64): the result is exact.  Two launches, no atomics, no host synchronisation.  RNC_ERR_BAD_SHAPE
+ * unless 1 <= H, W <= 4096 and 1 <= B <= 65535.  Bad arguments return before any launch.
+ *
+ * rnc_region_metrics: per image and per cell, the five counts and the fp64 EPE sum of rnc_flow_metrics (each pixel rounded
+ * as it rounds it, valid where valid >= 0.5, NULL: every pixel is valid).  A cell is one joint label of a pixel:
+ *   RNC_REGIONS_SINTEL (32 cells): 16*occluded + 4*d + s, occluded where mask (occ) >= 0.5; d from d2 (rnc_boundary_dist2's
+ *     output, int32 [B][H][W] contiguous): 0 for d2 < 100, 1 for < 3600, 2 for < 19600, else 3; s from mag = |gt|: 0 for
+ *     mag < 10, 1 for < 40, 2 for >= 40, 3 for NaN.  fg must be NULL.
+ *   RNC_REGIONS_KITTI (4 cells): 2*(mask (noc) < 0.5) + (fg >= 0.5); fg NULL: every pixel is background.  d2 must be NULL.
+ *   mask, fg   : fp32 through element strides (mb..mx, qb..qx), as valid; 4-byte aligned
+ *   counts     : int64 [B][cells][5] (valid, epe < 1, < 3, < 5, KITTI outliers); 8-byte aligned
+ *   epe_sum    : fp64 [B][cells]; 8-byte aligned
+ *   workspace  : rnc_region_metrics_workspace_bytes(kind, B, H, W) bytes, 16-byte aligned, no zeroing needed
+ * Two launches, no host synchronisation, no floating-point atomics; the sums are added in a fixed order that depends only on
+ * H*W and the cell count, so an image's results are bit for bit the same whatever B, its position in the batch or the GPU.
+ * RNC_ERR_UNSUPPORTED for an unknown kind.  Bad arguments return before any launch. */
+#define RNC_DIST2_NONE 2147483647
+#define RNC_REGIONS_SINTEL 0
+#define RNC_REGIONS_KITTI 1
+#define RNC_REGION_CELLS_SINTEL 32
+#define RNC_REGION_CELLS_KITTI 4
+int rnc_boundary_dist2(const float* occ, long long ob, long long oy, long long ox, int B, int H, int W, int* d2,
+                       void* stream);
+size_t rnc_region_metrics_workspace_bytes(int kind, int B, int H, int W);   /* 0 for a bad kind or shape */
+int rnc_region_metrics(int kind, const float* flow, long long fb, long long fc, long long fy, long long fx, const float* gt,
+                       long long gb, long long gc, long long gy, long long gx, const float* valid, long long vb, long long vy,
+                       long long vx, const float* mask, long long mb, long long my, long long mx, const int* d2,
+                       const float* fg, long long qb, long long qy, long long qx, int B, int H, int W, long long* counts,
+                       double* epe_sum, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -2,15 +2,14 @@
 // against their ground truth: per image, the number of valid pixels, of EPE < 1, < 3 and < 5, of KITTI outliers, and the fp64
 // sum of the valid pixels' EPE.
 //
-// Each pixel is what torch computes in float32 on the host: dx = flow - gt, epe = sqrt(dx*dx + dy*dy), mag the same from gt,
-// valid >= 0.5, outlier = epe > 3 & epe / mag > 0.05 (a Python float compared with a float32 tensor is rounded to float32).
-// The *_rn intrinsics keep nvcc from contracting any of it into an FMA, and IEEE division gives x/0 = inf and 0/0 = NaN, so
-// a zero-magnitude ground truth, NaN and inf count as the torch comparisons count them.
+// Each pixel is what torch computes in float32 on the host (pixel_metrics.cuh, shared with rnc_region_metrics), valid where
+// valid >= 0.5.
 //
 // Two kernels, no host synchronisation: CTA (x, b) of the first writes the partials of its 2048 pixels of image b to the
 // workspace, and the second adds each image's partials in a fixed order (a warp per image: lane-strided sums, then a fixed
 // shuffle tree).  The grid's x extent depends only on H*W, so an image's sums depend only on that image: not on B, on its
 // position in the batch or on which GPU ran it.
+#include "pixel_metrics.cuh"
 #include "rnc_common.cuh"
 
 namespace rnc {
@@ -47,16 +46,13 @@ __global__ void __launch_bounds__(kMetThreads) metrics_part_kernel(MetricsArgs a
     if (a.valid && !(a.valid[b * a.vb + y * a.vy + x * a.vx] >= 0.5f)) continue;
     const float* f = a.flow + b * a.fb + y * a.fy + x * a.fx;
     const float* g = a.gt + b * a.gb + y * a.gy + x * a.gx;
-    const float g0 = g[0], g1 = g[a.gc];
-    const float dx = __fsub_rn(f[0], g0), dy = __fsub_rn(f[a.fc], g1);
-    const float epe = __fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));
-    const float mag = __fsqrt_rn(__fadd_rn(__fmul_rn(g0, g0), __fmul_rn(g1, g1)));
+    const PixelMetrics m = pixel_metrics(f[0], f[a.fc], g[0], g[a.gc]);
     n[0] += 1;
-    n[1] += epe < 1.0f;
-    n[2] += epe < 3.0f;
-    n[3] += epe < 5.0f;
-    n[4] += (epe > 3.0f) & (__fdiv_rn(epe, mag) > 0.05f);
-    sum += static_cast<double>(epe);
+    n[1] += m.epe < 1.0f;
+    n[2] += m.epe < 3.0f;
+    n[3] += m.epe < 5.0f;
+    n[4] += m.outlier;
+    sum += static_cast<double>(m.epe);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);

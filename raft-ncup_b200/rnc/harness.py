@@ -18,11 +18,13 @@ from utils import frame_utils
 from utils.utils import InputPadder, forward_interpolate
 
 
-def _shape_batches(samples, batch_size):
-    """Consecutive samples of one frame size, batch_size at a time; a new size (KITTI's vary) closes the batch."""
+def _shape_batches(samples, batch_size, regions=False):
+    """Consecutive samples of one frame size, batch_size at a time; a new size (KITTI's vary) closes the batch.  With
+    regions, samples are _region_sample's 5-tuples and stay as they are."""
     batch = []
     for s in samples:
-        s = tuple(s) if len(s) == 4 else (s[0], s[1], s[2], None)
+        if not regions:
+            s = tuple(s) if len(s) == 4 else (s[0], s[1], s[2], None)
         if batch and batch[0][0].shape != s[0].shape:
             yield batch
             batch = []
@@ -34,30 +36,72 @@ def _shape_batches(samples, batch_size):
         yield batch
 
 
-_Staged = namedtuple("_Staged", "im1 im2 gt valid sparse ready")
+_Staged = namedtuple("_Staged", "im1 im2 gt valid sparse ready masks regions")
+# a sample's region masks, checked: its index in the split, "sintel" or "kitti", and the masks ({"occ"} or {"noc"[, "fg"]})
+_Regions = namedtuple("_Regions", "index kind masks")
+_REGION_KEYS = {frozenset({"occ"}): "sintel", frozenset({"noc"}): "kitti", frozenset({"noc", "fg"}): "kitti"}
 
 
-def _stage(batch, dev, copy_stream):
+def _region_samples(samples, world, rank):
+    """validate(regions=True)'s samples (this rank's share of the split), each checked and returned as (image1, image2,
+    flow_gt, valid, _Regions).  ValueError naming the sample's index in the split when it has no fifth item, the item is not
+    one of the dicts {"occ"}, {"noc"}, {"noc", "fg"}, a mask is not [H,W] of the frame's size, or it is of the other style
+    than the samples before it."""
+    first = None
+    for k, s in enumerate(samples):
+        i = rank + world * k
+        if len(s) != 5:
+            raise ValueError(f"validate(regions=True): sample {i} has {len(s)} items; expected (image1, image2, flow_gt, valid, "
+                             f"masks) with masks {{'occ': mask}} or {{'noc': mask[, 'fg': mask]}}")
+        masks = s[4]
+        kind = _REGION_KEYS.get(frozenset(masks)) if isinstance(masks, dict) else None
+        if kind is None:
+            raise ValueError(f"validate(regions=True): sample {i}'s fifth item must be {{'occ': mask}} or {{'noc': mask[, 'fg': "
+                             f"mask]}}, got {sorted(masks) if isinstance(masks, dict) else type(masks).__name__}")
+        hw = tuple(s[0].shape[-2:])
+        for name, m in masks.items():
+            if tuple(m.shape) != hw:
+                raise ValueError(f"validate(regions=True): sample {i}'s {name} mask is {tuple(m.shape)}, expected [H,W] = {hw}")
+        if first is None:
+            first = (i, kind)
+        elif kind != first[1]:
+            raise ValueError(f"validate(regions=True): sample {i} is {kind.capitalize()}-style but sample {first[0]} is "
+                             f"{first[1].capitalize()}-style; one split is one or the other")
+        yield (s[0], s[1], s[2], s[3], _Regions(i, kind, masks))
+
+
+def _stage(batch, dev, copy_stream, regions=False):
     """Enqueue the upload of a batch: each field stacked into a pinned host tensor and copied without blocking on copy_stream,
     so that it overlaps the forward running on the compute stream.  valid is None when no sample has one; a sample without
-    one among samples with one counts every pixel valid."""
+    one among samples with one counts every pixel valid.  With regions, the region masks travel the same way: occ, or noc
+    and fg (fg when a sample of the batch has one; a sample without counts every pixel as background)."""
     sparse = [s[3] is not None for s in batch]
     H, W = batch[0][0].shape[-2:]
     fields = [[s[0] for s in batch], [s[1] for s in batch], [s[2].float() for s in batch]]
     if any(sparse):
         fields.append([torch.ones(H, W) if s[3] is None else s[3].float() for s in batch])
+    names = []
+    if regions:
+        for name in ("occ", "noc", "fg"):
+            if any(name in s[4].masks for s in batch):
+                names.append(name)
+                fields.append([s[4].masks[name].float() if name in s[4].masks else torch.zeros(H, W) for s in batch])
+    nv = 4 if any(sparse) else 3
+    meta = [s[4] for s in batch] if regions else None
     if dev.type != "cuda":
         host = [torch.stack(f).to(dev) for f in fields]
-        return _Staged(*host[:3], host[3] if len(host) == 4 else None, sparse, None)
-    out = []
-    for f in fields:
-        pinned = torch.empty((len(f),) + tuple(f[0].shape), dtype=f[0].dtype, pin_memory=True)
-        torch.stack(f, out=pinned)
-        with torch.cuda.stream(copy_stream):          # allocated on copy_stream: its memory is never in use by older work
-            out.append(pinned.to(dev, non_blocking=True))
-    ready = torch.cuda.Event()
-    ready.record(copy_stream)
-    return _Staged(*out[:3], out[3] if len(out) == 4 else None, sparse, ready)
+    else:
+        host = []
+        for f in fields:
+            pinned = torch.empty((len(f),) + tuple(f[0].shape), dtype=f[0].dtype, pin_memory=True)
+            torch.stack(f, out=pinned)
+            with torch.cuda.stream(copy_stream):          # allocated on copy_stream: its memory is never in use by older work
+                host.append(pinned.to(dev, non_blocking=True))
+    ready = None
+    if dev.type == "cuda":
+        ready = torch.cuda.Event()
+        ready.record(copy_stream)
+    return _Staged(*host[:3], host[3] if nv == 4 else None, sparse, ready, dict(zip(names, host[nv:])), meta)
 
 
 def bidirectional_flow(model, image1, image2, iters=32, flow_init=None, mode="sintel", return_confidence=False, alpha1=0.01,
@@ -89,7 +133,8 @@ def bidirectional_flow(model, image1, image2, iters=32, flow_init=None, mode="si
 
 
 @torch.no_grad()
-def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda", confidence=False, consistency=False):
+def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda", confidence=False, consistency=False,
+             regions=False):
     """samples: iterable of (image1 [3,H,W], image2 [3,H,W], flow_gt [2,H,W], valid [H,W] or None).
     Returns the metrics validate_sintel / validate_kitti print: EPE, 1px/3px/5px, and KITTI F1 when `valid` is given
     (rnc.metrics.summarize: Sintel-style pools every pixel, KITTI-style averages the per-image mean EPE).
@@ -110,29 +155,43 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
     rnc.metrics.fb_consistency.  The dict gains "fb_sparsification", "fb_ause" and "ideal" (which depends on the EPE only,
     so one serves both scores).  The forward rows of the bidirectional pass are the flows of model(image1, image2), so the
     other keys are those of consistency=False: bit for bit wherever the forward itself repeats bit for bit (the exact lookup
-    under torch.use_deterministic_algorithms), and within its run-to-run spread otherwise."""
+    under torch.use_deterministic_algorithms), and within its run-to-run spread otherwise.
+
+    regions=True also gives the per-region errors the Sintel and KITTI 2015 benchmarks publish (the definitions are in
+    rnc.metrics).  Each sample is then (image1, image2, flow_gt, valid or None, masks), masks {"occ": [H,W]} for a Sintel-style
+    split or {"noc": [H,W]} / {"noc": [H,W], "fg": [H,W]} for a KITTI-style one.  The masks travel with valid; per batch
+    rnc.metrics.region_partials (rnc_boundary_dist2 and rnc_region_metrics on CUDA) takes per-image partials that stay on the
+    device with the others and are gathered with them.  The dict gains rnc.metrics.summarize_regions' keys: epe_matched,
+    epe_unmatched, epe_d0-10, epe_d10-60, epe_d60-140, epe_s0-10, epe_s10-40, epe_s40+ (Sintel-style) or fl_all, fl_all_noc
+    and, when every sample has fg, fl_bg, fl_fg, fl_bg_noc, fl_fg_noc (KITTI-style), and region_pixels.  With consistency=True
+    and a Sintel-style split it also gains occ_precision, occ_recall and occ_f1, which score fb_consistency's occlusion mask
+    of the forward flow (rnc.metrics.occlusion_counts) against occ over the valid pixels.  The other keys are those of
+    regions=False, bit for bit.  ValueError, naming the sample's index, for a sample without masks, with a mask of the wrong
+    shape, or of the other style than the rest of the split."""
     from .dist import gather_strided, strided_items, world_rank
-    from .metrics import (FRACTIONS, Partials, SparsPartials, cat, confidence_score, fb_consistency, flow_metrics, sparsification,
-                          summarize, summarize_sparsification)
+    from .metrics import (FRACTIONS, Partials, RegionPartials, SparsPartials, cat, cat_regions, confidence_score, fb_consistency,
+                          flow_metrics, occlusion_counts, region_partials, sparsification, summarize, summarize_occlusion,
+                          summarize_regions, summarize_sparsification)
     model.eval()
     world, rank = world_rank()
     dev = torch.device(device)
     if dev.type == "cuda" and dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     copy_stream = torch.cuda.Stream(dev) if dev.type == "cuda" else None
-    parts, sparse, sparts, fparts = [], [], [], []
-    batches = _shape_batches(strided_items(samples, world, rank), batch_size)
+    parts, sparse, sparts, fparts, rparts, oparts, rmeta = [], [], [], [], [], [], []
+    items = strided_items(samples, world, rank)
+    batches = _shape_batches(_region_samples(items, world, rank) if regions else items, batch_size, regions)
 
     def stage_next():
         b = next(batches, None)
-        return None if b is None else _stage(b, dev, copy_stream)
+        return None if b is None else _stage(b, dev, copy_stream, regions)
     nxt = stage_next()
     while nxt is not None:
         cur = nxt
         if cur.ready is not None:
             compute = torch.cuda.current_stream(dev)
             compute.wait_event(cur.ready)
-            for t in cur[:4]:
+            for t in (*cur[:4], *cur.masks.values()):
                 if t is not None:
                     t.record_stream(compute)
         padder = InputPadder(cur.im1.shape, mode=mode)
@@ -151,10 +210,16 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
         if confidence:
             sparts.append(sparsification(flow, cur.gt, cur.valid, confidence_score(padder.unpad(conf))))
             del conf
+        if regions:
+            rp = region_partials(flow, cur.gt, cur.valid, **cur.masks)
+            rparts.append(rp._replace(fg=torch.tensor(["fg" in r.masks for r in cur.regions])))
+            rmeta += cur.regions
         if consistency:
-            fb_err = fb_consistency(flow, flow_bw)[2]
+            occ_fw, _, fb_err, _ = fb_consistency(flow, flow_bw)
             fparts.append(sparsification(flow, cur.gt, cur.valid, -fb_err))
-            del flow_bw, fb_err
+            if regions and "occ" in cur.masks:
+                oparts.append(occlusion_counts(occ_fw, cur.masks["occ"], cur.valid))
+            del flow_bw, fb_err, occ_fw
         sparse += cur.sparse
         del cur, p1, p2, flow_pr, flow
         nxt = stage_next()                          # staged while this batch computes
@@ -164,6 +229,11 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
     for sp in scores:
         cols = [torch.cat(c).cpu().tolist() for c in zip(*sp)] if sp else [[], [], []]
         rows = [r + s for r, s in zip(rows, zip(*cols))]
+    if regions:                             # one more item per row: (index, style, cell counts, cell sums, fg, occ counts)
+        rp = cat_regions(rparts) if rparts else RegionPartials(torch.zeros(0, 0, 5), torch.zeros(0, 0), torch.zeros(0))
+        occ = torch.cat(oparts).cpu().tolist() if oparts else [None] * len(rmeta)
+        rows = [r + ((m.index, m.kind, c, e, f, o),) for r, m, c, e, f, o in
+                zip(rows, rmeta, rp.counts.cpu().tolist(), rp.epe_sum.cpu().tolist(), rp.fg.tolist(), occ)]
     rows = gather_strided(rows, world)
     every = Partials(torch.tensor([r[0] for r in rows], dtype=torch.int64).view(-1, 5),
                      torch.tensor([r[1] for r in rows], dtype=torch.float64))
@@ -175,6 +245,18 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
             torch.tensor([r[c + 1] for r in rows], dtype=torch.float64).view(-1, FRACTIONS),
             torch.tensor([r[c + 2] for r in rows], dtype=torch.float64).view(-1, FRACTIONS)))
         res.update({prefix + "sparsification": summ["sparsification"], "ideal": summ["ideal"], prefix + "ause": summ["ause"]})
+    if regions:
+        reg = [r[-1] for r in rows]
+        for g in reg:
+            if g[1] != reg[0][1]:
+                raise ValueError(f"validate(regions=True): sample {g[0]} is {g[1].capitalize()}-style but sample {reg[0][0]} is "
+                                 f"{reg[0][1].capitalize()}-style; one split is one or the other")
+        if reg:
+            res.update(summarize_regions(RegionPartials(torch.tensor([g[2] for g in reg], dtype=torch.int64),
+                                                        torch.tensor([g[3] for g in reg], dtype=torch.float64),
+                                                        torch.tensor([g[4] for g in reg], dtype=torch.bool))))
+            if consistency and reg[0][1] == "sintel":
+                res.update(summarize_occlusion(torch.tensor([g[5] for g in reg], dtype=torch.int64)))
     return res
 
 

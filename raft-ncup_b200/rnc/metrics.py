@@ -11,6 +11,12 @@ depend on the batch size or on how the images were spread over ranks.
 curve (the mean EPE of the valid pixels left once the lowest-scored fraction f_k = k/100 is removed) and its ideal (the
 largest errors removed instead) as partial sums; `summarize_sparsification` gives the split's curves and their AUSE.  CUDA
 tensors go through rnc_sparsification (csrc/sparsification.cu), CPU tensors through `host_sparsification`.
+
+`region_partials(flow, gt, valid, occ=..., noc=..., fg=...)` splits the flow metrics' partials by region (Sintel's matched /
+unmatched, occlusion-boundary distance and speed bins; KITTI's background / foreground over all and non-occluded pixels; the
+definitions are below), and `summarize_regions` gives the split's per-region EPE or Fl.  `boundary_dist2(occ)` is the exact
+distance transform they use.  CUDA tensors go through rnc_boundary_dist2 and rnc_region_metrics (csrc/region_metrics.cu),
+CPU tensors through `host_boundary_dist2` and `host_region_partials`.
 """
 from collections import namedtuple
 
@@ -316,3 +322,259 @@ def host_fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5):
     occ_fw, err_fw = _fb_direction(f, g, a1, a2)
     occ_bw, err_bw = _fb_direction(g, f, a1, a2)
     return occ_fw, occ_bw, err_fw, err_bw
+
+
+# ----------------------------------------------------------------------------------------------------------- region metrics
+#
+# The per-region errors the Sintel and KITTI 2015 benchmarks publish, as this project defines them (the Sintel server does not
+# publish its pixel conventions, so these are not claimed to reproduce its values to the last pixel).  Per pixel: epe, mag =
+# |gt| and the outlier test epe > 3 & epe / mag > 0.05 in rnc_flow_metrics' float32 arithmetic.  A region counts only the
+# pixels with valid >= 0.5 (every pixel when valid is None), and every region metric is pooled over the pixels of the whole
+# split.
+#
+# Sintel-style (occ: [H,W] per image, occluded where >= 0.5):
+#   matched = not occluded, unmatched = occluded.
+#   A boundary pixel has a 4-neighbour inside the image whose occlusion label differs from its own (pixels on both sides of
+#   the boundary count).  d2(p) is the exact squared Euclidean distance, in pixels, from p to the nearest boundary pixel of
+#   its image, over the whole image whatever valid says (DIST2_NONE in an image without a boundary).
+#   d0-10: d2 < 100; d10-60: 100 <= d2 < 3600; d60-140: 3600 <= d2 < 19600; farther, or no boundary: no d-bin.
+#   s0-10: mag < 10; s10-40: 10 <= mag < 40; s40+: mag >= 40; a NaN mag: no s-bin.
+# KITTI-style (noc: [H,W], the validity of the non-occluded ground truth, where >= 0.5; fg: [H,W] or None, foreground where
+#   >= 0.5, from the object map): Fl (the outlier rate, in percent) over all, background and foreground pixels, each over all
+#   valid pixels and over the valid pixels inside noc.
+#
+# A cell is one joint label of a pixel; region_partials gives per image and per cell the five counts and the fp64 EPE sum of
+# flow_metrics, and a region is a sum of cells.  Sintel: cell = 16*occluded + 4*d + s (d, s: the bin's index, 3 for none),
+# 32 cells.  KITTI: cell = 2*(not noc) + fg, 4 cells.
+
+DIST2_NONE = native.DIST2_NONE
+SINTEL_CELLS, KITTI_CELLS = native.REGION_CELLS[native.REGIONS_SINTEL], native.REGION_CELLS[native.REGIONS_KITTI]
+# counts: int64 [N, cells, 5] (as Partials.counts, per cell); epe_sum: float64 [N, cells]; fg: bool [N] (KITTI: the image
+# came with a foreground mask)
+RegionPartials = namedtuple("RegionPartials", "counts epe_sum fg")
+# region -> its cells, in increasing order
+SINTEL_REGIONS = {"matched": list(range(16)), "unmatched": list(range(16, 32)),
+                  **{k: [c for c in range(32) if (c >> 2) & 3 == i] for i, k in enumerate(("d0-10", "d10-60", "d60-140"))},
+                  **{k: [c for c in range(32) if c & 3 == i] for i, k in enumerate(("s0-10", "s10-40", "s40+"))}}
+KITTI_REGIONS = {"all": [0, 1, 2, 3], "bg": [0, 2], "fg": [1, 3], "all_noc": [0, 1], "bg_noc": [0], "fg_noc": [1]}
+
+
+def _check_mask(name, m, flow):
+    want = (flow.shape[0],) + tuple(flow.shape[2:])
+    if tuple(m.shape) != want:
+        raise ValueError(f"region_partials: expected {name} [B,H,W] = {want}, got {tuple(m.shape)}")
+    if m.device != flow.device:
+        raise ValueError(f"region_partials: {name} is on {m.device}, the flow on {flow.device}; they must be on one device")
+
+
+def _check_regions(flow, gt, valid, occ, noc, fg):
+    _check(flow, gt, valid)
+    if (occ is None) == (noc is None):
+        raise ValueError("region_partials: give occ (Sintel-style) or noc (KITTI-style), not both or neither")
+    if occ is not None and fg is not None:
+        raise ValueError("region_partials: fg goes with noc (KITTI-style), not with occ")
+    for name, m in (("occ", occ), ("noc", noc), ("fg", fg)):
+        if m is not None:
+            _check_mask(name, m, flow)
+
+
+def boundary_dist2(occ):
+    """occ: [B,H,W] (any strides; float32, or converted to it), occluded where >= 0.5.  Returns int32 [B,H,W]: per pixel the
+    exact squared Euclidean distance to the nearest occlusion-boundary pixel of its image, DIST2_NONE in an image without
+    one.  CUDA tensors go through rnc_boundary_dist2 (enqueued on the current stream; 1 <= H, W <= 4096), CPU tensors through
+    host_boundary_dist2; both are exact integers, so they are equal."""
+    if occ.dim() != 3 or occ.numel() == 0:
+        raise ValueError(f"boundary_dist2: expected a non-empty [B,H,W] mask, got {tuple(occ.shape)}")
+    if not occ.is_cuda:
+        return host_boundary_dist2(occ)
+    occ = occ.float()
+    B, H, W = occ.shape
+    d2 = torch.empty(B, H, W, dtype=torch.int32, device=occ.device)
+    with torch.cuda.device(occ.device):
+        native.rnc.boundary_dist2(occ, *occ.stride(), B, H, W, d2)
+    return d2
+
+
+def _boundary(lab):
+    """Boundary pixels of a bool [B,H,W] label map: a 4-neighbour inside the image holds the other label."""
+    bnd = np.zeros_like(lab)
+    dy = lab[:, 1:] != lab[:, :-1]
+    bnd[:, 1:] |= dy
+    bnd[:, :-1] |= dy
+    dx = lab[:, :, 1:] != lab[:, :, :-1]
+    bnd[:, :, 1:] |= dx
+    bnd[:, :, :-1] |= dx
+    return bnd
+
+
+def host_boundary_dist2(occ):
+    """boundary_dist2 in numpy int64, exact: the distance along each column to its nearest boundary pixel, then along each row
+    the lower envelope of the parabolas q -> g(q)^2 + (x - q)^2 (Felzenszwalb and Huttenlocher), with the intersections
+    compared by cross-multiplying, every row of the batch at once."""
+    lab = (occ.detach().cpu().float() >= 0.5).numpy()
+    B, H, W = lab.shape
+    bnd = _boundary(lab)
+    none = np.int64(1) << 40
+    g = np.full((B, H, W), none, dtype=np.int64)
+    last = np.full((B, W), -1, dtype=np.int64)
+    for y in range(H):
+        last = np.where(bnd[:, y], y, last)
+        g[:, y] = np.where(last >= 0, y - last, none)
+    nxt = np.full((B, W), -1, dtype=np.int64)
+    for y in range(H - 1, -1, -1):
+        nxt = np.where(bnd[:, y], y, nxt)
+        g[:, y] = np.where(nxt >= 0, np.minimum(g[:, y], nxt - y), g[:, y])
+    g = g.reshape(B * H, W)
+    R = B * H
+    q_all = np.arange(W, dtype=np.int64)
+    F = np.where(g < none, g * g + q_all * q_all, -1)
+    v = np.zeros((R, W), dtype=np.int64)
+    n = np.zeros(R, dtype=np.int64)
+    rows = np.arange(R)
+    for q in range(W):
+        fq = F[:, q]
+        popping = fq >= 0
+        while True:
+            idx = rows[popping & (n > 1)]
+            if idx.size == 0:
+                break
+            p, r = v[idx, n[idx] - 1], v[idx, n[idx] - 2]
+            fp, fr = F[idx, p], F[idx, r]
+            pop = (fq[idx] - fp) * (p - r) <= (fp - fr) * (q - p)
+            n[idx[pop]] -= 1
+            popping[idx[~pop]] = False
+        push = rows[fq >= 0]
+        v[push, n[push]] = q
+        n[push] += 1
+    out = np.full((R, W), DIST2_NONE, dtype=np.int64)
+    k = np.zeros(R, dtype=np.int64)
+    some = rows[n > 0]
+    for x in range(W):
+        while True:                 # move on to the next parabola while x is at or past where it takes over
+            idx = some[k[some] + 1 < n[some]]
+            a, c = v[idx, k[idx]], v[idx, k[idx] + 1]
+            step = 2 * x * (c - a) >= F[idx, c] - F[idx, a]
+            if not step.any():
+                break
+            k[idx[step]] += 1
+        q = v[some, k[some]]
+        out[some, x] = F[some, q] - q * q + (x - q) * (x - q)
+    return torch.from_numpy(out.reshape(B, H, W).astype(np.int32))
+
+
+def region_partials(flow, gt, valid=None, occ=None, noc=None, fg=None):
+    """flow, gt: [B,2,H,W]; valid: [B,H,W] or None (every pixel valid); then either occ (Sintel-style) or noc and optionally
+    fg (KITTI-style), each [B,H,W] (any strides; float32, or converted to it).  Returns RegionPartials of B images on the
+    tensors' device (the region definitions above).  CUDA tensors go through rnc_boundary_dist2 and rnc_region_metrics
+    (enqueued on the current stream), CPU tensors through host_region_partials; the counts are equal and the sums agree to
+    the last few bits.  An image's partials do not depend on the batch it came in."""
+    _check_regions(flow, gt, valid, occ, noc, fg)
+    if not flow.is_cuda:
+        return host_region_partials(flow, gt, valid, occ, noc, fg)
+    flow, gt = flow.float(), gt.float()
+    valid = None if valid is None else valid.float()
+    B, _, H, W = flow.shape
+    dev = flow.device
+    kind = native.REGIONS_SINTEL if occ is not None else native.REGIONS_KITTI
+    cells = native.REGION_CELLS[kind]
+    mask = (occ if occ is not None else noc).float()
+    fg = None if fg is None else fg.float()
+    counts = torch.empty(B, cells, 5, dtype=torch.int64, device=dev)
+    epe_sum = torch.empty(B, cells, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        d2 = boundary_dist2(mask) if occ is not None else None
+        ws = torch.empty(native.rnc.region_metrics_workspace_bytes(kind, B, H, W), dtype=torch.uint8, device=dev)
+        vs = (0, 0, 0) if valid is None else valid.stride()
+        qs = (0, 0, 0) if fg is None else fg.stride()
+        native.rnc.region_metrics(kind, flow, *flow.stride(), gt, *gt.stride(), valid, *vs, mask, *mask.stride(), d2, fg, *qs,
+                                  B, H, W, counts, epe_sum, ws, ws.numel())
+    return RegionPartials(counts, epe_sum, torch.full((B,), fg is not None, dtype=torch.bool))
+
+
+def host_region_partials(flow, gt, valid=None, occ=None, noc=None, fg=None):
+    """region_partials' definition, one image at a time: the pixel values as host_partials rounds them, the cell of each valid
+    pixel, and per cell the counts and the fp64 sum of its EPEs (numpy.bincount)."""
+    _check_regions(flow, gt, valid, occ, noc, fg)
+    B = flow.shape[0]
+    cells = SINTEL_CELLS if occ is not None else KITTI_CELLS
+    d2 = host_boundary_dist2(occ).to(torch.int64) if occ is not None else None
+    counts = torch.zeros(B, cells, 5, dtype=torch.int64)
+    sums = torch.zeros(B, cells, dtype=torch.float64)
+    for b in range(B):
+        f, g = flow[b].detach().cpu().float().double(), gt[b].detach().cpu().float().double()
+        epe = _norm(_f32(f - g))
+        mag = _norm(g)
+        val = torch.ones_like(epe, dtype=torch.bool) if valid is None else valid[b].cpu() >= 0.5
+        out = (epe > 3.0) & (_f32(epe / mag).float() > 0.05)
+        if occ is not None:
+            d = (d2[b] >= 100).long() + (d2[b] >= 3600).long() + (d2[b] >= 19600).long()    # DIST2_NONE: 3
+            s = torch.where(torch.isnan(mag), 3, (mag >= 10).long() + (mag >= 40).long())
+            cell = 16 * (occ[b].cpu().float() >= 0.5).long() + 4 * d + s
+        else:
+            cell = 2 * (~(noc[b].cpu().float() >= 0.5)).long()
+            if fg is not None:
+                cell = cell + (fg[b].cpu().float() >= 0.5).long()
+        c, e = cell[val].numpy(), epe[val].numpy()
+        o = out[val].numpy()
+        counts[b] = torch.from_numpy(np.stack([np.bincount(c[m], minlength=cells)
+                                               for m in (np.ones_like(o), e < 1, e < 3, e < 5, o)], 1))
+        sums[b] = torch.from_numpy(np.bincount(c, weights=e, minlength=cells).astype(np.float64))
+    return RegionPartials(counts, sums, torch.full((B,), fg is not None, dtype=torch.bool))
+
+
+def cat_regions(parts):
+    """One RegionPartials of a list of them (of one style), in order."""
+    return RegionPartials(torch.cat([p.counts for p in parts]), torch.cat([p.epe_sum for p in parts]),
+                          torch.cat([p.fg for p in parts]))
+
+
+def summarize_regions(partials):
+    """The split's region metrics from its per-image RegionPartials, pooled over pixels.  Each region's counts are exact
+    integer sums; its EPE sum adds, image by image in order, the image's cells of the region in increasing order (fp64).
+    Sintel-style (32 cells): epe_matched, epe_unmatched, epe_d0-10, epe_d10-60, epe_d60-140, epe_s0-10, epe_s10-40, epe_s40+.
+    KITTI-style (4 cells): fl_all and fl_all_noc, and when every image came with fg also fl_bg, fl_fg, fl_bg_noc and
+    fl_fg_noc, in percent as summarize's f1 (fl_all counts f1's pixels, so it equals f1 bit for bit).  region_pixels: each
+    returned region's valid-pixel count.  A region without a pixel gives NaN."""
+    counts = partials.counts.cpu().tolist()
+    sums = partials.epe_sum.cpu().tolist()
+    cells = partials.counts.shape[1]
+    if cells not in (SINTEL_CELLS, KITTI_CELLS):
+        raise ValueError(f"summarize_regions: expected {SINTEL_CELLS} (Sintel) or {KITTI_CELLS} (KITTI) cells, got {cells}")
+    res, pixels = {}, {}
+    if cells == SINTEL_CELLS:
+        for name, cs in SINTEL_REGIONS.items():
+            n = sum(c[k][0] for c in counts for k in cs)
+            epe = 0.0
+            for s in sums:
+                si = 0.0
+                for k in cs:
+                    si += s[k]
+                epe += si
+            res["epe_" + name] = _ratio(epe, n)
+            pixels[name] = n
+    else:
+        names = list(KITTI_REGIONS) if bool(partials.fg.all()) else ["all", "all_noc"]
+        for name in names:
+            cs = KITTI_REGIONS[name]
+            n = sum(c[k][0] for c in counts for k in cs)
+            res["fl_" + name] = 100 * _ratio(sum(c[k][4] for c in counts for k in cs), n)
+            pixels[name] = n
+    res["region_pixels"] = pixels
+    return res
+
+
+def occlusion_counts(pred, occ, valid=None):
+    """Scores a predicted occlusion mask against the ground truth: pred [B,H,W], occluded where non-zero (fb_consistency's
+    occ: inconsistent or leaving the frame); occ [B,H,W], occluded where >= 0.5; valid [B,H,W] or None.  Returns int64 [B,3]
+    on their device: per image the valid pixels predicted and truly occluded, predicted occluded, and truly occluded (integer
+    sums, so the same on any device and in any order)."""
+    p, t = pred != 0, occ >= 0.5
+    v = torch.ones_like(p) if valid is None else valid >= 0.5
+    return torch.stack([(p & t & v).sum((1, 2)), (p & v).sum((1, 2)), (t & v).sum((1, 2))], 1).to(torch.int64)
+
+
+def summarize_occlusion(counts):
+    """occ_precision, occ_recall and occ_f1 of the split from occlusion_counts' rows, pooled over pixels; NaN when a
+    denominator is 0."""
+    tp, pp, ap = (sum(r[k] for r in counts.cpu().tolist()) for k in range(3))
+    return {"occ_precision": _ratio(tp, pp), "occ_recall": _ratio(tp, ap), "occ_f1": _ratio(2 * tp, pp + ap)}

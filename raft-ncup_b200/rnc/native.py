@@ -150,7 +150,15 @@ SIGNATURES = {
                                 _vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
     "rnc_fb_consistency": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _f, _f, _vp, _vp, _vp, _vp,
                                 _vp]),
+    "rnc_boundary_dist2": (_i, [_vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp]),
+    "rnc_region_metrics_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
+    "rnc_region_metrics": (_i, [_i, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 3,
+                                _vp, *[C.c_longlong] * 3, _vp, _vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp, _vp,
+                                C.c_size_t, _vp]),
 }
+DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
+REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind
+REGION_CELLS = {REGIONS_SINTEL: 32, REGIONS_KITTI: 4}
 
 _lib = None
 _lock = threading.Lock()
