@@ -277,6 +277,10 @@ int rnc_coords_to_flow(const float* coords1, float* flow, int B, int H, int W, v
  * keep samples landing strictly inside the image, give each grid point the flow of its nearest kept sample
  * (scipy griddata 'nearest', fill 0).  flow, out: NCHW [B][2][H][W]. */
 int rnc_forward_interpolate_fwd(const float* flow, int B, int H, int W, float* out, void* stream);
+/* Both warm starts of a bidirectional sequence step in one launch.  flow, out: NCHW [2B][2][H][W]; rows [0, B) are
+ * forward flows and get rnc_forward_interpolate_fwd's result; rows [B, 2B) are backward flows b, whose samples move to
+ * x - b(x) carrying b(x) (the constant-velocity warm start of the next backward pair), i.e. -forward_interpolate(-b). */
+int rnc_forward_interpolate_bidir_fwd(const float* flow, int B, int H, int W, float* out, void* stream);
 
 /* Layout plumbing between the reference's NCHW tensors and the resident CL buffers. */
 int rnc_nchw_to_cl(const float* src, int B, int C, int H, int W, float* dst, int ldd, int ch_off, void* stream);

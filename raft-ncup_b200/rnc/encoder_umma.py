@@ -248,6 +248,68 @@ class EncoderRunner:
         self._context(pc, bufs, ws, image1, h8, w8)
         return h8, w8
 
+    def run_bidirectional_step(self, model, ws, image1, image2, carry, restart, ctx):
+        """One step of bidirectional sequence inference (rnc.model.BidirectionalSequenceStage) on a workspace of 2B slots:
+        slot j holds the forward pair (image1[j], image2[j]), slot B + j the backward pair (image2[j], image1[j]).  For the
+        `carry` slots, frame 1 of the forward pair is the last step's frame 2, whose features are still level 0 of
+        ws.f2_pyr: they are copied into slot j's rows of ws.f1_cl / ws.f1h and into level 0 of slot B + j.  Then fnet runs on
+        cat(image2 of every slot, image1 of the `restart` slots), the images run_step encodes; its head writes level 0 of
+        f2_pyr for slots 0..B-1, a copy of those gives the f1_cl rows of slots B..2B-1, and a restarted slot's own frame 1
+        fills its f1_cl rows and level 0 of slot B + j.  cnet runs on the same B + R images: image2 is the context of the
+        backward slots, a restarted slot's image1 that of its forward slot, and a carried forward slot takes the last step's
+        backward context from ctx (h, hi, lo: [B*H8*W8, 128] fp32 and two [B*H8*W8, 256] fp16, the stage's buffer), which
+        is then refilled with this step's.  Slots in neither list keep their forward f1 rows and backward f2 level 0 (an idle
+        slot recomputes its last pair; its forward context is left as it is and its results are dropped).  The caller
+        converts the f1 rows of the restarted forward slots and of every backward slot to halves."""
+        eng, E = self.eng, native
+        B, _, Hin, Win = image1.shape
+        dev = image1.device
+        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
+        bufs = self.buffers(dev, 2 * B, Hin, Win)         # B + R <= 2B images: an ordinary forward's buffers
+        h8, w8, _ = bufs.dims[2]
+        P = h8 * w8
+        n = P * 256                                         # elements of one slot's feature map
+        eng.alloc_fmaps(ws, 2 * B, 256, h8, w8, 4, dev)
+        f1, halves = ws.f1_cl.view(-1), eng.lookup_mode == "umma"
+        for j0, k in _runs(carry):                          # before the fnet head overwrites level 0
+            src = ws.f2_pyr[j0 * n:(j0 + k) * n]
+            f1[j0 * n:(j0 + k) * n].copy_(src)
+            ws.f2_pyr[(B + j0) * n:(B + j0 + k) * n].copy_(src)
+            if halves:
+                ws.f1h[j0 * n:(j0 + k) * n].copy_(ws.f2h[j0 * n:(j0 + k) * n])
+        both = (torch.cat([image2] + [image1[j:j + 1] for j in restart]) if restart else image2).contiguous()
+        self._trunk(pf, bufs, both, B + len(restart), Hin, Win)
+        xs = bufs.XS[2]
+        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
+        f1[B * n:2 * B * n].copy_(ws.f2_pyr[:B * n])
+        for r, j in enumerate(restart):
+            i = (B + r) * P                                 # image B + r inside the 128-channel split planes
+            eng.uconv(1, h8, w8, (xs.hi[i:].data_ptr(), xs.lo[i:].data_ptr()), 128, 128, pf.head, E.EPI_LINEAR,
+                      out_f32=f1[j * n:].data_ptr(), ldo_f32=256)
+            ws.f2_pyr[(B + j) * n:(B + j + 1) * n].copy_(f1[j * n:(j + 1) * n])
+        # ---- cnet on the same images
+        self._trunk(pc, bufs, both, B + len(restart), Hin, Win)
+        ws.gru_const_valid = False                          # inp changes: the GRU's hoisted share must be recomputed
+        xs = bufs.XS[2]
+        hx_hi, hx_lo = ws.hx.hi[:, :256], ws.hx.lo[:, :256]
+        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pc.head, E.EPI_TANH_RELU, out_f32=ws.h[B * P:].data_ptr(), ldo_f32=128,
+                  out_split=(ws.hx.hi[B * P:].data_ptr(), ws.hx.lo[B * P:].data_ptr()), ldo_split=HX_LD)
+        for r, j in enumerate(restart):
+            i = (B + r) * P
+            eng.uconv(1, h8, w8, (xs.hi[i:].data_ptr(), xs.lo[i:].data_ptr()), 128, 128, pc.head, E.EPI_TANH_RELU,
+                      out_f32=ws.h[j * P:].data_ptr(), ldo_f32=128,
+                      out_split=(ws.hx.hi[j * P:].data_ptr(), ws.hx.lo[j * P:].data_ptr()), ldo_split=HX_LD)
+        ch, chi, clo = ctx
+        for j0, k in _runs(carry):
+            rows = slice(j0 * P, (j0 + k) * P)
+            ws.h[rows].copy_(ch[rows])
+            hx_hi[rows].copy_(chi[rows])
+            hx_lo[rows].copy_(clo[rows])
+        ch.copy_(ws.h[B * P:])
+        chi.copy_(hx_hi[B * P:])
+        clo.copy_(hx_lo[B * P:])
+        return h8, w8
+
 
 def _runs(slots):
     """Sorted slot indices -> (first, count) of each run of consecutive ones: one copy per run."""

@@ -313,6 +313,47 @@ def _stack(frames, device, padder):
     return padder.pad(x.to(device, non_blocking=True).float())[0]
 
 
+def _sequence_setup(sequences, batch_size, mode, model, return_confidence):
+    """The argument checks and the schedule shared by run_sequences and run_sequences_bidirectional: ValueError for frames
+    of more than one [3,H,W] size and for return_confidence on the convex model.  Returns (sequence_schedule's steps, the
+    InputPadder of the frame size), or ([], None) when no sequence has a pair."""
+    sizes = [tuple(f.shape) for seq in sequences for f in seq]
+    for s in sizes:
+        if len(s) != 3 or s != sizes[0]:
+            raise ValueError(f"all frames of one call must have the same [3,H,W] size: got {sizes[0]} and {s}")
+    if return_confidence and not model.ncup:
+        raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
+    steps = sequence_schedule([len(seq) for seq in sequences], batch_size)
+    return steps, (InputPadder(sizes[0], mode=mode) if steps else None)
+
+
+def _step_images(sequences, step, device, padder):
+    """Frames 1 and 2 of every slot of one step, padded, on the device."""
+    return (_stack([sequences[c.seq][c.pair] for c in step], device, padder),
+            _stack([sequences[c.seq][c.pair + 1] for c in step], device, padder))
+
+
+def _sequence_engine(model, im1):
+    """(device, engine) of a sequence generator's first step; ValueError when the model is on another device."""
+    from .engine import _require_cuda, engine_for, module_device
+    dev = _require_cuda(im1)
+    if module_device(model) != dev:
+        raise ValueError(f"model parameters are on {module_device(model)} but device is {dev}")
+    return dev, engine_for(dev)
+
+
+def _sequence_workspace(eng, model, dev, slots, im1):
+    """A sequence generator's own workspace of `slots` slots: the features carried from step to step live in it, so the
+    caller may run other forwards of the same shape between two steps."""
+    pk = eng.packed_update(model.update_block)
+    return eng.WS(dev, slots, im1.shape[2] // 8, im1.shape[3] // 8, pk.has_mask, model.ncup)
+
+
+def _assign_slots(stage, step):
+    stage.restart = [j for j, c in enumerate(step) if c.restart]
+    stage.carry = [j for j, c in enumerate(step) if not c.restart and not c.idle]
+
+
 @torch.no_grad()
 def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
                   return_confidence=False):
@@ -325,43 +366,29 @@ def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mo
     frame 2, whose fnet features are handed over on the device (rnc.model.SequenceStage).  With warm_start, a slot starts
     from forward_interpolate of its own previous low-resolution flow, and from zero (a cold start) at pair 0.  The steps
     run eagerly and never wait for the host; the caller moves or writes the flows."""
-    sizes = [tuple(f.shape) for seq in sequences for f in seq]
-    for s in sizes:
-        if len(s) != 3 or s != sizes[0]:
-            raise ValueError(f"all frames of one call must have the same [3,H,W] size: got {sizes[0]} and {s}")
-    if return_confidence and not model.ncup:
-        raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
-    steps = sequence_schedule([len(seq) for seq in sequences], batch_size)
+    steps, padder = _sequence_setup(sequences, batch_size, mode, model, return_confidence)
     if not steps:
         return
-    from .engine import _require_cuda, engine_for, module_device
+    from .engine import _Timed
     from .model import SequenceStage
     model.eval()
-    padder = InputPadder(sizes[0], mode=mode)
     stage = SequenceStage(model)
     ws = fi = zero = None
     for step in steps:
-        im1 = _stack([sequences[c.seq][c.pair] for c in step], device, padder)
-        im2 = _stack([sequences[c.seq][c.pair + 1] for c in step], device, padder)
+        im1, im2 = _step_images(sequences, step, device, padder)
         if ws is None:
-            dev = _require_cuda(im1)
-            if module_device(model) != dev:
-                raise ValueError(f"model parameters are on {module_device(model)} but device is {dev}")
-            eng = engine_for(dev)
-        stage.restart = [j for j, c in enumerate(step) if c.restart]
-        stage.carry = [j for j, c in enumerate(step) if not c.restart and not c.idle]
+            dev, eng = _sequence_engine(model, im1)
+        _assign_slots(stage, step)
         with torch.cuda.device(dev), eng.lock:
             if ws is None:
-                # this generator's own workspace: the features carried from step to step live in it, so the caller may run
-                # other forwards of the same shape between two steps
-                pk = eng.packed_update(model.update_block)
-                ws = eng.WS(dev, len(step), im1.shape[2] // 8, im1.shape[3] // 8, pk.has_mask, model.ncup)
+                ws = _sequence_workspace(eng, model, dev, len(step), im1)
             for j in stage.restart if fi is not None else ():
                 fi[j].copy_(zero)           # cold start: coords0 + 0.0 is exactly coords0, as with flow_init=None
             flow_low, flow_up, *conf = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws,
                                                             return_confidence=return_confidence)
             if warm_start:
-                fi = forward_interpolate(flow_low)
+                with _Timed(eng, "warm_start"):
+                    fi = forward_interpolate(flow_low)
                 if zero is None:
                     zero = torch.zeros_like(fi[0])
         for j, c in enumerate(step):
@@ -370,6 +397,93 @@ def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mo
                     yield c.seq, c.pair, padder.unpad(flow_up[j]), padder.unpad(conf[0][j])
                 else:
                     yield c.seq, c.pair, padder.unpad(flow_up[j])
+
+
+def bidirectional_warm_start(flow_low):
+    """Warm starts of the next step of bidirectional sequence inference, both directions in one launch
+    (rnc_forward_interpolate_bidir_fwd).  flow_low: [2B,2,H,W] on a CUDA device, rows [0, B) forward flows f_{k->k+1},
+    rows [B, 2B) backward flows b_{k+1->k}.  Row j of the result is forward_interpolate(f) (the reference's warm start);
+    row B + j assumes constant velocity backwards: the point at x in frame k+1 is at x - b(x) in frame k+2 and its backward
+    flow there is b(x), so each sample moves to x - b(x) and carries b(x), with forward_interpolate's validity test,
+    nearest-sample rule and fill 0.  As an identity it is -forward_interpolate(-b), bit for bit."""
+    from .engine import _require_cuda
+    from .native import rnc
+    dev = _require_cuda(flow_low)
+    if flow_low.dim() != 4 or flow_low.shape[0] % 2 or flow_low.shape[1] != 2:
+        raise ValueError(f"bidirectional_warm_start: expected [2B,2,H,W], got {tuple(flow_low.shape)}")
+    f = flow_low.detach().float().contiguous()
+    N, _, H, W = f.shape
+    out = torch.empty_like(f)
+    with torch.cuda.device(dev):
+        rnc.forward_interpolate_bidir_fwd(f, N // 2, H, W, out)
+    return out
+
+
+def run_sequences_bidirectional(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
+                                return_confidence=False, alpha1=0.01, alpha2=0.5):
+    """Forward and backward flow, with forward-backward occlusion masks, for every consecutive frame pair of many
+    sequences, each frame encoded once.  sequences: list of frame lists, every frame [3,H,W] of one size.  Yields
+    (seq_index, pair_index, result) for pair k = frames (k, k + 1) of every sequence; result has bidirectional_flow's keys
+    (flow_low, flow_up, flow_low_bw, flow_up_bw, occ, occ_bw, fb_err, fb_err_bw, and with return_confidence (NCUP model)
+    confidence, confidence_bw), each that pair's slice without the batch dimension, on the device, unpadded as
+    bidirectional_flow's.  Cold, pair k's result is bidirectional_flow(model, f_k[None], f_{k+1}[None], iters, mode=mode)'s.
+    With warm_start, pair k > 0 starts from bidirectional_warm_start of pair k - 1's flow_low and flow_low_bw (the forward
+    rule of run_sequences, and its mirror for the backward flow); pair 0 starts cold in both directions.  The forward rows
+    are run_sequences(model, sequences, ...)'s flows.
+
+    Slots run in lockstep as in run_sequences (sequence_schedule), on a workspace of 2B slots: slot j holds a sequence's
+    forward pair, slot B + j its backward pair.  fnet and cnet encode each new frame once per step: a frame's features
+    and context serve the backward pair that starts at it and, one step later, the forward pair that starts at it
+    (rnc.model.BidirectionalSequenceStage).  Each step checks consistency on both directions in one launch
+    (rnc.metrics.fb_consistency with alpha1, alpha2) and computes both warm starts in one launch; the steps never wait for
+    the host.  Inference only: with grad enabled on a model that requires grad it raises ValueError."""
+    steps, padder = _sequence_setup(sequences, batch_size, mode, model, return_confidence)
+    if not steps:
+        return
+    if model._needs_grad():
+        raise ValueError("run_sequences_bidirectional is inference only: call it under torch.no_grad() (training through the "
+                         "bidirectional pass is not built)")
+    yield from _bidirectional_steps(model, sequences, steps, padder, iters, warm_start, device, return_confidence, alpha1,
+                                    alpha2)
+
+
+@torch.no_grad()
+def _bidirectional_steps(model, sequences, steps, padder, iters, warm_start, device, return_confidence, alpha1, alpha2):
+    from .engine import _Timed
+    from .metrics import fb_consistency
+    from .model import BidirectionalSequenceStage
+    model.eval()
+    stage = BidirectionalSequenceStage(model)
+    B = len(steps[0])
+    ws = fi = zero = None
+    for step in steps:
+        im1, im2 = _step_images(sequences, step, device, padder)
+        if ws is None:
+            dev, eng = _sequence_engine(model, im1)
+        _assign_slots(stage, step)
+        with torch.cuda.device(dev), eng.lock:
+            if ws is None:
+                ws = _sequence_workspace(eng, model, dev, 2 * B, im1)
+            for j in stage.restart if fi is not None else ():
+                fi[j::B].copy_(zero)        # rows j and B + j: a cold start in both directions
+            flow_low, flow_up, *conf = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws,
+                                                            return_confidence=return_confidence)
+            up = padder.unpad(flow_up)
+            occ, occ_bw, err, err_bw = fb_consistency(up[:B], up[B:], alpha1, alpha2)
+            if warm_start:
+                with _Timed(eng, "warm_start"):
+                    fi = bidirectional_warm_start(flow_low)
+                if zero is None:
+                    zero = torch.zeros_like(fi[0::B])
+        conf = padder.unpad(conf[0]) if return_confidence else None
+        for j, c in enumerate(step):
+            if c.idle:
+                continue
+            res = {"flow_low": flow_low[j], "flow_up": up[j], "flow_low_bw": flow_low[B + j], "flow_up_bw": up[B + j],
+                   "occ": occ[j], "occ_bw": occ_bw[j], "fb_err": err[j], "fb_err_bw": err_bw[j]}
+            if return_confidence:
+                res["confidence"], res["confidence_bw"] = conf[j], conf[B + j]
+            yield c.seq, c.pair, res
 
 
 def size_batches(items, batch_size, key):

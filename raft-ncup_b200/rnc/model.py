@@ -379,6 +379,62 @@ class BidirectionalStage:
         eng.load_state(ws, net, inp)
 
 
+class BidirectionalSequenceStage:
+    """Encoder stage of one step of bidirectional sequence inference (rnc.harness.run_sequences_bidirectional), for
+    _forward_eager(encode=...) on a workspace of 2B slots: slot j holds the forward pair (image1[j], image2[j]) of one
+    sequence, slot B + j the backward pair (image2[j], image1[j]).  `carry` and `restart` are set per step as for
+    SequenceStage.  fnet and cnet run on the B + R images cat(image2, image1 of the restarted slots): frame 2's features and
+    context serve the backward slots and frame 2 of the forward ones; a carried forward slot's frame 1 features are the last
+    step's frame 2 features and its context is the last step's backward context, which the stage keeps (cnet of frame k is
+    the context of both backward pair (k, k-1) and forward pair (k, k+1)).  One stage belongs to one workspace."""
+
+    def __init__(self, model):
+        self.model = model
+        self.carry, self.restart = [], []
+        self.ctx = None             # tensor-core route: the last step's backward context rows (h, hx hi, hx lo)
+        self.fmap1 = self.fmap2 = self.net = self.inp = None    # torch-encoder route: NCHW [2B,...] of the last step
+
+    def __call__(self, eng, ws, image1, image2):
+        m = self.model
+        B = image1.shape[0]
+        if m._umma_encoders(eng):
+            if self.ctx is None:
+                rows, dev = B * ws.H8 * ws.W8, image1.device
+                self.ctx = (torch.empty(rows, 128, dtype=torch.float32, device=dev),
+                            torch.empty(rows, 256, dtype=torch.float16, device=dev),
+                            torch.empty(rows, 256, dtype=torch.float16, device=dev))
+            with _Timed(eng, "encoders"):
+                eng.encoder().run_bidirectional_step(m, ws, image1.float().contiguous(), image2.float().contiguous(),
+                                                     self.carry, self.restart, self.ctx)
+                eng.finish_fmaps(ws, f1_slots=sorted(self.restart) + list(range(B, 2 * B)))
+            return
+        new = torch.cat([image2] + [image1[j:j + 1] for j in self.restart]) if self.restart else image2
+        new = (2 * (new / 255.0) - 1.0).contiguous()
+        with torch.autocast("cuda", enabled=bool(getattr(m.args, "mixed_precision", False))):
+            f = m.fnet(new)
+        f = f.float().contiguous()
+        net, inp = m._context(new)
+        if self.fmap1 is None:
+            self.fmap1, self.fmap2 = (f.new_empty((2 * B,) + f.shape[1:]) for _ in range(2))
+            self.net, self.inp = (net.new_empty((2 * B,) + net.shape[1:]) for _ in range(2))
+        for j in self.carry:        # frame k: the last step's frame 2 of the forward pair, frame 1 of the backward one
+            self.fmap1[j].copy_(self.fmap2[j])
+            self.fmap2[B + j].copy_(self.fmap2[j])
+            self.net[j].copy_(self.net[B + j])
+            self.inp[j].copy_(self.inp[B + j])
+        self.fmap2[:B].copy_(f[:B])
+        self.fmap1[B:].copy_(f[:B])
+        self.net[B:].copy_(net[:B])
+        self.inp[B:].copy_(inp[:B])
+        for r, j in enumerate(self.restart):
+            self.fmap1[j].copy_(f[B + r])
+            self.fmap2[B + j].copy_(f[B + r])
+            self.net[j].copy_(net[B + r])
+            self.inp[j].copy_(inp[B + r])
+        eng.fmap_prepare(ws, self.fmap1, self.fmap2, 4)
+        eng.load_state(ws, self.net, self.inp)
+
+
 class _Dims:
     def __init__(self, B, H8, W8):
         self.B, self.H8, self.W8 = B, H8, W8

@@ -109,6 +109,7 @@ SIGNATURES = {
     "rnc_flow_im2col7_split_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _i, _vp]),
     "rnc_flow_tap_gather_fwd": (_i, [_vp, _i, _vp, _i, _i, _i, _vp, _vp, _vp]),
     "rnc_forward_interpolate_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp]),
+    "rnc_forward_interpolate_bidir_fwd": (_i, [_vp, _i, _i, _i, _vp, _vp]),
     "rnc_coords_init": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "rnc_coords_to_flow": (_i, [_vp, _vp, _i, _i, _i, _vp]),
     "rnc_nchw_to_cl": (_i, [_vp, _i, _i, _i, _i, _vp, _i, _i, _vp]),
