@@ -608,6 +608,50 @@ int rnc_region_metrics(int kind, const float* flow, long long fb, long long fc, 
                        const float* fg, long long qb, long long qy, long long qx, int B, int H, int W, long long* counts,
                        double* epe_sum, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V6  frame interpolation from both flows and the occlusion masks, and the interpolation error (definition: rnc/interp.py,
+ * DESIGN §3.15).
+ *
+ * rnc_interpolate: for each pair b and each time t_k, the frame between frame0 and frame1 at t_k.
+ *   frame0, frame1 : fp32 [B,3,H,W] (0..255) through element strides (ab..ax, bb..bx); 4-byte aligned
+ *   flow, flow_bw  : fp32 [B,2,H,W] through element strides, F (frame 0 -> 1) and G (1 -> 0); 4-byte aligned
+ *   occ0, occ1     : uint8 [B][H][W] contiguous, rnc_fb_consistency's occ_fw / occ_bw of F and G; a pixel is visible where 0
+ *   times          : T host floats, each 0 < t < 1; 1 <= T <= RNC_INTERP_MAX_TIMES
+ *   out            : fp32 [B][T][3][H][W] contiguous; 4-byte aligned
+ *   workspace      : rnc_interpolate_workspace_bytes(B, T, H, W) bytes, 16-byte aligned, no zeroing needed: the uint64 splat
+ *                    map [B][T][H][W], then the int32 nearest-site map [B][T][H][W]
+ * 1. Splat: a pixel x of frame 0 with occ0 == 0 and a finite F(x) proposes u = F(x) at q = rint(x + t F(x)) (half to even)
+ *    when q is in the frame, keyed by e = sum_c |I1^_c(x + F(x)) - I0_c(x)| (channels in order); a pixel y of frame 1 likewise
+ *    proposes u = -G(y) at rint(y + (1 - t) G(y)) with occ1 and e = sum_c |I0^_c(y + G(y)) - I1_c(y)|.  I^ is bilinear with
+ *    the coordinates clamped to the frame.  Each pixel keeps the smallest (e, source index), frame 0's sources 0..HW-1 and
+ *    frame 1's HW..2HW-1: an integer atomicMin of (float bits of e) << 32 | index.
+ * 2. Fill: a pixel without a proposal takes the u of the nearest pixel with one (exact squared distance, ties to the smallest
+ *    column, then row); u = 0 in an image without a proposal.
+ * 3. Composite: x0 = x - t u, x1 = x + (1 - t) u; v0 when x0 is in the frame and occ0(rint(x0)) == 0, v1 likewise; the output
+ *    is (1 - t) I0^(x0) + t I1^(x1) when v0 == v1, else the visible sample.
+ * Every operation rounded once in float32 (no FMA).  A memset and four launches, no host synchronisation, no floating-point
+ * atomics: an output depends only on its own pair and time.  RNC_ERR_BAD_SHAPE for a time outside (0, 1), H or W above 4096,
+ * or B*T above 65535.  Bad arguments return before any launch.
+ *
+ * rnc_interp_error: per image n, sq_sum[n] = the fp64 sum over its pixels of sum_c (pred - gt)^2 (each difference and square in
+ * fp64) and count[n] = H*W.
+ *   pred, gt  : fp32 [N,3,H,W] through element strides; 4-byte aligned
+ *   sq_sum    : fp64 [N], 8-byte aligned; count: int64 [N], 8-byte aligned
+ *   workspace : rnc_interp_error_workspace_bytes(N, H, W) bytes, 16-byte aligned, no zeroing needed (per-CTA partials)
+ * Two launches, no host synchronisation; the sums are added in a fixed order that depends only on H*W, so an image's result is
+ * bit for bit the same whatever N, its position in the batch or the GPU.  Bad arguments return before any launch. */
+#define RNC_INTERP_MAX_TIMES 64
+size_t rnc_interpolate_workspace_bytes(int B, int T, int H, int W);   /* 0 for a bad shape */
+int rnc_interpolate(const float* frame0, long long ab, long long ac, long long ay, long long ax, const float* frame1,
+                    long long bb, long long bc, long long by, long long bx, const float* flow, long long fb, long long fc,
+                    long long fy, long long fx, const float* flow_bw, long long gb, long long gc, long long gy, long long gx,
+                    const unsigned char* occ0, const unsigned char* occ1, const float* times, int T, int B, int H, int W,
+                    float* out, void* workspace, size_t workspace_bytes, void* stream);
+size_t rnc_interp_error_workspace_bytes(int N, int H, int W);   /* 0 for a bad shape */
+int rnc_interp_error(const float* pred, long long pb, long long pc, long long py, long long px, const float* gt, long long gb,
+                     long long gc, long long gy, long long gx, int N, int H, int W, double* sq_sum, long long* count,
+                     void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

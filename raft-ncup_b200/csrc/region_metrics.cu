@@ -3,14 +3,9 @@
 //
 // rnc_boundary_dist2: the exact squared Euclidean distance of every pixel to the nearest occlusion-boundary pixel of its image
 // (a pixel with a 4-neighbour inside the image whose label differs), as a separable transform in integers (Felzenszwalb and
-// Huttenlocher, "Distance Transforms of Sampled Functions", 2012):
-//   1. dist2_column_kernel, a thread per column of one image: the boundary test, then a downward and an upward sweep give
-//      g(y, x), the distance to the nearest boundary pixel in the same column (RNC_DIST2_NONE if the column has none).
-//   2. dist2_row_kernel, a warp per row: d2(y, x) = min_q g(y, q)^2 + (x - q)^2.  Lane 0 builds the lower envelope of the
-//      parabolas q -> g(y, q)^2 + (x - q)^2, comparing intersections by cross-multiplying in int64 (no division, so every
-//      comparison is exact); then each lane finds, by binary search on the same comparisons, the parabola of each of its pixels.
-//   The row pass reads its row of g into shared memory before it writes d2 over it, so d2 holds g in between and no workspace
-//   is needed.  No atomics, no host synchronisation; each pixel's value is an exact integer.
+// Huttenlocher, "Distance Transforms of Sampled Functions", 2012): dist_transform.cuh's column pass, with the boundary test as
+// its sites, then its row pass writing d2(y, x) = min_q g(y, q)^2 + (x - q)^2.  d2 holds the column pass's nearest rows in
+// between, so no workspace is needed.  No atomics, no host synchronisation; each pixel's value is an exact integer.
 //
 // rnc_region_metrics: per image and per cell (one joint label of a pixel; Sintel 2 occlusion x 4 distance x 4 speed classes,
 // KITTI 2 noc x 2 fg) the five counts and the fp64 EPE sum of rnc_flow_metrics, from the same per-pixel float32 arithmetic
@@ -20,6 +15,7 @@
 // memory.  The CTA adds its 8 warps in order, and a second kernel adds each (image, cell)'s CTAs in a fixed order (a warp per
 // pair: lane-strided sums, then a fixed shuffle tree).  The order depends only on H*W and the cell count: an image's results
 // do not depend on B, on its position in the batch or on the GPU, and no floating-point atomics are used.
+#include "dist_transform.cuh"
 #include "pixel_metrics.cuh"
 #include "rnc_common.cuh"
 
@@ -27,95 +23,24 @@ namespace rnc {
 namespace {
 
 constexpr int kNone = RNC_DIST2_NONE;
-constexpr int kMaxSide = 4096;          // H, W of rnc_boundary_dist2; the row pass keeps 6 W bytes of shared memory
-constexpr int kColThreads = 128;
 
-__global__ void __launch_bounds__(kColThreads) dist2_column_kernel(const float* __restrict__ occ, long long ob, long long oy,
-                                                                   long long ox, int H, int W, int* __restrict__ d2) {
-  const int b = blockIdx.y;
-  const int x = blockIdx.x * kColThreads + threadIdx.x;
-  if (x >= W) return;
-  const float* base = occ + b * ob + x * ox;
-  int* col = d2 + static_cast<long long>(b) * H * W + x;
-  // downward: distance to the nearest boundary pixel at or above y
-  bool up = false, cur = base[0] >= 0.5f;
-  int last = -1;
-#pragma unroll 4
-  for (int y = 0; y < H; ++y) {
-    const float* r = base + y * oy;
-    const bool down = y + 1 < H ? r[oy] >= 0.5f : cur;
-    const bool left = x > 0 ? r[-ox] >= 0.5f : cur;
-    const bool right = x + 1 < W ? r[ox] >= 0.5f : cur;
-    if ((y > 0 && up != cur) || down != cur || left != cur || right != cur) last = y;
-    col[static_cast<long long>(y) * W] = last < 0 ? kNone : y - last;
-    up = cur;
-    cur = down;
+// the sites of rnc_boundary_dist2: pixels with a 4-neighbour inside the image whose label (occluded where >= 0.5) differs
+struct BoundarySites {
+  const float* occ;
+  long long ob, oy, ox;
+  int H, W;
+  __device__ bool operator()(int b, int y, int x) const {
+    const float* r = occ + b * ob + y * oy + x * ox;
+    const bool cur = r[0] >= 0.5f;
+    return (y > 0 && (r[-oy] >= 0.5f) != cur) || (y + 1 < H && (r[oy] >= 0.5f) != cur) ||
+           (x > 0 && (r[-ox] >= 0.5f) != cur) || (x + 1 < W && (r[ox] >= 0.5f) != cur);
   }
-  // upward: the nearest boundary pixel at or below y (a boundary pixel holds 0)
-  int next = -1;
-  for (int y = H - 1; y >= 0; --y) {
-    int* c = col + static_cast<long long>(y) * W;
-    const int g = *c;
-    if (g == 0) {
-      next = y;
-    } else if (next >= 0 && next - y < g) {
-      *c = next - y;
-    }
-  }
-}
+};
 
-__global__ void __launch_bounds__(32) dist2_row_kernel(int H, int W, int* __restrict__ d2) {
-  extern __shared__ int smem[];
-  int* F = smem;                                                  // F[q] = g(q)^2 + q^2; -1: the column has no boundary
-  unsigned short* v = reinterpret_cast<unsigned short*>(F + W);  // the lower envelope's parabolas, left to right
-  const int lane = threadIdx.x;
-  int* row = d2 + (static_cast<long long>(blockIdx.y) * H + blockIdx.x) * W;
-  for (int q = lane; q < W; q += 32) {
-    const int g = row[q];
-    F[q] = g == kNone ? -1 : g * g + q * q;
-  }
-  __syncwarp();
-  int n = 0;
-  if (lane == 0) {
-    for (int q = 0; q < W; ++q) {
-      const int fq = F[q];
-      if (fq < 0) continue;
-      // with s(a, b) = (F_b - F_a) / (2 (b - a)) where the parabolas of a < b meet: drop the top p while q overtakes it no
-      // later than p overtook the one below it, r: s(p, q) <= s(r, p)
-      while (n > 1) {
-        const int p = v[n - 1], r = v[n - 2];
-        const int fp = F[p], fr = F[r];
-        if (static_cast<long long>(fq - fp) * (p - r) <= static_cast<long long>(fp - fr) * (q - p)) {
-          --n;
-        } else {
-          break;
-        }
-      }
-      v[n++] = static_cast<unsigned short>(q);
-    }
-  }
-  __syncwarp();
-  n = __shfl_sync(0xffffffffu, n, 0);
-  for (int x = lane; x < W; x += 32) {
-    if (n == 0) {                          // no boundary in the image
-      row[x] = kNone;
-      continue;
-    }
-    // the last k with k == 0 or x >= s(v[k-1], v[k]); on a tie both parabolas give the same value
-    int lo = 0, hi = n - 1;
-    while (lo < hi) {
-      const int mid = (lo + hi + 1) >> 1;
-      const int a = v[mid - 1], c = v[mid];
-      if (2ll * x * (c - a) >= static_cast<long long>(F[c] - F[a])) {
-        lo = mid;
-      } else {
-        hi = mid - 1;
-      }
-    }
-    const int q = v[lo];
-    row[x] = F[q] - q * q + (x - q) * (x - q);
-  }
-}
+struct Dist2Out {                       // the squared distance to the nearest boundary pixel
+  static constexpr int none = kNone;
+  __device__ int operator()(int, int x, int q, int, int fq) const { return fq - q * q + (x - q) * (x - q); }
+};
 
 constexpr int kRegThreads = 256;
 constexpr int kRegWarps = kRegThreads / 32;
@@ -246,7 +171,7 @@ __global__ void __launch_bounds__(kRegThreads) region_reduce_kernel(const Region
 }
 
 bool dist2_shape_ok(int B, int H, int W) {
-  return B > 0 && H > 0 && W > 0 && B <= 65535 && H <= kMaxSide && W <= kMaxSide;
+  return B > 0 && H > 0 && W > 0 && B <= 65535 && H <= kSiteMaxSide && W <= kSiteMaxSide;
 }
 
 int region_cells(int kind) {
@@ -273,10 +198,10 @@ int rnc_boundary_dist2(const float* occ, long long ob, long long oy, long long o
   if (!dist2_shape_ok(B, H, W)) return RNC_ERR_BAD_SHAPE;
   if (!occ || !d2 || !aligned(occ, 4) || !aligned(d2, 4)) return RNC_ERR_BAD_POINTER;
   cudaStream_t s = as_stream(stream);
-  dist2_column_kernel<<<dim3((W + kColThreads - 1) / kColThreads, B), kColThreads, 0, s>>>(occ, ob, oy, ox, H, W, d2);
+  dist2_column_kernel<<<dim3((W + kSiteColThreads - 1) / kSiteColThreads, B), kSiteColThreads, 0, s>>>(
+      BoundarySites{occ, ob, oy, ox, H, W}, H, W, d2);
   if (int st = after_launch()) return st;
-  const size_t smem = static_cast<size_t>(W) * (sizeof(int) + sizeof(unsigned short));
-  dist2_row_kernel<<<dim3(H, B), 32, smem, s>>>(H, W, d2);
+  dist2_row_kernel<<<dim3(H, B), 32, dist2_row_smem(W), s>>>(H, W, d2, Dist2Out{});
   return after_launch();
 }
 

@@ -486,6 +486,63 @@ def _bidirectional_steps(model, sequences, steps, padder, iters, warm_start, dev
             yield c.seq, c.pair, res
 
 
+def interpolate_frames(model, frame0, frame1, times=(0.5,), iters=32, mode="sintel", alpha1=0.01, alpha2=0.5):
+    """The frames between frame0 and frame1 ([B,3,H,W], 0..255, on the model's device, any size) at each of `times`:
+    bidirectional_flow(model, frame0, frame1, iters, mode=mode, alpha1=alpha1, alpha2=alpha2), then rnc.interp.interpolate of
+    its unpadded flows and occlusion masks.  Returns float32 [B,T,3,H,W].  Inference only: with grad enabled on a model that
+    requires grad it raises ValueError."""
+    from .interp import _times, interpolate
+    if model._needs_grad():
+        raise ValueError("interpolate_frames is inference only: call it under torch.no_grad()")
+    _times(times)                                   # a bad time raises before the flow pass
+    r = bidirectional_flow(model, frame0, frame1, iters, mode=mode, alpha1=alpha1, alpha2=alpha2)
+    return interpolate(frame0, frame1, r["flow_up"], r["flow_up_bw"], r["occ"], r["occ_bw"], times)
+
+
+@torch.no_grad()
+def validate_interpolation(model, sequences, iters=32, mode="sintel", batch_size=8, warm_start=False, device="cuda"):
+    """Middlebury's interpolation error of a split of videos, which needs no ground-truth flow: for every triplet of frames
+    (k, k + 1, k + 2) of every sequence, frame k + 1 is interpolated at t = 0.5 from frames k and k + 2 and scored against the
+    real one.  sequences: list of frame lists, every frame [3,H,W] (0..255) of one size.  The pairs (k, k + 2) are the
+    consecutive pairs of each sequence's even-indexed and odd-indexed frames, which run_sequences_bidirectional(model, ...,
+    iters, warm_start, batch_size, mode, device) runs side by side; each pair's flows and masks go through rnc.interp.interpolate
+    and rnc.interp.interpolation_error on the device.  Returns rnc.interp.summarize_interpolation of the per-triplet partials
+    in (sequence, k) order: ie, psnr and frames.  Cold, each triplet's partials are those of bidirectional_flow + interpolate +
+    interpolation_error of its pair alone; warm, each pair starts from the previous pair of its subsequence.  Either way
+    they do not depend on batch_size.  Under torch.distributed rank r takes the sequences of index = r (mod world), the partials are
+    all-gathered, and every rank returns the single-process result."""
+    from .dist import strided_items, world_rank
+    from .interp import InterpPartials, interpolate, interpolation_error, summarize_interpolation
+    world, rank = world_rank()
+    mine = list(strided_items(range(len(sequences)), world, rank))
+    subs, origin = [], []                           # origin[i]: (sequence index, offset) of subsequence i
+    for s in mine:
+        for off in (0, 1):
+            subs.append(sequences[s][off::2])
+            origin.append((s, off))
+    keys, parts = [], []
+    for i, p, r in run_sequences_bidirectional(model, subs, iters, warm_start=warm_start, batch_size=batch_size, mode=mode,
+                                               device=device):
+        s, off = origin[i]
+        k = off + 2 * p
+        seq = sequences[s]
+        dev = r["flow_up"].device
+        f0, f2, gt = (seq[j][None].to(dev).float() for j in (k, k + 2, k + 1))
+        pred = interpolate(f0, f2, r["flow_up"][None], r["flow_up_bw"][None], r["occ"][None], r["occ_bw"][None], (0.5,))
+        parts.append(interpolation_error(pred[:, 0], gt))
+        keys.append((s, k))
+    rows = list(zip(keys, (torch.cat([q.sq_sum for q in parts]).cpu().tolist() if parts else []),
+                    (torch.cat([q.count for q in parts]).cpu().tolist() if parts else [])))
+    if world > 1:
+        import torch.distributed as dist
+        every = [None] * world
+        dist.all_gather_object(every, rows)
+        rows = [r for part in every for r in part]
+    rows.sort(key=lambda r: r[0])
+    return summarize_interpolation(InterpPartials(torch.tensor([r[1] for r in rows], dtype=torch.float64),
+                                                  torch.tensor([r[2] for r in rows], dtype=torch.int64)))
+
+
 def size_batches(items, batch_size, key):
     """Batches of create_kitti_submission: the items of one key(item) (a frame size) in order of appearance, batch_size at a
     time.  A batch is yielded as soon as it is full, the partial batches at the end in order of their size's first

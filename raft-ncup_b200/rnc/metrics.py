@@ -407,35 +407,37 @@ def _boundary(lab):
     return bnd
 
 
-def host_boundary_dist2(occ):
-    """boundary_dist2 in numpy int64, exact: the distance along each column to its nearest boundary pixel, then along each row
-    the lower envelope of the parabolas q -> g(q)^2 + (x - q)^2 (Felzenszwalb and Huttenlocher), with the intersections
-    compared by cross-multiplying, every row of the batch at once."""
-    lab = (occ.detach().cpu().float() >= 0.5).numpy()
-    B, H, W = lab.shape
-    bnd = _boundary(lab)
-    none = np.int64(1) << 40
-    g = np.full((B, H, W), none, dtype=np.int64)
-    last = np.full((B, W), -1, dtype=np.int64)
+def nearest_site(sites):
+    """An exact feature transform: sites, bool numpy [N,H,W] -> int64 [N,H,W], per pixel the row-major index of its
+    nearest site in exact squared Euclidean distance, ties to the smallest column and then the smallest row; -1 in an image
+    without a site.  host_boundary_dist2 and rnc.interp's hole fill use it.  The kernels' algorithm (csrc/dist_transform.cuh)
+    in numpy, every row of the batch at once: the nearest site in each column (the upper one on a tie), then along each row
+    the lower envelope of the parabolas q -> g(q)^2 + (x - q)^2 (Felzenszwalb and Huttenlocher), intersections compared by
+    cross-multiplying, and per pixel the leftmost parabola of least value."""
+    N, H, W = sites.shape
+    rows = np.empty((N, H, W), dtype=np.int64)
+    last = np.full((N, W), -1, dtype=np.int64)
     for y in range(H):
-        last = np.where(bnd[:, y], y, last)
-        g[:, y] = np.where(last >= 0, y - last, none)
-    nxt = np.full((B, W), -1, dtype=np.int64)
+        last = np.where(sites[:, y], y, last)
+        rows[:, y] = last
+    nxt = np.full((N, W), -1, dtype=np.int64)
     for y in range(H - 1, -1, -1):
-        nxt = np.where(bnd[:, y], y, nxt)
-        g[:, y] = np.where(nxt >= 0, np.minimum(g[:, y], nxt - y), g[:, y])
-    g = g.reshape(B * H, W)
-    R = B * H
+        nxt = np.where(sites[:, y], y, nxt)
+        r = rows[:, y]
+        rows[:, y] = np.where((nxt >= 0) & ((r < 0) | (nxt - y < y - r)), nxt, r)
+    R = N * H
+    rows = rows.reshape(R, W)
+    y_of = np.tile(np.arange(H, dtype=np.int64), N)[:, None]
     q_all = np.arange(W, dtype=np.int64)
-    F = np.where(g < none, g * g + q_all * q_all, -1)
+    F = np.where(rows >= 0, (y_of - rows) ** 2 + q_all * q_all, -1)
     v = np.zeros((R, W), dtype=np.int64)
     n = np.zeros(R, dtype=np.int64)
-    rows = np.arange(R)
+    idx_all = np.arange(R)
     for q in range(W):
         fq = F[:, q]
         popping = fq >= 0
         while True:
-            idx = rows[popping & (n > 1)]
+            idx = idx_all[popping & (n > 1)]
             if idx.size == 0:
                 break
             p, r = v[idx, n[idx] - 1], v[idx, n[idx] - 2]
@@ -443,23 +445,35 @@ def host_boundary_dist2(occ):
             pop = (fq[idx] - fp) * (p - r) <= (fp - fr) * (q - p)
             n[idx[pop]] -= 1
             popping[idx[~pop]] = False
-        push = rows[fq >= 0]
+        push = idx_all[fq >= 0]
         v[push, n[push]] = q
         n[push] += 1
-    out = np.full((R, W), DIST2_NONE, dtype=np.int64)
+    out = np.full((R, W), -1, dtype=np.int64)
     k = np.zeros(R, dtype=np.int64)
-    some = rows[n > 0]
+    some = idx_all[n > 0]
     for x in range(W):
-        while True:                 # move on to the next parabola while x is at or past where it takes over
+        while True:                 # move on to the next parabola while it is strictly below the current one at x
             idx = some[k[some] + 1 < n[some]]
             a, c = v[idx, k[idx]], v[idx, k[idx] + 1]
-            step = 2 * x * (c - a) >= F[idx, c] - F[idx, a]
+            step = 2 * x * (c - a) > F[idx, c] - F[idx, a]
             if not step.any():
                 break
             k[idx[step]] += 1
         q = v[some, k[some]]
-        out[some, x] = F[some, q] - q * q + (x - q) * (x - q)
-    return torch.from_numpy(out.reshape(B, H, W).astype(np.int32))
+        out[some, x] = rows[some, q] * W + q
+    return out.reshape(N, H, W)
+
+
+def host_boundary_dist2(occ):
+    """boundary_dist2 in numpy int64, exact: the squared distance from each pixel to its nearest boundary pixel (nearest_site,
+    the kernels' separable transform)."""
+    lab = (occ.detach().cpu().float() >= 0.5).numpy()
+    B, H, W = lab.shape
+    site = nearest_site(_boundary(lab))
+    y = np.arange(H, dtype=np.int64).reshape(1, H, 1)
+    x = np.arange(W, dtype=np.int64).reshape(1, 1, W)
+    d2 = (y - site // W) ** 2 + (x - site % W) ** 2
+    return torch.from_numpy(np.where(site >= 0, d2, DIST2_NONE).astype(np.int32))
 
 
 def region_partials(flow, gt, valid=None, occ=None, noc=None, fg=None):

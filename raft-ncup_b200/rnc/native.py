@@ -156,10 +156,16 @@ SIGNATURES = {
     "rnc_region_metrics": (_i, [_i, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 3,
                                 _vp, *[C.c_longlong] * 3, _vp, _vp, *[C.c_longlong] * 3, _i, _i, _i, _vp, _vp, _vp,
                                 C.c_size_t, _vp]),
+    "rnc_interpolate_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
+    "rnc_interpolate": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp,
+                             *[C.c_longlong] * 4, _vp, _vp, C.POINTER(_f), _i, _i, _i, _i, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_interp_error_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "rnc_interp_error": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind
 REGION_CELLS = {REGIONS_SINTEL: 32, REGIONS_KITTI: 4}
+INTERP_MAX_TIMES = 64                                      # RNC_INTERP_MAX_TIMES
 
 _lib = None
 _lock = threading.Lock()
