@@ -15,6 +15,7 @@ from . import native
 from .engine import fold_bn
 from .engine_umma import HX_LD, SplitBuf, UmmaWeights
 from .native import rnc
+from .slot_plan import CARRY, NEW, SAVED, images, runs, slot_plan
 
 EPS = 1e-5
 
@@ -167,156 +168,67 @@ class EncoderRunner:
         return bufs.dims[2]
 
     # ------------------------------------------------------------------ public
-    def run(self, model, ws, image1, image2):
-        """image1/image2: raw [B,3,H,W] fp32 in 0..255 (the stem normalises).  Fills ws.f1_cl, ws.f2_pyr (level 0), ws.h,
-        ws.hx[:, :256]; the caller finishes the pyramid."""
+    def run(self, model, ws, image1, image2, plan=None, saved=None):
+        """One encoder call of rnc.slot_plan's `plan` (None: the pair plan, fnet on both frames and cnet on frame 1).
+        image1/image2: raw [B,3,H,W] fp32 in 0..255 (the stem normalises).  Fills the slots' rows of ws.f1_cl, level 0 of
+        ws.f2_pyr, ws.h and ws.hx[:, :256], then finishes the pyramid and the halves.  saved: (h, hx hi, hx lo) rows of the
+        plan's `save` slots, restored into the slots that take a saved context and then refilled with this call's."""
         eng, E = self.eng, native
         B, _, Hin, Win = image1.shape
         dev = image1.device
-        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
-        bufs = self.buffers(dev, 2 * B, Hin, Win)
-        # ---- fnet on both frames (extractor.py:168-172 concatenates them along the batch)
-        both = torch.cat([image1, image2], 0).contiguous()
-        h8, w8, _ = self._trunk(pf, bufs, both, 2 * B, Hin, Win)
-        P = h8 * w8
-        eng.alloc_fmaps(ws, B, 256, h8, w8, 4, dev)
-        xs = bufs.XS[2]
-        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f1_cl.data_ptr(), ldo_f32=256)
-        # the second half of the batch inside the split planes
-        eng.uconv(B, h8, w8, (xs.hi[B * P:].data_ptr(), xs.lo[B * P:].data_ptr()), 128, 128, pf.head, E.EPI_LINEAR,
-                  out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
-        self._context(pc, bufs, ws, image1, h8, w8)
-        return h8, w8
-
-    def _context(self, pc, bufs, ws, image1, h8, w8):
-        """cnet on frame 1 -> ws.h, ws.hx[:, :256]."""
-        B, _, Hin, Win = image1.shape
-        self._trunk(pc, bufs, image1.contiguous(), B, Hin, Win)
-        ws.gru_const_valid = False                              # inp changes: the GRU's hoisted share must be recomputed
-        self.eng.uconv(B, h8, w8, bufs.XS[2].ptrs(), 128, 128, pc.head, native.EPI_TANH_RELU, out_f32=ws.h.data_ptr(),
-                       ldo_f32=128, out_split=ws.hx.ptrs(), ldo_split=HX_LD)
-
-    def run_bidirectional(self, model, ws, image1, image2):
-        """The encoders of the bidirectional pass (rnc.model.BidirectionalStage) on a workspace of 2B slots: fnet on the 2B
-        frames cat(image1, image2), in the encoder buffers of an ordinary B-pair forward; its head writes ws.f1_cl for all 2B
-        slots in frame order, and two device-to-device copies of the halves give level 0 of ws.f2_pyr (slot j: image2[j],
-        slot B + j: image1[j]).  cnet on the same 2B frames -> ws.h, ws.hx[:, :256].  The caller finishes the pyramid."""
-        eng, E = self.eng, native
-        B, _, Hin, Win = image1.shape
-        dev = image1.device
-        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
-        bufs = self.buffers(dev, 2 * B, Hin, Win)
-        both = torch.cat([image1, image2], 0).contiguous()
-        h8, w8, _ = self._trunk(pf, bufs, both, 2 * B, Hin, Win)
-        eng.alloc_fmaps(ws, 2 * B, 256, h8, w8, 4, dev)
-        eng.uconv(2 * B, h8, w8, bufs.XS[2].ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f1_cl.data_ptr(), ldo_f32=256)
-        n = B * h8 * w8 * 256                               # elements of one half's feature maps
-        f1 = ws.f1_cl.view(-1)
-        ws.f2_pyr[:n].copy_(f1[n:])
-        ws.f2_pyr[n:2 * n].copy_(f1[:n])
-        self._context(pc, bufs, ws, both, h8, w8)
-        return h8, w8
-
-    def run_step(self, model, ws, image1, image2, carry, restart):
-        """One step of sequence inference (rnc.model.SequenceStage): like run, but frame 1 of the `carry` slots is the last
-        step's frame 2, whose features are still level 0 of ws.f2_pyr (and of ws.f2h, the tensor-core lookup's halves): they
-        are copied into those slots' rows of ws.f1_cl / ws.f1h, then fnet runs on cat(image2 of every slot, image1 of the
-        `restart` slots) and its head writes level 0 of f2_pyr for all slots and the f1_cl rows of the restarted ones.  Slots
-        in neither list keep their f1 rows (an idle slot recomputes its last pair).  The caller converts only the restarted
-        slots' f1 rows to halves (finish_fmaps(ws, f1_slots=restart))."""
-        eng, E = self.eng, native
-        B, _, Hin, Win = image1.shape
-        dev = image1.device
-        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
-        bufs = self.buffers(dev, 2 * B, Hin, Win)         # the size of an ordinary forward's: no reallocation as R varies
-        h8, w8, _ = bufs.dims[2]
-        n = h8 * w8 * 256                                   # elements of one slot's feature map
-        eng.alloc_fmaps(ws, B, 256, h8, w8, 4, dev)
-        f1, halves = ws.f1_cl.view(-1), eng.lookup_mode == "umma"
-        for j0, k in _runs(carry):                          # before the fnet head overwrites level 0
-            f1[j0 * n:(j0 + k) * n].copy_(ws.f2_pyr[j0 * n:(j0 + k) * n])
-            if halves:
-                ws.f1h[j0 * n:(j0 + k) * n].copy_(ws.f2h[j0 * n:(j0 + k) * n])
-        both = torch.cat([image2] + [image1[j:j + 1] for j in restart]) if restart else image2
-        self._trunk(pf, bufs, both.contiguous(), B + len(restart), Hin, Win)
-        xs = bufs.XS[2]
-        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
-        for r, j in enumerate(restart):
-            i = (B + r) * h8 * w8                           # image B + r inside the 128-channel split planes
-            eng.uconv(1, h8, w8, (xs.hi[i:].data_ptr(), xs.lo[i:].data_ptr()), 128, 128, pf.head, E.EPI_LINEAR,
-                      out_f32=f1[j * n:].data_ptr(), ldo_f32=256)
-        self._context(pc, bufs, ws, image1, h8, w8)
-        return h8, w8
-
-    def run_bidirectional_step(self, model, ws, image1, image2, carry, restart, ctx):
-        """One step of bidirectional sequence inference (rnc.model.BidirectionalSequenceStage) on a workspace of 2B slots:
-        slot j holds the forward pair (image1[j], image2[j]), slot B + j the backward pair (image2[j], image1[j]).  For the
-        `carry` slots, frame 1 of the forward pair is the last step's frame 2, whose features are still level 0 of
-        ws.f2_pyr: they are copied into slot j's rows of ws.f1_cl / ws.f1h and into level 0 of slot B + j.  Then fnet runs on
-        cat(image2 of every slot, image1 of the `restart` slots), the images run_step encodes; its head writes level 0 of
-        f2_pyr for slots 0..B-1, a copy of those gives the f1_cl rows of slots B..2B-1, and a restarted slot's own frame 1
-        fills its f1_cl rows and level 0 of slot B + j.  cnet runs on the same B + R images: image2 is the context of the
-        backward slots, a restarted slot's image1 that of its forward slot, and a carried forward slot takes the last step's
-        backward context from ctx (h, hi, lo: [B*H8*W8, 128] fp32 and two [B*H8*W8, 256] fp16, the stage's buffer), which
-        is then refilled with this step's.  Slots in neither list keep their forward f1 rows and backward f2 level 0 (an idle
-        slot recomputes its last pair; its forward context is left as it is and its results are dropped).  The caller
-        converts the f1 rows of the restarted forward slots and of every backward slot to halves."""
-        eng, E = self.eng, native
-        B, _, Hin, Win = image1.shape
-        dev = image1.device
-        pf, pc = self.packed(model.fnet), self.packed(model.cnet)
-        bufs = self.buffers(dev, 2 * B, Hin, Win)         # B + R <= 2B images: an ordinary forward's buffers
+        plan = plan or slot_plan(B)
+        S = len(plan.f1)
+        bufs = self.buffers(dev, 2 * B, Hin, Win)         # fnet_in and cnet_in have at most 2B images
         h8, w8, _ = bufs.dims[2]
         P = h8 * w8
         n = P * 256                                         # elements of one slot's feature map
-        eng.alloc_fmaps(ws, 2 * B, 256, h8, w8, 4, dev)
-        f1, halves = ws.f1_cl.view(-1), eng.lookup_mode == "umma"
-        for j0, k in _runs(carry):                          # before the fnet head overwrites level 0
-            src = ws.f2_pyr[j0 * n:(j0 + k) * n]
-            f1[j0 * n:(j0 + k) * n].copy_(src)
-            ws.f2_pyr[(B + j0) * n:(B + j0 + k) * n].copy_(src)
-            if halves:
-                ws.f1h[j0 * n:(j0 + k) * n].copy_(ws.f2h[j0 * n:(j0 + k) * n])
-        both = (torch.cat([image2] + [image1[j:j + 1] for j in restart]) if restart else image2).contiguous()
-        self._trunk(pf, bufs, both, B + len(restart), Hin, Win)
+        eng.alloc_fmaps(ws, S, 256, h8, w8, 4, dev)
+        fmap = {"f1": ws.f1_cl.view(-1), "f2": ws.f2_pyr}
+        # carried features are level 0 of the last call's f2: copy them before the fnet head overwrites it
+        for name in ("f1", "f2"):
+            for j, kind, s, k in runs(getattr(plan, name)):
+                if kind == CARRY:
+                    fmap[name][j * n:(j + k) * n].copy_(ws.f2_pyr[s * n:(s + k) * n])
+                    if name == "f1" and eng.lookup_mode == "umma":
+                        ws.f1h[j * n:(j + k) * n].copy_(ws.f2h[s * n:(s + k) * n])
+        frames = (image1, image2)
+        x = images(frames, plan.fnet_in)
+        pf = self.packed(model.fnet)
+        self._trunk(pf, bufs, x, len(plan.fnet_in), Hin, Win)
         xs = bufs.XS[2]
-        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pf.head, E.EPI_LINEAR, out_f32=ws.f2_pyr.data_ptr(), ldo_f32=256)
-        f1[B * n:2 * B * n].copy_(ws.f2_pyr[:B * n])
-        for r, j in enumerate(restart):
-            i = (B + r) * P                                 # image B + r inside the 128-channel split planes
-            eng.uconv(1, h8, w8, (xs.hi[i:].data_ptr(), xs.lo[i:].data_ptr()), 128, 128, pf.head, E.EPI_LINEAR,
-                      out_f32=f1[j * n:].data_ptr(), ldo_f32=256)
-            ws.f2_pyr[(B + j) * n:(B + j + 1) * n].copy_(f1[j * n:(j + 1) * n])
-        # ---- cnet on the same images
-        self._trunk(pc, bufs, both, B + len(restart), Hin, Win)
-        ws.gru_const_valid = False                          # inp changes: the GRU's hoisted share must be recomputed
+        written = {}                                        # fnet image -> (feature map, slot) it was first written to
+        for name in ("f1", "f2"):
+            for j, kind, i, k in runs(getattr(plan, name)):
+                if kind != NEW:
+                    continue
+                # an image already written in this call is copied from there (encoded once); the others go through the head
+                for t, src, s, m in runs([written.get(i + t, (None, i + t)) for t in range(k)]):
+                    out = fmap[name][(j + t) * n:(j + t + m) * n]
+                    if src is None:
+                        eng.uconv(m, h8, w8, (xs.hi[s * P:].data_ptr(), xs.lo[s * P:].data_ptr()), 128, 128, pf.head,
+                                  E.EPI_LINEAR, out_f32=out.data_ptr(), ldo_f32=256)
+                        written.update((s + u, (name, j + t + u)) for u in range(m))
+                    else:
+                        out.copy_(fmap[src][s * n:(s + m) * n])
+        pc = self.packed(model.cnet)
+        self._trunk(pc, bufs, x if plan.cnet_in == plan.fnet_in else images(frames, plan.cnet_in), len(plan.cnet_in),
+                    Hin, Win)
         xs = bufs.XS[2]
         hx_hi, hx_lo = ws.hx.hi[:, :256], ws.hx.lo[:, :256]
-        eng.uconv(B, h8, w8, xs.ptrs(), 128, 128, pc.head, E.EPI_TANH_RELU, out_f32=ws.h[B * P:].data_ptr(), ldo_f32=128,
-                  out_split=(ws.hx.hi[B * P:].data_ptr(), ws.hx.lo[B * P:].data_ptr()), ldo_split=HX_LD)
-        for r, j in enumerate(restart):
-            i = (B + r) * P
-            eng.uconv(1, h8, w8, (xs.hi[i:].data_ptr(), xs.lo[i:].data_ptr()), 128, 128, pc.head, E.EPI_TANH_RELU,
-                      out_f32=ws.h[j * P:].data_ptr(), ldo_f32=128,
-                      out_split=(ws.hx.hi[j * P:].data_ptr(), ws.hx.lo[j * P:].data_ptr()), ldo_split=HX_LD)
-        ch, chi, clo = ctx
-        for j0, k in _runs(carry):
-            rows = slice(j0 * P, (j0 + k) * P)
-            ws.h[rows].copy_(ch[rows])
-            hx_hi[rows].copy_(chi[rows])
-            hx_lo[rows].copy_(clo[rows])
-        ch.copy_(ws.h[B * P:])
-        chi.copy_(hx_hi[B * P:])
-        clo.copy_(hx_lo[B * P:])
-        return h8, w8
+        for j, kind, i, k in runs(plan.ctx):
+            if kind == NEW:
+                eng.uconv(k, h8, w8, (xs.hi[i * P:].data_ptr(), xs.lo[i * P:].data_ptr()), 128, 128, pc.head,
+                          E.EPI_TANH_RELU, out_f32=ws.h[j * P:].data_ptr(), ldo_f32=128,
+                          out_split=(ws.hx.hi[j * P:].data_ptr(), ws.hx.lo[j * P:].data_ptr()), ldo_split=HX_LD)
+            elif kind == SAVED:
+                rows, src = slice(j * P, (j + k) * P), slice((i - plan.save.start) * P, (i + k - plan.save.start) * P)
+                for buf, sv in zip((ws.h, hx_hi, hx_lo), saved):
+                    buf[rows].copy_(sv[src])
+        if plan.save:
+            rows = slice(plan.save.start * P, plan.save.stop * P)
+            for buf, sv in zip((ws.h, hx_hi, hx_lo), saved):
+                sv.copy_(buf[rows])
+        ws.gru_const_valid = False                          # inp changed: the GRU's hoisted share must be recomputed
+        f1_slots = [j for j, s in enumerate(plan.f1) if s is not None and s[0] == NEW]
+        eng.finish_fmaps(ws, f1_slots=None if len(f1_slots) == S else f1_slots)
 
-
-def _runs(slots):
-    """Sorted slot indices -> (first, count) of each run of consecutive ones: one copy per run."""
-    out = []
-    for j in sorted(slots):
-        if out and out[-1][0] + out[-1][1] == j:
-            out[-1][1] += 1
-        else:
-            out.append([j, 1])
-    return out

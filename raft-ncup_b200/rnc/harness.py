@@ -349,11 +349,6 @@ def _sequence_workspace(eng, model, dev, slots, im1):
     return eng.WS(dev, slots, im1.shape[2] // 8, im1.shape[3] // 8, pk.has_mask, model.ncup)
 
 
-def _assign_slots(stage, step):
-    stage.restart = [j for j, c in enumerate(step) if c.restart]
-    stage.carry = [j for j, c in enumerate(step) if not c.restart and not c.idle]
-
-
 @torch.no_grad()
 def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
                   return_confidence=False):
@@ -363,40 +358,54 @@ def run_sequences(model, sequences, iters=32, warm_start=False, batch_size=8, mo
     model): yields (seq_index, pair_index, flow, confidence), the upsampler's output confidence unpadded like the flow.
 
     Slots run in lockstep (sequence_schedule).  Each step encodes only new frames: a continuing slot's frame 1 is its last
-    frame 2, whose fnet features are handed over on the device (rnc.model.SequenceStage).  With warm_start, a slot starts
-    from forward_interpolate of its own previous low-resolution flow, and from zero (a cold start) at pair 0.  The steps
-    run eagerly and never wait for the host; the caller moves or writes the flows."""
+    frame 2, whose fnet features are handed over on the device (rnc.slot_plan).  With warm_start, a slot starts from
+    forward_interpolate of its own previous low-resolution flow, and from zero (a cold start) at pair 0.  The steps run
+    eagerly and never wait for the host; the caller moves or writes the flows."""
     steps, padder = _sequence_setup(sequences, batch_size, mode, model, return_confidence)
     if not steps:
         return
+    for step, _, flow_up, conf in _sequence_steps(model, sequences, steps, padder, iters, warm_start, device,
+                                                  return_confidence, False):
+        for j, c in enumerate(step):
+            if not c.idle:
+                if return_confidence:
+                    yield c.seq, c.pair, padder.unpad(flow_up[j]), padder.unpad(conf[j])
+                else:
+                    yield c.seq, c.pair, padder.unpad(flow_up[j])
+
+
+@torch.no_grad()
+def _sequence_steps(model, sequences, steps, padder, iters, warm_start, device, return_confidence, bidirectional):
+    """The step loop of run_sequences (B slots) and, with bidirectional, of run_sequences_bidirectional (2B slots, slot
+    B + j the backward pair of slot j).  Yields (step, flow_low, flow_up, confidence or None) of each step, every slot,
+    padded.  A step is _forward_eager with the step's slot plan on the generator's own workspace; with warm_start the next
+    step starts from this one's flow_low (forward_interpolate, or bidirectional_warm_start), a restarted slot from zero."""
     from .engine import _Timed
-    from .model import SequenceStage
+    from .model import EncoderStage
+    from .slot_plan import slot_plan
     model.eval()
-    stage = SequenceStage(model)
+    stage = EncoderStage(model)
+    B = len(steps[0])
     ws = fi = zero = None
     for step in steps:
         im1, im2 = _step_images(sequences, step, device, padder)
         if ws is None:
             dev, eng = _sequence_engine(model, im1)
-        _assign_slots(stage, step)
+        restart = [j for j, c in enumerate(step) if c.restart]
+        stage.plan = slot_plan(B, [j for j, c in enumerate(step) if not c.restart and not c.idle], restart, bidirectional)
         with torch.cuda.device(dev), eng.lock:
             if ws is None:
-                ws = _sequence_workspace(eng, model, dev, len(step), im1)
-            for j in stage.restart if fi is not None else ():
-                fi[j].copy_(zero)           # cold start: coords0 + 0.0 is exactly coords0, as with flow_init=None
+                ws = _sequence_workspace(eng, model, dev, (2 if bidirectional else 1) * B, im1)
+            for j in restart if fi is not None else ():
+                fi[j::B].copy_(zero)        # rows j (and B + j): a cold start, coords0 + 0.0 is exactly coords0
             flow_low, flow_up, *conf = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws,
                                                             return_confidence=return_confidence)
             if warm_start:
                 with _Timed(eng, "warm_start"):
-                    fi = forward_interpolate(flow_low)
+                    fi = bidirectional_warm_start(flow_low) if bidirectional else forward_interpolate(flow_low)
                 if zero is None:
-                    zero = torch.zeros_like(fi[0])
-        for j, c in enumerate(step):
-            if not c.idle:
-                if return_confidence:
-                    yield c.seq, c.pair, padder.unpad(flow_up[j]), padder.unpad(conf[0][j])
-                else:
-                    yield c.seq, c.pair, padder.unpad(flow_up[j])
+                    zero = torch.zeros_like(fi[0::B])
+        yield step, flow_low, flow_up, (conf[0] if return_confidence else None)
 
 
 def bidirectional_warm_start(flow_low):
@@ -434,7 +443,7 @@ def run_sequences_bidirectional(model, sequences, iters=32, warm_start=False, ba
     Slots run in lockstep as in run_sequences (sequence_schedule), on a workspace of 2B slots: slot j holds a sequence's
     forward pair, slot B + j its backward pair.  fnet and cnet encode each new frame once per step: a frame's features
     and context serve the backward pair that starts at it and, one step later, the forward pair that starts at it
-    (rnc.model.BidirectionalSequenceStage).  Each step checks consistency on both directions in one launch
+    (rnc.slot_plan).  Each step checks consistency on both directions in one launch
     (rnc.metrics.fb_consistency with alpha1, alpha2) and computes both warm starts in one launch; the steps never wait for
     the host.  Inference only: with grad enabled on a model that requires grad it raises ValueError."""
     steps, padder = _sequence_setup(sequences, batch_size, mode, model, return_confidence)
@@ -443,39 +452,13 @@ def run_sequences_bidirectional(model, sequences, iters=32, warm_start=False, ba
     if model._needs_grad():
         raise ValueError("run_sequences_bidirectional is inference only: call it under torch.no_grad() (training through the "
                          "bidirectional pass is not built)")
-    yield from _bidirectional_steps(model, sequences, steps, padder, iters, warm_start, device, return_confidence, alpha1,
-                                    alpha2)
-
-
-@torch.no_grad()
-def _bidirectional_steps(model, sequences, steps, padder, iters, warm_start, device, return_confidence, alpha1, alpha2):
-    from .engine import _Timed
     from .metrics import fb_consistency
-    from .model import BidirectionalSequenceStage
-    model.eval()
-    stage = BidirectionalSequenceStage(model)
     B = len(steps[0])
-    ws = fi = zero = None
-    for step in steps:
-        im1, im2 = _step_images(sequences, step, device, padder)
-        if ws is None:
-            dev, eng = _sequence_engine(model, im1)
-        _assign_slots(stage, step)
-        with torch.cuda.device(dev), eng.lock:
-            if ws is None:
-                ws = _sequence_workspace(eng, model, dev, 2 * B, im1)
-            for j in stage.restart if fi is not None else ():
-                fi[j::B].copy_(zero)        # rows j and B + j: a cold start in both directions
-            flow_low, flow_up, *conf = model._forward_eager(eng, im1, im2, iters, fi, True, encode=stage, ws=ws,
-                                                            return_confidence=return_confidence)
-            up = padder.unpad(flow_up)
-            occ, occ_bw, err, err_bw = fb_consistency(up[:B], up[B:], alpha1, alpha2)
-            if warm_start:
-                with _Timed(eng, "warm_start"):
-                    fi = bidirectional_warm_start(flow_low)
-                if zero is None:
-                    zero = torch.zeros_like(fi[0::B])
-        conf = padder.unpad(conf[0]) if return_confidence else None
+    for step, flow_low, flow_up, conf in _sequence_steps(model, sequences, steps, padder, iters, warm_start, device,
+                                                         return_confidence, True):
+        up = padder.unpad(flow_up)
+        occ, occ_bw, err, err_bw = fb_consistency(up[:B], up[B:], alpha1, alpha2)
+        conf = padder.unpad(conf) if return_confidence else None
         for j, c in enumerate(step):
             if c.idle:
                 continue

@@ -14,6 +14,7 @@ import torch.nn as nn
 from .engine import _Timed, _require_cuda, engine_for, module_device, module_tensors
 from .modules import BasicEncoder, BasicUpdateBlock, get_upsampler
 from .native import rnc
+from .slot_plan import CARRY, NEW, images, runs, slot_plan
 
 
 class _RAFTBase(nn.Module):
@@ -96,10 +97,11 @@ class _RAFTBase(nn.Module):
                        return_confidence=False):
         """The iteration loop on the engine's resident buffers.  upsample(eng, ws, pu) produces each full-resolution prediction
         from the workspace; the default is the inference upsampler (self._upsample on packed weights).  encode(eng, ws, image1,
-        image2) fills the feature maps and the GRU state; the default encodes both frames (self._encode).  ws: a workspace the
-        caller owns instead of the engine's shared one of this shape; with an encode that fills more slots than the images'
-        batch (BidirectionalStage), flow_init is [ws.B,2,H/8,W/8].  return_confidence: upsample(eng, ws, pu, True) returns
-        (flow, confidence), and the forward returns the confidences next to the flows (forward's return_confidence)."""
+        image2) fills the feature maps and the GRU state; the default is EncoderStage's pair plan (fnet on both frames, cnet on
+        frame 1).  ws: a workspace the caller owns instead of the engine's shared one of this shape; with an encode that fills
+        more slots than the images' batch (the bidirectional plan), flow_init is [ws.B,2,H/8,W/8].  return_confidence:
+        upsample(eng, ws, pu, True) returns (flow, confidence), and the forward returns the confidences next to the flows
+        (forward's return_confidence)."""
         B, _, Him, Wim = image1.shape
         H8, W8 = Him // 8, Wim // 8
         pk = eng.packed_update(self.update_block)
@@ -112,7 +114,7 @@ class _RAFTBase(nn.Module):
                                           "or eval mode: call .eval() / freeze_bn()")
         if ws is None:
             ws = eng.workspace(image1.device, B, H8, W8, pk.has_mask, self.ncup)
-        (encode or self._encode)(eng, ws, image1, image2)
+        (encode or EncoderStage(self))(eng, ws, image1, image2)
         fi = None
         if flow_init is not None:
             fi = flow_init.to(image1.device).float().contiguous()
@@ -185,43 +187,19 @@ class _RAFTBase(nn.Module):
 
     def _forward_bidirectional(self, eng, image1, image2, iters, flow_init, return_confidence=False):
         """The bidirectional pass on the engine: _forward_eager over 2B slots of the engine's workspace, slot j holding
-        (image1[j], image2[j]) and slot B + j (image2[j], image1[j]), encoded by BidirectionalStage.  flow_init: [2B,2,H/8,W/8]
-        or None."""
+        (image1[j], image2[j]) and slot B + j (image2[j], image1[j]), encoded by EncoderStage's bidirectional plan.  flow_init:
+        [2B,2,H/8,W/8] or None."""
         B, _, Him, Wim = image1.shape
         pk = eng.packed_update(self.update_block)
         ws = eng.workspace(image1.device, 2 * B, Him // 8, Wim // 8, pk.has_mask, self.ncup)
-        return self._forward_eager(eng, image1, image2, iters, flow_init, True, encode=BidirectionalStage(self), ws=ws,
+        return self._forward_eager(eng, image1, image2, iters, flow_init, True,
+                                   encode=EncoderStage(self, slot_plan(B, bidirectional=True)), ws=ws,
                                    return_confidence=return_confidence)
 
     def _umma_encoders(self, eng):
         """Do the encoders run on the tensor-core path (else on torch modules: RNC_ENCODER=cudnn, RNC_CONV=ffma, amp)?"""
         amp = bool(getattr(self.args, "mixed_precision", False))
         return eng.mode == "umma" and not amp and os.environ.get("RNC_ENCODER", "umma").lower() == "umma"
-
-    def _context(self, image1):
-        """cnet on the normalised frame 1 -> (tanh(net), relu(inp)) NCHW fp32 (raft_nc_dbl.py:137-140)."""
-        with torch.autocast("cuda", enabled=bool(getattr(self.args, "mixed_precision", False))):
-            cnet = self.cnet(image1)
-            net, inp = torch.split(cnet, [128, 128], dim=1)
-            net, inp = torch.tanh(net), torch.relu(inp)
-        return net.float().contiguous(), inp.float().contiguous()
-
-    def _encode(self, eng, ws, image1, image2):
-        """Encoder stage of a forward: fnet on both frames, cnet on frame 1 (raft_nc_dbl.py:118-140)."""
-        if self._umma_encoders(eng):
-            # encoders on the tensor-core path, writing straight into the resident buffers
-            with _Timed(eng, "encoders"):
-                eng.encoder().run(self, ws, image1.float().contiguous(), image2.float().contiguous())
-                eng.finish_fmaps(ws)
-            return
-        image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
-        image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
-        with torch.autocast("cuda", enabled=bool(getattr(self.args, "mixed_precision", False))):
-            fmap1, fmap2 = self.fnet([image1, image2])
-        fmap1, fmap2 = fmap1.float().contiguous(), fmap2.float().contiguous()
-        net, inp = self._context(image1)
-        eng.fmap_prepare(ws, fmap1, fmap2, 4)
-        eng.load_state(ws, net, inp)
 
     def _upsample(self, eng, ws, pu):
         raise NotImplementedError
@@ -310,129 +288,48 @@ def frozen_trunk(model, image1=None, image2=None, flow_init=None):
     return not getattr(model.args, "mixed_precision", False)
 
 
-class SequenceStage:
-    """Encoder stage of one step of sequence inference (rnc.harness.run_sequences), for _forward_eager(encode=...).
+class EncoderStage:
+    """Encoder stage of a forward, for _forward_eager(encode=...): runs `plan` (rnc.slot_plan; None: the pair plan) on the
+    tensor-core encoders (EncoderRunner.run) or on the torch modules (RNC_ENCODER=cudnn, RNC_CONV=ffma, mixed_precision).
+    The sequence drivers set `plan` before each step.  The object keeps what crosses calls: the saved context rows of the
+    tensor-core route, and the last call's NCHW fmap1 / fmap2 / net / inp of the torch route; the feature maps in the
+    workspace are the rest, so one stage belongs to one workspace."""
 
-    Slot j of the batch holds one pair of one sequence.  Before each call the driver sets `carry` (slots whose frame 1 is the
-    previous step's frame 2) and `restart` (slots that start a sequence: their frame 1 is new); every other slot is idle and
-    recomputes its previous pair.  fnet runs on frame 2 of every slot and frame 1 of the restarted ones only: fnet normalises
-    each image on its own (InstanceNorm), so a carried slot's frame-1 features are the previous step's frame-2 features.  cnet
-    runs on frame 1 of every slot.  The object keeps the state that carries between steps; the feature maps in the workspace
-    are the rest, so one stage belongs to one workspace."""
-
-    def __init__(self, model):
-        self.model = model
-        self.carry, self.restart = [], []
-        self.fmap1 = self.fmap2 = None          # torch-encoder route: NCHW features of the last step's frames
+    def __init__(self, model, plan=None):
+        self.model, self.plan = model, plan
+        self.saved = None       # tensor-core route: (h, hx hi, hx lo) rows of plan.save
+        self.rows = None        # torch route: (fmap1, fmap2, net, inp) of the last call
 
     def __call__(self, eng, ws, image1, image2):
         m = self.model
+        plan = self.plan or slot_plan(image1.shape[0])
         if m._umma_encoders(eng):
+            if plan.save and self.saved is None:
+                rows, dev = len(plan.save) * ws.H8 * ws.W8, image1.device
+                self.saved = (torch.empty(rows, 128, dtype=torch.float32, device=dev),
+                              torch.empty(rows, 256, dtype=torch.float16, device=dev),
+                              torch.empty(rows, 256, dtype=torch.float16, device=dev))
             with _Timed(eng, "encoders"):
-                eng.encoder().run_step(m, ws, image1.float().contiguous(), image2.float().contiguous(), self.carry, self.restart)
-                eng.finish_fmaps(ws, f1_slots=self.restart)
+                eng.encoder().run(m, ws, image1.float().contiguous(), image2.float().contiguous(), plan, self.saved)
             return
-        B = image1.shape[0]
-        image1 = (2 * (image1 / 255.0) - 1.0).contiguous()
-        image2 = (2 * (image2 / 255.0) - 1.0).contiguous()
-        new = torch.cat([image2] + [image1[j:j + 1] for j in self.restart]) if self.restart else image2
+        frames = (image1, image2)
+        x = (2 * (images(frames, plan.fnet_in) / 255.0) - 1.0).contiguous()
+        xc = x if plan.cnet_in == plan.fnet_in else (2 * (images(frames, plan.cnet_in) / 255.0) - 1.0).contiguous()
         with torch.autocast("cuda", enabled=bool(getattr(m.args, "mixed_precision", False))):
-            f = m.fnet(new)
-        f = f.float().contiguous()
-        if self.fmap1 is None:
-            self.fmap1 = torch.empty_like(f[:B])
-        for j in self.carry:
-            self.fmap1[j].copy_(self.fmap2[j])
-        for r, j in enumerate(self.restart):
-            self.fmap1[j].copy_(f[B + r])
-        self.fmap2 = f[:B]
-        net, inp = m._context(image1)
-        eng.fmap_prepare(ws, self.fmap1, self.fmap2, 4)
-        eng.load_state(ws, net, inp)
+            f = m.fnet(x)
+            net, inp = torch.split(m.cnet(xc), [128, 128], dim=1)      # raft_nc_dbl.py:137-140
+            net, inp = torch.tanh(net), torch.relu(inp)
+        f, net, inp = f.float().contiguous(), net.float().contiguous(), inp.float().contiguous()
+        last = self.rows or (None,) * 4
 
-
-class BidirectionalStage:
-    """Encoder stage of the bidirectional pass (_RAFTBase.forward_bidirectional), for _forward_eager(encode=...) on a
-    workspace of 2B slots: slot j holds the pair (image1[j], image2[j]), slot B + j the pair (image2[j], image1[j]).  fnet
-    runs once on the 2B frames cat(image1, image2), the images a one-directional forward encodes: its features are fmap1 of
-    the slots in frame order, and fmap2 with the two halves swapped.  cnet runs on the same 2B frames, so each direction gets
-    the context of its own first frame."""
-
-    def __init__(self, model):
-        self.model = model
-
-    def __call__(self, eng, ws, image1, image2):
-        m = self.model
-        if m._umma_encoders(eng):
-            with _Timed(eng, "encoders"):
-                eng.encoder().run_bidirectional(m, ws, image1.float().contiguous(), image2.float().contiguous())
-                eng.finish_fmaps(ws)
-            return
-        B = image1.shape[0]
-        both = torch.cat([image1, image2])
-        both = (2 * (both / 255.0) - 1.0).contiguous()
-        with torch.autocast("cuda", enabled=bool(getattr(m.args, "mixed_precision", False))):
-            f = m.fnet(both)
-        f = f.float().contiguous()
-        net, inp = m._context(both)
-        eng.fmap_prepare(ws, f, torch.cat([f[B:], f[:B]]), 4)
-        eng.load_state(ws, net, inp)
-
-
-class BidirectionalSequenceStage:
-    """Encoder stage of one step of bidirectional sequence inference (rnc.harness.run_sequences_bidirectional), for
-    _forward_eager(encode=...) on a workspace of 2B slots: slot j holds the forward pair (image1[j], image2[j]) of one
-    sequence, slot B + j the backward pair (image2[j], image1[j]).  `carry` and `restart` are set per step as for
-    SequenceStage.  fnet and cnet run on the B + R images cat(image2, image1 of the restarted slots): frame 2's features and
-    context serve the backward slots and frame 2 of the forward ones; a carried forward slot's frame 1 features are the last
-    step's frame 2 features and its context is the last step's backward context, which the stage keeps (cnet of frame k is
-    the context of both backward pair (k, k-1) and forward pair (k, k+1)).  One stage belongs to one workspace."""
-
-    def __init__(self, model):
-        self.model = model
-        self.carry, self.restart = [], []
-        self.ctx = None             # tensor-core route: the last step's backward context rows (h, hx hi, hx lo)
-        self.fmap1 = self.fmap2 = self.net = self.inp = None    # torch-encoder route: NCHW [2B,...] of the last step
-
-    def __call__(self, eng, ws, image1, image2):
-        m = self.model
-        B = image1.shape[0]
-        if m._umma_encoders(eng):
-            if self.ctx is None:
-                rows, dev = B * ws.H8 * ws.W8, image1.device
-                self.ctx = (torch.empty(rows, 128, dtype=torch.float32, device=dev),
-                            torch.empty(rows, 256, dtype=torch.float16, device=dev),
-                            torch.empty(rows, 256, dtype=torch.float16, device=dev))
-            with _Timed(eng, "encoders"):
-                eng.encoder().run_bidirectional_step(m, ws, image1.float().contiguous(), image2.float().contiguous(),
-                                                     self.carry, self.restart, self.ctx)
-                eng.finish_fmaps(ws, f1_slots=sorted(self.restart) + list(range(B, 2 * B)))
-            return
-        new = torch.cat([image2] + [image1[j:j + 1] for j in self.restart]) if self.restart else image2
-        new = (2 * (new / 255.0) - 1.0).contiguous()
-        with torch.autocast("cuda", enabled=bool(getattr(m.args, "mixed_precision", False))):
-            f = m.fnet(new)
-        f = f.float().contiguous()
-        net, inp = m._context(new)
-        if self.fmap1 is None:
-            self.fmap1, self.fmap2 = (f.new_empty((2 * B,) + f.shape[1:]) for _ in range(2))
-            self.net, self.inp = (net.new_empty((2 * B,) + net.shape[1:]) for _ in range(2))
-        for j in self.carry:        # frame k: the last step's frame 2 of the forward pair, frame 1 of the backward one
-            self.fmap1[j].copy_(self.fmap2[j])
-            self.fmap2[B + j].copy_(self.fmap2[j])
-            self.net[j].copy_(self.net[B + j])
-            self.inp[j].copy_(self.inp[B + j])
-        self.fmap2[:B].copy_(f[:B])
-        self.fmap1[B:].copy_(f[:B])
-        self.net[B:].copy_(net[:B])
-        self.inp[B:].copy_(inp[:B])
-        for r, j in enumerate(self.restart):
-            self.fmap1[j].copy_(f[B + r])
-            self.fmap2[B + j].copy_(f[B + r])
-            self.net[j].copy_(net[B + r])
-            self.inp[j].copy_(inp[B + r])
-        eng.fmap_prepare(ws, self.fmap1, self.fmap2, 4)
-        eng.load_state(ws, self.net, self.inp)
+        def rows(sources, new, prev):
+            """One field's S rows: views of this call's outputs and of the last call's rows, concatenated by runs."""
+            pieces = [{NEW: new, CARRY: last[1]}.get(kind, prev)[i:i + k] for _, kind, i, k in runs(sources)]
+            return pieces[0] if len(pieces) == 1 else torch.cat(pieces)
+        self.rows = (rows(plan.f1, f, last[0]), rows(plan.f2, f, last[1]), rows(plan.ctx, net, last[2]),
+                     rows(plan.ctx, inp, last[3]))
+        eng.fmap_prepare(ws, *self.rows[:2], 4)
+        eng.load_state(ws, *self.rows[2:])
 
 
 class _Dims:
