@@ -9,27 +9,23 @@
 // Every operation is a __*_rn intrinsic in the order rnc/metrics.py:host_fb_consistency writes it, so nothing is contracted
 // into an FMA and the host restatement gives the same bits.  One launch for both directions of B pairs (grid z), a thread per
 // pixel, no atomics and no host synchronisation; a pixel's outputs depend only on its own image.
-#include "rnc_common.cuh"
+#include "eval_common.cuh"
 
 namespace rnc {
 namespace {
 
 constexpr int kFbThreads = 256;
 
-struct FbFlow {
-  const float* p;
-  long long b, c, y, x;
-};
-
 struct FbArgs {
-  FbFlow flow[2];               // [0] forward, [1] backward
+  View flow[2];                 // [0] forward, [1] backward
   unsigned char* occ[2];
   float* err[2];
   int H, W;
   float alpha1, alpha2;
 };
 
-__device__ __forceinline__ float sample_at(const FbFlow& g, const float* base, int H, int W, int x, int y, int c) {
+// g's value at (x, y) of the image at base, 0 outside the frame
+__device__ __forceinline__ float sample_at(const View& g, const float* base, int H, int W, int x, int y, int c) {
   return (x >= 0 && x < W && y >= 0 && y < H) ? base[c * g.c + y * g.y + x * g.x] : 0.0f;
 }
 
@@ -40,10 +36,10 @@ __global__ void __launch_bounds__(kFbThreads) fb_consistency_kernel(FbArgs a) {
   const long long p = static_cast<long long>(blockIdx.x) * kFbThreads + threadIdx.x;
   if (p >= hw) return;
   const int v = static_cast<int>(p / W), u = static_cast<int>(p - static_cast<long long>(v) * W);
-  const FbFlow& f = a.flow[dir];
-  const FbFlow& g = a.flow[dir ^ 1];
-  const float* fp = f.p + b * f.b + v * f.y + u * f.x;
-  const float fu = fp[0], fv = fp[f.c];
+  const View& f = a.flow[dir];
+  const View& g = a.flow[dir ^ 1];
+  const float fu = f.at(b, 0, v, u), fv = f.at(b, 1, v, u);
+  const float* gb = g.pixel(b, 0, 0);
   const float px = __fadd_rn(static_cast<float>(u), fu), py = __fadd_rn(static_cast<float>(v), fv);
   const long long o = static_cast<long long>(b) * hw + p;
   if (!(px >= 0.0f && px <= static_cast<float>(W - 1) && py >= 0.0f && py <= static_cast<float>(H - 1))) {
@@ -56,7 +52,6 @@ __global__ void __launch_bounds__(kFbThreads) fb_consistency_kernel(FbArgs a) {
   const float bx = __fsub_rn(1.0f, ax), by = __fsub_rn(1.0f, ay);
   const float w00 = __fmul_rn(bx, by), w01 = __fmul_rn(ax, by), w10 = __fmul_rn(bx, ay), w11 = __fmul_rn(ax, ay);
   const int ix = static_cast<int>(x0), iy = static_cast<int>(y0);
-  const float* gb = g.p + b * g.b;
   float gs[2];
 #pragma unroll
   for (int c = 0; c < 2; ++c) {
@@ -75,12 +70,11 @@ __global__ void __launch_bounds__(kFbThreads) fb_consistency_kernel(FbArgs a) {
   a.occ[dir][o] = (!finite || lhs > rhs) ? 1 : 0;
 }
 
+// its own limits, wider than eval_shape_ok's: H*W < 2^31, and H, W < 2^24 so that every pixel coordinate is exact in float32
 bool shape_ok(int B, int H, int W) {
   return B > 0 && H > 0 && W > 0 && B <= 65535 && static_cast<long long>(H) * W < (1ll << 31) && H < (1 << 24) &&
          W < (1 << 24);
 }
-
-bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 
 }  // namespace
 }  // namespace rnc

@@ -15,12 +15,11 @@
 // contracted into an FMA and the host restatement gives the same bits.  No floating-point atomics: an output depends only on
 // its own image and time.
 //
-// rnc_interp_error: per image, the fp64 sum over its pixels of sum_c (pred - gt)^2 and its pixel count.  CTA (x, n) adds
-// 2048 pixels (a fixed xor-shuffle tree per warp, then its 8 warps in order) and a second kernel adds each image's CTAs in a
-// fixed order (a warp per image: lane-strided sums, then a fixed shuffle tree), as rnc_flow_metrics does: the order depends only
-// on H*W, so an image's sum does not depend on N, on its position in the batch or on the GPU.
+// rnc_interp_error: per image, the fp64 sum over its pixels of sum_c (pred - gt)^2 and its pixel count, by eval_common.cuh's
+// two fixed-order reductions, as rnc_flow_metrics: the order depends only on H*W, so an image's sum does not depend on N, on
+// its position in the batch or on the GPU.
 #include "dist_transform.cuh"
-#include "rnc_common.cuh"
+#include "eval_common.cuh"
 
 namespace rnc {
 namespace {
@@ -29,15 +28,9 @@ constexpr int kInterpThreads = 256;
 constexpr int kMaxTimes = RNC_INTERP_MAX_TIMES;
 constexpr unsigned long long kNoProposal = ~0ull;
 
-struct Planes {                         // an fp32 [B,C,H,W] tensor through element strides
-  const float* p;
-  long long b, c, y, x;
-  __device__ float at(int bi, int ci, int y_, int x_) const { return p[bi * b + ci * c + y_ * y + x_ * x]; }
-};
-
 struct InterpArgs {
-  Planes frame[2];                      // I0, I1
-  Planes flow[2];                       // F (0 -> 1), G (1 -> 0)
+  View frame[2];                        // I0, I1
+  View flow[2];                         // F (0 -> 1), G (1 -> 0)
   const unsigned char* occ[2];          // [B][H][W]: occ0 of F on frame 0, occ1 of G on frame 1
   unsigned long long* map;              // [B][T][H][W]
   int* site;                            // [B][T][H][W]
@@ -47,7 +40,7 @@ struct InterpArgs {
 };
 
 // frame c-plane at (px, py), bilinear with the coordinates clamped to [0, W-1] x [0, H-1]
-__device__ __forceinline__ float sample(const Planes& im, int b, int c, float px, float py, int H, int W) {
+__device__ __forceinline__ float sample(const View& im, int b, int c, float px, float py, int H, int W) {
   px = fminf(fmaxf(px, 0.0f), static_cast<float>(W - 1));
   py = fminf(fmaxf(py, 0.0f), static_cast<float>(H - 1));
   const float x0 = floorf(px), y0 = floorf(py);
@@ -70,7 +63,7 @@ __global__ void __launch_bounds__(kInterpThreads) interp_splat_kernel(InterpArgs
   if (p >= hw) return;
   if (a.occ[s][static_cast<long long>(b) * hw + p] != 0) return;
   const int y = p / W, x = p - y * W;
-  const Planes& f = a.flow[s];
+  const View& f = a.flow[s];
   const float fu = f.at(b, 0, y, x), fv = f.at(b, 1, y, x);
   if (!finite(fu) || !finite(fv)) return;
   // e = sum_c |I_other(x + f) - I_own(x)|, channels in order
@@ -144,52 +137,28 @@ __global__ void __launch_bounds__(kInterpThreads) interp_composite_kernel(Interp
   }
 }
 
-constexpr int kErrPerThread = 8;
-constexpr int kErrPerCta = kInterpThreads * kErrPerThread;
-constexpr int kErrWarps = kInterpThreads / 32;
-
-__global__ void __launch_bounds__(kInterpThreads) interp_error_part_kernel(Planes pred, Planes gt, int H, int W,
-                                                                           double* __restrict__ parts) {
-  const int n = blockIdx.y, hw = H * W;
-  double sum = 0.0;
-  for (int p = blockIdx.x * kErrPerCta + threadIdx.x, e = 0; e < kErrPerThread && p < hw; ++e, p += kInterpThreads) {
-    const int y = p / W, x = p - y * W;
+struct SquaredError {                   // sum_c (pred - gt)^2 in fp64, channels in order
+  View pred, gt;
+  __device__ void operator()(double& acc, int n, int y, int x) const {
     double d2 = 0.0;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const double d = __dsub_rn(static_cast<double>(pred.at(n, c, y, x)), static_cast<double>(gt.at(n, c, y, x)));
       d2 = c == 0 ? __dmul_rn(d, d) : __dadd_rn(d2, __dmul_rn(d, d));
     }
-    sum += d2;
+    acc += d2;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  __shared__ double ssum[kErrWarps];
-  if ((threadIdx.x & 31) == 0) ssum[threadIdx.x >> 5] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double out = 0.0;
-    for (int w = 0; w < kErrWarps; ++w) out += ssum[w];
-    parts[static_cast<long long>(n) * gridDim.x + blockIdx.x] = out;
-  }
-}
+};
 
-// a warp per image: parts [N][nblk] -> sq_sum [N], count [N]
-__global__ void __launch_bounds__(kInterpThreads) interp_error_reduce_kernel(const double* __restrict__ parts, int N, int nblk,
-                                                                             long long hw, double* __restrict__ sq_sum,
-                                                                             long long* __restrict__ count) {
-  const int n = blockIdx.x * kErrWarps + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (n >= N) return;
-  double sum = 0.0;
-  for (int k = lane; k < nblk; k += 32) sum += parts[static_cast<long long>(n) * nblk + k];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
-  if (lane == 0) {
-    sq_sum[n] = sum;
+struct ErrorStore {                     // image n -> sq_sum [n], count [n] = H*W
+  double* sq_sum;
+  long long* count;
+  long long hw;
+  __device__ void operator()(int n, double v) const {
+    sq_sum[n] = v;
     count[n] = hw;
   }
-}
+};
 
 bool interp_shape_ok(int B, int T, int H, int W) {
   return B > 0 && T > 0 && T <= kMaxTimes && H > 0 && W > 0 && H <= kSiteMaxSide && W <= kSiteMaxSide &&
@@ -199,14 +168,6 @@ bool interp_shape_ok(int B, int T, int H, int W) {
 size_t map_bytes(int B, int T, int H, int W) {
   return static_cast<size_t>(B) * T * H * W * sizeof(unsigned long long);
 }
-
-bool error_shape_ok(int N, int H, int W) {
-  return N > 0 && H > 0 && W > 0 && N <= 65535 && static_cast<long long>(H) * W < (1ll << 30);
-}
-
-int error_blocks(int H, int W) { return (H * W + kErrPerCta - 1) / kErrPerCta; }
-
-bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 
 }  // namespace
 }  // namespace rnc
@@ -256,27 +217,24 @@ int rnc_interpolate(const float* frame0, long long ab, long long ac, long long a
 }
 
 size_t rnc_interp_error_workspace_bytes(int N, int H, int W) {
-  return error_shape_ok(N, H, W) ? static_cast<size_t>(N) * error_blocks(H, W) * sizeof(double) : 0;
+  return eval_shape_ok(N, H, W) ? static_cast<size_t>(N) * eval_blocks(H, W) * sizeof(double) : 0;
 }
 
 int rnc_interp_error(const float* pred, long long pb, long long pc, long long py, long long px, const float* gt, long long gb,
                      long long gc, long long gy, long long gx, int N, int H, int W, double* sq_sum, long long* count,
                      void* workspace, size_t workspace_bytes, void* stream) {
-  if (!error_shape_ok(N, H, W)) return RNC_ERR_BAD_SHAPE;
+  if (!eval_shape_ok(N, H, W)) return RNC_ERR_BAD_SHAPE;
   if (!pred || !gt || !sq_sum || !count || !workspace) return RNC_ERR_BAD_POINTER;
   if (!aligned(pred, 4) || !aligned(gt, 4) || !aligned(sq_sum, 8) || !aligned(count, 8) || !aligned(workspace, 16))
     return RNC_ERR_BAD_POINTER;
   if (workspace_bytes < rnc_interp_error_workspace_bytes(N, H, W)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
-  const int nblk = error_blocks(H, W);
+  const int nblk = eval_blocks(H, W);
   double* parts = static_cast<double*>(workspace);
-  interp_error_part_kernel<<<dim3(nblk, N), kInterpThreads, 0, s>>>(Planes{pred, pb, pc, py, px}, Planes{gt, gb, gc, gy, gx},
-                                                                     H, W, parts);
+  cta_partials_kernel<<<dim3(nblk, N), kEvalThreads, 0, s>>>(SquaredError{{pred, pb, pc, py, px}, {gt, gb, gc, gy, gx}}, H, W,
+                                                              parts);
   if (int st = after_launch()) return st;
-  interp_error_reduce_kernel<<<(N + kErrWarps - 1) / kErrWarps, kInterpThreads, 0, s>>>(parts, N, nblk,
-                                                                                       static_cast<long long>(H) * W, sq_sum,
-                                                                                       count);
-  return after_launch();
+  return launch_image_reduce(parts, N, nblk, 1, ErrorStore{sq_sum, count, static_cast<long long>(H) * W}, s);
 }
 
 }  // extern "C"

@@ -9,15 +9,14 @@
 //
 // rnc_region_metrics: per image and per cell (one joint label of a pixel; Sintel 2 occlusion x 4 distance x 4 speed classes,
 // KITTI 2 noc x 2 fg) the five counts and the fp64 EPE sum of rnc_flow_metrics, from the same per-pixel float32 arithmetic
-// (pixel_metrics.cuh).  CTA (x, b) covers the 2048 pixels of image b that rnc_flow_metrics' CTA x covers.  Each warp takes its
-// 32 pixels at a time; for each cell present among them (a ballot loop) it counts with ballots and adds the members' EPE with
-// a fixed xor-shuffle tree (non-members add 0.0, which changes no sum), into the warp's own per-cell accumulator in shared
-// memory.  The CTA adds its 8 warps in order, and a second kernel adds each (image, cell)'s CTAs in a fixed order (a warp per
-// pair: lane-strided sums, then a fixed shuffle tree).  The order depends only on H*W and the cell count: an image's results
-// do not depend on B, on its position in the batch or on the GPU, and no floating-point atomics are used.
+// (eval_common.cuh's pixel_metrics).  CTA (x, b) covers the kEvalPerCta pixels of image b that rnc_flow_metrics' CTA x covers.
+// Each warp takes its 32 pixels at a time; for each cell present among them (a ballot loop) it counts with ballots and adds
+// the members' EPE with a fixed xor-shuffle tree (non-members add 0.0, which changes no sum), into the warp's own per-cell
+// accumulator in shared memory.  The CTA adds its warps in order, and eval_common.cuh's image_reduce_kernel adds each (image,
+// cell)'s CTAs in a fixed order.  The order depends only on H*W and the cell count: an image's results do not depend on B, on
+// its position in the batch or on the GPU, and no floating-point atomics are used.
 #include "dist_transform.cuh"
-#include "pixel_metrics.cuh"
-#include "rnc_common.cuh"
+#include "eval_common.cuh"
 
 namespace rnc {
 namespace {
@@ -42,37 +41,16 @@ struct Dist2Out {                       // the squared distance to the nearest b
   __device__ int operator()(int, int x, int q, int, int fq) const { return fq - q * q + (x - q) * (x - q); }
 };
 
-constexpr int kRegThreads = 256;
-constexpr int kRegWarps = kRegThreads / 32;
-constexpr int kRegPerThread = 8;
-constexpr int kRegPerCta = kRegThreads * kRegPerThread;
-constexpr int kRegCounts = 5;         // valid, epe < 1, < 3, < 5, KITTI outliers
 constexpr int kMaxCells = RNC_REGION_CELLS_SINTEL;
 
-struct RegionPart {                   // one (CTA, cell)'s partials; 32 bytes
-  double epe_sum;
-  unsigned n[kRegCounts];
-  unsigned pad;
-};
-
-struct Plane {
-  const float* p;
-  long long b, y, x;
-};
-
 struct RegionArgs {
-  const float* flow;
-  long long fb, fc, fy, fx;
-  const float* gt;
-  long long gb, gc, gy, gx;
-  Plane valid;                        // p == nullptr: every pixel is valid
-  Plane mask;                         // Sintel: occ; KITTI: noc
+  View flow, gt;
+  View valid;                         // p == nullptr: every pixel is valid
+  View mask;                          // Sintel: occ; KITTI: noc
   const int* d2;                      // Sintel: [B][H][W]
-  Plane fg;                           // KITTI; p == nullptr: every pixel is background
+  View fg;                            // KITTI; p == nullptr: every pixel is background
   int H, W, kind, cells;
 };
-
-__device__ __forceinline__ float at(const Plane& q, int b, int y, int x) { return q.p[b * q.b + y * q.y + x * q.x]; }
 
 __device__ __forceinline__ int sintel_cell(bool occluded, int d2, float mag) {
   const int d = d2 < 100 ? 0 : d2 < 3600 ? 1 : d2 < 19600 ? 2 : 3;
@@ -80,28 +58,26 @@ __device__ __forceinline__ int sintel_cell(bool occluded, int d2, float mag) {
   return (occluded ? 16 : 0) + d * 4 + s;
 }
 
-__global__ void __launch_bounds__(kRegThreads) region_part_kernel(RegionArgs a, RegionPart* __restrict__ parts) {
-  __shared__ RegionPart acc[kRegWarps][kMaxCells];
+__global__ void __launch_bounds__(kEvalThreads) region_part_kernel(RegionArgs a, MetricsPart* __restrict__ parts) {
+  __shared__ MetricsPart acc[kEvalWarps][kMaxCells];
   const int b = blockIdx.y;
   const int hw = a.H * a.W;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  acc[warp][lane] = RegionPart{};
+  acc[warp][lane] = MetricsPart{};
   __syncwarp();
-  for (int p = blockIdx.x * kRegPerCta + threadIdx.x, e = 0; e < kRegPerThread; ++e, p += kRegThreads) {
+  for (int p = blockIdx.x * kEvalPerCta + threadIdx.x, e = 0; e < kEvalPerThread; ++e, p += kEvalThreads) {
     bool has = p < hw;
     int cell = 0;
     PixelMetrics m{};
     if (has) {
       const int y = p / a.W, x = p - y * a.W;
-      has = !a.valid.p || at(a.valid, b, y, x) >= 0.5f;
+      has = !a.valid.p || a.valid.at(b, y, x) >= 0.5f;
       if (has) {
-        const float* f = a.flow + b * a.fb + y * a.fy + x * a.fx;
-        const float* g = a.gt + b * a.gb + y * a.gy + x * a.gx;
-        m = pixel_metrics(f[0], f[a.fc], g[0], g[a.gc]);
+        m = pixel_metrics(a.flow.at(b, 0, y, x), a.flow.at(b, 1, y, x), a.gt.at(b, 0, y, x), a.gt.at(b, 1, y, x));
         if (a.kind == RNC_REGIONS_SINTEL) {
-          cell = sintel_cell(at(a.mask, b, y, x) >= 0.5f, a.d2[static_cast<long long>(b) * hw + p], m.mag);
+          cell = sintel_cell(a.mask.at(b, y, x) >= 0.5f, a.d2[static_cast<long long>(b) * hw + p], m.mag);
         } else {
-          cell = (at(a.mask, b, y, x) >= 0.5f ? 0 : 2) + ((a.fg.p && at(a.fg, b, y, x) >= 0.5f) ? 1 : 0);
+          cell = (a.mask.at(b, y, x) >= 0.5f ? 0 : 2) + ((a.fg.p && a.fg.at(b, y, x) >= 0.5f) ? 1 : 0);
         }
       }
     }
@@ -118,7 +94,7 @@ __global__ void __launch_bounds__(kRegThreads) region_part_kernel(RegionArgs a, 
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
       if (lane == 0) {
-        RegionPart& r = acc[warp][c];
+        MetricsPart& r = acc[warp][c];
         r.epe_sum += s;
         r.n[0] += __popc(members);
         r.n[1] += n1;
@@ -130,43 +106,9 @@ __global__ void __launch_bounds__(kRegThreads) region_part_kernel(RegionArgs a, 
   }
   __syncthreads();
   if (threadIdx.x < a.cells) {
-    RegionPart out{};
-    for (int w = 0; w < kRegWarps; ++w) {
-      const RegionPart& r = acc[w][threadIdx.x];
-      out.epe_sum += r.epe_sum;
-#pragma unroll
-      for (int c = 0; c < kRegCounts; ++c) out.n[c] += r.n[c];
-    }
+    MetricsPart out{};
+    for (int w = 0; w < kEvalWarps; ++w) out += acc[w][threadIdx.x];
     parts[(static_cast<long long>(b) * gridDim.x + blockIdx.x) * a.cells + threadIdx.x] = out;
-  }
-}
-
-// a warp per (image, cell): parts [B][nblk][cells] -> counts [B][cells][5], epe_sum [B][cells]
-__global__ void __launch_bounds__(kRegThreads) region_reduce_kernel(const RegionPart* __restrict__ parts, int B, int nblk,
-                                                                    int cells, long long* __restrict__ counts,
-                                                                    double* __restrict__ epe_sum) {
-  const int i = blockIdx.x * kRegWarps + (threadIdx.x >> 5);
-  const int lane = threadIdx.x & 31;
-  if (i >= B * cells) return;
-  const int b = i / cells, cell = i - b * cells;
-  double sum = 0.0;
-  unsigned long long n[kRegCounts] = {0, 0, 0, 0, 0};
-  for (int k = lane; k < nblk; k += 32) {
-    const RegionPart& q = parts[(static_cast<long long>(b) * nblk + k) * cells + cell];
-    sum += q.epe_sum;
-#pragma unroll
-    for (int c = 0; c < kRegCounts; ++c) n[c] += q.n[c];
-  }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    sum += __shfl_xor_sync(0xffffffffu, sum, o);
-#pragma unroll
-    for (int c = 0; c < kRegCounts; ++c) n[c] += __shfl_xor_sync(0xffffffffu, n[c], o);
-  }
-  if (lane == 0) {
-    epe_sum[i] = sum;
-#pragma unroll
-    for (int c = 0; c < kRegCounts; ++c) counts[static_cast<long long>(i) * kRegCounts + c] = static_cast<long long>(n[c]);
   }
 }
 
@@ -177,14 +119,6 @@ bool dist2_shape_ok(int B, int H, int W) {
 int region_cells(int kind) {
   return kind == RNC_REGIONS_SINTEL ? RNC_REGION_CELLS_SINTEL : kind == RNC_REGIONS_KITTI ? RNC_REGION_CELLS_KITTI : 0;
 }
-
-bool region_shape_ok(int B, int H, int W) {
-  return B > 0 && H > 0 && W > 0 && B <= 65535 && static_cast<long long>(H) * W < (1ll << 30);
-}
-
-int region_blocks(int H, int W) { return (H * W + kRegPerCta - 1) / kRegPerCta; }
-
-bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 
 }  // namespace
 }  // namespace rnc
@@ -207,7 +141,7 @@ int rnc_boundary_dist2(const float* occ, long long ob, long long oy, long long o
 
 size_t rnc_region_metrics_workspace_bytes(int kind, int B, int H, int W) {
   const int cells = region_cells(kind);
-  return cells && region_shape_ok(B, H, W) ? static_cast<size_t>(B) * region_blocks(H, W) * cells * sizeof(RegionPart) : 0;
+  return cells && eval_shape_ok(B, H, W) ? static_cast<size_t>(B) * eval_blocks(H, W) * cells * sizeof(MetricsPart) : 0;
 }
 
 int rnc_region_metrics(int kind, const float* flow, long long fb, long long fc, long long fy, long long fx, const float* gt,
@@ -217,7 +151,7 @@ int rnc_region_metrics(int kind, const float* flow, long long fb, long long fc, 
                        double* epe_sum, void* workspace, size_t workspace_bytes, void* stream) {
   const int cells = region_cells(kind);
   if (!cells) return RNC_ERR_UNSUPPORTED;
-  if (!region_shape_ok(B, H, W)) return RNC_ERR_BAD_SHAPE;
+  if (!eval_shape_ok(B, H, W)) return RNC_ERR_BAD_SHAPE;
   if (!flow || !gt || !mask || !counts || !epe_sum || !workspace) return RNC_ERR_BAD_POINTER;
   if (kind == RNC_REGIONS_SINTEL ? (!d2 || fg) : d2 != nullptr) return RNC_ERR_BAD_POINTER;
   if (!aligned(flow, 4) || !aligned(gt, 4) || !aligned(valid, 4) || !aligned(mask, 4) || !aligned(d2, 4) ||
@@ -225,15 +159,13 @@ int rnc_region_metrics(int kind, const float* flow, long long fb, long long fc, 
     return RNC_ERR_BAD_POINTER;
   if (workspace_bytes < rnc_region_metrics_workspace_bytes(kind, B, H, W)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
-  const RegionArgs a{flow, fb, fc, fy, fx, gt, gb, gc, gy, gx, {valid, vb, vy, vx}, {mask, mb, my, mx}, d2, {fg, qb, qy, qx},
-                     H, W, kind, cells};
-  const int nblk = region_blocks(H, W);
-  RegionPart* parts = static_cast<RegionPart*>(workspace);
-  region_part_kernel<<<dim3(nblk, B), kRegThreads, 0, s>>>(a, parts);
+  const RegionArgs a{{flow, fb, fc, fy, fx}, {gt, gb, gc, gy, gx}, {valid, vb, 0, vy, vx}, {mask, mb, 0, my, mx}, d2,
+                     {fg, qb, 0, qy, qx}, H, W, kind, cells};
+  const int nblk = eval_blocks(H, W);
+  MetricsPart* parts = static_cast<MetricsPart*>(workspace);
+  region_part_kernel<<<dim3(nblk, B), kEvalThreads, 0, s>>>(a, parts);
   if (int st = after_launch()) return st;
-  region_reduce_kernel<<<(B * cells + kRegWarps - 1) / kRegWarps, kRegThreads, 0, s>>>(parts, B, nblk, cells, counts,
-                                                                                      epe_sum);
-  return after_launch();
+  return launch_image_reduce(parts, B * cells, nblk, cells, MetricsStore{counts, epe_sum}, s);
 }
 
 }  // extern "C"

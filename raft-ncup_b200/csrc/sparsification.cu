@@ -3,7 +3,7 @@
 // of lowest score are removed, and the same sum when the pixels of largest EPE are removed instead (the ideal curve,
 // which the AUSE literature calls the oracle).
 //
-// Each pixel's EPE is the one rnc_flow_metrics computes: float32, no FMA contraction (the *_rn intrinsics).
+// Each pixel's EPE is the one rnc_flow_metrics computes: eval_common.cuh's pixel_metrics.
 //
 // Keys.  Pixel p of image b sits at position b*H*W + p of a device-wide radix sort whose key is (b << 32) | low, so a stable
 // sort keeps every image in its own H*W slot, orders it by `low`, and breaks ties by row-major pixel index.  `low` is:
@@ -20,7 +20,7 @@
 // GPU.
 #include <cub/device/device_radix_sort.cuh>
 
-#include "rnc_common.cuh"
+#include "eval_common.cuh"
 
 namespace rnc {
 namespace {
@@ -30,14 +30,9 @@ constexpr int kSpThreads = 256;
 constexpr unsigned kSpInvalid = 0xffffffffu;
 
 struct SparsArgs {
-  const float* flow;
-  long long fb, fc, fy, fx;
-  const float* gt;
-  long long gb, gc, gy, gx;
-  const float* valid;          // nullptr: every pixel is valid
-  long long vb, vy, vx;
-  const float* score;
-  long long sb, sy, sx;
+  View flow, gt;
+  View valid;                  // p == nullptr: every pixel is valid
+  View score;
   int H, W;
 };
 
@@ -53,12 +48,9 @@ __global__ void __launch_bounds__(kSpThreads) spars_keys_kernel(SparsArgs a, uns
   const int p = blockIdx.x * kSpThreads + threadIdx.x;
   if (p >= hw) return;
   const int y = p / a.W, x = p - y * a.W;
-  const float* f = a.flow + b * a.fb + y * a.fy + x * a.fx;
-  const float* g = a.gt + b * a.gb + y * a.gy + x * a.gx;
-  const float dx = __fsub_rn(f[0], g[0]), dy = __fsub_rn(f[a.fc], g[a.gc]);
-  const float epe = __fsqrt_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)));
-  const bool ok = !a.valid || a.valid[b * a.vb + y * a.vy + x * a.vx] >= 0.5f;
-  const float s = a.score[b * a.sb + y * a.sy + x * a.sx];
+  const float epe = pixel_metrics(a.flow.at(b, 0, y, x), a.flow.at(b, 1, y, x), a.gt.at(b, 0, y, x), a.gt.at(b, 1, y, x)).epe;
+  const bool ok = !a.valid.p || a.valid.at(b, y, x) >= 0.5f;
+  const float s = a.score.at(b, y, x);
   const unsigned sk = !ok ? kSpInvalid : (s != s) ? 0u : monotone(s == 0.0f ? 0.0f : s);
   const unsigned ek = !ok ? kSpInvalid : (epe != epe) ? 0u : ~monotone(epe);
   const unsigned long long hi = static_cast<unsigned long long>(b) << 32;
@@ -128,10 +120,8 @@ __global__ void spars_suffix_kernel(const double* __restrict__ part, const int* 
   }
 }
 
-bool shape_ok(int B, int H, int W) {
-  return B > 0 && H > 0 && W > 0 && B <= 65535 && static_cast<long long>(H) * W < (1ll << 30) &&
-         static_cast<long long>(B) * H * W < (1ll << 31);
-}
+// the sort ranks the whole batch with int offsets: B*H*W < 2^31 besides the per-image limits
+bool shape_ok(int B, int H, int W) { return eval_shape_ok(B, H, W) && static_cast<long long>(B) * H * W < (1ll << 31); }
 
 size_t up256(size_t x) { return (x + 255) & ~size_t{255}; }
 
@@ -155,8 +145,6 @@ SparsPlan plan(int B, int H, int W) {
   while (p.end_bit < 64 && (1ll << (p.end_bit - 32)) < B) ++p.end_bit;
   return p;
 }
-
-bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 
 int cuda_status(cudaError_t e) {
   if (e == cudaSuccess) return RNC_OK;
@@ -204,7 +192,7 @@ int rnc_sparsification(const float* flow, long long fb, long long fc, long long 
   if (int st = cuda_status(cub::DeviceRadixSort::SortKeys(nullptr, need_o, ok, n, 0, p.end_bit, s))) return st;
   if (need_s > p.scratch || need_o > p.scratch) return RNC_ERR_WORKSPACE;
 
-  const SparsArgs a{flow, fb, fc, fy, fx, gt, gb, gc, gy, gx, valid, vb, vy, vx, score, sb, sy, sx, H, W};
+  const SparsArgs a{{flow, fb, fc, fy, fx}, {gt, gb, gc, gy, gx}, {valid, vb, 0, vy, vx}, {score, sb, 0, sy, sx}, H, W};
   spars_keys_kernel<<<dim3((H * W + kSpThreads - 1) / kSpThreads, B), kSpThreads, 0, s>>>(a, sk0, sv0, ok0);
   if (int st = after_launch()) return st;
   if (int st = cuda_status(cub::DeviceRadixSort::SortPairs(scratch, need_s, sk, sv, n, 0, p.end_bit, s))) return st;

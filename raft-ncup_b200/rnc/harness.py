@@ -169,8 +169,8 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
     regions=False, bit for bit.  ValueError, naming the sample's index, for a sample without masks, with a mask of the wrong
     shape, or of the other style than the rest of the split."""
     from .dist import gather_strided, strided_items, world_rank
-    from .metrics import (FRACTIONS, Partials, RegionPartials, SparsPartials, cat, cat_regions, confidence_score, fb_consistency,
-                          flow_metrics, occlusion_counts, region_partials, sparsification, summarize, summarize_occlusion,
+    from .metrics import (Partials, RegionPartials, SparsPartials, cat, confidence_score, fb_consistency, flow_metrics,
+                          from_images, images, occlusion_counts, region_partials, sparsification, summarize, summarize_occlusion,
                           summarize_regions, summarize_sparsification)
     model.eval()
     world, rank = world_rank()
@@ -178,7 +178,16 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
     if dev.type == "cuda" and dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
     copy_stream = torch.cuda.Stream(dev) if dev.type == "cuda" else None
-    parts, sparse, sparts, fparts, rparts, oparts, rmeta = [], [], [], [], [], [], []
+    # this rank's per-batch partials by name, with the type each concatenates to
+    kinds = {"flow": Partials}
+    if confidence:
+        kinds["confidence"] = SparsPartials
+    if consistency:
+        kinds["consistency"] = SparsPartials
+    if regions:
+        kinds["regions"] = RegionPartials
+    parts = {name: [] for name in kinds}
+    occlusion, sparse, rmeta = [], [], []
     items = strided_items(samples, world, rank)
     batches = _shape_batches(_region_samples(items, world, rank) if regions else items, batch_size, regions)
 
@@ -206,57 +215,49 @@ def validate(model, samples, iters=32, mode="sintel", batch_size=8, device="cuda
         else:
             _, flow_pr = model(p1, p2, iters=iters, test_mode=True)
         flow = padder.unpad(flow_pr)
-        parts.append(flow_metrics(flow, cur.gt, cur.valid))
+        parts["flow"].append(flow_metrics(flow, cur.gt, cur.valid))
         if confidence:
-            sparts.append(sparsification(flow, cur.gt, cur.valid, confidence_score(padder.unpad(conf))))
+            parts["confidence"].append(sparsification(flow, cur.gt, cur.valid, confidence_score(padder.unpad(conf))))
             del conf
         if regions:
             rp = region_partials(flow, cur.gt, cur.valid, **cur.masks)
-            rparts.append(rp._replace(fg=torch.tensor(["fg" in r.masks for r in cur.regions])))
+            parts["regions"].append(rp._replace(fg=torch.tensor(["fg" in r.masks for r in cur.regions])))
             rmeta += cur.regions
         if consistency:
             occ_fw, _, fb_err, _ = fb_consistency(flow, flow_bw)
-            fparts.append(sparsification(flow, cur.gt, cur.valid, -fb_err))
+            parts["consistency"].append(sparsification(flow, cur.gt, cur.valid, -fb_err))
             if regions and "occ" in cur.masks:
-                oparts.append(occlusion_counts(occ_fw, cur.masks["occ"], cur.valid))
+                occlusion.append(occlusion_counts(occ_fw, cur.masks["occ"], cur.valid))
             del flow_bw, fb_err, occ_fw
         sparse += cur.sparse
         del cur, p1, p2, flow_pr, flow
         nxt = stage_next()                          # staged while this batch computes
-    local = cat(parts)
-    rows = list(zip(local.counts.cpu().tolist(), local.epe_sum.cpu().tolist(), sparse))
-    scores = [sp for on, sp in ((confidence, sparts), (consistency, fparts)) if on]
-    for sp in scores:
-        cols = [torch.cat(c).cpu().tolist() for c in zip(*sp)] if sp else [[], [], []]
-        rows = [r + s for r, s in zip(rows, zip(*cols))]
-    if regions:                             # one more item per row: (index, style, cell counts, cell sums, fg, occ counts)
-        rp = cat_regions(rparts) if rparts else RegionPartials(torch.zeros(0, 0, 5), torch.zeros(0, 0), torch.zeros(0))
-        occ = torch.cat(oparts).cpu().tolist() if oparts else [None] * len(rmeta)
-        rows = [r + ((m.index, m.kind, c, e, f, o),) for r, m, c, e, f, o in
-                zip(rows, rmeta, rp.counts.cpu().tolist(), rp.epe_sum.cpu().tolist(), rp.fg.tolist(), occ)]
-    rows = gather_strided(rows, world)
-    every = Partials(torch.tensor([r[0] for r in rows], dtype=torch.int64).view(-1, 5),
-                     torch.tensor([r[1] for r in rows], dtype=torch.float64))
-    res = summarize(every, "kitti" if any(r[2] for r in rows) else "sintel")
-    for i, prefix in enumerate(p for on, p in ((confidence, ""), (consistency, "fb_")) if on):
-        c = 3 + 3 * i
-        summ = summarize_sparsification(SparsPartials(
-            torch.tensor([r[c] for r in rows], dtype=torch.int64).view(-1, FRACTIONS),
-            torch.tensor([r[c + 1] for r in rows], dtype=torch.float64).view(-1, FRACTIONS),
-            torch.tensor([r[c + 2] for r in rows], dtype=torch.float64).view(-1, FRACTIONS)))
-        res.update({prefix + "sparsification": summ["sparsification"], "ideal": summ["ideal"], prefix + "ause": summ["ause"]})
+    # one record per image of this rank, {name: value}: its partials, whether it had a valid mask, and with regions its index
+    # and style (and, Sintel-style with consistency, its occlusion counts), gathered back into sample order
+    local = {name: images(cat(kind, parts[name])) for name, kind in kinds.items()}
+    local["sparse"] = sparse
     if regions:
-        reg = [r[-1] for r in rows]
-        for g in reg:
-            if g[1] != reg[0][1]:
-                raise ValueError(f"validate(regions=True): sample {g[0]} is {g[1].capitalize()}-style but sample {reg[0][0]} is "
-                                 f"{reg[0][1].capitalize()}-style; one split is one or the other")
-        if reg:
-            res.update(summarize_regions(RegionPartials(torch.tensor([g[2] for g in reg], dtype=torch.int64),
-                                                        torch.tensor([g[3] for g in reg], dtype=torch.float64),
-                                                        torch.tensor([g[4] for g in reg], dtype=torch.bool))))
-            if consistency and reg[0][1] == "sintel":
-                res.update(summarize_occlusion(torch.tensor([g[5] for g in reg], dtype=torch.int64)))
+        local["style"] = [(m.index, m.kind) for m in rmeta]
+    if occlusion:
+        local["occlusion"] = torch.cat(occlusion).cpu().tolist()
+    rows = gather_strided([dict(zip(local, r)) for r in zip(*local.values())], world)
+
+    def gathered(name):
+        return from_images(kinds[name], [r[name] for r in rows])
+    res = summarize(gathered("flow"), "kitti" if any(r["sparse"] for r in rows) else "sintel")
+    for name, prefix in (("confidence", ""), ("consistency", "fb_")):
+        if name in kinds:
+            summ = summarize_sparsification(gathered(name))
+            res.update({prefix + "sparsification": summ["sparsification"], "ideal": summ["ideal"], prefix + "ause": summ["ause"]})
+    if regions and rows:
+        i0, kind0 = rows[0]["style"]
+        for i, kind in (r["style"] for r in rows):
+            if kind != kind0:
+                raise ValueError(f"validate(regions=True): sample {i} is {kind.capitalize()}-style but sample {i0} is "
+                                 f"{kind0.capitalize()}-style; one split is one or the other")
+        res.update(summarize_regions(gathered("regions")))
+        if consistency and kind0 == "sintel":
+            res.update(summarize_occlusion(torch.tensor([r["occlusion"] for r in rows], dtype=torch.int64)))
     return res
 
 
@@ -494,8 +495,9 @@ def validate_interpolation(model, sequences, iters=32, mode="sintel", batch_size
     interpolation_error of its pair alone; warm, each pair starts from the previous pair of its subsequence.  Either way
     they do not depend on batch_size.  Under torch.distributed rank r takes the sequences of index = r (mod world), the partials are
     all-gathered, and every rank returns the single-process result."""
-    from .dist import strided_items, world_rank
-    from .interp import InterpPartials, interpolate, interpolation_error, summarize_interpolation
+    from .dist import gather_strided, strided_items, world_rank
+    from .interp import interpolate, interpolation_error, summarize_interpolation
+    from .metrics import InterpPartials, cat, from_images, images
     world, rank = world_rank()
     mine = list(strided_items(range(len(sequences)), world, rank))
     subs, origin = [], []                           # origin[i]: (sequence index, offset) of subsequence i
@@ -503,7 +505,7 @@ def validate_interpolation(model, sequences, iters=32, mode="sintel", batch_size
         for off in (0, 1):
             subs.append(sequences[s][off::2])
             origin.append((s, off))
-    keys, parts = [], []
+    parts = {s: [None] * max(len(sequences[s]) - 2, 0) for s in mine}      # per sequence, triplet k's partials
     for i, p, r in run_sequences_bidirectional(model, subs, iters, warm_start=warm_start, batch_size=batch_size, mode=mode,
                                                device=device):
         s, off = origin[i]
@@ -512,18 +514,9 @@ def validate_interpolation(model, sequences, iters=32, mode="sintel", batch_size
         dev = r["flow_up"].device
         f0, f2, gt = (seq[j][None].to(dev).float() for j in (k, k + 2, k + 1))
         pred = interpolate(f0, f2, r["flow_up"][None], r["flow_up_bw"][None], r["occ"][None], r["occ_bw"][None], (0.5,))
-        parts.append(interpolation_error(pred[:, 0], gt))
-        keys.append((s, k))
-    rows = list(zip(keys, (torch.cat([q.sq_sum for q in parts]).cpu().tolist() if parts else []),
-                    (torch.cat([q.count for q in parts]).cpu().tolist() if parts else [])))
-    if world > 1:
-        import torch.distributed as dist
-        every = [None] * world
-        dist.all_gather_object(every, rows)
-        rows = [r for part in every for r in part]
-    rows.sort(key=lambda r: r[0])
-    return summarize_interpolation(InterpPartials(torch.tensor([r[1] for r in rows], dtype=torch.float64),
-                                                  torch.tensor([r[2] for r in rows], dtype=torch.int64)))
+        parts[s][k] = interpolation_error(pred[:, 0], gt)
+    every = gather_strided([images(cat(InterpPartials, parts[s])) for s in mine], world)
+    return summarize_interpolation(from_images(InterpPartials, [t for seq in every for t in seq]))
 
 
 def size_batches(items, batch_size, key):

@@ -34,16 +34,13 @@ error (IE) and the PSNR.
 """
 import ctypes as C
 import math
-from collections import namedtuple
 
 import numpy as np
 import torch
 
 from . import native
-from .metrics import _f32, nearest_site
+from .metrics import InterpPartials, _f32, nearest_site
 
-# sq_sum: float64 [N], per frame the sum over pixels of sum_c (pred - gt)^2; count: int64 [N], its pixels
-InterpPartials = namedtuple("InterpPartials", "sq_sum count")
 NO_PROPOSAL = np.uint64(0xFFFFFFFFFFFFFFFF)
 
 
@@ -221,13 +218,6 @@ def host_interpolation_error(pred, gt):
     d2 = d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2]
     N, _, H, W = pred.shape
     return InterpPartials(torch.from_numpy(d2.reshape(N, -1).sum(1)), torch.full((N,), H * W, dtype=torch.int64))
-
-
-def cat_interpolation(parts):
-    """One InterpPartials of a list of them, in order."""
-    if not parts:
-        return InterpPartials(torch.zeros(0, dtype=torch.float64), torch.zeros(0, dtype=torch.int64))
-    return InterpPartials(torch.cat([p.sq_sum for p in parts]), torch.cat([p.count for p in parts]))
 
 
 def summarize_interpolation(partials):

@@ -30,6 +30,44 @@ Partials = namedtuple("Partials", "counts epe_sum")
 # count: int64 [N, 100] (valid pixels kept at f_k); kept_epe, ideal_epe: float64 [N, 100] (their EPE sum, score / ideal order)
 SparsPartials = namedtuple("SparsPartials", "count kept_epe ideal_epe")
 FRACTIONS = 100
+# counts: int64 [N, cells, 5] (as Partials.counts, per cell); epe_sum: float64 [N, cells]; fg: bool [N] (KITTI: the image
+# came with a foreground mask)
+RegionPartials = namedtuple("RegionPartials", "counts epe_sum fg")
+# sq_sum: float64 [N], per frame the sum over pixels of sum_c (pred - gt)^2; count: int64 [N], its pixels (rnc.interp)
+InterpPartials = namedtuple("InterpPartials", "sq_sum count")
+
+# the partials of no image, per type (RegionPartials with 0 cells)
+_EMPTY = {Partials: Partials(torch.zeros(0, 5, dtype=torch.int64), torch.zeros(0, dtype=torch.float64)),
+          SparsPartials: SparsPartials(torch.zeros(0, FRACTIONS, dtype=torch.int64),
+                                       *(torch.zeros(0, FRACTIONS, dtype=torch.float64) for _ in range(2))),
+          RegionPartials: RegionPartials(torch.zeros(0, 0, 5, dtype=torch.int64), torch.zeros(0, 0, dtype=torch.float64),
+                                         torch.zeros(0, dtype=torch.bool)),
+          InterpPartials: InterpPartials(torch.zeros(0, dtype=torch.float64), torch.zeros(0, dtype=torch.int64))}
+
+
+def cat(kind, parts):
+    """One `kind` partials (Partials, SparsPartials, RegionPartials or InterpPartials) of a list of them, in image order."""
+    if not parts:
+        return _EMPTY[kind]
+    return kind(*(torch.cat(f) for f in zip(*parts)))
+
+
+def images(partials):
+    """Per-image records of partials: one tuple per image of its fields' values as Python numbers and lists (what
+    validate gathers over ranks)."""
+    return list(zip(*(f.cpu().tolist() for f in partials)))
+
+
+def from_images(kind, records):
+    """The `kind` partials of per-image records, on the CPU: the inverse of images."""
+    if not records:
+        return _EMPTY[kind]
+    return kind(*(torch.tensor(col, dtype=e.dtype) for col, e in zip(zip(*records), _EMPTY[kind])))
+
+
+def _strides(t):
+    """The element strides of an optional [B,H,W] mask; zeros for None, which the kernels do not read."""
+    return (0, 0, 0) if t is None else t.stride()
 
 
 def _check(flow, gt, valid):
@@ -57,8 +95,8 @@ def flow_metrics(flow, gt, valid=None):
     epe_sum = torch.empty(B, dtype=torch.float64, device=dev)
     with torch.cuda.device(dev):
         ws = torch.empty(native.rnc.flow_metrics_workspace_bytes(B, H, W), dtype=torch.uint8, device=dev)
-        vs = (0, 0, 0) if valid is None else valid.stride()
-        native.rnc.flow_metrics(flow, *flow.stride(), gt, *gt.stride(), valid, *vs, B, H, W, counts, epe_sum, ws, ws.numel())
+        native.rnc.flow_metrics(flow, *flow.stride(), gt, *gt.stride(), valid, *_strides(valid), B, H, W, counts, epe_sum, ws,
+                                ws.numel())
     return Partials(counts, epe_sum)
 
 
@@ -90,13 +128,6 @@ def host_partials(flow, gt, valid=None):
     if not counts:
         return Partials(torch.zeros(0, 5, dtype=torch.int64), torch.zeros(0, dtype=torch.float64))
     return Partials(torch.stack(counts).to(torch.int64), torch.stack(sums))
-
-
-def cat(parts):
-    """One Partials of a list of them, in order."""
-    if not parts:
-        return Partials(torch.zeros(0, 5, dtype=torch.int64), torch.zeros(0, dtype=torch.float64))
-    return Partials(torch.cat([p.counts for p in parts]), torch.cat([p.epe_sum for p in parts]))
 
 
 def _ratio(a, b):
@@ -159,9 +190,8 @@ def sparsification(flow, gt, valid, score):
         if nbytes == 0:
             raise ValueError(f"sparsification: {B} images of {H}x{W} exceed the sort's 2^31 pixels")
         ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-        vs = (0, 0, 0) if valid is None else valid.stride()
-        native.rnc.sparsification(flow, *flow.stride(), gt, *gt.stride(), valid, *vs, score, *score.stride(), B, H, W, count,
-                                  kept, ideal, ws, ws.numel())
+        native.rnc.sparsification(flow, *flow.stride(), gt, *gt.stride(), valid, *_strides(valid), score, *score.stride(), B, H,
+                                  W, count, kept, ideal, ws, ws.numel())
     return SparsPartials(count, kept, ideal)
 
 
@@ -349,9 +379,6 @@ def host_fb_consistency(flow_fw, flow_bw, alpha1=0.01, alpha2=0.5):
 
 DIST2_NONE = native.DIST2_NONE
 SINTEL_CELLS, KITTI_CELLS = native.REGION_CELLS[native.REGIONS_SINTEL], native.REGION_CELLS[native.REGIONS_KITTI]
-# counts: int64 [N, cells, 5] (as Partials.counts, per cell); epe_sum: float64 [N, cells]; fg: bool [N] (KITTI: the image
-# came with a foreground mask)
-RegionPartials = namedtuple("RegionPartials", "counts epe_sum fg")
 # region -> its cells, in increasing order
 SINTEL_REGIONS = {"matched": list(range(16)), "unmatched": list(range(16, 32)),
                   **{k: [c for c in range(32) if (c >> 2) & 3 == i] for i, k in enumerate(("d0-10", "d10-60", "d60-140"))},
@@ -498,10 +525,8 @@ def region_partials(flow, gt, valid=None, occ=None, noc=None, fg=None):
     with torch.cuda.device(dev):
         d2 = boundary_dist2(mask) if occ is not None else None
         ws = torch.empty(native.rnc.region_metrics_workspace_bytes(kind, B, H, W), dtype=torch.uint8, device=dev)
-        vs = (0, 0, 0) if valid is None else valid.stride()
-        qs = (0, 0, 0) if fg is None else fg.stride()
-        native.rnc.region_metrics(kind, flow, *flow.stride(), gt, *gt.stride(), valid, *vs, mask, *mask.stride(), d2, fg, *qs,
-                                  B, H, W, counts, epe_sum, ws, ws.numel())
+        native.rnc.region_metrics(kind, flow, *flow.stride(), gt, *gt.stride(), valid, *_strides(valid), mask, *mask.stride(),
+                                  d2, fg, *_strides(fg), B, H, W, counts, epe_sum, ws, ws.numel())
     return RegionPartials(counts, epe_sum, torch.full((B,), fg is not None, dtype=torch.bool))
 
 
@@ -537,9 +562,8 @@ def host_region_partials(flow, gt, valid=None, occ=None, noc=None, fg=None):
 
 
 def cat_regions(parts):
-    """One RegionPartials of a list of them (of one style), in order."""
-    return RegionPartials(torch.cat([p.counts for p in parts]), torch.cat([p.epe_sum for p in parts]),
-                          torch.cat([p.fg for p in parts]))
+    """One RegionPartials of a list of them (of one style), in order: cat(RegionPartials, parts), under its public name."""
+    return cat(RegionPartials, parts)
 
 
 def summarize_regions(partials):

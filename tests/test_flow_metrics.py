@@ -370,7 +370,7 @@ def test_flow_metrics_cu_does_not_spill(tmp_path):
     out = subprocess.run(cmd, capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
     log = out.stdout + out.stderr
-    kernels = re.findall(r"Function properties for \S*(metrics_\w+_kernel)", log)
-    assert sorted(kernels) == ["metrics_part_kernel", "metrics_reduce_kernel"], kernels
+    kernels = re.findall(r"Function properties for \S*?\d((?:cta|image)_[a-z_]+_kernel)", log)
+    assert sorted(kernels) == ["cta_partials_kernel", "image_reduce_kernel"], kernels
     spills = re.findall(r"(\d+) bytes spill stores, (\d+) bytes spill loads", log)
     assert len(spills) == 2 and all(a == "0" and b == "0" for a, b in spills), spills

@@ -215,6 +215,56 @@ def test_validate_interpolation_checks_frame_sizes():
         validate_interpolation(build_model("raft"), seqs)
 
 
+def _stub_bidirectional(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda"):
+    """run_sequences_bidirectional's yields in its step order, on the CPU: flows from the frames' first two channels, the
+    masks of host_fb_consistency."""
+    from rnc.harness import sequence_schedule
+    for step in sequence_schedule([len(s) for s in sequences], batch_size):
+        for c in step:
+            if not c.idle:
+                a, b = sequences[c.seq][c.pair], sequences[c.seq][c.pair + 1]
+                fw, bw = ((b[:2] - a[:2]) / 8)[None], ((a[1:] - b[1:]) / 8)[None]
+                occ, occ_bw, _, _ = host_fb_consistency(fw, bw)
+                yield c.seq, c.pair, {"flow_up": fw[0], "flow_up_bw": bw[0], "occ": occ[0], "occ_bw": occ_bw[0]}
+
+
+def interpolation_sequences():
+    """Seven sequences of 2 to 9 frames, one without a triplet."""
+    return [shift_sequence(n, 12, 20, seed=n, dy=k % 3, dx=2) for k, n in enumerate((5, 2, 9, 3, 6, 4, 7))]
+
+
+def _interpolation_worker(rank, world, port, q):
+    import os
+    import torch.distributed as dist
+    from rnc import harness
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    try:
+        harness.run_sequences_bidirectional = _stub_bidirectional
+        q.put((rank, harness.validate_interpolation(None, interpolation_sequences(), batch_size=2, device="cpu")))
+    finally:
+        dist.destroy_process_group()
+
+
+@pytest.mark.parametrize("world", [2, 3])
+def test_validate_interpolation_gloo_equals_world_1(world, monkeypatch):
+    from test_flow_metrics import run_ranks
+    from rnc import harness
+    monkeypatch.setattr(harness, "run_sequences_bidirectional", _stub_bidirectional)
+    seqs = interpolation_sequences()
+    want = harness.validate_interpolation(None, seqs, batch_size=2, device="cpu")
+    parts = []                                      # per triplet in (sequence, k) order, as the host defines it
+    for seq in seqs:
+        for k in range(len(seq) - 2):
+            r = {name: v[None] for name, v in next(_stub_bidirectional(None, [[seq[k], seq[k + 2]]]))[2].items()}
+            pred = host_interpolate(seq[k][None], seq[k + 2][None], r["flow_up"], r["flow_up_bw"], r["occ"], r["occ_bw"])
+            parts.append(host_interpolation_error(pred[:, 0], seq[k + 1][None]))
+    assert want == summarize_interpolation(InterpPartials(*(torch.cat(f) for f in zip(*parts))))
+    assert want["frames"] == sum(len(s) - 2 for s in seqs if len(s) > 2)
+    for got in run_ranks(_interpolation_worker, world):
+        assert got == want                                  # bit for bit, on every rank
+
+
 def test_interp_cu_does_not_spill(tmp_path):
     import os
     import re
@@ -225,8 +275,8 @@ def test_interp_cu_does_not_spill(tmp_path):
     out = subprocess.run(cmd, capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
     log = out.stdout + out.stderr
-    kernels = re.findall(r"Function properties for \S*?\d((?:dist2|interp)_[a-z0-9_]+_kernel)", log)
-    assert sorted(kernels) == ["dist2_column_kernel", "dist2_row_kernel", "interp_composite_kernel", "interp_error_part_kernel",
-                               "interp_error_reduce_kernel", "interp_splat_kernel"], kernels
+    kernels = re.findall(r"Function properties for \S*?\d((?:dist2|interp|cta|image)_[a-z0-9_]+_kernel)", log)
+    assert sorted(kernels) == ["cta_partials_kernel", "dist2_column_kernel", "dist2_row_kernel", "image_reduce_kernel",
+                               "interp_composite_kernel", "interp_splat_kernel"], kernels
     spills = re.findall(r"(\d+) bytes spill stores, (\d+) bytes spill loads", log)
     assert len(spills) == 6 and all(a == "0" and b == "0" for a, b in spills), spills

@@ -411,7 +411,7 @@ def test_region_metrics_cu_does_not_spill(tmp_path):
     out = subprocess.run(cmd, capture_output=True, text=True)
     assert out.returncode == 0, out.stdout + out.stderr
     log = out.stdout + out.stderr
-    kernels = re.findall(r"Function properties for \S*\d((?:dist2|region)_[a-z0-9_]+_kernel)", log)
-    assert sorted(kernels) == ["dist2_column_kernel", "dist2_row_kernel", "region_part_kernel", "region_reduce_kernel"], kernels
+    kernels = re.findall(r"Function properties for \S*?\d((?:dist2|region|image)_[a-z0-9_]+_kernel)", log)
+    assert sorted(kernels) == ["dist2_column_kernel", "dist2_row_kernel", "image_reduce_kernel", "region_part_kernel"], kernels
     spills = re.findall(r"(\d+) bytes spill stores, (\d+) bytes spill loads", log)
     assert len(spills) == 4 and all(a == "0" and b == "0" for a, b in spills), spills
