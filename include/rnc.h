@@ -652,6 +652,53 @@ int rnc_interp_error(const float* pred, long long pb, long long pc, long long py
                      long long gc, long long gy, long long gx, int N, int H, int W, double* sq_sum, long long* count,
                      void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V7  unsupervised losses of N rows (source image I1, target image I2, flow F), forward and backward (definition:
+ * rnc/unsupervised.py, DESIGN §3.16).  Shapes: 1 <= N <= 65535, H, W >= 8, H*W < 2^30; RNC_ERR_BAD_SHAPE otherwise.  Bad
+ * arguments return before any launch.  No atomics: every output is a fixed-order sum, bit-identical from run to run, and a
+ * row's results are the same bits whatever N or its position in the batch.
+ *
+ * rnc_census_loss_fwd: per row r, S_r = sum_p v l (fp64) and M_r = sum_p v, where g(I) = 0.2989 R + 0.5870 G + 0.1140 B,
+ * W^ = g(I2) sampled bilinearly at p + F(p) (align_corners pixel coordinates, taps outside the frame 0), c_d(A)(p) =
+ * delta / sqrt(0.81 + delta^2) with delta = A(p+d) - A(p) over the 7x7 offsets d (A = 0 outside the frame), h = sum_d e^2 /
+ * (0.1 + e^2) with e = c_d(g(I1)) - c_d(W^), l = (h + 0.01)^0.4, and v = mask(p) for 3 <= x <= W-4, 3 <= y <= H-4, else 0.
+ *   image1, image2 : fp32 [N,3,H,W] (0..255) through element strides (ab..ax, bb..bx); 4-byte aligned
+ *   flow           : fp32 [N,2,H,W] through element strides; 4-byte aligned
+ *   mask           : uint8 [N][H][W] contiguous, weight where != 0; NULL: all ones
+ *   loss_sum       : fp64 [N] S_r; count: int64 [N] M_r; total: fp64 [2] = (sum_r S_r, sum_r M_r), rows added in row order
+ *   state          : 28 N H W bytes, 8-byte aligned: the fp64 planes g(I1) and W^ ([N][H][W] each), then the fp32 planes
+ *                    dW^/dpx, dW^/dpy (the floor convention at integer positions) and v dl/dh; what rnc_census_loss_bwd reads
+ *   workspace      : rnc_census_loss_workspace_bytes(N, H, W) bytes, 16-byte aligned, no zeroing needed
+ * Five launches, no host synchronisation.
+ *
+ * rnc_census_loss_bwd: grad_flow (fp32 [N][2][H][W] contiguous) = *scale (a device fp32 scalar: the upstream gradient over
+ * sum_r M_r + 1e-6) times the gradient of sum_r S_r with respect to F, gathered per pixel over its 7x7 window from state.  One
+ * launch.
+ *
+ * rnc_smoothness_fwd: per row, sum_x[r] = sum over 1 <= x <= W-2, all y, and both flow channels of
+ * rho(F(x+1,y) - 2F(x,y) + F(x-1,y)) exp(-edge_constant mean_c |I_c(x,y) - I_c(x-1,y)| / 255), rho(d) = sqrt(d^2 + 1e-6),
+ * and sum_y[r] the same along y (fp64); total: fp64 [2] = (sum_r sum_x, sum_r sum_y) in row order.
+ *   image          : fp32 [N,3,H,W] through element strides; flow: fp32 [N,2,H,W] through element strides; 4-byte aligned
+ *   workspace      : rnc_smoothness_workspace_bytes(N, H, W) bytes, 16-byte aligned, no zeroing needed
+ * Three launches, no host synchronisation.
+ *
+ * rnc_smoothness_bwd: grad_flow (fp32 [N][2][H][W] contiguous) = scale[0] d(sum_x)/dF + scale[1] d(sum_y)/dF, scale a
+ * device fp32 [2]; per pixel a gather of the three x- and three y-terms that hold it.  One launch. */
+size_t rnc_census_loss_workspace_bytes(int N, int H, int W);   /* 0 for a bad shape */
+int rnc_census_loss_fwd(const float* image1, long long ab, long long ac, long long ay, long long ax, const float* image2,
+                        long long bb, long long bc, long long by, long long bx, const float* flow, long long fb, long long fc,
+                        long long fy, long long fx, const unsigned char* mask, int N, int H, int W, double* loss_sum,
+                        long long* count, double* total, void* state, void* workspace, size_t workspace_bytes,
+                        void* stream);
+int rnc_census_loss_bwd(const void* state, int N, int H, int W, const float* scale, float* grad_flow, void* stream);
+size_t rnc_smoothness_workspace_bytes(int N, int H, int W);    /* 0 for a bad shape */
+int rnc_smoothness_fwd(const float* image, long long ib, long long ic, long long iy, long long ix, const float* flow,
+                       long long fb, long long fc, long long fy, long long fx, int N, int H, int W, float edge_constant,
+                       double* sum_x, double* sum_y, double* total, void* workspace, size_t workspace_bytes, void* stream);
+int rnc_smoothness_bwd(const float* image, long long ib, long long ic, long long iy, long long ix, const float* flow,
+                       long long fb, long long fc, long long fy, long long fx, int N, int H, int W, float edge_constant,
+                       const float* scale, float* grad_flow, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -452,7 +452,7 @@ def run_sequences_bidirectional(model, sequences, iters=32, warm_start=False, ba
         return
     if model._needs_grad():
         raise ValueError("run_sequences_bidirectional is inference only: call it under torch.no_grad() (training through the "
-                         "bidirectional pass is not built)")
+                         "bidirectional pass is model(..., bidirectional=True))")
     from .metrics import fb_consistency
     B = len(steps[0])
     for step, flow_low, flow_up, conf in _sequence_steps(model, sequences, steps, padder, iters, warm_start, device,

@@ -56,14 +56,23 @@ class _RAFTBase(nn.Module):
     def _needs_grad(self):
         return torch.is_grad_enabled() and any(t.requires_grad for t in module_tensors(self))
 
-    def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False, return_confidence=False):
+    def forward(self, image1, image2, iters=12, flow_init=None, upsample=True, test_mode=False, return_confidence=False,
+                bidirectional=False):
         """Estimate optical flow between a pair of frames (raft_nc_dbl.py:115-173 / raft.py:87-143).
 
         return_confidence (NCUP model only): also return the NCUP upsampler's per-pixel output confidence in [0, 1], shaped
         like flow_up ([N,2,H,W], one plane per flow component): (flow_low, flow_up, confidence_up) in test mode, else
-        (flow_predictions, confidence_predictions), one entry per iteration.  The flows are the same as without it."""
+        (flow_predictions, confidence_predictions), one entry per iteration.  The flows are the same as without it.
+
+        bidirectional: both directions of the B pairs from one encoder pass, as 2B rows: row j is image1[j] -> image2[j],
+        row B + j image2[j] -> image1[j], each what forward(cat(image1, image2), cat(image2, image1)) gives for it.
+        flow_init is then a pair (fw, bw), each [B,2,H/8,W/8] or None (a cold start for that direction).  Every route runs
+        it: test-mode inference (forward_bidirectional's result), list mode, the frozen-trunk route and full training (the
+        unsupervised fine-tuning of rnc.train.unsupervised_step trains through it)."""
         if return_confidence and not self.ncup:
             raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
+        if bidirectional:
+            flow_init = _bidirectional_init(image1, image2, flow_init)
         dev = _require_cuda(image1, image2, flow_init)
         pdev = module_device(self)
         if pdev != dev:
@@ -72,9 +81,9 @@ class _RAFTBase(nn.Module):
         # the kernels launch on `dev`'s current stream whatever device is current in the calling thread (nn.DataParallel
         # worker threads, a model on cuda:1 in a cuda:0 process); one forward at a time per device
         with torch.cuda.device(dev), eng.lock:
-            return self._forward(eng, image1, image2, iters, flow_init, test_mode, bool(return_confidence))
+            return self._forward(eng, image1, image2, iters, flow_init, test_mode, bool(return_confidence), bool(bidirectional))
 
-    def _forward(self, eng, image1, image2, iters, flow_init, test_mode, conf=False):
+    def _forward(self, eng, image1, image2, iters, flow_init, test_mode, conf=False, bidirectional=False):
         if iters < 1:
             raise ValueError("iters must be >= 1")
         if hasattr(self, "data_idx"):
@@ -85,12 +94,18 @@ class _RAFTBase(nn.Module):
             # training path (train.py:215): the same graph with autograd, exact-fp32 kernels forward and backward
             if frozen_trunk(self, image1, image2, flow_init):
                 # only the upsampler trains: the trunk runs on the inference engine, the upsampler on autograd
+                if bidirectional:
+                    return self._forward_bidirectional(eng, image1, image2, iters, flow_init, conf, test_mode,
+                                                       upsample=self._upsample_frozen)
                 return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, upsample=self._upsample_frozen,
                                            return_confidence=conf)
             from .train import raft_forward_train
-            return raft_forward_train(self, image1, image2, iters, flow_init, test_mode, return_confidence=conf)
+            return raft_forward_train(self, image1, image2, iters, flow_init, test_mode, return_confidence=conf,
+                                      bidirectional=bidirectional)
         if test_mode and eng.graphs_enabled(self):
-            return eng.graph_forward(self, image1, image2, iters, flow_init, return_confidence=conf)
+            return eng.graph_forward(self, image1, image2, iters, flow_init, return_confidence=conf, bidirectional=bidirectional)
+        if bidirectional:
+            return self._forward_bidirectional(eng, image1, image2, iters, flow_init, conf, test_mode)
         return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, return_confidence=conf)
 
     def _forward_eager(self, eng, image1, image2, iters, flow_init, test_mode, upsample=None, encode=None, ws=None,
@@ -151,48 +166,19 @@ class _RAFTBase(nn.Module):
             raise ValueError("return_confidence: the convex-upsampling RAFT has no NCUP upsampler and so no output confidence")
         if self._needs_grad():
             raise ValueError("forward_bidirectional is inference only: call it under torch.no_grad() (training through the "
-                             "bidirectional pass is not built)")
-        if image1.shape != image2.shape or image1.dim() != 4:
-            raise ValueError(f"forward_bidirectional: expected two [B,3,H,W] images of one shape, got {tuple(image1.shape)} "
-                             f"and {tuple(image2.shape)}")
-        B, _, Him, Wim = image1.shape
-        fi = None
-        if flow_init is not None:
-            if not isinstance(flow_init, (tuple, list)) or len(flow_init) != 2:
-                raise ValueError("flow_init: expected a pair (fw, bw), each [B,2,H/8,W/8] or None")
-            fw, bw = flow_init
-            for f in (fw, bw):
-                if f is not None and tuple(f.shape) != (B, 2, Him // 8, Wim // 8):
-                    raise ValueError(f"flow_init: expected [B,2,H/8,W/8] = {(B, 2, Him // 8, Wim // 8)}, got {tuple(f.shape)}")
-            if fw is not None or bw is not None:
-                ref = fw if fw is not None else bw
-                # a missing direction starts cold: coords0 + 0.0 is exactly coords0, as with no flow_init
-                fi = torch.cat([(f if f is not None else torch.zeros_like(ref)).float() for f in (fw, bw)])
-        dev = _require_cuda(image1, image2, fi)
-        pdev = module_device(self)
-        if pdev != dev:
-            raise ValueError(f"model parameters are on {pdev} but the images are on {dev}")
-        eng = engine_for(dev)
-        conf = bool(return_confidence)
-        with torch.cuda.device(dev), eng.lock:
-            if iters < 1:
-                raise ValueError("iters must be >= 1")
-            if Him % 8 or Wim % 8:
-                raise ValueError("image height/width must be multiples of 8 (pad with utils.utils.InputPadder, evaluate.py:125)")
-            if hasattr(self, "data_idx"):
-                self.data_idx += 1
-            if eng.graphs_enabled(self):
-                return eng.graph_forward(self, image1, image2, iters, fi, return_confidence=conf, bidirectional=True)
-            return self._forward_bidirectional(eng, image1, image2, iters, fi, conf)
+                             "bidirectional pass is forward(..., bidirectional=True))")
+        return self.forward(image1, image2, iters, flow_init, test_mode=True, return_confidence=return_confidence,
+                            bidirectional=True)
 
-    def _forward_bidirectional(self, eng, image1, image2, iters, flow_init, return_confidence=False):
+    def _forward_bidirectional(self, eng, image1, image2, iters, flow_init, return_confidence=False, test_mode=True,
+                               upsample=None):
         """The bidirectional pass on the engine: _forward_eager over 2B slots of the engine's workspace, slot j holding
         (image1[j], image2[j]) and slot B + j (image2[j], image1[j]), encoded by EncoderStage's bidirectional plan.  flow_init:
-        [2B,2,H/8,W/8] or None."""
+        [2B,2,H/8,W/8] or None; upsample: _forward_eager's (the frozen-trunk route passes _upsample_frozen)."""
         B, _, Him, Wim = image1.shape
         pk = eng.packed_update(self.update_block)
         ws = eng.workspace(image1.device, 2 * B, Him // 8, Wim // 8, pk.has_mask, self.ncup)
-        return self._forward_eager(eng, image1, image2, iters, flow_init, True,
+        return self._forward_eager(eng, image1, image2, iters, flow_init, test_mode, upsample=upsample,
                                    encode=EncoderStage(self, slot_plan(B, bidirectional=True)), ws=ws,
                                    return_confidence=return_confidence)
 
@@ -266,6 +252,27 @@ class RAFTNcup(_RAFTBase):
         """raft_nc_dbl.py:107-112 (without the caller's x8): nearest x2, then the NConv upsampler."""
         x4 = torch.nn.functional.interpolate(flow_lr, scale_factor=2, mode="nearest")
         return self.upsampler(x4, guidance)
+
+
+def _bidirectional_init(image1, image2, flow_init):
+    """The bidirectional forward's images checked and its flow_init pair (fw, bw) as one [2B,2,H/8,W/8] tensor, or None.  A
+    missing direction starts cold: coords0 + 0.0 is exactly coords0, as with no flow_init."""
+    if image1.shape != image2.shape or image1.dim() != 4:
+        raise ValueError(f"forward_bidirectional: expected two [B,3,H,W] images of one shape, got {tuple(image1.shape)} "
+                         f"and {tuple(image2.shape)}")
+    if flow_init is None:
+        return None
+    B, _, Him, Wim = image1.shape
+    if not isinstance(flow_init, (tuple, list)) or len(flow_init) != 2:
+        raise ValueError("flow_init: expected a pair (fw, bw), each [B,2,H/8,W/8] or None")
+    fw, bw = flow_init
+    for f in (fw, bw):
+        if f is not None and tuple(f.shape) != (B, 2, Him // 8, Wim // 8):
+            raise ValueError(f"flow_init: expected [B,2,H/8,W/8] = {(B, 2, Him // 8, Wim // 8)}, got {tuple(f.shape)}")
+    if fw is None and bw is None:
+        return None
+    ref = fw if fw is not None else bw
+    return torch.cat([(f if f is not None else torch.zeros_like(ref)).float() for f in (fw, bw)])
 
 
 def frozen_trunk(model, image1=None, image2=None, flow_init=None):

@@ -161,6 +161,14 @@ SIGNATURES = {
                              *[C.c_longlong] * 4, _vp, _vp, C.POINTER(_f), _i, _i, _i, _i, _vp, _vp, C.c_size_t, _vp]),
     "rnc_interp_error_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
     "rnc_interp_error": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_census_loss_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "rnc_census_loss_fwd": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _vp, _i, _i, _i,
+                                 _vp, _vp, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_census_loss_bwd": (_i, [_vp, _i, _i, _i, _vp, _vp, _vp]),
+    "rnc_smoothness_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "rnc_smoothness_fwd": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _f, _vp, _vp, _vp, _vp,
+                                C.c_size_t, _vp]),
+    "rnc_smoothness_bwd": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _f, _vp, _vp, _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind

@@ -39,6 +39,7 @@ from .engine import CORR_CH, _require_cuda, engine_for, pack_conv
 from .engine_umma import UmmaWeights, _ceil32
 from .native import rnc
 from .nconv_unet import is_fused, live_chain, nconv_fwd, pool_fwd, unused_parameters
+from .unsupervised import unsupervised_loss
 
 _PACK_CACHE = {}          # (id(weight), version, kind, fmt, cin_pad) -> (weight, packed); flushed at every training forward
 
@@ -644,20 +645,29 @@ def convex_upsample_train(flow, mask):
     return up.reshape(n, 2, 8 * h, 8 * w)
 
 
-def raft_forward_train(model, image1, image2, iters=12, flow_init=None, test_mode=False, return_confidence=False):
+def raft_forward_train(model, image1, image2, iters=12, flow_init=None, test_mode=False, return_confidence=False,
+                       bidirectional=False):
     """RAFT.forward with autograd (raft_nc_dbl.py:115-173 / raft.py:87-143): returns the list of `iters` full-resolution
     predictions (or (flow_low, flow_up) in test_mode).  return_confidence (NCUP model): also the NCUP output confidences,
-    as (predictions, confidences) or (flow_low, flow_up, confidence_up)."""
+    as (predictions, confidences) or (flow_low, flow_up, confidence_up).  bidirectional: 2B rows, row j image1[j] ->
+    image2[j] and row B + j the reverse, from one fnet and one cnet pass over cat(image1, image2): fmap1 is the 2B feature
+    rows, fmap2 the same rows with the halves swapped; flow_init [2B,2,H/8,W/8] or None."""
     _PACK_CACHE.clear()
     B, _, Him, Wim = image1.shape
     H8, W8 = Him // 8, Wim // 8
     dev = image1.device
     im1 = 2 * (image1.float() / 255.0) - 1.0
     im2 = 2 * (image2.float() / 255.0) - 1.0
-    fmaps = encoder_cl(model.fnet, to_cl(torch.cat([im1, im2], 0))).float()       # [2B,H8,W8,256]
-    f1, f2 = fmaps[:B].contiguous(), fmaps[B:].contiguous()
+    x = to_cl(torch.cat([im1, im2], 0))
+    fmaps = encoder_cl(model.fnet, x).float()                                       # [2B,H8,W8,256]
+    if bidirectional:
+        f1, f2 = fmaps.contiguous(), torch.cat([fmaps[B:], fmaps[:B]]).contiguous()
+        cnet = encoder_cl(model.cnet, x)
+        B = 2 * B
+    else:
+        f1, f2 = fmaps[:B].contiguous(), fmaps[B:].contiguous()
+        cnet = encoder_cl(model.cnet, to_cl(im1))
     pyr = CorrPyramid.apply(f2, 4)
-    cnet = encoder_cl(model.cnet, to_cl(im1))
     net, inp = torch.tanh(cnet[..., :128]), torch.relu(cnet[..., 128:])
     ys, xs = torch.meshgrid(torch.arange(H8, device=dev), torch.arange(W8, device=dev), indexing="ij")
     coords0 = torch.stack([xs, ys], 0).float()[None].repeat(B, 1, 1, 1)
@@ -723,6 +733,23 @@ def train_step(model, optimizer, scheduler, image1, image2, flow_gt, valid, iter
     optimizer.zero_grad()
     preds = model(image1, image2, iters=iters)
     loss, metrics = sequence_loss(preds, flow_gt, valid, gamma)
+    loss.backward()
+    torch.nn.utils.clip_grad_norm_(model.parameters(), clip)
+    optimizer.step()
+    if scheduler is not None:
+        scheduler.step()
+    return loss.detach(), (metrics if return_metrics else None)
+
+
+def unsupervised_step(model, optimizer, scheduler, image1, image2, iters=12, gamma=0.85, clip=1.0, smooth_weight=2.0,
+                      return_metrics=True):
+    """One unsupervised optimisation step on frame pairs without ground-truth flow: train_step's sequence with
+    model(image1, image2, iters=iters, bidirectional=True) (both directions, 2B rows) and rnc.unsupervised.unsupervised_loss
+    (census and smoothness terms, occlusion masks from the last prediction).  Through ddp_model the gradients are
+    all-reduced as train_step's are.  Returns (loss, metrics or None)."""
+    optimizer.zero_grad()
+    preds = model(image1, image2, iters=iters, bidirectional=True)
+    loss, metrics = unsupervised_loss(preds, image1, image2, gamma, smooth_weight)
     loss.backward()
     torch.nn.utils.clip_grad_norm_(model.parameters(), clip)
     optimizer.step()
