@@ -699,6 +699,47 @@ int rnc_smoothness_bwd(const float* image, long long ib, long long ic, long long
                        long long fb, long long fc, long long fy, long long fx, int N, int H, int W, float edge_constant,
                        const float* scale, float* grad_flow, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V8  point tracking through video by chaining the bidirectional flows, and the TAP-Vid metrics of the tracks (definition:
+ * rnc/track.py, DESIGN §3.17).  Shapes: 1 <= V <= 65535 videos, N >= 1 points, T >= 2 frames, N*T < 2^30, 1 <= H, W <= 2^24;
+ * RNC_ERR_BAD_SHAPE otherwise.  Bad arguments return before any launch.
+ *
+ * rnc_track: for each query (t, x, y) of video v, its position and visible flag in every frame.
+ *   flow, flow_bw : fp32 [V][T-1][2][H][W] through element strides (fv, fk, fc, fy, fx), F_k (frame k -> k+1) and G_k
+ *                   (frame k+1 -> k); 4-byte aligned
+ *   occ, occ_bw   : uint8 [V][T-1][H][W] through element strides, occ_k on frame k (of F_k) and occ_bw_k on frame k+1 (of G_k);
+ *                   a pixel is visible where 0
+ *   queries       : fp32 [V][N][3] contiguous, (t, x, y) with t an integer in [0, T-1] and (x, y) in [0, W-1] x [0, H-1]
+ *   tracks        : fp32 [V][N][T][2] contiguous (x, y), 8-byte aligned; visible: uint8 [V][N][T] contiguous
+ * At frame t the position is the query, visible.  Forward, for k = t .. T-2 from p at frame k: u = F_k^(p) (bilinear, the
+ * coordinates clamped to the frame); p' = p + u when both components are finite, else p; the point is lost at k+1 (and
+ * after) when it was lost at k, u is not finite, occ_k(rint(p)) != 0 (half to even) or p' is outside the frame; positions
+ * advance while lost.  Backward, for k = t-1 .. 0, the same with G_k and occ_bw_k from frame k+1 to frame k.  Every
+ * operation rounded once in float32 (no FMA).  One launch, a thread per query, no atomics, no host synchronisation.  A
+ * query outside the bounds above gets NaN positions and visible 0 in every frame.
+ *
+ * rnc_track_metrics: per video v, counts[v][RNC_TRACK_COUNTS] over the (point, frame) pairs except each point's query frame,
+ * with positions scaled to 256x256 (x * 256 / W, y * 256 / H, rounded once) and within_d = dx^2 + dy^2 < d^2 for
+ * d = 1, 2, 4, 8, 16: [0] pairs evaluated, [1] occlusion agreements (pred visible == gt visible), [2] gt visible,
+ * [3 + j] within_dj & gt visible, [8 + j] within_dj & gt visible & pred visible (true positives),
+ * [13 + j] pred visible & (!gt visible | !within_dj) (false positives).
+ *   tracks, gt_tracks   : fp32 [V][N][T][2] contiguous, 8-byte aligned; visible, gt_visible: uint8 [V][N][T] contiguous
+ *   queries             : fp32 [V][N][3] contiguous, as rnc_track's
+ *   counts              : int64 [V][RNC_TRACK_COUNTS], 8-byte aligned
+ *   workspace           : rnc_track_metrics_workspace_bytes(V, N, T) bytes, 16-byte aligned, no zeroing needed
+ * Two launches, no atomics, no host synchronisation: the counts are exact, whatever V or the video's position. */
+#define RNC_TRACK_THRESHOLDS 5
+#define RNC_TRACK_COUNTS 18
+int rnc_track(const float* flow, long long fv, long long fk, long long fc, long long fy, long long fx, const float* flow_bw,
+              long long gv, long long gk, long long gc, long long gy, long long gx, const unsigned char* occ, long long ov,
+              long long ok, long long oy, long long ox, const unsigned char* occ_bw, long long pv, long long pk, long long py,
+              long long px, const float* queries, int V, int N, int T, int H, int W, float* tracks, unsigned char* visible,
+              void* stream);
+size_t rnc_track_metrics_workspace_bytes(int V, int N, int T);   /* 0 for a bad shape */
+int rnc_track_metrics(const float* tracks, const unsigned char* visible, const float* gt_tracks,
+                      const unsigned char* gt_visible, const float* queries, int V, int N, int T, int H, int W,
+                      long long* counts, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,14 +28,17 @@ __device__ __forceinline__ PixelMetrics pixel_metrics(float f0, float f1, float 
   return {epe, mag, static_cast<bool>((epe > 3.0f) & (__fdiv_rn(epe, mag) > 0.05f))};
 }
 
-// An fp32 tensor through element strides: [B,C,H,W], or a [B,H,W] mask with c unused.
-struct View {
-  const float* p;
+// A tensor through element strides: [B,C,H,W], or a [B,H,W] mask with c unused.
+template <typename T>
+struct StridedView {
+  const T* p;
   long long b, c, y, x;
-  __device__ __forceinline__ const float* pixel(int bi, int yi, int xi) const { return p + bi * b + yi * y + xi * x; }
-  __device__ __forceinline__ float at(int bi, int ci, int yi, int xi) const { return pixel(bi, yi, xi)[ci * c]; }
-  __device__ __forceinline__ float at(int bi, int yi, int xi) const { return *pixel(bi, yi, xi); }
+  __device__ __forceinline__ const T* pixel(int bi, int yi, int xi) const { return p + bi * b + yi * y + xi * x; }
+  __device__ __forceinline__ T at(int bi, int ci, int yi, int xi) const { return pixel(bi, yi, xi)[ci * c]; }
+  __device__ __forceinline__ T at(int bi, int yi, int xi) const { return *pixel(bi, yi, xi); }
 };
+using View = StridedView<float>;
+using MaskView = StridedView<unsigned char>;       // uint8 masks, visible where 0
 
 inline bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 

@@ -18,6 +18,7 @@
 // rnc_interp_error: per image, the fp64 sum over its pixels of sum_c (pred - gt)^2 and its pixel count, by eval_common.cuh's
 // two fixed-order reductions, as rnc_flow_metrics: the order depends only on H*W, so an image's sum does not depend on N, on
 // its position in the batch or on the GPU.
+#include "bilinear.cuh"
 #include "dist_transform.cuh"
 #include "eval_common.cuh"
 
@@ -38,23 +39,6 @@ struct InterpArgs {
   int B, T, H, W;
   float t[kMaxTimes];
 };
-
-// frame c-plane at (px, py), bilinear with the coordinates clamped to [0, W-1] x [0, H-1]
-__device__ __forceinline__ float sample(const View& im, int b, int c, float px, float py, int H, int W) {
-  px = fminf(fmaxf(px, 0.0f), static_cast<float>(W - 1));
-  py = fminf(fmaxf(py, 0.0f), static_cast<float>(H - 1));
-  const float x0 = floorf(px), y0 = floorf(py);
-  const float ax = __fsub_rn(px, x0), ay = __fsub_rn(py, y0);
-  const float bx = __fsub_rn(1.0f, ax), by = __fsub_rn(1.0f, ay);
-  const int ix = static_cast<int>(x0), iy = static_cast<int>(y0);
-  const int ix1 = min(ix + 1, W - 1), iy1 = min(iy + 1, H - 1);
-  float s = __fmul_rn(im.at(b, c, iy, ix), __fmul_rn(bx, by));
-  s = __fadd_rn(s, __fmul_rn(im.at(b, c, iy, ix1), __fmul_rn(ax, by)));
-  s = __fadd_rn(s, __fmul_rn(im.at(b, c, iy1, ix), __fmul_rn(bx, ay)));
-  return __fadd_rn(s, __fmul_rn(im.at(b, c, iy1, ix1), __fmul_rn(ax, ay)));
-}
-
-__device__ __forceinline__ bool finite(float v) { return fabsf(v) <= 3.402823466e38f; }   // false for +-inf and NaN
 
 __global__ void __launch_bounds__(kInterpThreads) interp_splat_kernel(InterpArgs a) {
   const int s = blockIdx.z, b = blockIdx.y;

@@ -519,6 +519,82 @@ def validate_interpolation(model, sequences, iters=32, mode="sintel", batch_size
     return summarize_interpolation(from_images(InterpPartials, [t for seq in every for t in seq]))
 
 
+def track_points(model, sequences, queries, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
+                 alpha1=0.01, alpha2=0.5):
+    """Tracks of query points through whole videos (rnc.track's rule: the bidirectional flows chained from each query frame,
+    with a visible flag that turns off for good at the first occlusion, non-finite flow or exit from the frame).
+    sequences: list of V frame lists, every frame [3,H,W] (0..255) of one size, each video of T_v >= 2 frames; queries: V
+    float32 [N_v,3] tensors (or a [V,N,3] tensor) of (t, x, y), t an integer frame index and (x, y) pixel coordinates in the
+    frame (rnc.track.grid_queries gives dense queries).  Returns a list of V (tracks float32 [N_v,T_v,2], visible uint8
+    [N_v,T_v]) on the device.
+
+    run_sequences_bidirectional(model, sequences, iters, warm_start, batch_size, mode, device, alpha1=alpha1, alpha2=alpha2)
+    runs first, and each pair's flow_up, flow_up_bw, occ and occ_bw are copied into stacked device tensors as they are yielded:
+    with T the longest video's frame count, V (T - 1) (2 flows x 2 channels x 4 B + 2 masks x 1 B) = 18 V (T - 1) bytes per
+    pixel, e.g. 3.2 GB for eight 50-frame videos of 436x1024.  A shorter video's missing pairs are zero flows with every
+    pixel occluded; they only extend its tracks past its last frame, and those frames are dropped.  Then rnc.track.track runs
+    once over all videos, one launch, so each track is what rnc.track.track gives for its video alone.  ValueError before the
+    flow pass for a video of fewer than two frames, a bad query or a query count that does not match the videos.  Inference
+    only: with grad enabled on a model that requires grad it raises ValueError."""
+    from .track import check_queries, track
+    if model._needs_grad():
+        raise ValueError("track_points is inference only: call it under torch.no_grad()")
+    qs = list(queries)
+    if len(qs) != len(sequences):
+        raise ValueError(f"track_points: {len(sequences)} videos but {len(qs)} query sets")
+    if not sequences:
+        return []
+    H, W = sequences[0][0].shape[-2:]
+    lens = [len(seq) for seq in sequences]
+    for T, q in zip(lens, qs):
+        if q.dim() != 2:
+            raise ValueError(f"track_points: expected each video's queries as [N,3], got {tuple(q.shape)}")
+        check_queries(q, T, H, W, "track_points")
+    V, T, N = len(sequences), max(lens), max(q.shape[0] for q in qs)
+    flows = None
+    for s, k, r in run_sequences_bidirectional(model, sequences, iters, warm_start=warm_start, batch_size=batch_size,
+                                               mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
+        if flows is None:
+            dev = r["flow_up"].device
+            flows = {name: torch.zeros(V, T - 1, 2, H, W, dtype=torch.float32, device=dev) for name in ("flow_up", "flow_up_bw")}
+            flows.update({name: torch.ones(V, T - 1, H, W, dtype=torch.uint8, device=dev) for name in ("occ", "occ_bw")})
+        for name, t in flows.items():
+            t[s, k].copy_(r[name])
+    q = torch.zeros(V, N, 3, dtype=torch.float32, device=dev)   # (0, 0, 0) pads a video's queries to N; its tracks are dropped
+    for v, qv in enumerate(qs):
+        q[v, :qv.shape[0]] = qv
+    tracks, visible = track(flows["flow_up"], flows["flow_up_bw"], flows["occ"], flows["occ_bw"], q)
+    return [(tracks[v, :qv.shape[0], :lens[v]], visible[v, :qv.shape[0], :lens[v]]) for v, qv in enumerate(qs)]
+
+
+@torch.no_grad()
+def validate_tracking(model, sequences, queries, gt_tracks, gt_visible, iters=32, warm_start=False, batch_size=8,
+                      mode="sintel", device="cuda", alpha1=0.01, alpha2=0.5):
+    """TAP-Vid's metrics of track_points on a split of videos: occlusion_accuracy, average_pts_within_thresh (< delta^x_avg),
+    average_jaccard, their per-threshold terms and the video count (rnc.track.summarize_tracking).  sequences and queries as
+    track_points'; gt_tracks: V [N_v,T_v,2] (x, y) pixel positions; gt_visible: V [N_v,T_v] (non-zero is visible, TAP-Vid's
+    `occluded` negated).  Each video's counts come from rnc.track.track_metrics on the device; they are integers, so the
+    result does not depend on batch_size or on the order of the videos.  Under torch.distributed rank r takes the videos of
+    index = r (mod world), the per-video counts are all-gathered, and every rank returns the single-process result."""
+    from .dist import gather_strided, strided_items, world_rank
+    from .track import summarize_tracking, track_metrics
+    world, rank = world_rank()
+    mine = list(strided_items(range(len(sequences)), world, rank))
+    if len(queries) != len(sequences) or len(gt_tracks) != len(sequences) or len(gt_visible) != len(sequences):
+        raise ValueError(f"validate_tracking: {len(sequences)} videos but {len(queries)} query sets, {len(gt_tracks)} "
+                         f"ground-truth tracks and {len(gt_visible)} visibility sets")
+    got = track_points(model, [sequences[i] for i in mine], [queries[i] for i in mine], iters, warm_start, batch_size, mode,
+                       device, alpha1, alpha2)
+    counts = []
+    for i, (tr, vis) in zip(mine, got):
+        H, W = sequences[i][0].shape[-2:]
+        dev = tr.device
+        c = track_metrics(tr[None], vis[None], gt_tracks[i][None].to(dev), gt_visible[i][None].to(dev),
+                          queries[i][None].to(dev), H, W)
+        counts.append(c[0].tolist())
+    return summarize_tracking(gather_strided(counts, world))
+
+
 def size_batches(items, batch_size, key):
     """Batches of create_kitti_submission: the items of one key(item) (a frame size) in order of appearance, batch_size at a
     time.  A batch is yielded as soon as it is full, the partial batches at the end in order of their size's first
