@@ -740,6 +740,46 @@ int rnc_track_metrics(const float* tracks, const unsigned char* visible, const f
                       const unsigned char* gt_visible, const float* queries, int V, int N, int T, int H, int W,
                       long long* counts, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V9  video object segmentation: first-frame labels propagated along the backward flows, and the DAVIS semi-supervised
+ * metrics J and F as exact counts (definition: rnc/segment.py, DESIGN §3.18).  Bad arguments return before any launch.
+ *
+ * rnc_propagate_labels: one step k -> k+1 of V videos, L_{k+1} from L_k, G_k and occ_bw_k.
+ *   labels    : uint8 [V][H][W] through element strides (lv, ly, lx), L_k; 0 background, 1..254 objects (255 is not a label)
+ *   flow_bw   : fp32 [V][2][H][W] through element strides (gv, gc, gy, gx), G_k (frame k+1 -> k); 4-byte aligned
+ *   occ_bw    : uint8 [V][H][W] through element strides, on frame k+1; a pixel is visible where 0
+ *   out       : uint8 [V][H][W] through element strides (qv, qy, qx), L_{k+1}; must not overlap labels
+ *   workspace : rnc_propagate_labels_workspace_bytes(V, H, W) bytes, 16-byte aligned, no zeroing needed (an int32 map)
+ * A pixel p of frame k+1 is matched when u = G_k(p) has both components finite, occ_bw_k(p) == 0 and p' = p + u lies in
+ * [0, W-1] x [0, H-1]; it takes the bilinear vote of L_k at p': taps (y0,x0), (y0,x1), (y1,x0), (y1,x1) (x1 = min(x0+1, W-1),
+ * y1 likewise) weighted bx*by, ax*by, bx*ay, ax*ay, each label's weights added in tap order, the largest sum winning and a
+ * tie going to the smaller label.  An unmatched pixel takes the label of the nearest matched pixel of frame k+1 (exact squared
+ * distance, ties to the smallest column, then row); 0 in a frame without a matched pixel.  Every operation rounded once in
+ * float32 (no FMA).  Three launches, no atomics, no host synchronisation.  RNC_ERR_BAD_SHAPE unless 1 <= V <= 65535 and
+ * 1 <= H, W <= 4096.
+ *
+ * rnc_segmentation_counts: per frame n and object o = 1..K, counts[n][o-1][RNC_SEGMENT_COUNTS] with void = gt == 255,
+ * M = pred == o & !void, G = gt == o, and bM, bG their boundary maps (the DAVIS toolkit's seg2bmap at full resolution:
+ * s differs from its right, lower or lower-right neighbour; on the last row from its right one, on the last column from its
+ * lower one; never the bottom-right pixel): [0] |M & G|, [1] |M | G|, [2] |bM|, [3] |bG|, [4] bM pixels with a bG pixel at
+ * squared distance <= r^2, [5] bG pixels with a bM pixel at squared distance <= r^2, r = ceil(0.008 sqrt(H^2 + W^2)) in fp64.
+ *   pred, gt  : uint8 [N][H][W] through element strides (pn, py, px), (gn, gy, gx)
+ *   counts    : int64 [N][K][RNC_SEGMENT_COUNTS], 8-byte aligned
+ *   workspace : rnc_segmentation_counts_workspace_bytes(N, K, H, W) bytes, 16-byte aligned, no zeroing needed: the int32
+ *               distance maps [2][N][K][H][W], then the per-CTA partials
+ * Four launches, no atomics, no host synchronisation: the counts are exact, whatever N or the frame's position.
+ * RNC_ERR_BAD_SHAPE unless N, K >= 1, K <= 254, 2 N K <= 65535 and 1 <= H, W <= 4096. */
+#define RNC_SEGMENT_COUNTS 6
+size_t rnc_propagate_labels_workspace_bytes(int V, int H, int W);   /* 0 for a bad shape */
+int rnc_propagate_labels(const unsigned char* labels, long long lv, long long ly, long long lx, const float* flow_bw,
+                         long long gv, long long gc, long long gy, long long gx, const unsigned char* occ_bw, long long ov,
+                         long long oy, long long ox, int V, int H, int W, unsigned char* out, long long qv, long long qy,
+                         long long qx, void* workspace, size_t workspace_bytes, void* stream);
+size_t rnc_segmentation_counts_workspace_bytes(int N, int K, int H, int W);   /* 0 for a bad shape */
+int rnc_segmentation_counts(const unsigned char* pred, long long pn, long long py, long long px, const unsigned char* gt,
+                            long long gn, long long gy, long long gx, int N, int K, int H, int W, long long* counts,
+                            void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,7 +1,8 @@
 // The exact nearest "site" of every pixel of a batch of images, as a separable transform in integers (Felzenszwalb and
 // Huttenlocher, "Distance Transforms of Sampled Functions", 2012).  Shared by rnc_boundary_dist2 (region_metrics.cu: the sites
 // are occlusion-boundary pixels, the output the squared distance) and rnc_interpolate (interp.cu: the sites are the pixels that
-// received a splatted motion, the output the index of the nearest one, a feature transform).
+// received a splatted motion, the output the index of the nearest one, a feature transform), and by segment.cu
+// (rnc_propagate_labels: the voted pixels, the output their label; rnc_segmentation_counts: mask boundaries, squared distances).
 //   1. dist2_column_kernel<Sites>, a thread per column of one image: a downward and an upward sweep give the row of the nearest
 //      site in the same column (the upper one on a tie; -1 if the column has none).
 //   2. dist2_row_kernel<Out>, a warp per row: with g(q) the distance from (y, q) to column q's nearest site, the nearest site
@@ -16,9 +17,18 @@
 // Sites: `__device__ bool operator()(int image, int y, int x) const`, true at a site.  Out: `none`, written in an image without
 // a site, and `__device__ int operator()(int y, int x, int q, int r, int fq) const`, the value of pixel (y, x) whose nearest site
 // is (r, q), with fq = (y - r)^2 + q^2.  Images are [images][H][W] contiguous in the int map; 1 <= H, W <= kSiteMaxSide.
+// An Out with `static constexpr bool kStores = true` writes each pixel's result itself instead, through
+// `__device__ void store(int image, int y, int x, int q, int r) const` (q = r = -1 in an image without a site), and the row
+// pass leaves the int map as the column pass wrote it (rnc_propagate_labels: the site's label, gathered into a uint8 map).
 #pragma once
+#include <type_traits>
 
 namespace rnc {
+
+template <class Out, class = void>
+struct out_stores : std::false_type {};
+template <class Out>
+struct out_stores<Out, std::void_t<decltype(Out::kStores)>> : std::bool_constant<Out::kStores> {};
 
 constexpr int kSiteMaxSide = 4096;        // the row pass keeps 8 W bytes of shared memory and 16-bit column / row indices
 constexpr int kSiteColThreads = 128;
@@ -87,7 +97,11 @@ __global__ void __launch_bounds__(32) dist2_row_kernel(int H, int W, int* __rest
   n = __shfl_sync(0xffffffffu, n, 0);
   for (int x = lane; x < W; x += 32) {
     if (n == 0) {                          // no site in the image
-      row[x] = o.none;
+      if constexpr (out_stores<Out>::value) {
+        o.store(blockIdx.y, y, x, -1, -1);
+      } else {
+        row[x] = o.none;
+      }
       continue;
     }
     // the last k with k == 0 or x > s(v[k-1], v[k]): on a tie the left parabola, the smaller column, is kept
@@ -102,7 +116,11 @@ __global__ void __launch_bounds__(32) dist2_row_kernel(int H, int W, int* __rest
       }
     }
     const int q = v[lo];
-    row[x] = o(y, x, q, R[q], F[q]);
+    if constexpr (out_stores<Out>::value) {
+      o.store(blockIdx.y, y, x, q, R[q]);
+    } else {
+      row[x] = o(y, x, q, R[q], F[q]);
+    }
   }
 }
 

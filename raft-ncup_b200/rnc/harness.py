@@ -595,6 +595,92 @@ def validate_tracking(model, sequences, queries, gt_tracks, gt_visible, iters=32
     return summarize_tracking(gather_strided(counts, world))
 
 
+def propagate_masks(model, sequences, first_labels, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
+                    alpha1=0.01, alpha2=0.5):
+    """The labels of every frame of V videos from those of frame 0 (rnc.segment's rule: each pixel of frame k+1 takes the
+    bilinear vote of frame k's labels at the end of its backward flow, or, where that flow is occluded, non-finite or leaves
+    the frame, the label of its nearest pixel that has a vote).  sequences: list of V frame lists, every frame [3,H,W]
+    (0..255) of one size, each video of T_v >= 2 frames; first_labels: V integer [H,W] label maps of frame 0 (0 background,
+    1..254 objects).  Returns a list of V uint8 [T_v,H,W] label tensors on the device.
+
+    run_sequences_bidirectional(model, sequences, iters, warm_start, batch_size, mode, device, alpha1=alpha1, alpha2=alpha2)
+    yields each video's pairs in order, and pair k's flow_up_bw and occ_bw step that video's labels from frame k to k + 1 at
+    once (rnc.segment.propagate_step's rule, one rnc_propagate_labels call), so no flow is kept: the memory is the labels, one
+    byte per pixel per frame.  ValueError before the flow pass for a video of fewer than two frames, first labels of another
+    size, a label outside 0..254 or a label-map count that does not match the videos.  Inference only: with grad enabled on
+    a model that requires grad it raises ValueError."""
+    from . import native
+    from .segment import _check_sides, _step, check_labels
+    if model._needs_grad():
+        raise ValueError("propagate_masks is inference only: call it under torch.no_grad()")
+    firsts = list(first_labels)
+    if len(firsts) != len(sequences):
+        raise ValueError(f"propagate_masks: {len(sequences)} videos but {len(firsts)} first-frame label maps")
+    if not sequences:
+        return []
+    for seq, first in zip(sequences, firsts):
+        if len(seq) < 2:
+            raise ValueError(f"propagate_masks: a video needs T >= 2 frames, got {len(seq)}")
+        if tuple(first.shape) != tuple(seq[0].shape[-2:]):
+            raise ValueError(f"propagate_masks: expected first labels {list(seq[0].shape[-2:])}, got {list(first.shape)}")
+        _check_sides(*first.shape, "propagate_masks")
+        check_labels(first, "propagate_masks")
+    out, ws = None, None
+    for s, k, r in run_sequences_bidirectional(model, sequences, iters, warm_start=warm_start, batch_size=batch_size,
+                                               mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
+        if out is None:
+            dev = r["flow_up_bw"].device
+            out = [torch.empty(len(seq), *first.shape, dtype=torch.uint8, device=dev) for seq, first in zip(sequences, firsts)]
+            for o, first in zip(out, firsts):
+                o[0] = first
+            if dev.type == "cuda":
+                ws = torch.empty(native.rnc.propagate_labels_workspace_bytes(1, *firsts[0].shape), dtype=torch.uint8,
+                                 device=dev)
+        labels = out[s]
+        _step(labels[k][None], r["flow_up_bw"][None], r["occ_bw"][None], labels[k + 1][None], ws)
+    return out
+
+
+@torch.no_grad()
+def validate_segmentation(model, sequences, gt_labels, iters=32, warm_start=False, batch_size=8, mode="sintel",
+                          device="cuda", alpha1=0.01, alpha2=0.5):
+    """DAVIS's semi-supervised J and F of propagate_masks on a split of videos: J&F-Mean, J-Mean, J-Recall, J-Decay, F-Mean,
+    F-Recall, F-Decay and the object and video counts (rnc.segment.summarize_segmentation).  sequences: list of V frame
+    lists, every frame [3,H,W] (0..255), each video of T_v >= 3 frames and one size (videos may differ in size); gt_labels: V
+    integer [T_v,H,W] label maps (0 background, 1..254 objects, 255 void).  Each video starts from its ground truth's frame 0
+    with void mapped to 0; its objects are 1..K, K its frame 0's largest non-void label, scored on frames 1..T_v-2 by
+    rnc.segment.segmentation_counts on the device.  Videos of one frame size run through one propagate_masks call.  The
+    counts are integers, so the result does not depend on batch_size or on the order of the videos.  Under
+    torch.distributed rank r takes the videos of index = r (mod world), the per-video counts are all-gathered, and every rank
+    returns the single-process result."""
+    from .dist import gather_strided, strided_items, world_rank
+    from .segment import VOID, segmentation_counts, summarize_segmentation
+    world, rank = world_rank()
+    if len(gt_labels) != len(sequences):
+        raise ValueError(f"validate_segmentation: {len(sequences)} videos but {len(gt_labels)} ground-truth label sets")
+    for seq, gt in zip(sequences, gt_labels):
+        if len(seq) < 3:
+            raise ValueError(f"validate_segmentation: a video needs T >= 3 frames (the first and last are not scored), got "
+                             f"{len(seq)}")
+        if tuple(gt.shape) != (len(seq), *seq[0].shape[-2:]):
+            raise ValueError(f"validate_segmentation: expected ground truth {[len(seq), *seq[0].shape[-2:]]}, got "
+                             f"{list(gt.shape)}")
+    mine = list(strided_items(range(len(sequences)), world, rank))
+    by_size = {}
+    for i in mine:
+        by_size.setdefault(tuple(sequences[i][0].shape[-2:]), []).append(i)
+    counts = {}
+    for idx in by_size.values():
+        firsts = [torch.where(gt_labels[i][0] == VOID, 0, gt_labels[i][0]) for i in idx]
+        preds = propagate_masks(model, [sequences[i] for i in idx], firsts, iters, warm_start, batch_size, mode, device,
+                                alpha1, alpha2)
+        for i, first, pred in zip(idx, firsts, preds):
+            K = int(first.max())
+            gt = gt_labels[i].to(pred.device)
+            counts[i] = segmentation_counts(pred[1:-1], gt[1:-1], K).tolist()
+    return summarize_segmentation(gather_strided([counts[i] for i in mine], world))
+
+
 def size_batches(items, batch_size, key):
     """Batches of create_kitti_submission: the items of one key(item) (a frame size) in order of appearance, batch_size at a
     time.  A batch is yielded as soon as it is full, the partial batches at the end in order of their size's first

@@ -173,12 +173,19 @@ SIGNATURES = {
                        _vp, _i, _i, _i, _i, _i, _vp, _vp, _vp]),
     "rnc_track_metrics_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
     "rnc_track_metrics": (_i, [_vp, _vp, _vp, _vp, _vp, _i, _i, _i, _i, _i, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_propagate_labels_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "rnc_propagate_labels": (_i, [_vp, *[C.c_longlong] * 3, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 3, _i, _i, _i,
+                                  _vp, *[C.c_longlong] * 3, _vp, C.c_size_t, _vp]),
+    "rnc_segmentation_counts_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
+    "rnc_segmentation_counts": (_i, [_vp, *[C.c_longlong] * 3, _vp, *[C.c_longlong] * 3, _i, _i, _i, _i, _vp, _vp, C.c_size_t,
+                                     _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind
 REGION_CELLS = {REGIONS_SINTEL: 32, REGIONS_KITTI: 4}
 INTERP_MAX_TIMES = 64                                      # RNC_INTERP_MAX_TIMES
 TRACK_THRESHOLDS, TRACK_COUNTS = 5, 18                     # RNC_TRACK_THRESHOLDS, RNC_TRACK_COUNTS
+SEGMENT_COUNTS = 6                                         # RNC_SEGMENT_COUNTS
 
 _lib = None
 _lock = threading.Lock()
