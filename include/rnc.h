@@ -780,6 +780,69 @@ int rnc_segmentation_counts(const unsigned char* pred, long long pn, long long p
                             long long gn, long long gy, long long gx, int N, int K, int H, int W, long long* counts,
                             void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V10  flow-guided video inpainting: the harmonic fill that completes a field inside a hole, the temporal propagation of
+ * colours along the completed flows, and SSIM's per-frame partials (definition: rnc/inpaint.py, DESIGN §3.19).  Every
+ * floating-point operation rounded once in float32 (no FMA); no atomics, no host synchronisation.  Bad arguments return
+ * before any launch.
+ *
+ * rnc_harmonic_fill: N = A*B images of C channels, image (a, b).
+ *   values    : fp32 [A][B][C][H][W] through element strides (va, vb, vc, vy, vx); 4-byte aligned
+ *   unknown   : uint8 [A][B][H][W] through element strides; a pixel is filled where non-zero
+ *   out       : fp32 [A][B][C][H][W] through element strides (oa, ob, oc, oy, ox); may be values itself, otherwise must not
+ *               overlap it
+ *   workspace : rnc_harmonic_fill_workspace_bytes(A, B, C, H, W) bytes, 16-byte aligned, no zeroing needed
+ * A pixel is known when unknown is 0 there and all C values are finite; out holds it unchanged.  Every other pixel starts from
+ * its nearest known pixel's values (exact squared distance, ties to the smallest column, then row), 0 in an image without one,
+ * and then `sweeps` red-black SOR sweeps ((x + y) even first) run over the unknown pixels: per channel s = the in-frame
+ * 4-neighbours added up, left, right, down, u += omega (s / n - u), omega = 2 / (1 + pi_f32 / (L + 1)) with L the larger
+ * side of the image's unknown pixels' bounding box.  5 + 2 sweeps launches.  RNC_ERR_BAD_SHAPE unless 1 <= A*B <= 65535,
+ * 1 <= C <= RNC_HARMONIC_MAX_CHANNELS, 1 <= H, W <= 4096 and sweeps >= 0.
+ *
+ * rnc_inpaint_propagate: V videos of T frames, the colour of every hole pixel from the nearest frames along its chains.
+ *   frames    : fp32 [V][T][3][H][W] through element strides (iv, it, ic, iy, ix), I_t in 0..255
+ *   masks     : uint8 [V][T][H][W] through element strides, M_t; a hole where non-zero
+ *   flow      : fp32 [V][T-1][2][H][W] through element strides, the completed F~_k; flow_bw likewise G~_k
+ *   occ       : uint8 [V][T-1][H][W] through element strides, occ~_k on frame k; occ_bw likewise occ~_bw_k on frame k+1
+ *   out       : fp32 [V][T][3][H][W] contiguous; source : uint8 [V][T][H][W] contiguous (RNC_INPAINT_*)
+ * A hole pixel's forward chain from x = p at frame k = t stops without a candidate at k = T-1, after max_distance steps, at
+ * occ~_k(rint(x)) != 0 or when x + F~_k^(x) (bilinear.cuh's clamped sample) leaves [0, W-1] x [0, H-1]; it ends with a
+ * candidate at the first frame k where M_k(rint(x)) == 0, whose colour is the bilinear taps of I_k at x outside the hole,
+ * weights and weighted colours added in tap order, over their weights' sum.  The backward chain likewise with G~_{k-1} and
+ * occ~_bw_{k-1}.  Both: (d_b c_f + d_f c_b) / (d_f + d_b); one: its colour; none: 0 and RNC_INPAINT_SPATIAL.  A pixel
+ * outside the holes copies its colour.  One launch.  RNC_ERR_BAD_SHAPE unless 1 <= V <= 65535, 2 <= T <= 65535,
+ * 1 <= H, W <= 4096 and max_distance >= 1.
+ *
+ * rnc_ssim_partials: per frame n, SSIM (Wang et al. 2004) of pred against gt over the 3 channels and the pixels whose 11x11
+ * window lies inside the frame: the separable Gaussian of sigma 1.5 (normalised in fp64, float32 taps), rows then columns,
+ * C1 = (0.01*255)^2, C2 = (0.03*255)^2.  sum[n] is the fp64 sum of the map, count[n] its number of terms, through the
+ * evaluation kernels' fixed-order reductions, so a frame's result does not depend on N, its position or the GPU.
+ *   pred, gt  : fp32 [N][3][H][W] through element strides; sum fp64 [N], count int64 [N], 8-byte aligned
+ *   workspace : rnc_ssim_partials_workspace_bytes(N, H, W) bytes, 16-byte aligned
+ * RNC_ERR_BAD_SHAPE unless 1 <= N <= 65535, H, W >= 11 and H*W < 2^30. */
+#define RNC_HARMONIC_MAX_CHANNELS 4
+#define RNC_INPAINT_KNOWN 0
+#define RNC_INPAINT_FORWARD 1
+#define RNC_INPAINT_BACKWARD 2
+#define RNC_INPAINT_BOTH 3
+#define RNC_INPAINT_SPATIAL 4
+size_t rnc_harmonic_fill_workspace_bytes(int A, int B, int C, int H, int W);   /* 0 for a bad shape */
+int rnc_harmonic_fill(const float* values, long long va, long long vb, long long vc, long long vy, long long vx,
+                      const unsigned char* unknown, long long ua, long long ub, long long uy, long long ux, int A, int B,
+                      int C, int H, int W, int sweeps, float* out, long long oa, long long ob, long long oc, long long oy,
+                      long long ox, void* workspace, size_t workspace_bytes, void* stream);
+int rnc_inpaint_propagate(const float* frames, long long iv, long long it, long long ic, long long iy, long long ix,
+                          const unsigned char* masks, long long mv, long long mt, long long my, long long mx,
+                          const float* flow, long long fv, long long fk, long long fc, long long fy, long long fx,
+                          const float* flow_bw, long long gv, long long gk, long long gc, long long gy, long long gx,
+                          const unsigned char* occ, long long ov, long long ok, long long oy, long long ox,
+                          const unsigned char* occ_bw, long long pv, long long pk, long long py, long long px, int V, int T,
+                          int H, int W, int max_distance, float* out, unsigned char* source, void* stream);
+size_t rnc_ssim_partials_workspace_bytes(int N, int H, int W);   /* 0 for a bad shape */
+int rnc_ssim_partials(const float* pred, long long pn, long long pc, long long py, long long px, const float* gt,
+                      long long gn, long long gc, long long gy, long long gx, int N, int H, int W, double* sum,
+                      long long* count, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -681,6 +681,103 @@ def validate_segmentation(model, sequences, gt_labels, iters=32, warm_start=Fals
     return summarize_segmentation(gather_strided([counts[i] for i in mine], world))
 
 
+def inpaint_videos(model, sequences, masks, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
+                   alpha1=0.01, alpha2=0.5, sweeps=512, max_distance=None):
+    """Remove the masked regions of V videos (rnc.inpaint's rule: complete the flows inside the holes, carry each hole pixel
+    along them to the nearest frames that see it, fill what no frame sees spatially).  sequences: list of V frame lists,
+    every frame [3,H,W] (0..255), each video of T_v >= 2 frames and one size (videos may differ in size); masks: V [T_v,H,W]
+    tensors, non-zero where a pixel is to be filled.  Returns a list of V (frames float32 [T_v,3,H,W], source uint8
+    [T_v,H,W]) on the device, source being rnc.inpaint's SOURCE_* map.
+
+    The model sees the frames with every hole pixel set to 0, so the result depends only on the known pixels, as an
+    inpainting benchmark feeds a corrupted video.  Videos of one frame size run together:
+    run_sequences_bidirectional(model, ..., iters, warm_start, batch_size, mode, device) runs first, and each pair's flow_up
+    and flow_up_bw are copied into stacked device tensors as they are yielded; a shorter video's missing pairs are zero flows
+    occluded in both directions, so no chain enters them.  rnc.inpaint's steps 2-4 then complete the stacked flows in place
+    (harmonic_fill with `sweeps`), check them with fb_consistency(alpha1, alpha2), propagate (chains of at most
+    max_distance frames; None: no limit) and fill the rest.  With T the longest video's frame count, a size group keeps
+    V T (12 B frames + 12 B result + 1 B mask + 1 B source) + V (T - 1) (2 flows x 2 channels x 4 B + 2 masks x 1 B) ~ 44
+    V T bytes per pixel, plus at most 1 GiB of fill workspace: e.g. 7.2 GB for eight 50-frame videos of 480x854.
+    ValueError before the flow pass for a video of fewer than two frames, a mask of another shape, a side above 4096, a
+    mask count that does not match the videos, sweeps < 0 or max_distance < 1.  Inference only: with grad enabled on a
+    model that requires grad it raises ValueError."""
+    from .inpaint import _check_sides, _check_sweeps, _max_distance, _run
+    if model._needs_grad():
+        raise ValueError("inpaint_videos is inference only: call it under torch.no_grad()")
+    masks = list(masks)
+    if len(masks) != len(sequences):
+        raise ValueError(f"inpaint_videos: {len(sequences)} videos but {len(masks)} mask sets")
+    _check_sweeps(sweeps, "inpaint_videos")
+    for seq, m in zip(sequences, masks):
+        if len(seq) < 2:
+            raise ValueError(f"inpaint_videos: a video needs T >= 2 frames, got {len(seq)}")
+        if tuple(m.shape) != (len(seq), *seq[0].shape[-2:]):
+            raise ValueError(f"inpaint_videos: expected masks {[len(seq), *seq[0].shape[-2:]]}, got {list(m.shape)}")
+        _check_sides(*m.shape[-2:], "inpaint_videos")
+        _max_distance(max_distance, len(seq), "inpaint_videos")
+    by_size = {}
+    for i, seq in enumerate(sequences):
+        by_size.setdefault(tuple(seq[0].shape[-2:]), []).append(i)
+    out = [None] * len(sequences)
+    for idx in by_size.values():
+        seqs = [sequences[i] for i in idx]
+        holes = [masks[i] != 0 for i in idx]
+        seen = [[torch.where(h[t].to(f.device), 0.0, f.float()) for t, f in enumerate(seq)] for seq, h in zip(seqs, holes)]
+        lens = [len(seq) for seq in seqs]
+        V, T = len(seqs), max(lens)
+        H, W = seqs[0][0].shape[-2:]
+        flows = None
+        for s, k, r in run_sequences_bidirectional(model, seen, iters, warm_start=warm_start, batch_size=batch_size,
+                                                   mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
+            if flows is None:
+                dev = r["flow_up"].device
+                flows = [torch.zeros(V, T - 1, 2, H, W, dtype=torch.float32, device=dev) for _ in range(2)]
+            flows[0][s, k].copy_(r["flow_up"])
+            flows[1][s, k].copy_(r["flow_up_bw"])
+        frames = torch.zeros(V, T, 3, H, W, dtype=torch.float32, device=dev)
+        hole = torch.zeros(V, T, H, W, dtype=torch.uint8, device=dev)
+        for v, (seq, h) in enumerate(zip(seqs, holes)):
+            frames[v, :lens[v]] = torch.stack([f.to(dev).float() for f in seq])
+            hole[v, :lens[v]] = h.to(dev)
+        res, source = _run(frames, hole, flows[0], flows[1], sweeps, max_distance, alpha1, alpha2, lengths=lens)
+        for v, i in enumerate(idx):
+            out[i] = (res[v, :lens[v]], source[v, :lens[v]])
+    return out
+
+
+@torch.no_grad()
+def validate_inpainting(model, sequences, masks, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
+                        alpha1=0.01, alpha2=0.5, sweeps=512, max_distance=None):
+    """PSNR and SSIM of inpaint_videos against the uncorrupted videos: psnr, ssim, and the scored frame and video counts
+    (rnc.inpaint.summarize_inpainting).  sequences: the ground-truth videos, as inpaint_videos takes them; masks: V [T_v,H,W]
+    hole masks.  Only frames with at least one hole pixel are scored: PSNR from rnc.interp.interpolation_error's fp64
+    squared-error sum (100 dB for a frame without error), SSIM from rnc.inpaint.ssim, each averaged over a video's scored
+    frames and then over videos.  A frame's partials do not depend on the batch.  Under torch.distributed rank r takes the
+    videos of index = r (mod world), the per-frame partials are all-gathered, and every rank returns the single-process
+    result."""
+    from .dist import gather_strided, strided_items, world_rank
+    from .inpaint import ssim, summarize_inpainting
+    from .interp import interpolation_error
+    world, rank = world_rank()
+    if len(masks) != len(sequences):
+        raise ValueError(f"validate_inpainting: {len(sequences)} videos but {len(masks)} mask sets")
+    mine = list(strided_items(range(len(sequences)), world, rank))
+    got = inpaint_videos(model, [sequences[i] for i in mine], [masks[i] for i in mine], iters, warm_start, batch_size, mode,
+                         device, alpha1, alpha2, sweeps, max_distance)
+    records = []
+    for i, (pred, _) in zip(mine, got):
+        dev = pred.device
+        scored = (masks[i] != 0).flatten(1).any(1).nonzero().flatten().tolist()
+        if not scored:
+            records.append([])
+            continue
+        gt = torch.stack([sequences[i][t].to(dev).float() for t in scored])
+        err = interpolation_error(pred[scored], gt)
+        s, c = ssim(pred[scored], gt)
+        records.append([list(r) for r in zip(err.sq_sum.tolist(), err.count.tolist(), s.tolist(), c.tolist())])
+    return summarize_inpainting(gather_strided(records, world))
+
+
 def size_batches(items, batch_size, key):
     """Batches of create_kitti_submission: the items of one key(item) (a frame size) in order of appearance, batch_size at a
     time.  A batch is yielded as soon as it is full, the partial batches at the end in order of their size's first

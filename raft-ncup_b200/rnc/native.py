@@ -179,6 +179,14 @@ SIGNATURES = {
     "rnc_segmentation_counts_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
     "rnc_segmentation_counts": (_i, [_vp, *[C.c_longlong] * 3, _vp, *[C.c_longlong] * 3, _i, _i, _i, _i, _vp, _vp, C.c_size_t,
                                      _vp]),
+    "rnc_harmonic_fill_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i]),
+    "rnc_harmonic_fill": (_i, [_vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 4, _i, _i, _i, _i, _i, _i, _vp,
+                               *[C.c_longlong] * 5, _vp, C.c_size_t, _vp]),
+    "rnc_inpaint_propagate": (_i, [_vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 5, _vp,
+                                   *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _i, _i,
+                                   _vp, _vp, _vp]),
+    "rnc_ssim_partials_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
+    "rnc_ssim_partials": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind
@@ -186,6 +194,9 @@ REGION_CELLS = {REGIONS_SINTEL: 32, REGIONS_KITTI: 4}
 INTERP_MAX_TIMES = 64                                      # RNC_INTERP_MAX_TIMES
 TRACK_THRESHOLDS, TRACK_COUNTS = 5, 18                     # RNC_TRACK_THRESHOLDS, RNC_TRACK_COUNTS
 SEGMENT_COUNTS = 6                                         # RNC_SEGMENT_COUNTS
+HARMONIC_MAX_CHANNELS = 4                                  # RNC_HARMONIC_MAX_CHANNELS
+# RNC_INPAINT_KNOWN, _FORWARD, _BACKWARD, _BOTH, _SPATIAL: rnc_inpaint_propagate's source map
+INPAINT_KNOWN, INPAINT_FORWARD, INPAINT_BACKWARD, INPAINT_BOTH, INPAINT_SPATIAL = range(5)
 
 _lib = None
 _lock = threading.Lock()
