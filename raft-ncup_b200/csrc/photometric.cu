@@ -65,8 +65,9 @@ __global__ void __launch_bounds__(kWarpThreads) census_warp_kernel(WarpArgs a) {
   double ax = 0.0, ay = 0.0;
   // a NaN coordinate fails both range tests and samples nothing
   if (x0 >= -1.0f && x0 <= static_cast<float>(W - 1) && y0 >= -1.0f && y0 <= static_cast<float>(H - 1)) {
-    ax = px - x0;
-    ay = py - y0;
+    // in fp64: the fraction of a target in (-1, 0), px + 1, takes more than float32's 24 bits
+    ax = static_cast<double>(px) - x0;
+    ay = static_cast<double>(py) - y0;
     const int ix = static_cast<int>(x0), iy = static_cast<int>(y0);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {

@@ -6,7 +6,9 @@ The losses work on N rows; row r has a source image I1 and a target image I2 ([3
 
 Census term.  g(I) = 0.2989 R + 0.5870 G + 0.1140 B.  W^(x, y) is the bilinear sample of g(I2) at (x + F0, y + F1): align_corners
 pixel coordinates, x0 = floor(px), taps outside the frame = 0 (the sampling of rnc_fb_consistency and bilinear_sampler); its
-derivative with respect to F is that formula's, with the floor convention at integer positions.  The census of an intensity
+derivative with respect to F is that formula's, with the floor convention at integer positions.  Where x + F0 or y + F1 is not
+finite (a NaN or infinite flow), W^ samples nothing: W^ = 0 with a zero derivative, as fb_consistency marks such a pixel
+occluded and samples nothing there.  (The smoothness term of a non-finite flow is not finite.)  The census of an intensity
 image A at p: for each of the 49 offsets d in {-3..3}^2, c_d(p) = delta / sqrt(0.81 + delta^2), delta = A(p+d) - A(p), A = 0
 outside the frame.  h(p) = sum_d e^2 / (0.1 + e^2) with e = c_d^{g(I1)}(p) - c_d^{W^}(p) (the soft Hamming distance),
 l(p) = (h(p) + 0.01)^0.4, v(p) = m(p) [3 <= x <= W-4 and 3 <= y <= H-4], and
@@ -173,11 +175,14 @@ def _gray(im):
 
 def _warp(img, flow):
     """img [N,H,W] sampled bilinearly at (x + flow0, y + flow1): taps outside the frame 0, x0 = floor(px) (so the derivative
-    at an integer position is the right one), written out tap by tap."""
+    at an integer position is the right one), written out tap by tap.  A non-finite coordinate samples nothing: 0, with a
+    zero derivative."""
     N, H, W = img.shape
     xs = torch.arange(W, dtype=flow.dtype, device=flow.device).view(1, 1, W)
     ys = torch.arange(H, dtype=flow.dtype, device=flow.device).view(1, H, 1)
     px, py = xs + flow[:, 0], ys + flow[:, 1]
+    finite = torch.isfinite(px.detach()) & torch.isfinite(py.detach())
+    px, py = torch.where(finite, px, -2.0), torch.where(finite, py, -2.0)      # every tap of (-2, -2) lies outside
     x0, y0 = torch.floor(px.detach()), torch.floor(py.detach())
     ax, ay = px - x0, py - y0
     n = torch.arange(N, device=flow.device).view(N, 1, 1)

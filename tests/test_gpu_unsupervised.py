@@ -1,20 +1,19 @@
 """Unsupervised fine-tuning on the GPU (rnc/unsupervised.py, csrc/photometric.cu, model.forward(..., bidirectional=True),
-rnc.train.unsupervised_step): the census and smoothness kernels against the fp64 restatements at the shapes training uses,
-their determinism and batch independence, the bidirectional forward on every route against the forward of the concatenated
-pairs, one encoder pass per frame, the loss's parameter gradients against the host restatements in fp32, and a few steps."""
+rnc.train.unsupervised_step): the census and smoothness kernels' determinism and batch independence (their accuracy is held
+to the fp64 error model in test_gpu_photometric_error_model.py), the bidirectional forward on every route against the forward
+of the concatenated pairs, one encoder pass per frame, the loss's parameter gradients against the host restatements in fp32,
+and a few steps."""
 import pytest
 import torch
 
 from conftest import build_model
 from rnc.native import rnc
 from rnc.synth import frames
-from rnc.unsupervised import (_census_fwd, census_loss, host_census_loss, host_smoothness_loss, host_unsupervised_loss,
-                              smoothness_loss, unsupervised_loss)
+from rnc.unsupervised import _census_fwd, census_loss, host_unsupervised_loss, smoothness_loss, unsupervised_loss
 from test_gpu_ncup_finetune import frozen_model
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
-SHAPES = [(1, 8, 8), (3, 48, 64), (4, 384, 512), (2, 440, 1024)]
 H, W, ITERS = 128, 160, 3
 
 
@@ -43,42 +42,11 @@ def loss_inputs(N, h, w, seed=0):
     return i1, i2, flow, mask.to(DEV)
 
 
-def snapped(flow):
-    """flow in fp64 with x + F and y + F rounded to float32 as the kernels round them, so that the fp64 restatement takes its
-    bilinear taps at the same floor (elsewhere the derivative of the sample jumps)."""
-    h, w = flow.shape[-2:]
-    xs = torch.arange(w, device=flow.device, dtype=torch.float32).view(1, w)
-    ys = torch.arange(h, device=flow.device, dtype=torch.float32).view(h, 1)
-    return torch.stack([(xs + flow[:, 0]).double() - xs.double(), (ys + flow[:, 1]).double() - ys.double()], 1)
-
-
 def grad_of(fn, flow, *args):
     f = flow.detach().clone().requires_grad_()
     loss = fn(*args, f)
     loss.backward()
     return loss.detach(), f.grad
-
-
-@pytest.mark.parametrize("N,h,w", SHAPES)
-def test_census_loss_matches_fp64(N, h, w):
-    i1, i2, flow, mask = loss_inputs(N, h, w, seed=N + h)
-    loss, grad = grad_of(lambda f: census_loss(i1, i2, f, mask), flow)
-    ref, ref_grad = grad_of(lambda f: host_census_loss(i1.double(), i2.double(), f, mask), snapped(flow))
-    rel = abs(float(loss) - float(ref)) / abs(float(ref))
-    gerr = float((grad.double() - ref_grad).abs().max() / ref_grad.abs().max())
-    print(f"census {N}x{h}x{w}: loss {float(loss):.8f} rel err {rel:.2e}; grad max err / max|grad| {gerr:.2e}")
-    assert rel < 1e-5 and gerr < 1e-4
-
-
-@pytest.mark.parametrize("N,h,w", SHAPES)
-def test_smoothness_loss_matches_fp64(N, h, w):
-    i1, _, flow, _ = loss_inputs(N, h, w, seed=N + w)
-    loss, grad = grad_of(lambda f: smoothness_loss(i1, f), flow)
-    ref, ref_grad = grad_of(lambda f: host_smoothness_loss(i1.double(), f), flow.double())
-    rel = abs(float(loss) - float(ref)) / abs(float(ref))
-    gerr = float((grad.double() - ref_grad).abs().max() / ref_grad.abs().max())
-    print(f"smoothness {N}x{h}x{w}: loss {float(loss):.8f} rel err {rel:.2e}; grad max err / max|grad| {gerr:.2e}")
-    assert rel < 1e-5 and gerr < 1e-4
 
 
 def test_an_all_zero_mask_gives_zero_loss_and_gradient():

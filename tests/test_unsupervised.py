@@ -14,7 +14,7 @@ import torch.nn as nn
 from conftest import ROOT, build_model
 from rnc import native
 from rnc.synth import smooth_shift_frames
-from rnc.unsupervised import (census_loss, host_census_hamming, host_census_loss, host_smoothness_loss,
+from rnc.unsupervised import (_warp, census_loss, host_census_hamming, host_census_loss, host_smoothness_loss,
                               host_unsupervised_loss, smoothness_loss)
 
 CSRC = os.path.join(ROOT, "raft-ncup_b200", "csrc")
@@ -44,6 +44,8 @@ def naive_census(i1, i2, flow, mask):
         for y in range(H):
             for x in range(W):
                 px, py = x + flow[n, 0, y, x], y + flow[n, 1, y, x]
+                if not (math.isfinite(px) and math.isfinite(py)):
+                    continue                                            # samples nothing: W^ = 0
                 x0, y0 = math.floor(px), math.floor(py)
                 ax, ay = px - x0, py - y0
                 wh[y, x] = ((1 - ay) * ((1 - ax) * at(g2, y0, x0) + ax * at(g2, y0, x0 + 1)) +
@@ -90,6 +92,28 @@ def test_host_census_loss_matches_naive_loops(with_mask):
     mask = mask if with_mask else None
     got = float(host_census_loss(i1, i2, flow, mask))
     assert got == pytest.approx(naive_census(i1, i2, flow, mask), rel=1e-12)
+    # non-finite flows sample nothing: W^ = 0 with a zero derivative; +-1e12 leaves the frame
+    bad = flow.clone()
+    for k, v in enumerate((math.nan, math.inf, -math.inf, 1e12, -1e12)):
+        bad[0, k % 2, 2 + k, 1:9] = v
+    bad[1, :, 4:7, 3:8] = math.nan
+    f = bad.clone().requires_grad_()
+    got = host_census_loss(i1, i2, f, mask)
+    assert float(got) == pytest.approx(naive_census(i1, i2, bad, mask), rel=1e-12)
+    got.backward()
+    nonfinite = ~torch.isfinite(bad).all(1, keepdim=True).expand_as(bad)
+    assert torch.isfinite(f.grad).all() and not f.grad[nonfinite].any()
+    w = _warp(i2[:, 0], bad)
+    assert not w[nonfinite[:, 0]].any() and torch.isfinite(w).all()
+
+
+def test_host_smoothness_loss_of_a_non_finite_flow_is_not_finite():
+    i1, _, flow, _ = rows(2, 9, 11, seed=3)
+    for v in (math.nan, math.inf):
+        bad = flow.clone()
+        bad[1, 0, 4, 5] = v
+        got, want = float(host_smoothness_loss(i1, bad)), naive_smoothness(i1, bad)
+        assert not math.isfinite(got) and (math.isnan(got) == math.isnan(want) == math.isnan(v))
 
 
 def test_host_census_loss_with_an_all_zero_mask_row():
