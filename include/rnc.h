@@ -843,6 +843,56 @@ int rnc_ssim_partials(const float* pred, long long pn, long long pc, long long p
                       long long gn, long long gc, long long gy, long long gx, int N, int H, int W, double* sum,
                       long long* count, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V11  blind video temporal consistency: one step of the screened Poisson solve of Bonneel et al. 2015 along the backward
+ * flows, and the warping error's per-frame partials (Lai et al. 2018) (definition: rnc/temporal.py, DESIGN §3.20).  Every
+ * float32 operation rounded once (no FMA); no atomics, no host synchronisation.  Bad arguments return before any launch.
+ *
+ * rnc_temporal_step: one step k -> k+1 of V videos of C channels, O_{k+1} from O_k, P_{k+1}, I_k, I_{k+1}, G_k, occ_bw_k.
+ *   out_prev  : fp32 [V][C][H][W] through element strides (av, ac, ay, ax), O_k
+ *   processed : fp32 [V][C][H][W] through element strides (pv, pc, py, px), P_{k+1}
+ *   frame_prev, frame : fp32 [V][3][H][W] through element strides, I_k and I_{k+1} in 0..255
+ *   flow_bw   : fp32 [V][2][H][W] through element strides, G_k (frame k+1 -> k)
+ *   occ_bw    : uint8 [V][H][W] through element strides, on frame k+1; a pixel is visible where 0
+ *   out       : fp32 [V][C][H][W] through element strides (qv, qc, qy, qx), O_{k+1}; may be processed or out_prev itself,
+ *               otherwise must not overlap the inputs
+ *   workspace : rnc_temporal_step_workspace_bytes(V, C, H, W) bytes, 16-byte aligned, no zeroing needed
+ *   All float pointers 4-byte aligned.
+ * A pixel p of frame k+1 is matched when u = G_k(p) has both components finite, occ_bw_k(p) == 0 and p' = p + u lies in
+ * [0, W-1] x [0, H-1].  A matched pixel has T = O_k(p') and J = I_k(p') (the clamped bilinear sample), d2 = the sum over the
+ * 3 channels of ((I_{k+1}(p) - J) / 255)^2 and w = lam / (1 + alpha d2); an unmatched one w = 0.  With n the pixel's in-frame
+ * 4-neighbours, D = O_{k+1} - P_{k+1} solves (n + w) D_p - sum_q D_q = w (T - P) by `sweeps` red-black SOR sweeps from D = 0
+ * ((x + y) even first; D_p += omega ((sum_q D_q + w (T - P)) / (n + w) - D_p), neighbours added up, left, right, down;
+ * w (T - P) is 0 where w is 0).  omega = 2 / (1 + s) per image: a pixel is weak when w < lam / 4; D2 is the largest exact
+ * squared distance from a weak pixel to its nearest non-weak pixel; s = sigma when D2 is 0 (no weak pixel, or no other
+ * kind), otherwise min(pi_f32 / (L + 1), sigma) with L the least integer such that L^2 >= 4 D2.  sigma is float32(sqrt(lam /
+ * 2)), computed by the caller.  5 + 2 sweeps launches.  RNC_ERR_BAD_SHAPE unless 1 <= V <= 65535,
+ * 1 <= C <= RNC_HARMONIC_MAX_CHANNELS, 1 <= H, W <= 4096, sweeps >= 0 and lam, alpha, sigma are finite and >= 0.
+ *
+ * rnc_warping_error_partials: per video v and pair k, sum[v (T-1) + k] = the fp64 sum over the matched pixels p of frame k+1
+ * (the matching above, with flow_bw[v][k] and occ_bw[v][k]) and the C channels of ((V_{k+1}(p) - V_k(p')) / 255)^2, the
+ * sample in float32 and the rest in fp64; count[v (T-1) + k] = the number of matched pixels.  Through the evaluation kernels'
+ * fixed-order reductions, so a frame's result does not depend on V, its position or the GPU.
+ *   video     : fp32 [V][T][C][H][W] through element strides (vv, vt, vc, vy, vx)
+ *   flow_bw   : fp32 [V][T-1][2][H][W] through element strides; occ_bw : uint8 [V][T-1][H][W] through element strides
+ *   sum       : fp64 [V][T-1]; count : int64 [V][T-1]; both 8-byte aligned
+ *   workspace : rnc_warping_error_partials_workspace_bytes(V, T, C, H, W) bytes, 16-byte aligned
+ * Two launches.  RNC_ERR_BAD_SHAPE unless V >= 1, T >= 2, V (T - 1) <= 65535, C >= 1, H, W >= 1 and H*W < 2^30. */
+size_t rnc_temporal_step_workspace_bytes(int V, int C, int H, int W);   /* 0 for a bad shape */
+int rnc_temporal_step(const float* out_prev, long long av, long long ac, long long ay, long long ax, const float* processed,
+                      long long pv, long long pc, long long py, long long px, const float* frame_prev, long long iv,
+                      long long ic, long long iy, long long ix, const float* frame, long long jv, long long jc, long long jy,
+                      long long jx, const float* flow_bw, long long gv, long long gc, long long gy, long long gx,
+                      const unsigned char* occ_bw, long long ov, long long oy, long long ox, int V, int C, int H, int W,
+                      float lam, float alpha, float sigma, int sweeps, float* out, long long qv, long long qc, long long qy,
+                      long long qx, void* workspace, size_t workspace_bytes, void* stream);
+size_t rnc_warping_error_partials_workspace_bytes(int V, int T, int C, int H, int W);   /* 0 for a bad shape */
+int rnc_warping_error_partials(const float* video, long long vv, long long vt, long long vc, long long vy, long long vx,
+                               const float* flow_bw, long long gv, long long gk, long long gc, long long gy, long long gx,
+                               const unsigned char* occ_bw, long long ov, long long ok, long long oy, long long ox, int V,
+                               int T, int C, int H, int W, double* sum, long long* count, void* workspace,
+                               size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

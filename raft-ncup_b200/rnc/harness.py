@@ -8,6 +8,7 @@ warm-start forward interpolation runs on the GPU.  Metrics aggregate as the refe
 (`valid` absent) pools all pixels (evaluate.py:131-137), KITTI-style averages per-image means (evaluate.py:172-179).  Under
 torch.distributed every rank takes a share of the samples, sequences or pairs (rnc.dist).
 """
+import math
 import os
 from collections import deque, namedtuple
 from concurrent.futures import ThreadPoolExecutor
@@ -776,6 +777,114 @@ def validate_inpainting(model, sequences, masks, iters=32, warm_start=False, bat
         s, c = ssim(pred[scored], gt)
         records.append([list(r) for r in zip(err.sq_sum.tolist(), err.count.tolist(), s.tolist(), c.tolist())])
     return summarize_inpainting(gather_strided(records, world))
+
+
+def _consistent_steps(model, sequences, processed, iters, warm_start, batch_size, mode, device, alpha1, alpha2, lam, alpha,
+                      sweeps, what):
+    """make_temporally_consistent's loop: yields (video, pair, result, outputs) after each step, outputs being the list of
+    V [T_v,C,H,W] results on the device, frame pair + 1 of the video just written."""
+    from . import native
+    from .temporal import _check_params, _check_sides, temporal_step
+    if model._needs_grad():
+        raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
+    procs = list(processed)
+    if len(procs) != len(sequences):
+        raise ValueError(f"{what}: {len(sequences)} videos but {len(procs)} processed videos")
+    _check_params(lam, alpha, sweeps, what)
+    for seq, p in zip(sequences, procs):
+        if len(seq) < 2:
+            raise ValueError(f"{what}: a video needs T >= 2 frames, got {len(seq)}")
+        if p.dim() != 4 or p.shape[0] != len(seq) or tuple(p.shape[2:]) != tuple(seq[0].shape[-2:]):
+            raise ValueError(f"{what}: expected processed frames [{len(seq)},C,{seq[0].shape[-2]},{seq[0].shape[-1]}], got "
+                             f"{list(p.shape)}")
+        if not 1 <= p.shape[1] <= native.HARMONIC_MAX_CHANNELS:
+            raise ValueError(f"{what}: expected 1 to {native.HARMONIC_MAX_CHANNELS} processed channels, got {p.shape[1]}")
+        _check_sides(*p.shape[-2:], what)
+    out, ws = None, {}
+    for s, k, r in run_sequences_bidirectional(model, sequences, iters, warm_start=warm_start, batch_size=batch_size,
+                                               mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
+        dev = r["flow_up_bw"].device
+        if out is None:
+            out = [torch.empty(p.shape, dtype=torch.float32, device=dev) for p in procs]
+            for o, p in zip(out, procs):
+                o[0] = p[0]
+        o, seq = out[s], sequences[s]
+        C = o.shape[1]
+        if dev.type == "cuda" and C not in ws:
+            ws[C] = torch.empty(native.rnc.temporal_step_workspace_bytes(1, C, *o.shape[-2:]), dtype=torch.uint8, device=dev)
+        i0, i1 = (seq[j].to(dev).float()[None] for j in (k, k + 1))
+        temporal_step(o[k][None], procs[s][k + 1].to(dev)[None], i0, i1, r["flow_up_bw"][None], r["occ_bw"][None], lam, alpha,
+                      sweeps, out=o[k + 1][None], workspace=ws.get(C))
+        yield s, k, r, out
+
+
+def make_temporally_consistent(model, sequences, processed, iters=32, warm_start=False, batch_size=8, mode="sintel",
+                               device="cuda", alpha1=0.01, alpha2=0.5, lam=0.1, alpha=50.0, sweeps=512):
+    """Remove the flicker of V videos processed frame by frame (rnc.temporal's rule: each output frame keeps its processed
+    frame's gradients and is pulled toward the previous output, warped along the backward flow, where the flow is matched
+    and the frames agree).  sequences: list of V original frame lists, every frame [3,H,W] (0..255) of one size, each video
+    of T_v >= 2 frames; processed: V tensors [T_v,C,H,W], 1 <= C <= 4, the per-frame results (any range).  Returns a list of
+    V float32 [T_v,C,H,W] tensors on the device, frame 0 being the processed frame 0.
+
+    The flows come from the original frames: run_sequences_bidirectional(model, sequences, iters, warm_start, batch_size,
+    mode, device, alpha1=alpha1, alpha2=alpha2) yields each video's pairs in order, and pair k's flow_up_bw and occ_bw step
+    that video from frame k to k + 1 at once (rnc.temporal.temporal_step with lam, alpha and sweeps, one rnc_temporal_step
+    call), so no flow is kept: the memory is the outputs.  ValueError before the flow pass for a video of fewer than two
+    frames, processed frames of another shape, a channel count outside 1..4, a side above 4096, a processed-video count that
+    does not match the videos or a bad lam, alpha or sweeps.  Inference only: with grad enabled on a model that requires
+    grad it raises ValueError."""
+    out = []
+    for *_, out in _consistent_steps(model, sequences, processed, iters, warm_start, batch_size, mode, device, alpha1, alpha2,
+                                     lam, alpha, sweeps, "make_temporally_consistent"):
+        pass
+    return out if sequences else []
+
+
+@torch.no_grad()
+def validate_temporal_consistency(model, sequences, processed, iters=32, warm_start=False, batch_size=8, mode="sintel",
+                                  device="cuda", alpha1=0.01, alpha2=0.5, lam=0.1, alpha=50.0, sweeps=512):
+    """The warping error of a split's processed videos and of make_temporally_consistent's outputs, with the outputs'
+    fidelity to the processed frames (so that freezing a video does not score well): warping_error_processed,
+    warping_error, psnr, ssim, and the frame and video counts (rnc.temporal.summarize_temporal).  sequences and processed as
+    make_temporally_consistent's.  Each pair's flows score frame k + 1 of both videos as it is stepped
+    (rnc.temporal.warping_error, on the device); psnr (rnc.interp.interpolation_error, 100 dB cap) and ssim (rnc.inpaint.ssim)
+    compare O_t with P_t over frames 1..T_v-1 (frame 0 is P_0 by the rule) when C = 3 and the frames are at least 11x11,
+    and are NaN otherwise.  The partials are per frame, so the result does not depend on batch_size or on the order of the
+    videos.  Under torch.distributed rank r takes the videos of index = r (mod world), the per-frame partials are
+    all-gathered, and every rank returns the single-process result."""
+    from .dist import gather_strided, strided_items, world_rank
+    from .inpaint import SSIM_RADIUS, ssim
+    from .interp import interpolation_error
+    from .temporal import summarize_temporal, warping_error
+    world, rank = world_rank()
+    procs = list(processed)
+    if len(procs) != len(sequences):
+        raise ValueError(f"validate_temporal_consistency: {len(sequences)} videos but {len(procs)} processed videos")
+    mine = list(strided_items(range(len(sequences)), world, rank))
+    warp = {i: [None] * (len(sequences[i]) - 1) for i in mine}
+    got = None
+    for s, k, r, out in _consistent_steps(model, [sequences[i] for i in mine], [procs[i] for i in mine], iters, warm_start,
+                                          batch_size, mode, device, alpha1, alpha2, lam, alpha, sweeps,
+                                          "validate_temporal_consistency"):
+        dev = out[s].device
+        g, m = r["flow_up_bw"][None, None], r["occ_bw"][None, None]
+        wp = warping_error(procs[mine[s]][k:k + 2].to(dev)[None], g, m)
+        wo = warping_error(out[s][k:k + 2][None], g, m)
+        warp[mine[s]][k] = (wp[0][0, 0], wo[0][0, 0], wp[1][0, 0])
+        got = out
+    records = []
+    for j, i in enumerate(mine):
+        o = got[j]
+        p = procs[i].to(o.device).float()
+        T, C, H, W = o.shape
+        rows = [[float(a), float(b), int(c)] for a, b, c in warp[i]]
+        nan = [[math.nan] * 4 for _ in range(T - 1)]
+        if C == 3 and min(H, W) >= 2 * SSIM_RADIUS + 1:
+            err = interpolation_error(o[1:], p[1:])
+            ss, sc = ssim(o[1:], p[1:])
+            nan = [list(x) for x in zip(err.sq_sum.tolist(), err.count.tolist(), ss.tolist(), sc.tolist())]
+        records.append([a + b for a, b in zip(rows, nan)])
+    return summarize_temporal(gather_strided(records, world))
 
 
 def size_batches(items, batch_size, key):

@@ -187,6 +187,12 @@ SIGNATURES = {
                                    _vp, _vp, _vp]),
     "rnc_ssim_partials_workspace_bytes": (C.c_size_t, [_i, _i, _i]),
     "rnc_ssim_partials": (_i, [_vp, *[C.c_longlong] * 4, _vp, *[C.c_longlong] * 4, _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_temporal_step_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i]),
+    "rnc_temporal_step": (_i, [*[_vp, *[C.c_longlong] * 4] * 5, _vp, *[C.c_longlong] * 3, _i, _i, _i, _i, _f, _f, _f, _i, _vp,
+                               *[C.c_longlong] * 4, _vp, C.c_size_t, _vp]),
+    "rnc_warping_error_partials_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i]),
+    "rnc_warping_error_partials": (_i, [_vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 4, _i, _i,
+                                        _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind
