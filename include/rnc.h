@@ -893,6 +893,57 @@ int rnc_warping_error_partials(const float* video, long long vv, long long vt, l
                                int T, int C, int H, int W, double* sum, long long* count, void* workspace,
                                size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V12  video stabilization: a RANSAC homography fit of each pair's camera motion to its forward flow, the smoothed camera
+ * path of Matsushita et al. (PAMI 2006) with its closed-form crop, and the warp (definition: rnc/stabilize.py, DESIGN
+ * §3.21).  Every fp32 and fp64 operation rounded once (no FMA), no transcendental function; no atomics, no host
+ * synchronisation.  Bad arguments return before any launch.
+ *
+ * rnc_homography_fit: per pair n of N, A_k (frame k -> frame k+1 pixel coordinates, h33 = 1) fitted to the flow F_k.
+ *   flow      : fp32 [N][2][H][W] through element strides (fn, fc, fy, fx), channel 0 = x
+ *   A         : fp64 [N][3][3], 8-byte aligned; inliers, matched, status : int32 [N], 4-byte aligned
+ *   workspace : rnc_homography_fit_workspace_bytes(N, H, W, stride, hypotheses) bytes, 16-byte aligned, no zeroing needed
+ * Points p = (s/2 + j s, s/2 + i s) (s = stride) are matched when both components of F_k(p) are finite and q = p + F_k(p)
+ * (fp64) lies in [0, W-1] x [0, H-1]; the matched points form the list L in raster order, in fp64 coordinates normalized
+ * by ((x - (W-1)/2) / nu, (y - (H-1)/2) / nu), nu = max(H, W) / 2.  Hypothesis h draws indices splitmix64(seed, 4h + j)
+ * mod n, j = 0..3, and solves the 8x8 DLT system (h33 = 1) by Gaussian elimination with partial pivoting; it is degenerate
+ * when two indices are equal, three source or three destination points have |cross| < 1e-9, or a pivot is under 1e-12.  A
+ * point is an inlier of H when w > 0 and nu^2 |H p^ - q^|^2 < tau^2; the most inliers wins, ties to the smaller h.  Then
+ * `refine` rounds refit H by algebraic least squares over the current inliers (at least 4; a singular refit keeps H), the
+ * normal equations summed in chunks of 256 points of L in order and the chunks in order.  With hypotheses = 0 the first
+ * round fits all of L.  inliers[n] is the final H's count, matched[n] = n.  status RNC_HOMOGRAPHY_FEW (A = identity,
+ * inliers 0) when n < 4, no hypothesis is non-degenerate, the first refit of hypotheses = 0 fails, or H sends the frame
+ * centre to infinity; RNC_HOMOGRAPHY_OK otherwise.  5 + 2 (refine + 1) launches (4 + ... with hypotheses = 0).
+ * RNC_ERR_BAD_SHAPE unless 1 <= N <= 65535, 1 <= H, W <= 4096, 1 <= stride <= 256, 0 <= hypotheses <= 65536,
+ * 0 <= refine <= 64, hypotheses + refine > 0 and tau is finite and > 0.
+ *
+ * rnc_stabilize_path: V videos of T frames.  A : fp64 [V][T-1][3][3] contiguous, the pairs' homographies; taps : fp64
+ * [radius + 1], w_0..w_radius.  S_t = sum_j w_|j| T_t^{t+j} over -min(radius, t) <= j <= min(radius, T-1-t), j = 0 first,
+ * then 1, 2, ..., then -1, -2, ...; T_t^{t+j} the chained products of the A's (j > 0) or of their adjugate inverses (j < 0),
+ * each product divided by its [2][2]; S_t divided by its [2][2].  alpha[v] = the largest alpha in [0, 1] such that every
+ * frame's S_t^-1 maps the corners of the centred alpha (W-1) x alpha (H-1) rectangle into the frame with w > 0 (0 when the
+ * centre leaves the frame).  M[v][t] = Z S_t with crop (Z the zoom by 1 / (max(alpha, crop_min) (1 - 2^-36)) about the
+ * centre), S_t without; Minv[v][t] = its adjugate inverse.  M, Minv : fp64 [V][T][3][3]; alpha : fp64 [V]; all 8-byte
+ * aligned.  One launch.  RNC_ERR_BAD_SHAPE unless 1 <= V <= 65535, 2 <= T <= 2^24, 0 <= radius <= 1024, 1 <= H, W <= 4096
+ * and 0 < crop_min <= 1.
+ *
+ * rnc_stabilize_warp: out[n][c](u) = sample(frames[n][c], q) where q = maps[n] u in fp64, divided by w and rounded once to
+ * fp32, when w > 0 and q lies in [0, W-1] x [0, H-1] (valid[n](u) = 1); 0 otherwise (valid 0).
+ *   frames : fp32 [N][C][H][W] through element strides; maps : fp64 [N][3][3] contiguous, output -> input
+ *   out    : fp32 [N][C][H][W] through element strides, not overlapping frames; valid : uint8 [N][H][W] through strides
+ * One launch.  RNC_ERR_BAD_SHAPE unless 1 <= N <= 65535, 1 <= C <= 4 and 1 <= H, W <= 4096. */
+#define RNC_HOMOGRAPHY_OK 0
+#define RNC_HOMOGRAPHY_FEW 1
+size_t rnc_homography_fit_workspace_bytes(int N, int H, int W, int stride, int hypotheses);   /* 0 for a bad shape */
+int rnc_homography_fit(const float* flow, long long fn, long long fc, long long fy, long long fx, int N, int H, int W,
+                       int stride, int hypotheses, double tau, int refine, unsigned long long seed, double* A, int* inliers,
+                       int* matched, int* status, void* workspace, size_t workspace_bytes, void* stream);
+int rnc_stabilize_path(const double* A, int V, int T, const double* taps, int radius, int H, int W, int crop, double crop_min,
+                       double* M, double* Minv, double* alpha, void* stream);
+int rnc_stabilize_warp(const float* frames, long long in, long long ic, long long iy, long long ix, const double* maps, int N,
+                       int C, int H, int W, float* out, long long on, long long oc, long long oy, long long ox,
+                       unsigned char* valid, long long vn, long long vy, long long vx, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

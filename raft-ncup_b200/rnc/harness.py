@@ -887,6 +887,82 @@ def validate_temporal_consistency(model, sequences, processed, iters=32, warm_st
     return summarize_temporal(gather_strided(records, world))
 
 
+def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda", radius=30,
+                     sigma=10.0, crop=True, crop_min=0.5, stride=8, hypotheses=256, tau=2.0, refine=4, seed=0):
+    """Stabilize V videos (rnc.stabilize's rule: fit each pair's camera motion to its forward flow by RANSAC, smooth the
+    camera path with a Gaussian of sigma frames over +-radius frames, zoom in to crop the uncovered borders, and warp).
+    sequences: list of V frame lists, every frame [3,H,W] (0..255) of one size, each video of T_v >= 2 frames.  Returns a
+    list of V dicts on the device: frames float32 [T_v,3,H,W], valid uint8 [T_v,H,W] (0 where the output pixel has no input,
+    which happens only when the video's alpha is under crop_min or crop=False), motion fp64 [T_v-1,3,3] (A_k, frame k ->
+    k+1), transforms fp64 [T_v,3,3] (M_t, input frame t -> output frame t), alpha (fp64 scalar tensor, the closed-form
+    crop scale before crop_min applies), and inliers, matched and status int32 [T_v-1] of each pair's fit.
+
+    run_sequences(model, sequences, iters, warm_start, batch_size, mode, device) yields each pair's forward flow, which is
+    fitted at once (rnc.stabilize.fit_homographies with stride, hypotheses, tau, refine and seed) and dropped: only its 3x3
+    matrix is kept.  The forward flow is enough: RANSAC rejects the pixels a backward check would flag.  Then each video's
+    path is smoothed (smooth_path) and its frames warped (warp_frames) on the device.  ValueError before the flow pass for a
+    video of fewer than two frames, a side above 4096 or a bad radius, sigma, crop_min, stride, hypotheses, tau, refine or
+    seed.  Inference only: with grad enabled on a model that requires grad it raises ValueError."""
+    from .stabilize import _check_fit_params, _check_path_params, _check_sides, fit_homographies, smooth_path, warp_frames
+    what = "stabilize_videos"
+    if model._needs_grad():
+        raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
+    _check_fit_params(stride, hypotheses, tau, refine, seed, what)
+    _check_path_params(radius, sigma, crop_min, what)
+    for seq in sequences:
+        if len(seq) < 2:
+            raise ValueError(f"{what}: a video needs T >= 2 frames, got {len(seq)}")
+        _check_sides(*seq[0].shape[-2:], what)
+    from . import native
+    fits = [[None] * (len(seq) - 1) for seq in sequences]
+    ws = None
+    for s, k, flow in run_sequences(model, sequences, iters, warm_start=warm_start, batch_size=batch_size, mode=mode,
+                                    device=device):
+        if flow.is_cuda and ws is None:
+            H, W = flow.shape[-2:]
+            ws = torch.empty(native.rnc.homography_fit_workspace_bytes(1, H, W, stride, hypotheses), dtype=torch.uint8,
+                             device=flow.device)
+        fits[s][k] = fit_homographies(flow[None], stride, hypotheses, tau, refine, seed, workspace=ws)
+    out = []
+    for seq, fit in zip(sequences, fits):
+        A, inl, mat, st = (torch.cat([f[j] for f in fit]) for j in range(4))
+        dev = A.device
+        H, W = seq[0].shape[-2:]
+        M, Minv, alpha = smooth_path(A[None], H, W, radius, sigma, crop, crop_min)
+        frames, valid = warp_frames(torch.stack([f.to(dev).float() for f in seq]), Minv[0])
+        out.append({"frames": frames, "valid": valid, "motion": A, "transforms": M[0], "alpha": alpha[0], "inliers": inl,
+                    "matched": mat, "status": st})
+    return out
+
+
+@torch.no_grad()
+def validate_stabilization(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda", radius=30,
+                           sigma=10.0, crop=True, crop_min=0.5, stride=8, hypotheses=256, tau=2.0, refine=4, seed=0):
+    """The standard stabilization scores of stabilize_videos' output beside the input's (Liu et al. 2013; ITF of Matsushita
+    et al. 2006), from the known maps rather than re-estimated features (rnc.stabilize.stabilization_metrics, on the host in
+    fp64): cropping, distortion, stability_translation, stability_rotation and stability of the output, and the input's
+    input_stability_*; itf and input_itf, each the mean over a video's consecutive frame pairs of their PSNR
+    (rnc.interp.interpolation_error's partials on the device, rnc.inpaint.psnr's 100 dB cap), then over videos; frames and
+    videos, their numbers (rnc.stabilize.summarize_stabilization).  Arguments as stabilize_videos'.  Under
+    torch.distributed rank r takes the videos of index = r (mod world), the per-video records are all-gathered, and every
+    rank returns the single-process result."""
+    from .dist import gather_strided, strided_items, world_rank
+    from .interp import interpolation_error
+    from .stabilize import stabilization_metrics, summarize_stabilization
+    world, rank = world_rank()
+    mine = [sequences[i] for i in strided_items(range(len(sequences)), world, rank)]
+    res = stabilize_videos(model, mine, iters, warm_start, batch_size, mode, device, radius, sigma, crop, crop_min, stride,
+                           hypotheses, tau, refine, seed)
+    records = []
+    for seq, r in zip(mine, res):
+        out = r["frames"]
+        inp = torch.stack([f.to(out.device).float() for f in seq])
+        rows = [interpolation_error(v[1:], v[:-1]) for v in (out, inp)]
+        records.append((stabilization_metrics(r["motion"], r["transforms"]),
+                        *[list(zip(e.sq_sum.tolist(), e.count.tolist())) for e in rows]))
+    return summarize_stabilization(gather_strided(records, world))
+
+
 def size_batches(items, batch_size, key):
     """Batches of create_kitti_submission: the items of one key(item) (a frame size) in order of appearance, batch_size at a
     time.  A batch is yielded as soon as it is full, the partial batches at the end in order of their size's first

@@ -193,6 +193,12 @@ SIGNATURES = {
     "rnc_warping_error_partials_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i]),
     "rnc_warping_error_partials": (_i, [_vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 4, _i, _i,
                                         _i, _i, _i, _vp, _vp, _vp, C.c_size_t, _vp]),
+    "rnc_homography_fit_workspace_bytes": (C.c_size_t, [_i, _i, _i, _i, _i]),
+    "rnc_homography_fit": (_i, [_vp, *[C.c_longlong] * 4, _i, _i, _i, _i, _i, C.c_double, _i, C.c_ulonglong, _vp, _vp, _vp,
+                                _vp, _vp, C.c_size_t, _vp]),
+    "rnc_stabilize_path": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, C.c_double, _vp, _vp, _vp, _vp]),
+    "rnc_stabilize_warp": (_i, [_vp, *[C.c_longlong] * 4, _vp, _i, _i, _i, _i, _vp, *[C.c_longlong] * 4, _vp,
+                                *[C.c_longlong] * 3, _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind
@@ -203,6 +209,7 @@ SEGMENT_COUNTS = 6                                         # RNC_SEGMENT_COUNTS
 HARMONIC_MAX_CHANNELS = 4                                  # RNC_HARMONIC_MAX_CHANNELS
 # RNC_INPAINT_KNOWN, _FORWARD, _BACKWARD, _BOTH, _SPATIAL: rnc_inpaint_propagate's source map
 INPAINT_KNOWN, INPAINT_FORWARD, INPAINT_BACKWARD, INPAINT_BOTH, INPAINT_SPATIAL = range(5)
+HOMOGRAPHY_OK, HOMOGRAPHY_FEW = 0, 1                       # RNC_HOMOGRAPHY_OK, RNC_HOMOGRAPHY_FEW: rnc_homography_fit's status
 
 _lib = None
 _lock = threading.Lock()

@@ -59,3 +59,43 @@ def motion_boundary_flow_init(b, h8, w8, jump=24.0):
     f[:, 0, :, w8 // 2:] = jump
     f[:, 1, 2 * h8 // 3:, :] = -jump * 0.75
     return f
+
+
+def shaky_sequence(n, h, w, seed=0, pan=(2.0, 0.5), jitter_px=3.0, jitter_rot=0.01, jitter_scale=0.01):
+    """A handheld-looking video of n frames [3,h,w] with known camera motion, for video stabilization: frame t shows a smooth
+    canvas (a seeded sum of sinusoids per channel, 0..255, evaluated in fp64 at the exact point, so no resampling blurs it)
+    through the camera homography C_t, canvas -> frame t pixel coordinates: C_t = Tc R(theta_t) s_t Tc^-1 Tr(-o_t), Tc the
+    translation to the frame centre, o_t = pan t plus a seeded translation jitter of std jitter_px, and theta_t and s_t - 1
+    seeded jitters of std jitter_rot (radians) and jitter_scale.  Returns (frames: list of float32 [3,h,w], C fp64 [n,3,3],
+    flows float32 [n-1,2,h,w]), flow k being the exact forward flow C_{k+1} C_k^-1 p - p of frame k's pixels p."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    K = 8
+    freq = rng.uniform(2 * np.pi / 60, 2 * np.pi / 12, (3, K)) * np.exp(1j * rng.uniform(0, 2 * np.pi, (3, K)))
+    amp = rng.uniform(0.5, 1.0, (3, K))
+    amp *= 110 / amp.sum(1, keepdims=True)
+    phase = rng.uniform(0, 2 * np.pi, (3, K))
+    jit = rng.normal(0, 1, (n, 4))
+    cx, cy = (w - 1) / 2, (h - 1) / 2
+    Tc = np.array([[1.0, 0, cx], [0, 1.0, cy], [0, 0, 1]])
+    Tci = np.array([[1.0, 0, -cx], [0, 1.0, -cy], [0, 0, 1]])
+    C = np.empty((n, 3, 3))
+    for t in range(n):
+        th, s = jitter_rot * jit[t, 0], 1 + jitter_scale * jit[t, 1]
+        ox, oy = pan[0] * t + jitter_px * jit[t, 2], pan[1] * t + jitter_px * jit[t, 3]
+        R = np.array([[s * np.cos(th), -s * np.sin(th), 0], [s * np.sin(th), s * np.cos(th), 0], [0, 0, 1]])
+        C[t] = Tc @ R @ Tci @ np.array([[1.0, 0, -ox], [0, 1.0, -oy], [0, 0, 1]])
+    ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    P = np.stack([xs, ys, np.ones_like(xs)]).reshape(3, -1)
+    frames = []
+    for t in range(n):
+        X, Y, Wh = np.linalg.inv(C[t]) @ P
+        X, Y = X / Wh, Y / Wh
+        img = 127.5 + (amp[..., None] * np.sin(freq.real[..., None] * X + freq.imag[..., None] * Y + phase[..., None])).sum(1)
+        frames.append(torch.from_numpy(img.reshape(3, h, w)).float())
+    flows = np.empty((n - 1, 2, h, w))
+    for k in range(n - 1):
+        X, Y, Wh = C[k + 1] @ np.linalg.inv(C[k]) @ P
+        flows[k, 0] = (X / Wh - P[0]).reshape(h, w)
+        flows[k, 1] = (Y / Wh - P[1]).reshape(h, w)
+    return frames, torch.from_numpy(C), torch.from_numpy(flows).float()
