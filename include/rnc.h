@@ -944,6 +944,35 @@ int rnc_stabilize_warp(const float* frames, long long in, long long ic, long lon
                        int C, int H, int W, float* out, long long on, long long oc, long long oy, long long ox,
                        unsigned char* valid, long long vn, long long vy, long long vx, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * V13  full-frame video stabilization: the motion inpainting of Matsushita et al. (PAMI 2006).  The forward and backward
+ * flows are moved into the stabilized frames with the camera's known global motion taken out, the residual is completed
+ * across the uncovered border (rnc_harmonic_fill), and the global motion is added back; the chains of rnc_inpaint_propagate
+ * then carry each uncovered pixel to the frames that see it (definition: rnc/stabilize.py step 5, DESIGN §3.22).  Every
+ * fp32 and fp64 operation rounded once (no FMA), no transcendental function; no atomics, no host synchronisation.  Bad
+ * arguments return before any launch.  Per video v of V and pair k of T-1: A_k = motion[v][k] (frame k -> k+1, fp64
+ * [V][T-1][3][3] contiguous), M_t = maps[v][t] (input -> output) and M_t^-1 = maps_inv[v][t] (fp64 [V][T][3][3]
+ * contiguous, rnc_stabilize_path's M and Minv); pi(P p) = ((P p)_x / (P p)_w, (P p)_y / (P p)_w), defined when (P p)_w > 0;
+ * inv(A) the adjugate divided by its [2][2].  res, res_bw, flow, flow_bw below are fp32 [V][T-1][2][H][W] contiguous.
+ *
+ * rnc_stabilize_flow_residual: for output pixel u of frame k, q = M_k^-1 u as rnc_stabilize_warp computes it (fp64, rounded
+ * once to fp32, valid when w > 0 and q lies in [0, W-1] x [0, H-1]), F = sample(flow[v][k], q), and
+ * res[v][k](u) = pi(M_{k+1} (q + F)) - pi(M_{k+1} pi(A_k q)) in fp64, rounded once to fp32.  res_bw[v][k] likewise for
+ * output frame k+1 with M_{k+1}^-1, flow_bw[v][k], M_k and inv(A_k).  NaN where q is not valid, F is not finite or a
+ * projection is undefined.  flow, flow_bw : fp32 [V][T-1][2][H][W] through element strides (channel 0 = x).  One launch.
+ *
+ * rnc_stabilize_flow_readd: in place on the completed residuals, flow[v][k](u) = (pi(M_{k+1} pi(A_k q)) - u) + flow[v][k](u)
+ * in fp64, rounded once to fp32, q = M_k^-1 u rounded to fp32 as above (every pixel, inside the frame or not); flow_bw
+ * likewise.  NaN where a projection is undefined.  One launch.
+ *
+ * Both: RNC_ERR_BAD_SHAPE unless 1 <= V <= 65535, 2 <= T <= 65536 and 1 <= H, W <= 4096. */
+int rnc_stabilize_flow_residual(const float* flow, long long fv, long long fk, long long fc, long long fy, long long fx,
+                                const float* flow_bw, long long bv, long long bk, long long bc, long long by, long long bx,
+                                const double* motion, const double* maps, const double* maps_inv, int V, int T, int H, int W,
+                                float* res, float* res_bw, void* stream);
+int rnc_stabilize_flow_readd(const double* motion, const double* maps, const double* maps_inv, int V, int T, int H, int W,
+                             float* flow, float* flow_bw, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -888,7 +888,8 @@ def validate_temporal_consistency(model, sequences, processed, iters=32, warm_st
 
 
 def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda", radius=30,
-                     sigma=10.0, crop=True, crop_min=0.5, stride=8, hypotheses=256, tau=2.0, refine=4, seed=0):
+                     sigma=10.0, crop=True, crop_min=0.5, stride=8, hypotheses=256, tau=2.0, refine=4, seed=0, fill=False,
+                     sweeps=512, max_distance=None, alpha1=0.01, alpha2=0.5):
     """Stabilize V videos (rnc.stabilize's rule: fit each pair's camera motion to its forward flow by RANSAC, smooth the
     camera path with a Gaussian of sigma frames over +-radius frames, zoom in to crop the uncovered borders, and warp).
     sequences: list of V frame lists, every frame [3,H,W] (0..255) of one size, each video of T_v >= 2 frames.  Returns a
@@ -901,28 +902,56 @@ def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8,
     fitted at once (rnc.stabilize.fit_homographies with stride, hypotheses, tau, refine and seed) and dropped: only its 3x3
     matrix is kept.  The forward flow is enough: RANSAC rejects the pixels a backward check would flag.  Then each video's
     path is smoothed (smooth_path) and its frames warped (warp_frames) on the device.  ValueError before the flow pass for a
-    video of fewer than two frames, a side above 4096 or a bad radius, sigma, crop_min, stride, hypotheses, tau, refine or
-    seed.  Inference only: with grad enabled on a model that requires grad it raises ValueError."""
-    from .stabilize import _check_fit_params, _check_path_params, _check_sides, fit_homographies, smooth_path, warp_frames
+    video of fewer than two frames, a side above 4096 or a bad radius, sigma, crop_min, stride, hypotheses, tau, refine,
+    seed, sweeps, max_distance, alpha1 or alpha2.  Inference only: with grad enabled on a model that requires grad it raises
+    ValueError.
+
+    fill=True fills every pixel with valid = 0 from the neighbouring frames (rnc.stabilize's step 5, the motion inpainting
+    of Matsushita et al.), and each dict gains source uint8 [T_v,H,W] (rnc.inpaint's SOURCE_* map, SOURCE_KNOWN where the
+    pixel comes from its own frame).  crop and fill are independent: crop=False, fill=True is the full-frame stabilizer;
+    crop=True with crop_min above the video's alpha zooms part of the way and fills the rest.  The flow pass is then
+    run_sequences_bidirectional(..., alpha1=alpha1, alpha2=alpha2), whose forward flows are run_sequences' bit for bit, so
+    motion, transforms, alpha, the fit counts, valid and the pixels with valid != 0 are fill=False's; both flows of every
+    pair are kept in stacked device tensors, a shorter video padded as inpaint_videos pads it.  Then
+    rnc.stabilize.fill_uncovered(..., sweeps, max_distance, alpha1, alpha2) runs on the stack.  With T the longest video's
+    frame count it keeps V T (12 B warped + 12 B filled frames + 1 B valid + 1 B hole + 1 B source) + V (T - 1) (2 flows
+    and 2 residuals x 2 channels x 4 B + 2 occlusion masks x 1 B + 2 x 4 B of consistency error while it is checked) ~ 69
+    V T bytes per pixel, plus at most 1 GiB of fill workspace: e.g. 11.3 GB for eight 50-frame videos of 480x854 (17.3 GB
+    peak measured on that workload with the model, its workspace and the input frames on the device)."""
+    from .stabilize import (_check_fill_params, _check_fit_params, _check_path_params, _check_sides, _fill, fit_homographies,
+                            smooth_path, warp_frames)
     what = "stabilize_videos"
     if model._needs_grad():
         raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
     _check_fit_params(stride, hypotheses, tau, refine, seed, what)
     _check_path_params(radius, sigma, crop_min, what)
+    if fill:
+        _check_fill_params(sweeps, max_distance, alpha1, alpha2, what)
     for seq in sequences:
         if len(seq) < 2:
             raise ValueError(f"{what}: a video needs T >= 2 frames, got {len(seq)}")
         _check_sides(*seq[0].shape[-2:], what)
     from . import native
     fits = [[None] * (len(seq) - 1) for seq in sequences]
-    ws = None
-    for s, k, flow in run_sequences(model, sequences, iters, warm_start=warm_start, batch_size=batch_size, mode=mode,
-                                    device=device):
+    ws = flows = None
+    kw = dict(warm_start=warm_start, batch_size=batch_size, mode=mode, device=device)
+    if fill:
+        pairs = ((s, k, r["flow_up"], r["flow_up_bw"])
+                 for s, k, r in run_sequences_bidirectional(model, sequences, iters, alpha1=alpha1, alpha2=alpha2, **kw))
+    else:
+        pairs = ((s, k, flow, None) for s, k, flow in run_sequences(model, sequences, iters, **kw))
+    for s, k, flow, flow_bw in pairs:
         if flow.is_cuda and ws is None:
             H, W = flow.shape[-2:]
             ws = torch.empty(native.rnc.homography_fit_workspace_bytes(1, H, W, stride, hypotheses), dtype=torch.uint8,
                              device=flow.device)
         fits[s][k] = fit_homographies(flow[None], stride, hypotheses, tau, refine, seed, workspace=ws)
+        if flow_bw is not None:
+            if flows is None:
+                V, T = len(sequences), max(len(seq) for seq in sequences)
+                flows = torch.zeros(2, V, T - 1, *flow.shape, dtype=torch.float32, device=flow.device)
+            flows[0, s, k].copy_(flow)
+            flows[1, s, k].copy_(flow_bw)
     out = []
     for seq, fit in zip(sequences, fits):
         A, inl, mat, st = (torch.cat([f[j] for f in fit]) for j in range(4))
@@ -932,35 +961,76 @@ def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8,
         frames, valid = warp_frames(torch.stack([f.to(dev).float() for f in seq]), Minv[0])
         out.append({"frames": frames, "valid": valid, "motion": A, "transforms": M[0], "alpha": alpha[0], "inliers": inl,
                     "matched": mat, "status": st})
+        if fill:
+            out[-1]["transforms_inv"] = Minv[0]
+    if fill and out:
+        _fill_stabilized(out, flows, sweeps, max_distance, alpha1, alpha2, _fill)
     return out
+
+
+def _fill_stabilized(out, flows, sweeps, max_distance, alpha1, alpha2, fill):
+    """stabilize_videos' fill: the results stacked and padded (zero frames without holes, identity motion and maps, and
+    fill's padding pairs occluded in both directions), filled, and written back into each dict with its source map."""
+    lens = [r["frames"].shape[0] for r in out]
+    V, T = len(out), max(lens)
+    _, C, H, W = out[0]["frames"].shape
+    dev = out[0]["frames"].device
+    eye = torch.eye(3, dtype=torch.float64, device=dev)
+    frames = torch.zeros(V, T, C, H, W, dtype=torch.float32, device=dev)
+    valid = torch.ones(V, T, H, W, dtype=torch.uint8, device=dev)
+    motion = eye.repeat(V, T - 1, 1, 1)
+    maps, maps_inv = eye.repeat(V, T, 1, 1), eye.repeat(V, T, 1, 1)
+    for v, r in enumerate(out):
+        n = lens[v]
+        frames[v, :n], valid[v, :n], motion[v, :n - 1] = r["frames"], r["valid"], r["motion"]
+        maps[v, :n], maps_inv[v, :n] = r["transforms"], r.pop("transforms_inv")
+    res, source = fill(frames, valid, flows[0], flows[1], motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2,
+                       lengths=lens)
+    for v, r in enumerate(out):
+        r["frames"], r["source"] = res[v, :lens[v]], source[v, :lens[v]]
 
 
 @torch.no_grad()
 def validate_stabilization(model, sequences, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda", radius=30,
-                           sigma=10.0, crop=True, crop_min=0.5, stride=8, hypotheses=256, tau=2.0, refine=4, seed=0):
+                           sigma=10.0, crop=True, crop_min=0.5, stride=8, hypotheses=256, tau=2.0, refine=4, seed=0, fill=False,
+                           sweeps=512, max_distance=None, alpha1=0.01, alpha2=0.5):
     """The standard stabilization scores of stabilize_videos' output beside the input's (Liu et al. 2013; ITF of Matsushita
     et al. 2006), from the known maps rather than re-estimated features (rnc.stabilize.stabilization_metrics, on the host in
     fp64): cropping, distortion, stability_translation, stability_rotation and stability of the output, and the input's
     input_stability_*; itf and input_itf, each the mean over a video's consecutive frame pairs of their PSNR
     (rnc.interp.interpolation_error's partials on the device, rnc.inpaint.psnr's 100 dB cap), then over videos; frames and
-    videos, their numbers (rnc.stabilize.summarize_stabilization).  Arguments as stabilize_videos'.  Under
-    torch.distributed rank r takes the videos of index = r (mod world), the per-video records are all-gathered, and every
-    rank returns the single-process result."""
+    videos, their numbers (rnc.stabilize.summarize_stabilization).  Arguments as stabilize_videos'.  With fill=True two
+    scores are added, each the mean over a video's frames and then over videos: filled, the share of output pixels not
+    taken from their own frame (source != SOURCE_KNOWN), and filled_spatial, the share filled spatially (SOURCE_SPATIAL).
+    Under torch.distributed rank r takes the videos of index = r (mod world), the per-video records are all-gathered, and
+    every rank returns the single-process result."""
     from .dist import gather_strided, strided_items, world_rank
+    from .inpaint import SOURCE_KNOWN, SOURCE_SPATIAL
     from .interp import interpolation_error
     from .stabilize import stabilization_metrics, summarize_stabilization
     world, rank = world_rank()
     mine = [sequences[i] for i in strided_items(range(len(sequences)), world, rank)]
     res = stabilize_videos(model, mine, iters, warm_start, batch_size, mode, device, radius, sigma, crop, crop_min, stride,
-                           hypotheses, tau, refine, seed)
+                           hypotheses, tau, refine, seed, fill, sweeps, max_distance, alpha1, alpha2)
     records = []
     for seq, r in zip(mine, res):
         out = r["frames"]
         inp = torch.stack([f.to(out.device).float() for f in seq])
         rows = [interpolation_error(v[1:], v[:-1]) for v in (out, inp)]
-        records.append((stabilization_metrics(r["motion"], r["transforms"]),
-                        *[list(zip(e.sq_sum.tolist(), e.count.tolist())) for e in rows]))
-    return summarize_stabilization(gather_strided(records, world))
+        rec = (stabilization_metrics(r["motion"], r["transforms"]),
+               *[list(zip(e.sq_sum.tolist(), e.count.tolist())) for e in rows])
+        if fill:                                         # per frame: pixels, filled pixels, spatially filled pixels
+            src = r["source"].flatten(1)
+            rec += ([[src.shape[1], a, b] for a, b in zip((src != SOURCE_KNOWN).sum(1).tolist(),
+                                                          (src == SOURCE_SPATIAL).sum(1).tolist())],)
+        records.append(rec)
+    records = gather_strided(records, world)
+    summary = summarize_stabilization([r[:3] for r in records])
+    if fill:
+        n = len(records)
+        for j, key in ((1, "filled"), (2, "filled_spatial")):
+            summary[key] = sum(sum(f[j] / f[0] for f in r[3]) / len(r[3]) for r in records) / n if n else math.nan
+    return summary
 
 
 def size_batches(items, batch_size, key):

@@ -199,6 +199,9 @@ SIGNATURES = {
     "rnc_stabilize_path": (_i, [_vp, _i, _i, _vp, _i, _i, _i, _i, C.c_double, _vp, _vp, _vp, _vp]),
     "rnc_stabilize_warp": (_i, [_vp, *[C.c_longlong] * 4, _vp, _i, _i, _i, _i, _vp, *[C.c_longlong] * 4, _vp,
                                 *[C.c_longlong] * 3, _vp]),
+    "rnc_stabilize_flow_residual": (_i, [_vp, *[C.c_longlong] * 5, _vp, *[C.c_longlong] * 5, _vp, _vp, _vp, _i, _i, _i, _i,
+                                         _vp, _vp, _vp]),
+    "rnc_stabilize_flow_readd": (_i, [_vp, _vp, _vp, _i, _i, _i, _i, _vp, _vp, _vp]),
 }
 DIST2_NONE = 2147483647                                    # RNC_DIST2_NONE
 REGIONS_SINTEL, REGIONS_KITTI = 0, 1                       # rnc_region_metrics' kind

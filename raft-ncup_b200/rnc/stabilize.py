@@ -1,4 +1,5 @@
-"""Video stabilization from the forward flows: fit each pair's camera motion, smooth the camera path, warp and crop, and score.
+"""Video stabilization from the forward flows: fit each pair's camera motion, smooth the camera path, warp and crop or fill the
+uncovered borders from neighbouring frames, and score.
 
 Inputs: one video of T >= 2 frames [C,H,W] and the forward flows F_k (frame k -> k+1, float32 [2,H,W], channel 0 = x) that
 rnc.harness.run_sequences yields.  Every step below is fixed down to the order of its floating-point operations, each rounded
@@ -56,6 +57,31 @@ once (no FMA, no transcendental function on the device), so the kernels (csrc/st
 4. Warp (rnc_stabilize_warp): output pixel u = (x, y) of frame t takes q = inv(M_t) u, ((m0 x + m1 y) + m2) / ((m6 x + m7 y)
    + m8) and the same for y, in fp64, rounded once to float32.  It is valid when w > 0 and q lies in [0, W-1] x [0, H-1];
    its value is then csrc/bilinear.cuh's sample of each channel, otherwise 0 with valid = 0.
+5. Fill (fill_uncovered, the motion inpainting of Matsushita et al.; csrc/stabilize_fill.cu): the pixels with valid = 0 are
+   carried along the flows from the frames that see them, instead of being cropped.  Inputs, per video: the warped frames
+   and valid masks of step 4, the maps M_t and M_t^-1 of step 2, the motions A_k of step 1, and the forward flows F_k (frame
+   k -> k+1) and backward flows G_k (frame k+1 -> k) in input coordinates (run_sequences_bidirectional's flow_up and
+   flow_up_bw).  pi(P p) is ((p0 x + p1 y) + p2) / ((p6 x + p7 y) + p8) and the same for y in fp64 (each product, sum and
+   quotient rounded once), defined when the denominator is > 0; inv(A) is the adjugate divided by its [2][2] (as in step 2).
+   a. Residual transfer (rnc_stabilize_flow_residual), forward, output pixel u of frame k: q = M_k^-1 u exactly as step 4
+      computes it, with its validity; F = csrc/bilinear.cuh's sample of each channel of F_k at q; then
+      R_k(u) = pi(M_{k+1} (q + F)) - pi(M_{k+1} pi(A_k q)), q + F added in fp64, the subtraction in fp64, rounded once to
+      float32.  Backward, output pixel u of frame k+1: the same with M_{k+1}^-1, G_k, M_k and inv(A_k).  R is NaN where q is
+      not valid, where F is not finite and where a projection is undefined.  So the camera's motion, known exactly, is taken
+      out, and for a static scene R is 0 up to the flow's own error.
+   b. Residual completion: R~ = rnc.inpaint.harmonic_fill(R, valid == 0, sweeps), the unknown set being output frame k's
+      pixels with valid = 0 (frame k+1's for the backward residual) plus R's NaNs, which are exactly them when the flow is
+      finite and every projection defined.
+   c. Global re-add (rnc_stabilize_flow_readd): F~_k(u) = (pi(M_{k+1} pi(A_k q)) - u) + R~_k(u), q = M_k^-1 u rounded to
+      float32 as in a (for every pixel, inside the frame or not), the subtraction and the addition in fp64, rounded once to
+      float32; NaN where a projection is undefined; backward likewise.  The global term is exact for a homography across
+      the whole border, where completing the full flow by a Laplace fill would bend it.
+   d. Chains (rnc.inpaint's steps 3-4 on the output frames): occ, occ_bw = rnc.metrics.fb_consistency(F~, G~, alpha1,
+      alpha2); rnc.inpaint.inpaint_propagate(warped frames, valid == 0, F~, G~, occ, occ_bw, max_distance); then
+      harmonic_fill of the colours of the SOURCE_SPATIAL pixels.  The pixels with valid != 0 keep step 4's bits; source
+      holds rnc.inpaint's SOURCE_* values, SOURCE_KNOWN for a pixel taken from its own frame.  In a stack of videos of
+      different lengths, a shorter video's padding pairs are occluded in both directions, as rnc.harness.inpaint_videos
+      pads them, so each video's result does not depend on the others.
 
 Scores (stabilization_metrics, on the host in fp64, from the known maps rather than re-estimated features; Liu et al.,
 "Bundled camera paths for video stabilization", SIGGRAPH 2013): cropping, the mean over frames of 1 / |det| of M_t's affine
@@ -544,6 +570,204 @@ def host_warp_frames(frames, maps):
             out[n] = torch.where(okt, s, 0.0).float()
             valid[n] = okt.to(torch.uint8)
     return out, valid
+
+
+# ------------------------------------------------------------------------------------------------------------ the fill
+
+
+def _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, what):
+    """(V, T, H, W) of stacked flows [V,T-1,2,H,W], motion [V,T-1,3,3] and maps [V,T,3,3] on one device."""
+    if flow.dim() != 5 or flow.shape[2] != 2 or flow.shape[0] == 0 or flow.shape[1] == 0:
+        raise ValueError(f"{what}: expected flow [V,T-1,2,H,W], got {tuple(flow.shape)}")
+    V, T1, _, H, W = flow.shape
+    T = T1 + 1
+    for name, t, shape in (("flow_bw", flow_bw, (V, T1, 2, H, W)), ("motion", motion, (V, T1, 3, 3)),
+                           ("maps", maps, (V, T, 3, 3)), ("maps_inv", maps_inv, (V, T, 3, 3))):
+        if tuple(t.shape) != shape:
+            raise ValueError(f"{what}: expected {name} {list(shape)}, got {tuple(t.shape)}")
+    devs = {t.device for t in (flow, flow_bw, motion, maps, maps_inv)}
+    if len(devs) != 1:
+        raise ValueError(f"{what}: the flows, motion and maps must be on one device, got {sorted(map(str, devs))}")
+    if V > 65535 or T > 65536:
+        raise ValueError(f"{what}: at most 65535 videos of 65536 frames per call, got {V} of {T}")
+    _check_sides(H, W, what)
+    return V, T, H, W
+
+
+def _mats(*ts):
+    return [t.detach().to(torch.float64).contiguous() for t in ts]
+
+
+def flow_residual(flow, flow_bw, motion, maps, maps_inv):
+    """Step 5a for V videos: flow, flow_bw [V,T-1,2,H,W] (forward and backward flows in input coordinates, any strides,
+    float32 or converted to it), motion fp64 [V,T-1,3,3] (A_k), maps and maps_inv fp64 [V,T,3,3] (smooth_path's M and
+    Minv).  Returns (res, res_bw) float32 [V,T-1,2,H,W], contiguous, on the flows' device: pair k's residual in output frame
+    k's pixels and its backward residual in output frame k+1's, NaN where unknown.  CUDA tensors go through
+    rnc_stabilize_flow_residual (one launch), CPU tensors through host_flow_residual; they give the same bits.  ValueError
+    before any launch for mismatched shapes or devices, or a side above 4096."""
+    V, T, H, W = _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, "flow_residual")
+    if not flow.is_cuda:
+        return host_flow_residual(flow, flow_bw, motion, maps, maps_inv)
+    f, b = flow.detach().float(), flow_bw.detach().float()
+    A, M, Mi = _mats(motion, maps, maps_inv)
+    res = torch.empty(2, V, T - 1, 2, H, W, dtype=torch.float32, device=flow.device)
+    with torch.cuda.device(flow.device):
+        native.rnc.stabilize_flow_residual(f, *f.stride(), b, *b.stride(), A, M, Mi, V, T, H, W, res[0], res[1])
+    return res[0], res[1]
+
+
+def _readd_(res, res_bw, motion, maps, maps_inv):
+    """Step 5c in place on float32 contiguous res, res_bw [V,T-1,2,H,W]."""
+    V, T1, _, H, W = res.shape
+    if not res.is_cuda:
+        r = _host_flows(res, res_bw, motion, maps, maps_inv, True)
+        res.copy_(r[0])
+        res_bw.copy_(r[1])
+        return
+    A, M, Mi = _mats(motion, maps, maps_inv)
+    with torch.cuda.device(res.device):
+        native.rnc.stabilize_flow_readd(A, M, Mi, V, T1 + 1, H, W, res, res_bw)
+
+
+def add_global_motion(res, res_bw, motion, maps, maps_inv):
+    """Step 5c for V videos: the completed residuals res, res_bw [V,T-1,2,H,W] (any strides, float32 or converted to it)
+    with the camera's motion added back, as new float32 [V,T-1,2,H,W] tensors: the flows of the output frames, forward
+    (frame k -> k+1, in frame k's pixels) and backward (frame k+1 -> k).  CUDA tensors go through rnc_stabilize_flow_readd
+    (one launch), CPU tensors through host_add_global_motion; they give the same bits.  ValueError before any launch for
+    mismatched shapes or devices, or a side above 4096."""
+    _check_flow_maps(res, res_bw, motion, maps, maps_inv, "add_global_motion")
+    if not res.is_cuda:
+        return host_add_global_motion(res, res_bw, motion, maps, maps_inv)
+    out = torch.stack([res.detach().float(), res_bw.detach().float()])
+    _readd_(out[0], out[1], motion, maps, maps_inv)
+    return out[0], out[1]
+
+
+def _host_project(m, x, y):
+    """pi(m (x, y, 1)) in numpy fp64, each operation rounded once: (X / w, Y / w, w > 0)."""
+    X = (m[0] * x + m[1] * y) + m[2]
+    Y = (m[3] * x + m[4] * y) + m[5]
+    w = (m[6] * x + m[7] * y) + m[8]
+    return X / w, Y / w, w > 0
+
+
+def _host_direction(src, dst, A, f, r):
+    """One direction of step 5a (r None: f fp64 [2,H,W] holding the flow's float32 values) or 5c (r: the completed residual,
+    fp64 [2,H,W] holding float32 values) over every output pixel: float32 [2,H,W]."""
+    H, W = f.shape[-2:] if r is None else r.shape[-2:]
+    y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
+    X, Y, ok = _host_project(src, x, y)
+    qx, qy = X.astype(np.float32).astype(np.float64), Y.astype(np.float32).astype(np.float64)
+    bx, by, ok_b = _host_project(A, qx, qy)
+    gx, gy, ok_g = _host_project(dst, bx, by)
+    ok = ok & ok_b & ok_g
+    if r is not None:
+        out = np.stack([(gx - x) + r[0], (gy - y) + r[1]])
+        return np.where(ok, out, np.nan).astype(np.float32)
+    ok &= (qx >= 0) & (qx <= W - 1) & (qy >= 0) & (qy <= H - 1)
+    px = torch.from_numpy(np.where(ok, qx, 0.0))
+    py = torch.from_numpy(np.where(ok, qy, 0.0))
+    u = _sample(torch.from_numpy(f), px, py).numpy()
+    ok &= np.isfinite(u).all(0)
+    ax, ay, ok_a = _host_project(dst, qx + u[0], qy + u[1])
+    ok &= ok_a
+    return np.where(ok, np.stack([ax - gx, ay - gy]), np.nan).astype(np.float32)
+
+
+def _host_flows(a, b, motion, maps, maps_inv, readd):
+    """Steps 5a (readd False: a, b the flows) and 5c (readd True: a, b the completed residuals), every video and pair."""
+    V, T1, _, H, W = a.shape
+    out = torch.empty(2, V, T1, 2, H, W, dtype=torch.float32)
+    A, M, Mi = (t.detach().cpu().to(torch.float64).numpy().reshape(t.shape[0], t.shape[1], 9) for t in (motion, maps, maps_inv))
+    with np.errstate(all="ignore"):
+        for v in range(V):
+            for k in range(T1):
+                fa, fb = (t[v, k].detach().cpu().float().double().numpy() for t in (a, b))
+                Ai = _inv(A[v, k].reshape(3, 3)).ravel()
+                fw = _host_direction(Mi[v, k], M[v, k + 1], A[v, k], None if readd else fa, fa if readd else None)
+                bw = _host_direction(Mi[v, k + 1], M[v, k], Ai, None if readd else fb, fb if readd else None)
+                out[0, v, k], out[1, v, k] = torch.from_numpy(fw), torch.from_numpy(bw)
+    return out[0], out[1]
+
+
+def host_flow_residual(flow, flow_bw, motion, maps, maps_inv):
+    """flow_residual's rule in numpy fp64, one output frame at a time and all its pixels at once; the flow sampled by
+    rnc.interp._sample.  Serves CPU tensors and is the kernel's test reference.  Returns (res, res_bw) on the CPU."""
+    _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, "flow_residual")
+    return _host_flows(flow, flow_bw, motion, maps, maps_inv, False)
+
+
+def host_add_global_motion(res, res_bw, motion, maps, maps_inv):
+    """add_global_motion's rule in numpy fp64, one output frame at a time.  Returns (flow, flow_bw) on the CPU."""
+    _check_flow_maps(res, res_bw, motion, maps, maps_inv, "add_global_motion")
+    return _host_flows(res, res_bw, motion, maps, maps_inv, True)
+
+
+def _check_fill_params(sweeps, max_distance, alpha1, alpha2, what):
+    from .inpaint import _check_sweeps
+    _check_sweeps(sweeps, what)
+    if max_distance is not None and (not isinstance(max_distance, int) or max_distance < 1):
+        raise ValueError(f"{what}: expected max_distance >= 1 or None, got {max_distance!r}")
+    for name, a in (("alpha1", alpha1), ("alpha2", alpha2)):
+        if not isinstance(a, (int, float)) or isinstance(a, bool) or not 0 <= a <= 1e30:
+            raise ValueError(f"{what}: expected a finite {name} >= 0, got {a!r}")
+
+
+def _check_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2):
+    from .inpaint import _check_video
+    V, T, H, W = _check_video(frames, valid, flow, flow_bw, "fill_uncovered")
+    _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, "fill_uncovered")
+    if frames.device != flow.device or valid.device != flow.device:
+        raise ValueError(f"fill_uncovered: the frames, valid masks, flows, motion and maps must be on one device, got "
+                         f"{frames.device}, {valid.device} and {flow.device}")
+    _check_fill_params(sweeps, max_distance, alpha1, alpha2, "fill_uncovered")
+    return V, T, H, W
+
+
+def _fill(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2, lengths=None):
+    """Step 5 on the tensors' device.  With lengths, video v's pairs from lengths[v] - 1 on are padding: occluded in both
+    directions, so no chain enters them."""
+    from .inpaint import SOURCE_SPATIAL, harmonic_fill, inpaint_propagate
+    from .metrics import fb_consistency
+    V, T1, _, H, W = flow.shape
+    res, res_bw = flow_residual(flow, flow_bw, motion, maps, maps_inv)
+    hole = (valid == 0).to(torch.uint8)
+    harmonic_fill(res, hole[:, :-1], sweeps, out=res)
+    harmonic_fill(res_bw, hole[:, 1:], sweeps, out=res_bw)
+    _readd_(res, res_bw, motion, maps, maps_inv)
+    occ, occ_bw, _, _ = fb_consistency(res.view(V * T1, 2, H, W), res_bw.view(V * T1, 2, H, W), alpha1, alpha2)
+    occ, occ_bw = occ.view(V, T1, H, W), occ_bw.view(V, T1, H, W)
+    for v, n in enumerate(lengths or ()):
+        occ[v, n - 1:] = 1
+        occ_bw[v, n - 1:] = 1
+    out, source = inpaint_propagate(frames, hole, res, res_bw, occ, occ_bw, max_distance)
+    harmonic_fill(out, source == SOURCE_SPATIAL, sweeps, out=out)
+    return out, source
+
+
+def fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps=512, max_distance=None, alpha1=0.01,
+                   alpha2=0.5):
+    """Step 5 for V videos stacked as rnc.inpaint stacks them: frames [V,T,3,H,W] and valid [V,T,H,W] (warp_frames' output,
+    0..255), flow, flow_bw [V,T-1,2,H,W] (forward and backward flows in input coordinates), motion fp64 [V,T-1,3,3], maps
+    and maps_inv fp64 [V,T,3,3] (smooth_path's M and Minv); any strides, the inputs are not modified.  sweeps is
+    harmonic_fill's, for the residuals and the spatial fill; max_distance the longest chain in frames (None: T - 1);
+    alpha1, alpha2 fb_consistency's.  Returns (frames float32 [V,T,3,H,W], source uint8 [V,T,H,W]): every pixel with
+    valid != 0 keeps its bits and is SOURCE_KNOWN, every other one is filled.  CUDA tensors run on the kernels, CPU tensors
+    through host_fill_uncovered; they give the same bits.  ValueError before any launch for mismatched shapes or devices,
+    T < 2, a side above 4096, sweeps < 0, max_distance < 1 or a negative or non-finite alpha1 or alpha2."""
+    _check_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2)
+    if not frames.is_cuda:
+        return host_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2)
+    return _fill(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2)
+
+
+def host_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps=512, max_distance=None, alpha1=0.01,
+                        alpha2=0.5):
+    """fill_uncovered on CPU copies of the inputs, so through host_flow_residual, rnc.inpaint.host_harmonic_fill,
+    host_add_global_motion, rnc.metrics.host_fb_consistency and rnc.inpaint.host_inpaint_propagate.  Returns CPU tensors."""
+    _check_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2)
+    return _fill(*(t.detach().cpu() for t in (frames, valid, flow, flow_bw, motion, maps, maps_inv)), sweeps, max_distance,
+                 alpha1, alpha2)
 
 
 # -------------------------------------------------------------------------------------------------------------- scores

@@ -69,12 +69,7 @@ def shaky_sequence(n, h, w, seed=0, pan=(2.0, 0.5), jitter_px=3.0, jitter_rot=0.
     seeded jitters of std jitter_rot (radians) and jitter_scale.  Returns (frames: list of float32 [3,h,w], C fp64 [n,3,3],
     flows float32 [n-1,2,h,w]), flow k being the exact forward flow C_{k+1} C_k^-1 p - p of frame k's pixels p."""
     import numpy as np
-    rng = np.random.default_rng(seed)
-    K = 8
-    freq = rng.uniform(2 * np.pi / 60, 2 * np.pi / 12, (3, K)) * np.exp(1j * rng.uniform(0, 2 * np.pi, (3, K)))
-    amp = rng.uniform(0.5, 1.0, (3, K))
-    amp *= 110 / amp.sum(1, keepdims=True)
-    phase = rng.uniform(0, 2 * np.pi, (3, K))
+    rng, freq, amp, phase = _shaky_canvas_draws(seed)
     jit = rng.normal(0, 1, (n, 4))
     cx, cy = (w - 1) / 2, (h - 1) / 2
     Tc = np.array([[1.0, 0, cx], [0, 1.0, cy], [0, 0, 1]])
@@ -91,11 +86,52 @@ def shaky_sequence(n, h, w, seed=0, pan=(2.0, 0.5), jitter_px=3.0, jitter_rot=0.
     for t in range(n):
         X, Y, Wh = np.linalg.inv(C[t]) @ P
         X, Y = X / Wh, Y / Wh
-        img = 127.5 + (amp[..., None] * np.sin(freq.real[..., None] * X + freq.imag[..., None] * Y + phase[..., None])).sum(1)
+        img = _shaky_canvas(freq, amp, phase, X, Y)
         frames.append(torch.from_numpy(img.reshape(3, h, w)).float())
-    flows = np.empty((n - 1, 2, h, w))
-    for k in range(n - 1):
-        X, Y, Wh = C[k + 1] @ np.linalg.inv(C[k]) @ P
+    return frames, torch.from_numpy(C), _shaky_flows(C, h, w, False)
+
+
+def _shaky_canvas_draws(seed):
+    """The generator of shaky_sequence after its canvas draws, and those draws: (rng, freq, amp, phase)."""
+    import numpy as np
+    rng = np.random.default_rng(seed)
+    K = 8
+    freq = rng.uniform(2 * np.pi / 60, 2 * np.pi / 12, (3, K)) * np.exp(1j * rng.uniform(0, 2 * np.pi, (3, K)))
+    amp = rng.uniform(0.5, 1.0, (3, K))
+    amp *= 110 / amp.sum(1, keepdims=True)
+    phase = rng.uniform(0, 2 * np.pi, (3, K))
+    return rng, freq, amp, phase
+
+
+def _shaky_canvas(freq, amp, phase, X, Y):
+    import numpy as np
+    return 127.5 + (amp[..., None] * np.sin(freq.real[..., None] * X + freq.imag[..., None] * Y + phase[..., None])).sum(1)
+
+
+def _shaky_flows(C, h, w, backward):
+    import numpy as np
+    ys, xs = np.mgrid[0:h, 0:w].astype(np.float64)
+    P = np.stack([xs, ys, np.ones_like(xs)]).reshape(3, -1)
+    flows = np.empty((C.shape[0] - 1, 2, h, w))
+    for k in range(C.shape[0] - 1):
+        a, b = (k, k + 1) if backward else (k + 1, k)
+        X, Y, Wh = C[a] @ np.linalg.inv(C[b]) @ P
         flows[k, 0] = (X / Wh - P[0]).reshape(h, w)
         flows[k, 1] = (Y / Wh - P[1]).reshape(h, w)
-    return frames, torch.from_numpy(C), torch.from_numpy(flows).float()
+    return torch.from_numpy(flows).float()
+
+
+def shaky_canvas(x, y, seed=0):
+    """shaky_sequence(..., seed)'s canvas (the same draws) at canvas points x, y (fp64 arrays of one shape), evaluated in fp64
+    as shaky_sequence renders it.  Returns fp64 [3, *x.shape] (numpy): the true content of any output pixel, e.g. of a
+    stabilized frame's uncovered border, whose canvas point is C_t^-1 M_t^-1 u."""
+    import numpy as np
+    _, freq, amp, phase = _shaky_canvas_draws(seed)
+    x, y = np.asarray(x, dtype=np.float64), np.asarray(y, dtype=np.float64)
+    return _shaky_canvas(freq, amp, phase, x.reshape(-1), y.reshape(-1)).reshape(3, *x.shape)
+
+
+def shaky_backward_flows(C, h, w):
+    """The exact backward flows of a shaky_sequence video with cameras C (fp64 [n,3,3]) at h x w: float32 [n-1,2,h,w], flow
+    k being C_k C_{k+1}^-1 p - p of frame k+1's pixels p."""
+    return _shaky_flows(torch.as_tensor(C).double().numpy(), h, w, True)
