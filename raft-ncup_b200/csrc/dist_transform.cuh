@@ -124,6 +124,13 @@ __global__ void __launch_bounds__(32) dist2_row_kernel(int H, int W, int* __rest
   }
 }
 
+// the Out of a squared-distance map: each pixel's squared distance to its nearest site, None in an image without a site
+template <int None>
+struct Dist2 {
+  static constexpr int none = None;
+  __device__ int operator()(int, int x, int q, int, int fq) const { return fq - q * q + (x - q) * (x - q); }
+};
+
 inline size_t dist2_row_smem(int W) { return static_cast<size_t>(W) * (sizeof(int) + 2 * sizeof(unsigned short)); }
 
 }  // namespace rnc

@@ -8,6 +8,8 @@
 // (image, cell)'s CTAs with a warp: lane-strided, then warp_sum.  The grid's x extent depends only on H*W, so the order of every
 // addition depends only on the image's size.
 #pragma once
+#include <type_traits>
+
 #include "rnc_common.cuh"
 
 namespace rnc {
@@ -31,14 +33,26 @@ __device__ __forceinline__ PixelMetrics pixel_metrics(float f0, float f1, float 
 // A tensor through element strides: [B,C,H,W], or a [B,H,W] mask with c unused.
 template <typename T>
 struct StridedView {
-  const T* p;
+  T* p;
   long long b, c, y, x;
-  __device__ __forceinline__ const T* pixel(int bi, int yi, int xi) const { return p + bi * b + yi * y + xi * x; }
-  __device__ __forceinline__ T at(int bi, int ci, int yi, int xi) const { return pixel(bi, yi, xi)[ci * c]; }
-  __device__ __forceinline__ T at(int bi, int yi, int xi) const { return *pixel(bi, yi, xi); }
+  __device__ __forceinline__ T* pixel(int bi, int yi, int xi) const { return p + bi * b + yi * y + xi * x; }
+  __device__ __forceinline__ std::remove_const_t<T> at(int bi, int ci, int yi, int xi) const { return pixel(bi, yi, xi)[ci * c]; }
+  __device__ __forceinline__ std::remove_const_t<T> at(int bi, int yi, int xi) const { return *pixel(bi, yi, xi); }
 };
-using View = StridedView<float>;
-using MaskView = StridedView<unsigned char>;       // uint8 masks, visible where 0
+using View = StridedView<const float>;
+using MaskView = StridedView<const unsigned char>;   // uint8 masks, visible where 0
+using OutView = StridedView<float>;
+using OutMaskView = StridedView<unsigned char>;
+
+// A stack of such tensors, one per video ([V][B,C,H,W]) through the stride v between videos: video(i) is video i's view.
+template <typename T>
+struct VideoView {
+  T* p;
+  long long v, b, c, y, x;
+  __device__ __forceinline__ StridedView<T> video(int i) const { return {p + i * v, b, c, y, x}; }
+};
+using Video = VideoView<const float>;
+using VideoMask = VideoView<const unsigned char>;
 
 inline bool aligned(const void* p, uintptr_t n) { return (reinterpret_cast<uintptr_t>(p) & (n - 1)) == 0; }
 
@@ -82,6 +96,57 @@ __device__ __forceinline__ MetricsPart warp_sum(MetricsPart v) {
   for (int c = 0; c < kMetCounts; ++c) v.n[c] = __reduce_add_sync(0xffffffffu, v.n[c]);
   return v;
 }
+
+struct SumCount {                     // a set of pixels' fp64 sum and count; 16 bytes
+  double sum;
+  unsigned n, pad;
+  __device__ __forceinline__ SumCount& operator+=(const SumCount& o) {
+    sum += o.sum;
+    n += o.n;
+    return *this;
+  }
+};
+
+__device__ __forceinline__ SumCount warp_sum(SumCount v) {
+  v.sum = warp_sum(v.sum);
+  v.n = __reduce_add_sync(0xffffffffu, v.n);
+  return v;
+}
+
+struct SumCountStore {                // partials of (image, cell) i -> sum [i], count [i]
+  double* sum;
+  long long* count;
+  __device__ void operator()(int i, const SumCount& v) const {
+    sum[i] = v.sum;
+    count[i] = v.n;
+  }
+};
+
+template <int N>
+struct Counts {                       // N exact counts of a set of pixels
+  unsigned n[N];
+  __device__ __forceinline__ Counts& operator+=(const Counts& o) {
+#pragma unroll
+    for (int c = 0; c < N; ++c) n[c] += o.n[c];
+    return *this;
+  }
+};
+
+template <int N>
+__device__ __forceinline__ Counts<N> warp_sum(Counts<N> v) {
+#pragma unroll
+  for (int c = 0; c < N; ++c) v.n[c] = __reduce_add_sync(0xffffffffu, v.n[c]);
+  return v;
+}
+
+template <int N>
+struct CountsStore {                  // partials of (image, cell) i -> counts [i][N]
+  long long* counts;
+  __device__ void operator()(int i, const Counts<N>& v) const {
+#pragma unroll
+    for (int c = 0; c < N; ++c) counts[static_cast<long long>(i) * N + c] = v.n[c];
+  }
+};
 
 struct MetricsStore {                 // partials of (image, cell) i -> counts [i][5], epe_sum [i]
   long long* counts;

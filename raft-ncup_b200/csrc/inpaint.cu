@@ -36,36 +36,12 @@ constexpr int kPropThreads = 256;
 constexpr int kSsimRadius = 5;
 constexpr float kPiF32 = 3.14159265358979f;
 
-// [A][B][C][H][W] through element strides
-struct View5 {
-  const float* p;
-  long long a, b, c, y, x;
-  int B;
-  __device__ __forceinline__ const float* pixel(int i, int yi, int xi) const {
-    const int ia = i / B, ib = i - ia * B;
-    return p + ia * a + ib * b + yi * y + xi * x;
-  }
-};
-
-struct Mask4 {                                // [A][B][H][W] through element strides
-  const unsigned char* p;
-  long long a, b, y, x;
-  int B;
-  __device__ __forceinline__ unsigned char at(int i, int yi, int xi) const {
-    const int ia = i / B, ib = i - ia * B;
-    return p[ia * a + ib * b + yi * y + xi * x];
-  }
-};
-
-struct Out5 {
-  float* p;
-  long long a, b, c, y, x;
-  int B;
-  __device__ __forceinline__ float* pixel(int i, int yi, int xi) const {
-    const int ia = i / B, ib = i - ia * B;
-    return p + ia * a + ib * b + yi * y + xi * x;
-  }
-};
+// image i of the A*B images of a [A][B][C][H][W] view (v the A stride, b the B stride)
+template <typename T>
+__device__ __forceinline__ T* image_pixel(const VideoView<T>& t, int B, int i, int y, int x) {
+  const int ia = i / B, ib = i - ia * B;
+  return t.video(ia).pixel(ib, y, x);
+}
 
 struct FillBlock {                            // one CTA's part of an image: unknown pixels per colour and their bounding box
   int n[2];
@@ -86,31 +62,19 @@ struct FillLayout {                           // the workspace
   FillImage* images;                          // [N]
 };
 
-__host__ __device__ __forceinline__ size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
-
-FillLayout fill_layout(void* ws, int N, int H, int W) {
+FillLayout fill_layout(Carve& ws, int N, int H, int W) {
   const size_t px = static_cast<size_t>(N) * H * W;
   const int nblk = (H * W + kFillThreads - 1) / kFillThreads;
-  char* p = static_cast<char*>(ws);
   FillLayout l;
-  l.map = reinterpret_cast<int*>(p);
-  p += align16(px * sizeof(int));
-  l.blocks = reinterpret_cast<FillBlock*>(p);
-  p += align16(static_cast<size_t>(N) * nblk * sizeof(FillBlock));
-  l.images = reinterpret_cast<FillImage*>(p);
-  p += align16(static_cast<size_t>(N) * sizeof(FillImage));
-  l.known = reinterpret_cast<unsigned char*>(p);
+  l.map = ws.take<int>(px);
+  l.blocks = ws.take<FillBlock>(static_cast<size_t>(N) * nblk);
+  l.images = ws.take<FillImage>(N);
+  l.known = ws.take<unsigned char>(px);
   return l;
 }
 
-size_t fill_bytes(int N, int H, int W) {
-  const size_t px = static_cast<size_t>(N) * H * W;
-  const int nblk = (H * W + kFillThreads - 1) / kFillThreads;
-  return align16(px * sizeof(int)) + align16(static_cast<size_t>(N) * nblk * sizeof(FillBlock)) +
-         align16(static_cast<size_t>(N) * sizeof(FillImage)) + align16(px);
-}
-
-__global__ void __launch_bounds__(kFillThreads) known_kernel(View5 in, Mask4 unknown, int C, int H, int W, FillLayout l) {
+__global__ void __launch_bounds__(kFillThreads) known_kernel(Video in, VideoMask unknown, int B, int C, int H, int W,
+                                                             FillLayout l) {
   const int i = blockIdx.y, hw = H * W;
   const int p = blockIdx.x * kFillThreads + threadIdx.x;
   bool unk = false;
@@ -118,8 +82,8 @@ __global__ void __launch_bounds__(kFillThreads) known_kernel(View5 in, Mask4 unk
   if (p < hw) {
     y = p / W;
     x = p - y * W;
-    bool known = unknown.at(i, y, x) == 0;
-    const float* v = in.pixel(i, y, x);
+    bool known = *image_pixel(unknown, B, i, y, x) == 0;
+    const float* v = image_pixel(in, B, i, y, x);
     for (int c = 0; c < C; ++c) known = known && finite(v[c * in.c]);
     l.known[static_cast<long long>(i) * hw + p] = known;
     unk = !known;
@@ -151,16 +115,16 @@ struct KnownSites {
 
 struct InitOut {                              // a known pixel keeps its values, an unknown one takes its nearest known pixel's
   static constexpr bool kStores = true;
-  View5 in;
-  Out5 out;
-  int C;
+  Video in;
+  VideoView<float> out;
+  int B, C;
   __device__ void store(int i, int y, int x, int q, int r) const {
-    float* o = out.pixel(i, y, x);
+    float* o = image_pixel(out, B, i, y, x);
     if (q < 0) {
       for (int c = 0; c < C; ++c) o[c * out.c] = 0.0f;
       return;
     }
-    const float* v = in.pixel(i, r, q);
+    const float* v = image_pixel(in, B, i, r, q);
     for (int c = 0; c < C; ++c) o[c * out.c] = v[c * in.c];
   }
 };
@@ -244,14 +208,14 @@ __global__ void __launch_bounds__(kFillThreads) compact_kernel(int H, int W, Fil
 }
 
 template <int Colour>
-__global__ void __launch_bounds__(kFillThreads) sor_kernel(Out5 u, int C, int H, int W, FillLayout l) {
+__global__ void __launch_bounds__(kFillThreads) sor_kernel(VideoView<float> u, int B, int C, int H, int W, FillLayout l) {
   const int i = blockIdx.y, hw = H * W;
   const FillImage im = l.images[i];
   const int n = im.n[Colour];
   const int* list = l.map + static_cast<long long>(i) * hw + (Colour ? im.n[0] : 0);
   for (int e = blockIdx.x * kFillThreads + threadIdx.x; e < n; e += gridDim.x * kFillThreads) {
     const int p = list[e], y = p / W, x = p - y * W;
-    float* o = u.pixel(i, y, x);
+    float* o = image_pixel(u, B, i, y, x);
     const bool up = y > 0, left = x > 0, right = x < W - 1, down = y < H - 1;
     const int nb = up + left + right + down;
     if (nb == 0) continue;                    // a 1x1 image: no neighbour, the value stays
@@ -281,18 +245,12 @@ struct PropArgs {
   long long iv, it, ic, iy, ix;
   const unsigned char* masks;                 // M [V][T][H][W]
   long long mv, mt, my, mx;
-  View flow[2];                               // F~_k, G~_k: b is the pair index k
-  long long flow_v[2];
-  MaskView occ[2];                            // occ~_k on frame k, occ~_bw_k on frame k+1
-  long long occ_v[2];
+  Video flow[2];                              // F~_k, G~_k: b is the pair index k
+  VideoMask occ[2];                           // occ~_k on frame k, occ~_bw_k on frame k+1
   float* out;                                 // [V][T][3][H][W] contiguous
   unsigned char* source;                      // [V][T][H][W] contiguous
   int T, H, W, max_distance;
 };
-
-__device__ __forceinline__ bool inside(float x, float y, int H, int W) {
-  return x >= 0.0f && x <= static_cast<float>(W - 1) && y >= 0.0f && y <= static_cast<float>(H - 1);
-}
 
 __device__ __forceinline__ unsigned char mask_at(const PropArgs& a, int v, int t, int y, int x) {
   return a.masks[v * a.mv + t * a.mt + y * a.my + x * a.mx];
@@ -302,11 +260,8 @@ __device__ __forceinline__ unsigned char mask_at(const PropArgs& a, int v, int t
 template <int Dir>
 __device__ __forceinline__ bool chain(const PropArgs& a, int v, int t, float x, float y, float c[3], int& d) {
   const int T = a.T, H = a.H, W = a.W;
-  const View& f = a.flow[Dir > 0 ? 0 : 1];
-  const MaskView& m = a.occ[Dir > 0 ? 0 : 1];
-  const long long fv = v * a.flow_v[Dir > 0 ? 0 : 1], mv = v * a.occ_v[Dir > 0 ? 0 : 1];
-  const View fl{f.p + fv, f.b, f.c, f.y, f.x};
-  const MaskView oc{m.p + mv, m.b, m.c, m.y, m.x};
+  const View fl = a.flow[Dir > 0 ? 0 : 1].video(v);
+  const MaskView oc = a.occ[Dir > 0 ? 0 : 1].video(v);
   int k = t;
   d = 0;
   for (;;) {
@@ -323,15 +278,16 @@ __device__ __forceinline__ bool chain(const PropArgs& a, int v, int t, float x, 
   }
   // the masked bilinear colour of I_k at (x, y): the taps outside the hole, weights and weighted colours added in tap order
   const BilinearTaps tp = bilinear_taps(x, y, H, W);
+  const float w[4] = {tp.w(0), tp.w(1), tp.w(2), tp.w(3)};
   float ws = -0.0f, s[3] = {-0.0f, -0.0f, -0.0f};
   const float* img = a.frames + v * a.iv + k * a.it;
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const int ty = tp.y[j >> 1], tx = tp.x[j & 1];
     if (mask_at(a, v, k, ty, tx) != 0) continue;
-    ws = __fadd_rn(ws, tp.w[j]);
+    ws = __fadd_rn(ws, w[j]);
 #pragma unroll
-    for (int ch = 0; ch < 3; ++ch) s[ch] = __fadd_rn(s[ch], __fmul_rn(tp.w[j], img[ch * a.ic + ty * a.iy + tx * a.ix]));
+    for (int ch = 0; ch < 3; ++ch) s[ch] = __fadd_rn(s[ch], __fmul_rn(w[j], img[ch * a.ic + ty * a.iy + tx * a.ix]));
   }
 #pragma unroll
   for (int ch = 0; ch < 3; ++ch) c[ch] = __fdiv_rn(s[ch], ws);
@@ -384,26 +340,10 @@ __constant__ float kGauss[2 * kSsimRadius + 1] = {
     1.028380124e-03f, 7.598758209e-03f, 3.600077331e-02f, 1.093606874e-01f, 2.130055428e-01f, 2.660117149e-01f,
     2.130055428e-01f, 1.093606874e-01f, 3.600077331e-02f, 7.598758209e-03f, 1.028380124e-03f};
 
-struct SsimPart {
-  double sum;
-  unsigned n, pad;
-  __device__ __forceinline__ SsimPart& operator+=(const SsimPart& o) {
-    sum += o.sum;
-    n += o.n;
-    return *this;
-  }
-};
-
-__device__ __forceinline__ SsimPart warp_sum(SsimPart v) {
-  v.sum = rnc::warp_sum(v.sum);
-  v.n = __reduce_add_sync(0xffffffffu, v.n);
-  return v;
-}
-
 struct SsimPixel {                            // cta_partials_kernel's pixel (n, y, x): the window centred on (y, x)
   View pred, gt;
   int H, W;
-  __device__ void operator()(SsimPart& acc, int n, int y, int x) const {
+  __device__ void operator()(SumCount& acc, int n, int y, int x) const {
     if (y < kSsimRadius || y >= H - kSsimRadius || x < kSsimRadius || x >= W - kSsimRadius) return;
     constexpr float C1 = 6.5025f, C2 = 58.5225f;          // (0.01 * 255)^2, (0.03 * 255)^2
     for (int c = 0; c < 3; ++c) {
@@ -431,15 +371,6 @@ struct SsimPixel {                            // cta_partials_kernel's pixel (n,
   }
 };
 
-struct SsimStore {
-  double* sum;
-  long long* count;
-  __device__ void operator()(int i, const SsimPart& p) const {
-    sum[i] = p.sum;
-    count[i] = p.n;
-  }
-};
-
 bool ssim_shape_ok(int N, int H, int W) { return eval_shape_ok(N, H, W) && H >= 2 * kSsimRadius + 1 && W >= 2 * kSsimRadius + 1; }
 
 }  // namespace
@@ -450,7 +381,10 @@ using namespace rnc;
 extern "C" {
 
 size_t rnc_harmonic_fill_workspace_bytes(int A, int B, int C, int H, int W) {
-  return fill_shape_ok(A, B, C, H, W) ? fill_bytes(A * B, H, W) : 0;
+  if (!fill_shape_ok(A, B, C, H, W)) return 0;
+  Carve ws{nullptr};
+  fill_layout(ws, A * B, H, W);
+  return ws.bytes;
 }
 
 int rnc_harmonic_fill(const float* values, long long va, long long vb, long long vc, long long vy, long long vx,
@@ -463,16 +397,17 @@ int rnc_harmonic_fill(const float* values, long long va, long long vb, long long
   if (workspace_bytes < rnc_harmonic_fill_workspace_bytes(A, B, C, H, W)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
   const int N = A * B, hw = H * W, nblk = (hw + kFillThreads - 1) / kFillThreads;
-  const View5 in{values, va, vb, vc, vy, vx, B};
-  const Mask4 unk{unknown, ua, ub, uy, ux, B};
-  const Out5 o{out, oa, ob, oc, oy, ox, B};
-  const FillLayout l = fill_layout(workspace, N, H, W);
-  known_kernel<<<dim3(nblk, N), kFillThreads, 0, s>>>(in, unk, C, H, W, l);
+  const Video in{values, va, vb, vc, vy, vx};
+  const VideoMask unk{unknown, ua, ub, 0, uy, ux};
+  const VideoView<float> o{out, oa, ob, oc, oy, ox};
+  Carve ws{static_cast<char*>(workspace)};
+  const FillLayout l = fill_layout(ws, N, H, W);
+  known_kernel<<<dim3(nblk, N), kFillThreads, 0, s>>>(in, unk, B, C, H, W, l);
   if (int st = after_launch()) return st;
   dist2_column_kernel<<<dim3((W + kSiteColThreads - 1) / kSiteColThreads, N), kSiteColThreads, 0, s>>>(
       KnownSites{l.known, hw, W}, H, W, l.map);
   if (int st = after_launch()) return st;
-  dist2_row_kernel<<<dim3(H, N), 32, dist2_row_smem(W), s>>>(H, W, l.map, InitOut{in, o, C});
+  dist2_row_kernel<<<dim3(H, N), 32, dist2_row_smem(W), s>>>(H, W, l.map, InitOut{in, o, B, C});
   if (int st = after_launch()) return st;
   list_offsets_kernel<<<N, kFillThreads, 0, s>>>(nblk, l);
   if (int st = after_launch()) return st;
@@ -481,9 +416,9 @@ int rnc_harmonic_fill(const float* values, long long va, long long vb, long long
   // a fixed grid row per image, wide enough for a full-frame hole's half and for the whole GPU when there are few images
   const int row = max(1, min((kSorRowCtas + N - 1) / N, (hw / 2 + kFillThreads) / kFillThreads));
   for (int k = 0; k < sweeps; ++k) {
-    sor_kernel<0><<<dim3(row, N), kFillThreads, 0, s>>>(o, C, H, W, l);
+    sor_kernel<0><<<dim3(row, N), kFillThreads, 0, s>>>(o, B, C, H, W, l);
     if (int st = after_launch()) return st;
-    sor_kernel<1><<<dim3(row, N), kFillThreads, 0, s>>>(o, C, H, W, l);
+    sor_kernel<1><<<dim3(row, N), kFillThreads, 0, s>>>(o, B, C, H, W, l);
     if (int st = after_launch()) return st;
   }
   return RNC_OK;
@@ -500,15 +435,15 @@ int rnc_inpaint_propagate(const float* frames, long long iv, long long it, long 
   if (!frames || !masks || !flow || !flow_bw || !occ || !occ_bw || !out || !source) return RNC_ERR_BAD_POINTER;
   if (!aligned(frames, 4) || !aligned(flow, 4) || !aligned(flow_bw, 4) || !aligned(out, 4)) return RNC_ERR_BAD_POINTER;
   const PropArgs a{frames, iv, it, ic, iy, ix, masks, mv, mt, my, mx,
-                   {{flow, fk, fc, fy, fx}, {flow_bw, gk, gc, gy, gx}}, {fv, gv},
-                   {{occ, ok, 0, oy, ox}, {occ_bw, pk, 0, py, px}}, {ov, pv},
+                   {{flow, fv, fk, fc, fy, fx}, {flow_bw, gv, gk, gc, gy, gx}},
+                   {{occ, ov, ok, 0, oy, ox}, {occ_bw, pv, pk, 0, py, px}},
                    out, source, T, H, W, max_distance};
   propagate_kernel<<<dim3((H * W + kPropThreads - 1) / kPropThreads, T, V), kPropThreads, 0, as_stream(stream)>>>(a);
   return after_launch();
 }
 
 size_t rnc_ssim_partials_workspace_bytes(int N, int H, int W) {
-  return ssim_shape_ok(N, H, W) ? static_cast<size_t>(N) * eval_blocks(H, W) * sizeof(SsimPart) : 0;
+  return ssim_shape_ok(N, H, W) ? static_cast<size_t>(N) * eval_blocks(H, W) * sizeof(SumCount) : 0;
 }
 
 int rnc_ssim_partials(const float* pred, long long pn, long long pc, long long py, long long px, const float* gt,
@@ -521,11 +456,11 @@ int rnc_ssim_partials(const float* pred, long long pn, long long pc, long long p
   if (workspace_bytes < rnc_ssim_partials_workspace_bytes(N, H, W)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
   const int nblk = eval_blocks(H, W);
-  SsimPart* parts = static_cast<SsimPart*>(workspace);
+  SumCount* parts = static_cast<SumCount*>(workspace);
   cta_partials_kernel<<<dim3(nblk, N), kEvalThreads, 0, s>>>(SsimPixel{{pred, pn, pc, py, px}, {gt, gn, gc, gy, gx}, H, W},
                                                             H, W, parts);
   if (int st = after_launch()) return st;
-  return launch_image_reduce(parts, N, nblk, 1, SsimStore{sum, count}, s);
+  return launch_image_reduce(parts, N, nblk, 1, SumCountStore{sum, count}, s);
 }
 
 }  // extern "C"

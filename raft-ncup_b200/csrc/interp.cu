@@ -65,7 +65,7 @@ __global__ void __launch_bounds__(kInterpThreads) interp_splat_kernel(InterpArgs
     const float tt = s == 0 ? a.t[k] : __fsub_rn(1.0f, a.t[k]);     // frame 1 travels 1 - t along G
     const float qx = rintf(__fadd_rn(static_cast<float>(x), __fmul_rn(tt, fu)));
     const float qy = rintf(__fadd_rn(static_cast<float>(y), __fmul_rn(tt, fv)));
-    if (qx >= 0.0f && qx <= static_cast<float>(W - 1) && qy >= 0.0f && qy <= static_cast<float>(H - 1))
+    if (inside(qx, qy, H, W))
       atomicMin(map + static_cast<int>(qy) * W + static_cast<int>(qx), key);
   }
 }
@@ -107,12 +107,9 @@ __global__ void __launch_bounds__(kInterpThreads) interp_composite_kernel(Interp
   const float t = a.t[k], omt = __fsub_rn(1.0f, t);
   const float x0 = __fsub_rn(static_cast<float>(x), __fmul_rn(t, uu)), y0 = __fsub_rn(static_cast<float>(y), __fmul_rn(t, uv));
   const float x1 = __fadd_rn(static_cast<float>(x), __fmul_rn(omt, uu)), y1 = __fadd_rn(static_cast<float>(y), __fmul_rn(omt, uv));
-  const float wm = static_cast<float>(W - 1), hm = static_cast<float>(H - 1);
   const long long ob = static_cast<long long>(b) * hw;
-  const bool v0 = x0 >= 0.0f && x0 <= wm && y0 >= 0.0f && y0 <= hm &&
-                  a.occ[0][ob + static_cast<int>(rintf(y0)) * W + static_cast<int>(rintf(x0))] == 0;
-  const bool v1 = x1 >= 0.0f && x1 <= wm && y1 >= 0.0f && y1 <= hm &&
-                  a.occ[1][ob + static_cast<int>(rintf(y1)) * W + static_cast<int>(rintf(x1))] == 0;
+  const bool v0 = inside(x0, y0, H, W) && a.occ[0][ob + static_cast<int>(rintf(y0)) * W + static_cast<int>(rintf(x0))] == 0;
+  const bool v1 = inside(x1, y1, H, W) && a.occ[1][ob + static_cast<int>(rintf(y1)) * W + static_cast<int>(rintf(x1))] == 0;
   float* out = a.out + img * 3 + p;
 #pragma unroll
   for (int c = 0; c < 3; ++c) {

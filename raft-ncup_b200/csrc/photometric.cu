@@ -176,38 +176,13 @@ __global__ void __launch_bounds__(kTileThreads) census_bwd_kernel(CensusBwdArgs 
   out[hw] = g * a.st.dwy[row + o];
 }
 
-struct CensusPart {                   // a set of pixels' sum of v l and count of v; 16 bytes
-  double s;
-  unsigned m, pad;
-  __device__ __forceinline__ CensusPart& operator+=(const CensusPart& o) {
-    s += o.s;
-    m += o.m;
-    return *this;
-  }
-};
-
-__device__ __forceinline__ CensusPart warp_sum(CensusPart v) {
-  v.s = rnc::warp_sum(v.s);
-  v.m = __reduce_add_sync(0xffffffffu, v.m);
-  return v;
-}
-
-struct CensusPixel {
+struct CensusPixel {                  // a set of pixels' sum of v l and count of v
   const float* loss;
   const unsigned char* mask;
   int H, W;
-  __device__ void operator()(CensusPart& acc, int n, int y, int x) const {
-    acc.s += static_cast<double>(loss[(static_cast<long long>(n) * H + y) * W + x]);
-    acc.m += weighted(mask, n, y, x, H, W);
-  }
-};
-
-struct CensusStore {                  // row n -> S[n], M[n]
-  double* s;
-  long long* m;
-  __device__ void operator()(int n, const CensusPart& v) const {
-    s[n] = v.s;
-    m[n] = v.m;
+  __device__ void operator()(SumCount& acc, int n, int y, int x) const {
+    acc.sum += static_cast<double>(loss[(static_cast<long long>(n) * H + y) * W + x]);
+    acc.n += weighted(mask, n, y, x, H, W);
   }
 };
 
@@ -328,9 +303,17 @@ bool photometric_shape_ok(int N, int H, int W) {
   return eval_shape_ok(N, H, W) && H >= 8 && W >= 8 && (H + kTileY - 1) / kTileY <= 65535;
 }
 
-size_t round16(size_t n) { return (n + 15) & ~static_cast<size_t>(15); }
+struct CensusLayout {                 // the workspace
+  float* loss;                        // [N][H][W]: each pixel's v l
+  SumCount* parts;                    // [N][eval_blocks]
+};
 
-size_t loss_buffer_bytes(int N, int H, int W) { return round16(static_cast<size_t>(N) * H * W * sizeof(float)); }
+CensusLayout census_layout(Carve& ws, int N, int H, int W) {
+  CensusLayout l;
+  l.loss = ws.take<float>(static_cast<size_t>(N) * H * W);
+  l.parts = ws.take<SumCount>(static_cast<size_t>(N) * eval_blocks(H, W));
+  return l;
+}
 
 }  // namespace
 }  // namespace rnc
@@ -340,9 +323,10 @@ using namespace rnc;
 extern "C" {
 
 size_t rnc_census_loss_workspace_bytes(int N, int H, int W) {
-  return photometric_shape_ok(N, H, W)
-             ? loss_buffer_bytes(N, H, W) + static_cast<size_t>(N) * eval_blocks(H, W) * sizeof(CensusPart)
-             : 0;
+  if (!photometric_shape_ok(N, H, W)) return 0;
+  Carve ws{nullptr};
+  census_layout(ws, N, H, W);
+  return ws.bytes;
 }
 
 int rnc_census_loss_fwd(const float* image1, long long ab, long long ac, long long ay, long long ax, const float* image2,
@@ -361,15 +345,15 @@ int rnc_census_loss_fwd(const float* image1, long long ab, long long ac, long lo
   census_warp_kernel<<<dim3(static_cast<unsigned>((hw + kWarpThreads - 1) / kWarpThreads), N), kWarpThreads, 0, s>>>(
       WarpArgs{{image1, ab, ac, ay, ax}, {image2, bb, bc, by, bx}, {flow, fb, fc, fy, fx}, State(state, N * hw), H, W});
   if (int st = after_launch()) return st;
-  float* loss = static_cast<float*>(workspace);
+  Carve ws{static_cast<char*>(workspace)};
+  const CensusLayout l = census_layout(ws, N, H, W);
   census_fwd_kernel<<<dim3((W + kTileX - 1) / kTileX, (H + kTileY - 1) / kTileY, N), kTileThreads, 0, s>>>(
-      CensusArgs{State(state, N * hw), mask, loss, H, W});
+      CensusArgs{State(state, N * hw), mask, l.loss, H, W});
   if (int st = after_launch()) return st;
   const int nblk = eval_blocks(H, W);
-  auto* parts = reinterpret_cast<CensusPart*>(static_cast<char*>(workspace) + loss_buffer_bytes(N, H, W));
-  cta_partials_kernel<<<dim3(nblk, N), kEvalThreads, 0, s>>>(CensusPixel{loss, mask, H, W}, H, W, parts);
+  cta_partials_kernel<<<dim3(nblk, N), kEvalThreads, 0, s>>>(CensusPixel{l.loss, mask, H, W}, H, W, l.parts);
   if (int st = after_launch()) return st;
-  if (int st = launch_image_reduce(parts, N, nblk, 1, CensusStore{loss_sum, count}, s)) return st;
+  if (int st = launch_image_reduce(l.parts, N, nblk, 1, SumCountStore{loss_sum, count}, s)) return st;
   row_totals_kernel<<<1, 1, 0, s>>>(loss_sum, count, N, total);
   return after_launch();
 }

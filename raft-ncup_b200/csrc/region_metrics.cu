@@ -36,11 +36,6 @@ struct BoundarySites {
   }
 };
 
-struct Dist2Out {                       // the squared distance to the nearest boundary pixel
-  static constexpr int none = kNone;
-  __device__ int operator()(int, int x, int q, int, int fq) const { return fq - q * q + (x - q) * (x - q); }
-};
-
 constexpr int kMaxCells = RNC_REGION_CELLS_SINTEL;
 
 struct RegionArgs {
@@ -135,7 +130,7 @@ int rnc_boundary_dist2(const float* occ, long long ob, long long oy, long long o
   dist2_column_kernel<<<dim3((W + kSiteColThreads - 1) / kSiteColThreads, B), kSiteColThreads, 0, s>>>(
       BoundarySites{occ, ob, oy, ox, H, W}, H, W, d2);
   if (int st = after_launch()) return st;
-  dist2_row_kernel<<<dim3(H, B), 32, dist2_row_smem(W), s>>>(H, W, d2, Dist2Out{});
+  dist2_row_kernel<<<dim3(H, B), 32, dist2_row_smem(W), s>>>(H, W, d2, Dist2<kNone>{});
   return after_launch();
 }
 

@@ -44,6 +44,20 @@ inline int after_launch(int n = 1) {
 
 inline cudaStream_t as_stream(void* s) { return reinterpret_cast<cudaStream_t>(s); }
 
+// Carves a workspace into buffers, in the order take() is called, each starting on a 16-byte boundary.  On a null base it
+// only counts: a layout function run once on nullptr gives the workspace's size in `bytes` and run on the real base gives its
+// pointers, so the two cannot disagree.
+struct Carve {
+  char* base;
+  size_t bytes = 0;
+  template <typename T>
+  T* take(size_t n) {
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += (n * sizeof(T) + 15) & ~size_t(15);
+    return p;
+  }
+};
+
 // Programmatic dependent launch (PDL).  A kernel launched with launch_pdl() may start while its predecessor in the stream is
 // still draining: it runs its prologue (barrier init, descriptor prefetch), then pdl_wait() blocks until the
 // predecessor has completed and its writes are visible.  pdl_trigger() in the predecessor lets the dependent start early;

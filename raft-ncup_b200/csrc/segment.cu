@@ -3,7 +3,7 @@
 //
 // rnc_propagate_labels, one step k -> k+1 for V videos, in three launches and no host synchronisation:
 //   1. vote_kernel, a thread per pixel p of frame k+1: u = G_k(p) at the pixel itself and p' = p + u.  A pixel with a finite u,
-//      occ_bw_k(p) == 0 and p' in the frame is matched and writes the bilinear vote of L_k at p' (bilinear.cuh's taps and
+//      occ_bw_k(p) == 0 and p' in the frame is matched (bilinear.cuh's follow) and writes the bilinear vote of L_k at p' (bilinear.cuh's taps and
 //      weights; per distinct label the weights of its taps added in tap order; the largest sum wins, ties to the smaller
 //      label).  Any other pixel writes kUnmatched (255, never a label), so the output is also the site map of the fill.
 //   2. dist_transform.cuh's column pass, with the matched pixels as sites, into the int workspace.
@@ -45,12 +45,11 @@ __global__ void __launch_bounds__(kVoteThreads) vote_kernel(PropagateArgs a) {
   const int p = blockIdx.x * kVoteThreads + threadIdx.x;
   if (p >= H * W) return;
   const int y = p / W, x = p - y * W;
-  const float ux = a.flow.at(v, 0, y, x), uy = a.flow.at(v, 1, y, x);
-  const float px = __fadd_rn(static_cast<float>(x), ux), py = __fadd_rn(static_cast<float>(y), uy);
+  float px, py;
   unsigned char label = kUnmatched;
-  if (finite(ux) && finite(uy) && a.occ.at(v, y, x) == 0 && px >= 0.0f && px <= static_cast<float>(W - 1) && py >= 0.0f &&
-      py <= static_cast<float>(H - 1)) {
+  if (follow(a.flow, a.occ, v, y, x, H, W, px, py)) {
     const BilinearTaps t = bilinear_taps(px, py, H, W);
+    const float w[4] = {t.w(0), t.w(1), t.w(2), t.w(3)};
     unsigned char l[4];
 #pragma unroll
     for (int i = 0; i < 4; ++i) l[i] = a.labels.at(v, t.y[i >> 1], t.x[i & 1]);
@@ -60,9 +59,9 @@ __global__ void __launch_bounds__(kVoteThreads) vote_kernel(PropagateArgs a) {
       bool first = true;                // tap i is its label's first tap: the label's sum starts here
 #pragma unroll
       for (int j = 0; j < i; ++j) first = first && l[j] != l[i];
-      float s = t.w[i];
+      float s = w[i];
 #pragma unroll
-      for (int j = i + 1; j < 4; ++j) s = l[j] == l[i] ? __fadd_rn(s, t.w[j]) : s;
+      for (int j = i + 1; j < 4; ++j) s = l[j] == l[i] ? __fadd_rn(s, w[j]) : s;
       if (first && (s > best || (s == best && l[i] < label))) {
         best = s;
         label = l[i];
@@ -116,25 +115,7 @@ struct BoundarySites {                  // seg2bmap at full resolution
   }
 };
 
-struct Dist2Out {                       // the squared distance to the nearest boundary pixel
-  static constexpr int none = RNC_DIST2_NONE;
-  __device__ int operator()(int, int x, int q, int, int fq) const { return fq - q * q + (x - q) * (x - q); }
-};
-
-struct SegPart {                        // the counts of RNC_SEGMENT_COUNTS over a set of pixels
-  unsigned n[kSegCounts];
-  __device__ __forceinline__ SegPart& operator+=(const SegPart& o) {
-#pragma unroll
-    for (int c = 0; c < kSegCounts; ++c) n[c] += o.n[c];
-    return *this;
-  }
-};
-
-__device__ __forceinline__ SegPart warp_sum(SegPart v) {
-#pragma unroll
-  for (int c = 0; c < kSegCounts; ++c) v.n[c] = __reduce_add_sync(0xffffffffu, v.n[c]);
-  return v;
-}
+using SegPart = Counts<kSegCounts>;     // the counts of RNC_SEGMENT_COUNTS over a set of pixels
 
 struct SegPixelCounts {                 // cta_partials_kernel's pixel (i, y, x): object o of frame n at (y, x)
   SegMasks m;
@@ -152,14 +133,6 @@ struct SegPixelCounts {                 // cta_partials_kernel's pixel (i, y, x)
     acc.n[3] += dgt == 0;
     acc.n[4] += dfg == 0 && dgt <= r2;
     acc.n[5] += dgt == 0 && dfg <= r2;
-  }
-};
-
-struct SegStore {                       // (frame, object) i -> counts [i][RNC_SEGMENT_COUNTS]
-  long long* counts;
-  __device__ void operator()(int i, const SegPart& p) const {
-#pragma unroll
-    for (int c = 0; c < kSegCounts; ++c) counts[static_cast<long long>(i) * kSegCounts + c] = p.n[c];
   }
 };
 
@@ -225,7 +198,7 @@ int rnc_segmentation_counts(const unsigned char* pred, long long pn, long long p
   dist2_column_kernel<<<dim3((W + kSiteColThreads - 1) / kSiteColThreads, 2 * nk), kSiteColThreads, 0, s>>>(
       BoundarySites{m, nk}, H, W, d2);
   if (int st = after_launch()) return st;
-  dist2_row_kernel<<<dim3(H, 2 * nk), 32, dist2_row_smem(W), s>>>(H, W, d2, Dist2Out{});
+  dist2_row_kernel<<<dim3(H, 2 * nk), 32, dist2_row_smem(W), s>>>(H, W, d2, Dist2<RNC_DIST2_NONE>{});
   if (int st = after_launch()) return st;
   // DAVIS's tolerance: ceil(0.008 * the frame diagonal), the diagonal as numpy's norm computes it
   const int r = static_cast<int>(std::ceil(0.008 * std::sqrt(static_cast<double>(H) * H + static_cast<double>(W) * W)));
@@ -234,7 +207,7 @@ int rnc_segmentation_counts(const unsigned char* pred, long long pn, long long p
   cta_partials_kernel<<<dim3(nblk, nk), kEvalThreads, 0, s>>>(
       SegPixelCounts{m, d2, static_cast<long long>(nk) * H * W, r * r}, H, W, parts);
   if (int st = after_launch()) return st;
-  return launch_image_reduce(parts, nk, nblk, 1, SegStore{counts}, s);
+  return launch_image_reduce(parts, nk, nblk, 1, CountsStore<kSegCounts>{counts}, s);
 }
 
 }  // extern "C"

@@ -24,6 +24,7 @@
 #include <cmath>
 
 #include "bilinear.cuh"
+#include "homography.cuh"
 
 namespace rnc {
 namespace {
@@ -38,13 +39,6 @@ constexpr double kPivotMin = 1e-12;
 constexpr double kCollinear = 1e-9;
 constexpr double kShrink = 1.0 - 1.0 / 68719476736.0;   // 1 - 2^-36: the crop's margin against rounding
 constexpr int kOk = RNC_HOMOGRAPHY_OK, kFew = RNC_HOMOGRAPHY_FEW;
-
-__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
-
-__host__ __device__ __forceinline__ size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
 
 // grid points along a side of n pixels at stride s: s/2, s/2 + s, ... < n
 __host__ __device__ __forceinline__ int grid_side(int n, int s) { return s / 2 < n ? (n - 1 - s / 2) / s + 1 : 0; }
@@ -76,32 +70,17 @@ FitDims fit_dims(int N, int H, int W, int stride, int K, double tau) {
   return d;
 }
 
-size_t fit_bytes(const FitDims& d) {
+FitLayout fit_layout(Carve& ws, const FitDims& d) {
   const size_t N = d.N, G = d.G, nch = d.nch, K = d.K;
-  return align16(N * G * 4 * sizeof(double)) + align16(N * nch * kSums * sizeof(double)) +
-         align16(N * K * 8 * sizeof(double)) + align16(N * 8 * sizeof(double)) + align16(N * K * sizeof(int)) +
-         align16(N * nch * sizeof(int)) + 2 * align16(N * sizeof(int));
-}
-
-FitLayout fit_layout(void* ws, const FitDims& d) {
-  const size_t N = d.N, G = d.G, nch = d.nch, K = d.K;
-  char* p = static_cast<char*>(ws);
   FitLayout l;
-  l.L = reinterpret_cast<double*>(p);
-  p += align16(N * G * 4 * sizeof(double));
-  l.chunk = reinterpret_cast<double*>(p);
-  p += align16(N * nch * kSums * sizeof(double));
-  l.hyp = reinterpret_cast<double*>(p);
-  p += align16(N * K * 8 * sizeof(double));
-  l.cur = reinterpret_cast<double*>(p);
-  p += align16(N * 8 * sizeof(double));
-  l.hcount = reinterpret_cast<int*>(p);
-  p += align16(N * K * sizeof(int));
-  l.bcount = reinterpret_cast<int*>(p);
-  p += align16(N * nch * sizeof(int));
-  l.npts = reinterpret_cast<int*>(p);
-  p += align16(N * sizeof(int));
-  l.status = reinterpret_cast<int*>(p);
+  l.L = ws.take<double>(N * G * 4);
+  l.chunk = ws.take<double>(N * nch * kSums);
+  l.hyp = ws.take<double>(N * K * 8);
+  l.cur = ws.take<double>(N * 8);
+  l.hcount = ws.take<int>(N * K);
+  l.bcount = ws.take<int>(N * nch);
+  l.npts = ws.take<int>(N);
+  l.status = ws.take<int>(N);
   return l;
 }
 
@@ -429,10 +408,6 @@ bool fit_args_ok(int N, int H, int W, int stride, int K, double tau, int refine)
 
 // ------------------------------------------------------------------------------------------------------------ path
 
-struct M3 {
-  double m[9];
-};
-
 // (X Y) with each entry ((x_i0 y_0j) + (x_i1 y_1j)) + x_i2 y_2j, then every entry divided by the product's [2][2]
 __device__ __forceinline__ M3 mul_norm(const M3& X, const M3& Y) {
   M3 P;
@@ -445,27 +420,6 @@ __device__ __forceinline__ M3 mul_norm(const M3& X, const M3& Y) {
 #pragma unroll
   for (int k = 0; k < 9; ++k) P.m[k] = ddiv(P.m[k], z);
   return P;
-}
-
-__device__ __forceinline__ double det2(double a, double b, double c, double d) { return dsub(dmul(a, b), dmul(c, d)); }
-
-// the adjugate, divided by its [2][2]
-__device__ __forceinline__ M3 inv_norm(const M3& A) {
-  const double* a = A.m;
-  M3 C;
-  C.m[0] = det2(a[4], a[8], a[5], a[7]);
-  C.m[1] = det2(a[2], a[7], a[1], a[8]);
-  C.m[2] = det2(a[1], a[5], a[2], a[4]);
-  C.m[3] = det2(a[5], a[6], a[3], a[8]);
-  C.m[4] = det2(a[0], a[8], a[2], a[6]);
-  C.m[5] = det2(a[2], a[3], a[0], a[5]);
-  C.m[6] = det2(a[3], a[7], a[4], a[6]);
-  C.m[7] = det2(a[1], a[6], a[0], a[7]);
-  C.m[8] = det2(a[0], a[4], a[1], a[3]);
-  const double z = C.m[8];
-#pragma unroll
-  for (int k = 0; k < 9; ++k) C.m[k] = ddiv(C.m[k], z);
-  return C;
 }
 
 __device__ __forceinline__ M3 load3(const double* p) {
@@ -541,14 +495,14 @@ __global__ void __launch_bounds__(kPathThreads) path_kernel(PathArgs p) {
     }
     P = I;
     for (int j = 1; j <= jm; ++j) {           // T_t^{t-j} = A_{t-j}^-1 T_t^{t-j+1}
-      P = mul_norm(inv_norm(load3(A + (t - j) * 9)), P);
+      P = mul_norm(inv_norm(A + (t - j) * 9), P);
       accumulate(num, p.taps[j], P);
     }
     const double z = num.m[8];
 #pragma unroll
     for (int k = 0; k < 9; ++k) num.m[k] = ddiv(num.m[k], z);
     store3(M + t * 9, num);
-    amin = fmin(amin, crop_alpha(inv_norm(num), p.H, p.W));
+    amin = fmin(amin, crop_alpha(inv_norm(num.m), p.H, p.W));
   }
   for (int o = 16; o > 0; o >>= 1) amin = fmin(amin, __shfl_down_sync(0xffffffffu, amin, o));
   if ((threadIdx.x & 31) == 0) mins[threadIdx.x >> 5] = amin;
@@ -563,7 +517,7 @@ __global__ void __launch_bounds__(kPathThreads) path_kernel(PathArgs p) {
     M3 S = load3(M + t * 9);
     if (p.crop) S = mul_norm(Z, S);
     store3(M + t * 9, S);
-    store3(Minv + t * 9, inv_norm(S));
+    store3(Minv + t * 9, inv_norm(S.m));
   }
 }
 
@@ -571,32 +525,20 @@ bool taps_radius_ok(int radius) { return radius >= 0 && radius <= 1024; }
 
 // ------------------------------------------------------------------------------------------------------------ warp
 
-struct OutView {                              // [N][C][H][W] through element strides
-  float* p;
-  long long n, c, y, x;
-};
-
-struct ValidView {                            // [N][H][W] through element strides
-  unsigned char* p;
-  long long n, y, x;
-};
-
 __global__ void __launch_bounds__(kWarpThreads) warp_kernel(View frames, const double* __restrict__ maps, int C, int H, int W,
-                                                           OutView out, ValidView valid) {
+                                                           OutView out, OutMaskView valid) {
   const int n = blockIdx.y, hw = H * W;
   const int p = blockIdx.x * kWarpThreads + threadIdx.x;
   if (p >= hw) return;
   const int y = p / W, x = p - y * W;
   const double* m = maps + n * 9;
-  const double ux = x, uy = y;
-  const double X = dadd(dadd(dmul(m[0], ux), dmul(m[1], uy)), m[2]);
-  const double Y = dadd(dadd(dmul(m[3], ux), dmul(m[4], uy)), m[5]);
-  const double w = dadd(dadd(dmul(m[6], ux), dmul(m[7], uy)), m[8]);
-  const float qx = __double2float_rn(ddiv(X, w)), qy = __double2float_rn(ddiv(Y, w));
-  const bool ok = w > 0.0 && qx >= 0.0f && qx <= static_cast<float>(W - 1) && qy >= 0.0f && qy <= static_cast<float>(H - 1);
+  double X, Y;
+  const bool wq = project(m, x, y, X, Y);
+  const float qx = __double2float_rn(X), qy = __double2float_rn(Y);
+  const bool ok = wq && inside(qx, qy, H, W);
   for (int c = 0; c < C; ++c)
-    out.p[n * out.n + c * out.c + y * out.y + x * out.x] = ok ? sample(frames, n, c, qx, qy, H, W) : 0.0f;
-  valid.p[n * valid.n + y * valid.y + x * valid.x] = ok;
+    out.p[n * out.b + c * out.c + y * out.y + x * out.x] = ok ? sample(frames, n, c, qx, qy, H, W) : 0.0f;
+  valid.p[n * valid.b + y * valid.y + x * valid.x] = ok;
 }
 
 bool warp_shape_ok(int N, int C, int H, int W) {
@@ -612,7 +554,9 @@ extern "C" {
 
 size_t rnc_homography_fit_workspace_bytes(int N, int H, int W, int stride, int hypotheses) {
   if (!fit_args_ok(N, H, W, stride, hypotheses, 1.0, 1)) return 0;
-  return fit_bytes(fit_dims(N, H, W, stride, hypotheses, 1.0));
+  Carve ws{nullptr};
+  fit_layout(ws, fit_dims(N, H, W, stride, hypotheses, 1.0));
+  return ws.bytes;
 }
 
 int rnc_homography_fit(const float* flow, long long fn, long long fc, long long fy, long long fx, int N, int H, int W,
@@ -624,9 +568,10 @@ int rnc_homography_fit(const float* flow, long long fn, long long fc, long long 
       !aligned(workspace, 16))
     return RNC_ERR_BAD_POINTER;
   const FitDims d = fit_dims(N, H, W, stride, hypotheses, tau);
-  if (workspace_bytes < fit_bytes(d)) return RNC_ERR_WORKSPACE;
+  if (workspace_bytes < rnc_homography_fit_workspace_bytes(N, H, W, stride, hypotheses)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
-  const FitLayout l = fit_layout(workspace, d);
+  Carve ws{static_cast<char*>(workspace)};
+  const FitLayout l = fit_layout(ws, d);
   const View f{flow, fn, fc, fy, fx};
   const int nb = d.nch > 0 ? d.nch : 1;
   count_kernel<<<dim3(nb, N), kPts, 0, s>>>(f, d, l);
@@ -670,7 +615,7 @@ int rnc_stabilize_warp(const float* frames, long long in, long long ic, long lon
   if (!frames || !maps || !out || !valid) return RNC_ERR_BAD_POINTER;
   if (!aligned(frames, 4) || !aligned(maps, 8) || !aligned(out, 4)) return RNC_ERR_BAD_POINTER;
   warp_kernel<<<dim3((H * W + kWarpThreads - 1) / kWarpThreads, N), kWarpThreads, 0, as_stream(stream)>>>(
-      View{frames, in, ic, iy, ix}, maps, C, H, W, OutView{out, on, oc, oy, ox}, ValidView{valid, vn, vy, vx});
+      View{frames, in, ic, iy, ix}, maps, C, H, W, OutView{out, on, oc, oy, ox}, OutMaskView{valid, vn, 0, vy, vx});
   return after_launch();
 }
 

@@ -15,6 +15,7 @@
 #include <cmath>
 
 #include "bilinear.cuh"
+#include "homography.cuh"
 
 namespace rnc {
 namespace {
@@ -22,44 +23,8 @@ namespace {
 constexpr int kFillThreads = 256;
 constexpr int kMaxSide = 4096;
 
-__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
-__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
-__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
-__device__ __forceinline__ double ddiv(double a, double b) { return __ddiv_rn(a, b); }
-
-// pi(m p): false when w <= 0 (or NaN)
-__device__ __forceinline__ bool project(const double* m, double x, double y, double& ox, double& oy) {
-  const double X = dadd(dadd(dmul(m[0], x), dmul(m[1], y)), m[2]);
-  const double Y = dadd(dadd(dmul(m[3], x), dmul(m[4], y)), m[5]);
-  const double w = dadd(dadd(dmul(m[6], x), dmul(m[7], y)), m[8]);
-  ox = ddiv(X, w);
-  oy = ddiv(Y, w);
-  return w > 0.0;
-}
-
-// the adjugate of a, divided by its [2][2]
-__device__ __forceinline__ void inv_norm(const double* a, double* c) {
-  c[0] = dsub(dmul(a[4], a[8]), dmul(a[5], a[7]));
-  c[1] = dsub(dmul(a[2], a[7]), dmul(a[1], a[8]));
-  c[2] = dsub(dmul(a[1], a[5]), dmul(a[2], a[4]));
-  c[3] = dsub(dmul(a[5], a[6]), dmul(a[3], a[8]));
-  c[4] = dsub(dmul(a[0], a[8]), dmul(a[2], a[6]));
-  c[5] = dsub(dmul(a[2], a[3]), dmul(a[0], a[5]));
-  c[6] = dsub(dmul(a[3], a[7]), dmul(a[4], a[6]));
-  c[7] = dsub(dmul(a[1], a[6]), dmul(a[0], a[7]));
-  c[8] = dsub(dmul(a[0], a[4]), dmul(a[1], a[3]));
-  const double z = c[8];
-#pragma unroll
-  for (int k = 0; k < 9; ++k) c[k] = ddiv(c[k], z);
-}
-
-struct FlowView {                             // [V][T-1][2][H][W] through element strides
-  const float* p;
-  long long v, k, c, y, x;
-};
-
 struct FillArgs {
-  FlowView fw, bw;                            // transfer: the flows F, G; re-add: unused
+  Video fw, bw;                               // [V][T-1][2][H][W], b the pair: transfer: the flows F, G; re-add: unused
   const double* motion;                       // [V][T-1][9]
   const double* maps;                         // [V][T][9], input -> output
   const double* maps_inv;                     // [V][T][9], output -> input
@@ -71,7 +36,7 @@ struct FillArgs {
 // one direction at output pixel (x, y): src = the output -> input map of the output frame, dst = the input -> output map of
 // the other frame, A = the motion from this frame's input to the other's.  Writes the two channels of the result.
 template <bool kReadd>
-__device__ __forceinline__ void direction(const double* src, const double* dst, const double* A, const FlowView& f, int v, int k,
+__device__ __forceinline__ void direction(const double* src, const double* dst, const double* A, const Video& f, int v, int k,
                                           int x, int y, int H, int W, float* out, long long plane) {
   const float nan = __int_as_float(0x7fc00000);            // the host's float32 NaN, so the bits agree
   double X, Y;
@@ -85,10 +50,10 @@ __device__ __forceinline__ void direction(const double* src, const double* dst, 
     out[plane] = ok ? __double2float_rn(dadd(dsub(gy, y), static_cast<double>(ry))) : nan;
     return;
   }
-  ok = ok && qx >= 0.0f && qx <= static_cast<float>(W - 1) && qy >= 0.0f && qy <= static_cast<float>(H - 1);
+  ok = ok && inside(qx, qy, H, W);
   double ax = 0.0, ay = 0.0;
   if (ok) {
-    const View im{f.p + v * f.v + k * f.k, 0, f.c, f.y, f.x};
+    const View im{f.video(v).pixel(k, 0, 0), 0, f.c, f.y, f.x};     // pair k's two planes
     const float ux = sample(im, 0, 0, qx, qy, H, W), uy = sample(im, 0, 1, qx, qy, H, W);
     ok = finite(ux) && finite(uy) &&
          project(dst, dadd(static_cast<double>(qx), static_cast<double>(ux)),
@@ -111,9 +76,8 @@ __global__ void __launch_bounds__(kFillThreads) flow_kernel(FillArgs a) {
   const double* Mi = a.maps_inv + (static_cast<long long>(v) * a.T + k) * 9;
   const long long off = pair * 2 * hw + p;
   direction<kReadd>(Mi, M + 9, A, a.fw, v, k, x, y, a.H, a.W, a.out + off, hw);
-  double Ai[9];
-  inv_norm(A, Ai);
-  direction<kReadd>(Mi + 9, M, Ai, a.bw, v, k, x, y, a.H, a.W, a.out_bw + off, hw);
+  const M3 Ai = inv_norm(A);
+  direction<kReadd>(Mi + 9, M, Ai.m, a.bw, v, k, x, y, a.H, a.W, a.out_bw + off, hw);
 }
 
 bool fill_shape_ok(int V, int T, int H, int W) {
@@ -155,7 +119,7 @@ int rnc_stabilize_flow_readd(const double* motion, const double* maps, const dou
   if (!motion || !maps || !maps_inv || !flow || !flow_bw) return RNC_ERR_BAD_POINTER;
   if (!aligned(motion, 8) || !aligned(maps, 8) || !aligned(maps_inv, 8) || !aligned(flow, 4) || !aligned(flow_bw, 4))
     return RNC_ERR_BAD_POINTER;
-  const FillArgs a{{nullptr, 0, 0, 0, 0, 0}, {nullptr, 0, 0, 0, 0, 0}, motion, maps, maps_inv, flow, flow_bw, T, H, W};
+  const FillArgs a{{}, {}, motion, maps, maps_inv, flow, flow_bw, T, H, W};
   return launch(a, V, true, stream);
 }
 

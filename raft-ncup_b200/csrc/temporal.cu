@@ -3,8 +3,8 @@
 // (Lai et al. 2018).
 //
 // rnc_temporal_step, V videos of C channels, in 5 + 2 * sweeps launches:
-//   1. target_kernel, a thread per pixel p of frame k+1: p is matched when u = G_k(p) is finite, occ_bw_k(p) == 0 and
-//      p' = p + u lies in the frame.  A matched pixel samples T = O_k(p') and J = I_k(p') (bilinear.cuh's sample) and weighs
+//   1. target_kernel, a thread per pixel p of frame k+1: p is matched (bilinear.cuh's follow) when u = G_k(p) is finite,
+//      occ_bw_k(p) == 0 and p' = p + u lies in the frame.  A matched pixel samples T = O_k(p') and J = I_k(p') (bilinear.cuh's sample) and weighs
 //      w = lam / (1 + alpha d2), d2 the squared colour distance of I_{k+1}(p) and J over 255; an unmatched one weighs 0.  It
 //      writes D = 0, r = w (T - P) (0 where w is 0), den = n + w (n the in-frame 4-neighbours) and weak = w < lam / 4.
 //   2. dist_transform.cuh's column and row passes with the non-weak pixels as sites: every pixel's exact squared distance to
@@ -43,40 +43,16 @@ struct StepLayout {                           // the workspace
   unsigned char* weak;                        // [V][H][W]
 };
 
-__host__ __device__ __forceinline__ size_t align16(size_t n) { return (n + 15) & ~size_t(15); }
-
-StepLayout step_layout(void* ws, int V, int C, int H, int W) {
+StepLayout step_layout(Carve& ws, int V, int C, int H, int W) {
   const size_t px = static_cast<size_t>(V) * H * W;
-  char* p = static_cast<char*>(ws);
   StepLayout l;
-  l.D = reinterpret_cast<float*>(p);
-  p += align16(px * C * sizeof(float));
-  l.r = reinterpret_cast<float*>(p);
-  p += align16(px * C * sizeof(float));
-  l.den = reinterpret_cast<float*>(p);
-  p += align16(px * sizeof(float));
-  l.map = reinterpret_cast<int*>(p);
-  p += align16(px * sizeof(int));
-  l.omega = reinterpret_cast<float*>(p);
-  p += align16(static_cast<size_t>(V) * sizeof(float));
-  l.weak = reinterpret_cast<unsigned char*>(p);
+  l.D = ws.take<float>(px * C);
+  l.r = ws.take<float>(px * C);
+  l.den = ws.take<float>(px);
+  l.map = ws.take<int>(px);
+  l.omega = ws.take<float>(V);
+  l.weak = ws.take<unsigned char>(px);
   return l;
-}
-
-size_t step_bytes(int V, int C, int H, int W) {
-  const size_t px = static_cast<size_t>(V) * H * W;
-  return 2 * align16(px * C * sizeof(float)) + align16(px * sizeof(float)) + align16(px * sizeof(int)) +
-         align16(static_cast<size_t>(V) * sizeof(float)) + align16(px);
-}
-
-// p = (x, y) of frame k+1 is matched when G_k(p) is finite, occ_bw_k(p) == 0 and p' = p + G_k(p) lies in the frame
-__device__ __forceinline__ bool match(const View& flow, const MaskView& occ, int v, int y, int x, int H, int W, float& px,
-                                      float& py) {
-  const float ux = flow.at(v, 0, y, x), uy = flow.at(v, 1, y, x);
-  px = __fadd_rn(static_cast<float>(x), ux);
-  py = __fadd_rn(static_cast<float>(y), uy);
-  return finite(ux) && finite(uy) && occ.at(v, y, x) == 0 && px >= 0.0f && px <= static_cast<float>(W - 1) && py >= 0.0f &&
-         py <= static_cast<float>(H - 1);
 }
 
 struct StepArgs {
@@ -93,7 +69,7 @@ __global__ void __launch_bounds__(kStepThreads) target_kernel(StepArgs a, StepLa
   if (p >= hw) return;
   const int y = p / W, x = p - y * W;
   float px, py, w = 0.0f;
-  const bool matched = match(a.flow, a.occ, v, y, x, H, W, px, py);
+  const bool matched = follow(a.flow, a.occ, v, y, x, H, W, px, py);
   if (matched) {
     float d2 = -0.0f;
 #pragma unroll
@@ -118,11 +94,6 @@ struct StrongSites {                          // the pixels that are not weak
   const unsigned char* weak;
   int hw, W;
   __device__ bool operator()(int v, int y, int x) const { return weak[static_cast<long long>(v) * hw + y * W + x] == 0; }
-};
-
-struct WeakDist2 {                            // the squared distance to the nearest non-weak pixel; 0 in an image without one
-  static constexpr int none = 0;
-  __device__ int operator()(int, int x, int q, int, int fq) const { return fq - q * q + (x - q) * (x - q); }
 };
 
 // a CTA per image: the largest squared distance D2, L = the least integer with L^2 >= 4 D2, and omega
@@ -175,18 +146,13 @@ __global__ void __launch_bounds__(kStepThreads) sor_kernel(int C, int H, int W, 
   }
 }
 
-struct OutView {                              // [V][C][H][W] through element strides
-  float* p;
-  long long v, c, y, x;
-};
-
 __global__ void __launch_bounds__(kStepThreads) finish_kernel(View proc, OutView out, int C, int H, int W, StepLayout l) {
   const int v = blockIdx.y, hw = H * W;
   const int p = blockIdx.x * kStepThreads + threadIdx.x;
   if (p >= hw) return;
   const int y = p / W, x = p - y * W;
   for (int c = 0; c < C; ++c)
-    out.p[v * out.v + c * out.c + y * out.y + x * out.x] =
+    out.p[v * out.b + c * out.c + y * out.y + x * out.x] =
         __fadd_rn(proc.at(v, c, y, x), l.D[(static_cast<long long>(v) * C + c) * hw + p]);
 }
 
@@ -198,35 +164,16 @@ bool step_shape_ok(int V, int C, int H, int W) {
 
 // ------------------------------------------------------------------------------------------------ warping error
 
-struct WarpPart {
-  double sum;
-  unsigned n, pad;
-  __device__ __forceinline__ WarpPart& operator+=(const WarpPart& o) {
-    sum += o.sum;
-    n += o.n;
-    return *this;
-  }
-};
-
-__device__ __forceinline__ WarpPart warp_sum(WarpPart v) {
-  v.sum = rnc::warp_sum(v.sum);
-  v.n = __reduce_add_sync(0xffffffffu, v.n);
-  return v;
-}
-
 struct WarpPixel {                            // cta_partials_kernel's pixel (i, y, x): frame k+1 of video v, i = v K + k
-  View video;                                 // [V][T][C][H][W]: p, the t, c, y, x strides, and the v stride below
-  View flow;                                  // [V][K][2][H][W]
-  MaskView occ;                               // [V][K][H][W]
-  long long video_v, flow_v, occ_v;
+  Video video;                                // [V][T][C][H][W], b the frame
+  Video flow;                                 // [V][K][2][H][W], b the pair
+  VideoMask occ;                              // [V][K][H][W], b the pair
   int K, C, H, W;
-  __device__ void operator()(WarpPart& acc, int i, int y, int x) const {
+  __device__ void operator()(SumCount& acc, int i, int y, int x) const {
     const int v = i / K, k = i - v * K;
-    const View fl{flow.p + v * flow_v, flow.b, flow.c, flow.y, flow.x};
-    const MaskView oc{occ.p + v * occ_v, occ.b, 0, occ.y, occ.x};
     float px, py;
-    if (!match(fl, oc, k, y, x, H, W, px, py)) return;
-    const View vid{video.p + v * video_v, video.b, video.c, video.y, video.x};
+    if (!follow(flow.video(v), occ.video(v), k, y, x, H, W, px, py)) return;
+    const View vid = video.video(v);
     double t = 0.0;
     for (int c = 0; c < C; ++c) {
       const double e = __ddiv_rn(__dsub_rn(vid.at(k + 1, c, y, x), sample(vid, k, c, px, py, H, W)), 255.0);
@@ -234,15 +181,6 @@ struct WarpPixel {                            // cta_partials_kernel's pixel (i,
     }
     acc.sum += t;
     acc.n += 1;
-  }
-};
-
-struct WarpStore {
-  double* sum;
-  long long* count;
-  __device__ void operator()(int i, const WarpPart& p) const {
-    sum[i] = p.sum;
-    count[i] = p.n;
   }
 };
 
@@ -258,7 +196,10 @@ using namespace rnc;
 extern "C" {
 
 size_t rnc_temporal_step_workspace_bytes(int V, int C, int H, int W) {
-  return step_shape_ok(V, C, H, W) ? step_bytes(V, C, H, W) : 0;
+  if (!step_shape_ok(V, C, H, W)) return 0;
+  Carve ws{nullptr};
+  step_layout(ws, V, C, H, W);
+  return ws.bytes;
 }
 
 int rnc_temporal_step(const float* out_prev, long long av, long long ac, long long ay, long long ax, const float* processed,
@@ -277,7 +218,8 @@ int rnc_temporal_step(const float* out_prev, long long av, long long ac, long lo
   if (workspace_bytes < rnc_temporal_step_workspace_bytes(V, C, H, W)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
   const int hw = H * W, nblk = (hw + kStepThreads - 1) / kStepThreads;
-  const StepLayout l = step_layout(workspace, V, C, H, W);
+  Carve ws{static_cast<char*>(workspace)};
+  const StepLayout l = step_layout(ws, V, C, H, W);
   const StepArgs a{{out_prev, av, ac, ay, ax}, {processed, pv, pc, py, px}, {frame_prev, iv, ic, iy, ix},
                    {frame, jv, jc, jy, jx},    {flow_bw, gv, gc, gy, gx},    {occ_bw, ov, 0, oy, ox},
                    lam, alpha, C, H, W};
@@ -286,7 +228,7 @@ int rnc_temporal_step(const float* out_prev, long long av, long long ac, long lo
   dist2_column_kernel<<<dim3((W + kSiteColThreads - 1) / kSiteColThreads, V), kSiteColThreads, 0, s>>>(
       StrongSites{l.weak, hw, W}, H, W, l.map);
   if (int st = after_launch()) return st;
-  dist2_row_kernel<<<dim3(H, V), 32, dist2_row_smem(W), s>>>(H, W, l.map, WeakDist2{});
+  dist2_row_kernel<<<dim3(H, V), 32, dist2_row_smem(W), s>>>(H, W, l.map, Dist2<0>{});
   if (int st = after_launch()) return st;
   omega_kernel<<<V, kStepThreads, 0, s>>>(hw, sigma, l);
   if (int st = after_launch()) return st;
@@ -302,7 +244,7 @@ int rnc_temporal_step(const float* out_prev, long long av, long long ac, long lo
 }
 
 size_t rnc_warping_error_partials_workspace_bytes(int V, int T, int C, int H, int W) {
-  return warp_shape_ok(V, T, C, H, W) ? static_cast<size_t>(V) * (T - 1) * eval_blocks(H, W) * sizeof(WarpPart) : 0;
+  return warp_shape_ok(V, T, C, H, W) ? static_cast<size_t>(V) * (T - 1) * eval_blocks(H, W) * sizeof(SumCount) : 0;
 }
 
 int rnc_warping_error_partials(const float* video, long long vv, long long vt, long long vc, long long vy, long long vx,
@@ -317,12 +259,12 @@ int rnc_warping_error_partials(const float* video, long long vv, long long vt, l
   if (workspace_bytes < rnc_warping_error_partials_workspace_bytes(V, T, C, H, W)) return RNC_ERR_WORKSPACE;
   cudaStream_t s = as_stream(stream);
   const int K = T - 1, N = V * K, nblk = eval_blocks(H, W);
-  WarpPart* parts = static_cast<WarpPart*>(workspace);
+  SumCount* parts = static_cast<SumCount*>(workspace);
   cta_partials_kernel<<<dim3(nblk, N), kEvalThreads, 0, s>>>(
-      WarpPixel{{video, vt, vc, vy, vx}, {flow_bw, gk, gc, gy, gx}, {occ_bw, ok, 0, oy, ox}, vv, gv, ov, K, C, H, W}, H, W,
+      WarpPixel{{video, vv, vt, vc, vy, vx}, {flow_bw, gv, gk, gc, gy, gx}, {occ_bw, ov, ok, 0, oy, ox}, K, C, H, W}, H, W,
       parts);
   if (int st = after_launch()) return st;
-  return launch_image_reduce(parts, N, nblk, 1, WarpStore{sum, count}, s);
+  return launch_image_reduce(parts, N, nblk, 1, SumCountStore{sum, count}, s);
 }
 
 }  // extern "C"

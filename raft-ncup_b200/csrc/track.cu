@@ -22,18 +22,13 @@ constexpr int kThresholds = RNC_TRACK_THRESHOLDS;       // delta = 1, 2, 4, 8, 1
 constexpr int kTrackCounts = RNC_TRACK_COUNTS;
 
 struct TrackArgs {
-  View flow[2];                         // F_k (frame k -> k+1), G_k (frame k+1 -> k): b is the pair index k
-  MaskView occ[2];                      // occ_k on frame k, occ_bw_k on frame k+1: b is k
-  long long flow_v[2], occ_v[2];        // the video strides of the four
+  Video flow[2];                        // F_k (frame k -> k+1), G_k (frame k+1 -> k): b is the pair index k
+  VideoMask occ[2];                     // occ_k on frame k, occ_bw_k on frame k+1: b is k
   const float* queries;                 // [V][N][3]: (t, x, y)
   float2* tracks;                       // [V][N][T]: (x, y)
   unsigned char* visible;               // [V][N][T]
   int V, N, T, H, W;
 };
-
-__device__ __forceinline__ bool inside(float x, float y, int H, int W) {
-  return x >= 0.0f && x <= static_cast<float>(W - 1) && y >= 0.0f && y <= static_cast<float>(H - 1);
-}
 
 // One direction of the rule from the query frame tq: with Dir = +1 steps k = tq .. T-2 through F_k / occ_k, each giving frame
 // k + 1; with Dir = -1 steps k = tq-1 .. 0 through G_k / occ_bw_k, each giving frame k.  While the point is not lost its
@@ -77,32 +72,13 @@ __global__ void __launch_bounds__(kTrackThreads) track_kernel(TrackArgs a) {
   const int tq = static_cast<int>(qt);
   tr[tq] = make_float2(qx, qy);
   vis[tq] = 1;
-  View f = a.flow[0], g = a.flow[1];
-  MaskView o = a.occ[0], ob = a.occ[1];
-  f.p += v * a.flow_v[0];
-  g.p += v * a.flow_v[1];
-  o.p += v * a.occ_v[0];
-  ob.p += v * a.occ_v[1];
-  chain<1>(f, o, qx, qy, tq, T, H, W, tr, vis);
-  chain<-1>(g, ob, qx, qy, tq, T, H, W, tr, vis);
+  chain<1>(a.flow[0].video(v), a.occ[0].video(v), qx, qy, tq, T, H, W, tr, vis);
+  chain<-1>(a.flow[1].video(v), a.occ[1].video(v), qx, qy, tq, T, H, W, tr, vis);
 }
 
 // counts of a set of (point, frame) pairs, in the order of RNC_TRACK_COUNTS: evaluated, occlusion agreements, gt visible, then
 // per threshold within & gt visible, then per threshold true positives, then per threshold false positives
-struct TrackPart {
-  unsigned n[kTrackCounts];
-  __device__ __forceinline__ TrackPart& operator+=(const TrackPart& o) {
-#pragma unroll
-    for (int c = 0; c < kTrackCounts; ++c) n[c] += o.n[c];
-    return *this;
-  }
-};
-
-__device__ __forceinline__ TrackPart warp_sum(TrackPart v) {
-#pragma unroll
-  for (int c = 0; c < kTrackCounts; ++c) v.n[c] = __reduce_add_sync(0xffffffffu, v.n[c]);
-  return v;
-}
+using TrackPart = Counts<kTrackCounts>;
 
 // x * 256 / size, rounded once: the multiplication by a power of two is exact
 __device__ __forceinline__ float to_256(float x, float size) { return __fdiv_rn(__fmul_rn(x, 256.0f), size); }
@@ -137,14 +113,6 @@ struct TrackPairCounts {                // cta_partials_kernel's pixel (v, n, t)
   }
 };
 
-struct TrackStore {                     // video v -> counts [v][RNC_TRACK_COUNTS]
-  long long* counts;
-  __device__ void operator()(int v, const TrackPart& p) const {
-#pragma unroll
-    for (int c = 0; c < kTrackCounts; ++c) counts[static_cast<long long>(v) * kTrackCounts + c] = p.n[c];
-  }
-};
-
 // V videos of N points over T >= 2 frames of H x W: a grid row per video, N*T < 2^30 (pairs indexed in int), and sides whose
 // pixel coordinates are exact in float32
 bool track_shape_ok(int V, int N, int T, int H, int W) {
@@ -166,10 +134,8 @@ int rnc_track(const float* flow, long long fv, long long fk, long long fc, long 
   if (!track_shape_ok(V, N, T, H, W)) return RNC_ERR_BAD_SHAPE;
   if (!flow || !flow_bw || !occ || !occ_bw || !queries || !tracks || !visible) return RNC_ERR_BAD_POINTER;
   if (!aligned(flow, 4) || !aligned(flow_bw, 4) || !aligned(queries, 4) || !aligned(tracks, 8)) return RNC_ERR_BAD_POINTER;
-  TrackArgs a{{{flow, fk, fc, fy, fx}, {flow_bw, gk, gc, gy, gx}},
-              {{occ, ok, 0, oy, ox}, {occ_bw, pk, 0, py, px}},
-              {fv, gv},
-              {ov, pv},
+  TrackArgs a{{{flow, fv, fk, fc, fy, fx}, {flow_bw, gv, gk, gc, gy, gx}},
+              {{occ, ov, ok, 0, oy, ox}, {occ_bw, pv, pk, 0, py, px}},
               queries,
               reinterpret_cast<float2*>(tracks),
               visible,
@@ -198,7 +164,7 @@ int rnc_track_metrics(const float* tracks, const unsigned char* visible, const f
                       queries, N, T, static_cast<float>(H), static_cast<float>(W)},
       N, T, parts);
   if (int st = after_launch()) return st;
-  return launch_image_reduce(parts, V, nblk, 1, TrackStore{counts}, s);
+  return launch_image_reduce(parts, V, nblk, 1, CountsStore<kTrackCounts>{counts}, s);
 }
 
 }  // extern "C"

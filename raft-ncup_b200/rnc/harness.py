@@ -18,6 +18,8 @@ import torch
 from utils import frame_utils
 from utils.utils import InputPadder, forward_interpolate
 
+from .restate import check_sides
+
 
 def _shape_batches(samples, batch_size, regions=False):
     """Consecutive samples of one frame size, batch_size at a time; a new size (KITTI's vary) closes the batch.  With
@@ -611,7 +613,7 @@ def propagate_masks(model, sequences, first_labels, iters=32, warm_start=False, 
     size, a label outside 0..254 or a label-map count that does not match the videos.  Inference only: with grad enabled on
     a model that requires grad it raises ValueError."""
     from . import native
-    from .segment import _check_sides, _step, check_labels
+    from .segment import _step, check_labels
     if model._needs_grad():
         raise ValueError("propagate_masks is inference only: call it under torch.no_grad()")
     firsts = list(first_labels)
@@ -624,7 +626,7 @@ def propagate_masks(model, sequences, first_labels, iters=32, warm_start=False, 
             raise ValueError(f"propagate_masks: a video needs T >= 2 frames, got {len(seq)}")
         if tuple(first.shape) != tuple(seq[0].shape[-2:]):
             raise ValueError(f"propagate_masks: expected first labels {list(seq[0].shape[-2:])}, got {list(first.shape)}")
-        _check_sides(*first.shape, "propagate_masks")
+        check_sides(*first.shape, "propagate_masks")
         check_labels(first, "propagate_masks")
     out, ws = None, None
     for s, k, r in run_sequences_bidirectional(model, sequences, iters, warm_start=warm_start, batch_size=batch_size,
@@ -702,7 +704,7 @@ def inpaint_videos(model, sequences, masks, iters=32, warm_start=False, batch_si
     ValueError before the flow pass for a video of fewer than two frames, a mask of another shape, a side above 4096, a
     mask count that does not match the videos, sweeps < 0 or max_distance < 1.  Inference only: with grad enabled on a
     model that requires grad it raises ValueError."""
-    from .inpaint import _check_sides, _check_sweeps, _max_distance, _run
+    from .inpaint import _check_sweeps, _max_distance, _run
     if model._needs_grad():
         raise ValueError("inpaint_videos is inference only: call it under torch.no_grad()")
     masks = list(masks)
@@ -714,7 +716,7 @@ def inpaint_videos(model, sequences, masks, iters=32, warm_start=False, batch_si
             raise ValueError(f"inpaint_videos: a video needs T >= 2 frames, got {len(seq)}")
         if tuple(m.shape) != (len(seq), *seq[0].shape[-2:]):
             raise ValueError(f"inpaint_videos: expected masks {[len(seq), *seq[0].shape[-2:]]}, got {list(m.shape)}")
-        _check_sides(*m.shape[-2:], "inpaint_videos")
+        check_sides(*m.shape[-2:], "inpaint_videos")
         _max_distance(max_distance, len(seq), "inpaint_videos")
     by_size = {}
     for i, seq in enumerate(sequences):
@@ -784,7 +786,7 @@ def _consistent_steps(model, sequences, processed, iters, warm_start, batch_size
     """make_temporally_consistent's loop: yields (video, pair, result, outputs) after each step, outputs being the list of
     V [T_v,C,H,W] results on the device, frame pair + 1 of the video just written."""
     from . import native
-    from .temporal import _check_params, _check_sides, temporal_step
+    from .temporal import _check_params, temporal_step
     if model._needs_grad():
         raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
     procs = list(processed)
@@ -799,7 +801,7 @@ def _consistent_steps(model, sequences, processed, iters, warm_start, batch_size
                              f"{list(p.shape)}")
         if not 1 <= p.shape[1] <= native.HARMONIC_MAX_CHANNELS:
             raise ValueError(f"{what}: expected 1 to {native.HARMONIC_MAX_CHANNELS} processed channels, got {p.shape[1]}")
-        _check_sides(*p.shape[-2:], what)
+        check_sides(*p.shape[-2:], what)
     out, ws = None, {}
     for s, k, r in run_sequences_bidirectional(model, sequences, iters, warm_start=warm_start, batch_size=batch_size,
                                                mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
@@ -918,8 +920,8 @@ def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8,
     and 2 residuals x 2 channels x 4 B + 2 occlusion masks x 1 B + 2 x 4 B of consistency error while it is checked) ~ 69
     V T bytes per pixel, plus at most 1 GiB of fill workspace: e.g. 11.3 GB for eight 50-frame videos of 480x854 (17.3 GB
     peak measured on that workload with the model, its workspace and the input frames on the device)."""
-    from .stabilize import (_check_fill_params, _check_fit_params, _check_path_params, _check_sides, _fill, fit_homographies,
-                            smooth_path, warp_frames)
+    from .stabilize import (_check_fill_params, _check_fit_params, _check_path_params, _fill, fit_homographies, smooth_path,
+                            warp_frames)
     what = "stabilize_videos"
     if model._needs_grad():
         raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
@@ -930,7 +932,7 @@ def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8,
     for seq in sequences:
         if len(seq) < 2:
             raise ValueError(f"{what}: a video needs T >= 2 frames, got {len(seq)}")
-        _check_sides(*seq[0].shape[-2:], what)
+        check_sides(*seq[0].shape[-2:], what)
     from . import native
     fits = [[None] * (len(seq) - 1) for seq in sequences]
     ws = flows = None

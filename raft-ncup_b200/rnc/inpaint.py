@@ -48,13 +48,12 @@ import numpy as np
 import torch
 
 from . import native
-from .metrics import _f32, fb_consistency, nearest_site
+from .metrics import fb_consistency, nearest_site
+from .restate import PI_F32, bilinear_taps, check_sides, f32, inside, sample
 
-MAX_SIDE = 4096                             # csrc/dist_transform.cuh's kSiteMaxSide
 DEFAULT_SWEEPS = 512
 SOURCE_KNOWN, SOURCE_FORWARD, SOURCE_BACKWARD, SOURCE_BOTH, SOURCE_SPATIAL = (
     native.INPAINT_KNOWN, native.INPAINT_FORWARD, native.INPAINT_BACKWARD, native.INPAINT_BOTH, native.INPAINT_SPATIAL)
-PI_F32 = float(np.float32(math.pi))
 SSIM_RADIUS = 5
 _g = np.exp(-(np.arange(-SSIM_RADIUS, SSIM_RADIUS + 1, dtype=np.float64) ** 2) / (2 * 1.5 ** 2))
 SSIM_TAPS = (_g / _g.sum()).astype(np.float32)          # csrc/inpaint.cu's kGauss
@@ -67,12 +66,7 @@ def omega(L):
     """The SOR factor of an image whose unknown pixels' bounding box has the larger side L: 2 / (1 + pi_f32 / (L + 1)), each
     operation rounded once to float32."""
     t = torch.tensor(float(L + 1), dtype=torch.float64)
-    return float(_f32(2.0 / _f32(1.0 + _f32(PI_F32 / t))))
-
-
-def _check_sides(H, W, what):
-    if not (1 <= H <= MAX_SIDE and 1 <= W <= MAX_SIDE):
-        raise ValueError(f"{what}: frames of {H}x{W}; the kernels take 1 <= H, W <= {MAX_SIDE}")
+    return float(f32(2.0 / f32(1.0 + f32(PI_F32 / t))))
 
 
 def _check_sweeps(sweeps, what):
@@ -90,7 +84,7 @@ def _check_fill(values, unknown, sweeps):
         raise ValueError(f"harmonic_fill: values and unknown must be on one device, got {values.device} and {unknown.device}")
     if not 1 <= C <= native.HARMONIC_MAX_CHANNELS:
         raise ValueError(f"harmonic_fill: expected 1 to {native.HARMONIC_MAX_CHANNELS} channels, got {C}")
-    _check_sides(H, W, "harmonic_fill")
+    check_sides(H, W, "harmonic_fill")
     _check_sweeps(sweeps, "harmonic_fill")
 
 
@@ -146,7 +140,7 @@ def _neighbour_sum(u):
         xs, xd = (slice(0, W + dx), slice(-dx, W)) if dx < 0 else (slice(dx, W), slice(0, W - dx))
         nb[:, yd, xd] = u[:, ys, xs]
         has[yd, xd] = True
-        s = torch.where(has, _f32(s + nb), s)
+        s = torch.where(has, f32(s + nb), s)
         n = n + has
     return s, n
 
@@ -170,7 +164,7 @@ def _host_fill_image(v, unk, sweeps):
     for _ in range(sweeps):
         for m in colours:
             s, _ = _neighbour_sum(u)
-            u = torch.where(m, _f32(u + _f32(w * _f32(_f32(s / n.clamp(min=1)) - u))), u)
+            u = torch.where(m, f32(u + f32(w * f32(f32(s / n.clamp(min=1)) - u))), u)
     return u
 
 
@@ -214,7 +208,7 @@ def _check_video(frames, masks, flow, flow_bw, what):
     for name, t in (("flow", flow), ("flow_bw", flow_bw)):
         if tuple(t.shape) != (V, T - 1, 2, H, W):
             raise ValueError(f"{what}: expected {name} {[V, T - 1, 2, H, W]}, got {tuple(t.shape)}")
-    _check_sides(H, W, what)
+    check_sides(H, W, what)
     return V, T, H, W
 
 
@@ -253,11 +247,6 @@ def inpaint_propagate(frames, masks, flow, flow_bw, occ, occ_bw, max_distance=No
     return out, source
 
 
-def _gather(img, k, iy, ix):
-    """img[k, :, iy, ix] for per-element frames k: img [K,C,H,W] -> [C, n]."""
-    return img[k, :, iy, ix].T
-
-
 def _host_chain(I, M, f, o, t, x, y, maxd, forward):
     """One direction of the chains of a video's hole pixels: I fp64 [T,3,H,W], M bool [T,H,W] (hole), f fp64 [T-1,2,H,W],
     o bool [T-1,H,W], start frames t [n] and positions x, y [n] (fp64).  Returns (found bool [n], colour fp64 [3,n],
@@ -275,43 +264,23 @@ def _host_chain(I, M, f, o, t, x, y, maxd, forward):
         pair = (k if forward else k - 1).clamp(0, T - 2)
         ix, iy = torch.round(x).long(), torch.round(y).long()
         live &= ~o[pair, iy, ix]
-        u = _sample_k(f, pair, x, y)
-        nx, ny = _f32(x + u[0]), _f32(y + u[1])
-        live &= (nx >= 0) & (nx <= W - 1) & (ny >= 0) & (ny <= H - 1)
+        u = sample(f, x, y, pair)
+        nx, ny = f32(x + u[0]), f32(y + u[1])
+        live &= inside(nx, ny, H, W)
         x, y = torch.where(live, nx, x), torch.where(live, ny, y)
         k, d = torch.where(live, k + step, k), torch.where(live, d + 1, d)
         hit = live & ~M[k, torch.round(y).long(), torch.round(x).long()]
         found |= hit
         live &= ~hit
     # the masked bilinear colour at each candidate's end (every element computes one; only found ones are kept)
-    x0, y0 = torch.floor(x), torch.floor(y)
-    ax, ay = _f32(x - x0), _f32(y - y0)
-    bx, by = _f32(1 - ax), _f32(1 - ay)
-    ix, iy = x0.long(), y0.long()
-    ix1, iy1 = (ix + 1).clamp(max=W - 1), (iy + 1).clamp(max=H - 1)
     ws = torch.full((n,), -0.0, dtype=torch.float64)
     s = torch.full((3, n), -0.0, dtype=torch.float64)
-    for ty, tx, w in ((iy, ix, _f32(bx * by)), (iy, ix1, _f32(ax * by)), (iy1, ix, _f32(bx * ay)), (iy1, ix1, _f32(ax * ay))):
+    for ty, tx, w in bilinear_taps(x, y, H, W):
         ok = ~M[k, ty, tx]
-        ws = torch.where(ok, _f32(ws + w), ws)
-        s = torch.where(ok, _f32(s + _f32(w * _gather(I, k, ty, tx))), s)
-    return found, _f32(s / ws), d
+        ws = torch.where(ok, f32(ws + w), ws)
+        s = torch.where(ok, f32(s + f32(w * I[k, :, ty, tx].T)), s)
+    return found, f32(s / ws), d
 
-
-def _sample_k(img, k, px, py):
-    """rnc.interp's bilinear sample of img (fp64 [K,C,H,W] holding float32 values) with per-element frames k at (px, py):
-    the coordinates clamped to the frame, each operation rounded once in the kernel's order.  Returns [C, n]."""
-    H, W = img.shape[-2:]
-    px, py = px.clamp(0, W - 1), py.clamp(0, H - 1)
-    x0, y0 = torch.floor(px), torch.floor(py)
-    ax, ay = _f32(px - x0), _f32(py - y0)
-    bx, by = _f32(1 - ax), _f32(1 - ay)
-    ix, iy = x0.long(), y0.long()
-    ix1, iy1 = (ix + 1).clamp(max=W - 1), (iy + 1).clamp(max=H - 1)
-    s = _f32(_gather(img, k, iy, ix) * _f32(bx * by))
-    s = _f32(s + _f32(_gather(img, k, iy, ix1) * _f32(ax * by)))
-    s = _f32(s + _f32(_gather(img, k, iy1, ix) * _f32(bx * ay)))
-    return _f32(s + _f32(_gather(img, k, iy1, ix1) * _f32(ax * ay)))
 
 
 def host_inpaint_propagate(frames, masks, flow, flow_bw, occ, occ_bw, max_distance=None):
@@ -331,7 +300,7 @@ def host_inpaint_propagate(frames, masks, flow, flow_bw, occ, occ_bw, max_distan
         bw = _host_chain(I, M, flow_bw[v].detach().cpu().float().double(), occ_bw[v].detach().cpu() != 0, t, xf, yf, maxd,
                          False)
         (hf, cf, df), (hb, cb, db) = fw, bw
-        both = _f32(_f32(_f32(db.double() * cf) + _f32(df.double() * cb)) / (df + db).double().clamp(min=1))
+        both = f32(f32(f32(db.double() * cf) + f32(df.double() * cb)) / (df + db).double().clamp(min=1))
         c = torch.where(hf & hb, both, torch.where(hf, cf, torch.where(hb, cb, 0.0)))
         o = torch.where(M[:, None], 0.0, I)
         o[t, :, y, x] = c.T
@@ -435,12 +404,12 @@ def _separable(q):
     H, W = q.shape[-2:]
     n = 2 * SSIM_RADIUS + 1
     g = [float(t) for t in SSIM_TAPS]
-    h = _f32(g[0] * q[..., :, 0:W - n + 1])
+    h = f32(g[0] * q[..., :, 0:W - n + 1])
     for j in range(1, n):
-        h = _f32(h + _f32(g[j] * q[..., :, j:j + W - n + 1]))
-    m = _f32(g[0] * h[..., 0:H - n + 1, :])
+        h = f32(h + f32(g[j] * q[..., :, j:j + W - n + 1]))
+    m = f32(g[0] * h[..., 0:H - n + 1, :])
     for i in range(1, n):
-        m = _f32(m + _f32(g[i] * h[..., i:i + H - n + 1, :]))
+        m = f32(m + f32(g[i] * h[..., i:i + H - n + 1, :]))
     return m
 
 
@@ -448,12 +417,12 @@ def host_ssim_map(pred, gt):
     """The float32 SSIM map of each frame and channel, [N,3,H-10,W-10] as float32: the kernel's operations in its order."""
     _check_ssim(pred, gt)
     a, b = (t.detach().cpu().float().double() for t in (pred, gt))
-    mx, my, sxx, syy, sxy = (_separable(q) for q in (a, b, _f32(a * a), _f32(b * b), _f32(a * b)))
-    mx2, my2, mxy = _f32(mx * mx), _f32(my * my), _f32(mx * my)
-    sx, sy, sxy = _f32(sxx - mx2), _f32(syy - my2), _f32(sxy - mxy)
-    num = _f32(_f32(_f32(2 * mxy) + SSIM_C1) * _f32(_f32(2 * sxy) + SSIM_C2))
-    den = _f32(_f32(_f32(mx2 + my2) + SSIM_C1) * _f32(_f32(sx + sy) + SSIM_C2))
-    return _f32(num / den).float()
+    mx, my, sxx, syy, sxy = (_separable(q) for q in (a, b, f32(a * a), f32(b * b), f32(a * b)))
+    mx2, my2, mxy = f32(mx * mx), f32(my * my), f32(mx * my)
+    sx, sy, sxy = f32(sxx - mx2), f32(syy - my2), f32(sxy - mxy)
+    num = f32(f32(f32(2 * mxy) + SSIM_C1) * f32(f32(2 * sxy) + SSIM_C2))
+    den = f32(f32(f32(mx2 + my2) + SSIM_C1) * f32(f32(sx + sy) + SSIM_C2))
+    return f32(num / den).float()
 
 
 def host_ssim(pred, gt):

@@ -39,7 +39,8 @@ import numpy as np
 import torch
 
 from . import native
-from .metrics import InterpPartials, _f32, nearest_site
+from .metrics import InterpPartials, nearest_site
+from .restate import f32, inside, sample
 
 NO_PROPOSAL = np.uint64(0xFFFFFFFFFFFFFFFF)
 
@@ -102,23 +103,6 @@ def interpolate(frame0, frame1, flow, flow_bw, occ, occ_bw, times=(0.5,)):
     return out
 
 
-def _sample(img, px, py):
-    """Bilinear samples of img (fp64 [3,H,W] holding float32 values) at (px, py) (fp64 [...], float32 values), the coordinates
-    clamped to the frame, each operation rounded once to float32 in the kernel's order.  Returns [3, ...]."""
-    H, W = img.shape[-2:]
-    px, py = px.clamp(0, W - 1), py.clamp(0, H - 1)
-    x0, y0 = torch.floor(px), torch.floor(py)
-    ax, ay = _f32(px - x0), _f32(py - y0)
-    bx, by = _f32(1 - ax), _f32(1 - ay)
-    ix, iy = x0.long(), y0.long()
-    ix1, iy1 = (ix + 1).clamp(max=W - 1), (iy + 1).clamp(max=H - 1)
-    w00, w01, w10, w11 = _f32(bx * by), _f32(ax * by), _f32(bx * ay), _f32(ax * ay)
-    s = _f32(img[:, iy, ix] * w00)
-    s = _f32(s + _f32(img[:, iy, ix1] * w01))
-    s = _f32(s + _f32(img[:, iy1, ix] * w10))
-    return _f32(s + _f32(img[:, iy1, ix1] * w11))
-
-
 def host_interpolate(frame0, frame1, flow, flow_bw, occ, occ_bw, times=(0.5,)):
     """interpolate's definition in torch and numpy, one image at a time: each floating-point operation evaluated in fp64 on
     float32 operands and rounded once to float32 (the IEEE float32 result, as rnc.metrics.host_fb_consistency does), in the
@@ -141,16 +125,16 @@ def host_interpolate(frame0, frame1, flow, flow_bw, occ, occ_bw, times=(0.5,)):
             f = flows[s][b]
             ok = (occs[s][b] == 0) & torch.isfinite(f[0]) & torch.isfinite(f[1])
             f = torch.where(ok, f, 0.0)
-            smp = _sample(frames[1 - s][b], _f32(xs + f[0]), _f32(ys + f[1]))
-            d = _f32(smp - frames[s][b]).abs()
-            e = _f32(_f32(d[0] + d[1]) + d[2])
+            smp = sample(frames[1 - s][b], f32(xs + f[0]), f32(ys + f[1]))
+            d = f32(smp - frames[s][b]).abs()
+            e = f32(f32(d[0] + d[1]) + d[2])
             bits = e.float().numpy().reshape(-1).view(np.uint32).astype(np.uint64)
             key = (bits << np.uint64(32)) | (index + np.uint64(s * hw))
             for k, t in enumerate(ts):
-                tt = t if s == 0 else float(_f32(torch.tensor(1.0 - t, dtype=torch.float64)))
-                qx = torch.round(_f32(xs + _f32(tt * f[0])))
-                qy = torch.round(_f32(ys + _f32(tt * f[1])))
-                go = (ok & (qx >= 0) & (qx <= W - 1) & (qy >= 0) & (qy <= H - 1)).reshape(-1).numpy()
+                tt = t if s == 0 else float(f32(torch.tensor(1.0 - t, dtype=torch.float64)))
+                qx = torch.round(f32(xs + f32(tt * f[0])))
+                qy = torch.round(f32(ys + f32(tt * f[1])))
+                go = (ok & inside(qx, qy, H, W)).reshape(-1).numpy()
                 target = (qy * W + qx).reshape(-1).numpy()[go].astype(np.int64)
                 np.minimum.at(keys[k], target, key[go])
         site = nearest_site((keys != NO_PROPOSAL).reshape(T, H, W)).reshape(T, hw)
@@ -162,17 +146,16 @@ def host_interpolate(frame0, frame1, flow, flow_bw, occ, occ_bw, times=(0.5,)):
             u = [torch.where(torch.from_numpy(has), torch.where(back, -flows[1][b, c].reshape(-1)[q],
                                                                 flows[0][b, c].reshape(-1)[q]), 0.0).view(H, W)
                  for c in (0, 1)]
-            omt = float(_f32(torch.tensor(1.0 - t, dtype=torch.float64)))
-            x0, y0 = _f32(xs - _f32(t * u[0])), _f32(ys - _f32(t * u[1]))
-            x1, y1 = _f32(xs + _f32(omt * u[0])), _f32(ys + _f32(omt * u[1]))
+            omt = float(f32(torch.tensor(1.0 - t, dtype=torch.float64)))
+            x0, y0 = f32(xs - f32(t * u[0])), f32(ys - f32(t * u[1]))
+            x1, y1 = f32(xs + f32(omt * u[0])), f32(ys + f32(omt * u[1]))
             vis = []
             for o, px, py in ((occs[0][b], x0, y0), (occs[1][b], x1, y1)):
-                inside = (px >= 0) & (px <= W - 1) & (py >= 0) & (py <= H - 1)
                 ix = torch.round(px).clamp(0, W - 1).long()
                 iy = torch.round(py).clamp(0, H - 1).long()
-                vis.append(inside & (o[iy, ix] == 0))
-            s0, s1 = _sample(frames[0][b], x0, y0), _sample(frames[1][b], x1, y1)
-            blend = _f32(_f32(omt * s0) + _f32(t * s1))
+                vis.append(inside(px, py, H, W) & (o[iy, ix] == 0))
+            s0, s1 = sample(frames[0][b], x0, y0), sample(frames[1][b], x1, y1)
+            blend = f32(f32(omt * s0) + f32(t * s1))
             out[b, k] = torch.where(vis[0] == vis[1], blend, torch.where(vis[0], s0, s1)).float()
     return out
 

@@ -24,6 +24,7 @@ import numpy as np
 import torch
 
 from . import native
+from .restate import f32
 
 # counts: int64 [N, 5] (valid, epe < 1, < 3, < 5, outliers); epe_sum: float64 [N]
 Partials = namedtuple("Partials", "counts epe_sum")
@@ -100,14 +101,8 @@ def flow_metrics(flow, gt, valid=None):
     return Partials(counts, epe_sum)
 
 
-def _f32(x):
-    """x (fp64) rounded to float32, kept in fp64.  Each of + - * / sqrt evaluated in fp64 on float32 operands and rounded once
-    to float32 is the IEEE float32 result (53 >= 2 * 24 + 2 bits), whatever the CPU's vector library rounds."""
-    return x.float().double()
-
-
 def _norm(v):
-    return _f32(_f32(_f32(v[0] * v[0]) + _f32(v[1] * v[1])).sqrt())
+    return f32(f32(f32(v[0] * v[0]) + f32(v[1] * v[1])).sqrt())
 
 
 def host_partials(flow, gt, valid=None):
@@ -118,10 +113,10 @@ def host_partials(flow, gt, valid=None):
     counts, sums = [], []
     for b in range(flow.shape[0]):
         f, g = flow[b].float().double(), gt[b].float().double()
-        epe = _norm(_f32(f - g))
+        epe = _norm(f32(f - g))
         mag = _norm(g)
         val = torch.ones_like(epe, dtype=torch.bool) if valid is None else valid[b] >= 0.5
-        out = (epe > 3.0) & (_f32(epe / mag).float() > 0.05)     # compared in float32: 0.05 is rounded to 0.05f
+        out = (epe > 3.0) & (f32(epe / mag).float() > 0.05)     # compared in float32: 0.05 is rounded to 0.05f
         counts.append(torch.stack([val.sum(), (val & (epe < 1)).sum(), (val & (epe < 3)).sum(), (val & (epe < 5)).sum(),
                                    (val & out).sum()]))
         sums.append(torch.where(val, epe, 0.0).double().sum())
@@ -215,7 +210,7 @@ def host_sparsification(flow, gt, valid, score):
     ideal = torch.zeros(B, FRACTIONS, dtype=torch.float64)
     for b in range(B):
         f, g = flow[b].float().double(), gt[b].float().double()
-        epe = _norm(_f32(f - g)).reshape(-1)
+        epe = _norm(f32(f - g)).reshape(-1)
         val = torch.ones_like(epe, dtype=torch.bool) if valid is None else (valid[b] >= 0.5).reshape(-1)
         e, s = epe[val], score[b].float().reshape(-1)[val]
         n = e.numel()
@@ -309,11 +304,11 @@ def _fb_direction(f, g, a1, a2):
     u = torch.arange(W, dtype=torch.float64).view(1, 1, W)
     v = torch.arange(H, dtype=torch.float64).view(1, H, 1)
     fu, fv = f[:, 0], f[:, 1]
-    px, py = _f32(u + fu), _f32(v + fv)
+    px, py = f32(u + fu), f32(v + fv)
     inside = (px >= 0) & (px <= W - 1) & (py >= 0) & (py <= H - 1)
     x0, y0 = torch.floor(px), torch.floor(py)
-    ax, ay = _f32(px - x0), _f32(py - y0)
-    bx, by = _f32(1 - ax), _f32(1 - ay)
+    ax, ay = f32(px - x0), f32(py - y0)
+    bx, by = f32(1 - ax), f32(1 - ay)
     ix = torch.where(inside, x0, 0).long()
     iy = torch.where(inside, y0, 0).long()
     bi = torch.arange(B).view(B, 1, 1).expand_as(ix)
@@ -323,21 +318,21 @@ def _fb_direction(f, g, a1, a2):
         ok = (x < W) & (y < H)
         return torch.where(ok, g[bi, c, y.clamp(max=H - 1), x.clamp(max=W - 1)], 0.0)
 
-    w00, w01, w10, w11 = _f32(bx * by), _f32(ax * by), _f32(bx * ay), _f32(ax * ay)
+    w00, w01, w10, w11 = f32(bx * by), f32(ax * by), f32(bx * ay), f32(ax * ay)
     gs = []
     for c in range(2):
-        s = _f32(tap(0, 0, c) * w00)
-        s = _f32(s + _f32(tap(1, 0, c) * w01))
-        s = _f32(s + _f32(tap(0, 1, c) * w10))
-        gs.append(_f32(s + _f32(tap(1, 1, c) * w11)))
-    su, sv = _f32(fu + gs[0]), _f32(fv + gs[1])
-    lhs = _f32(_f32(su * su) + _f32(sv * sv))
-    mf = _f32(_f32(fu * fu) + _f32(fv * fv))
-    mg = _f32(_f32(gs[0] * gs[0]) + _f32(gs[1] * gs[1]))
-    rhs = _f32(_f32(a1 * _f32(mf + mg)) + a2)
+        s = f32(tap(0, 0, c) * w00)
+        s = f32(s + f32(tap(1, 0, c) * w01))
+        s = f32(s + f32(tap(0, 1, c) * w10))
+        gs.append(f32(s + f32(tap(1, 1, c) * w11)))
+    su, sv = f32(fu + gs[0]), f32(fv + gs[1])
+    lhs = f32(f32(su * su) + f32(sv * sv))
+    mf = f32(f32(fu * fu) + f32(fv * fv))
+    mg = f32(f32(gs[0] * gs[0]) + f32(gs[1] * gs[1]))
+    rhs = f32(f32(a1 * f32(mf + mg)) + a2)
     finite = torch.isfinite(lhs)
     inf = torch.full_like(lhs, float("inf"))
-    err = torch.where(inside & finite, _f32(torch.where(finite, lhs, 0.0).sqrt()), inf)
+    err = torch.where(inside & finite, f32(torch.where(finite, lhs, 0.0).sqrt()), inf)
     occ = torch.where(inside, (~finite | (lhs > rhs)).to(torch.uint8), torch.full_like(lhs, 3, dtype=torch.uint8))
     return occ, err.float()
 
@@ -541,10 +536,10 @@ def host_region_partials(flow, gt, valid=None, occ=None, noc=None, fg=None):
     sums = torch.zeros(B, cells, dtype=torch.float64)
     for b in range(B):
         f, g = flow[b].detach().cpu().float().double(), gt[b].detach().cpu().float().double()
-        epe = _norm(_f32(f - g))
+        epe = _norm(f32(f - g))
         mag = _norm(g)
         val = torch.ones_like(epe, dtype=torch.bool) if valid is None else valid[b].cpu() >= 0.5
-        out = (epe > 3.0) & (_f32(epe / mag).float() > 0.05)
+        out = (epe > 3.0) & (f32(epe / mag).float() > 0.05)
         if occ is not None:
             d = (d2[b] >= 100).long() + (d2[b] >= 3600).long() + (d2[b] >= 19600).long()    # DIST2_NONE: 3
             s = torch.where(torch.isnan(mag), 3, (mag >= 10).long() + (mag >= 40).long())

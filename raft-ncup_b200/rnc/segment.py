@@ -48,9 +48,9 @@ import numpy as np
 import torch
 
 from . import native
-from .metrics import _f32, nearest_site
+from .metrics import nearest_site
+from .restate import bilinear_taps, check_sides, f32, follow
 
-MAX_SIDE = 4096                             # csrc/dist_transform.cuh's kSiteMaxSide
 VOID = 255
 # the columns of a (frame, object)'s counts (RNC_SEGMENT_COUNTS)
 COUNT_INTER, COUNT_UNION, COUNT_N_FG, COUNT_N_GT, COUNT_FG_MATCH, COUNT_GT_MATCH = range(6)
@@ -68,11 +68,6 @@ def check_labels(labels, what="propagate"):
         raise ValueError(f"{what}: labels must lie in 0..254 (255 is void, not a label), got {bad}")
 
 
-def _check_sides(H, W, what):
-    if not (1 <= H <= MAX_SIDE and 1 <= W <= MAX_SIDE):
-        raise ValueError(f"{what}: frames of {H}x{W}; the kernels take 1 <= H, W <= {MAX_SIDE}")
-
-
 def _check_step(labels, flow_bw, occ_bw):
     """(V, H, W) of propagate_step's arguments; ValueError for mismatched shapes, mixed devices or a frame side above 4096."""
     if labels.dim() != 3 or labels.shape[0] == 0:
@@ -85,7 +80,7 @@ def _check_step(labels, flow_bw, occ_bw):
     devs = {t.device for t in (labels, flow_bw, occ_bw)}
     if len(devs) != 1:
         raise ValueError(f"propagate_step: the labels, flow and mask must be on one device, got {sorted(map(str, devs))}")
-    _check_sides(H, W, "propagate_step")
+    check_sides(H, W, "propagate_step")
     return V, H, W
 
 
@@ -135,7 +130,7 @@ def _check_video(first_labels, flow_bw, occ_bw):
     devs = {t.device for t in (first_labels, flow_bw, occ_bw)}
     if len(devs) != 1:
         raise ValueError(f"propagate: the labels, flows and masks must be on one device, got {sorted(map(str, devs))}")
-    _check_sides(H, W, "propagate")
+    check_sides(H, W, "propagate")
     check_labels(first_labels, "propagate")
     return V, T1 + 1, H, W
 
@@ -161,20 +156,9 @@ def _host_vote(L, G, occ):
     """One frame of the rule on the host: L uint8 [H,W], G fp64 [2,H,W] holding float32 values, occ [H,W].  Returns the
     int64 labels [H,W]."""
     H, W = L.shape
-    ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
-    ux, uy = G[0], G[1]
-    px, py = _f32(xs + ux), _f32(ys + uy)
-    matched = (torch.isfinite(ux) & torch.isfinite(uy) & (occ == 0) & (px >= 0) & (px <= W - 1) & (py >= 0)
-               & (py <= H - 1))
-    cx, cy = torch.where(matched, px, 0.0), torch.where(matched, py, 0.0)      # an unmatched pixel's vote is discarded
-    x0, y0 = torch.floor(cx), torch.floor(cy)
-    ax, ay = _f32(cx - x0), _f32(cy - y0)
-    bx, by = _f32(1 - ax), _f32(1 - ay)
-    ix, iy = x0.long(), y0.long()
-    ix1, iy1 = (ix + 1).clamp(max=W - 1), (iy + 1).clamp(max=H - 1)
+    matched, px, py = follow(G, occ)                                          # an unmatched pixel's vote is discarded
     lab = L.long()
-    taps = [lab[iy, ix], lab[iy, ix1], lab[iy1, ix], lab[iy1, ix1]]
-    w = [_f32(bx * by), _f32(ax * by), _f32(bx * ay), _f32(ax * ay)]
+    taps, w = zip(*[(lab[ty, tx], wt) for ty, tx, wt in bilinear_taps(px, py, H, W)])
     best = torch.full((H, W), -1.0, dtype=torch.float64)
     vote = torch.full((H, W), VOID, dtype=torch.int64)
     for i in range(4):
@@ -183,7 +167,7 @@ def _host_vote(L, G, occ):
             first &= taps[j] != taps[i]
         s = w[i]
         for j in range(i + 1, 4):
-            s = torch.where(taps[j] == taps[i], _f32(s + w[j]), s)
+            s = torch.where(taps[j] == taps[i], f32(s + w[j]), s)
         take = first & ((s > best) | ((s == best) & (taps[i] < vote)))
         best, vote = torch.where(take, s, best), torch.where(take, taps[i], vote)
     site = torch.from_numpy(nearest_site(matched.numpy()[None])[0])
@@ -252,7 +236,7 @@ def _check_counts(pred, gt, K):
     for name, t in (("pred", pred), ("gt", gt)):
         if t.dtype.is_floating_point or t.dtype.is_complex:
             raise ValueError(f"segmentation_counts: expected integer {name} labels, got {t.dtype}")
-    _check_sides(pred.shape[1], pred.shape[2], "segmentation_counts")
+    check_sides(pred.shape[1], pred.shape[2], "segmentation_counts")
     return pred.shape
 
 

@@ -97,9 +97,8 @@ import numpy as np
 import torch
 
 from . import native
-from .interp import _sample
+from .restate import check_sides, inside, project, sample
 
-MAX_SIDE = 4096
 DEFAULT_STRIDE, DEFAULT_HYPOTHESES, DEFAULT_TAU, DEFAULT_REFINE = 8, 256, 2.0, 4
 DEFAULT_RADIUS, DEFAULT_SIGMA, DEFAULT_CROP_MIN = 30, 10.0, 0.5
 OK, FEW = native.HOMOGRAPHY_OK, native.HOMOGRAPHY_FEW
@@ -137,11 +136,6 @@ def _check_path_params(radius, sigma, crop_min, what):
         raise ValueError(f"{what}: expected 0 < crop_min <= 1, got {crop_min!r}")
 
 
-def _check_sides(H, W, what):
-    if not (1 <= H <= MAX_SIDE and 1 <= W <= MAX_SIDE):
-        raise ValueError(f"{what}: frames of {H}x{W}; the kernels take 1 <= H, W <= {MAX_SIDE}")
-
-
 # ------------------------------------------------------------------------------------------------------------- the fit
 
 
@@ -151,7 +145,7 @@ def _check_flow(flow, what="fit_homographies"):
     N, _, H, W = flow.shape
     if N > 65535:
         raise ValueError(f"{what}: at most 65535 pairs per call, got {N}")
-    _check_sides(H, W, what)
+    check_sides(H, W, what)
     return N, H, W
 
 
@@ -445,7 +439,7 @@ def _check_motion(motion, H, W, what):
         raise ValueError(f"{what}: expected motion [V,T-1,3,3], got {tuple(motion.shape)}")
     if motion.shape[0] > 65535:
         raise ValueError(f"{what}: at most 65535 videos per call, got {motion.shape[0]}")
-    _check_sides(H, W, what)
+    check_sides(H, W, what)
     return motion.shape[0], motion.shape[1] + 1
 
 
@@ -526,7 +520,7 @@ def _check_warp(frames, maps):
         raise ValueError(f"warp_frames: frames on {frames.device}, maps on {maps.device}; they must be on one device")
     if N > 65535:
         raise ValueError(f"warp_frames: at most 65535 frames per call, got {N}")
-    _check_sides(H, W, "warp_frames")
+    check_sides(H, W, "warp_frames")
     return N, C, H, W
 
 
@@ -549,7 +543,7 @@ def warp_frames(frames, maps):
 
 
 def host_warp_frames(frames, maps):
-    """warp_frames' rule on the host: q in numpy fp64, rounded to float32, and rnc.interp._sample.  Returns (out, valid) on
+    """warp_frames' rule on the host: q in numpy fp64, rounded to float32, and rnc.restate.sample.  Returns (out, valid) on
     the CPU."""
     N, C, H, W = _check_warp(frames, maps)
     out = torch.zeros(N, C, H, W, dtype=torch.float32)
@@ -558,14 +552,12 @@ def host_warp_frames(frames, maps):
     with np.errstate(all="ignore"):
         for n in range(N):
             m = maps[n].detach().cpu().to(torch.float64).numpy().ravel()
-            X = (m[0] * x + m[1] * y) + m[2]
-            Y = (m[3] * x + m[4] * y) + m[5]
-            w = (m[6] * x + m[7] * y) + m[8]
-            qx, qy = (X / w).astype(np.float32), (Y / w).astype(np.float32)
-            ok = (w > 0) & (qx >= 0) & (qx <= W - 1) & (qy >= 0) & (qy <= H - 1)
+            X, Y, ok = project(m, x, y)
+            qx, qy = X.astype(np.float32), Y.astype(np.float32)
+            ok &= inside(qx, qy, H, W)
             px = torch.from_numpy(np.where(ok, qx, 0).astype(np.float64))
             py = torch.from_numpy(np.where(ok, qy, 0).astype(np.float64))
-            s = _sample(frames[n].detach().cpu().float().double(), px, py)
+            s = sample(frames[n].detach().cpu().float().double(), px, py)
             okt = torch.from_numpy(ok)
             out[n] = torch.where(okt, s, 0.0).float()
             valid[n] = okt.to(torch.uint8)
@@ -590,7 +582,7 @@ def _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, what):
         raise ValueError(f"{what}: the flows, motion and maps must be on one device, got {sorted(map(str, devs))}")
     if V > 65535 or T > 65536:
         raise ValueError(f"{what}: at most 65535 videos of 65536 frames per call, got {V} of {T}")
-    _check_sides(H, W, what)
+    check_sides(H, W, what)
     return V, T, H, W
 
 
@@ -643,33 +635,25 @@ def add_global_motion(res, res_bw, motion, maps, maps_inv):
     return out[0], out[1]
 
 
-def _host_project(m, x, y):
-    """pi(m (x, y, 1)) in numpy fp64, each operation rounded once: (X / w, Y / w, w > 0)."""
-    X = (m[0] * x + m[1] * y) + m[2]
-    Y = (m[3] * x + m[4] * y) + m[5]
-    w = (m[6] * x + m[7] * y) + m[8]
-    return X / w, Y / w, w > 0
-
-
 def _host_direction(src, dst, A, f, r):
     """One direction of step 5a (r None: f fp64 [2,H,W] holding the flow's float32 values) or 5c (r: the completed residual,
     fp64 [2,H,W] holding float32 values) over every output pixel: float32 [2,H,W]."""
     H, W = f.shape[-2:] if r is None else r.shape[-2:]
     y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing="ij")
-    X, Y, ok = _host_project(src, x, y)
+    X, Y, ok = project(src, x, y)
     qx, qy = X.astype(np.float32).astype(np.float64), Y.astype(np.float32).astype(np.float64)
-    bx, by, ok_b = _host_project(A, qx, qy)
-    gx, gy, ok_g = _host_project(dst, bx, by)
+    bx, by, ok_b = project(A, qx, qy)
+    gx, gy, ok_g = project(dst, bx, by)
     ok = ok & ok_b & ok_g
     if r is not None:
         out = np.stack([(gx - x) + r[0], (gy - y) + r[1]])
         return np.where(ok, out, np.nan).astype(np.float32)
-    ok &= (qx >= 0) & (qx <= W - 1) & (qy >= 0) & (qy <= H - 1)
+    ok &= inside(qx, qy, H, W)
     px = torch.from_numpy(np.where(ok, qx, 0.0))
     py = torch.from_numpy(np.where(ok, qy, 0.0))
-    u = _sample(torch.from_numpy(f), px, py).numpy()
+    u = sample(torch.from_numpy(f), px, py).numpy()
     ok &= np.isfinite(u).all(0)
-    ax, ay, ok_a = _host_project(dst, qx + u[0], qy + u[1])
+    ax, ay, ok_a = project(dst, qx + u[0], qy + u[1])
     ok &= ok_a
     return np.where(ok, np.stack([ax - gx, ay - gy]), np.nan).astype(np.float32)
 
@@ -692,7 +676,7 @@ def _host_flows(a, b, motion, maps, maps_inv, readd):
 
 def host_flow_residual(flow, flow_bw, motion, maps, maps_inv):
     """flow_residual's rule in numpy fp64, one output frame at a time and all its pixels at once; the flow sampled by
-    rnc.interp._sample.  Serves CPU tensors and is the kernel's test reference.  Returns (res, res_bw) on the CPU."""
+    rnc.restate.sample.  Serves CPU tensors and is the kernel's test reference.  Returns (res, res_bw) on the CPU."""
     _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, "flow_residual")
     return _host_flows(flow, flow_bw, motion, maps, maps_inv, False)
 

@@ -51,14 +51,12 @@ import numpy as np
 import torch
 
 from . import native
-from .interp import _sample
-from .metrics import _f32, nearest_site
+from .metrics import nearest_site
+from .restate import PI_F32, check_sides, f32, follow, sample
 
-MAX_SIDE = 4096                             # csrc/dist_transform.cuh's kSiteMaxSide
 DEFAULT_LAM = 0.1
 DEFAULT_ALPHA = 50.0
 DEFAULT_SWEEPS = 512
-PI_F32 = float(np.float32(math.pi))
 
 
 def sigma(lam):
@@ -77,11 +75,6 @@ def omega(d2, lam):
         L += L * L < 4 * d2
         s = min(np.float32(PI_F32) / np.float32(L + 1), s)
     return float(np.float32(2.0) / (np.float32(1.0) + np.float32(s)))
-
-
-def _check_sides(H, W, what):
-    if not (1 <= H <= MAX_SIDE and 1 <= W <= MAX_SIDE):
-        raise ValueError(f"{what}: frames of {H}x{W}; the kernels take 1 <= H, W <= {MAX_SIDE}")
 
 
 def _check_params(lam, alpha, sweeps, what):
@@ -109,7 +102,7 @@ def _check_step(out_prev, processed, frame_prev, frame, flow_bw, occ_bw, lam, al
         raise ValueError(f"temporal_step: expected 1 to {native.HARMONIC_MAX_CHANNELS} processed channels, got {C}")
     if V > 65535:
         raise ValueError(f"temporal_step: at most 65535 videos per step, got {V}")
-    _check_sides(H, W, "temporal_step")
+    check_sides(H, W, "temporal_step")
     _check_params(lam, alpha, sweeps, "temporal_step")
     return V, C, H, W
 
@@ -152,25 +145,20 @@ def _host_step(O, P, I0, I1, G, occ, lam, alpha, sweeps):
     Returns float32 [C,H,W]."""
     C, H, W = P.shape
     lam32, alpha32 = float(np.float32(lam)), float(np.float32(alpha))
-    ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
-    ux, uy = G[0], G[1]
-    px, py = _f32(xs + ux), _f32(ys + uy)
-    matched = (torch.isfinite(ux) & torch.isfinite(uy) & (occ == 0) & (px >= 0) & (px <= W - 1) & (py >= 0)
-               & (py <= H - 1))
-    cx, cy = torch.where(matched, px, 0.0), torch.where(matched, py, 0.0)      # an unmatched pixel's sample is discarded
-    e = _f32(_f32(I1 - _sample(I0, cx, cy)) / 255.0)
+    matched, cx, cy = follow(G, occ)
+    e = f32(f32(I1 - sample(I0, cx, cy)) / 255.0)
     d2 = torch.full((H, W), -0.0, dtype=torch.float64)
     for c in range(3):
-        d2 = _f32(d2 + _f32(e[c] * e[c]))
-    w = torch.where(matched, _f32(lam32 / _f32(1.0 + _f32(alpha32 * d2))), 0.0)
-    r = torch.where(w > 0, _f32(w * _f32(_sample(O, cx, cy) - P)), 0.0)
+        d2 = f32(d2 + f32(e[c] * e[c]))
+    w = torch.where(matched, f32(lam32 / f32(1.0 + f32(alpha32 * d2))), 0.0)
+    r = torch.where(w > 0, f32(w * f32(sample(O, cx, cy) - P)), 0.0)
     n = torch.zeros(H, W, dtype=torch.float64)
     n[1:] += 1
     n[:, 1:] += 1
     n[:, :-1] += 1
     n[:-1] += 1
-    den = _f32(n + w)
-    weak = (w < _f32(torch.tensor(lam32 * 0.25, dtype=torch.float64))).numpy()
+    den = f32(n + w)
+    weak = (w < f32(torch.tensor(lam32 * 0.25, dtype=torch.float64))).numpy()
     site = nearest_site(~weak[None])[0]
     if site.min() < 0 or not weak.any():
         d2max = 0
@@ -238,7 +226,7 @@ def _check_video(processed, frames, flow_bw, occ_bw, what):
         raise ValueError(f"{what}: expected 1 to {native.HARMONIC_MAX_CHANNELS} processed channels, got {C}")
     if V > 65535:
         raise ValueError(f"{what}: at most 65535 videos, got {V}")
-    _check_sides(H, W, what)
+    check_sides(H, W, what)
     return V, T, C, H, W
 
 
@@ -325,17 +313,13 @@ def host_warping_error(video, flow_bw, occ_bw):
     V, T, C, H, W = _check_warp(video, flow_bw, occ_bw)
     s = torch.zeros(V, T - 1, dtype=torch.float64)
     count = torch.zeros(V, T - 1, dtype=torch.int64)
-    ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64), torch.arange(W, dtype=torch.float64), indexing="ij")
     for v in range(V):
         vid = video[v].detach().cpu().float().double()
         for k in range(T - 1):
             G = flow_bw[v, k].detach().cpu().float().double()
             occ = occ_bw[v, k].detach().cpu()
-            px, py = _f32(xs + G[0]), _f32(ys + G[1])
-            matched = (torch.isfinite(G[0]) & torch.isfinite(G[1]) & (occ == 0) & (px >= 0) & (px <= W - 1) & (py >= 0)
-                       & (py <= H - 1))
-            cx, cy = torch.where(matched, px, 0.0), torch.where(matched, py, 0.0)
-            e = ((vid[k + 1] - _sample(vid[k], cx, cy)) / 255.0).numpy()
+            matched, cx, cy = follow(G, occ)
+            e = ((vid[k + 1] - sample(vid[k], cx, cy)) / 255.0).numpy()
             t = np.zeros((H, W))
             for c in range(C):
                 t = t + e[c] * e[c]

@@ -32,8 +32,7 @@ import math
 import torch
 
 from . import native
-from .interp import _sample
-from .metrics import _f32
+from .restate import f32, inside, sample
 
 THRESHOLDS = (1, 2, 4, 8, 16)
 # the columns of a video's counts (RNC_TRACK_COUNTS): pairs evaluated, occlusion agreements, gt visible, then per threshold
@@ -63,7 +62,7 @@ def check_queries(queries, T, H, W, what="track"):
     q = queries.detach().float().reshape(-1, 3)
     t, x, y = q.unbind(1)
     bad_t = ~((t >= 0) & (t <= T - 1) & (t == torch.floor(t)))
-    bad_xy = ~((x >= 0) & (x <= W - 1) & (y >= 0) & (y <= H - 1))
+    bad_xy = ~inside(x, y, H, W)
     any_t, any_xy = torch.stack([bad_t.any(), bad_xy.any()]).tolist()
     if any_t:
         raise ValueError(f"{what}: every query t must be an integer in [0, {T - 1}], got {t[bad_t][:4].tolist()}")
@@ -132,13 +131,13 @@ def _chain(f, o, q, T, forward):
         act = tq <= k if forward else tq >= k + 1
         if not act.any():
             continue
-        u = _sample(f[k], x, y)
+        u = sample(f[k], x, y)
         fin = torch.isfinite(u[0]) & torch.isfinite(u[1])
         # a point not yet lost lies in the frame, so the clamp only keeps a lost point's index in range
         ix, iy = torch.round(x).clamp(0, W - 1).long(), torch.round(y).clamp(0, H - 1).long()
         now = lost | ~fin | (o[k][iy, ix] != 0)
-        nx, ny = torch.where(fin, _f32(x + u[0]), x), torch.where(fin, _f32(y + u[1]), y)
-        now = now | ~((nx >= 0) & (nx <= W - 1) & (ny >= 0) & (ny <= H - 1))
+        nx, ny = torch.where(fin, f32(x + u[0]), x), torch.where(fin, f32(y + u[1]), y)
+        now = now | ~inside(nx, ny, H, W)
         x, y, lost = torch.where(act, nx, x), torch.where(act, ny, y), torch.where(act, now, lost)
         t = k + 1 if forward else k
         pos[act, t, 0], pos[act, t, 1] = x[act], y[act]
@@ -221,8 +220,8 @@ def host_track_metrics(tracks, visible, gt_tracks, gt_visible, queries, H, W):
     p, g = (t.detach().cpu().float().double() for t in (tracks, gt_tracks))
     pv, gv = (t.detach().cpu() != 0 for t in (visible, gt_visible))
     scale = torch.tensor([W, H], dtype=torch.float64)
-    d = _f32(_f32(_f32(p * 256) / scale) - _f32(_f32(g * 256) / scale))
-    d2 = _f32(_f32(d[..., 0] * d[..., 0]) + _f32(d[..., 1] * d[..., 1]))
+    d = f32(f32(f32(p * 256) / scale) - f32(f32(g * 256) / scale))
+    d2 = f32(f32(d[..., 0] * d[..., 0]) + f32(d[..., 1] * d[..., 1]))
     tq = queries.detach().cpu().float()[..., 0].long()
     ev = torch.ones(V, N, T, dtype=torch.bool)
     ev.scatter_(2, tq[..., None], False)

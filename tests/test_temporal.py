@@ -14,8 +14,9 @@ import torch
 from scipy.ndimage import zoom
 
 from rnc import native
-from rnc.temporal import (PI_F32, host_temporal_step, host_temporally_consistent, host_warping_error, omega, sigma,
-                          summarize_temporal, temporal_step, temporally_consistent, warping_error)
+from rnc.restate import PI_F32
+from rnc.temporal import (host_temporal_step, host_temporally_consistent, host_warping_error, omega, sigma, summarize_temporal,
+                          temporal_step, temporally_consistent, warping_error)
 from rnc.synth import shift_sequence
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
