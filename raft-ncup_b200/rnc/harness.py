@@ -453,9 +453,8 @@ def run_sequences_bidirectional(model, sequences, iters=32, warm_start=False, ba
     steps, padder = _sequence_setup(sequences, batch_size, mode, model, return_confidence)
     if not steps:
         return
-    if model._needs_grad():
-        raise ValueError("run_sequences_bidirectional is inference only: call it under torch.no_grad() (training through the "
-                         "bidirectional pass is model(..., bidirectional=True))")
+    _check_inference(model, "run_sequences_bidirectional",
+                     " (training through the bidirectional pass is model(..., bidirectional=True))")
     from .metrics import fb_consistency
     B = len(steps[0])
     for step, flow_low, flow_up, conf in _sequence_steps(model, sequences, steps, padder, iters, warm_start, device,
@@ -479,8 +478,7 @@ def interpolate_frames(model, frame0, frame1, times=(0.5,), iters=32, mode="sint
     its unpadded flows and occlusion masks.  Returns float32 [B,T,3,H,W].  Inference only: with grad enabled on a model that
     requires grad it raises ValueError."""
     from .interp import _times, interpolate
-    if model._needs_grad():
-        raise ValueError("interpolate_frames is inference only: call it under torch.no_grad()")
+    _check_inference(model, "interpolate_frames")
     _times(times)                                   # a bad time raises before the flow pass
     r = bidirectional_flow(model, frame0, frame1, iters, mode=mode, alpha1=alpha1, alpha2=alpha2)
     return interpolate(frame0, frame1, r["flow_up"], r["flow_up_bw"], r["occ"], r["occ_bw"], times)
@@ -522,6 +520,63 @@ def validate_interpolation(model, sequences, iters=32, mode="sintel", batch_size
     return summarize_interpolation(from_images(InterpPartials, [t for seq in every for t in seq]))
 
 
+def _check_inference(model, what, why=""):
+    if model._needs_grad():
+        raise ValueError(f"{what} is inference only: call it under torch.no_grad(){why}")
+
+
+def _check_counts(sequences, what, *lists):
+    """Each (noun, items) of lists as a list of items; ValueError unless every one holds one item per video."""
+    items = [list(x) for _, x in lists]
+    if any(len(x) != len(sequences) for x in items):
+        got = [f"{len(x)} {noun}" for (noun, _), x in zip(lists, items)]
+        if len(got) > 1:
+            got = [", ".join(got[:-1]), got[-1]]
+        raise ValueError(f"{what}: {len(sequences)} videos but {' and '.join(got)}")
+    return items
+
+
+def _check_frames(seq, what, need=2, why=""):
+    """ValueError for a video of fewer than `need` frames: each application's first check of a video."""
+    if len(seq) < need:
+        raise ValueError(f"{what}: a video needs T >= {need} frames{why}, got {len(seq)}")
+
+
+def _by_size(sequences, indices):
+    """The indices grouped by their video's frame size, in order of first appearance."""
+    groups = {}
+    for i in indices:
+        groups.setdefault(tuple(sequences[i][0].shape[-2:]), []).append(i)
+    return list(groups.values())
+
+
+class _PairStack(dict):
+    """Named results of the flow pass over `sequences`, stacked by add into [V,T-1,...] tensors, T the longest video's frame
+    count, allocated at the first pair on its results' device: float32 `flows` padded with 0, uint8 `masks` padded with 1,
+    so a shorter video's missing pairs are zero flows occluded in both directions."""
+
+    def __init__(self, sequences, flows, masks=()):
+        super().__init__()
+        self.pairs = (len(sequences), max((len(seq) for seq in sequences), default=1) - 1)
+        self.pads = [(name, 0, torch.float32) for name in flows] + [(name, 1, torch.uint8) for name in masks]
+
+    def add(self, s, k, r):
+        for name, pad, dtype in self.pads:
+            if name not in self:
+                self[name] = torch.full((*self.pairs, *r[name].shape), pad, dtype=dtype, device=r[name].device)
+            self[name][s, k].copy_(r[name])
+
+
+def _pad_videos(videos, pad):
+    """Per-video tensors [n_v,...] of one dtype and device stacked into [V,n,...], n the largest n_v, the items past a video's
+    n_v set to pad (a number, or a tensor that broadcasts to one item)."""
+    out = videos[0].new_empty((len(videos), max(t.shape[0] for t in videos), *videos[0].shape[1:]))
+    out[:] = pad
+    for v, t in enumerate(videos):
+        out[v, :t.shape[0]] = t
+    return out
+
+
 def track_points(model, sequences, queries, iters=32, warm_start=False, batch_size=8, mode="sintel", device="cuda",
                  alpha1=0.01, alpha2=0.5):
     """Tracks of query points through whole videos (rnc.track's rule: the bidirectional flows chained from each query frame,
@@ -540,11 +595,8 @@ def track_points(model, sequences, queries, iters=32, warm_start=False, batch_si
     flow pass for a video of fewer than two frames, a bad query or a query count that does not match the videos.  Inference
     only: with grad enabled on a model that requires grad it raises ValueError."""
     from .track import check_queries, track
-    if model._needs_grad():
-        raise ValueError("track_points is inference only: call it under torch.no_grad()")
-    qs = list(queries)
-    if len(qs) != len(sequences):
-        raise ValueError(f"track_points: {len(sequences)} videos but {len(qs)} query sets")
+    _check_inference(model, "track_points")
+    qs, = _check_counts(sequences, "track_points", ("query sets", queries))
     if not sequences:
         return []
     H, W = sequences[0][0].shape[-2:]
@@ -553,19 +605,12 @@ def track_points(model, sequences, queries, iters=32, warm_start=False, batch_si
         if q.dim() != 2:
             raise ValueError(f"track_points: expected each video's queries as [N,3], got {tuple(q.shape)}")
         check_queries(q, T, H, W, "track_points")
-    V, T, N = len(sequences), max(lens), max(q.shape[0] for q in qs)
-    flows = None
+    flows = _PairStack(sequences, ("flow_up", "flow_up_bw"), ("occ", "occ_bw"))
     for s, k, r in run_sequences_bidirectional(model, sequences, iters, warm_start=warm_start, batch_size=batch_size,
                                                mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
-        if flows is None:
-            dev = r["flow_up"].device
-            flows = {name: torch.zeros(V, T - 1, 2, H, W, dtype=torch.float32, device=dev) for name in ("flow_up", "flow_up_bw")}
-            flows.update({name: torch.ones(V, T - 1, H, W, dtype=torch.uint8, device=dev) for name in ("occ", "occ_bw")})
-        for name, t in flows.items():
-            t[s, k].copy_(r[name])
-    q = torch.zeros(V, N, 3, dtype=torch.float32, device=dev)   # (0, 0, 0) pads a video's queries to N; its tracks are dropped
-    for v, qv in enumerate(qs):
-        q[v, :qv.shape[0]] = qv
+        flows.add(s, k, r)
+    # (0, 0, 0) pads a video's queries to the largest count; their tracks are dropped
+    q = _pad_videos([qv.to(flows["flow_up"].device, torch.float32) for qv in qs], 0)
     tracks, visible = track(flows["flow_up"], flows["flow_up_bw"], flows["occ"], flows["occ_bw"], q)
     return [(tracks[v, :qv.shape[0], :lens[v]], visible[v, :qv.shape[0], :lens[v]]) for v, qv in enumerate(qs)]
 
@@ -583,9 +628,8 @@ def validate_tracking(model, sequences, queries, gt_tracks, gt_visible, iters=32
     from .track import summarize_tracking, track_metrics
     world, rank = world_rank()
     mine = list(strided_items(range(len(sequences)), world, rank))
-    if len(queries) != len(sequences) or len(gt_tracks) != len(sequences) or len(gt_visible) != len(sequences):
-        raise ValueError(f"validate_tracking: {len(sequences)} videos but {len(queries)} query sets, {len(gt_tracks)} "
-                         f"ground-truth tracks and {len(gt_visible)} visibility sets")
+    _check_counts(sequences, "validate_tracking", ("query sets", queries), ("ground-truth tracks", gt_tracks),
+                  ("visibility sets", gt_visible))
     got = track_points(model, [sequences[i] for i in mine], [queries[i] for i in mine], iters, warm_start, batch_size, mode,
                        device, alpha1, alpha2)
     counts = []
@@ -614,16 +658,12 @@ def propagate_masks(model, sequences, first_labels, iters=32, warm_start=False, 
     a model that requires grad it raises ValueError."""
     from . import native
     from .segment import _step, check_labels
-    if model._needs_grad():
-        raise ValueError("propagate_masks is inference only: call it under torch.no_grad()")
-    firsts = list(first_labels)
-    if len(firsts) != len(sequences):
-        raise ValueError(f"propagate_masks: {len(sequences)} videos but {len(firsts)} first-frame label maps")
+    _check_inference(model, "propagate_masks")
+    firsts, = _check_counts(sequences, "propagate_masks", ("first-frame label maps", first_labels))
     if not sequences:
         return []
     for seq, first in zip(sequences, firsts):
-        if len(seq) < 2:
-            raise ValueError(f"propagate_masks: a video needs T >= 2 frames, got {len(seq)}")
+        _check_frames(seq, "propagate_masks")
         if tuple(first.shape) != tuple(seq[0].shape[-2:]):
             raise ValueError(f"propagate_masks: expected first labels {list(seq[0].shape[-2:])}, got {list(first.shape)}")
         check_sides(*first.shape, "propagate_masks")
@@ -659,21 +699,15 @@ def validate_segmentation(model, sequences, gt_labels, iters=32, warm_start=Fals
     from .dist import gather_strided, strided_items, world_rank
     from .segment import VOID, segmentation_counts, summarize_segmentation
     world, rank = world_rank()
-    if len(gt_labels) != len(sequences):
-        raise ValueError(f"validate_segmentation: {len(sequences)} videos but {len(gt_labels)} ground-truth label sets")
+    _check_counts(sequences, "validate_segmentation", ("ground-truth label sets", gt_labels))
     for seq, gt in zip(sequences, gt_labels):
-        if len(seq) < 3:
-            raise ValueError(f"validate_segmentation: a video needs T >= 3 frames (the first and last are not scored), got "
-                             f"{len(seq)}")
+        _check_frames(seq, "validate_segmentation", 3, " (the first and last are not scored)")
         if tuple(gt.shape) != (len(seq), *seq[0].shape[-2:]):
             raise ValueError(f"validate_segmentation: expected ground truth {[len(seq), *seq[0].shape[-2:]]}, got "
                              f"{list(gt.shape)}")
     mine = list(strided_items(range(len(sequences)), world, rank))
-    by_size = {}
-    for i in mine:
-        by_size.setdefault(tuple(sequences[i][0].shape[-2:]), []).append(i)
     counts = {}
-    for idx in by_size.values():
+    for idx in _by_size(sequences, mine):
         firsts = [torch.where(gt_labels[i][0] == VOID, 0, gt_labels[i][0]) for i in idx]
         preds = propagate_masks(model, [sequences[i] for i in idx], firsts, iters, warm_start, batch_size, mode, device,
                                 alpha1, alpha2)
@@ -705,44 +739,30 @@ def inpaint_videos(model, sequences, masks, iters=32, warm_start=False, batch_si
     mask count that does not match the videos, sweeps < 0 or max_distance < 1.  Inference only: with grad enabled on a
     model that requires grad it raises ValueError."""
     from .inpaint import _check_sweeps, _max_distance, _run
-    if model._needs_grad():
-        raise ValueError("inpaint_videos is inference only: call it under torch.no_grad()")
-    masks = list(masks)
-    if len(masks) != len(sequences):
-        raise ValueError(f"inpaint_videos: {len(sequences)} videos but {len(masks)} mask sets")
+    _check_inference(model, "inpaint_videos")
+    masks, = _check_counts(sequences, "inpaint_videos", ("mask sets", masks))
     _check_sweeps(sweeps, "inpaint_videos")
     for seq, m in zip(sequences, masks):
-        if len(seq) < 2:
-            raise ValueError(f"inpaint_videos: a video needs T >= 2 frames, got {len(seq)}")
+        _check_frames(seq, "inpaint_videos")
         if tuple(m.shape) != (len(seq), *seq[0].shape[-2:]):
             raise ValueError(f"inpaint_videos: expected masks {[len(seq), *seq[0].shape[-2:]]}, got {list(m.shape)}")
         check_sides(*m.shape[-2:], "inpaint_videos")
-        _max_distance(max_distance, len(seq), "inpaint_videos")
-    by_size = {}
-    for i, seq in enumerate(sequences):
-        by_size.setdefault(tuple(seq[0].shape[-2:]), []).append(i)
+        _max_distance(max_distance, "inpaint_videos", len(seq))
     out = [None] * len(sequences)
-    for idx in by_size.values():
+    for idx in _by_size(sequences, range(len(sequences))):
         seqs = [sequences[i] for i in idx]
         holes = [masks[i] != 0 for i in idx]
         seen = [[torch.where(h[t].to(f.device), 0.0, f.float()) for t, f in enumerate(seq)] for seq, h in zip(seqs, holes)]
-        lens = [len(seq) for seq in seqs]
-        V, T = len(seqs), max(lens)
-        H, W = seqs[0][0].shape[-2:]
-        flows = None
+        flows = _PairStack(seqs, ("flow_up", "flow_up_bw"))
         for s, k, r in run_sequences_bidirectional(model, seen, iters, warm_start=warm_start, batch_size=batch_size,
                                                    mode=mode, device=device, alpha1=alpha1, alpha2=alpha2):
-            if flows is None:
-                dev = r["flow_up"].device
-                flows = [torch.zeros(V, T - 1, 2, H, W, dtype=torch.float32, device=dev) for _ in range(2)]
-            flows[0][s, k].copy_(r["flow_up"])
-            flows[1][s, k].copy_(r["flow_up_bw"])
-        frames = torch.zeros(V, T, 3, H, W, dtype=torch.float32, device=dev)
-        hole = torch.zeros(V, T, H, W, dtype=torch.uint8, device=dev)
-        for v, (seq, h) in enumerate(zip(seqs, holes)):
-            frames[v, :lens[v]] = torch.stack([f.to(dev).float() for f in seq])
-            hole[v, :lens[v]] = h.to(dev)
-        res, source = _run(frames, hole, flows[0], flows[1], sweeps, max_distance, alpha1, alpha2, lengths=lens)
+            flows.add(s, k, r)
+        dev = flows["flow_up"].device
+        frames = _pad_videos([torch.stack([f.to(dev).float() for f in seq]) for seq in seqs], 0)
+        hole = _pad_videos([h.to(dev, torch.uint8) for h in holes], 0)
+        lens = [len(seq) for seq in seqs]
+        res, source = _run(frames, hole, flows["flow_up"], flows["flow_up_bw"], sweeps, max_distance, alpha1, alpha2,
+                           lengths=lens)
         for v, i in enumerate(idx):
             out[i] = (res[v, :lens[v]], source[v, :lens[v]])
     return out
@@ -762,8 +782,7 @@ def validate_inpainting(model, sequences, masks, iters=32, warm_start=False, bat
     from .inpaint import ssim, summarize_inpainting
     from .interp import interpolation_error
     world, rank = world_rank()
-    if len(masks) != len(sequences):
-        raise ValueError(f"validate_inpainting: {len(sequences)} videos but {len(masks)} mask sets")
+    _check_counts(sequences, "validate_inpainting", ("mask sets", masks))
     mine = list(strided_items(range(len(sequences)), world, rank))
     got = inpaint_videos(model, [sequences[i] for i in mine], [masks[i] for i in mine], iters, warm_start, batch_size, mode,
                          device, alpha1, alpha2, sweeps, max_distance)
@@ -787,15 +806,11 @@ def _consistent_steps(model, sequences, processed, iters, warm_start, batch_size
     V [T_v,C,H,W] results on the device, frame pair + 1 of the video just written."""
     from . import native
     from .temporal import _check_params, temporal_step
-    if model._needs_grad():
-        raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
-    procs = list(processed)
-    if len(procs) != len(sequences):
-        raise ValueError(f"{what}: {len(sequences)} videos but {len(procs)} processed videos")
+    _check_inference(model, what)
+    procs, = _check_counts(sequences, what, ("processed videos", processed))
     _check_params(lam, alpha, sweeps, what)
     for seq, p in zip(sequences, procs):
-        if len(seq) < 2:
-            raise ValueError(f"{what}: a video needs T >= 2 frames, got {len(seq)}")
+        _check_frames(seq, what)
         if p.dim() != 4 or p.shape[0] != len(seq) or tuple(p.shape[2:]) != tuple(seq[0].shape[-2:]):
             raise ValueError(f"{what}: expected processed frames [{len(seq)},C,{seq[0].shape[-2]},{seq[0].shape[-1]}], got "
                              f"{list(p.shape)}")
@@ -859,9 +874,7 @@ def validate_temporal_consistency(model, sequences, processed, iters=32, warm_st
     from .interp import interpolation_error
     from .temporal import summarize_temporal, warping_error
     world, rank = world_rank()
-    procs = list(processed)
-    if len(procs) != len(sequences):
-        raise ValueError(f"validate_temporal_consistency: {len(sequences)} videos but {len(procs)} processed videos")
+    procs, = _check_counts(sequences, "validate_temporal_consistency", ("processed videos", processed))
     mine = list(strided_items(range(len(sequences)), world, rank))
     warp = {i: [None] * (len(sequences[i]) - 1) for i in mine}
     got = None
@@ -920,40 +933,35 @@ def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8,
     and 2 residuals x 2 channels x 4 B + 2 occlusion masks x 1 B + 2 x 4 B of consistency error while it is checked) ~ 69
     V T bytes per pixel, plus at most 1 GiB of fill workspace: e.g. 11.3 GB for eight 50-frame videos of 480x854 (17.3 GB
     peak measured on that workload with the model, its workspace and the input frames on the device)."""
-    from .stabilize import (_check_fill_params, _check_fit_params, _check_path_params, _fill, fit_homographies, smooth_path,
+    from .stabilize import (_check_fill_params, _check_fit_params, _check_path_params, fit_homographies, smooth_path,
                             warp_frames)
     what = "stabilize_videos"
-    if model._needs_grad():
-        raise ValueError(f"{what} is inference only: call it under torch.no_grad()")
+    _check_inference(model, what)
     _check_fit_params(stride, hypotheses, tau, refine, seed, what)
     _check_path_params(radius, sigma, crop_min, what)
     if fill:
         _check_fill_params(sweeps, max_distance, alpha1, alpha2, what)
     for seq in sequences:
-        if len(seq) < 2:
-            raise ValueError(f"{what}: a video needs T >= 2 frames, got {len(seq)}")
+        _check_frames(seq, what)
         check_sides(*seq[0].shape[-2:], what)
     from . import native
     fits = [[None] * (len(seq) - 1) for seq in sequences]
-    ws = flows = None
+    ws = None
+    flows = _PairStack(sequences, ("flow_up", "flow_up_bw")) if fill else None
     kw = dict(warm_start=warm_start, batch_size=batch_size, mode=mode, device=device)
     if fill:
-        pairs = ((s, k, r["flow_up"], r["flow_up_bw"])
-                 for s, k, r in run_sequences_bidirectional(model, sequences, iters, alpha1=alpha1, alpha2=alpha2, **kw))
+        pairs = run_sequences_bidirectional(model, sequences, iters, alpha1=alpha1, alpha2=alpha2, **kw)
     else:
-        pairs = ((s, k, flow, None) for s, k, flow in run_sequences(model, sequences, iters, **kw))
-    for s, k, flow, flow_bw in pairs:
+        pairs = ((s, k, {"flow_up": flow}) for s, k, flow in run_sequences(model, sequences, iters, **kw))
+    for s, k, r in pairs:
+        flow = r["flow_up"]
         if flow.is_cuda and ws is None:
             H, W = flow.shape[-2:]
             ws = torch.empty(native.rnc.homography_fit_workspace_bytes(1, H, W, stride, hypotheses), dtype=torch.uint8,
                              device=flow.device)
         fits[s][k] = fit_homographies(flow[None], stride, hypotheses, tau, refine, seed, workspace=ws)
-        if flow_bw is not None:
-            if flows is None:
-                V, T = len(sequences), max(len(seq) for seq in sequences)
-                flows = torch.zeros(2, V, T - 1, *flow.shape, dtype=torch.float32, device=flow.device)
-            flows[0, s, k].copy_(flow)
-            flows[1, s, k].copy_(flow_bw)
+        if fill:
+            flows.add(s, k, r)
     out = []
     for seq, fit in zip(sequences, fits):
         A, inl, mat, st = (torch.cat([f[j] for f in fit]) for j in range(4))
@@ -966,28 +974,22 @@ def stabilize_videos(model, sequences, iters=32, warm_start=False, batch_size=8,
         if fill:
             out[-1]["transforms_inv"] = Minv[0]
     if fill and out:
-        _fill_stabilized(out, flows, sweeps, max_distance, alpha1, alpha2, _fill)
+        _fill_stabilized(out, flows, sweeps, max_distance, alpha1, alpha2)
     return out
 
 
-def _fill_stabilized(out, flows, sweeps, max_distance, alpha1, alpha2, fill):
+def _fill_stabilized(out, flows, sweeps, max_distance, alpha1, alpha2):
     """stabilize_videos' fill: the results stacked and padded (zero frames without holes, identity motion and maps, and
-    fill's padding pairs occluded in both directions), filled, and written back into each dict with its source map."""
+    _fill's padding pairs occluded in both directions), filled, and written back into each dict with its source map."""
+    from .stabilize import _fill
     lens = [r["frames"].shape[0] for r in out]
-    V, T = len(out), max(lens)
-    _, C, H, W = out[0]["frames"].shape
-    dev = out[0]["frames"].device
-    eye = torch.eye(3, dtype=torch.float64, device=dev)
-    frames = torch.zeros(V, T, C, H, W, dtype=torch.float32, device=dev)
-    valid = torch.ones(V, T, H, W, dtype=torch.uint8, device=dev)
-    motion = eye.repeat(V, T - 1, 1, 1)
-    maps, maps_inv = eye.repeat(V, T, 1, 1), eye.repeat(V, T, 1, 1)
-    for v, r in enumerate(out):
-        n = lens[v]
-        frames[v, :n], valid[v, :n], motion[v, :n - 1] = r["frames"], r["valid"], r["motion"]
-        maps[v, :n], maps_inv[v, :n] = r["transforms"], r.pop("transforms_inv")
-    res, source = fill(frames, valid, flows[0], flows[1], motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2,
-                       lengths=lens)
+    eye = torch.eye(3, dtype=torch.float64, device=out[0]["frames"].device)
+    frames = _pad_videos([r["frames"] for r in out], 0)
+    valid = _pad_videos([r["valid"] for r in out], 1)
+    motion, maps = (_pad_videos([r[key] for r in out], eye) for key in ("motion", "transforms"))
+    maps_inv = _pad_videos([r.pop("transforms_inv") for r in out], eye)
+    res, source = _fill(frames, valid, flows["flow_up"], flows["flow_up_bw"], motion, maps, maps_inv, sweeps, max_distance,
+                        alpha1, alpha2, lengths=lens)
     for v, r in enumerate(out):
         r["frames"], r["source"] = res[v, :lens[v]], source[v, :lens[v]]
 

@@ -186,7 +186,8 @@ def host_harmonic_fill(values, unknown, sweeps=DEFAULT_SWEEPS):
 # ------------------------------------------------------------------------------------------------------- propagation
 
 
-def _max_distance(max_distance, T, what):
+def _max_distance(max_distance, what, T=2):
+    """max_distance, or max(T - 1, 1) for None (so only a caller that uses the value needs T); else ValueError unless >= 1."""
     if max_distance is None:
         return max(T - 1, 1)
     if not isinstance(max_distance, int) or max_distance < 1:
@@ -233,7 +234,7 @@ def inpaint_propagate(frames, masks, flow, flow_bw, occ, occ_bw, max_distance=No
     give the same bits.  ValueError before any launch for mismatched shapes, mixed devices, T < 2, a side above 4096 or
     max_distance < 1."""
     V, T, H, W = _check_propagate(frames, masks, flow, flow_bw, occ, occ_bw)
-    maxd = _max_distance(max_distance, T, "inpaint_propagate")
+    maxd = _max_distance(max_distance, "inpaint_propagate", T)
     if not frames.is_cuda:
         return host_inpaint_propagate(frames, masks, flow, flow_bw, occ, occ_bw, max_distance)
     dev = frames.device
@@ -288,7 +289,7 @@ def host_inpaint_propagate(frames, masks, flow, flow_bw, occ, occ_bw, max_distan
     evaluated in fp64 on float32 operands and rounded once to float32, in the kernel's order.  Serves CPU tensors and is the
     kernel's test reference.  Returns (frames float32 [V,T,3,H,W], source uint8 [V,T,H,W]) on the CPU."""
     V, T, H, W = _check_propagate(frames, masks, flow, flow_bw, occ, occ_bw)
-    maxd = _max_distance(max_distance, T, "inpaint_propagate")
+    maxd = _max_distance(max_distance, "inpaint_propagate", T)
     out = torch.empty(V, T, 3, H, W, dtype=torch.float32)
     source = torch.zeros(V, T, H, W, dtype=torch.uint8)
     for v in range(V):
@@ -320,25 +321,35 @@ def _check_inpaint(frames, masks, flow, flow_bw, sweeps, max_distance):
     if len(devs) != 1:
         raise ValueError(f"inpaint: the frames, masks and flows must be on one device, got {sorted(map(str, devs))}")
     _check_sweeps(sweeps, "inpaint")
-    _max_distance(max_distance, T, "inpaint")
+    _max_distance(max_distance, "inpaint", T)
     return V, T, H, W
 
 
-def _run(frames, masks, flow, flow_bw, sweeps, max_distance, alpha1, alpha2, lengths=None):
-    """Steps 2-4 with the flows (float32) completed in place, on the tensors' device.  With lengths, video v's pairs from
-    lengths[v] - 1 on are padding: occluded in both directions, so no chain enters them."""
+def _complete(flow, flow_bw, hole, sweeps):
+    """Step 2's completion in place: forward flows under their pair's first frame's holes, backward under the second's."""
+    harmonic_fill(flow, hole[:, :-1], sweeps, out=flow)
+    harmonic_fill(flow_bw, hole[:, 1:], sweeps, out=flow_bw)
+
+
+def _propagate(frames, hole, flow, flow_bw, sweeps, max_distance, alpha1, alpha2, lengths=None):
+    """Step 2's consistency check and steps 3-4 on the completed flows, on the tensors' device.  With lengths, video v's
+    pairs from lengths[v] - 1 on are padding: occluded in both directions, so no chain enters them."""
     V, T1, _, H, W = flow.shape
-    m = masks.detach().to(torch.uint8)
-    harmonic_fill(flow, m[:, :-1], sweeps, out=flow)
-    harmonic_fill(flow_bw, m[:, 1:], sweeps, out=flow_bw)
     occ, occ_bw, _, _ = fb_consistency(flow.reshape(V * T1, 2, H, W), flow_bw.reshape(V * T1, 2, H, W), alpha1, alpha2)
     occ, occ_bw = occ.reshape(V, T1, H, W), occ_bw.reshape(V, T1, H, W)
     for v, n in enumerate(lengths or ()):
         occ[v, n - 1:] = 1
         occ_bw[v, n - 1:] = 1
-    out, source = inpaint_propagate(frames, m, flow, flow_bw, occ, occ_bw, max_distance)
+    out, source = inpaint_propagate(frames, hole, flow, flow_bw, occ, occ_bw, max_distance)
     harmonic_fill(out, source == SOURCE_SPATIAL, sweeps, out=out)
     return out, source
+
+
+def _run(frames, masks, flow, flow_bw, sweeps, max_distance, alpha1, alpha2, lengths=None):
+    """Steps 2-4 with the flows (float32) completed in place, on the tensors' device; lengths as _propagate's."""
+    m = masks.detach().to(torch.uint8)
+    _complete(flow, flow_bw, m, sweeps)
+    return _propagate(frames, m, flow, flow_bw, sweeps, max_distance, alpha1, alpha2, lengths)
 
 
 def inpaint(frames, masks, flow, flow_bw, sweeps=DEFAULT_SWEEPS, max_distance=None, alpha1=0.01, alpha2=0.5):

@@ -97,6 +97,7 @@ import numpy as np
 import torch
 
 from . import native
+from .inpaint import _check_sweeps, _check_video, _complete, _max_distance, _propagate, psnr
 from .restate import check_sides, inside, project, sample
 
 DEFAULT_STRIDE, DEFAULT_HYPOTHESES, DEFAULT_TAU, DEFAULT_REFINE = 8, 256, 2.0, 4
@@ -688,17 +689,14 @@ def host_add_global_motion(res, res_bw, motion, maps, maps_inv):
 
 
 def _check_fill_params(sweeps, max_distance, alpha1, alpha2, what):
-    from .inpaint import _check_sweeps
     _check_sweeps(sweeps, what)
-    if max_distance is not None and (not isinstance(max_distance, int) or max_distance < 1):
-        raise ValueError(f"{what}: expected max_distance >= 1 or None, got {max_distance!r}")
+    _max_distance(max_distance, what)
     for name, a in (("alpha1", alpha1), ("alpha2", alpha2)):
         if not isinstance(a, (int, float)) or isinstance(a, bool) or not 0 <= a <= 1e30:
             raise ValueError(f"{what}: expected a finite {name} >= 0, got {a!r}")
 
 
 def _check_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2):
-    from .inpaint import _check_video
     V, T, H, W = _check_video(frames, valid, flow, flow_bw, "fill_uncovered")
     _check_flow_maps(flow, flow_bw, motion, maps, maps_inv, "fill_uncovered")
     if frames.device != flow.device or valid.device != flow.device:
@@ -709,24 +707,13 @@ def _check_fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, 
 
 
 def _fill(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps, max_distance, alpha1, alpha2, lengths=None):
-    """Step 5 on the tensors' device.  With lengths, video v's pairs from lengths[v] - 1 on are padding: occluded in both
-    directions, so no chain enters them."""
-    from .inpaint import SOURCE_SPATIAL, harmonic_fill, inpaint_propagate
-    from .metrics import fb_consistency
-    V, T1, _, H, W = flow.shape
+    """Step 5 on the tensors' device: rnc.inpaint's two stages on the residuals, the motion re-added between them; lengths
+    as rnc.inpaint._propagate's."""
     res, res_bw = flow_residual(flow, flow_bw, motion, maps, maps_inv)
     hole = (valid == 0).to(torch.uint8)
-    harmonic_fill(res, hole[:, :-1], sweeps, out=res)
-    harmonic_fill(res_bw, hole[:, 1:], sweeps, out=res_bw)
+    _complete(res, res_bw, hole, sweeps)
     _readd_(res, res_bw, motion, maps, maps_inv)
-    occ, occ_bw, _, _ = fb_consistency(res.view(V * T1, 2, H, W), res_bw.view(V * T1, 2, H, W), alpha1, alpha2)
-    occ, occ_bw = occ.view(V, T1, H, W), occ_bw.view(V, T1, H, W)
-    for v, n in enumerate(lengths or ()):
-        occ[v, n - 1:] = 1
-        occ_bw[v, n - 1:] = 1
-    out, source = inpaint_propagate(frames, hole, res, res_bw, occ, occ_bw, max_distance)
-    harmonic_fill(out, source == SOURCE_SPATIAL, sweeps, out=out)
-    return out, source
+    return _propagate(frames, hole, res, res_bw, sweeps, max_distance, alpha1, alpha2, lengths)
 
 
 def fill_uncovered(frames, valid, flow, flow_bw, motion, maps, maps_inv, sweeps=512, max_distance=None, alpha1=0.01,
@@ -807,7 +794,6 @@ def summarize_stabilization(videos):
     being interpolation_error's (sq_sum, count) of frames (t + 1, t).  Each score is the mean over videos; itf and input_itf
     the mean over a video's pairs of rnc.inpaint.psnr (100 dB cap), then over videos; frames and videos, their numbers.  NaN
     without a video; in fp64."""
-    from .inpaint import psnr
     out = {k: 0.0 for k in SCORES}
     itf = itf_in = 0.0
     frames = 0
